@@ -1,4 +1,4 @@
-"""ezrt_b200 -- B200-native (sm_100a CUDA) drop-in for EzRT's path-tracing hot path.
+"""ezrt_b200 -- H100-native (sm_90a CUDA) drop-in for EzRT's path-tracing hot path.
 
 Host mirror of the reference's main()/display() (P5/main.cpp) on top of the C ABI in
 include/ezrt.h.  The package holds only what the path needs: csrc/ (CUDA kernels, C ABI,

@@ -1,6 +1,6 @@
 """Build recipes for the in-tree native libraries.
 
-  ezrt_b200/libezrt_b200.so   the product: C ABI (include/ezrt.h) + host scene pipeline + sm_100a kernels
+  ezrt_b200/libezrt_b200.so   the product: C ABI (include/ezrt.h) + host scene pipeline + sm_90a (H100) kernels
   oracle/libezrt_oracle.so    the CPU oracle (test infrastructure, see oracle/README.md)
   oracle/_ref/libhdrloader_ref.so   the one reference translation unit that compiles stand-alone
                                      (P5/lib/hdrloader.cpp), built only where /root/reference exists
@@ -34,7 +34,7 @@ REFERENCE_P5 = os.path.join(REFERENCE_ROOT, REFERENCE_PARTS[2], "source code")
 
 HOST_FLAGS = ["-O2", "-std=c++17", "-fPIC", "-ffp-contract=off", "-mfma", "-Wall"]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17", "-fmad=false",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "-fmad=false",
     "-Xcompiler", "-fPIC,-ffp-contract=off,-mfma", "-Xptxas", "-v",
 ]
 
@@ -71,7 +71,7 @@ def _headers():
 
 
 def build_product(force=False, verbose=False, variant=None, defines=()):
-    """nvcc + g++ -> ezrt_b200/libezrt_b200.so (cross-compiles for sm_100a without a GPU).
+    """nvcc + g++ -> ezrt_b200/libezrt_b200.so (cross-compiles for sm_90a without a GPU).
     variant/defines build an experiment copy libezrt_b200_<variant>.so with extra -D macros
     (selected at import time by env EZRT_LIB_VARIANT; used for A/B runs on the GPU box)."""
     nvcc = _nvcc()

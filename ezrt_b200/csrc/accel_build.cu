@@ -19,8 +19,7 @@
 // 2 * count(left) -- so no allocation counter is needed and a final compaction of the used slots yields the host builder's
 // dense pre-order array.  The children's boxes fall out of the parent's sweep (prefix at the split, suffix after it).
 //
-// 1 M triangles: 20-23 ms on a B200 (13 ms of level rounds, 6 ms read-back of the 660 k nodes) against 312 ms for the threaded host
-// builder (profiles/scene_create_r2.txt).
+// 1 M triangles: level rounds plus the read-back of the 660 k nodes, much faster than the threaded host builder.
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>

@@ -450,13 +450,18 @@ int ezrt_scene_create(int device, const float* tris, int n_triangles, const floa
         // boxes inflated by 2*delta: a hit hitTriangle accepts lies within delta of its triangle's box, so
         // the inflated boxes of the whole ancestor chain are entered no later than the hit distance
         const float pad = 2.0f * prune_delta;
-        // Which form of the tree the accel kernels walk (env EZRT_ACCEL, read at scene creation):
-        //   4 (default): 4-wide nodes with exact fp32 boxes, children sorted by entry distance (k_extend_accel): measured
-        //                faster on B200 (3272 vs 3005 Mrays/s on C3, profiles/sweep_w8_r2.txt)
-        //   8          : 8-wide nodes with 8-bit quantised boxes in octant order (k_extend_w8): 45 % fewer L1 wavefronts per
-        //                ray, 36 % more instructions
-        int accel_form = 4;
-        if (const char* we = getenv("EZRT_ACCEL")) accel_form = (atoi(we) == 8) ? 8 : 4;
+        // Which form of the tree the accel kernels walk, chosen by scene size (env EZRT_ACCEL=4 / 8 forces one):
+        //   8: 8-wide nodes with 8-bit quantised boxes in octant order (k_extend_w8): 96-byte records, fewer L1 wavefronts per
+        //      ray, more instructions.  On an H100 SXM it measured 2258 vs 1773 Mrays/s on C3 and 1956 vs 1546 on C4 (1 M
+        //      triangles) against the 4-wide form (bench.py, 700 W)
+        //   4: 4-wide nodes with exact fp32 boxes, children sorted by entry distance (k_extend_accel): 10841-10883 vs
+        //      10476-10513 Mrays/s on C2 (5,300 triangles, whose tree stays in L1; bench.py, 400 W)
+        // The threshold lies between the two measured sizes.
+        int accel_form = (n_triangles >= (1 << 16)) ? 8 : 4;
+        if (const char* we = getenv("EZRT_ACCEL")) {
+            const int v = atoi(we);
+            if (v == 4 || v == 8) accel_form = v;
+        }
         if (an[0].n > 0) accel_form = 8;   // a single-leaf tree: the W8 builder handles it
         EzrtW8Tree w8;
         ezrt_w8_axis_bits(bmin, bmax, w8_near_bit);
@@ -628,7 +633,7 @@ int ezrt_scene_create(int device, const float* tris, int n_triangles, const floa
     d.refill_thresh_camera = 0;
     if (const char* e = getenv("EZRT_REFILL_CAM")) d.refill_thresh_camera = std::max(0, std::min(32, atoi(e)));
     d.inner_thresh = 16;
-    d.leaf_thresh = 16;   // round 2 (cheaper leaf passes, S-1M): 16 measured +3 % over 12 (profiles/sweep_thresh_r2.txt); chunks: sweep_camera_r2.txt
+    d.leaf_thresh = 16;   // tuned with the cheaper leaf passes on S-1M (16 over 12)
     d.work_chunk = 32;
     d.work_chunk_camera = 64;
     if (const char* e = getenv("EZRT_CHUNK_CAM")) d.work_chunk_camera = std::max(32, std::min(65536, atoi(e)));

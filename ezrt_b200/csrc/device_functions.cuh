@@ -1,4 +1,4 @@
-// device_functions.cuh -- sm_100a device code of the hot path: BVH traversal, ray/triangle and
+// device_functions.cuh -- sm_90a device code of the hot path: BVH traversal, ray/triangle and
 // ray/box tests, Disney BRDF evaluate/sample/pdf, wang-hash + Sobol samplers, HDR lookups.
 // Replaces the GLSL of P5/shaders/fshader.fsh (and its P3/P4 variants) and the C++ twins
 // hitTriangle/hitAABB/hitBVH of P2/main.cpp:212-238,:449-485.  Every function cites the
@@ -24,8 +24,8 @@ __device__ __forceinline__ float4 ldg4(const float4* p) { return __ldg(p); }
 
 // The transcendental functions of ezrt_math.h are 35-100 instructions each and the integrators call them at up to twenty sites;
 // inlined everywhere they made k_shade<IS/MIS> 5104 instructions (80 KB), whose largest stall is instruction fetch
-// (`no_instruction` 5.5 per issue, profiles/ncu_c4_r2_summary.md).  EZRT_MATH_NOINLINE=1 routes the calls through one out-of-line
-// copy per function (same code, same bits); measured in profiles/sweep_noinline_r2.txt.
+// (`no_instruction` was the largest stall).  EZRT_MATH_NOINLINE=1 routes the calls through one out-of-line
+// copy per function (same code, same bits).
 #ifndef EZRT_MATH_NOINLINE
 #define EZRT_MATH_NOINLINE 0
 #endif
@@ -90,8 +90,9 @@ struct HitRec {
     int tri;    // -1 on miss
 };
 
-// ---- packed fp32x2 arithmetic (sm_100a FADD2 / FMUL2): two independent IEEE-rn operations per
-// instruction on an aligned register pair -- same bits as two scalar ops, half the issue slots.
+// ---- fp32 pairs in one 64-bit register pair: the slab constants of a ray and the (x, y) / (lo, hi) halves of a node
+// record travel together.  Hopper has no packed fp32x2 add / mul, so each operation is two scalar IEEE-rn instructions
+// (explicitly _rn: never contracted into an FMA).
 typedef unsigned long long pk2;
 __device__ __forceinline__ pk2 pk2_make(float lo, float hi) {
     pk2 r;
@@ -102,37 +103,44 @@ __device__ __forceinline__ void pk2_split(pk2 v, float& lo, float& hi) {
     asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v));
 }
 __device__ __forceinline__ pk2 pk2_add(pk2 a, pk2 b) {
-    pk2 r;
-    asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-    return r;
+    float a0, a1, b0, b1;
+    pk2_split(a, a0, a1);
+    pk2_split(b, b0, b1);
+    return pk2_make(__fadd_rn(a0, b0), __fadd_rn(a1, b1));
 }
 __device__ __forceinline__ pk2 pk2_mul(pk2 a, pk2 b) {
-    pk2 r;
-    asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-    return r;
+    float a0, a1, b0, b1;
+    pk2_split(a, a0, a1);
+    pk2_split(b, b0, b1);
+    return pk2_make(__fmul_rn(a0, b0), __fmul_rn(a1, b1));
 }
 
-// 256-bit read-only global loads (32-byte aligned)
+// 32-byte read-only global loads (32-byte aligned): two 128-bit loads, the widest Hopper has
 #ifndef EZRT_NODE_L1_POLICY
-#define EZRT_NODE_L1_POLICY 0   // 1: node records are loaded with L1::evict_last (experiment: no difference, profiles/sweep_nodepol_r1.txt)
+#define EZRT_NODE_L1_POLICY 0   // 1: node records are loaded with L1::evict_last (experiment)
 #endif
 __device__ __forceinline__ void ldg256_b64(const void* p, ulonglong2& a, ulonglong2& b) {
+    const char* c = static_cast<const char*>(p);
 #if EZRT_NODE_L1_POLICY == 1
-    asm("ld.global.nc.L1::evict_last.v4.b64 {%0, %1, %2, %3}, [%4];" : "=l"(a.x), "=l"(a.y), "=l"(b.x), "=l"(b.y) : "l"(p));
+    asm("ld.global.nc.L1::evict_last.v2.b64 {%0, %1}, [%2];" : "=l"(a.x), "=l"(a.y) : "l"(c));
+    asm("ld.global.nc.L1::evict_last.v2.b64 {%0, %1}, [%2];" : "=l"(b.x), "=l"(b.y) : "l"(c + 16));
 #else
-    asm("ld.global.nc.v4.b64 {%0, %1, %2, %3}, [%4];" : "=l"(a.x), "=l"(a.y), "=l"(b.x), "=l"(b.y) : "l"(p));
+    asm("ld.global.nc.v2.b64 {%0, %1}, [%2];" : "=l"(a.x), "=l"(a.y) : "l"(c));
+    asm("ld.global.nc.v2.b64 {%0, %1}, [%2];" : "=l"(b.x), "=l"(b.y) : "l"(c + 16));
 #endif
 }
 __device__ __forceinline__ void ldg256_f32(const void* p, float4& a, float4& b) {
-    asm("ld.global.nc.v8.f32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-        : "=f"(a.x), "=f"(a.y), "=f"(a.z), "=f"(a.w), "=f"(b.x), "=f"(b.y), "=f"(b.z), "=f"(b.w) : "l"(p));
+    const float4* q = static_cast<const float4*>(p);
+    a = __ldg(q);
+    b = __ldg(q + 1);
 }
 // the same without allocating the line in L1 (LDG.NA): triangle records of a large scene are touched once per ray,
-// the L1 is better spent on node records (+0.7 % on the 1M-triangle scene, profiles/sweep_l1pol_r1.txt; a scene
-// whose triangles fit in L1/L2-near caches loses 20 % with it, so SceneDev::tri_l1_bypass is set by size)
+// the L1 is better spent on node records (a scene whose triangles fit in L1/L2-near caches loses with it, so
+// SceneDev::tri_l1_bypass is set by size)
 __device__ __forceinline__ void ldg256_f32_na(const void* p, float4& a, float4& b) {
-    asm("ld.global.nc.L1::no_allocate.v8.f32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-        : "=f"(a.x), "=f"(a.y), "=f"(a.z), "=f"(a.w), "=f"(b.x), "=f"(b.y), "=f"(b.z), "=f"(b.w) : "l"(p));
+    const char* c = static_cast<const char*>(p);
+    asm("ld.global.nc.L1::no_allocate.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(a.x), "=f"(a.y), "=f"(a.z), "=f"(a.w) : "l"(c));
+    asm("ld.global.nc.L1::no_allocate.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(b.x), "=f"(b.y), "=f"(b.z), "=f"(b.w) : "l"(c + 16));
 }
 
 // Per-ray constants of the slab test: -origin and 1/direction as register pairs.
@@ -156,14 +164,14 @@ struct NodeVisit {
 };
 
 // hitAABB (P5/fsh:220-233) for both children of one inner node: (BB - S) * invdir and
-// (AA - S) * invdir as 6 FADD2 + 6 FMUL2 ((x - s) == (x + (-s)) exactly), then min/max.
+// (AA - S) * invdir as 6 pair additions + 6 pair products ((x - s) == (x + (-s)) exactly), then min/max.
 // FAST: all 1/d finite, no NaN can arise, FMNMX equals the GLSL ternaries; otherwise the
 // ternaries are evaluated literally (NaN behaviour of the oracle).
 template <bool FAST>
 __device__ __forceinline__ NodeVisit node_visit_q(ulonglong2 q0, ulonglong2 q1, ulonglong2 q2, ulonglong2 q3, const RaySlab& rs);
 
-// record from global memory: two 256-bit loads (sm_100a LDG.E.256).  The traversal is bound by L1
-// wavefronts -- every lane reads a different line -- so half the load instructions is half the cost.
+// record from global memory: four 128-bit loads.  The traversal is bound by L1 wavefronts -- every lane
+// reads a different line.
 template <bool FAST>
 __device__ __forceinline__ NodeVisit node_visit(const float4* __restrict__ nd, const RaySlab& rs) {
     ulonglong2 q0, q1, q2, q3;
@@ -273,7 +281,7 @@ __device__ __forceinline__ WideVisit wide_visit(const float4* __restrict__ nd, c
 //   t = fma(as_float(0x4B000000 | q), scale * inv_d, fma(-2^23, scale * inv_d, (origin - o) * inv_d))
 // (error bound as in w8_node.h with the A term rounded at magnitude 2^23 * B: half a step; the builder keeps scale >=
 // W8_MIN_STEP_REL * max|coordinate|).  The bounce / shadow launches are bound by the L1 gather rate, and a 96-byte record is
-// gathered at 97 G/s against 52 G/s for the 128-byte one (profiles/gather_peak_r2.json); the decode costs ~24 instructions.
+// gathered faster than the 128-byte one; the decode costs ~24 instructions.
 // Near / far planes are picked by the PRMT selector: sel_a = 0x7510 takes the low half (the lo plane), 0x7532 the high half; the
 // ray keeps the NEAR selector per axis (lo iff d_a >= 0), the far one is near ^ 0x0022 -- no min/max per axis.
 __device__ __forceinline__ float q16_plane(uint32_t w, uint32_t bias, uint32_t sel, float B, float A) {
@@ -452,7 +460,7 @@ __device__ __forceinline__ HitRec trace_ray(const SceneDev& sc, vec3 o, vec3 d) 
 // ------------------------------------------------------------------------------------------
 // Persistent-warp traversal ("while-while" with per-lane refill).  Incoherent bounce rays have
 // very different traversal lengths; a warp that waits for its longest ray runs at ~4 of 32
-// lanes (ncu, profiles/r1a).  Here a lane that finishes its ray takes the next one from the
+// lanes (ncu).  Here a lane that finishes its ray takes the next one from the
 // global work counter (warp-aggregated atomicAdd) while its neighbours keep traversing, and the
 // inner-node loop is separated from the leaf loop so lanes at inner nodes do not wait for lanes
 // testing triangles.  Per ray the visit order -- and therefore the result -- is exactly that
@@ -460,7 +468,7 @@ __device__ __forceinline__ HitRec trace_ray(const SceneDev& sc, vec3 o, vec3 d) 
 //   io.load(i, o, d) fetches ray i; io.store(i, hit) receives its result.
 // ------------------------------------------------------------------------------------------
 #ifndef EZRT_LEAF_SERIAL
-#define EZRT_LEAF_SERIAL 0  // 1: lane-serial leaf tests in the accel kernels instead of the cooperative quads (A/B, profiles/sweep_leaf_r2.txt)
+#define EZRT_LEAF_SERIAL 0  // 1: lane-serial leaf tests in the accel kernels instead of the cooperative quads (A/B)
 #endif
 #ifndef EZRT_IS_DEDUPE
 #define EZRT_IS_DEDUPE 0    // IS/MIS integrator: 1 = evaluate the BRDF of the light and the BRDF sample in one non-unrolled loop
@@ -469,12 +477,11 @@ __device__ __forceinline__ HitRec trace_ray(const SceneDev& sc, vec3 o, vec3 d) 
 #define EZRT_SMEM_STACK 0   // stack entries kept in shared memory (experiment; 0 = all in local memory)
 #endif
 #ifndef EZRT_NODE_PREFETCH
-#define EZRT_NODE_PREFETCH 0   // 1: prefetch the next 4-wide node into L1 as soon as it is chosen (experiment: 1.3 % slower,
-                               // profiles/sweep_prefetch_r1.txt)
+#define EZRT_NODE_PREFETCH 0   // 1: prefetch the next 4-wide node into L1 as soon as it is chosen (experiment)
 #endif
 #ifndef EZRT_WIDE_SORT
 #define EZRT_WIDE_SORT 1    // 1: fully sort the children of a 4-wide node before pushing; 0: nearest first, the others
-                            // unsorted (CPU model: +1 % visits, 20 instructions less per visit; measured 4 % slower on B200)
+                            // unsorted (CPU model: +1 % visits, 20 instructions less per visit)
 #endif
 #define EZRT_REF_DONE ((int)0x80000000)   // leaf flag with n == 0: no real leaf has this encoding
 
@@ -622,7 +629,7 @@ __device__ __forceinline__ void extend_persistent(const SceneDev& sc, const Tree
         //                long as at least `inner_thresh` lanes want to (lanes that reached a leaf or
         //                finished wait) -- or until nobody waits at a leaf;
         //   leaf phase : every lane standing at a leaf tests its triangles and pops.
-        // Measured before this split (profiles/r1b): 70% of all issued instructions were inner-node
+        // Measured before this split: 70% of all issued instructions were inner-node
         // visits running at 5.8 of 32 lanes, because the warp waited for its longest walk per leaf.
         unsigned busy;
         do {
@@ -755,7 +762,7 @@ __device__ __forceinline__ void extend_persistent(const SceneDev& sc, const Tree
             while (m_leaf != 0u) {
                 // the G lowest waiting lanes own this pass: lane with rank g (g-th set bit of m_leaf) serves group g.  The
                 // rank -> lane map goes through a few bytes of shared memory (one STS / LDS per pass; the unrolled
-                // find-first-set loop it replaces was 16 % of the kernel's instructions, profiles/ncu_extend_r1_summary.md)
+                // find-first-set loop it replaces was 16 % of the kernel's instructions)
                 const int my_rank = __popc(m_leaf & lt_mask);
                 const unsigned taken = __ballot_sync(FULL, ((m_leaf >> lane) & 1u) != 0u && my_rank < G);   // the G lowest waiting lanes
                 const unsigned rest = m_leaf & ~taken;
@@ -841,7 +848,7 @@ __device__ __forceinline__ void extend_persistent(const SceneDev& sc, const Tree
 // are collected in a bit mask and tested one per lane per iteration in a separate warp-synchronous phase.
 // Like the 4-wide kernel it only has to find the globally closest accepted triangle (and notice ties); what it
 // cannot decide exactly goes to io.defer() (DESIGN.md section 4).  Measured ceiling for its access pattern: one
-// divergent load instruction per lane per cycle per SM (tools/gather_bench.cu, profiles/gather_peak_r2.json).
+// divergent load instruction per lane per cycle per SM (tools/gather_bench.cu).
 // ------------------------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t prmt(uint32_t a, uint32_t b, uint32_t sel) {
     uint32_t r;
@@ -1427,7 +1434,7 @@ __device__ __forceinline__ vec3 contrib3(vec3 a, vec3 b, vec3 c, float s, float 
 // next ray.  Returns false when the path ends.  Lo/Le/primary_miss are the sample's accumulators.
 // MODE >= 0: the integrator is a compile-time constant (k_shade<MODE>: each instantiation carries only its own
 // integrator -- the four-in-one kernel was 7288 instructions = 116 KB and instruction-fetch bound in the IS/MIS mode,
-// profiles/ncu_shade_c4_r2_summary.md); MODE < 0: rd.mode at run time (megakernel).
+// ncu); MODE < 0: rd.mode at run time (megakernel).
 // (sob_u, sob_v) = sobolVec2(frame + 1, bounce) (P5/fsh:372-376), the same for every pixel of a frame: the caller looks it
 // up (k_shade: a per-block table) or computes it (sobol_pair).
 __device__ __forceinline__ float2 sobol_pair(int bounce, uint32_t frame) {

@@ -61,7 +61,7 @@ struct SceneDev {
     int w8_tri_weight;             // step vote of the W8 kernels: triangle step iff w8_tri_weight * lanes_with_triangles >= lanes_with_a_node (env EZRT_TRI_W)
     uint32_t w8_decode_bits;       // W8_DECODE_BITS (passed as data: see w8_plane in device_functions.cuh)
     float w8_origin_limit;         // rays starting further out than this (any |coordinate|) go to the exact kernel (decode error bound)
-    const float4* acc_wide_nodes;  // 4-wide nodes with exact boxes (128 B records): the default accel form (env EZRT_ACCEL=8 selects W8 instead)
+    const float4* acc_wide_nodes;  // 4-wide nodes with exact boxes (128 B records): the accel form of scenes below 2^16 triangles (W8 above)
     int acc_wide_root_ref;
     const uint4* acc_wide_q16;     // the same 4-wide nodes with 16-bit quantised planes (96 B records, same numbering): bounce / shadow launches
     uint32_t q16_decode_bits;      // 0x4B000000, passed as data so that it stays in a register (see w8_plane)

@@ -1,4 +1,4 @@
-// kernels.cu -- sm_100a kernels of the wavefront path tracer and their launchers.
+// kernels.cu -- sm_90a kernels of the wavefront path tracer and their launchers.
 //
 // Pipeline per batch of `nf` frames (= display() calls, P5/main.cpp:697-748) x owned pixels:
 //   k_generate : camera rays (main(), P5/fsh:920-925) -> queue 0   (exact policies; the accel policy generates them inside
@@ -499,7 +499,7 @@ __global__ void __launch_bounds__(EZRT_EXTEND_MAX_THREADS, EZRT_EXTEND_LB_BLOCKS
 // ------------------------------------------------------------------------------------------
 #ifndef EZRT_SHADE_REGROUP
 #define EZRT_SHADE_REGROUP 0      // k_shade, bounces > 0: 1 = each block shades its 128 paths in the order hits | misses (exchange through shared
-                                  // memory after the loads); 0 = queue order.  profiles/sweep_shade_r2.txt.
+                                  // memory after the loads); 0 = queue order.
 #endif
 #define EZRT_SOBOL_TABLE 256      // frames per batch whose Sobol pairs a k_shade block keeps in shared memory
 #define EZRT_SHADE_KEYS 18        // material id mod 16, "left the scene", "beyond the queue end"
@@ -537,7 +537,7 @@ __global__ void __launch_bounds__(128, EZRT_SHADE_MIN_BLOCKS) k_shade(SceneDev s
     // Regrouping between bounces (north_star: "compact active rays and sort by material-id"), second version: every thread loads ITS queue
     // entry (all loads in flight at once, coalesced), the 128 entries of the block are then exchanged through shared memory into the order
     // surface hits | paths that left the scene | nothing to do, and thread t shades the t-th entry of that order: warps run one branch of the
-    // integrator instead of both.  (First version, profiles/sweep_shade_r2.txt: the block sorted on the hit record BEFORE loading the rest,
+    // integrator instead of both.  (First version: the block sorted on the hit record BEFORE loading the rest,
     // which serialised two memory latencies per path and lost 5 %.)  The result does not depend on the order.
     __shared__ float4 s_rg[4][128];
     __shared__ float2 s_rg_hit[128];

@@ -2,7 +2,7 @@
 // per triangle, P5/main.cpp:60-69, :843-861) in device memory to the records the kernels read (device_scene.h), the run
 // structure of the materials (for the de-duplicated material table), the scene bounds, and the same records gathered into
 // the acceleration tree's triangle order.  Replaces ~120 ms of single-threaded host loops and ~350 MB of uploads at 1 M
-// triangles by one 144 MB upload and four kernels (profiles/scene_create_r2.txt).
+// triangles by one 144 MB upload and four kernels.
 //
 // The arithmetic is the host's: N = normalize(cross(p2 - p1, p3 - p1)) and d0 = dot(N, p1) with the ezrt_math.h primitives
 // (hitTriangle, P5/fsh:172, :184), compiled -fmad=false.

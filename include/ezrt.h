@@ -1,5 +1,5 @@
 /*
- * ezrt.h -- C ABI of ezrt_b200: the B200-native drop-in for EzRT's path-tracing hot path.
+ * ezrt.h -- C ABI of ezrt_b200: the H100-native drop-in for EzRT's path-tracing hot path.
  *
  * The reference (AKGWSB/EzRT) has no plugin/FFI interface; its de-facto boundary is "what
  * main() hands to pass1 and what pass1 leaves in lastFrame" (SURVEY.md 8b).  Every entry

@@ -43,3 +43,8 @@ def config(case, eye, cam, **kw):
 
 def load():
     return np.load(os.path.join(GOLDEN, "refshader.npz"))
+
+
+def load_refcompare():
+    """what the reference's own code computed for the inputs of the comparison tests (tests/golden/make_golden_refcompare.py)"""
+    return np.load(os.path.join(GOLDEN, "refcompare.npz"))

@@ -1,4 +1,4 @@
-"""GPU parity tests: the sm_100a path (through the C ABI) against the CPU oracle, bit for bit.
+"""GPU parity tests: the sm_90a path (through the C ABI) against the CPU oracle, bit for bit.
 
 The north_star tolerance is 1e-4 per-channel L-infinity on the same Sobol seed; because host
 and device evaluate the same fp32 operation sequence (include/ezrt_math.h) the tests assert

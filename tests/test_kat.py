@@ -8,7 +8,6 @@ import zlib
 import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-P5_FSH = "/root/reference/part 5 -- Importance Sampling & Low Discrepancy Sequence/source code/shaders/fshader.fsh"
 
 
 def _table():
@@ -41,14 +40,10 @@ def test_sobol_first_points_match_joe_kuo(oracle):
 
 
 def test_sobol_table_checksum_and_reference_literal():
+    # 0xAB08B2B2: crc32 of the V[8*32] literal of P5/fsh, which tests/golden/make_golden_refcompare.py compares with the table
     t = _table()
     assert len(t) == 256
     assert zlib.crc32(struct.pack("<256I", *t)) == 0xAB08B2B2
-    if os.path.exists(P5_FSH):  # only in the authoring container
-        src = open(P5_FSH).read()
-        m = re.search(r"const uint V\[8\*32\] = \{\s*([0-9u,\s]+)\};", src)
-        ref = [int(x.strip().rstrip("u")) for x in m.group(1).split(",") if x.strip()]
-        assert ref == t
 
 
 def test_cranley_patterson_seed_and_wrap(oracle):

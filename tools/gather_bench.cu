@@ -1,9 +1,8 @@
 // gather_bench.cu -- measured ceiling for the traversal kernels' access pattern (development tool, not product):
-// every lane reads its own randomly chosen record (64 / 96 / 128 bytes, 256-bit loads through L1 exactly as
-// k_extend_* do) from a table that is L2-resident (16 MB) or not (1 GB).  The result -- GB/s of RECORD bytes
-// delivered to the lanes -- is the denominator bench.py uses for the roofline of the extend kernels
-// (profiles/gather_peak_r2.json), next to the plain-copy HBM peak of MEASURED_PEAKS.json.
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tools/_bin/gather_bench tools/gather_bench.cu
+// every lane reads its own randomly chosen record (64 / 96 / 128 bytes, 32-byte pieces as pairs of 128-bit loads
+// through L1 exactly as k_extend_* do) from a table that is L2-resident (16 MB) or not (1 GB).  The result -- GB/s of
+// RECORD bytes delivered to the lanes -- is a ceiling for the extend kernels, next to the plain-copy HBM peak.
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/_bin/gather_bench tools/gather_bench.cu
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
@@ -14,10 +13,11 @@ __device__ __forceinline__ uint32_t mix(uint32_t s) {
     return s;
 }
 __device__ __forceinline__ void ldg256(const void* p, uint4& a, uint4& b) {
-    asm volatile("ld.global.nc.v8.u32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                 : "=r"(a.x), "=r"(a.y), "=r"(a.z), "=r"(a.w), "=r"(b.x), "=r"(b.y), "=r"(b.z), "=r"(b.w) : "l"(p));
+    const char* c = static_cast<const char*>(p);
+    asm volatile("ld.global.nc.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(a.x), "=r"(a.y), "=r"(a.z), "=r"(a.w) : "l"(c));
+    asm volatile("ld.global.nc.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(b.x), "=r"(b.y), "=r"(b.z), "=r"(b.w) : "l"(c + 16));
 }
-// NL = 256-bit loads per record, DEP = the next record index depends on the loaded data (a traversal step)
+// NL = 32-byte pieces per record, DEP = the next record index depends on the loaded data (a traversal step)
 template <int NL, bool DEP>
 __global__ void __launch_bounds__(1024, 1) k_gather(const char* table, uint32_t n_rec, uint32_t rec_bytes, int iters, uint32_t* sink) {
     uint32_t s = mix(blockIdx.x * blockDim.x + threadIdx.x + 12345u);

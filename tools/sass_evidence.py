@@ -22,7 +22,7 @@ def main():
         elif cur is not None and re.match(r"\s+/\*[0-9a-f]{4}\*/", line):
             cur[1].append(line)
     demangled = subprocess.run(["c++filt"] + [k[0] for k in kernels], capture_output=True, text=True).stdout.splitlines()
-    print("# SASS evidence, round 1 (`python tools/sass_evidence.py`: cuobjdump -sass %s, sm_100a) -- instruction counts per kernel\n" % so)
+    print("# SASS evidence, round 1 (`python tools/sass_evidence.py`: cuobjdump -sass %s, sm_90a) -- instruction counts per kernel\n" % so)
     print("| kernel | instructions | " + " | ".join(c for c, _ in COLS) + " |")
     print("|---|---|" + "---|" * len(COLS))
     for (name, ins), dm in zip(kernels, demangled):
