@@ -26,6 +26,11 @@ class RenderParams(C.Structure):
     ]
 
 
+class AdaptiveParams(C.Structure):
+    """struct ezrt_adaptive_params (include/ezrt.h)."""
+    _fields_ = [("threshold", C.c_float), ("min_spp", C.c_int32), ("check_interval", C.c_int32), ("reserved", C.c_int32)]
+
+
 class Counters(C.Structure):
     """struct ezrt_counters (include/ezrt.h)."""
     _fields_ = [
@@ -45,6 +50,9 @@ SIGNATURES = {
     "ezrt_scene_destroy": (C.c_int, [C.c_void_p]),
     "ezrt_render": (C.c_int, [C.c_void_p, C.POINTER(RenderParams), c_float_p]),
     "ezrt_render_device": (C.c_int, [C.c_void_p, C.POINTER(RenderParams), C.c_void_p, C.c_void_p]),
+    "ezrt_render_adaptive_device": (C.c_int, [C.c_void_p, C.POINTER(RenderParams), C.POINTER(AdaptiveParams), C.c_void_p, C.c_void_p,
+                                              C.c_void_p, C.c_void_p]),
+    "ezrt_render_adaptive": (C.c_int, [C.c_void_p, C.POINTER(RenderParams), C.POINTER(AdaptiveParams), c_float_p, c_int32_p, c_float_p]),
     "ezrt_get_counters": (C.c_int, [C.c_void_p, C.POINTER(Counters)]),
     "ezrt_get_kernel_times": (C.c_int, [C.c_void_p, C.POINTER(C.c_double), C.POINTER(C.c_uint64)]),
     "ezrt_partition_pixels": (C.c_int64, [C.c_int, C.c_int, C.c_int, C.c_int]),

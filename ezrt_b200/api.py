@@ -12,7 +12,7 @@ from dataclasses import dataclass, field
 import numpy as np
 
 from . import _lib
-from ._lib import Counters, EzrtError, RenderParams, check, lib
+from ._lib import AdaptiveParams, Counters, EzrtError, RenderParams, check, lib
 
 MODE_DIFFUSE_P3 = 0
 MODE_DISNEY_ANISO_P4 = 1
@@ -227,6 +227,13 @@ class RenderConfig:
         return p
 
 
+def adaptive_params(threshold, min_spp, check_interval):
+    """struct ezrt_adaptive_params (include/ezrt.h)."""
+    a = AdaptiveParams()
+    a.threshold, a.min_spp, a.check_interval, a.reserved = float(threshold), int(min_spp), int(check_interval), 0
+    return a
+
+
 class Scene:
     """Device-resident scene: the two texture buffers + two HDR textures of P5/main.cpp:878-906."""
 
@@ -274,6 +281,32 @@ class Scene:
         p = cfg.to_struct()
         check(lib.ezrt_render_device(self._h, C.byref(p), C.c_void_p(ptr), C.c_void_p(st)))
         return d_framebuffer
+
+    def render_adaptive(self, cfg, threshold, min_spp=16, check_interval=16):
+        """Tile-adaptive render from frame 0 (ezrt_render_adaptive): cfg.spp is the frame cap; a 16x16 tile stops at the
+        first test (after min_spp, then every check_interval frames) at which every pixel's relative standard error of
+        luminance is <= threshold.  Returns host arrays (image, spp_map, luma2): [H, W, C], [H, W], [H, W] for one part,
+        compact tile-major [n, C], [n], [n] otherwise.  spp_map = frames each pixel received, luma2 = running mean of the
+        squared sample luminance."""
+        n = partition_pixels(cfg.width, cfg.height, cfg.part_rank, cfg.part_count)
+        img = np.zeros((n, cfg.out_channels), dtype=np.float32)
+        spp = np.zeros(n, dtype=np.int32)
+        luma2 = np.zeros(n, dtype=np.float32)
+        p, a = cfg.to_struct(), adaptive_params(threshold, min_spp, check_interval)
+        check(lib.ezrt_render_adaptive(self._h, C.byref(p), C.byref(a), _fp(img), spp.ctypes.data_as(_lib.c_int32_p), _fp(luma2)))
+        if cfg.part_count == 1:
+            return img.reshape(cfg.height, cfg.width, cfg.out_channels), spp.reshape(cfg.height, cfg.width), luma2.reshape(cfg.height, cfg.width)
+        return img, spp, luma2
+
+    def render_adaptive_device(self, cfg, threshold, min_spp, check_interval, d_framebuffer, d_spp, d_luma2, stream=None):
+        """Enqueue a tile-adaptive render on a CUDA stream into device buffers (torch tensors or raw pointers): the
+        framebuffer, int32 frames per pixel, float32 running mean of the squared luminance.  Synchronises the stream once per test."""
+        ptr = lambda t: t.data_ptr() if hasattr(t, "data_ptr") else int(t)
+        st = 0 if stream is None else (stream.cuda_stream if hasattr(stream, "cuda_stream") else int(stream))
+        p, a = cfg.to_struct(), adaptive_params(threshold, min_spp, check_interval)
+        check(lib.ezrt_render_adaptive_device(self._h, C.byref(p), C.byref(a), C.c_void_p(ptr(d_framebuffer)), C.c_void_p(ptr(d_spp)),
+                                              C.c_void_p(ptr(d_luma2)), C.c_void_p(st)))
+        return d_framebuffer, d_spp, d_luma2
 
     def counters(self):
         c = Counters()

@@ -130,6 +130,22 @@ def build_oracle(force=False):
     return _oracle_recipes().build_oracle(force)
 
 
+ORACLE_ADAPTIVE_SO = os.path.join(ROOT, "build", "libezrt_oracle_adaptive.so")
+
+
+def build_oracle_adaptive(force=False):
+    """build/libezrt_oracle_adaptive.so: tests/oracle_adaptive.cpp, the CPU restatement of adaptive sampling over the
+    oracle's sample function (test infrastructure, loaded only by tests/oracle_adaptive.py)."""
+    src = os.path.join(ROOT, "tests", "oracle_adaptive.cpp")
+    deps = [src, os.path.join(ROOT, "oracle", "ezrt_oracle.cpp")] + [os.path.join(INCLUDE, f) for f in os.listdir(INCLUDE)]
+    if force or _newer(ORACLE_ADAPTIVE_SO, deps):
+        os.makedirs(os.path.dirname(ORACLE_ADAPTIVE_SO), exist_ok=True)
+        tmp = ORACLE_ADAPTIVE_SO + ".tmp%d" % os.getpid()
+        _run(["g++"] + HOST_FLAGS + ["-fopenmp", "-Wno-misleading-indentation", "-shared", "-I", INCLUDE, src, "-o", tmp])
+        os.replace(tmp, ORACLE_ADAPTIVE_SO)
+    return ORACLE_ADAPTIVE_SO
+
+
 def build_reference_hdrloader(force=False):
     return _oracle_recipes().build_reference_hdrloader(force)
 
@@ -188,6 +204,7 @@ def build_w4_check(force=False):
 def build_all(force=False, verbose=False):
     build_product(force=force, verbose=verbose)
     build_oracle(force=force)
+    build_oracle_adaptive(force=force)
     build_example(force=force)
     build_reference_hdrloader(force=force)
     build_reference_shaders(force=force)

@@ -4,6 +4,7 @@
 #include <cuda_runtime.h>
 
 #include <chrono>
+#include <cmath>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -86,6 +87,8 @@ struct ezrt_scene {
     int tree_depth = 0;
     // render state (lazily sized)
     DeviceBuffer tiles_buf, queue_buf[2], shadow_buf, lo_buf, le_buf, counters_buf, totals_buf, fb_buf, sort_buf;
+    // adaptive sampling: two surviving-tile lists (ping-pong), per-tile verdicts, the test's counters; the host entry point's spp map + luma2
+    DeviceBuffer adapt_buf, adapt_maps_buf;
     void* hot_base = nullptr;   // accel nodes | geometry | shading records (L2 persisting window)
     size_t hot_bytes = 0;
     size_t l2_persist_bytes = 0;
@@ -196,6 +199,26 @@ std::mutex& scatter_mutex() {
     static std::mutex mu;
     return mu;
 }
+
+int validate_adaptive(const ezrt_render_params* p, const ezrt_adaptive_params* a) {
+    if (!a) return ezrt_set_error(EZRT_ERR_INVALID, "render_adaptive: null adaptive params");
+    if (!std::isfinite(a->threshold) || !(a->threshold > 0.0f))
+        return ezrt_set_error(EZRT_ERR_INVALID, "render_adaptive: threshold must be finite and > 0 (got %g)", (double)a->threshold);
+    if (a->min_spp < 2) return ezrt_set_error(EZRT_ERR_INVALID, "render_adaptive: min_spp must be >= 2 (got %d)", a->min_spp);
+    if (a->check_interval < 1) return ezrt_set_error(EZRT_ERR_INVALID, "render_adaptive: check_interval must be >= 1 (got %d)", a->check_interval);
+    if (a->reserved != 0) return ezrt_set_error(EZRT_ERR_INVALID, "render_adaptive: reserved field must be 0");
+    if (p->first_frame != 0) return ezrt_set_error(EZRT_ERR_INVALID, "render_adaptive: first_frame must be 0 (an adaptive render cannot be resumed)");
+    if (p->pipeline != EZRT_PIPELINE_WAVEFRONT) return ezrt_set_error(EZRT_ERR_INVALID, "render_adaptive: only the wavefront pipeline samples adaptively");
+    return EZRT_OK;
+}
+
+// what the wavefront loop needs beyond a plain render: the criterion and the per-pixel outputs (device)
+struct AdaptiveRun {
+    float threshold;
+    int min_spp, check_interval;
+    int32_t* d_spp;
+    float* d_luma2;
+};
 
 RenderDev make_render_dev(const ezrt_scene* s, const ezrt_render_params* p) {
     RenderDev rd;
@@ -654,6 +677,7 @@ int ezrt_scene_destroy(ezrt_scene* s) {
     s->acc_tri_leaf.release(); s->ref_to_acc.release(); s->acc_wide.release(); s->acc_wide_q16.release();
     s->queue_buf[0].release(); s->queue_buf[1].release(); s->shadow_buf.release();
     s->lo_buf.release(); s->le_buf.release(); s->counters_buf.release(); s->totals_buf.release(); s->fb_buf.release(); s->sort_buf.release();
+    s->adapt_buf.release(); s->adapt_maps_buf.release();
     if (s->own_stream) cudaStreamDestroy(s->own_stream);
     if (s->copy_stream) cudaStreamDestroy(s->copy_stream);
     if (s->side_stream) cudaStreamDestroy(s->side_stream);
@@ -671,13 +695,10 @@ int ezrt_scene_destroy(ezrt_scene* s) {
 // ------------------------------------------------------------------------------------------
 // render
 // ------------------------------------------------------------------------------------------
-int ezrt_render_device(ezrt_scene* s, const ezrt_render_params* p, float* d_fb, void* cuda_stream) {
-    int rc = validate_params(s, p);
-    if (rc) return rc;
-    if (!d_fb) return ezrt_set_error(EZRT_ERR_INVALID, "render: null framebuffer");
+// The render of ezrt_render_device (ad == nullptr) and ezrt_render_adaptive_device: the arguments are validated.
+static int render_device_impl(ezrt_scene* s, const ezrt_render_params* p, float* d_fb, cudaStream_t st, const AdaptiveRun* ad) {
     CU_CHECK(cudaSetDevice(s->device));
-    cudaStream_t st = (cudaStream_t)cuda_stream;
-    rc = prepare_tiles(s, p, st);
+    int rc = prepare_tiles(s, p, st);
     if (rc) return rc;
     rc = s->totals_buf.ensure(sizeof(unsigned long long) * 8);
     if (rc) return rc;
@@ -801,9 +822,29 @@ int ezrt_render_device(ezrt_scene* s, const ezrt_render_params* p, float* d_fb, 
         cudaStreamSetAttribute(st, cudaStreamAttributeAccessPolicyWindow, &attr);
         cudaGetLastError();
     }
-    for (int done = 0; done < p->spp; done += F) {
-        const int nf = std::min(F, p->spp - done);
-        const uint32_t n_slots = (uint32_t)(per_frame * (size_t)nf);
+    // Adaptive sampling: batches end on the test points; after each test the next batches run over the surviving tiles only
+    // (rd.n_tiles, d_tiles), and with an automatic batch size they take more frames, up to the capacity sized above.
+    TileDev *tiles_a = nullptr, *tiles_b = nullptr;
+    unsigned char* keep = nullptr;
+    unsigned int* blocks_done = nullptr;
+    int32_t* test_counts = nullptr;
+    if (ad) {
+        const size_t list_bytes = ((sizeof(TileDev) * (size_t)rd.n_tiles + 255) / 256) * 256;
+        const size_t keep_bytes = (((size_t)rd.n_tiles + 255) / 256) * 256;
+        if ((rc = s->adapt_buf.ensure(2 * list_bytes + keep_bytes + 16))) return rc;
+        char* base = (char*)s->adapt_buf.p;
+        tiles_a = (TileDev*)base;
+        tiles_b = (TileDev*)(base + list_bytes);
+        keep = (unsigned char*)(base + 2 * list_bytes);
+        blocks_done = (unsigned int*)(base + 2 * list_bytes + keep_bytes);
+        test_counts = (int32_t*)(blocks_done + 1);
+        CU_CHECK(cudaMemsetAsync(blocks_done, 0, sizeof(unsigned int), st));
+    }
+    size_t active_pixels = s->n_pixels;
+    int next_test = ad ? ad->min_spp : p->spp;
+    for (int done = 0; done < p->spp && rd.n_tiles > 0;) {
+        const int nf = std::min(F, std::min(p->spp, next_test) - done);
+        const uint32_t n_slots = (uint32_t)((size_t)rd.n_tiles * EZRT_TILE_PIXELS * (size_t)nf);
         const uint32_t batch_first = p->first_frame + (uint32_t)done;
         CU_CHECK(cudaMemsetAsync(cnt, 0, sizeof(uint32_t) * n_counters, st));
         const bool fused_camera = accel;   // accel policy: camera rays are generated inside the first extend kernel
@@ -873,10 +914,29 @@ int ezrt_render_device(ezrt_scene* s, const ezrt_render_params* p, float* d_fb, 
             CU_CHECK(cudaStreamWaitEvent(st, s->fb_wait, 0));
             s->fb_wait = nullptr;
         }
-        launch_blend(rd, d_tiles, nf, batch_first, Lo, Le, d_fb, st);
-        launch_tally(q_count, s_count, d_ext, d_sh, p->max_bounce + 1, totals, fused_camera ? (uint32_t)(s->n_pixels * (size_t)nf) : 0u, st);
+        if (ad) launch_blend_adaptive(rd, d_tiles, nf, batch_first, Lo, Le, d_fb, ad->d_luma2, ad->d_spp, st);
+        else launch_blend(rd, d_tiles, nf, batch_first, Lo, Le, d_fb, st);
+        launch_tally(q_count, s_count, d_ext, d_sh, p->max_bounce + 1, totals, fused_camera ? (uint32_t)(active_pixels * (size_t)nf) : 0u, st);
         s->span_end(sp, st);
         s->launches += 2;
+        done += nf;
+        if (ad && done == next_test && done < p->spp) {
+            TileDev* survivors = (d_tiles == tiles_a) ? tiles_b : tiles_a;
+            sp = s->span_begin(3, st);
+            launch_adaptive_check(rd, d_tiles, done, ad->threshold, d_fb, ad->d_luma2, keep, blocks_done, survivors, test_counts, st);
+            s->span_end(sp, st);
+            s->launches++;
+            CU_CHECK(cudaGetLastError());
+            int32_t left[2] = {0, 0};   // surviving tiles, their pixels: the one synchronisation of a test
+            CU_CHECK(cudaMemcpyAsync(left, test_counts, sizeof(left), cudaMemcpyDeviceToHost, st));
+            CU_CHECK(cudaStreamSynchronize(st));
+            d_tiles = survivors;
+            rd.n_tiles = left[0];
+            active_pixels = (size_t)left[1];
+            if (p->frames_per_batch <= 0 && rd.n_tiles > 0)
+                F = (int)std::min<size_t>(capacity / ((size_t)rd.n_tiles * EZRT_TILE_PIXELS), (size_t)p->spp);
+            next_test += ad->check_interval;
+        }
     }
     if (l2_window) {  // leave the caller's stream as it was
         cudaStreamAttrValue attr;
@@ -888,6 +948,48 @@ int ezrt_render_device(ezrt_scene* s, const ezrt_render_params* p, float* d_fb, 
     CU_CHECK(cudaGetLastError());
     CU_CHECK(cudaEventRecord(s->ev_stop, st));
     s->have_timing = true;
+    return EZRT_OK;
+}
+
+int ezrt_render_device(ezrt_scene* s, const ezrt_render_params* p, float* d_fb, void* cuda_stream) {
+    int rc = validate_params(s, p);
+    if (rc) return rc;
+    if (!d_fb) return ezrt_set_error(EZRT_ERR_INVALID, "render: null framebuffer");
+    return render_device_impl(s, p, d_fb, (cudaStream_t)cuda_stream, nullptr);
+}
+
+int ezrt_render_adaptive_device(ezrt_scene* s, const ezrt_render_params* p, const ezrt_adaptive_params* a, float* d_fb, int32_t* d_spp,
+                                float* d_luma2, void* cuda_stream) {
+    int rc = validate_params(s, p);
+    if (!rc) rc = validate_adaptive(p, a);
+    if (rc) return rc;
+    if (!d_fb || !d_spp || !d_luma2) return ezrt_set_error(EZRT_ERR_INVALID, "render_adaptive: null output buffer");
+    const AdaptiveRun ad{a->threshold, a->min_spp, a->check_interval, d_spp, d_luma2};
+    return render_device_impl(s, p, d_fb, (cudaStream_t)cuda_stream, &ad);
+}
+
+int ezrt_render_adaptive(ezrt_scene* s, const ezrt_render_params* p, const ezrt_adaptive_params* a, float* framebuffer, int32_t* spp,
+                         float* luma2) {
+    int rc = validate_params(s, p);
+    if (!rc) rc = validate_adaptive(p, a);
+    if (rc) return rc;
+    if (!framebuffer || !spp || !luma2) return ezrt_set_error(EZRT_ERR_INVALID, "render_adaptive: null output buffer");
+    CU_CHECK(cudaSetDevice(s->device));
+    const size_t npix = (size_t)ezrt_partition_pixels(p->width, p->height, p->part_rank, p->part_count);
+    const size_t fb_bytes = sizeof(float) * npix * p->out_channels;
+    const size_t map_bytes = ((sizeof(float) * npix + 255) / 256) * 256;
+    if ((rc = s->fb_buf.ensure(std::max<size_t>(fb_bytes, 16)))) return rc;
+    if ((rc = s->adapt_maps_buf.ensure(2 * map_bytes + 16))) return rc;
+    int32_t* d_spp = (int32_t*)s->adapt_maps_buf.p;
+    float* d_luma2 = (float*)((char*)s->adapt_maps_buf.p + map_bytes);
+    cudaStream_t st = s->own_stream;
+    s->fb_wait = nullptr;
+    const AdaptiveRun ad{a->threshold, a->min_spp, a->check_interval, d_spp, d_luma2};
+    if ((rc = render_device_impl(s, p, (float*)s->fb_buf.p, st, &ad))) return rc;
+    CU_CHECK(cudaMemcpyAsync(framebuffer, s->fb_buf.p, fb_bytes, cudaMemcpyDeviceToHost, st));
+    CU_CHECK(cudaMemcpyAsync(spp, d_spp, sizeof(int32_t) * npix, cudaMemcpyDeviceToHost, st));
+    CU_CHECK(cudaMemcpyAsync(luma2, d_luma2, sizeof(float) * npix, cudaMemcpyDeviceToHost, st));
+    CU_CHECK(cudaStreamSynchronize(st));
     return EZRT_OK;
 }
 

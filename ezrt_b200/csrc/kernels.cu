@@ -13,6 +13,8 @@
 //     k_shadow_accel / k_shadow : any-hit trace of the environment shadow rays (IS mode only): marks each ray lit / occluded
 //     k_nee          : the lit light samples' contributions (BRDF, environment, MIS) -> Lo
 //   k_blend    : running mean into the framebuffer in frame order (P5/fsh:942-947)
+// Adaptive sampling adds k_blend<true> (also the running mean of the squared luminance and the spp map) and, at each test
+// point, k_adaptive_check (drops converged tiles from the tile list the next batches run on).
 // No host synchronisation inside a render: queue sizes live in device counters.
 #include "kernels.h"
 
@@ -719,8 +721,12 @@ __device__ __forceinline__ size_t fb_index(const RenderDev& rd, const TileDev& t
     return (size_t)(t.y0 + iy) * rd.width + (t.x0 + ix);
 }
 
+// ADAPTIVE: also the running mean of the squared sample luminance (luma2) and the frames the pixel received (spp_map), both
+// indexed like the framebuffer's pixels (ezrt_math.h, "adaptive sampling").  The plain instantiation never touches them.
+template <bool ADAPTIVE>
 __global__ void __launch_bounds__(256) k_blend(RenderDev rd, const TileDev* __restrict__ tiles, int nf, uint32_t batch_first_frame,
-                                               const float4* __restrict__ Lo, const float4* __restrict__ Le, float* __restrict__ fb) {
+                                               const float4* __restrict__ Lo, const float4* __restrict__ Le, float* __restrict__ fb,
+                                               float* __restrict__ luma2, int32_t* __restrict__ spp_map) {
     uint32_t per_frame = (uint32_t)rd.n_tiles * EZRT_TILE_PIXELS;
     uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
     if (r >= per_frame) return;
@@ -728,8 +734,11 @@ __global__ void __launch_bounds__(256) k_blend(RenderDev rd, const TileDev* __re
     int ix, iy;
     in_tile_xy((int)(r & 255u), ix, iy);
     if (ix >= t.w || iy >= t.h) return;
-    size_t idx = fb_index(rd, t, ix, iy) * (size_t)rd.out_channels;
+    const size_t pix = fb_index(rd, t, ix, iy);
+    size_t idx = pix * (size_t)rd.out_channels;
     vec3 acc = (batch_first_frame == 0u) ? splat3(0.0f) : ez_v3(fb[idx], fb[idx + 1], fb[idx + 2]);
+    float m2 = 0.0f;
+    if (ADAPTIVE && batch_first_frame != 0u) m2 = luma2[pix];
     for (int f = 0; f < nf; f++) {
         float4 lo = Lo[(size_t)f * per_frame + r];
         vec3 color = ez_v3(lo.x, lo.y, lo.z);   // primary miss: the sky; no emission at the first hit: 0 + Lo = Lo
@@ -739,9 +748,69 @@ __global__ void __launch_bounds__(256) k_blend(RenderDev rd, const TileDev* __re
         }
         float a = EZ_DIV(1.0f, __uint2float_rn(batch_first_frame + (uint32_t)f + 1u));
         acc = ez_vmix(acc, color, a);
+        if (ADAPTIVE) {
+            const float y = ez_luminance(color);
+            m2 = ez_mix(m2, y * y, a);
+        }
     }
     fb[idx] = acc.x; fb[idx + 1] = acc.y; fb[idx + 2] = acc.z;
     if (rd.out_channels == 4) fb[idx + 3] = 1.0f;
+    if (ADAPTIVE) {
+        luma2[pix] = m2;
+        spp_map[pix] = (int32_t)(batch_first_frame + (uint32_t)nf);
+    }
+}
+
+// The convergence test of adaptive sampling: one block per active tile, one thread per pixel.  A tile survives unless every
+// in-image pixel has err <= threshold (ez_adaptive_error; a NaN survives).  Each block leaves its verdict in keep[]; the last
+// block to finish compacts the surviving tiles, in their input order, into tiles_out and writes (tiles, pixels) to counts.
+// The input order is kept so that the tile order and the launch shapes of the next batches do not depend on block timing.
+__global__ void __launch_bounds__(256) k_adaptive_check(RenderDev rd, const TileDev* __restrict__ tiles_in, int n_frames, float threshold,
+                                                        const float* __restrict__ fb, const float* __restrict__ luma2,
+                                                        unsigned char* __restrict__ keep, unsigned int* __restrict__ blocks_done,
+                                                        TileDev* __restrict__ tiles_out, int32_t* __restrict__ counts) {
+    __shared__ uint32_t s_scan[34];
+    __shared__ uint32_t s_tiles, s_pixels;
+    __shared__ bool s_last;
+    const TileDev t = tiles_in[blockIdx.x];
+    int ix, iy;
+    in_tile_xy((int)threadIdx.x, ix, iy);
+    bool ok = true;
+    if (ix < t.w && iy < t.h) {
+        const size_t pix = fb_index(rd, t, ix, iy);
+        const size_t idx = pix * (size_t)rd.out_channels;
+        const float err = ez_adaptive_error(luma2[pix], ez_v3(fb[idx], fb[idx + 1], fb[idx + 2]), n_frames);
+        ok = (err <= threshold);
+    }
+    const bool converged = __syncthreads_and(ok) != 0;
+    if (threadIdx.x == 0) {
+        keep[blockIdx.x] = converged ? 0 : 1;
+        __threadfence();
+        s_last = (atomicAdd(blocks_done, 1u) == gridDim.x - 1);
+    }
+    __syncthreads();
+    if (!s_last) return;
+    // last block: order-preserving compaction of the surviving tiles.  block_append on a shared-memory counter ranks the
+    // survivors of each chunk of 256 by thread index and the chunks run in order, so tiles_out keeps the order of tiles_in.
+    __threadfence();
+    if (threadIdx.x == 0) { s_tiles = 0u; s_pixels = 0u; }
+    __syncthreads();
+    for (uint32_t i0 = 0; i0 < gridDim.x; i0 += blockDim.x) {
+        const uint32_t i = i0 + threadIdx.x;
+        const bool k = (i < gridDim.x) && ((volatile const unsigned char*)keep)[i] != 0;
+        const uint32_t pos = block_append(k, &s_tiles, s_scan);
+        if (k) {
+            const TileDev ti = tiles_in[i];
+            tiles_out[pos] = ti;
+            atomicAdd(&s_pixels, (uint32_t)(ti.w * ti.h));
+        }
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        counts[0] = (int32_t)s_tiles;
+        counts[1] = (int32_t)s_pixels;
+        *blocks_done = 0u;   // ready for the next test
+    }
 }
 
 // totals[0..2] += primary, bounce, shadow rays of this batch; totals[3] += samples; totals[4] += deferred rays
@@ -1096,7 +1165,17 @@ void launch_nee(const SceneDev& sc, const RenderDev& rd, ShadowQueue sq, const u
 void launch_blend(const RenderDev& rd, const TileDev* tiles, int nf, uint32_t batch_first_frame, const float4* Lo,
                   const float4* Le, float* fb, cudaStream_t st) {
     uint32_t per_frame = (uint32_t)rd.n_tiles * EZRT_TILE_PIXELS;
-    k_blend<<<div_up(per_frame, 256), 256, 0, st>>>(rd, tiles, nf, batch_first_frame, Lo, Le, fb);
+    k_blend<false><<<div_up(per_frame, 256), 256, 0, st>>>(rd, tiles, nf, batch_first_frame, Lo, Le, fb, nullptr, nullptr);
+}
+void launch_blend_adaptive(const RenderDev& rd, const TileDev* tiles, int nf, uint32_t batch_first_frame, const float4* Lo,
+                           const float4* Le, float* fb, float* luma2, int32_t* spp_map, cudaStream_t st) {
+    uint32_t per_frame = (uint32_t)rd.n_tiles * EZRT_TILE_PIXELS;
+    k_blend<true><<<div_up(per_frame, 256), 256, 0, st>>>(rd, tiles, nf, batch_first_frame, Lo, Le, fb, luma2, spp_map);
+}
+void launch_adaptive_check(const RenderDev& rd, const TileDev* tiles_in, int n_frames, float threshold, const float* fb, const float* luma2,
+                           unsigned char* keep, unsigned int* blocks_done, TileDev* tiles_out, int32_t* counts, cudaStream_t st) {
+    if (rd.n_tiles <= 0) return;
+    k_adaptive_check<<<rd.n_tiles, EZRT_TILE_PIXELS, 0, st>>>(rd, tiles_in, n_frames, threshold, fb, luma2, keep, blocks_done, tiles_out, counts);
 }
 void launch_tally(const uint32_t* q_counts, const uint32_t* s_counts, const uint32_t* d_ext, const uint32_t* d_sh, int n_stages,
                   unsigned long long* totals, uint32_t n_primary, cudaStream_t st) {

@@ -45,6 +45,13 @@ void launch_deferred_lane(const SceneDev& sc, const RenderDev& rd, const TileDev
 void launch_nee(const SceneDev& sc, const RenderDev& rd, ShadowQueue sq, const uint32_t* s_count, float4* Lo, uint32_t n_max, int n_sms, cudaStream_t st);
 void launch_blend(const RenderDev& rd, const TileDev* tiles, int nf, uint32_t batch_first_frame, const float4* Lo,
                   const float4* Le, float* fb, cudaStream_t st);
+// adaptive sampling: k_blend<true> also keeps the running mean of the squared sample luminance and the per-pixel frame count
+void launch_blend_adaptive(const RenderDev& rd, const TileDev* tiles, int nf, uint32_t batch_first_frame, const float4* Lo,
+                           const float4* Le, float* fb, float* luma2, int32_t* spp_map, cudaStream_t st);
+// convergence test of the rd.n_tiles tiles of tiles_in after n_frames frames: the surviving tiles -> tiles_out (input order),
+// counts[0] = surviving tiles, counts[1] = their in-image pixels; keep holds rd.n_tiles bytes, *blocks_done must be 0 (left 0)
+void launch_adaptive_check(const RenderDev& rd, const TileDev* tiles_in, int n_frames, float threshold, const float* fb, const float* luma2,
+                           unsigned char* keep, unsigned int* blocks_done, TileDev* tiles_out, int32_t* counts, cudaStream_t st);
 void launch_tally(const uint32_t* q_counts, const uint32_t* s_counts, const uint32_t* d_ext, const uint32_t* d_sh, int n_stages,
                   unsigned long long* totals, uint32_t n_primary, cudaStream_t st);
 void launch_megakernel(const SceneDev& sc, const RenderDev& rd, const TileDev* tiles, bool prune, int spp, float* fb,

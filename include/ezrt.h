@@ -150,6 +150,31 @@ int ezrt_render(ezrt_scene* scene, const ezrt_render_params* params, float* fram
 int ezrt_render_device(ezrt_scene* scene, const ezrt_render_params* params, float* d_framebuffer,
                        void* cuda_stream);
 
+/* Tile-adaptive sampling (DESIGN.md section 8; the criterion is defined in ezrt_math.h).  The image is rendered in 16x16
+ * tiles; after min_spp frames and then every check_interval frames, each tile whose pixels all have a relative standard
+ * error of luminance <= threshold stops, the others go on, up to params->spp frames.  Every tile holds exactly the bits a
+ * plain render with spp = (the frames it received) gives it. */
+typedef struct ezrt_adaptive_params {
+    float threshold;        /* > 0: relative standard error of pixel luminance at which a tile stops */
+    int32_t min_spp;        /* >= 2: frames before the first test */
+    int32_t check_interval; /* >= 1: frames between tests */
+    int32_t reserved;       /* 0 */
+} ezrt_adaptive_params;
+
+/* params->spp = frame cap, params->first_frame must be 0, wavefront pipeline only; any traversal policy, mode and partition
+ * (the decision is per tile, so a part's tiles stop where they would in the whole image).
+ * d_spp:   int32 per pixel, frames the pixel received.
+ * d_luma2: float per pixel, the running mean of the squared sample luminance (M of the criterion).
+ * Both use the framebuffer's pixel layout (tile-major compact when part_count > 1).  Device buffers, enqueued on cuda_stream
+ * like ezrt_render_device, except that each test reads back 8 bytes (surviving tiles and pixels): one stream
+ * synchronisation per test.  ezrt_get_counters reports the work done: samples = sum of the spp map, rays of active tiles
+ * only; with params->profile = 1 the test kernel is timed in class 3 ("other"). */
+int ezrt_render_adaptive_device(ezrt_scene* scene, const ezrt_render_params* params, const ezrt_adaptive_params* adaptive,
+                                float* d_framebuffer, int32_t* d_spp, float* d_luma2, void* cuda_stream);
+/* Same with host buffers (synchronous). */
+int ezrt_render_adaptive(ezrt_scene* scene, const ezrt_render_params* params, const ezrt_adaptive_params* adaptive,
+                         float* framebuffer, int32_t* spp, float* luma2);
+
 /* Counters of the most recent render on this scene (synchronises the stream). */
 int ezrt_get_counters(ezrt_scene* scene, ezrt_counters* out);
 

@@ -288,13 +288,31 @@ EZ_HD float ez_asin(float xx) {
 }
 
 /* ------------------------------------------------------------------ post pass */
+/* the luminance of pass3.fsh:16 */
+EZ_HD float ez_luminance(ez_vec3 c) { return 0.3f * c.x + 0.6f * c.y + 0.1f * c.z; }
+
 /* pass3.fsh:14-25: toneMapping(c, limit) = c * 1.0 / (1.0 + lum / limit), then pow(c, vec3(1.0/2.2)) */
 EZ_HD ez_vec3 ez_tonemap_pass3(ez_vec3 c, float limit) {
-    float luminance = 0.3f * c.x + 0.6f * c.y + 0.1f * c.z;
+    float luminance = ez_luminance(c);
     float den = 1.0f + EZ_DIV(luminance, limit);
     ez_vec3 t = ez_v3(EZ_DIV(c.x * 1.0f, den), EZ_DIV(c.y * 1.0f, den), EZ_DIV(c.z * 1.0f, den));
     const float g = EZ_DIV(1.0f, 2.2f);
     return ez_v3(ez_pow(t.x, g), ez_pow(t.y, g), ez_pow(t.z, g));
+}
+
+/* ------------------------------------------------------------------ adaptive sampling (DESIGN.md section 8)
+ * Per pixel after n frames (frames 0 .. n-1):  y = ez_luminance(c) of each sample colour c;  M = running mean of y*y,
+ * updated in frame order as the colour is (M = ez_mix(M, y*y, 1/(frame+1)), from +0);  Y = ez_luminance of the mean colour.
+ *   var = max(M - Y*Y, 0) (NaN stays NaN),   err = sqrt(var / n) / (Y + EZRT_ADAPTIVE_LUMA_FLOOR)
+ * A 16x16 tile has converged when err <= threshold holds for every pixel of it inside the image (a NaN fails).
+ * The floor lets black pixels with zero variance converge. */
+#define EZRT_ADAPTIVE_LUMA_FLOOR 1e-3f
+
+EZ_HD float ez_adaptive_error(float M, ez_vec3 mean, int n) {
+    float Y = ez_luminance(mean);
+    float var = M - Y * Y;
+    var = (var < 0.0f) ? 0.0f : var;
+    return EZ_DIV(EZ_SQRT(EZ_DIV(var, (float)n)), Y + EZRT_ADAPTIVE_LUMA_FLOOR);
 }
 
 #endif /* EZRT_MATH_H */
