@@ -304,7 +304,14 @@ int ezrt_build_w8(const std::vector<EzrtAccelNode>& an, const std::vector<uint32
             }
         }
         memcpy(&w[W8_W_ORIGIN], origin, 12);
-        memcpy(&w[W8_W_SCALE], scale, 12);
+        uint32_t exp_imask = imask << 24;
+        for (int a = 0; a < 3; a++) {   // a normal power of two is its exponent byte alone
+            uint32_t bits;
+            memcpy(&bits, &scale[a], 4);
+            if ((bits & 0x007fffffu) != 0u || (bits >> 23) == 0u || (bits >> 23) >= 255u) return -5;
+            exp_imask |= (bits >> 23) << (8 * a);
+        }
+        w[W8_W_EXP_IMASK] = exp_imask;
         w[W8_W_CHILD_BASE] = child_base;
         w[W8_W_TRI_BASE] = tri_base;
         for (int a = 0; a < 3; a++) {
@@ -312,7 +319,6 @@ int ezrt_build_w8(const std::vector<EzrtAccelNode>& an, const std::vector<uint32
             memcpy(&w[W8_W_QHI + 2 * a], qhi[a], 8);
         }
         memcpy(&w[W8_W_META], meta, 8);
-        w[W8_W_IMASK] = imask;
         out.nodes.insert(out.nodes.end(), w, w + W8_NODE_WORDS);
     }
     out.n_nodes = (int)queue.size();

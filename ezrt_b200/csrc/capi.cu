@@ -1035,7 +1035,7 @@ int ezrt_get_counters(ezrt_scene* s, ezrt_counters* out) {
     unsigned long long t[8] = {0, 0, 0, 0, 0, 0, 0, 0};
     CU_CHECK(cudaMemcpy(t, s->totals_buf.p, sizeof(t), cudaMemcpyDeviceToHost));
     out->deferred_rays = t[4];
-    out->node_visits = t[5] + t[7];          // t[5]: visits of 128-byte exact nodes, t[7]: of 96-byte nodes (Q16 form, W8)
+    out->node_visits = t[5] + t[7];          // t[5]: visits of 128-byte exact nodes, t[7]: of quantised nodes (Q16 form 96 B, W8 80 B)
     out->tri_tests = t[6];
     out->node_bytes = t[5] * 128ull + t[7] * 96ull;
     out->tri_bytes = t[6] * 64ull;

@@ -129,18 +129,22 @@ __device__ __forceinline__ void ldg256_b64(const void* p, ulonglong2& a, ulonglo
     asm("ld.global.nc.v2.b64 {%0, %1}, [%2];" : "=l"(b.x), "=l"(b.y) : "l"(c + 16));
 #endif
 }
-__device__ __forceinline__ void ldg256_f32(const void* p, float4& a, float4& b) {
-    const float4* q = static_cast<const float4*>(p);
-    a = __ldg(q);
-    b = __ldg(q + 1);
+__device__ __forceinline__ uint4 ldg128_u32(const uint4* p) {
+    uint4 a;
+#if EZRT_NODE_L1_POLICY == 1
+    asm("ld.global.nc.L1::evict_last.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(a.x), "=r"(a.y), "=r"(a.z), "=r"(a.w) : "l"(p));
+#else
+    asm("ld.global.nc.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(a.x), "=r"(a.y), "=r"(a.z), "=r"(a.w) : "l"(p));
+#endif
+    return a;
 }
-// the same without allocating the line in L1 (LDG.NA): triangle records of a large scene are touched once per ray,
+// ldg4 without allocating the line in L1 (LDG.NA): triangle records of a large scene are touched once per ray,
 // the L1 is better spent on node records (a scene whose triangles fit in L1/L2-near caches loses with it, so
-// SceneDev::tri_l1_bypass is set by size)
-__device__ __forceinline__ void ldg256_f32_na(const void* p, float4& a, float4& b) {
-    const char* c = static_cast<const char*>(p);
-    asm("ld.global.nc.L1::no_allocate.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(a.x), "=f"(a.y), "=f"(a.z), "=f"(a.w) : "l"(c));
-    asm("ld.global.nc.L1::no_allocate.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(b.x), "=f"(b.y), "=f"(b.z), "=f"(b.w) : "l"(c + 16));
+// SceneDev::tri_l1_bypass is set by size).  volatile: the load stays behind the branches that guard it.
+__device__ __forceinline__ float4 ldg4_na(const float4* p) {
+    float4 a;
+    asm volatile("ld.global.nc.L1::no_allocate.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(a.x), "=f"(a.y), "=f"(a.z), "=f"(a.w) : "l"(p));
+    return a;
 }
 
 // Per-ray constants of the slab test: -origin and 1/direction as register pairs.
@@ -339,27 +343,27 @@ __device__ __forceinline__ void cswap(float& ka, int& ra, float& kb, int& rb) { 
     ka = tk; kb = uk; ra = tr; rb = ur;
 }
 
-// Ray/triangle test against the repacked record.  Accepts exactly the hits hitTriangle accepts
+// Ray/triangle test against the repacked record (N, d0), p1, p2, p3.  Accepts exactly the hits hitTriangle accepts
 // that are also strictly closer than `best` (the only ones hitArray/hitBVH can keep).
 // TIES (accel policy): a hit at exactly t == best is also reported (return 2) so the caller can
 // detect that two triangles tie and let the exact reference-order traversal decide.
+// The distance checks need only the first 16 bytes; the vertices are loaded for the candidates that pass them.
 template <bool TIES>
 __device__ __forceinline__ int tri_test_t(const float4* __restrict__ rec, vec3 o, vec3 d, float best, float& tout, const bool l1_bypass = false) {
-    float4 q0, q1, q2, q3;
-    if (l1_bypass) {  // warp-uniform
-        ldg256_f32_na(rec, q0, q1);
-        ldg256_f32_na(rec + 2, q2, q3);
-    } else {
-        ldg256_f32(rec, q0, q1);
-        ldg256_f32(rec + 2, q2, q3);
-    }
-    vec3 N = ez_v3(q0.w, q1.w, q2.w);
+    const float4 q0 = l1_bypass ? ldg4_na(rec) : ldg4(rec);   // l1_bypass is warp-uniform
+    vec3 N = f4xyz(q0);
     float nd = ez_dot(N, d);
     if (ez_abs(nd) < 0.00001f) return 0;                        // :181 (|dot(+-N,d)| is sign-free)
-    float t = EZ_DIV(q3.x - ez_dot(o, N), nd);                  // :184 (sign of N cancels exactly)
+    float t = EZ_DIV(q0.w - ez_dot(o, N), nd);                  // :184 (sign of N cancels exactly)
     if (t < 0.0005f) return 0;                                  // :185
     if (TIES ? !(t <= best) : !(t < best)) return 0;            // :245, :273 strict <, first wins
-    vec3 p1 = f4xyz(q0), p2 = f4xyz(q1), p3 = f4xyz(q2);
+    float4 q1, q2, q3;
+    if (l1_bypass) {
+        q1 = ldg4_na(rec + 1); q2 = ldg4_na(rec + 2); q3 = ldg4_na(rec + 3);
+    } else {
+        q1 = ldg4(rec + 1); q2 = ldg4(rec + 2); q3 = ldg4(rec + 3);
+    }
+    vec3 p1 = f4xyz(q1), p2 = f4xyz(q2), p3 = f4xyz(q3);
     vec3 P = ez_add(o, ez_scale(d, t));                         // :188
     float s1 = ez_dot(ez_cross(ez_sub(p2, p1), ez_sub(P, p1)), N);  // :191-195 (N unflipped: r1/r2 swap)
     float s2 = ez_dot(ez_cross(ez_sub(p3, p2), ez_sub(P, p2)), N);
@@ -841,14 +845,14 @@ __device__ __forceinline__ void extend_persistent(const SceneDev& sc, const Tree
 #undef STACK_POP
 
 // ------------------------------------------------------------------------------------------
-// W8: the default traversal of the accel policy.  8-wide nodes with 8-bit quantised child boxes (96-byte records,
-// three 256-bit loads; layout, decode arithmetic and error bound in w8_node.h), children visited in octant order
+// W8: the default traversal of the accel policy.  8-wide nodes with 8-bit quantised child boxes (80-byte records,
+// five 128-bit loads; layout, decode arithmetic and error bound in w8_node.h), children visited in octant order
 // from a hit bit mask -- no distance sort, at most one stack push per node visit -- and a per-lane stack of
 // (child base | slot masks) groups in SHARED memory at [entry][thread].  The triangles of all hit leaf slots of a node
 // are collected in a bit mask and tested one per lane per iteration in a separate warp-synchronous phase.
 // Like the 4-wide kernel it only has to find the globally closest accepted triangle (and notice ties); what it
-// cannot decide exactly goes to io.defer() (DESIGN.md section 4).  Measured ceiling for its access pattern: one
-// divergent load instruction per lane per cycle per SM (tools/gather_bench.cu).
+// cannot decide exactly goes to io.defer() (DESIGN.md section 4).  Measured ceiling for its access pattern on an H100: at
+// most one divergent 128-bit load per lane per SM-cycle (tools/gather_bench.cu, DESIGN.md section 4).
 // ------------------------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t prmt(uint32_t a, uint32_t b, uint32_t sel) {
     uint32_t r;
@@ -978,8 +982,8 @@ __device__ __forceinline__ void extend_w8(const SceneDev& sc, uint32_t n, uint32
             continue;
         }
         // ---------------- traverse: every iteration the warp runs ONE of two steps, chosen by a vote ----------------
-        //   node step     : every lane holding a node visits it (three 256-bit loads, eight slab tests; ~200 instructions)
-        //   triangle step : every lane with pending triangles tests one (two 256-bit loads; ~100 instructions)
+        //   node step     : every lane holding a node visits it (five 128-bit loads, eight slab tests; ~200 instructions)
+        //   triangle step : every lane with pending triangles tests one (one 128-bit load, three more past the distance checks; ~100 instructions)
         // A lane with pending triangles cannot take a node step (its next node depends on them), so the warp takes the
         // triangle step as soon as  tri_weight * (lanes with triangles) >= (lanes with a node)  -- the step that serves
         // more lanes per instruction (tri_weight ~ cost ratio of the two steps, env EZRT_TRI_W).
@@ -993,32 +997,23 @@ __device__ __forceinline__ void extend_w8(const SceneDev& sc, uint32_t n, uint32
             if ((m_node | m_tri) == 0u) { busy = 0u; break; }
             if (m_node != 0u && tri_weight * __popc(m_tri) < __popc(m_node)) {
                 if (at_node) {
-                    const uint4* nd = nodes + (size_t)node * 6;
-                    uint4 h0, h1, l0, l1, u0, u1;
-                    {
-                        ulonglong2 a, b;
-                        ldg256_b64(nd, a, b);
-                        h0 = make_uint4((uint32_t)a.x, (uint32_t)(a.x >> 32), (uint32_t)a.y, (uint32_t)(a.y >> 32));
-                        h1 = make_uint4((uint32_t)b.x, (uint32_t)(b.x >> 32), (uint32_t)b.y, (uint32_t)(b.y >> 32));
-                        ldg256_b64(nd + 2, a, b);
-                        l0 = make_uint4((uint32_t)a.x, (uint32_t)(a.x >> 32), (uint32_t)a.y, (uint32_t)(a.y >> 32));
-                        l1 = make_uint4((uint32_t)b.x, (uint32_t)(b.x >> 32), (uint32_t)b.y, (uint32_t)(b.y >> 32));
-                        ldg256_b64(nd + 4, a, b);
-                        u0 = make_uint4((uint32_t)a.x, (uint32_t)(a.x >> 32), (uint32_t)a.y, (uint32_t)(a.y >> 32));
-                        u1 = make_uint4((uint32_t)b.x, (uint32_t)(b.x >> 32), (uint32_t)b.y, (uint32_t)(b.y >> 32));
-                    }
+                    // the 20 words of the record (w8_node.h): h = w0..3, c = w4..7, l = w8..11, m = w12..15, u = w16..19
+                    const uint4* nd = nodes + (size_t)node * (W8_NODE_WORDS / 4);
+                    const uint4 h = ldg128_u32(nd), c = ldg128_u32(nd + 1), l = ldg128_u32(nd + 2), m = ldg128_u32(nd + 3), u = ldg128_u32(nd + 4);
                     if (COUNT) n_visits++;
                     const float limit = best + (best * 0.000244140625f + slack);
                     // B = scale * inv, A = fma(-2^15, B, (origin - o) * inv)
-                    const float Bx = __uint_as_float(h0.w) * inv.x, By = __uint_as_float(h1.x) * inv.y, Bz = __uint_as_float(h1.y) * inv.z;
-                    const float Ax = __fmaf_rn(-W8_DECODE_BIAS, Bx, (__uint_as_float(h0.x) - o.x) * inv.x);
-                    const float Ay = __fmaf_rn(-W8_DECODE_BIAS, By, (__uint_as_float(h0.y) - o.y) * inv.y);
-                    const float Az = __fmaf_rn(-W8_DECODE_BIAS, Bz, (__uint_as_float(h0.z) - o.z) * inv.z);
+                    const float Bx = __uint_as_float(W8_SCALE_BITS(h.w, 0)) * inv.x, By = __uint_as_float(W8_SCALE_BITS(h.w, 1)) * inv.y,
+                                Bz = __uint_as_float(W8_SCALE_BITS(h.w, 2)) * inv.z;
+                    const float Ax = __fmaf_rn(-W8_DECODE_BIAS, Bx, (__uint_as_float(h.x) - o.x) * inv.x);
+                    const float Ay = __fmaf_rn(-W8_DECODE_BIAS, By, (__uint_as_float(h.y) - o.y) * inv.y);
+                    const float Az = __fmaf_rn(-W8_DECODE_BIAS, Bz, (__uint_as_float(h.z) - o.z) * inv.z);
                     // near / far plane words per axis (slots 0..3 | 4..7): low planes are near iff d >= 0
+                    // qlo_x = c.z, c.w  qlo_y = l.x, l.y  qlo_z = l.z, l.w   qhi_x = m.z, m.w  qhi_y = u.x, u.y  qhi_z = u.z, u.w
                     const bool px = d.x >= 0.0f, py = d.y >= 0.0f, pz = d.z >= 0.0f;
-                    const uint32_t nx0 = px ? l0.x : u0.x, nx1 = px ? l0.y : u0.y, fx0 = px ? u0.x : l0.x, fx1 = px ? u0.y : l0.y;
-                    const uint32_t ny0 = py ? l0.z : u0.z, ny1 = py ? l0.w : u0.w, fy0 = py ? u0.z : l0.z, fy1 = py ? u0.w : l0.w;
-                    const uint32_t nz0 = pz ? l1.x : u1.x, nz1 = pz ? l1.y : u1.y, fz0 = pz ? u1.x : l1.x, fz1 = pz ? u1.y : l1.y;
+                    const uint32_t nx0 = px ? c.z : m.z, nx1 = px ? c.w : m.w, fx0 = px ? m.z : c.z, fx1 = px ? m.w : c.w;
+                    const uint32_t ny0 = py ? l.x : u.x, ny1 = py ? l.y : u.y, fy0 = py ? u.x : l.x, fy1 = py ? u.y : l.y;
+                    const uint32_t nz0 = pz ? l.z : u.z, nz1 = pz ? l.w : u.w, fz0 = pz ? u.z : l.z, fz1 = pz ? u.w : l.w;
                     uint32_t hits = 0u;
                     if (w8_slot_hit<0>(nx0, ny0, nz0, fx0, fy0, fz0, Bx, By, Bz, Ax, Ay, Az, limit, bias)) hits |= 1u;
                     if (w8_slot_hit<1>(nx0, ny0, nz0, fx0, fy0, fz0, Bx, By, Bz, Ax, Ay, Az, limit, bias)) hits |= 2u;
@@ -1028,20 +1023,20 @@ __device__ __forceinline__ void extend_w8(const SceneDev& sc, uint32_t n, uint32
                     if (w8_slot_hit<1>(nx1, ny1, nz1, fx1, fy1, fz1, Bx, By, Bz, Ax, Ay, Az, limit, bias)) hits |= 32u;
                     if (w8_slot_hit<2>(nx1, ny1, nz1, fx1, fy1, fz1, Bx, By, Bz, Ax, Ay, Az, limit, bias)) hits |= 64u;
                     if (w8_slot_hit<3>(nx1, ny1, nz1, fx1, fy1, fz1, Bx, By, Bz, Ax, Ay, Az, limit, bias)) hits |= 128u;
-                    const uint32_t imask = u1.z & 0xffu;
+                    const uint32_t imask = h.w >> 24;
                     const uint32_t inner = hits & imask;
                     uint32_t leaf = hits & ~imask;
                     // the rest of the group this node came from waits on the stack
                     if ((g_bits >> 8) != 0u) W8_PUSH(make_uint2(g_base, g_bits));
-                    g_base = h1.z;
+                    g_base = c.x;
                     g_bits = imask | ((uint32_t)s_perm[near_mask * 256u + inner] << 8);
                     // triangles of the hit leaf slots: meta byte = (count << 5) | offset
-                    t_base = h1.w;
+                    t_base = c.y;
                     t_mask = 0u;
                     while (leaf != 0u) {
                         const int s = __ffs(leaf) - 1;
                         leaf &= leaf - 1u;
-                        const uint32_t mb = ((s < 4 ? l1.z : l1.w) >> ((s & 3) * 8)) & 0xffu;
+                        const uint32_t mb = ((s < 4 ? m.x : m.y) >> ((s & 3) * 8)) & 0xffu;
                         t_mask |= ((1u << (mb >> 5)) - 1u) << (mb & 31u);
                     }
                     node = -1;
@@ -1109,11 +1104,11 @@ struct SurfaceHit {
 // barycentric denominators (P3/fsh:273-274) instead of P5's "+1e-7" (P5/fsh:206-207).
 __device__ __forceinline__ SurfaceHit surface_hit(const SceneDev& sc, vec3 o, vec3 d, float t, int tri, bool p3fudge, bool accel_space = false) {
     const float4* g = (accel_space ? sc.acc_tri_geo : sc.tri_geo) + (size_t)tri * 4;
-    float4 q0 = ldg4(g), q1 = ldg4(g + 1), q2 = ldg4(g + 2);
+    float4 q0 = ldg4(g), q1 = ldg4(g + 1), q2 = ldg4(g + 2), q3 = ldg4(g + 3);
     const float4* s = (accel_space ? sc.acc_tri_shade : sc.tri_shade) + (size_t)tri * 3;
     float4 m0 = ldg4(s), m1 = ldg4(s + 1), m2 = ldg4(s + 2);
-    vec3 p1 = f4xyz(q0), p2 = f4xyz(q1), p3 = f4xyz(q2);
-    vec3 Ng = ez_v3(q0.w, q1.w, q2.w);
+    vec3 p1 = f4xyz(q1), p2 = f4xyz(q2), p3 = f4xyz(q3);
+    vec3 Ng = f4xyz(q0);
     bool inside = ez_dot(Ng, d) > 0.0f;  // :175
     vec3 P = ez_add(o, ez_scale(d, t));
     float alpha, beta;

@@ -41,7 +41,7 @@
 
 struct SceneDev {
     const float4* nodes;      // 4 float4 per inner node
-    const float4* tri_geo;    // 4 float4 per triangle
+    const float4* tri_geo;    // 4 float4 per triangle: (N, d0), (p1, 0), (p2, 0), (p3, 0)
     const float4* tri_shade;  // 3 float4 per triangle
     const float4* materials;  // 5 float4 per material
     const float* hdr;         // W*H*3 or null
@@ -55,7 +55,7 @@ struct SceneDev {
     const uint32_t* ref_to_acc;    // reference triangle index -> accel order
     const float4* acc_tri_shade;   // tri_shade in accel order (shading reads the arrays traversal keeps hot in L2)
     const int* acc_tri_leaf;       // reference leaf (slot in leaf_box) of every triangle, accel order
-    const uint4* w8_nodes;         // the tree as 8-wide nodes with 8-bit quantised child boxes (96 B records, w8_node.h); null = none
+    const uint4* w8_nodes;         // the tree as 8-wide nodes with 8-bit quantised child boxes (80 B records, w8_node.h); null = none
     int w8_near_bit[3];            // significance of axis a in the slot index (octant order)
     int w8_stack_entries;          // per-lane stack entries kept in shared memory (>= depth of the 8-wide tree, or the smem cap)
     int w8_tri_weight;             // step vote of the W8 kernels: triangle step iff w8_tri_weight * lanes_with_triangles >= lanes_with_a_node (env EZRT_TRI_W)

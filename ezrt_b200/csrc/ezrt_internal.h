@@ -81,7 +81,7 @@ int ezrt_build_accel_device(const float* d_tris, int n_tris, int leaf_n, std::ve
                             int* levels);
 
 // scene_prep.cu (current device): per-triangle records from the Triangle_encoded array in device memory.
-// d_geo: 4 float4 per triangle (p1|N.x, p2|N.y, p3|N.z, d0), d_shade: 3 float4 (n1|material id, n2, n3); info: scene bounds and
+// d_geo: 4 float4 per triangle (N|d0, p1, p2, p3), d_shade: 3 float4 (n1|material id, n2, n3); info: scene bounds and
 // the de-duplicated material table (ids in order of first occurrence).
 struct EzrtPrepInfo {
     float max_abs = 0.0f, bmin[3] = {0, 0, 0}, bmax[3] = {0, 0, 0};

@@ -901,7 +901,7 @@ __global__ void k_trace_finish(SceneDev sc, int n, PathQueue q, int p3fudge, int
         P = s.P;
         N = s.N;
         const float4* g = (accel_space ? sc.acc_tri_geo : sc.tri_geo) + (size_t)ht * 4;
-        vec3 Ng = ez_v3(ldg4(g).w, ldg4(g + 1).w, ldg4(g + 2).w);
+        vec3 Ng = f4xyz(ldg4(g));
         ins = ez_dot(Ng, rdv) > 0.0f;
     }
     inside[i] = ins;

@@ -61,10 +61,10 @@ __global__ void k_records(const float* __restrict__ raw, int n, float4* __restri
         }
         const ez_vec3 N = ez_normalize(ez_cross(ez_sub(p2, p1), ez_sub(p3, p1)));   // hitTriangle, P5/fsh:172
         const float d0 = ez_dot(N, p1);                                              // P5/fsh:184
-        geo[(size_t)i * 4 + 0] = make_float4(p1.x, p1.y, p1.z, N.x);
-        geo[(size_t)i * 4 + 1] = make_float4(p2.x, p2.y, p2.z, N.y);
-        geo[(size_t)i * 4 + 2] = make_float4(p3.x, p3.y, p3.z, N.z);
-        geo[(size_t)i * 4 + 3] = make_float4(d0, 0.0f, 0.0f, 0.0f);
+        geo[(size_t)i * 4 + 0] = make_float4(N.x, N.y, N.z, d0);   // first: the distance checks of tri_test_t read only this
+        geo[(size_t)i * 4 + 1] = make_float4(p1.x, p1.y, p1.z, 0.0f);
+        geo[(size_t)i * 4 + 2] = make_float4(p2.x, p2.y, p2.z, 0.0f);
+        geo[(size_t)i * 4 + 3] = make_float4(p3.x, p3.y, p3.z, 0.0f);
         shade[(size_t)i * 3 + 0] = make_float4(v[9], v[10], v[11], 0.0f);
         shade[(size_t)i * 3 + 1] = make_float4(v[12], v[13], v[14], 0.0f);
         shade[(size_t)i * 3 + 2] = make_float4(v[15], v[16], v[17], 0.0f);

@@ -7,22 +7,23 @@
 // deferral rule whether that is also the shader's answer), so its tree is free in shape, order and box
 // precision as long as every child box is a SUPERSET of the exact (2*delta-inflated) box of its sub-tree:
 //
-//   record = 24 words = 96 bytes, 32-byte aligned, read with three 256-bit loads
+//   record = 20 words = 80 bytes, 16-byte aligned, read with five 128-bit loads
 //     w0..2   origin.xyz (float)      one quantisation step below the lowest child plane of the node
-//     w3..5   scale.xyz  (float)      a power of two per axis, >= W8 minimum step of the scene (fp error bound below)
-//     w6      child_base              node index of the first inner child; inner children are numbered consecutively
+//     w3      ex | ey << 8 | ez << 16 | imask << 24
+//             ex, ey, ez              biased IEEE exponents of the per-axis scale: scale_a = as_float(e_a << 23), a power
+//                                     of two in [2^-126, 2^127], >= W8 minimum step of the scene (fp error bound below)
+//             imask                   bit s: slot s holds an inner child
+//     w4      child_base              node index of the first inner child; inner children are numbered consecutively
 //                                     in slot order: child of slot s = child_base + popc(imask & ((1 << s) - 1))
-//     w7      tri_base                first triangle (accel order) of the node's leaf children, consecutive in slot order
-//     w8..13  qlo_x[8] qlo_y[8] qlo_z[8]   low planes of the eight slots, one byte each (slot s = byte s)
-//     w14,15  meta[8]                 leaf slot: (count << 5) | offset of its first triangle from tri_base (count 1..4,
+//     w5      tri_base                first triangle (accel order) of the node's leaf children, consecutive in slot order
+//     w6..11  qlo_x[8] qlo_y[8] qlo_z[8]   low planes of the eight slots, one byte each (slot s = byte s)
+//     w12,13  meta[8]                 leaf slot: (count << 5) | offset of its first triangle from tri_base (count 1..4,
 //                                     offset 0..28); inner or empty slot: 0
-//     w16..21 qhi_x[8] qhi_y[8] qhi_z[8]   high planes
-//     w22     imask                   bit s: slot s holds an inner child
-//     w23     unused (0)
+//     w14..19 qhi_x[8] qhi_y[8] qhi_z[8]   high planes
 //   plane value = origin + q * scale; an empty slot has qlo = 255, qhi = 0 (inverted, never hit).
 //
 // Decode (one FMA per plane, same formula on host model and device):
-//     B = scale * inv_d            (exact: scale is a power of two)
+//     B = as_float(e << 23) * inv_d   (= scale * inv_d, exact: scale is a power of two)
 //     A = fma(-2^15, B, (origin - o) * inv_d)
 //     f = as_float(0x47000000 | q << 8) = 2^15 + q        (one PRMT on the device: the byte goes to mantissa bits 8..15)
 //     t = fma(f, B, A)             = (origin + q*scale - o) * inv_d up to rounding (the 2^15 * B terms cancel exactly)
@@ -44,8 +45,8 @@
 
 #include <stdint.h>
 
-#define W8_NODE_WORDS 24
-#define W8_NODE_BYTES 96
+#define W8_NODE_WORDS 20
+#define W8_NODE_BYTES 80
 #define W8_MAX_LEAF_TRIS 4            // triangles per leaf slot (meta count field)
 #define W8_MAX_NODE_TRIS 32           // triangles of all leaf slots of one node (bits of the triangle mask)
 #define W8_SLACK_STEPS 0.25                  // outward slack of the stored planes, in quantisation steps
@@ -59,12 +60,14 @@
 #define W8_LOCAL_STACK 48                    // stack entries beyond the shared-memory part (local memory)
 
 #define W8_W_ORIGIN 0
-#define W8_W_SCALE 3
-#define W8_W_CHILD_BASE 6
-#define W8_W_TRI_BASE 7
-#define W8_W_QLO 8
-#define W8_W_META 14
-#define W8_W_QHI 16
-#define W8_W_IMASK 22
+#define W8_W_EXP_IMASK 3
+#define W8_W_CHILD_BASE 4
+#define W8_W_TRI_BASE 5
+#define W8_W_QLO 6
+#define W8_W_META 12
+#define W8_W_QHI 14
+
+// bits of the scale of axis a (0..2) from word W8_W_EXP_IMASK: the exponent byte moved to the float's exponent field
+#define W8_SCALE_BITS(w, a) ((((uint32_t)(w) >> (8 * (a))) & 0xffu) << 23)
 
 #endif

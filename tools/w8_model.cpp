@@ -22,13 +22,15 @@
 
 struct TriRec { ez_vec3 p1, p2, p3, N; float d0; };
 
-// tri_test_t<TIES> of device_functions.cuh (hitTriangle P5/fsh:160-217 on the repacked record)
-static int tri_test(const TriRec& r, ez_vec3 o, ez_vec3 d, float best, float& tout) {
+// tri_test_t<TIES> of device_functions.cuh (hitTriangle P5/fsh:160-217 on the repacked record); *passed: the test got past the
+// distance checks, i.e. the device loaded the vertices
+static int tri_test(const TriRec& r, ez_vec3 o, ez_vec3 d, float best, float& tout, bool* passed = nullptr) {
     float nd = ez_dot(r.N, d);
     if (ez_abs(nd) < 0.00001f) return 0;
     float t = EZ_DIV(r.d0 - ez_dot(o, r.N), nd);
     if (t < 0.0005f) return 0;
     if (!(t <= best)) return 0;
+    if (passed) *passed = true;
     ez_vec3 P = ez_add(o, ez_scale(d, t));
     float s1 = ez_dot(ez_cross(ez_sub(r.p2, r.p1), ez_sub(P, r.p1)), r.N);
     float s2 = ez_dot(ez_cross(ez_sub(r.p3, r.p2), ez_sub(P, r.p2)), r.N);
@@ -74,7 +76,7 @@ int main(int argc, char** argv) {
     const int rc = ezrt_build_w8(an, order, pad, maxc, axis_bit, w8);
     if (rc) { fprintf(stderr, "ezrt_build_w8 failed: %d\n", rc); return 1; }
     printf("binary nodes %zu, 8-wide nodes %d (%.1f MB), depth %d, mean fill %.2f, axis bits x%d y%d z%d\n", an.size(), w8.n_nodes,
-           w8.n_nodes * 96.0 / 1e6, w8.depth, (double)w8.n_children / w8.n_nodes, axis_bit[0], axis_bit[1], axis_bit[2]);
+           w8.n_nodes * (double)W8_NODE_BYTES / 1e6, w8.depth, (double)w8.n_children / w8.n_nodes, axis_bit[0], axis_bit[1], axis_bit[2]);
     {   // the 4-wide collapse the default kernel uses (same dynamic programme, width 4): every triangle in exactly one leaf of <= 4
         EzrtCollapse c4;
         if (c4.build(an, 4, W8_MAX_LEAF_TRIS, 1.0, 0.3) != 0) { fprintf(stderr, "4-wide collapse failed\n"); return 1; }
@@ -116,7 +118,7 @@ int main(int argc, char** argv) {
     // W8M_GMIN=1 keep the smallest entry distance of a pushed group and drop the group at pop when it is beyond the best hit;
     // W8M_EXACT=1 exact child boxes instead of the quantised ones (how much the 8-bit planes cost)
     const bool x_sort = getenv("W8M_SORT") && atoi(getenv("W8M_SORT")), x_gmin = getenv("W8M_GMIN") && atoi(getenv("W8M_GMIN"));
-    double nv[3] = {0, 0, 0}, nt[3] = {0, 0, 0}, npush[3] = {0, 0, 0}, cntk[3] = {0, 0, 0};
+    double nv[3] = {0, 0, 0}, nt[3] = {0, 0, 0}, npass[3] = {0, 0, 0}, npush[3] = {0, 0, 0}, cntk[3] = {0, 0, 0};
     long mismatch = 0, skipped = 0, ties = 0;
     int max_sp = 0;
 #pragma omp parallel for schedule(dynamic, 256) reduction(+ : mismatch, skipped, ties) reduction(max : max_sp)
@@ -145,7 +147,7 @@ int main(int argc, char** argv) {
         int sp = 0;
         uint32_t g_base = 0, g_bits = 0;   // bits: imask (low 8) | hits in priority positions (bits 8..15)
         int node = 0;
-        double my_nv = 0, my_nt = 0, my_push = 0;
+        double my_nv = 0, my_nt = 0, my_pass = 0, my_push = 0;
         while (true) {
             uint32_t t_base = 0, t_mask = 0;
             if (node >= 0) {
@@ -155,15 +157,16 @@ int main(int argc, char** argv) {
                 float A[3], B[3];
                 for (int a = 0; a < 3; a++) {
                     float org, sc;
+                    const uint32_t sc_bits = W8_SCALE_BITS(w[W8_W_EXP_IMASK], a);
                     memcpy(&org, &w[W8_W_ORIGIN + a], 4);
-                    memcpy(&sc, &w[W8_W_SCALE + a], 4);
+                    memcpy(&sc, &sc_bits, 4);
                     B[a] = sc * inv[a];
                     A[a] = fmaf(-W8_DECODE_BIAS, B[a], (org - oo[a]) * inv[a]);
                 }
                 const uint8_t* qlo = (const uint8_t*)&w[W8_W_QLO];
                 const uint8_t* qhi = (const uint8_t*)&w[W8_W_QHI];
                 const uint8_t* meta = (const uint8_t*)&w[W8_W_META];
-                const uint32_t imask = w[W8_W_IMASK] & 255u;
+                const uint32_t imask = w[W8_W_EXP_IMASK] >> 24;
                 uint32_t hits8 = 0;
                 float tmin_s[8];
                 for (int s = 0; s < 8; s++) {
@@ -204,7 +207,9 @@ int main(int argc, char** argv) {
                 t_mask &= t_mask - 1;
                 my_nt += 1;
                 float t;
-                const int h = tri_test(rec[t_base + k], o, d, best, t);
+                bool passed = false;
+                const int h = tri_test(rec[t_base + k], o, d, best, t, &passed);
+                my_pass += passed ? 1 : 0;
                 if (h == 2) tie = true;
                 else if (h == 1) { best = t; tie = false; }
             }
@@ -273,12 +278,17 @@ int main(int argc, char** argv) {
         }
         if (memcmp(&want, &best, 4) != 0) mismatch++;
 #pragma omp critical
-        { nv[kind] += my_nv; nt[kind] += my_nt; npush[kind] += my_push; cntk[kind] += 1; }
+        { nv[kind] += my_nv; nt[kind] += my_nt; npass[kind] += my_pass; npush[kind] += my_push; cntk[kind] += 1; }
     }
     const char* names[3] = {"camera", "bounce", "shadow"};
     for (int k = 0; k < 3; k++)
         if (cntk[k] > 0)
-            printf("%s rays %.0f: %.2f node visits, %.2f triangle tests, %.2f pushes per ray\n", names[k], cntk[k], nv[k] / cntk[k], nt[k] / cntk[k], npush[k] / cntk[k]);
+            printf("%s rays %.0f: %.2f node visits, %.2f triangle tests, %.2f pushes per ray; %.3f of the tests pass the distance checks\n", names[k], cntk[k],
+                   nv[k] / cntk[k], nt[k] / cntk[k], npush[k] / cntk[k], nt[k] > 0 ? npass[k] / nt[k] : 0.0);
+    for (int k = 0; k < 3; k++)   // 128-bit loads of the device kernel: five per node visit, one per triangle test and three per vertex stage
+        if (cntk[k] > 0)
+            printf("%s rays: %.1f 16-byte loads per ray (%.1f with the 96-byte node and the 64-byte triangle loaded whole)\n", names[k],
+                   (W8_NODE_BYTES / 16 * nv[k] + nt[k] + 3 * npass[k]) / cntk[k], (6 * nv[k] + 4 * nt[k]) / cntk[k]);
     printf("max stack depth %d, rays left to the exact kernel %ld, rays with a tie %ld\n", max_sp, skipped, ties);
     printf("closest-hit distances differing from %s: %ld of %d rays\n", brute ? "brute force" : "the exact-box traversal", mismatch, NR);
     return mismatch == 0 ? 0 : 3;
