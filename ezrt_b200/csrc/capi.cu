@@ -612,7 +612,7 @@ int ezrt_scene_create(int device, const float* tris, int n_triangles, const floa
     d.w8_stack_entries = std::max(1, std::min(w8_depth, EZRT_W8_SMEM_STACK));
     d.w8_origin_limit = W8_ORIGIN_LIMIT_REL * max_abs;
     d.w8_decode_bits = W8_DECODE_BITS;
-    d.w8_tri_weight = 2;
+    d.w8_tri_weight = 1;   // cooperative triangle step: 1 over 2 is +1 % on C3 and C4 (H100, DESIGN.md section 6)
     if (const char* e = getenv("EZRT_TRI_W")) d.w8_tri_weight = std::max(1, std::min(64, atoi(e)));
     d.acc_tri_geo = (const float4*)((const char*)sc->acc_hot.p + acc_nodes_bytes);
     d.acc_tri_ref = (const uint32_t*)sc->acc_tri_ref.p;

@@ -849,7 +849,8 @@ __device__ __forceinline__ void extend_persistent(const SceneDev& sc, const Tree
 // five 128-bit loads; layout, decode arithmetic and error bound in w8_node.h), children visited in octant order
 // from a hit bit mask -- no distance sort, at most one stack push per node visit -- and a per-lane stack of
 // (child base | slot masks) groups in SHARED memory at [entry][thread].  The triangles of all hit leaf slots of a node
-// are collected in a bit mask and tested one per lane per iteration in a separate warp-synchronous phase.
+// are collected in a bit mask; a triangle step tests up to 32 of the warp's pending triangles, one per lane, whichever
+// lanes they belong to.
 // Like the 4-wide kernel it only has to find the globally closest accepted triangle (and notice ties); what it
 // cannot decide exactly goes to io.defer() (DESIGN.md section 4).  Measured ceiling for its access pattern on an H100: at
 // most one divergent 128-bit load per lane per SM-cycle (tools/gather_bench.cu, DESIGN.md section 4).
@@ -879,6 +880,19 @@ __device__ __forceinline__ bool w8_slot_hit(uint32_t nx, uint32_t ny, uint32_t n
     return tmin <= tmax;
 }
 
+// position of the r-th lowest set bit of m (r < popc(m))
+__device__ __forceinline__ int nth_set_bit(uint32_t m, int r) {
+    int pos = 0, c = __popc(m & 0xffffu);
+    if (r >= c) { r -= c; m >>= 16; pos += 16; }
+    c = __popc(m & 0xffu);
+    if (r >= c) { r -= c; m >>= 8; pos += 8; }
+    c = __popc(m & 0xfu);
+    if (r >= c) { r -= c; m >>= 4; pos += 4; }
+    c = __popc(m & 0x3u);
+    if (r >= c) { r -= c; m >>= 2; pos += 2; }
+    return pos + ((r >= (int)(m & 1u)) ? 1 : 0);
+}
+
 // s_perm: 8 x 256 bytes in shared memory, s_perm[m * 256 + x] = the bits of x moved from position s to position s ^ m
 // stack : uint2 [entries][blockDim.x] in shared memory
 template <bool ANYHIT, bool COUNT, class RayIO>
@@ -896,6 +910,8 @@ __device__ __forceinline__ void extend_w8(const SceneDev& sc, uint32_t n, uint32
     const uint4* __restrict__ nodes = sc.w8_nodes;
     const float origin_limit = sc.w8_origin_limit;
     const uint32_t bias = sc.w8_decode_bits;   // = W8_DECODE_BITS; a run-time value so that ptxas keeps it in a register (see w8_plane)
+    __shared__ unsigned char s_owner_all[EZRT_EXTEND_MAX_THREADS];   // triangle step: first tested pair -> owner lane, 32 bytes per warp
+    unsigned char* const s_owner = s_owner_all + (threadIdx.x & ~31u);
 
     int ray = -1;                 // index of the ray this lane traces, -1 = idle
     int node = -1;                // next node to visit, -1 = none (waiting for the triangle phase, or idle)
@@ -907,7 +923,7 @@ __device__ __forceinline__ void extend_w8(const SceneDev& sc, uint32_t n, uint32
     uint32_t near_mask = 0;       // bit of axis a set iff d_a >= 0 (children towards -a come first)
     uint32_t g_base = 0, g_bits = 0;   // current group: first inner child | imask (bits 0..7), unvisited hit slots in priority positions (bits 8..15)
     uint32_t t_base = 0, t_mask = 0;   // pending triangles of the node just visited
-    unsigned long long n_visits = 0, n_tests = 0;
+    uint32_t n_visits = 0, n_tests = 0;   // per lane; 32 bits keep the COUNT instantiations within 64 registers
     bool exhausted = false;
     uint32_t chunk_pos = 0, chunk_end = 0;
     const uint32_t chunk = (uint32_t)sc.work_chunk;
@@ -983,19 +999,19 @@ __device__ __forceinline__ void extend_w8(const SceneDev& sc, uint32_t n, uint32
         }
         // ---------------- traverse: every iteration the warp runs ONE of two steps, chosen by a vote ----------------
         //   node step     : every lane holding a node visits it (five 128-bit loads, eight slab tests; ~200 instructions)
-        //   triangle step : every lane with pending triangles tests one (one 128-bit load, three more past the distance checks; ~100 instructions)
+        //   triangle step : the warp tests up to 32 pending (lane, triangle) pairs, one per lane (one 128-bit load, three more
+        //                   past the distance checks, plus the shuffles that hand out the pairs)
         // A lane with pending triangles cannot take a node step (its next node depends on them), so the warp takes the
-        // triangle step as soon as  tri_weight * (lanes with triangles) >= (lanes with a node)  -- the step that serves
-        // more lanes per instruction (tri_weight ~ cost ratio of the two steps, env EZRT_TRI_W).
+        // triangle step as soon as  tri_weight * min(pending pairs, 32) >= (lanes with a node).  A node step costs about two
+        // triangle steps, but a triangle step also frees its lanes for the next node step: 1 measured best (env EZRT_TRI_W).
         const int tri_weight = leaf_thresh;
         unsigned busy;
         do {
             const bool at_node = node >= 0;
-            const bool has_tri = t_mask != 0u;
             const unsigned m_node = __ballot_sync(FULL, at_node);
-            const unsigned m_tri = __ballot_sync(FULL, has_tri);
-            if ((m_node | m_tri) == 0u) { busy = 0u; break; }
-            if (m_node != 0u && tri_weight * __popc(m_tri) < __popc(m_node)) {
+            const uint32_t pairs = __reduce_add_sync(FULL, (uint32_t)__popc(t_mask));
+            if (m_node == 0u && pairs == 0u) { busy = 0u; break; }
+            if (m_node != 0u && tri_weight * (int)min(pairs, 32u) < __popc(m_node)) {
                 if (at_node) {
                     // the 20 words of the record (w8_node.h): h = w0..3, c = w4..7, l = w8..11, m = w12..15, u = w16..19
                     const uint4* nd = nodes + (size_t)node * (W8_NODE_WORDS / 4);
@@ -1042,22 +1058,97 @@ __device__ __forceinline__ void extend_w8(const SceneDev& sc, uint32_t n, uint32
                     node = -1;
                     if (t_mask == 0u) select_next();
                 }
-            } else if (has_tri) {
-                const int k = __ffs(t_mask) - 1;
-                t_mask &= t_mask - 1u;
-                const int tri = (int)t_base + k;
-                if (COUNT) n_tests++;
-                float t;
-                const int r = tri_test_t<true>(sc.acc_tri_geo + (size_t)tri * 4, o, d, best, t, tri_na);
-                if (r == 2) {
-                    tie = true;              // a second triangle at exactly the best distance: visit order would decide
-                } else if (r == 1) {
-                    best = t;
-                    best_tri = tri;
-                    tie = false;
-                    if (ANYHIT) { t_mask = 0u; g_bits = 0u; sp = 0; }   // any accepted hit ends a shadow ray
+            } else {
+                // Cooperative triangle step.  The warp's pending (lane, triangle) pairs are numbered lane by lane, lowest triangle
+                // first; lane j tests pair j with its owner's ray and best distance (by shuffle).  Pairs from 32 on stay pending.
+                // Each owner then applies its pairs' results with the semantics of testing them one after the other in that
+                // order (tri_test_t<true>: t <= best accepted, t == best reported as a tie):
+                //   closest hit: m = the least accepted t.  m < best: best = m, best_tri = the first triangle holding m, tie iff
+                //   a second one holds it (the serial order clears `tie` at the first holder's strict improvement and sets it
+                //   again at the second).  m == best: tie.
+                //   ANYHIT: the first strict hit ends the ray (with `tie` cleared); without one, a hit at exactly best is a tie.
+                // The pairs are tested against the owner's best from before the step, not the best after the earlier pairs.  That
+                // changes no result: a stale best is never smaller, so every triangle the serial order accepts is still accepted
+                // at the same t; an extra one lies beyond the best the serial order had reached at it, so strictly above m: it
+                // changes neither the minimum nor its holders.  ANYHIT rays keep best until their first strict hit: nothing is stale.
+                const uint32_t cnt = (uint32_t)__popc(t_mask);
+                uint32_t incl = cnt;                               // inclusive prefix sum of the pending counts
+#pragma unroll
+                for (int s = 1; s < 32; s <<= 1) {
+                    const uint32_t v = __shfl_up_sync(FULL, incl, s);
+                    if (lane >= s) incl += v;
                 }
-                if (t_mask == 0u) select_next();
+                const uint32_t first = incl - cnt;                 // this lane's pairs are numbered first, first + 1, ...
+                const bool owns = cnt != 0u && first < 32u;        // ... and some of them are tested in this step
+                const unsigned starts = __reduce_or_sync(FULL, owns ? 1u << first : 0u);
+                __syncwarp();
+                if (owns) s_owner[first] = (unsigned char)lane;   // the first lane testing an owner's pairs -> owner
+                __syncwarp();
+                const int start = 31 - __clz(starts & (FULL >> (31 - lane)));   // first lane of the owner this lane tests for
+                const bool act = (uint32_t)lane < pairs;
+                const int src = act ? (int)s_owner[start] : lane;
+                vec3 ro, rd;
+                ro.x = __shfl_sync(FULL, o.x, src); ro.y = __shfl_sync(FULL, o.y, src); ro.z = __shfl_sync(FULL, o.z, src);
+                rd.x = __shfl_sync(FULL, d.x, src); rd.y = __shfl_sync(FULL, d.y, src); rd.z = __shfl_sync(FULL, d.z, src);
+                const float rbest = __shfl_sync(FULL, best, src);
+                const uint32_t rmask = __shfl_sync(FULL, t_mask, src);
+                const int k = nth_set_bit(rmask, lane - start);
+                const int tri = (int)__shfl_sync(FULL, t_base, src) + k;
+                float t = 0.0f;
+                int r = 0;
+                if (act) {
+                    if (COUNT) n_tests++;
+                    r = tri_test_t<true>(sc.acc_tri_geo + (size_t)tri * 4, ro, rd, rbest, t, tri_na);
+                }
+                const uint32_t taken = owns ? min(cnt, 32u - first) : 0u;   // this lane's pairs tested in this step ...
+                const unsigned seg = (taken == 32u) ? FULL : ((1u << taken) - 1u) << (first & 31u);   // ... by these lanes
+                bool stop = false;
+                if (ANYHIT) {
+                    const unsigned strict = __ballot_sync(FULL, r == 1) & seg, level = __ballot_sync(FULL, r == 2) & seg;
+                    const int p = strict ? __ffs(strict) - 1 : lane;
+                    const float tw = __shfl_sync(FULL, t, p);
+                    const int triw = __shfl_sync(FULL, tri, p);
+                    if (strict) {
+                        best = tw;
+                        best_tri = triw;
+                        tie = false;
+                        stop = true;
+                    } else if (level) {
+                        tie = true;
+                    }
+                } else {
+                    // per-owner minimum of the t bits (t > 0, so bit order = value order): a suffix minimum within each owner's
+                    // run of lanes leaves the run's minimum in its first lane
+                    const unsigned tb = (r != 0) ? __float_as_uint(t) : 0xffffffffu;
+                    const unsigned above = starts & ~(FULL >> (31 - lane));
+                    const int end = above ? __ffs(above) - 1 : (int)min(pairs, 32u);
+                    unsigned mn = tb;
+#pragma unroll
+                    for (int s = 1; s < 32; s <<= 1) {
+                        const unsigned v = __shfl_down_sync(FULL, mn, s);
+                        if (lane + s < end) mn = min(mn, v);
+                    }
+                    const unsigned run_min = __shfl_sync(FULL, mn, start);
+                    const unsigned win = __ballot_sync(FULL, act && tb != 0xffffffffu && tb == run_min) & seg;   // holders of the minimum
+                    const int p = win ? __ffs(win) - 1 : lane;   // the first holder
+                    const int triw = __shfl_sync(FULL, tri, p);
+                    const float tn = __uint_as_float(__shfl_sync(FULL, tb, p));
+                    if (win) {
+                        if (tn < best) {
+                            best = tn;
+                            best_tri = triw;
+                            tie = __popc(win) > 1;
+                        } else {
+                            tie = true;   // tn == best
+                        }
+                    }
+                }
+                const int k_last = __shfl_sync(FULL, k, 31);   // the last pair tested: its owner keeps the triangles above it
+                if (owns) {
+                    t_mask = (taken < cnt && !stop) ? t_mask & ~((2u << k_last) - 1u) : 0u;
+                    if (stop) { g_bits = 0u; sp = 0; }   // any accepted hit ends a shadow ray
+                    if (t_mask == 0u) select_next();
+                }
             }
             busy = __ballot_sync(FULL, ray >= 0);
         } while (busy != 0u && (exhausted || __popc(busy) >= refill_thresh));
@@ -1065,8 +1156,8 @@ __device__ __forceinline__ void extend_w8(const SceneDev& sc, uint32_t n, uint32
 #undef W8_PUSH
 #undef W8_POP
     if (COUNT) {
-        atomicAdd(counts.node_visits, n_visits);
-        atomicAdd(counts.tri_tests, n_tests);
+        atomicAdd(counts.node_visits, (unsigned long long)n_visits);
+        atomicAdd(counts.tri_tests, (unsigned long long)n_tests);
     }
 }
 

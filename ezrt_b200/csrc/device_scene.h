@@ -58,7 +58,7 @@ struct SceneDev {
     const uint4* w8_nodes;         // the tree as 8-wide nodes with 8-bit quantised child boxes (80 B records, w8_node.h); null = none
     int w8_near_bit[3];            // significance of axis a in the slot index (octant order)
     int w8_stack_entries;          // per-lane stack entries kept in shared memory (>= depth of the 8-wide tree, or the smem cap)
-    int w8_tri_weight;             // step vote of the W8 kernels: triangle step iff w8_tri_weight * lanes_with_triangles >= lanes_with_a_node (env EZRT_TRI_W)
+    int w8_tri_weight;             // step vote of the W8 kernels: triangle step iff w8_tri_weight * min(pending_triangles, 32) >= lanes_with_a_node (env EZRT_TRI_W)
     uint32_t w8_decode_bits;       // W8_DECODE_BITS (passed as data: see w8_plane in device_functions.cuh)
     float w8_origin_limit;         // rays starting further out than this (any |coordinate|) go to the exact kernel (decode error bound)
     const float4* acc_wide_nodes;  // 4-wide nodes with exact boxes (128 B records): the accel form of scenes below 2^16 triangles (W8 above)

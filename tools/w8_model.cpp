@@ -2,7 +2,8 @@
 // Builds the tree with the PRODUCT builders (ezrt_build_accel + ezrt_build_w8), then walks it with exactly the decode
 // arithmetic and visit rule of the device kernel (w8_node.h, device_functions.cuh: octant-ordered hit masks, group
 // stack, triangle masks) and checks every ray's closest-hit distance against brute force over all triangles
-// (small scenes) or against the exact-box traversal of the binary tree (large scenes).  Prints work counts per ray.
+// (small scenes) or against the exact-box traversal of the binary tree (large scenes).  Prints work counts per ray, the
+// triangles pending per node visit and a warp-level replay of the kernel's schedule (serial vs cooperative triangle step).
 //   g++ -O2 -std=c++17 -fopenmp -ffp-contract=off -mfma -Iinclude -Iezrt_b200/csrc tools/w8_model.cpp \
 //       ezrt_b200/csrc/host_scene.cpp ezrt_b200/csrc/accel_w8.cpp ezrt_b200/csrc/errors.cpp -o build/w8_model
 //   build/w8_model tris.f32 n_tris rays.f32 [brute]        rays: 7-float records (o, d, kind) as oracle_set_ray_dump writes
@@ -39,6 +40,67 @@ static int tri_test(const TriRec& r, ez_vec3 o, ez_vec3 d, float best, float& to
     if (!(r1 || r2)) return 0;
     tout = t;
     return (t == best) ? 2 : 1;
+}
+
+// Warp-level replay of extend_w8's schedule (device_functions.cuh) for rays in queue order: a warp takes `chunk` rays at a
+// time, refills its idle lanes when fewer than `refill` are busy, and every iteration votes for ONE step -- a node step
+// (every lane holding a node visits it) or a triangle step.  Serial triangle step: one test per lane with pending triangles;
+// cooperative: up to 32 (lane, triangle) pairs of all lanes, lowest lane first.  Vote: triangle step iff
+// tri_w * (lanes served by a triangle step) >= lanes holding a node.  trace[r] = triangles pending after each node visit of ray r.
+struct Replay { double node_steps = 0, tri_steps = 0, node_lanes = 0, tri_lanes = 0; };
+static Replay replay(const std::vector<const std::vector<uint8_t>*>& trace, bool coop, int tri_w, int refill, int chunk) {
+    Replay R;
+    const size_t n = trace.size();
+    int ray[32], vi[32], pend[32];
+    for (int l = 0; l < 32; l++) ray[l] = -1;
+    size_t next = 0, chunk_pos = 0, chunk_end = 0;
+    bool exhausted = false;
+    auto after = [&](int l) { if (pend[l] == 0 && vi[l] == (int)trace[ray[l]]->size()) ray[l] = -1; };   // nothing left: ray done
+    while (true) {
+        int need = 0;
+        for (int l = 0; l < 32; l++) need += ray[l] < 0;
+        if (need && !exhausted) {
+            if (chunk_pos >= chunk_end) {
+                chunk_pos = next;
+                next += chunk;
+                chunk_end = std::min(chunk_pos + chunk, n);
+                if (chunk_pos >= n) exhausted = true;
+            }
+            if (!exhausted) {
+                size_t idx = chunk_pos;
+                for (int l = 0; l < 32; l++)
+                    if (ray[l] < 0 && idx < chunk_end) { ray[l] = (int)idx++; vi[l] = 0; pend[l] = 0; }
+                chunk_pos = std::min(chunk_pos + need, chunk_end);
+            }
+        }
+        int busy = 0;
+        for (int l = 0; l < 32; l++) busy += ray[l] >= 0;
+        if (!busy) { if (exhausted) break; continue; }
+        do {
+            int nn = 0, nt = 0, pairs = 0;
+            for (int l = 0; l < 32; l++)
+                if (ray[l] >= 0) { nn += pend[l] == 0; nt += pend[l] > 0; pairs += pend[l]; }
+            const int served = coop ? std::min(pairs, 32) : nt;
+            if (nn && tri_w * served < nn) {
+                R.node_steps++; R.node_lanes += nn;
+                for (int l = 0; l < 32; l++)
+                    if (ray[l] >= 0 && pend[l] == 0) { pend[l] = (*trace[ray[l]])[vi[l]++]; after(l); }
+            } else {
+                R.tri_steps++; R.tri_lanes += served;
+                int slots = 32;
+                for (int l = 0; l < 32; l++)
+                    if (ray[l] >= 0 && pend[l] > 0) {
+                        const int take = coop ? std::min(pend[l], slots) : 1;
+                        slots -= take;
+                        pend[l] -= take;
+                        after(l);
+                    }
+            }
+            busy = 0;
+            for (int l = 0; l < 32; l++) busy += ray[l] >= 0;
+        } while (busy && (exhausted || busy >= refill));
+    }
+    return R;
 }
 
 int main(int argc, char** argv) {
@@ -121,6 +183,8 @@ int main(int argc, char** argv) {
     double nv[3] = {0, 0, 0}, nt[3] = {0, 0, 0}, npass[3] = {0, 0, 0}, npush[3] = {0, 0, 0}, cntk[3] = {0, 0, 0};
     long mismatch = 0, skipped = 0, ties = 0;
     int max_sp = 0;
+    std::vector<std::vector<uint8_t>> trace(NR);   // triangles pending after each node visit, for the warp replay
+    std::vector<int> ray_kind(NR, -1);              // -1: left to the exact kernel
 #pragma omp parallel for schedule(dynamic, 256) reduction(+ : mismatch, skipped, ties) reduction(max : max_sp)
     for (int r = 0; r < NR; r++) {
         const float* R = &rays[(size_t)r * 7];
@@ -133,6 +197,7 @@ int main(int argc, char** argv) {
             skipped++;  // the kernel hands these to the exact traversal
             continue;
         }
+        ray_kind[r] = kind;
         const float slack = delta * fmaxf(ax, fmaxf(ay, az));
         uint32_t near_mask = 0;
         for (int a = 0; a < 3; a++) if (dd[a] >= 0.0f) near_mask |= 1u << axis_bit[a];
@@ -187,6 +252,7 @@ int main(int argc, char** argv) {
                 for (int s = 0; s < 8; s++)
                     if (leaf >> s & 1) t_mask |= ((1u << (meta[s] >> 5)) - 1u) << (meta[s] & 31u);
                 t_base = w[W8_W_TRI_BASE];
+                trace[r].push_back((uint8_t)__builtin_popcount(t_mask));
                 if (g_bits >> 8) { st[sp].base = g_base; st[sp].bits = g_bits; st[sp].tmin = g_tmin; st[sp].order = g_order; memcpy(st[sp].ts, g_ts, sizeof(g_ts)); sp++; my_push += 1; max_sp = std::max(max_sp, sp); }
                 g_base = w[W8_W_CHILD_BASE];
                 g_bits = imask | (perm << 8);
@@ -289,6 +355,35 @@ int main(int argc, char** argv) {
         if (cntk[k] > 0)
             printf("%s rays: %.1f 16-byte loads per ray (%.1f with the 96-byte node and the 64-byte triangle loaded whole)\n", names[k],
                    (W8_NODE_BYTES / 16 * nv[k] + nt[k] + 3 * npass[k]) / cntk[k], (6 * nv[k] + 4 * nt[k]) / cntk[k]);
+    for (int k = 0; k < 3; k++) {   // triangles pending per node visit that pends any
+        long hist[W8_MAX_NODE_TRIS + 1] = {0}, visits = 0;
+        for (int r = 0; r < NR; r++)
+            if (ray_kind[r] == k)
+                for (uint8_t c : trace[r]) { hist[c]++; visits++; }
+        long pending = 0, sum = 0;
+        for (int c = 1; c <= W8_MAX_NODE_TRIS; c++) { pending += hist[c]; sum += (long)c * hist[c]; }
+        if (!pending) continue;
+        printf("%s rays: %.3f of the node visits pend triangles, %.2f on average; distribution", names[k], (double)pending / visits, (double)sum / pending);
+        for (int c = 1; c <= W8_MAX_NODE_TRIS; c++)
+            if (hist[c]) printf(" %d:%.3f", c, (double)hist[c] / pending);
+        printf("\n");
+    }
+    // the replay uses the device's defaults (capi.cu: w8_tri_weight, refill_thresh, work_chunk); W8M_TRI_W / W8M_REFILL override
+    // (the serial step is replayed with its own tuned weight, 2)
+    const int tri_w = getenv("W8M_TRI_W") ? atoi(getenv("W8M_TRI_W")) : 1, refill = getenv("W8M_REFILL") ? atoi(getenv("W8M_REFILL")) : 24;
+    for (int k = 0; k < 3; k++) {
+        std::vector<const std::vector<uint8_t>*> q;
+        for (int r = 0; r < NR; r++)
+            if (ray_kind[r] == k) q.push_back(&trace[r]);
+        if (q.size() < 32) continue;
+        for (int coop = 0; coop < 2; coop++) {
+            const Replay R = replay(q, coop != 0, coop ? tri_w : 2, refill, 32);
+            const double per = 32.0 / q.size();
+            printf("%s rays, warp replay, %s triangle step (tri_w %d, refill %d): per 32 rays %.1f node steps (%.1f lanes busy), "
+                   "%.1f triangle steps (%.1f lanes busy); 2 x node + triangle steps = %.1f\n", names[k], coop ? "cooperative" : "serial", coop ? tri_w : 2, refill,
+                   R.node_steps * per, R.node_lanes / R.node_steps, R.tri_steps * per, R.tri_lanes / R.tri_steps, (2 * R.node_steps + R.tri_steps) * per);
+        }
+    }
     printf("max stack depth %d, rays left to the exact kernel %ld, rays with a tie %ld\n", max_sp, skipped, ties);
     printf("closest-hit distances differing from %s: %ld of %d rays\n", brute ? "brute force" : "the exact-box traversal", mismatch, NR);
     return mismatch == 0 ? 0 : 3;
