@@ -54,6 +54,36 @@ void ezrt_w8_axis_bits(const float bmin[3], const float bmax[3], int axis_bit[3]
     for (int k = 0; k < 3; k++) axis_bit[idx[k]] = k;
 }
 
+// Decode range of a quantised tree (w8_node.h): the decode forms A = fma(-bias, B, (origin - o) * inv) with B = scale * inv, so
+// bias * scale * |inv| and |origin - o| * |inv| <= 5 max|coordinate| * |inv| must stay finite.  The limit keeps the larger of
+// the two at or below 2^124, a factor 16 below the overflow threshold 2^128.
+float ezrt_quant_inv_limit(double max_scale, double bias, float max_abs_coord) {
+    const double m = std::max(bias * max_scale, 5.0 * (double)max_abs_coord);
+    double lim = (double)W8_INV_LIMIT;
+    while (lim * m > ldexp(1.0, 124) && lim > ldexp(1.0, -126)) lim *= 0.5;
+    return (float)lim;
+}
+
+float ezrt_w8_max_scale(const uint32_t* nodes, size_t n_nodes) {
+    uint32_t e = 0;
+    for (size_t i = 0; i < n_nodes; i++)
+        for (int a = 0; a < 3; a++) e = std::max(e, W8_SCALE_BITS(nodes[i * W8_NODE_WORDS + W8_W_EXP_IMASK], a));
+    float s;
+    memcpy(&s, &e, 4);
+    return s;
+}
+
+float ezrt_q16_max_scale(const uint32_t* nodes, size_t n_nodes) {
+    float s = 0.0f;
+    for (size_t i = 0; i < n_nodes; i++)
+        for (int a = 0; a < 3; a++) {
+            float v;
+            memcpy(&v, &nodes[i * 24 + 3 + a], 4);
+            s = std::max(s, v);
+        }
+    return s;
+}
+
 // ------------------------------------------------------------------------------------------
 // Optimal collapse of the binary tree to `width`-wide nodes by dynamic programming over the binary tree (surface-area
 // heuristic, after Ylitie et al. 2017 section 3.1; children have larger indices than their parent):

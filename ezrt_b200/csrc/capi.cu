@@ -611,6 +611,10 @@ int ezrt_scene_create(int device, const float* tris, int n_triangles, const floa
     for (int k = 0; k < 3; k++) d.w8_near_bit[k] = w8_near_bit[k];
     d.w8_stack_entries = std::max(1, std::min(w8_depth, EZRT_W8_SMEM_STACK));
     d.w8_origin_limit = W8_ORIGIN_LIMIT_REL * max_abs;
+    // decode range of the quantised form in use (W8, else Q16) with its decode bias: 2^15 for W8, 2^23 for Q16 (device_functions.cuh)
+    d.quant_inv_limit = !w8_words.empty() ? ezrt_quant_inv_limit(ezrt_w8_max_scale(w8_words.data(), w8_words.size() / W8_NODE_WORDS), W8_DECODE_BIAS, max_abs)
+                      : !acc_wide_q.empty() ? ezrt_quant_inv_limit(ezrt_q16_max_scale(acc_wide_q.data(), acc_wide_q.size() / 24), 8388608.0, max_abs)
+                                            : W8_INV_LIMIT;
     d.w8_decode_bits = W8_DECODE_BITS;
     d.w8_tri_weight = 1;   // cooperative triangle step: 1 over 2 is +1 % on C3 and C4 (H100, DESIGN.md section 6)
     if (const char* e = getenv("EZRT_TRI_W")) d.w8_tri_weight = std::max(1, std::min(64, atoi(e)));

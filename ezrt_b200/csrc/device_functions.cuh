@@ -600,7 +600,7 @@ __device__ __forceinline__ void extend_persistent(const SceneDev& sc, const Tree
                     bool traceable = (ax < 3.0e38f) && (ay < 3.0e38f) && (az < 3.0e38f);
                     if (Q16) {   // the quantised planes are conservative only within the decode error bound (w8_node.h): the rest goes to the exact kernel
                         const float ao = fmaxf(ez_abs(o.x), fmaxf(ez_abs(o.y), ez_abs(o.z)));
-                        traceable = traceable && (fmaxf(ax, fmaxf(ay, az)) <= W8_INV_LIMIT) && (fminf(ax, fminf(ay, az)) >= W8_INV_MIN) && (ao <= sc.w8_origin_limit);
+                        traceable = traceable && (fmaxf(ax, fmaxf(ay, az)) <= sc.quant_inv_limit) && (fminf(ax, fminf(ay, az)) >= W8_INV_MIN) && (ao <= sc.w8_origin_limit);
                     }
                     if (traceable) {
                         rs = make_ray_slab(o, inv);
@@ -908,7 +908,7 @@ __device__ __forceinline__ void extend_w8(const SceneDev& sc, uint32_t n, uint32
     uint2 stack_local[W8_LOCAL_STACK];   // entries beyond the shared-memory part (trees deeper than the smem stack)
     uint2* const my_stack = stack_sm + threadIdx.x;
     const uint4* __restrict__ nodes = sc.w8_nodes;
-    const float origin_limit = sc.w8_origin_limit;
+    const float origin_limit = sc.w8_origin_limit, inv_limit = sc.quant_inv_limit;
     const uint32_t bias = sc.w8_decode_bits;   // = W8_DECODE_BITS; a run-time value so that ptxas keeps it in a register (see w8_plane)
     __shared__ unsigned char s_owner_all[EZRT_EXTEND_MAX_THREADS];   // triangle step: first tested pair -> owner lane, 32 bytes per warp
     unsigned char* const s_owner = s_owner_all + (threadIdx.x & ~31u);
@@ -971,7 +971,7 @@ __device__ __forceinline__ void extend_w8(const SceneDev& sc, uint32_t n, uint32
                     const float ax = ez_abs(inv.x), ay = ez_abs(inv.y), az = ez_abs(inv.z);
                     const float ao = fmaxf(ez_abs(o.x), fmaxf(ez_abs(o.y), ez_abs(o.z)));
                     const float amin = fminf(ax, fminf(ay, az)), amax = fmaxf(ax, fmaxf(ay, az));
-                    if ((amax <= W8_INV_LIMIT) && (amin >= W8_INV_MIN) && (ao <= origin_limit)) {  // false for inf / NaN
+                    if ((amax <= inv_limit) && (amin >= W8_INV_MIN) && (ao <= origin_limit)) {  // false for inf / NaN
                         slack = sc.prune_delta * ez_max(ax, ez_max(ay, az));
                         near_mask = (d.x >= 0.0f ? (1u << sc.w8_near_bit[0]) : 0u) | (d.y >= 0.0f ? (1u << sc.w8_near_bit[1]) : 0u) |
                                     (d.z >= 0.0f ? (1u << sc.w8_near_bit[2]) : 0u);

@@ -61,6 +61,7 @@ struct SceneDev {
     int w8_tri_weight;             // step vote of the W8 kernels: triangle step iff w8_tri_weight * min(pending_triangles, 32) >= lanes_with_a_node (env EZRT_TRI_W)
     uint32_t w8_decode_bits;       // W8_DECODE_BITS (passed as data: see w8_plane in device_functions.cuh)
     float w8_origin_limit;         // rays starting further out than this (any |coordinate|) go to the exact kernel (decode error bound)
+    float quant_inv_limit;         // ... and rays with a larger |1/d_a| (decode range of the W8 or Q16 nodes: ezrt_quant_inv_limit, <= W8_INV_LIMIT)
     const float4* acc_wide_nodes;  // 4-wide nodes with exact boxes (128 B records): the accel form of scenes below 2^16 triangles (W8 above)
     int acc_wide_root_ref;
     const uint4* acc_wide_q16;     // the same 4-wide nodes with 16-bit quantised planes (96 B records, same numbering): bounce / shadow launches

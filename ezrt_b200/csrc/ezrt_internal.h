@@ -132,6 +132,13 @@ struct EzrtW8Tree {
 void ezrt_w8_axis_bits(const float bmin[3], const float bmax[3], int axis_bit[3]);
 int ezrt_build_w8(const std::vector<EzrtAccelNode>& an, const std::vector<uint32_t>& order_in, float pad, float max_abs_coord,
                   const int axis_bit[3], EzrtW8Tree& out);
+
+// accel_w8.cpp: the largest |1/d_a| a quantised tree may be walked with (w8_node.h, "decode range"): a power of two, at most
+// W8_INV_LIMIT, small enough that the decode's terms bias * scale * |1/d_a| and 5 * max|coordinate| * |1/d_a| stay finite for
+// the largest per-axis scale of the tree.  Rays with a larger |1/d_a| go to the exact kernel.
+float ezrt_quant_inv_limit(double max_scale, double bias, float max_abs_coord);
+float ezrt_w8_max_scale(const uint32_t* nodes, size_t n_nodes);    // W8 records (W8_NODE_WORDS words each)
+float ezrt_q16_max_scale(const uint32_t* nodes, size_t n_nodes);   // Q16 records (24 words each)
 #endif
 
 // Image partition shared by host and device code (ezrt_render_params.part_rank/part_count):

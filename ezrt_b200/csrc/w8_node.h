@@ -31,9 +31,14 @@
 // planes (x = exact plane in steps).  Rounding error of the decode: A is rounded once at magnitude <= 2^15 * B + |t|, i.e.
 // 2^-9 step + 2^-24 |t|; (origin - o) * inv_d carries 2 * 2^-24 * |origin - o| * |inv_d|; the final FMA 2^-24 |t|.  The
 // builder keeps scale >= W8_MIN_STEP_REL * max|coordinate| and the kernel only traces rays with
-// |o| <= W8_ORIGIN_LIMIT_REL * max|coordinate| and 2^-60 <= |inv_d| <= 2^96 on this tree (all others go to the exact kernel), so
-// with |plane|, |o| <= 5 max|coordinate| the total stays below 4 * 2^-24 * 5 * max|coordinate| * |inv_d| + 2^-9 step
-// < 0.16 step + 0.002 step < W8_SLACK_STEPS (0.25).
+// |o| <= W8_ORIGIN_LIMIT_REL * max|coordinate| and 2^-60 <= |inv_d| <= the scene's decode range on this tree (all others go to
+// the exact kernel), so with |plane|, |o| <= 5 max|coordinate| the total stays below 4 * 2^-24 * 5 * max|coordinate| * |inv_d|
+// + 2^-9 step < 0.16 step + 0.002 step < W8_SLACK_STEPS (0.25).
+// Decode range: the bound above holds only while every term is finite.  2^15 * B = 2^15 * scale * |inv_d| reaches 2^128 for
+// large scenes (a root scale of 2^19, a scene 10^8 wide, overflows at |inv_d| = 2^94): A becomes +-inf, every slot's exit
+// distance -inf, and the ray misses the whole tree.  ezrt_quant_inv_limit (accel_w8.cpp) therefore derives the limit on
+// |inv_d| per scene from the largest per-axis scale of the tree and max|coordinate|: a power of two, at most W8_INV_LIMIT, that
+// keeps 2^15 * scale * |inv_d| and 5 * max|coordinate| * |inv_d| at or below 2^124 (the Q16 nodes: 2^23 * scale).
 //
 // Slot order ("octant order", after Ylitie, Karras, Laine 2017): the builder places a child in the slot whose
 // corner direction (bit a of the slot index set = towards +axis_a) matches the child's offset from the node
@@ -54,7 +59,7 @@
 #define W8_DECODE_BITS 0x47000000u
 #define W8_MIN_STEP_REL 7.62939453125e-06f   // 2^-17: smallest quantisation step relative to max |coordinate|
 #define W8_ORIGIN_LIMIT_REL 4.0f
-#define W8_INV_LIMIT 7.9228162514264338e28f  // 2^96: rays with a larger |1/d_a| go to the exact kernel (no overflow in the decode)
+#define W8_INV_LIMIT 7.9228162514264338e28f  // 2^96: the largest decode range of any scene (SceneDev::quant_inv_limit)
 #define W8_INV_MIN 8.6736173798840355e-19f   // 2^-60: ... or a smaller one (no underflow)
 
 #define W8_LOCAL_STACK 48                    // stack entries beyond the shared-memory part (local memory)

@@ -2,6 +2,7 @@
 device's decode arithmetic and visit rule (CPU model tools/w8_model.cpp, built over the PRODUCT builders) finds, for every
 ray, exactly the closest-hit distance brute force over all triangles finds.  No GPU needed."""
 import os
+import re
 import subprocess
 
 import numpy as np
@@ -66,6 +67,89 @@ def test_w8_traversal_large_grid_against_exact_boxes(tmp_path):
     tris, _, _, _ = scenes.s_grid(4, 3, 2, mesh="bunny")
     out = _run_model(str(tmp_path), tris, _rays(tris, 40000, 3), brute=False)
     print(out)
+
+
+def _far_copy_rays(n, comp, seed):
+    """Rays from below the floor of the P3 scene, under the bunny, along +z with x and y components `comp`."""
+    rng = np.random.default_rng(seed)
+    rays = np.zeros((n, 7), np.float32)
+    rays[:, 0], rays[:, 1], rays[:, 2] = rng.uniform(-0.4, 1.0, n), rng.uniform(-2.5, -1.45, n), -3.0
+    rays[:, 3:6] = (comp, comp, 1.0)
+    rays[:, 6] = 1
+    return rays
+
+
+def _model_stat(out, pattern):
+    m = re.search(pattern, out)
+    assert m, (pattern, out)
+    return m
+
+
+def test_w8_decode_range_on_a_scene_10e8_wide(tmp_path):
+    """The P3 scene and a copy 10^8 along x: the root's scale is 2^19, so 2^15 * scale * |1/d| overflows float for |1/d| =
+    2^95, A = fma(-2^15, B, ...) becomes -inf and a ray with d_a > 0 misses every child.  The gate on |1/d| is derived from
+    the tree (here 2^90): such rays go to the exact kernel, the others keep every hit."""
+    tris, _, _, _ = scenes.s_p3_bunny()
+    far = tris.copy()
+    far[:, 0:9:3] += 1e8
+    both = np.concatenate([tris, far])
+    rays = np.concatenate([_far_copy_rays(256, 2.0 ** -95, 0), _far_copy_rays(256, 2.0 ** -80, 0)])
+    out = _run_model(str(tmp_path), both, rays, brute=True)
+    assert _model_stat(out, r"decode range \|1/d\| <= (\S+)").group(1) == "%g" % 2.0 ** 90
+    assert _model_stat(out, r"rays left to the exact kernel (\d+)").group(1) == "256"
+    assert int(_model_stat(out, r"\((\d+) of them hit\)").group(1)) > 100
+
+
+def _pending_hist(out, kind="bounce"):
+    """{pending triangles: share of the node visits that pend any} of the model's distribution line"""
+    line = _model_stat(out, kind + r" rays: \S+ of the node visits pend triangles.*distribution(.*)").group(1)
+    return {int(k): float(v) for k, v in (p.split(":") for p in line.split())}
+
+
+def _model_rays(o, d):
+    rays = np.zeros((len(o), 7), np.float32)
+    rays[:, :3], rays[:, 3:6], rays[:, 6] = o, d, 1
+    return rays
+
+
+def _ties(out):
+    return int(_model_stat(out, r"rays with a tie (\d+)").group(1))
+
+
+def test_w8_gpu_scenes_load_the_cooperative_step(tmp_path):
+    """The scenes and rays of tests/test_gpu_w8.py through the CPU model: node visits that leave all 32 triangle bits pending,
+    and many rays with a tie, so that the GPU tests run the cooperative step's split owners and tie rules."""
+    from tests import test_gpu_w8 as g
+    tris = g.twin_scene()[0]
+    o, d = g.grid_rays(20000, 31, 2.5)
+    out = _run_model(str(tmp_path), tris, _model_rays(o, d), brute=False)
+    assert _ties(out) > 0.2 * len(o)
+    for ulps in (0, 3):
+        tris = g.stack_scene(ulps, 40 + ulps)[0]
+        o, d = g.stack_rays(tris, 600, 7 + ulps)
+        out = _run_model(str(tmp_path), tris, _model_rays(o, d), brute=False)
+        hist = _pending_hist(out)
+        assert hist.get(32, 0.0) > 0.0, hist
+        if ulps == 0:
+            assert _ties(out) > 0.5 * len(o)
+    tris = g.huge_floor_scene()[0]
+    o, d = g.grid_rays(20000, 23, 1.2)
+    out = _run_model(str(tmp_path), tris, _model_rays(o, d), brute=False)
+    assert max(_pending_hist(out)) >= 24
+
+
+def test_w8_decode_range_of_the_wide_gpu_scenes(tmp_path):
+    """The 10^8 and 10^9 wide scenes of tests/test_gpu_w8.py: the model walks them with the same gate and finds every hit."""
+    from tests import test_gpu_w8 as g
+    for shift in (1e8, 1e9):
+        tris, nodes, _, _ = g.far_scene(shift, 6)
+        assert g.regular_tree(tris, nodes)
+        o, d = g.far_rays(tris, 6000, 3)
+        out = _run_model(str(tmp_path), tris, _model_rays(o, d), brute=False)
+        limit = float(_model_stat(out, r"decode range \|1/d\| <= (\S+)").group(1))
+        assert limit < 2.0 ** 96
+        tiny = (np.abs(d) == 2.0 ** -95).any(1)
+        assert int(_model_stat(out, r"rays left to the exact kernel (\d+)").group(1)) >= tiny.sum() > 1000
 
 
 def _run_w4_check(tmp_path, tris):

@@ -139,6 +139,10 @@ int main(int argc, char** argv) {
     if (rc) { fprintf(stderr, "ezrt_build_w8 failed: %d\n", rc); return 1; }
     printf("binary nodes %zu, 8-wide nodes %d (%.1f MB), depth %d, mean fill %.2f, axis bits x%d y%d z%d\n", an.size(), w8.n_nodes,
            w8.n_nodes * (double)W8_NODE_BYTES / 1e6, w8.depth, (double)w8.n_children / w8.n_nodes, axis_bit[0], axis_bit[1], axis_bit[2]);
+    // the kernel's gate on |1/d_a| (capi.cu: SceneDev::quant_inv_limit)
+    const float max_scale = ezrt_w8_max_scale(w8.nodes.data(), (size_t)w8.n_nodes);
+    const float inv_limit = ezrt_quant_inv_limit(max_scale, W8_DECODE_BIAS, maxc);
+    printf("largest node scale %g, decode range |1/d| <= %g\n", max_scale, inv_limit);
     {   // the 4-wide collapse the default kernel uses (same dynamic programme, width 4): every triangle in exactly one leaf of <= 4
         EzrtCollapse c4;
         if (c4.build(an, 4, W8_MAX_LEAF_TRIS, 1.0, 0.3) != 0) { fprintf(stderr, "4-wide collapse failed\n"); return 1; }
@@ -181,11 +185,11 @@ int main(int argc, char** argv) {
     // W8M_EXACT=1 exact child boxes instead of the quantised ones (how much the 8-bit planes cost)
     const bool x_sort = getenv("W8M_SORT") && atoi(getenv("W8M_SORT")), x_gmin = getenv("W8M_GMIN") && atoi(getenv("W8M_GMIN"));
     double nv[3] = {0, 0, 0}, nt[3] = {0, 0, 0}, npass[3] = {0, 0, 0}, npush[3] = {0, 0, 0}, cntk[3] = {0, 0, 0};
-    long mismatch = 0, skipped = 0, ties = 0;
+    long mismatch = 0, skipped = 0, ties = 0, hits = 0;
     int max_sp = 0;
     std::vector<std::vector<uint8_t>> trace(NR);   // triangles pending after each node visit, for the warp replay
     std::vector<int> ray_kind(NR, -1);              // -1: left to the exact kernel
-#pragma omp parallel for schedule(dynamic, 256) reduction(+ : mismatch, skipped, ties) reduction(max : max_sp)
+#pragma omp parallel for schedule(dynamic, 256) reduction(+ : mismatch, skipped, ties, hits) reduction(max : max_sp)
     for (int r = 0; r < NR; r++) {
         const float* R = &rays[(size_t)r * 7];
         const ez_vec3 o = ez_v3(R[0], R[1], R[2]), d = ez_v3(R[3], R[4], R[5]);
@@ -193,7 +197,7 @@ int main(int argc, char** argv) {
         const float inv[3] = {EZ_DIV(1.0f, d.x), EZ_DIV(1.0f, d.y), EZ_DIV(1.0f, d.z)}, oo[3] = {o.x, o.y, o.z}, dd[3] = {d.x, d.y, d.z};
         const float ax = fabsf(inv[0]), ay = fabsf(inv[1]), az = fabsf(inv[2]);
         const float olim = W8_ORIGIN_LIMIT_REL * maxc;
-        if (!(ax <= W8_INV_LIMIT && ay <= W8_INV_LIMIT && az <= W8_INV_LIMIT && ax >= W8_INV_MIN && ay >= W8_INV_MIN && az >= W8_INV_MIN) || !(fabsf(oo[0]) <= olim && fabsf(oo[1]) <= olim && fabsf(oo[2]) <= olim)) {
+        if (!(ax <= inv_limit && ay <= inv_limit && az <= inv_limit && ax >= W8_INV_MIN && ay >= W8_INV_MIN && az >= W8_INV_MIN) || !(fabsf(oo[0]) <= olim && fabsf(oo[1]) <= olim && fabsf(oo[2]) <= olim)) {
             skipped++;  // the kernel hands these to the exact traversal
             continue;
         }
@@ -343,6 +347,7 @@ int main(int argc, char** argv) {
             }
         }
         if (memcmp(&want, &best, 4) != 0) mismatch++;
+        if (want < EZ_INF) hits++;
 #pragma omp critical
         { nv[kind] += my_nv; nt[kind] += my_nt; npass[kind] += my_pass; npush[kind] += my_push; cntk[kind] += 1; }
     }
@@ -385,6 +390,6 @@ int main(int argc, char** argv) {
         }
     }
     printf("max stack depth %d, rays left to the exact kernel %ld, rays with a tie %ld\n", max_sp, skipped, ties);
-    printf("closest-hit distances differing from %s: %ld of %d rays\n", brute ? "brute force" : "the exact-box traversal", mismatch, NR);
+    printf("closest-hit distances differing from %s: %ld of %d rays (%ld of them hit)\n", brute ? "brute force" : "the exact-box traversal", mismatch, NR, hits);
     return mismatch == 0 ? 0 : 3;
 }
