@@ -31,6 +31,12 @@ class AdaptiveParams(C.Structure):
     _fields_ = [("threshold", C.c_float), ("min_spp", C.c_int32), ("check_interval", C.c_int32), ("reserved", C.c_int32)]
 
 
+class DenoiseParams(C.Structure):
+    """struct ezrt_denoise_params (include/ezrt.h)."""
+    _fields_ = [("iterations", C.c_int32), ("sigma_l", C.c_float), ("sigma_n", C.c_float), ("sigma_z", C.c_float), ("sigma_a", C.c_float),
+                ("reserved", C.c_int32)]
+
+
 class Counters(C.Structure):
     """struct ezrt_counters (include/ezrt.h)."""
     _fields_ = [
@@ -53,6 +59,12 @@ SIGNATURES = {
     "ezrt_render_adaptive_device": (C.c_int, [C.c_void_p, C.POINTER(RenderParams), C.POINTER(AdaptiveParams), C.c_void_p, C.c_void_p,
                                               C.c_void_p, C.c_void_p]),
     "ezrt_render_adaptive": (C.c_int, [C.c_void_p, C.POINTER(RenderParams), C.POINTER(AdaptiveParams), c_float_p, c_int32_p, c_float_p]),
+    "ezrt_render_aov_device": (C.c_int, [C.c_void_p, C.POINTER(RenderParams), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "ezrt_render_aov": (C.c_int, [C.c_void_p, C.POINTER(RenderParams), c_float_p, c_float_p, c_float_p]),
+    "ezrt_denoise_device": (C.c_int, [C.c_void_p, C.POINTER(DenoiseParams), C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
+                                      C.c_int, C.c_void_p, C.c_void_p]),
+    "ezrt_denoise": (C.c_int, [C.c_void_p, C.POINTER(DenoiseParams), c_float_p, C.c_int, c_float_p, c_float_p, C.c_int, C.c_int, C.c_int,
+                               c_float_p]),
     "ezrt_get_counters": (C.c_int, [C.c_void_p, C.POINTER(Counters)]),
     "ezrt_get_kernel_times": (C.c_int, [C.c_void_p, C.POINTER(C.c_double), C.POINTER(C.c_uint64)]),
     "ezrt_partition_pixels": (C.c_int64, [C.c_int, C.c_int, C.c_int, C.c_int]),

@@ -12,7 +12,7 @@ from dataclasses import dataclass, field
 import numpy as np
 
 from . import _lib
-from ._lib import AdaptiveParams, Counters, EzrtError, RenderParams, check, lib
+from ._lib import AdaptiveParams, Counters, DenoiseParams, EzrtError, RenderParams, check, lib
 
 MODE_DIFFUSE_P3 = 0
 MODE_DISNEY_ANISO_P4 = 1
@@ -234,6 +234,19 @@ def adaptive_params(threshold, min_spp, check_interval):
     return a
 
 
+# defaults of the denoiser (ezrt_denoise_params, DESIGN.md section 9)
+DENOISE_DEFAULTS = dict(iterations=5, sigma_l=4.0, sigma_n=128.0, sigma_z=1.0, sigma_a=0.1)
+AOV_CHANNELS = 8   # albedo.rgb, coverage, normal.xyz, depth
+
+
+def denoise_params(iterations=5, sigma_l=4.0, sigma_n=128.0, sigma_z=1.0, sigma_a=0.1):
+    """struct ezrt_denoise_params (include/ezrt.h)."""
+    d = DenoiseParams()
+    d.iterations, d.sigma_l, d.sigma_n, d.sigma_z, d.sigma_a, d.reserved = int(iterations), float(sigma_l), float(sigma_n), float(sigma_z), \
+        float(sigma_a), 0
+    return d
+
+
 class Scene:
     """Device-resident scene: the two texture buffers + two HDR textures of P5/main.cpp:878-906."""
 
@@ -307,6 +320,57 @@ class Scene:
         check(lib.ezrt_render_adaptive_device(self._h, C.byref(p), C.byref(a), C.c_void_p(ptr(d_framebuffer)), C.c_void_p(ptr(d_spp)),
                                               C.c_void_p(ptr(d_luma2)), C.c_void_p(st)))
         return d_framebuffer, d_spp, d_luma2
+
+    def render_aov(self, cfg, framebuffer=None, aov=None, luma2=None):
+        """Plain render that also returns the first-hit feature buffers (ezrt_render_aov).  Returns host arrays
+        (image, aov, luma2): [H, W, C], [H, W, 8], [H, W] for one part, compact tile-major [n, C], [n, 8], [n] otherwise.
+        aov = running means of (albedo.rgb, coverage, normal.xyz, depth) of the first hit, 0 for a primary miss; luma2 =
+        running mean of the squared sample luminance.  When cfg.first_frame > 0 pass the previous three arrays: they are in/out."""
+        n = partition_pixels(cfg.width, cfg.height, cfg.part_rank, cfg.part_count)
+        img = np.zeros((n, cfg.out_channels), np.float32) if framebuffer is None else framebuffer
+        feat = np.zeros((n, AOV_CHANNELS), np.float32) if aov is None else aov
+        m2 = np.zeros(n, np.float32) if luma2 is None else luma2
+        for a, k in ((img, cfg.out_channels), (feat, AOV_CHANNELS), (m2, 1)):
+            assert a.dtype == np.float32 and a.size == n * k and a.flags.c_contiguous
+        p = cfg.to_struct()
+        check(lib.ezrt_render_aov(self._h, C.byref(p), _fp(img), _fp(feat), _fp(m2)))
+        if cfg.part_count == 1:
+            return (img.reshape(cfg.height, cfg.width, cfg.out_channels), feat.reshape(cfg.height, cfg.width, AOV_CHANNELS),
+                    m2.reshape(cfg.height, cfg.width))
+        return img.reshape(n, cfg.out_channels), feat.reshape(n, AOV_CHANNELS), m2.reshape(n)
+
+    def render_aov_device(self, cfg, d_framebuffer, d_aov, d_luma2, stream=None):
+        """Enqueue a feature-buffer render on a CUDA stream into device buffers (torch tensors or raw pointers): the
+        framebuffer, 8 float32 per pixel (16-byte aligned), float32 per pixel.  In/out when cfg.first_frame > 0."""
+        ptr = lambda t: t.data_ptr() if hasattr(t, "data_ptr") else int(t)
+        st = 0 if stream is None else (stream.cuda_stream if hasattr(stream, "cuda_stream") else int(stream))
+        p = cfg.to_struct()
+        check(lib.ezrt_render_aov_device(self._h, C.byref(p), C.c_void_p(ptr(d_framebuffer)), C.c_void_p(ptr(d_aov)),
+                                         C.c_void_p(ptr(d_luma2)), C.c_void_p(st)))
+        return d_framebuffer, d_aov, d_luma2
+
+    def denoise(self, image, aov, luma2, n, out=None, **sigmas):
+        """A-trous denoiser (ezrt_denoise) of a full image [H, W, 3 or 4] after n frames, with render_aov's aov [H, W, 8] and
+        luma2 [H, W].  sigmas: iterations, sigma_l, sigma_n, sigma_z, sigma_a (DENOISE_DEFAULTS).  out may be image."""
+        img = _f32(image)
+        assert img.ndim == 3 and img.shape[2] in (3, 4)
+        h, w, ch = img.shape
+        feat, m2 = _f32(aov, (h, w, AOV_CHANNELS)), _f32(luma2, (h, w))
+        if out is None:
+            out = np.empty_like(img)
+        assert out.dtype == np.float32 and out.shape == img.shape and out.flags.c_contiguous
+        d = denoise_params(**{**DENOISE_DEFAULTS, **sigmas})
+        check(lib.ezrt_denoise(self._h, C.byref(d), _fp(img), ch, _fp(feat), _fp(m2), w, h, int(n), _fp(out)))
+        return out
+
+    def denoise_device(self, d_image, channels, d_aov, d_luma2, width, height, n, d_out, stream=None, **sigmas):
+        """Enqueue the denoiser on a CUDA stream over device buffers (torch tensors or raw pointers); d_out may be d_image."""
+        ptr = lambda t: t.data_ptr() if hasattr(t, "data_ptr") else int(t)
+        st = 0 if stream is None else (stream.cuda_stream if hasattr(stream, "cuda_stream") else int(stream))
+        d = denoise_params(**{**DENOISE_DEFAULTS, **sigmas})
+        check(lib.ezrt_denoise_device(self._h, C.byref(d), C.c_void_p(ptr(d_image)), int(channels), C.c_void_p(ptr(d_aov)),
+                                      C.c_void_p(ptr(d_luma2)), int(width), int(height), int(n), C.c_void_p(ptr(d_out)), C.c_void_p(st)))
+        return d_out
 
     def counters(self):
         c = Counters()

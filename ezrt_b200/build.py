@@ -146,6 +146,22 @@ def build_oracle_adaptive(force=False):
     return ORACLE_ADAPTIVE_SO
 
 
+ORACLE_AOV_SO = os.path.join(ROOT, "build", "libezrt_oracle_aov.so")
+
+
+def build_oracle_aov(force=False):
+    """build/libezrt_oracle_aov.so: tests/oracle_aov.cpp, the CPU restatement of the feature-buffer render over the oracle's
+    sample function and of the denoiser (test infrastructure, loaded only by tests/oracle_aov.py)."""
+    src = os.path.join(ROOT, "tests", "oracle_aov.cpp")
+    deps = [src, os.path.join(ROOT, "oracle", "ezrt_oracle.cpp")] + [os.path.join(INCLUDE, f) for f in os.listdir(INCLUDE)]
+    if force or _newer(ORACLE_AOV_SO, deps):
+        os.makedirs(os.path.dirname(ORACLE_AOV_SO), exist_ok=True)
+        tmp = ORACLE_AOV_SO + ".tmp%d" % os.getpid()
+        _run(["g++"] + HOST_FLAGS + ["-fopenmp", "-Wno-misleading-indentation", "-shared", "-I", INCLUDE, src, "-o", tmp])
+        os.replace(tmp, ORACLE_AOV_SO)
+    return ORACLE_AOV_SO
+
+
 def build_reference_hdrloader(force=False):
     return _oracle_recipes().build_reference_hdrloader(force)
 
@@ -205,6 +221,7 @@ def build_all(force=False, verbose=False):
     build_product(force=force, verbose=verbose)
     build_oracle(force=force)
     build_oracle_adaptive(force=force)
+    build_oracle_aov(force=force)
     build_example(force=force)
     build_reference_hdrloader(force=force)
     build_reference_shaders(force=force)

@@ -89,6 +89,9 @@ struct ezrt_scene {
     DeviceBuffer tiles_buf, queue_buf[2], shadow_buf, lo_buf, le_buf, counters_buf, totals_buf, fb_buf, sort_buf;
     // adaptive sampling: two surviving-tile lists (ping-pong), per-tile verdicts, the test's counters; the host entry point's spp map + luma2
     DeviceBuffer adapt_buf, adapt_maps_buf;
+    // feature-buffer renders: the first-hit records of a batch (32 B per sample slot); the host entry point's aov + luma2.
+    // The denoiser: its ping-pong (colour, variance) images; the host entry point's device copies of its inputs
+    DeviceBuffer aov_rec_buf, aov_maps_buf, denoise_buf, denoise_io_buf;
     void* hot_base = nullptr;   // accel nodes | geometry | shading records (L2 persisting window)
     size_t hot_bytes = 0;
     size_t l2_persist_bytes = 0;
@@ -217,6 +220,17 @@ struct AdaptiveRun {
     float threshold;
     int min_spp, check_interval;
     int32_t* d_spp;
+    float* d_luma2;
+};
+
+int validate_aov(const ezrt_render_params* p) {
+    if (p->pipeline != EZRT_PIPELINE_WAVEFRONT) return ezrt_set_error(EZRT_ERR_INVALID, "render_aov: only the wavefront pipeline writes feature buffers");
+    return EZRT_OK;
+}
+
+// the feature-buffer render's per-pixel outputs (device): 8 floats of first-hit features, the running mean of the squared luminance
+struct AovRun {
+    float* d_aov;
     float* d_luma2;
 };
 
@@ -682,6 +696,7 @@ int ezrt_scene_destroy(ezrt_scene* s) {
     s->queue_buf[0].release(); s->queue_buf[1].release(); s->shadow_buf.release();
     s->lo_buf.release(); s->le_buf.release(); s->counters_buf.release(); s->totals_buf.release(); s->fb_buf.release(); s->sort_buf.release();
     s->adapt_buf.release(); s->adapt_maps_buf.release();
+    s->aov_rec_buf.release(); s->aov_maps_buf.release(); s->denoise_buf.release(); s->denoise_io_buf.release();
     if (s->own_stream) cudaStreamDestroy(s->own_stream);
     if (s->copy_stream) cudaStreamDestroy(s->copy_stream);
     if (s->side_stream) cudaStreamDestroy(s->side_stream);
@@ -699,8 +714,10 @@ int ezrt_scene_destroy(ezrt_scene* s) {
 // ------------------------------------------------------------------------------------------
 // render
 // ------------------------------------------------------------------------------------------
-// The render of ezrt_render_device (ad == nullptr) and ezrt_render_adaptive_device: the arguments are validated.
-static int render_device_impl(ezrt_scene* s, const ezrt_render_params* p, float* d_fb, cudaStream_t st, const AdaptiveRun* ad) {
+// The render of ezrt_render_device (ad == av == nullptr), ezrt_render_adaptive_device (ad) and ezrt_render_aov_device (av): the
+// arguments are validated.
+static int render_device_impl(ezrt_scene* s, const ezrt_render_params* p, float* d_fb, cudaStream_t st, const AdaptiveRun* ad,
+                              const AovRun* av = nullptr) {
     CU_CHECK(cudaSetDevice(s->device));
     int rc = prepare_tiles(s, p, st);
     if (rc) return rc;
@@ -753,13 +770,14 @@ static int render_device_impl(ezrt_scene* s, const ezrt_render_params* p, float*
     {   // bound the batch by the memory that is actually there (scratch already held by this scene counts as available);
         // asked once per (slots per frame, integrator): cudaMemGetInfo is a driver round trip, the render path is launch-only
         const size_t per_slot = 2 * (sizeof(float4) * 4 + sizeof(float2)) + 2 * sizeof(float4) + sizeof(uint32_t) +
-                                (is_mode ? (size_t)EZRT_SHADOW_SLOT_BYTES : 0) + (s->sort_rays ? 2 * sizeof(uint32_t) : 0);
+                                (is_mode ? (size_t)EZRT_SHADOW_SLOT_BYTES : 0) + (s->sort_rays ? 2 * sizeof(uint32_t) : 0) +
+                                (av ? 2 * sizeof(float4) : 0);
         if (s->fmax_key[0] != per_frame || s->fmax_key[1] != per_slot) {
             size_t free_b = 0, total_b = 0;
             s->fmax = (size_t)1 << 30;
             if (cudaMemGetInfo(&free_b, &total_b) == cudaSuccess) {
                 const size_t held = s->queue_buf[0].bytes + s->queue_buf[1].bytes + s->shadow_buf.bytes + s->lo_buf.bytes + s->le_buf.bytes +
-                                    s->defer_buf.bytes + s->sort_buf.bytes;
+                                    s->defer_buf.bytes + s->sort_buf.bytes + s->aov_rec_buf.bytes;
                 const size_t avail = (size_t)((double)(free_b + held) * 0.9);
                 s->fmax = avail / per_slot / per_frame;
                 if (s->fmax < 1) return ezrt_set_error(EZRT_ERR_NOMEM, "render: %zu MB free, one frame of wavefront state needs %zu MB", free_b >> 20, (per_slot * per_frame) >> 20);
@@ -778,6 +796,11 @@ static int render_device_impl(ezrt_scene* s, const ezrt_render_params* p, float*
     if ((rc = carve_shadow(s->shadow_buf, is_mode ? capacity : 1, sq))) return rc;
     if ((rc = s->lo_buf.ensure(sizeof(float4) * capacity))) return rc;
     if ((rc = s->le_buf.ensure(sizeof(float4) * capacity))) return rc;
+    float4* aov_rec = nullptr;   // feature-buffer render only: the first-hit record of every sample slot
+    if (av) {
+        if ((rc = s->aov_rec_buf.ensure(2 * sizeof(float4) * capacity))) return rc;
+        aov_rec = (float4*)s->aov_rec_buf.p;
+    }
     const int n_stages = p->max_bounce + 2;
     // counters: [0,n) queue sizes, [n,2n) shadow sizes, [2n,3n) extend work, [3n,4n) shadow work,
     // [4n,6n) deferred-ray counts of the accel passes (extend, shadow), [6n,8n) work counters of their exact passes
@@ -888,13 +911,13 @@ static int render_device_impl(ezrt_scene* s, const ezrt_render_params* p, float*
                 CU_CHECK(cudaEventRecord(s->ev_fork, st));
                 CU_CHECK(cudaStreamWaitEvent(s->side_stream, s->ev_fork, 0));
                 launch_deferred_lane(s->dev, rd, d_tiles, b, batch_first, qin, defer_list, &d_ext[b], &dw_ext[b], side_hit, qout, &q_count[b + 1], sq, &s_count[b],
-                                     Lo, Le, n_fused, (uint32_t)nf, s->n_sms, s->side_stream);
+                                     Lo, Le, n_fused, (uint32_t)nf, s->n_sms, s->side_stream, b == 0 ? aov_rec : nullptr);
                 CU_CHECK(cudaEventRecord(s->ev_join, s->side_stream));
                 s->launches += 2;
             }
             sp = s->span_begin(1, st);
             launch_shade(s->dev, rd, d_tiles, b, batch_first, qin, &q_count[b], qout, &q_count[b + 1], sq, &s_count[b], Lo, Le,
-                         n_slots, n_fused, (uint32_t)nf, s->n_sms, st);
+                         n_slots, n_fused, (uint32_t)nf, s->n_sms, st, b == 0 ? aov_rec : nullptr);
             if (lane) CU_CHECK(cudaStreamWaitEvent(st, s->ev_join, 0));   // ... while this k_shade shades all the others; join
             s->span_end(sp, st);
             s->launches += 2;
@@ -918,7 +941,8 @@ static int render_device_impl(ezrt_scene* s, const ezrt_render_params* p, float*
             CU_CHECK(cudaStreamWaitEvent(st, s->fb_wait, 0));
             s->fb_wait = nullptr;
         }
-        if (ad) launch_blend_adaptive(rd, d_tiles, nf, batch_first, Lo, Le, d_fb, ad->d_luma2, ad->d_spp, st);
+        if (av) launch_blend_aov(rd, d_tiles, nf, batch_first, Lo, Le, aov_rec, d_fb, av->d_aov, av->d_luma2, st);
+        else if (ad) launch_blend_adaptive(rd, d_tiles, nf, batch_first, Lo, Le, d_fb, ad->d_luma2, ad->d_spp, st);
         else launch_blend(rd, d_tiles, nf, batch_first, Lo, Le, d_fb, st);
         launch_tally(q_count, s_count, d_ext, d_sh, p->max_bounce + 1, totals, fused_camera ? (uint32_t)(active_pixels * (size_t)nf) : 0u, st);
         s->span_end(sp, st);
@@ -1026,6 +1050,105 @@ int ezrt_render(ezrt_scene* s, const ezrt_render_params* p, float* framebuffer) 
     }
     if (rc) return rc;
     CU_CHECK(cudaMemcpyAsync(framebuffer, s->fb_buf.p, bytes, cudaMemcpyDeviceToHost, st));
+    CU_CHECK(cudaStreamSynchronize(st));
+    return EZRT_OK;
+}
+
+int ezrt_render_aov_device(ezrt_scene* s, const ezrt_render_params* p, float* d_fb, float* d_aov, float* d_luma2, void* cuda_stream) {
+    int rc = validate_params(s, p);
+    if (!rc) rc = validate_aov(p);
+    if (rc) return rc;
+    if (!d_fb || !d_aov || !d_luma2) return ezrt_set_error(EZRT_ERR_INVALID, "render_aov: null output buffer");
+    if ((uintptr_t)d_aov % 16) return ezrt_set_error(EZRT_ERR_INVALID, "render_aov: the aov buffer must be 16-byte aligned");
+    const AovRun av{d_aov, d_luma2};
+    return render_device_impl(s, p, d_fb, (cudaStream_t)cuda_stream, nullptr, &av);
+}
+
+int ezrt_render_aov(ezrt_scene* s, const ezrt_render_params* p, float* framebuffer, float* aov, float* luma2) {
+    int rc = validate_params(s, p);
+    if (!rc) rc = validate_aov(p);
+    if (rc) return rc;
+    if (!framebuffer || !aov || !luma2) return ezrt_set_error(EZRT_ERR_INVALID, "render_aov: null output buffer");
+    CU_CHECK(cudaSetDevice(s->device));
+    const size_t npix = (size_t)ezrt_partition_pixels(p->width, p->height, p->part_rank, p->part_count);
+    const size_t fb_bytes = sizeof(float) * npix * p->out_channels;
+    const size_t aov_bytes = ((sizeof(float) * 8 * npix + 255) / 256) * 256;
+    if ((rc = s->fb_buf.ensure(std::max<size_t>(fb_bytes, 16)))) return rc;
+    if ((rc = s->aov_maps_buf.ensure(aov_bytes + sizeof(float) * npix + 16))) return rc;
+    float* d_aov = (float*)s->aov_maps_buf.p;
+    float* d_luma2 = (float*)((char*)s->aov_maps_buf.p + aov_bytes);
+    cudaStream_t st = s->own_stream;
+    s->fb_wait = nullptr;
+    if (p->first_frame > 0) {   // all three are in/out: the render goes on from where they stand
+        CU_CHECK(cudaMemcpyAsync(s->fb_buf.p, framebuffer, fb_bytes, cudaMemcpyHostToDevice, st));
+        CU_CHECK(cudaMemcpyAsync(d_aov, aov, sizeof(float) * 8 * npix, cudaMemcpyHostToDevice, st));
+        CU_CHECK(cudaMemcpyAsync(d_luma2, luma2, sizeof(float) * npix, cudaMemcpyHostToDevice, st));
+    }
+    const AovRun av{d_aov, d_luma2};
+    if ((rc = render_device_impl(s, p, (float*)s->fb_buf.p, st, nullptr, &av))) return rc;
+    CU_CHECK(cudaMemcpyAsync(framebuffer, s->fb_buf.p, fb_bytes, cudaMemcpyDeviceToHost, st));
+    CU_CHECK(cudaMemcpyAsync(aov, d_aov, sizeof(float) * 8 * npix, cudaMemcpyDeviceToHost, st));
+    CU_CHECK(cudaMemcpyAsync(luma2, d_luma2, sizeof(float) * npix, cudaMemcpyDeviceToHost, st));
+    CU_CHECK(cudaStreamSynchronize(st));
+    return EZRT_OK;
+}
+
+static int validate_denoise(const ezrt_scene* s, const ezrt_denoise_params* dp, int channels, int width, int height, int n_frames) {
+    if (!s || !dp) return ezrt_set_error(EZRT_ERR_INVALID, "denoise: null argument");
+    if (dp->iterations < 1 || dp->iterations > 10) return ezrt_set_error(EZRT_ERR_INVALID, "denoise: iterations must be in 1..10 (got %d)", dp->iterations);
+    const float sg[4] = {dp->sigma_l, dp->sigma_n, dp->sigma_z, dp->sigma_a};
+    for (float v : sg)
+        if (!std::isfinite(v) || !(v > 0.0f)) return ezrt_set_error(EZRT_ERR_INVALID, "denoise: every sigma must be finite and > 0 (got %g)", (double)v);
+    if (dp->reserved != 0) return ezrt_set_error(EZRT_ERR_INVALID, "denoise: reserved field must be 0");
+    if (channels != 3 && channels != 4) return ezrt_set_error(EZRT_ERR_INVALID, "denoise: channels must be 3 or 4");
+    if (width <= 0 || height <= 0) return ezrt_set_error(EZRT_ERR_INVALID, "denoise: bad image size");
+    if (n_frames < 1) return ezrt_set_error(EZRT_ERR_INVALID, "denoise: n_frames must be >= 1 (got %d)", n_frames);
+    return EZRT_OK;
+}
+
+static int denoise_impl(ezrt_scene* s, const ezrt_denoise_params* dp, const float* d_color, int channels, const float* d_aov, const float* d_luma2,
+                        int width, int height, int n_frames, float* d_out, cudaStream_t st) {
+    const size_t npix = (size_t)width * height;
+    const size_t half = ((sizeof(float4) * npix + 255) / 256) * 256;
+    int rc = s->denoise_buf.ensure(2 * half);
+    if (rc) return rc;
+    float4* cv0 = (float4*)s->denoise_buf.p;
+    float4* cv1 = (float4*)((char*)s->denoise_buf.p + half);
+    launch_denoise(d_color, channels, d_aov, d_luma2, n_frames, width, height, dp->iterations, dp->sigma_l, dp->sigma_n, dp->sigma_z,
+                   dp->sigma_a, cv0, cv1, d_out, st);
+    CU_CHECK(cudaGetLastError());
+    return EZRT_OK;
+}
+
+int ezrt_denoise_device(ezrt_scene* s, const ezrt_denoise_params* dp, const float* d_color, int channels, const float* d_aov,
+                        const float* d_luma2, int width, int height, int n_frames, float* d_out, void* cuda_stream) {
+    int rc = validate_denoise(s, dp, channels, width, height, n_frames);
+    if (rc) return rc;
+    if (!d_color || !d_aov || !d_luma2 || !d_out) return ezrt_set_error(EZRT_ERR_INVALID, "denoise: null buffer");
+    if ((uintptr_t)d_aov % 16) return ezrt_set_error(EZRT_ERR_INVALID, "denoise: the aov buffer must be 16-byte aligned");
+    CU_CHECK(cudaSetDevice(s->device));
+    return denoise_impl(s, dp, d_color, channels, d_aov, d_luma2, width, height, n_frames, d_out, (cudaStream_t)cuda_stream);
+}
+
+int ezrt_denoise(ezrt_scene* s, const ezrt_denoise_params* dp, const float* color, int channels, const float* aov, const float* luma2,
+                 int width, int height, int n_frames, float* out) {
+    int rc = validate_denoise(s, dp, channels, width, height, n_frames);
+    if (rc) return rc;
+    if (!color || !aov || !luma2 || !out) return ezrt_set_error(EZRT_ERR_INVALID, "denoise: null buffer");
+    CU_CHECK(cudaSetDevice(s->device));
+    const size_t npix = (size_t)width * height;
+    const size_t aov_bytes = ((sizeof(float) * 8 * npix + 255) / 256) * 256;
+    const size_t color_bytes = ((sizeof(float) * channels * npix + 255) / 256) * 256;
+    if ((rc = s->denoise_io_buf.ensure(aov_bytes + color_bytes + sizeof(float) * npix))) return rc;
+    float* d_aov = (float*)s->denoise_io_buf.p;
+    float* d_color = (float*)((char*)s->denoise_io_buf.p + aov_bytes);
+    float* d_luma2 = (float*)((char*)s->denoise_io_buf.p + aov_bytes + color_bytes);
+    cudaStream_t st = s->own_stream;
+    CU_CHECK(cudaMemcpyAsync(d_aov, aov, sizeof(float) * 8 * npix, cudaMemcpyHostToDevice, st));
+    CU_CHECK(cudaMemcpyAsync(d_color, color, sizeof(float) * channels * npix, cudaMemcpyHostToDevice, st));
+    CU_CHECK(cudaMemcpyAsync(d_luma2, luma2, sizeof(float) * npix, cudaMemcpyHostToDevice, st));
+    if ((rc = denoise_impl(s, dp, d_color, channels, d_aov, d_luma2, width, height, n_frames, d_color, st))) return rc;
+    CU_CHECK(cudaMemcpyAsync(out, d_color, sizeof(float) * channels * npix, cudaMemcpyDeviceToHost, st));
     CU_CHECK(cudaStreamSynchronize(st));
     return EZRT_OK;
 }

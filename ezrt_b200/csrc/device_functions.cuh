@@ -1542,10 +1542,13 @@ __device__ __forceinline__ vec3 nee_contrib(const SceneDev& sc, const RenderDev&
 // DEFER_NEE (wavefront pipeline, IS/MIS mode): the shadow ray carries the inputs of nee_contrib instead of its value -- the
 // BRDF / environment evaluation of the light sample runs after the shadow pass, only for the rays that got through, and is
 // no longer part of k_shade (5104 instructions, instruction-fetch bound).
-template <int MODE, bool DEFER_NEE = false>
+// AOV: at bounce 0 a surface hit also writes its first-hit record to aov_rec[0..1] = (base colour, t), (shading normal as
+// surface_hit returns it, 0) -- as soon as they are known, so that they are not held through the rest of the step.  A primary
+// miss writes nothing.
+template <int MODE, bool DEFER_NEE = false, bool AOV = false>
 __device__ __forceinline__ bool shade_step(const SceneDev& sc, const RenderDev& rd, int bounce, PathRegs& p, float hit_t,
                                            int hit_tri, uint32_t px, uint32_t py, float2 sob, vec3& Lo, vec3& Le,
-                                           bool& primary_miss, ShadowRay& sh) {
+                                           bool& primary_miss, ShadowRay& sh, float4* aov_rec = nullptr) {
     sh.valid = false;
     const int mode = (MODE < 0) ? rd.mode : MODE;
     const bool is_mode = (mode == EZRT_MODE_DISNEY_IS_MIS_P5);
@@ -1578,6 +1581,10 @@ __device__ __forceinline__ bool shade_step(const SceneDev& sc, const RenderDev& 
     MaterialDev mat = load_material(sc, hit.matId);
     if (bounce == 0) {
         Le = mat.emissive;  // P5/fsh:936
+        if (AOV) {
+            aov_rec[0] = make_float4(mat.baseColor.x, mat.baseColor.y, mat.baseColor.z, hit_t);
+            aov_rec[1] = make_float4(hit.N.x, hit.N.y, hit.N.z, 0.0f);
+        }
     } else {
         Lo = ez_add(Lo, contrib3(p.history, mat.emissive, p.f_r, p.cosine_i, p.pdf));
         p.history = ez_mul(p.history, ez_divs(ez_scale(p.f_r, p.cosine_i), p.pdf));

@@ -514,12 +514,16 @@ __global__ void __launch_bounds__(EZRT_EXTEND_MAX_THREADS, EZRT_EXTEND_LB_BLOCKS
 // LIST (the pass over the accel policy's deferred rays, on the side stream beside the main k_shade): entry k is queue entry /
 // sample slot list[k], its hit is side_hit[k]; nothing to do when the list overflowed (then the in-line exact pass filled the
 // queue's hit records and the main k_shade found no pending ones).
-template <int MODE, bool LIST>
+// AOV (feature-buffer renders): at bounce 0 every surface hit also writes its first-hit record, 32 bytes per sample slot:
+// aov_rec[2 slot] = (albedo, t), aov_rec[2 slot + 1] = (shading normal, 0).  A primary miss writes nothing (k_blend knows
+// it from Lo.w == 1).  The plain instantiations never touch aov_rec.
+template <int MODE, bool LIST, bool AOV = false>
 __global__ void __launch_bounds__(128, EZRT_SHADE_MIN_BLOCKS) k_shade(SceneDev sc, RenderDev rd, const TileDev* __restrict__ tiles, int bounce,
                                                uint32_t batch_first_frame, PathQueue qin, const uint32_t* __restrict__ in_count,
                                                PathQueue qout, uint32_t* out_count, ShadowQueue sq, uint32_t* s_count,
                                                float4* __restrict__ Lo, float4* __restrict__ Le, uint32_t n_fused, uint32_t n_frames,
-                                               const uint32_t* __restrict__ list, const float2* __restrict__ side_hit) {
+                                               const uint32_t* __restrict__ list, const float2* __restrict__ side_hit,
+                                               float4* __restrict__ aov_rec) {
     // The Sobol pair of (bounce, frame) is the same for every pixel of a frame (P5/fsh:361-376: up to 2 x 32 table XORs per path): each
     // block computes the pairs of the batch's frames once into shared memory (batches of more than EZRT_SOBOL_TABLE frames compute per path).
     __shared__ float2 s_sobol[EZRT_SOBOL_TABLE];
@@ -642,7 +646,8 @@ __global__ void __launch_bounds__(128, EZRT_SHADE_MIN_BLOCKS) k_shade(SceneDev s
             }
 #endif
             if (LIST || __float_as_int(hit.y) != EZRT_TRI_PENDING) {   // pending: deferred by the accel kernel, shaded by the LIST pass
-                alive = shade_step<MODE, MODE == EZRT_MODE_DISNEY_IS_MIS_P5>(sc, rd, bounce, p, hit.x, __float_as_int(hit.y), px, py, sob, lo, le, pmiss, sh);
+                alive = shade_step<MODE, MODE == EZRT_MODE_DISNEY_IS_MIS_P5, AOV>(sc, rd, bounce, p, hit.x, __float_as_int(hit.y), px, py, sob, lo, le,
+                                                                                 pmiss, sh, AOV ? aov_rec + 2 * (size_t)slot : nullptr);
                 if (bounce == 0) {
                     // Le is zero for every surface that does not emit: it is stored (and read back by k_blend) only otherwise.
                     // color = Le + Lo with Le = +-0 is Lo bit for bit, because Lo is never -0.0 (it starts at +0.0 and only grows by additions)
@@ -723,10 +728,13 @@ __device__ __forceinline__ size_t fb_index(const RenderDev& rd, const TileDev& t
 
 // ADAPTIVE: also the running mean of the squared sample luminance (luma2) and the frames the pixel received (spp_map), both
 // indexed like the framebuffer's pixels (ezrt_math.h, "adaptive sampling").  The plain instantiation never touches them.
-template <bool ADAPTIVE>
+// AOV (with ADAPTIVE; no spp map): also the running means of the first-hit features, 8 floats per pixel (albedo, coverage,
+// normal, depth; 0 for a primary miss) from the records k_shade<.., AOV> left in aov_rec, blended with the colour's weights.
+template <bool ADAPTIVE, bool AOV = false>
 __global__ void __launch_bounds__(256) k_blend(RenderDev rd, const TileDev* __restrict__ tiles, int nf, uint32_t batch_first_frame,
                                                const float4* __restrict__ Lo, const float4* __restrict__ Le, float* __restrict__ fb,
-                                               float* __restrict__ luma2, int32_t* __restrict__ spp_map) {
+                                               float* __restrict__ luma2, int32_t* __restrict__ spp_map,
+                                               const float4* __restrict__ aov_rec, float* __restrict__ aov) {
     uint32_t per_frame = (uint32_t)rd.n_tiles * EZRT_TILE_PIXELS;
     uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
     if (r >= per_frame) return;
@@ -739,6 +747,11 @@ __global__ void __launch_bounds__(256) k_blend(RenderDev rd, const TileDev* __re
     vec3 acc = (batch_first_frame == 0u) ? splat3(0.0f) : ez_v3(fb[idx], fb[idx + 1], fb[idx + 2]);
     float m2 = 0.0f;
     if (ADAPTIVE && batch_first_frame != 0u) m2 = luma2[pix];
+    float feat[8];
+    if (AOV) {
+#pragma unroll
+        for (int k = 0; k < 8; k++) feat[k] = (batch_first_frame == 0u) ? 0.0f : aov[pix * 8 + k];
+    }
     for (int f = 0; f < nf; f++) {
         float4 lo = Lo[(size_t)f * per_frame + r];
         vec3 color = ez_v3(lo.x, lo.y, lo.z);   // primary miss: the sky; no emission at the first hit: 0 + Lo = Lo
@@ -752,12 +765,28 @@ __global__ void __launch_bounds__(256) k_blend(RenderDev rd, const TileDev* __re
             const float y = ez_luminance(color);
             m2 = ez_mix(m2, y * y, a);
         }
+        if (AOV) {
+            float4 r0 = make_float4(0.0f, 0.0f, 0.0f, 0.0f), r1 = r0;
+            float cov = 0.0f;
+            if (lo.w != 1.0f) {   // Lo.w == 1: the primary ray left the scene
+                const size_t s = (size_t)f * per_frame + r;
+                r0 = aov_rec[2 * s];
+                r1 = aov_rec[2 * s + 1];
+                cov = 1.0f;
+            }
+            const float v[8] = {r0.x, r0.y, r0.z, cov, r1.x, r1.y, r1.z, r0.w};
+#pragma unroll
+            for (int k = 0; k < 8; k++) feat[k] = ez_mix(feat[k], v[k], a);
+        }
     }
     fb[idx] = acc.x; fb[idx + 1] = acc.y; fb[idx + 2] = acc.z;
     if (rd.out_channels == 4) fb[idx + 3] = 1.0f;
-    if (ADAPTIVE) {
-        luma2[pix] = m2;
-        spp_map[pix] = (int32_t)(batch_first_frame + (uint32_t)nf);
+    if (ADAPTIVE) luma2[pix] = m2;
+    if (ADAPTIVE && !AOV) spp_map[pix] = (int32_t)(batch_first_frame + (uint32_t)nf);
+    if (AOV) {
+        float4* o = (float4*)(aov + pix * 8);
+        o[0] = make_float4(feat[0], feat[1], feat[2], feat[3]);
+        o[1] = make_float4(feat[4], feat[5], feat[6], feat[7]);
     }
 }
 
@@ -974,6 +1003,75 @@ __global__ void k_partition_scatter(const float* __restrict__ compact, float* __
 }
 
 // ------------------------------------------------------------------------------------------
+// denoiser (ezrt_math.h "denoiser", DESIGN.md section 9): k_denoise_init, then one k_atrous per iteration.  cv holds
+// (colour, variance) per pixel; aov 2 float4 per pixel: (albedo, coverage), (normal, depth).  Full images, row-major.
+// ------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256) k_denoise_init(const float* __restrict__ color, int channels, const float* __restrict__ luma2,
+                                                      int n_frames, long long n, float4* __restrict__ cv) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const vec3 c = ez_v3(color[i * channels], color[i * channels + 1], color[i * channels + 2]);
+    cv[i] = make_float4(c.x, c.y, c.z, ez_denoise_var0(luma2[i], c, n_frames));
+}
+
+// One iteration, step s, one thread per pixel (16x16 blocks).  The last iteration writes the image (out, `channels` floats per
+// pixel, alpha copied from color_in, which may be out itself) instead of cv_out.
+__global__ void __launch_bounds__(256) k_atrous(int width, int height, int step, float sigma_l, float sigma_n, float sigma_z, float sigma_a,
+                                                const float4* __restrict__ cv_in, const float4* __restrict__ aov, float4* __restrict__ cv_out,
+                                                const float* color_in, float* out, int channels) {
+    const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y * blockDim.y + threadIdx.y;
+    if (x >= width || y >= height) return;
+    const size_t p = (size_t)y * width + x;
+    const float4 cp = cv_in[p];
+    float4 res = cp;
+    const float4 ap0 = aov[2 * p];
+    if (ap0.w != 0.0f) {   // coverage 0: passed through
+        const float4 ap1 = aov[2 * p + 1];
+        const vec3 a_p = ez_v3(ap0.x, ap0.y, ap0.z), n_p = ez_v3(ap1.x, ap1.y, ap1.z);
+        const float Y_p = ez_luminance(ez_v3(cp.x, cp.y, cp.z)), sd_p = EZ_SQRT(cp.w);
+        float sw = 0.0f, sv = 0.0f;
+        vec3 sc = splat3(0.0f);
+#pragma unroll 1
+        for (int j = -2; j <= 2; j++) {
+            const int qy = y + step * j;
+            if (qy < 0 || qy >= height) continue;
+#pragma unroll
+            for (int i = -2; i <= 2; i++) {
+                const int qx = x + step * i;
+                if (qx < 0 || qx >= width) continue;
+                const float h = ez_b3(i) * ez_b3(j);
+                float w;
+                float4 cq;
+                if (i == 0 && j == 0) {
+                    w = h;
+                    cq = cp;
+                } else {
+                    const size_t q = (size_t)qy * width + qx;
+                    cq = cv_in[q];
+                    const float4 aq0 = aov[2 * q];
+                    if (aq0.w == 0.0f || !ez_finite(cq.x) || !ez_finite(cq.y) || !ez_finite(cq.z) || !ez_finite(cq.w)) continue;
+                    const float4 aq1 = aov[2 * q + 1];
+                    const int d = max(abs(i), abs(j));
+                    w = ez_atrous_weight(h, (float)(step * d), n_p, ez_v3(aq1.x, aq1.y, aq1.z), ap1.w, aq1.w, Y_p, ez_luminance(ez_v3(cq.x, cq.y, cq.z)),
+                                         sd_p, a_p, ez_v3(aq0.x, aq0.y, aq0.z), sigma_l, sigma_n, sigma_z, sigma_a);
+                }
+                sw = sw + w;
+                sc = ez_add(sc, ez_scale(ez_v3(cq.x, cq.y, cq.z), w));
+                sv = sv + (w * w) * cq.w;
+            }
+        }
+        res = make_float4(EZ_DIV(sc.x, sw), EZ_DIV(sc.y, sw), EZ_DIV(sc.z, sw), EZ_DIV(sv, sw * sw));
+    }
+    if (out) {
+        const size_t o = p * (size_t)channels;
+        if (channels == 4) out[o + 3] = color_in[o + 3];
+        out[o] = res.x; out[o + 1] = res.y; out[o + 2] = res.z;
+    } else {
+        cv_out[p] = res;
+    }
+}
+
+// ------------------------------------------------------------------------------------------
 // launchers
 // ------------------------------------------------------------------------------------------
 static inline int div_up(long long a, long long b) { return (int)((a + b - 1) / b); }
@@ -1128,10 +1226,14 @@ void launch_shadow_accel(const SceneDev& sc, ShadowQueue sq, const uint32_t* s_c
 }
 void launch_shade(const SceneDev& sc, const RenderDev& rd, const TileDev* tiles, int bounce, uint32_t batch_first_frame,
                   PathQueue qin, const uint32_t* in_count, PathQueue qout, uint32_t* out_count, ShadowQueue sq,
-                  uint32_t* s_count, float4* Lo, float4* Le, uint32_t n_max, uint32_t n_fused, uint32_t n_frames, int n_sms, cudaStream_t st) {
+                  uint32_t* s_count, float4* Lo, float4* Le, uint32_t n_max, uint32_t n_fused, uint32_t n_frames, int n_sms, cudaStream_t st,
+                  float4* aov_rec) {
     int blocks = std::min(div_up(n_max, 128), n_sms * 4 * EZRT_SHADE_MIN_BLOCKS);
     if (blocks < 1) blocks = 1;
-#define EZRT_LAUNCH_SHADE(M) k_shade<M, false><<<blocks, 128, 0, st>>>(sc, rd, tiles, bounce, batch_first_frame, qin, in_count, qout, out_count, sq, s_count, Lo, Le, n_fused, n_frames, nullptr, nullptr)
+#define EZRT_LAUNCH_SHADE(M)                                                                                                                  \
+    if (aov_rec) k_shade<M, false, true><<<blocks, 128, 0, st>>>(sc, rd, tiles, bounce, batch_first_frame, qin, in_count, qout, out_count, sq, s_count, Lo, Le, \
+                                                                 n_fused, n_frames, nullptr, nullptr, aov_rec);                              \
+    else k_shade<M, false><<<blocks, 128, 0, st>>>(sc, rd, tiles, bounce, batch_first_frame, qin, in_count, qout, out_count, sq, s_count, Lo, Le, n_fused, n_frames, nullptr, nullptr, nullptr)
     switch (rd.mode) {
         case EZRT_MODE_DIFFUSE_P3: EZRT_LAUNCH_SHADE(EZRT_MODE_DIFFUSE_P3); break;
         case EZRT_MODE_DISNEY_ANISO_P4: EZRT_LAUNCH_SHADE(EZRT_MODE_DISNEY_ANISO_P4); break;
@@ -1146,10 +1248,13 @@ void launch_shade(const SceneDev& sc, const RenderDev& rd, const TileDev* tiles,
 void launch_deferred_lane(const SceneDev& sc, const RenderDev& rd, const TileDev* tiles, int bounce, uint32_t batch_first_frame, PathQueue qin,
                           const uint32_t* defer_list, const uint32_t* defer_count, uint32_t* defer_work, float2* side_hit, PathQueue qout,
                           uint32_t* out_count, ShadowQueue sq, uint32_t* s_count, float4* Lo, float4* Le, uint32_t n_fused, uint32_t n_frames,
-                          int n_sms, cudaStream_t st) {
+                          int n_sms, cudaStream_t st, float4* aov_rec) {
     launch_extend(sc, true, false, qin, defer_count, defer_work, defer_list, 1, EZRT_SIDE_CAP, n_sms, st, side_hit, 1);
     const int blocks = 8;
-#define EZRT_LAUNCH_SHADE(M) k_shade<M, true><<<blocks, 128, 0, st>>>(sc, rd, tiles, bounce, batch_first_frame, qin, defer_count, qout, out_count, sq, s_count, Lo, Le, n_fused, n_frames, defer_list, side_hit)
+#define EZRT_LAUNCH_SHADE(M)                                                                                                                  \
+    if (aov_rec) k_shade<M, true, true><<<blocks, 128, 0, st>>>(sc, rd, tiles, bounce, batch_first_frame, qin, defer_count, qout, out_count, sq, s_count, Lo, \
+                                                                Le, n_fused, n_frames, defer_list, side_hit, aov_rec);                         \
+    else k_shade<M, true><<<blocks, 128, 0, st>>>(sc, rd, tiles, bounce, batch_first_frame, qin, defer_count, qout, out_count, sq, s_count, Lo, Le, n_fused, n_frames, defer_list, side_hit, nullptr)
     switch (rd.mode) {
         case EZRT_MODE_DIFFUSE_P3: EZRT_LAUNCH_SHADE(EZRT_MODE_DIFFUSE_P3); break;
         case EZRT_MODE_DISNEY_ANISO_P4: EZRT_LAUNCH_SHADE(EZRT_MODE_DISNEY_ANISO_P4); break;
@@ -1165,12 +1270,17 @@ void launch_nee(const SceneDev& sc, const RenderDev& rd, ShadowQueue sq, const u
 void launch_blend(const RenderDev& rd, const TileDev* tiles, int nf, uint32_t batch_first_frame, const float4* Lo,
                   const float4* Le, float* fb, cudaStream_t st) {
     uint32_t per_frame = (uint32_t)rd.n_tiles * EZRT_TILE_PIXELS;
-    k_blend<false><<<div_up(per_frame, 256), 256, 0, st>>>(rd, tiles, nf, batch_first_frame, Lo, Le, fb, nullptr, nullptr);
+    k_blend<false><<<div_up(per_frame, 256), 256, 0, st>>>(rd, tiles, nf, batch_first_frame, Lo, Le, fb, nullptr, nullptr, nullptr, nullptr);
+}
+void launch_blend_aov(const RenderDev& rd, const TileDev* tiles, int nf, uint32_t batch_first_frame, const float4* Lo, const float4* Le,
+                      const float4* aov_rec, float* fb, float* aov, float* luma2, cudaStream_t st) {
+    uint32_t per_frame = (uint32_t)rd.n_tiles * EZRT_TILE_PIXELS;
+    k_blend<true, true><<<div_up(per_frame, 256), 256, 0, st>>>(rd, tiles, nf, batch_first_frame, Lo, Le, fb, luma2, nullptr, aov_rec, aov);
 }
 void launch_blend_adaptive(const RenderDev& rd, const TileDev* tiles, int nf, uint32_t batch_first_frame, const float4* Lo,
                            const float4* Le, float* fb, float* luma2, int32_t* spp_map, cudaStream_t st) {
     uint32_t per_frame = (uint32_t)rd.n_tiles * EZRT_TILE_PIXELS;
-    k_blend<true><<<div_up(per_frame, 256), 256, 0, st>>>(rd, tiles, nf, batch_first_frame, Lo, Le, fb, luma2, spp_map);
+    k_blend<true><<<div_up(per_frame, 256), 256, 0, st>>>(rd, tiles, nf, batch_first_frame, Lo, Le, fb, luma2, spp_map, nullptr, nullptr);
 }
 void launch_adaptive_check(const RenderDev& rd, const TileDev* tiles_in, int n_frames, float threshold, const float* fb, const float* luma2,
                            unsigned char* keep, unsigned int* blocks_done, TileDev* tiles_out, int32_t* counts, cudaStream_t st) {
@@ -1206,4 +1316,16 @@ void launch_partition_scatter(const float* compact, float* full, const TileDev* 
                               cudaStream_t st) {
     if (n_tiles <= 0) return;
     k_partition_scatter<<<div_up((long long)n_tiles * EZRT_TILE_PIXELS, 256), 256, 0, st>>>(compact, full, tiles, n_tiles, width, channels);
+}
+void launch_denoise(const float* color, int channels, const float* aov, const float* luma2, int n_frames, int width, int height, int iterations,
+                    float sigma_l, float sigma_n, float sigma_z, float sigma_a, float4* cv0, float4* cv1, float* out, cudaStream_t st) {
+    const long long n = (long long)width * height;
+    if (n <= 0) return;
+    k_denoise_init<<<div_up(n, 256), 256, 0, st>>>(color, channels, luma2, n_frames, n, cv0);
+    const dim3 block(16, 16), grid(div_up(width, 16), div_up(height, 16));
+    for (int k = 0; k < iterations; k++) {
+        const bool last = (k == iterations - 1);
+        k_atrous<<<grid, block, 0, st>>>(width, height, 1 << k, sigma_l, sigma_n, sigma_z, sigma_a, (k & 1) ? cv1 : cv0, (const float4*)aov,
+                                         (k & 1) ? cv0 : cv1, color, last ? out : nullptr, channels);
+    }
 }

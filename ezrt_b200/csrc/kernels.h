@@ -33,14 +33,15 @@ void launch_shadow_accel(const SceneDev& sc, ShadowQueue sq, const uint32_t* s_c
                          uint32_t* defer_count, uint32_t* defer_work, uint32_t n_max, int n_sms, unsigned long long* counts, cudaStream_t st);
 void launch_shade(const SceneDev& sc, const RenderDev& rd, const TileDev* tiles, int bounce, uint32_t batch_first_frame,
                   PathQueue qin, const uint32_t* in_count, PathQueue qout, uint32_t* out_count, ShadowQueue sq,
-                  uint32_t* s_count, float4* Lo, float4* Le, uint32_t n_max, uint32_t n_fused, uint32_t n_frames, int n_sms, cudaStream_t st);
+                  uint32_t* s_count, float4* Lo, float4* Le, uint32_t n_max, uint32_t n_fused, uint32_t n_frames, int n_sms, cudaStream_t st,
+                  float4* aov_rec = nullptr);   // aov_rec: feature-buffer render, bounce 0 writes the first-hit records (k_shade<.., AOV>)
 void launch_extend_camera(const SceneDev& sc, const RenderDev& rd, const TileDev* tiles, uint32_t batch_first_frame, uint32_t n_slots, uint32_t n_frames, PathQueue q,
                           uint32_t* work, uint32_t* defer_list, uint32_t* defer_count, uint32_t* defer_work, int n_sms, unsigned long long* counts,
                           cudaStream_t st, int exact_gate = 0);
 void launch_deferred_lane(const SceneDev& sc, const RenderDev& rd, const TileDev* tiles, int bounce, uint32_t batch_first_frame, PathQueue qin,
                           const uint32_t* defer_list, const uint32_t* defer_count, uint32_t* defer_work, float2* side_hit, PathQueue qout,
                           uint32_t* out_count, ShadowQueue sq, uint32_t* s_count, float4* Lo, float4* Le, uint32_t n_fused, uint32_t n_frames,
-                          int n_sms, cudaStream_t st);
+                          int n_sms, cudaStream_t st, float4* aov_rec = nullptr);
 // after a shadow pass (accel or exact, including the exact pass over deferred shadow rays): contributions of the unoccluded light samples
 void launch_nee(const SceneDev& sc, const RenderDev& rd, ShadowQueue sq, const uint32_t* s_count, float4* Lo, uint32_t n_max, int n_sms, cudaStream_t st);
 void launch_blend(const RenderDev& rd, const TileDev* tiles, int nf, uint32_t batch_first_frame, const float4* Lo,
@@ -48,6 +49,9 @@ void launch_blend(const RenderDev& rd, const TileDev* tiles, int nf, uint32_t ba
 // adaptive sampling: k_blend<true> also keeps the running mean of the squared sample luminance and the per-pixel frame count
 void launch_blend_adaptive(const RenderDev& rd, const TileDev* tiles, int nf, uint32_t batch_first_frame, const float4* Lo,
                            const float4* Le, float* fb, float* luma2, int32_t* spp_map, cudaStream_t st);
+// feature-buffer render: k_blend<true, true> also blends the first-hit records of aov_rec into aov (8 floats per pixel) and keeps luma2
+void launch_blend_aov(const RenderDev& rd, const TileDev* tiles, int nf, uint32_t batch_first_frame, const float4* Lo, const float4* Le,
+                      const float4* aov_rec, float* fb, float* aov, float* luma2, cudaStream_t st);
 // convergence test of the rd.n_tiles tiles of tiles_in after n_frames frames: the surviving tiles -> tiles_out (input order),
 // counts[0] = surviving tiles, counts[1] = their in-image pixels; keep holds rd.n_tiles bytes, *blocks_done must be 0 (left 0)
 void launch_adaptive_check(const RenderDev& rd, const TileDev* tiles_in, int n_frames, float threshold, const float* fb, const float* luma2,
@@ -64,5 +68,9 @@ void launch_eval_math(int which, int n, const float* a, const float* b, float* o
 void launch_tonemap(const float* in, int channels, float* out, long long n, float limit, cudaStream_t st);
 void launch_partition_scatter(const float* compact, float* full, const TileDev* tiles, int n_tiles, int width, int channels,
                               cudaStream_t st);
+// the a-trous denoiser over a full width x height image: colour (channels 3 or 4) + aov (8 floats, 16-byte aligned) + luma2 after
+// n_frames frames -> out (may be color); cv0, cv1: width * height float4 each (ping-pong)
+void launch_denoise(const float* color, int channels, const float* aov, const float* luma2, int n_frames, int width, int height, int iterations,
+                    float sigma_l, float sigma_n, float sigma_z, float sigma_a, float4* cv0, float4* cv1, float* out, cudaStream_t st);
 
 #endif

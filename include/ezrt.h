@@ -176,6 +176,41 @@ int ezrt_render_adaptive_device(ezrt_scene* scene, const ezrt_render_params* par
 int ezrt_render_adaptive(ezrt_scene* scene, const ezrt_render_params* params, const ezrt_adaptive_params* adaptive,
                          float* framebuffer, int32_t* spp, float* luma2);
 
+/* Feature buffers (AOVs; DESIGN.md section 9): a plain render (params->spp frames from params->first_frame, the same
+ * framebuffer bits as ezrt_render_device) that also returns, per pixel, running means over its frames with the colour's
+ * weights (mix(acc, v, 1/(frame+1)) in frame order):
+ *   d_aov:   8 floats: albedo.rgb (the first hit's base colour), coverage (1 hit, 0 miss), normal.xyz (the first hit's shading
+ *            normal, flipped when hit from inside), depth (the first hit's distance); a primary miss contributes 0 to all 8.
+ *            16-byte aligned.
+ *   d_luma2: float, the running mean of the squared sample luminance (M of ezrt_math.h, bit for bit the adaptive render's).
+ * When first_frame > 0 all three buffers are in/out.  Layout of the framebuffer's pixels (tile-major compact when
+ * part_count > 1; ezrt_partition_scatter with channels = 8 / 1 scatters them).  Wavefront pipeline only.  The scratch
+ * grows by 32 bytes per sample slot for these renders only. */
+int ezrt_render_aov_device(ezrt_scene* scene, const ezrt_render_params* params, float* d_framebuffer, float* d_aov, float* d_luma2,
+                           void* cuda_stream);
+/* Same with host buffers (synchronous). */
+int ezrt_render_aov(ezrt_scene* scene, const ezrt_render_params* params, float* framebuffer, float* aov, float* luma2);
+
+/* Denoiser (DESIGN.md section 9; defined in ezrt_math.h): edge-avoiding a-trous wavelet filter with a variance-guided
+ * luminance weight, over a full width x height image (row-major; gather the parts of a partitioned render first). */
+typedef struct ezrt_denoise_params {
+    int32_t iterations;   /* 1..10: passes with steps 1, 2, 4, ... */
+    float sigma_l;        /* > 0: luminance weight, in standard deviations */
+    float sigma_n;        /* > 0: normal weight, exponent of dot(n_p, n_q) */
+    float sigma_z;        /* > 0: depth weight, relative depth difference per pixel of step */
+    float sigma_a;        /* > 0: albedo weight, L1 distance */
+    int32_t reserved;     /* 0 */
+} ezrt_denoise_params;
+
+/* d_color: channels (3 or 4) floats per pixel after n_frames frames; d_aov, d_luma2: ezrt_render_aov_device's outputs of the same
+ * render.  d_out may be d_color; alpha is copied.  Enqueued on cuda_stream; the scratch (32 bytes per pixel) belongs to the scene
+ * like the render's, so it is ordered with the scene's renders the same way. */
+int ezrt_denoise_device(ezrt_scene* scene, const ezrt_denoise_params* params, const float* d_color, int channels, const float* d_aov,
+                        const float* d_luma2, int width, int height, int n_frames, float* d_out, void* cuda_stream);
+/* Same with host buffers (synchronous); out may be color. */
+int ezrt_denoise(ezrt_scene* scene, const ezrt_denoise_params* params, const float* color, int channels, const float* aov,
+                 const float* luma2, int width, int height, int n_frames, float* out);
+
 /* Counters of the most recent render on this scene (synchronises the stream). */
 int ezrt_get_counters(ezrt_scene* scene, ezrt_counters* out);
 

@@ -308,11 +308,44 @@ EZ_HD ez_vec3 ez_tonemap_pass3(ez_vec3 c, float limit) {
  * The floor lets black pixels with zero variance converge. */
 #define EZRT_ADAPTIVE_LUMA_FLOOR 1e-3f
 
+/* the per-sample variance of the luminance: max(M - Y*Y, 0), NaN stays NaN */
+EZ_HD float ez_luma_variance(float M, float Y) {
+    float var = M - Y * Y;
+    return (var < 0.0f) ? 0.0f : var;
+}
+
 EZ_HD float ez_adaptive_error(float M, ez_vec3 mean, int n) {
     float Y = ez_luminance(mean);
-    float var = M - Y * Y;
-    var = (var < 0.0f) ? 0.0f : var;
+    float var = ez_luma_variance(M, Y);
     return EZ_DIV(EZ_SQRT(EZ_DIV(var, (float)n)), Y + EZRT_ADAPTIVE_LUMA_FLOOR);
+}
+
+/* ------------------------------------------------------------------ denoiser (DESIGN.md section 9)
+ * Edge-avoiding a-trous wavelet filter (Dammertz et al. 2010) with SVGF's variance-guided luminance weight (Schied et al.
+ * 2017), no temporal part.  Per pixel: colour c, variance v of the mean's luminance, and the first-hit feature buffers of
+ * the render (albedo a, coverage, normal n, depth z; means over the frames).  Start:  c = colour, v = ez_denoise_var0.
+ * Iteration k (step s = 2^k): taps q = p + s*(i, j), j outer, i inner, both -2..2; taps outside the image are skipped.
+ *   centre tap:  w = h = b3(i) * b3(j)
+ *   other taps:  skipped if coverage_p == 0 or coverage_q == 0 or c_q / v_q is not finite; else w = ez_atrous_weight(...)
+ *   c' = (sum w c_q) / (sum w),   v' = (sum (w*w) v_q) / ((sum w) * (sum w)),   sums in tap order, plain fp32 adds.
+ * A pixel with coverage 0 (no surface in any frame) is passed through unchanged. */
+#define EZRT_DENOISE_LUMA_EPS 1e-4f
+
+EZ_HD int ez_finite(float x) { return (ez_f2u(x) & 0x7f800000u) != 0x7f800000u; }
+/* the B3 spline {1/16, 1/4, 3/8, 1/4, 1/16} at i = -2..2 */
+EZ_HD float ez_b3(int i) { return (i == 0) ? 0.375f : ((i == 1 || i == -1) ? 0.25f : 0.0625f); }
+/* start variance: that of the mean's luminance after n frames, max(M - Y*Y, 0) / n (the term inside ez_adaptive_error) */
+EZ_HD float ez_denoise_var0(float M, ez_vec3 mean, int n) { return EZ_DIV(ez_luma_variance(M, ez_luminance(mean)), (float)n); }
+/* weight of tap q of pixel p: h = b3(i) b3(j), s_dist = s * max(|i|, |j|), sd_p = sqrt(v_p), Y = ez_luminance(c) */
+EZ_HD float ez_atrous_weight(float h, float s_dist, ez_vec3 n_p, ez_vec3 n_q, float z_p, float z_q, float Y_p, float Y_q, float sd_p,
+                             ez_vec3 a_p, ez_vec3 a_q, float sigma_l, float sigma_n, float sigma_z, float sigma_a) {
+    const float d = ez_dot(n_p, n_q);
+    const float w_n = (d > 0.0f) ? ez_pow(d, sigma_n) : 0.0f;
+    const float w_z = ez_exp(-EZ_DIV(ez_abs(z_p - z_q), (sigma_z * z_p) * s_dist));
+    const float w_l = ez_exp(-EZ_DIV(ez_abs(Y_p - Y_q), sigma_l * sd_p + EZRT_DENOISE_LUMA_EPS));
+    const float da = (ez_abs(a_p.x - a_q.x) + ez_abs(a_p.y - a_q.y)) + ez_abs(a_p.z - a_q.z);
+    const float w_a = ez_exp(-EZ_DIV(da, sigma_a));
+    return (((h * w_n) * w_z) * w_l) * w_a;
 }
 
 #endif /* EZRT_MATH_H */
