@@ -81,7 +81,7 @@ struct ezrt_scene {
     int n_sms = 148;
     SceneDev dev{};
     DeviceBuffer nodes, tri_geo, tri_shade, materials, hdr, hdr_cache;
-    DeviceBuffer acc_hot, acc_tri_ref, tri_leaf, leaf_box, defer_buf, acc_tri_leaf, ref_to_acc, acc_wide, acc_wide_q16;   // acc_hot = W8 nodes | geometry | shading records of the accel order
+    DeviceBuffer acc_hot, acc_tri_ref, tri_leaf, leaf_box, defer_buf, acc_tri_leaf, ref_to_acc, acc_wide, acc_wide_q16;   // acc_hot = W8 nodes | geometry (| vertices) | shading records of the accel order
     int acc_depth = 0;
     int n_materials = 0;
     int tree_depth = 0;
@@ -92,7 +92,7 @@ struct ezrt_scene {
     // feature-buffer renders: the first-hit records of a batch (32 B per sample slot); the host entry point's aov + luma2.
     // The denoiser: its ping-pong (colour, variance) images; the host entry point's device copies of its inputs
     DeviceBuffer aov_rec_buf, aov_maps_buf, denoise_buf, denoise_io_buf;
-    void* hot_base = nullptr;   // accel nodes | geometry | shading records (L2 persisting window)
+    void* hot_base = nullptr;   // accel nodes | geometry (| vertices) | shading records (L2 persisting window)
     size_t hot_bytes = 0;
     size_t l2_persist_bytes = 0;
     size_t max_window_bytes = 0;  // persisting L2 set-aside granted by the device (0 = feature off)
@@ -573,7 +573,7 @@ int ezrt_scene_create(int device, const float* tris, int n_triangles, const floa
     // acceleration tree nodes | triangle geometry | shading records in ONE allocation: the window the
     // L2 persisting-access policy is set on while a render runs (the data every ray touches at random)
     const size_t acc_nodes_bytes = ((std::max<size_t>(w8_words.size(), 4) * sizeof(uint32_t) + 255) / 256) * 256;
-    const size_t acc_geo_bytes = (((size_t)n_triangles * 4 * sizeof(float4) + 255) / 256) * 256;
+    size_t acc_geo_bytes = (((size_t)n_triangles * 4 * sizeof(float4) + 255) / 256) * 256;   // flat; the indexed layout below shrinks it
     const size_t acc_shade_bytes = (((size_t)n_triangles * 3 * sizeof(float4) + 255) / 256) * 256;
     if (!rc) rc = sc->acc_hot.ensure(acc_nodes_bytes + acc_geo_bytes + acc_shade_bytes);
     if (!rc) {
@@ -599,6 +599,46 @@ int ezrt_scene_create(int device, const float* tris, int n_triangles, const floa
                               (char*)sc->acc_hot.p + acc_nodes_bytes, (char*)sc->acc_hot.p + acc_nodes_bytes + acc_geo_bytes,
                               (int*)sc->acc_tri_leaf.p, (uint32_t*)sc->ref_to_acc.p);
     sub("gather");
+    // The W8 form's triangle records, indexed where that is smaller (32 T + 16 V < 64 T): 32 B per triangle, (N, d0) (i1, i2, i3, 0),
+    // plus 16 B per distinct vertex position, numbered by first use in the tree's order, instead of 64 B per triangle.  A scene that
+    // shares its vertices (a mesh: about one vertex per two triangles) then keeps its triangle records in H100's 50 MB L2 up to
+    // about 1.2 M triangles instead of 0.8 M (DESIGN.md section 4); a triangle soup keeps the flat records.  The 4-wide form and the
+    // reference-order tri_geo are always flat.
+    size_t acc_vert_bytes = 0;
+    int n_vert = 0;
+    bool tri_indexed = false;
+    if (!rc && !w8_words.empty()) {
+        DeviceBuffer ids, hot;
+        rc = ids.ensure((size_t)n_triangles * 6 * sizeof(uint32_t));
+        uint32_t* vid = (uint32_t*)ids.p;
+        uint32_t* vert_src = vid + (size_t)n_triangles * 3;
+        if (!rc) rc = ezrt_prep_vertex_ids((const char*)sc->acc_hot.p + acc_nodes_bytes, n_triangles, vid, vert_src, n_vert);
+        if (!rc && 32 * (size_t)n_triangles + 16 * (size_t)n_vert < 64 * (size_t)n_triangles) {
+            const size_t rec_bytes = (((size_t)n_triangles * 2 * sizeof(float4) + 255) / 256) * 256;
+            const size_t vert_bytes = (((size_t)n_vert * sizeof(float4) + 255) / 256) * 256;
+            rc = hot.ensure(acc_nodes_bytes + rec_bytes + vert_bytes + acc_shade_bytes);
+            const char* old_base = (const char*)sc->acc_hot.p;
+            char* base = (char*)hot.p;
+            if (!rc && (cudaMemcpy(base, old_base, acc_nodes_bytes, cudaMemcpyDeviceToDevice) != cudaSuccess ||
+                        cudaMemcpy(base + acc_nodes_bytes + rec_bytes + vert_bytes, old_base + acc_nodes_bytes + acc_geo_bytes, acc_shade_bytes,
+                                   cudaMemcpyDeviceToDevice) != cudaSuccess))
+                rc = ezrt_set_error(EZRT_ERR_CUDA, "scene_create: copy failed: %s", cudaGetErrorString(cudaGetLastError()));
+            if (!rc) rc = ezrt_prep_indexed(old_base + acc_nodes_bytes, n_triangles, vid, vert_src, n_vert, base + acc_nodes_bytes, base + acc_nodes_bytes + rec_bytes);
+            if (!rc) {
+                std::swap(sc->acc_hot, hot);
+                acc_geo_bytes = rec_bytes;
+                acc_vert_bytes = vert_bytes;
+                tri_indexed = true;
+                sc->hot_base = sc->acc_hot.p;
+                sc->hot_bytes = acc_nodes_bytes + acc_geo_bytes + acc_vert_bytes + acc_shade_bytes;
+            }
+        }
+        hot.release();
+        ids.release();
+    }
+    if (verbose && !rc && !w8_words.empty())
+        fprintf(stderr, "[ezrt_scene_create] triangle records: %s (%d triangles, %d distinct vertices)\n", tri_indexed ? "indexed" : "flat", n_triangles, n_vert);
+    sub("indexed triangle records");
     if (!rc && hdr) rc = upload(sc->hdr, hdr, sizeof(float) * 3 * (size_t)hdr_w * hdr_h);
     if (!rc && hdr_cache) rc = upload(sc->hdr_cache, hdr_cache, sizeof(float) * 3 * (size_t)hdr_w * hdr_h);
     sub("environment map, cache");
@@ -633,6 +673,8 @@ int ezrt_scene_create(int device, const float* tris, int n_triangles, const floa
     d.w8_tri_weight = 1;   // cooperative triangle step: 1 over 2 is +1 % on C3 and C4 (H100, DESIGN.md section 6)
     if (const char* e = getenv("EZRT_TRI_W")) d.w8_tri_weight = std::max(1, std::min(64, atoi(e)));
     d.acc_tri_geo = (const float4*)((const char*)sc->acc_hot.p + acc_nodes_bytes);
+    d.acc_tri_vert = tri_indexed ? (const float4*)((const char*)sc->acc_hot.p + acc_nodes_bytes + acc_geo_bytes) : nullptr;
+    d.acc_tri_indexed = tri_indexed ? 1 : 0;
     d.acc_tri_ref = (const uint32_t*)sc->acc_tri_ref.p;
     d.acc_wide_nodes = acc_wide.empty() ? nullptr : (const float4*)sc->acc_wide.p;
     d.acc_wide_root_ref = acc_wide_root;
@@ -640,7 +682,7 @@ int ezrt_scene_create(int device, const float* tris, int n_triangles, const floa
     d.q16_decode_bits = 0x4B000000u;
     d.tri_l1_bypass = ((size_t)n_triangles * 64 > ((size_t)4 << 20)) ? 1 : 0;  // > 4 MB of triangle records: stream them past L1
     if (const char* e = getenv("EZRT_TRI_L1_BYPASS")) d.tri_l1_bypass = atoi(e) != 0;
-    d.acc_tri_shade = (const float4*)((const char*)sc->acc_hot.p + acc_nodes_bytes + acc_geo_bytes);
+    d.acc_tri_shade = (const float4*)((const char*)sc->acc_hot.p + acc_nodes_bytes + acc_geo_bytes + acc_vert_bytes);
     d.acc_tri_leaf = (const int*)sc->acc_tri_leaf.p;
     d.ref_to_acc = (const uint32_t*)sc->ref_to_acc.p;
     d.tri_leaf = (const int*)sc->tri_leaf.p;

@@ -374,6 +374,36 @@ __device__ __forceinline__ int tri_test_t(const float4* __restrict__ rec, vec3 o
     tout = t;
     return (TIES && t == best) ? 2 : 1;
 }
+// The same test, statement for statement, on an indexed record (N, d0) (i1, i2, i3, 0) and the vertex array: both halves of
+// the record are loaded together (one 32-byte sector); the three vertices, independent of each other, for the candidates past
+// the distance checks.  The vertices are read through L1 even where the records bypass it: the triangles of a leaf, tested by
+// neighbouring lanes and steps, share them (C3, H100: 3 % faster than with the vertices past L1, which was no faster than flat).
+template <bool TIES>
+__device__ __forceinline__ int tri_test_idx_t(const float4* __restrict__ rec, const float4* __restrict__ vert, vec3 o, vec3 d, float best, float& tout,
+                                              const bool l1_bypass) {
+    const float4 q0 = l1_bypass ? ldg4_na(rec) : ldg4(rec);
+    const float4 qi = l1_bypass ? ldg4_na(rec + 1) : ldg4(rec + 1);
+    vec3 N = f4xyz(q0);
+    float nd = ez_dot(N, d);
+    if (ez_abs(nd) < 0.00001f) return 0;
+    float t = EZ_DIV(q0.w - ez_dot(o, N), nd);
+    if (t < 0.0005f) return 0;
+    if (TIES ? !(t <= best) : !(t < best)) return 0;
+    const float4* v1 = vert + __float_as_uint(qi.x);
+    const float4* v2 = vert + __float_as_uint(qi.y);
+    const float4* v3 = vert + __float_as_uint(qi.z);
+    const float4 q1 = ldg4(v1), q2 = ldg4(v2), q3 = ldg4(v3);   // through L1 whatever l1_bypass: the triangles of a leaf share them
+    vec3 p1 = f4xyz(q1), p2 = f4xyz(q2), p3 = f4xyz(q3);
+    vec3 P = ez_add(o, ez_scale(d, t));
+    float s1 = ez_dot(ez_cross(ez_sub(p2, p1), ez_sub(P, p1)), N);
+    float s2 = ez_dot(ez_cross(ez_sub(p3, p2), ez_sub(P, p2)), N);
+    float s3 = ez_dot(ez_cross(ez_sub(p1, p3), ez_sub(P, p3)), N);
+    bool r1 = (s1 > 0.0f && s2 > 0.0f && s3 > 0.0f);
+    bool r2 = (s1 < 0.0f && s2 < 0.0f && s3 < 0.0f);
+    if (!(r1 || r2)) return 0;
+    tout = t;
+    return (TIES && t == best) ? 2 : 1;
+}
 __device__ __forceinline__ bool tri_test(const float4* __restrict__ rec, vec3 o, vec3 d, float best, float& tout) {
     return tri_test_t<false>(rec, o, d, best, tout) != 0;
 }
@@ -895,7 +925,9 @@ __device__ __forceinline__ int nth_set_bit(uint32_t m, int r) {
 
 // s_perm: 8 x 256 bytes in shared memory, s_perm[m * 256 + x] = the bits of x moved from position s to position s ^ m
 // stack : uint2 [entries][blockDim.x] in shared memory
-template <bool ANYHIT, bool COUNT, class RayIO>
+// IDX: the scene's triangle records are indexed (SceneDev::acc_tri_indexed; one instantiation per layout keeps each within 64
+// registers without spilling)
+template <bool ANYHIT, bool COUNT, bool IDX, class RayIO>
 __device__ __forceinline__ void extend_w8(const SceneDev& sc, uint32_t n, uint32_t* work, RayIO io, const unsigned char* s_perm, uint2* stack_sm,
                                           W8Counts counts) {
     const bool tri_na = sc.tri_l1_bypass != 0;
@@ -1098,7 +1130,8 @@ __device__ __forceinline__ void extend_w8(const SceneDev& sc, uint32_t n, uint32
                 int r = 0;
                 if (act) {
                     if (COUNT) n_tests++;
-                    r = tri_test_t<true>(sc.acc_tri_geo + (size_t)tri * 4, ro, rd, rbest, t, tri_na);
+                    r = IDX ? tri_test_idx_t<true>(sc.acc_tri_geo + (size_t)tri * 2, sc.acc_tri_vert, ro, rd, rbest, t, tri_na)
+                            : tri_test_t<true>(sc.acc_tri_geo + (size_t)tri * 4, ro, rd, rbest, t, tri_na);
                 }
                 const uint32_t taken = owns ? min(cnt, 32u - first) : 0u;   // this lane's pairs tested in this step ...
                 const unsigned seg = (taken == 32u) ? FULL : ((1u << taken) - 1u) << (first & 31u);   // ... by these lanes
@@ -1193,9 +1226,20 @@ struct SurfaceHit {
 
 // Recomputes P and the interpolated normal for (ray, t, tri).  p3fudge selects the P3/P4
 // barycentric denominators (P3/fsh:273-274) instead of P5's "+1e-7" (P5/fsh:206-207).
+// The (N, d0) quad of triangle `tri` in the policy's index space: the first 16 bytes of its flat or indexed record.
+__device__ __forceinline__ const float4* tri_geo_rec(const SceneDev& sc, int tri, bool accel_space) {
+    return accel_space ? sc.acc_tri_geo + (size_t)tri * (sc.acc_tri_indexed ? 2 : 4) : sc.tri_geo + (size_t)tri * 4;
+}
 __device__ __forceinline__ SurfaceHit surface_hit(const SceneDev& sc, vec3 o, vec3 d, float t, int tri, bool p3fudge, bool accel_space = false) {
-    const float4* g = (accel_space ? sc.acc_tri_geo : sc.tri_geo) + (size_t)tri * 4;
-    float4 q0 = ldg4(g), q1 = ldg4(g + 1), q2 = ldg4(g + 2), q3 = ldg4(g + 3);
+    // vertices: v[i1], v[i2], v[i3] of the vertex array (indexed record) or g[1], g[2], g[3] (flat record)
+    const float4* g = tri_geo_rec(sc, tri, accel_space);
+    const float4* v = g;
+    uint32_t i1 = 1u, i2 = 2u, i3 = 3u;
+    if (accel_space && sc.acc_tri_indexed) {
+        const uint4 qi = __ldg(reinterpret_cast<const uint4*>(g + 1));
+        v = sc.acc_tri_vert; i1 = qi.x; i2 = qi.y; i3 = qi.z;
+    }
+    float4 q0 = ldg4(g), q1 = ldg4(v + i1), q2 = ldg4(v + i2), q3 = ldg4(v + i3);
     const float4* s = (accel_space ? sc.acc_tri_shade : sc.tri_shade) + (size_t)tri * 3;
     float4 m0 = ldg4(s), m1 = ldg4(s + 1), m2 = ldg4(s + 2);
     vec3 p1 = f4xyz(q1), p2 = f4xyz(q2), p3 = f4xyz(q3);

@@ -13,6 +13,8 @@
 //   triangle geometry (64 B): q0 = (p1, N.x) q1 = (p2, N.y) q2 = (p3, N.z) q3 = (d0,0,0,0)
 //       N = normalize(cross(p2-p1, p3-p1)) and d0 = dot(N,p1) are the ray-independent part of
 //       hitTriangle (P5/fsh:172,184), evaluated once with the same fp32 operations.
+//       (the accel-order copy of an 8-wide scene that shares its vertices is indexed instead, 32 B: (N, d0) (i1, i2, i3, 0)
+//       into a 16-byte vertex array (x, y, z, 0); SceneDev::acc_tri_indexed, DESIGN.md section 4)
 //   triangle shading (48 B): (n1, matId) (n2, 0) (n3, 0)  -- fetched only for the final hit
 //   material table (80 B each): the 18-float material block de-duplicated (SURVEY.md 0: materials
 //       are stored per triangle in the reference), padded to 5 x float4.
@@ -50,7 +52,9 @@ struct SceneDev {
     int root_ref;
     // acceleration tree (default traversal policy): sentinel-free SAH over the same triangles, boxes
     // inflated by 2*prune_delta; acc_tri_geo is tri_geo in the tree's own order, acc_tri_ref maps back
-    const float4* acc_tri_geo;
+    const float4* acc_tri_geo;     // flat: 4 float4 per triangle as tri_geo; indexed: 2 per triangle, (N, d0) (i1, i2, i3, 0 as int bits)
+    const float4* acc_tri_vert;    // indexed layout: the distinct vertex positions (x, y, z, 0) of acc_tri_geo, numbered by first use
+    int acc_tri_indexed;           // 1: acc_tri_geo holds 32-byte indexed records (W8 scenes whose vertices are shared), 0: flat
     const uint32_t* acc_tri_ref;   // accel order -> reference triangle index
     const uint32_t* ref_to_acc;    // reference triangle index -> accel order
     const float4* acc_tri_shade;   // tri_shade in accel order (shading reads the arrays traversal keeps hot in L2)

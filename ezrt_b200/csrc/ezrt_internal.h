@@ -92,6 +92,12 @@ int ezrt_prep_records(const float* d_raw, int n, void* d_geo, void* d_shade, Ezr
 // the same records gathered into the acceleration tree's triangle order (d_order[i] = caller index of tree triangle i)
 int ezrt_prep_gather(const void* d_geo, const void* d_shade, const int* d_tri_leaf, const uint32_t* d_order, int n, void* d_acc_geo,
                      void* d_acc_shade, int* d_acc_leaf, uint32_t* d_ref_to_acc);
+// indexed layout of the accel-order records d_acc_geo (flat, 4 float4 per triangle): d_vid[3 i + k] = vertex id of vertex k + 1 of
+// triangle i, vertices = the distinct (x, y, z) bit patterns numbered by first occurrence, d_vert_src[v] = its first position
+// (both 3 n entries; n_vert of d_vert_src are written) ...
+int ezrt_prep_vertex_ids(const void* d_acc_geo, int n, uint32_t* d_vid, uint32_t* d_vert_src, int& n_vert);
+// ... and from them the 32-byte records (N, d0) (i1, i2, i3, 0) and the vertex array (x, y, z, 0)
+int ezrt_prep_indexed(const void* d_acc_geo, int n, const uint32_t* d_vid, const uint32_t* d_vert_src, int n_vert, void* d_rec, void* d_vert);
 
 // accel_w8.cpp: SAH-optimal collapse of the binary tree to `width`-wide nodes (dynamic programming; shared by the 4-wide
 // exact-box form and the 8-wide quantised form)

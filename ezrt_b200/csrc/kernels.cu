@@ -199,7 +199,9 @@ __device__ __forceinline__ TreeView reference_tree(const SceneDev& sc) {
     t.nodes = sc.nodes; t.tri_geo = sc.tri_geo; t.root_ref = sc.root_ref; t.top_nodes = sc.top_nodes; t.wide = 0;
     return t;
 }
-__device__ __forceinline__ TreeView accel_tree(const SceneDev& sc) {  // the 4-wide exact-box form (round-1 kernel, env EZRT_ACCEL=4)
+// the 4-wide exact-box form (round-1 kernel, env EZRT_ACCEL=4).  Its kernels run only on scenes without a W8 tree, whose
+// acc_tri_geo is always flat (the indexed layout is chosen for W8 scenes only: capi.cu)
+__device__ __forceinline__ TreeView accel_tree(const SceneDev& sc) {
     TreeView t;
     t.nodes = sc.acc_wide_nodes; t.tri_geo = sc.acc_tri_geo; t.root_ref = sc.acc_wide_root_ref; t.top_nodes = 0; t.wide = 1;
     return t;
@@ -381,7 +383,7 @@ struct AccelCameraIO {
     }
 };
 
-template <bool COUNT>
+template <bool COUNT, bool IDX>
 __global__ void __launch_bounds__(EZRT_EXTEND_MAX_THREADS, EZRT_EXTEND_LB_BLOCKS) k_extend_w8_camera(SceneDev sc, RenderDev rd, const TileDev* __restrict__ tiles,
                                                                    uint32_t batch_first_frame, uint32_t n_slots, uint32_t n_frames, PathQueue q, uint32_t* work,
                                                                    uint32_t* defer_list, uint32_t* defer_count, W8Counts counts) {
@@ -399,10 +401,10 @@ __global__ void __launch_bounds__(EZRT_EXTEND_MAX_THREADS, EZRT_EXTEND_LB_BLOCKS
     io.leaf_box = sc.leaf_box;
     io.defer_list = defer_list;
     io.defer_count = defer_count;
-    extend_w8<false, COUNT>(sc, n_slots, work, io, s_perm, stack_sm, counts);
+    extend_w8<false, COUNT, IDX>(sc, n_slots, work, io, s_perm, stack_sm, counts);
 }
 
-template <bool COUNT>
+template <bool COUNT, bool IDX>
 __global__ void __launch_bounds__(EZRT_EXTEND_MAX_THREADS, EZRT_EXTEND_LB_BLOCKS) k_extend_w8(SceneDev sc, PathQueue q, const uint32_t* __restrict__ q_count, uint32_t* work,
                                                                    uint32_t* defer_list, uint32_t* defer_count, W8Counts counts, const uint32_t* __restrict__ perm) {
     unsigned char* s_perm;
@@ -415,7 +417,7 @@ __global__ void __launch_bounds__(EZRT_EXTEND_MAX_THREADS, EZRT_EXTEND_LB_BLOCKS
     io.defer_list = defer_list;
     io.defer_count = defer_count;
     io.perm = perm;
-    extend_w8<false, COUNT>(sc, *q_count, work, io, s_perm, stack_sm, counts);
+    extend_w8<false, COUNT, IDX>(sc, *q_count, work, io, s_perm, stack_sm, counts);
 }
 
 struct AccelShadowIO {
@@ -437,7 +439,7 @@ struct AccelShadowIO {
     }
 };
 
-template <bool COUNT>
+template <bool COUNT, bool IDX>
 __global__ void __launch_bounds__(EZRT_EXTEND_MAX_THREADS, EZRT_EXTEND_LB_BLOCKS) k_shadow_w8(SceneDev sc, ShadowQueue sq, const uint32_t* __restrict__ s_count, uint32_t* work,
                                                                    float4* __restrict__ Lo, uint32_t* defer_list, uint32_t* defer_count, W8Counts counts) {
     unsigned char* s_perm;
@@ -451,7 +453,7 @@ __global__ void __launch_bounds__(EZRT_EXTEND_MAX_THREADS, EZRT_EXTEND_LB_BLOCKS
     io.leaf_box = sc.leaf_box;
     io.defer_list = defer_list;
     io.defer_count = defer_count;
-    extend_w8<true, COUNT>(sc, *s_count, work, io, s_perm, stack_sm, counts);
+    extend_w8<true, COUNT, IDX>(sc, *s_count, work, io, s_perm, stack_sm, counts);
 }
 
 // ---- the same three passes on the 4-wide exact-box tree (default form, env EZRT_ACCEL): extend_persistent<ACCEL, WIDE>
@@ -637,10 +639,10 @@ __global__ void __launch_bounds__(128, EZRT_SHADE_MIN_BLOCKS) k_shade(SceneDev s
             // the geometry and shading records of the triangle this thread's NEXT path hit (its hit record was requested at the top of
             // this round): into L2 while this path is shaded -- the two random 48-byte gathers of surface_hit miss L2 three times in four
             if (!LIST && next_tri >= 0) {
-                const float4* g = (rd.accel_space ? sc.acc_tri_geo : sc.tri_geo) + (size_t)next_tri * 4;
+                const float4* g = tri_geo_rec(sc, next_tri, rd.accel_space != 0);   // an indexed record's vertices are not prefetched
                 const float4* sr = (rd.accel_space ? sc.acc_tri_shade : sc.tri_shade) + (size_t)next_tri * 3;
                 asm volatile("prefetch.global.L2 [%0];" ::"l"(g));
-                asm volatile("prefetch.global.L2 [%0];" ::"l"(g + 2));
+                if (!(rd.accel_space && sc.acc_tri_indexed)) asm volatile("prefetch.global.L2 [%0];" ::"l"(g + 2));
                 asm volatile("prefetch.global.L2 [%0];" ::"l"(sr));
                 asm volatile("prefetch.global.L2 [%0];" ::"l"(sr + 2));
             }
@@ -929,8 +931,7 @@ __global__ void k_trace_finish(SceneDev sc, int n, PathQueue q, int p3fudge, int
         SurfaceHit s = surface_hit(sc, ro, rdv, h.x, ht, p3fudge != 0, accel_space != 0);
         P = s.P;
         N = s.N;
-        const float4* g = (accel_space ? sc.acc_tri_geo : sc.tri_geo) + (size_t)ht * 4;
-        vec3 Ng = f4xyz(ldg4(g));
+        vec3 Ng = f4xyz(ldg4(tri_geo_rec(sc, ht, accel_space != 0)));
         ins = ez_dot(Ng, rdv) > 0.0f;
     }
     inside[i] = ins;
@@ -1152,8 +1153,10 @@ void launch_extend_accel(const SceneDev& sc, PathQueue q, const uint32_t* q_coun
         W8Counts c;
         c.node_visits = counts ? counts + 2 : nullptr;   // 96-byte records
         c.tri_tests = counts ? counts + 1 : nullptr;
-        if (counts) k_extend_w8<true><<<blocks, threads, w8_smem_for(k_extend_w8<true>, sc), st>>>(sc, q, q_count, work, defer_list, defer_count, c, perm);
-        else k_extend_w8<false><<<blocks, threads, w8_smem_for(k_extend_w8<false>, sc), st>>>(sc, q, q_count, work, defer_list, defer_count, c, perm);
+#define EZRT_LAUNCH_W8(C, I) k_extend_w8<C, I><<<blocks, threads, w8_smem_for(k_extend_w8<C, I>, sc), st>>>(sc, q, q_count, work, defer_list, defer_count, c, perm)
+        if (sc.acc_tri_indexed) { if (counts) EZRT_LAUNCH_W8(true, true); else EZRT_LAUNCH_W8(false, true); }
+        else { if (counts) EZRT_LAUNCH_W8(true, false); else EZRT_LAUNCH_W8(false, false); }
+#undef EZRT_LAUNCH_W8
     } else {
         W8Counts c;
         c.node_visits = counts ? (sc.acc_wide_q16 ? counts + 2 : counts) : nullptr;   // counts[2]: 96-byte records, counts[0]: 128-byte records
@@ -1193,8 +1196,11 @@ void launch_extend_camera(const SceneDev& sc, const RenderDev& rd, const TileDev
     c.node_visits = counts ? (sc.w8_nodes ? counts + 2 : counts) : nullptr;   // the 4-wide camera pass reads the 128-byte exact nodes
     c.tri_tests = counts ? counts + 1 : nullptr;
     if (sc.w8_nodes) {
-        if (counts) k_extend_w8_camera<true><<<blocks, threads, w8_smem_for(k_extend_w8_camera<true>, sc), st>>>(sc, rd, tiles, batch_first_frame, n_slots, n_frames, q, work, defer_list, defer_count, c);
-        else k_extend_w8_camera<false><<<blocks, threads, w8_smem_for(k_extend_w8_camera<false>, sc), st>>>(sc, rd, tiles, batch_first_frame, n_slots, n_frames, q, work, defer_list, defer_count, c);
+#define EZRT_LAUNCH_W8(C, I) \
+    k_extend_w8_camera<C, I><<<blocks, threads, w8_smem_for(k_extend_w8_camera<C, I>, sc), st>>>(sc, rd, tiles, batch_first_frame, n_slots, n_frames, q, work, defer_list, defer_count, c)
+        if (sc.acc_tri_indexed) { if (counts) EZRT_LAUNCH_W8(true, true); else EZRT_LAUNCH_W8(false, true); }
+        else { if (counts) EZRT_LAUNCH_W8(true, false); else EZRT_LAUNCH_W8(false, false); }
+#undef EZRT_LAUNCH_W8
     } else {
         if (counts) k_extend_accel_camera<true><<<blocks, threads, smem_for(k_extend_accel_camera<true>, 0), st>>>(sc, rd, tiles, batch_first_frame, n_slots, n_frames, q, work, defer_list, defer_count, c);
         else k_extend_accel_camera<false><<<blocks, threads, smem_for(k_extend_accel_camera<false>, 0), st>>>(sc, rd, tiles, batch_first_frame, n_slots, n_frames, q, work, defer_list, defer_count, c);
@@ -1208,8 +1214,10 @@ void launch_shadow_accel(const SceneDev& sc, ShadowQueue sq, const uint32_t* s_c
         W8Counts c;
         c.node_visits = counts ? counts + 2 : nullptr;
         c.tri_tests = counts ? counts + 1 : nullptr;
-        if (counts) k_shadow_w8<true><<<blocks, threads, w8_smem_for(k_shadow_w8<true>, sc), st>>>(sc, sq, s_count, work, Lo, defer_list, defer_count, c);
-        else k_shadow_w8<false><<<blocks, threads, w8_smem_for(k_shadow_w8<false>, sc), st>>>(sc, sq, s_count, work, Lo, defer_list, defer_count, c);
+#define EZRT_LAUNCH_W8(C, I) k_shadow_w8<C, I><<<blocks, threads, w8_smem_for(k_shadow_w8<C, I>, sc), st>>>(sc, sq, s_count, work, Lo, defer_list, defer_count, c)
+        if (sc.acc_tri_indexed) { if (counts) EZRT_LAUNCH_W8(true, true); else EZRT_LAUNCH_W8(false, true); }
+        else { if (counts) EZRT_LAUNCH_W8(true, false); else EZRT_LAUNCH_W8(false, false); }
+#undef EZRT_LAUNCH_W8
     } else {
         W8Counts c;
         c.node_visits = counts ? (sc.acc_wide_q16 ? counts + 2 : counts) : nullptr;

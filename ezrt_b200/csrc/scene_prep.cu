@@ -123,9 +123,73 @@ __global__ void k_gather(const float4* __restrict__ geo, const float4* __restric
     ref_to_acc[r] = (uint32_t)i;
 }
 
+// Vertex de-duplication of the accel-order records.  Position j = 3 i + k is vertex k + 1 of triangle i (acc_geo[4 i + 1 + k]);
+// positions are equal iff their (x, y, z) BIT PATTERNS are (+0 and -0 differ, NaNs are equal only with the same payload), and the
+// vertices are numbered by first occurrence in j.  Two stable radix sorts (z, then x:y) order the positions by key with equal
+// keys in ascending j, so the head of every run of equal keys is its first occurrence.
+__device__ __forceinline__ uint4 pos_bits(const float4* __restrict__ acc_geo, uint32_t j) {
+    const float4 p = acc_geo[(size_t)(j / 3u) * 4 + 1 + j % 3u];
+    return make_uint4(__float_as_uint(p.x), __float_as_uint(p.y), __float_as_uint(p.z), 0u);
+}
+__global__ void k_pos_z(const float4* __restrict__ acc_geo, uint32_t m, uint32_t* __restrict__ key_z, uint32_t* __restrict__ idx) {
+    const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= m) return;
+    key_z[j] = pos_bits(acc_geo, j).z;
+    idx[j] = j;
+}
+__global__ void k_pos_xy(const float4* __restrict__ acc_geo, uint32_t m, const uint32_t* __restrict__ idx, unsigned long long* __restrict__ key_xy) {
+    const uint32_t p = blockIdx.x * blockDim.x + threadIdx.x;
+    if (p >= m) return;
+    const uint4 b = pos_bits(acc_geo, idx[p]);
+    key_xy[p] = ((unsigned long long)b.x << 32) | b.y;
+}
+// head[p] = 1 iff sorted position p starts a run of equal keys; first[j] = 1 iff position j is that run's first occurrence
+__global__ void k_pos_heads(const float4* __restrict__ acc_geo, uint32_t m, const uint32_t* __restrict__ idx, uint32_t* __restrict__ head,
+                            uint32_t* __restrict__ first) {
+    const uint32_t p = blockIdx.x * blockDim.x + threadIdx.x;
+    if (p >= m) return;
+    const uint32_t j = idx[p];
+    bool h = p == 0;
+    if (!h) {
+        const uint4 a = pos_bits(acc_geo, j), b = pos_bits(acc_geo, idx[p - 1]);
+        h = a.x != b.x || a.y != b.y || a.z != b.z;
+    }
+    head[p] = h ? 1u : 0u;
+    if (h) first[j] = 1u;
+}
+// num = exclusive scan of first (vertex id of every first occurrence), run = inclusive scan of head (1-based run of p)
+__global__ void k_run_ids(uint32_t m, const uint32_t* __restrict__ idx, const uint32_t* __restrict__ head, const uint32_t* __restrict__ run,
+                          const uint32_t* __restrict__ num, uint32_t* __restrict__ run_vid, uint32_t* __restrict__ vert_src) {
+    const uint32_t p = blockIdx.x * blockDim.x + threadIdx.x;
+    if (p >= m || !head[p]) return;
+    const uint32_t j = idx[p], v = num[j];
+    run_vid[run[p] - 1] = v;
+    vert_src[v] = j;
+}
+__global__ void k_vertex_ids(uint32_t m, const uint32_t* __restrict__ idx, const uint32_t* __restrict__ run, const uint32_t* __restrict__ run_vid,
+                             uint32_t* __restrict__ vid) {
+    const uint32_t p = blockIdx.x * blockDim.x + threadIdx.x;
+    if (p >= m) return;
+    vid[idx[p]] = run_vid[run[p] - 1];
+}
+// indexed records (N, d0) (i1, i2, i3, 0) and the vertex array (x, y, z, 0)
+__global__ void k_indexed(const float4* __restrict__ acc_geo, int n, const uint32_t* __restrict__ vid, float4* __restrict__ rec) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    rec[(size_t)i * 2] = acc_geo[(size_t)i * 4];
+    rec[(size_t)i * 2 + 1] = make_float4(__uint_as_float(vid[(size_t)i * 3]), __uint_as_float(vid[(size_t)i * 3 + 1]), __uint_as_float(vid[(size_t)i * 3 + 2]), 0.0f);
+}
+__global__ void k_vertices(const float4* __restrict__ acc_geo, uint32_t n_vert, const uint32_t* __restrict__ vert_src, float4* __restrict__ vert) {
+    const uint32_t v = blockIdx.x * blockDim.x + threadIdx.x;
+    if (v >= n_vert) return;
+    const uint32_t j = vert_src[v];
+    const float4 p = acc_geo[(size_t)(j / 3u) * 4 + 1 + j % 3u];
+    vert[v] = make_float4(p.x, p.y, p.z, 0.0f);
+}
+
 }  // namespace
 
-#define PREP_OK(call)                                                                                            \
+#define PREP_OK(call)                                                                                           \
     do {                                                                                                         \
         cudaError_t e_ = (call);                                                                                 \
         if (e_ != cudaSuccess) {                                                                                 \
@@ -215,5 +279,67 @@ int ezrt_prep_gather(const void* d_geo, const void* d_shade, const int* d_tri_le
                                   d_acc_leaf, d_ref_to_acc);
     cudaError_t e = cudaDeviceSynchronize();
     if (e != cudaSuccess) return ezrt_set_error(EZRT_ERR_CUDA, "scene prep: gather: %s", cudaGetErrorString(e));
+    return EZRT_OK;
+}
+
+int ezrt_prep_vertex_ids(const void* d_acc_geo, int n, uint32_t* d_vid, uint32_t* d_vert_src, int& n_vert) {
+    int rc = EZRT_OK;
+    const uint32_t m = 3u * (uint32_t)n;
+    const int threads = 256, blocks = (int)((m + threads - 1) / threads);
+    const float4* geo = (const float4*)d_acc_geo;
+    char* scratch = nullptr;
+    size_t t_sort_z = 0, t_sort_xy = 0, t_scan = 0;
+    cub::DeviceRadixSort::SortPairs(nullptr, t_sort_z, (const uint32_t*)nullptr, (uint32_t*)nullptr, (const uint32_t*)nullptr, (uint32_t*)nullptr, (int)m);
+    cub::DeviceRadixSort::SortPairs(nullptr, t_sort_xy, (const unsigned long long*)nullptr, (unsigned long long*)nullptr, (const uint32_t*)nullptr, (uint32_t*)nullptr, (int)m);
+    cub::DeviceScan::InclusiveSum(nullptr, t_scan, (const uint32_t*)nullptr, (uint32_t*)nullptr, (int)m);
+    const size_t temp_bytes = std::max(t_sort_z, std::max(t_sort_xy, t_scan));
+    const size_t a4 = ((size_t)m * 4 + 255) / 256 * 256, a8 = 2 * a4;
+    // u32 arrays: key_z, key_z_sorted, idx0, idx1, idx2, head, run, first, num, run_vid; u64: key_xy, key_xy_sorted
+    PREP_OK(cudaMalloc((void**)&scratch, 10 * a4 + 2 * a8 + temp_bytes + 256));
+    {
+        uint32_t* key_z = (uint32_t*)scratch;
+        uint32_t* key_z_s = (uint32_t*)(scratch + a4);
+        uint32_t* idx0 = (uint32_t*)(scratch + 2 * a4);
+        uint32_t* idx1 = (uint32_t*)(scratch + 3 * a4);
+        uint32_t* idx2 = (uint32_t*)(scratch + 4 * a4);
+        uint32_t* head = (uint32_t*)(scratch + 5 * a4);
+        uint32_t* run = (uint32_t*)(scratch + 6 * a4);
+        uint32_t* first = (uint32_t*)(scratch + 7 * a4);
+        uint32_t* num = (uint32_t*)(scratch + 8 * a4);
+        uint32_t* run_vid = (uint32_t*)(scratch + 9 * a4);
+        unsigned long long* key_xy = (unsigned long long*)(scratch + 10 * a4);
+        unsigned long long* key_xy_s = (unsigned long long*)(scratch + 10 * a4 + a8);
+        void* temp = scratch + 10 * a4 + 2 * a8;
+        size_t tb = temp_bytes;
+        uint32_t last[2] = {0u, 0u};
+        k_pos_z<<<blocks, threads>>>(geo, m, key_z, idx0);
+        PREP_OK(cub::DeviceRadixSort::SortPairs(temp, tb, key_z, key_z_s, idx0, idx1, (int)m));
+        k_pos_xy<<<blocks, threads>>>(geo, m, idx1, key_xy);
+        tb = temp_bytes;
+        PREP_OK(cub::DeviceRadixSort::SortPairs(temp, tb, key_xy, key_xy_s, idx1, idx2, (int)m));   // stable: equal keys stay in ascending j
+        PREP_OK(cudaMemset(first, 0, (size_t)m * 4));
+        k_pos_heads<<<blocks, threads>>>(geo, m, idx2, head, first);
+        tb = temp_bytes;
+        PREP_OK(cub::DeviceScan::InclusiveSum(temp, tb, head, run, (int)m));
+        tb = temp_bytes;
+        PREP_OK(cub::DeviceScan::ExclusiveSum(temp, tb, first, num, (int)m));
+        PREP_OK(cudaMemcpy(&last[0], num + (m - 1), 4, cudaMemcpyDeviceToHost));
+        PREP_OK(cudaMemcpy(&last[1], first + (m - 1), 4, cudaMemcpyDeviceToHost));
+        n_vert = (int)(last[0] + last[1]);
+        k_run_ids<<<blocks, threads>>>(m, idx2, head, run, num, run_vid, d_vert_src);
+        k_vertex_ids<<<blocks, threads>>>(m, idx2, run, run_vid, d_vid);
+        PREP_OK(cudaDeviceSynchronize());
+    }
+done:
+    cudaFree(scratch);
+    return rc;
+}
+
+int ezrt_prep_indexed(const void* d_acc_geo, int n, const uint32_t* d_vid, const uint32_t* d_vert_src, int n_vert, void* d_rec, void* d_vert) {
+    const int threads = 256;
+    k_indexed<<<(n + threads - 1) / threads, threads>>>((const float4*)d_acc_geo, n, d_vid, (float4*)d_rec);
+    k_vertices<<<(n_vert + threads - 1) / threads, threads>>>((const float4*)d_acc_geo, (uint32_t)n_vert, d_vert_src, (float4*)d_vert);
+    cudaError_t e = cudaDeviceSynchronize();
+    if (e != cudaSuccess) return ezrt_set_error(EZRT_ERR_CUDA, "scene prep: indexed records: %s", cudaGetErrorString(e));
     return EZRT_OK;
 }

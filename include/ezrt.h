@@ -112,8 +112,9 @@ typedef struct ezrt_counters {
     uint64_t node_visits;   /* profile = 2: acceleration-tree node records fetched ...       */
     uint64_t tri_tests;     /*              ... and triangle records (64 B) fetched by the accel kernels */
     uint64_t node_visits_96;/*              of node_visits: quantised records (16-bit planes, 96 B / W8, 80 B); the rest are 128-byte records */
-    uint64_t node_bytes, tri_bytes; /*      96 B per quantised and 128 B per exact node visit, 64 B per triangle test: an upper
-                                               bound of the bytes fetched (a W8 node is 80 B; a test that fails its distance checks reads 16 B) */
+    uint64_t node_bytes, tri_bytes; /*      96 B per quantised and 128 B per exact node visit, 64 B per triangle test: nominal
+                                               figures, not bytes fetched (a W8 node is 80 B; a flat triangle test that fails its distance
+                                               checks reads 16 B, an indexed one 32 B, and 48 B of vertices more past them) */
 } ezrt_counters;
 
 typedef struct ezrt_scene ezrt_scene; /* device-resident scene (replaces the two TBOs + 2 textures) */

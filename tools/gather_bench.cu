@@ -170,6 +170,30 @@ int main() {
             cudaFree(table);
         }
     }
+    {   // the L2 cliff: 32-, 48- and 64-byte records (128-bit loads, dependent) from tables of 16 to 128 MB, around H100's
+        // 50 MB L2 -- where the W8 triangle records of a 1 M-triangle scene lie (64 MB flat, 32 MB indexed + the vertices)
+        const int tmb[6] = {16, 32, 48, 64, 96, 128};
+        for (int si = 0; si < 6; si++) {
+            const size_t bytes_t = (size_t)tmb[si] << 20;
+            char* table;
+            if (cudaMalloc(&table, bytes_t) != cudaSuccess) continue;
+            cudaMemset(table, 1, bytes_t);
+            for (int nl = 2; nl <= 4; nl++) {
+                const int rec = nl * 16;
+                const uint32_t n_rec = (uint32_t)(bytes_t / rec);
+                auto launch = [&]() {
+                    if (nl == 2) k_gather128<2><<<sms, 1024>>>(table, n_rec, rec, iters, sink);
+                    else if (nl == 3) k_gather128<3><<<sms, 1024>>>(table, n_rec, rec, iters, sink);
+                    else k_gather128<4><<<sms, 1024>>>(table, n_rec, rec, iters, sink);
+                };
+                const float ms = time_ms(launch);
+                const double bytes = (double)sms * 1024 * iters * rec;
+                printf(",\n  {\"table\": \"cliff_%dMB_ld128\", \"record_bytes\": %d, \"dependent\": 1, \"ms\": %.4f, \"gbs\": %.1f, \"grecords_per_s\": %.2f}", tmb[si], rec, ms,
+                       bytes / ms / 1e6, bytes / rec / ms / 1e6);
+            }
+            cudaFree(table);
+        }
+    }
     for (int nl = 2; nl <= 8; nl *= 2) {
         auto launch = [&]() {
             if (nl == 2) { cudaFuncSetAttribute(k_gather_smem<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 65536); k_gather_smem<2><<<sms, 1024, 65536>>>(4096, sink); }
