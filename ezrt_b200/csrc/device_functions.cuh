@@ -1195,6 +1195,184 @@ __device__ __forceinline__ void extend_w8(const SceneDev& sc, uint32_t n, uint32
 }
 
 // ------------------------------------------------------------------------------------------
+// W8 camera pass: the warp traces its 32 work items as ONE bundle.  In pixel-major order those are the jittered samples of
+// one or two pixels, which share the eye and walk the same nodes, so the node work is done once per warp: one warp-uniform
+// stack, and lanes 0..7 each test one slot of the node with the bundle bound of w8_node.h (conservative for every member
+// ray).  The triangles of the hit leaf slots are then tested one after the other, every member lane its own ray (tri_test_t
+// in its serial order: t <= best accepted, t == best a tie).
+// The result of every ray equals the per-ray traversal's: the bundle reaches every slot the ray's exact segment reaches
+// within its limit, so it tests every triangle the ray accepts at or below its final best -- the minimum and its holders
+// (best, tie) are the same, and best_tri is the first holder, which matters only without a tie.
+// ------------------------------------------------------------------------------------------
+template <int K>
+__device__ __forceinline__ float warp_reduce_f(float v) {   // K = 0: minimum, 1: maximum, over all 32 lanes
+#pragma unroll
+    for (int s = 16; s > 0; s >>= 1) {
+        const float u = __shfl_xor_sync(0xffffffffu, v, s);
+        v = K ? fmaxf(v, u) : fminf(v, u);
+    }
+    return v;
+}
+// one axis of the bundle bound (w8_node.h): entry / exit bounds of the slab [lo, hi] for every member ray
+__device__ __forceinline__ void w8_bundle_axis(float lo, float hi, uint32_t sign, const float4 b, float& entry, float& exit) {
+    const float omin = b.x, omax = b.y, vmin = b.z, vmax = b.w;
+    const bool pos = sign == 1u;
+    const float pn = pos ? lo : hi, pf = pos ? hi : lo;
+    const float xe = pos ? __fsub_rd(pn, omax) : __fsub_ru(pn, omin);
+    const float xx = pos ? __fsub_ru(pf, omin) : __fsub_rd(pf, omax);
+    entry = sign ? __fmul_rd(xe, xe >= 0.0f ? vmin : vmax) : -EZ_INF;   // sign 0: the members' d_a differ in sign
+    exit = sign ? __fmul_ru(xx, xx >= 0.0f ? vmax : vmin) : EZ_INF;
+}
+
+template <bool COUNT, bool IDX, class RayIO>
+__device__ __forceinline__ void extend_w8_bundle(const SceneDev& sc, uint32_t n, uint32_t* work, RayIO io, const unsigned char* s_perm, uint2* stack_sm,
+                                                 W8Counts counts) {
+    const bool tri_na = sc.tri_l1_bypass != 0;
+    const unsigned FULL = 0xffffffffu;
+    const int lane = threadIdx.x & 31;
+    uint2* const stack = stack_sm + (threadIdx.x >> 5) * W8_BUNDLE_STACK;   // the warp's stack: every lane writes the same entry
+    __shared__ float4 s_bnd_all[(EZRT_EXTEND_MAX_THREADS / 32) * 3];
+    float4* const bnd = s_bnd_all + (threadIdx.x >> 5) * 3;
+    __shared__ unsigned s_pend_all[EZRT_EXTEND_MAX_THREADS / 32];
+    unsigned* const s_pend = s_pend_all + (threadIdx.x >> 5);
+    const uint4* __restrict__ nodes = sc.w8_nodes;
+    const float origin_limit = sc.w8_origin_limit, inv_limit = sc.quant_inv_limit;
+    uint32_t n_tests = 0;
+    __shared__ uint32_t s_visits_all[EZRT_EXTEND_MAX_THREADS / 32];   // COUNT: node visits of the warp (lane 0), in shared memory
+    uint32_t* const s_visits = s_visits_all + (threadIdx.x >> 5);
+    if (COUNT && lane == 0) *s_visits = 0u;
+    // slot of this lane in a node step (lanes 0..7) and its byte in the plane words
+    const bool slot_hi = (lane & 7) >= 4;
+    const uint32_t slot_shift = (uint32_t)(lane & 3) * 8u;
+    auto slot_byte = [&](uint32_t w0, uint32_t w1) { return (float)(((slot_hi ? w1 : w0) >> slot_shift) & 0xffu); };
+
+    while (true) {
+        uint32_t base = 0;
+        if (lane == 0) base = atomicAdd(work, 32u);
+        base = __shfl_sync(FULL, base, 0);
+        if (base >= n) break;
+        const uint32_t idx = base + (uint32_t)lane;
+        vec3 o = splat3(0.0f), d = splat3(0.0f), inv = splat3(0.0f);
+        bool member = false;
+        if (idx < n && io.load(idx, o, d)) {
+            inv = ez_v3(EZ_DIV(1.0f, d.x), EZ_DIV(1.0f, d.y), EZ_DIV(1.0f, d.z));
+            const float ax = ez_abs(inv.x), ay = ez_abs(inv.y), az = ez_abs(inv.z);
+            const float ao = fmaxf(ez_abs(o.x), fmaxf(ez_abs(o.y), ez_abs(o.z)));
+            const float amin = fminf(ax, fminf(ay, az)), amax = fmaxf(ax, fmaxf(ay, az));
+            if ((amax <= inv_limit) && (amin >= W8_INV_MIN) && (ao <= origin_limit)) member = true;   // false for inf / NaN
+            else io.defer(idx, o, d);   // outside the decode error bound: the exact kernel traces it
+        }
+        // Sub-bundles: a member joins the first pending member's sub-bundle when every component of its 1/d has the leader's sign
+        // and lies within a factor 2 of the leader's.  Camera rays of neighbouring pixels almost always form one sub-bundle; where
+        // a component of d crosses zero its 1/d spreads without bound, and one bundle over such rays would bound nothing on that
+        // axis (and their slack makes the limit huge): those rays go in sub-bundles of their own.
+        // (the pending mask lives in shared memory, like the bundle's intervals: 64 registers without spilling)
+        *s_pend = __ballot_sync(FULL, member);
+        while (*s_pend != 0u) {
+        const unsigned pending = *s_pend;
+        const int lead = __ffs(pending) - 1;
+        const float lx = __shfl_sync(FULL, inv.x, lead), ly = __shfl_sync(FULL, inv.y, lead), lz = __shfl_sync(FULL, inv.z, lead);
+        auto close = [](float v, float w) { return (v > 0.0f) == (w > 0.0f) && ez_abs(v) <= 2.0f * ez_abs(w) && ez_abs(w) <= 2.0f * ez_abs(v); };
+        member = ((pending >> lane) & 1u) && close(inv.x, lx) && close(inv.y, ly) && close(inv.z, lz);
+        const unsigned members = __ballot_sync(FULL, member);
+        *s_pend = pending & ~members;
+        float best = EZ_INF;
+        int best_tri = -1;
+        bool tie = false;
+        // the bundle's intervals (w8_node.h "Bundle bound"): (omin, omax, vmin, vmax) per axis in shared memory, and the sign of
+        // axis a in bits 2a..2a+1: 1 all members d_a >= 0, 2 all d_a < 0, 0 mixed
+        uint32_t signs = 0u;
+        {
+            const float oa[3] = {o.x, o.y, o.z}, da[3] = {d.x, d.y, d.z}, va[3] = {inv.x, inv.y, inv.z};
+#pragma unroll
+            for (int a = 0; a < 3; a++) {
+                const unsigned p = __ballot_sync(FULL, member && da[a] >= 0.0f);
+                signs |= (p == members ? 1u : (p == 0u ? 2u : 0u)) << (2 * a);
+                const float4 b = make_float4(warp_reduce_f<0>(member ? oa[a] : INFINITY), warp_reduce_f<1>(member ? oa[a] : -INFINITY),
+                                             warp_reduce_f<0>(member ? va[a] : INFINITY), warp_reduce_f<1>(member ? va[a] : -INFINITY));
+                bnd[a] = b;   // every lane writes the same value and reads back its own write
+            }
+        }
+        // visit order: the octant order of the first member's ray (any order is correct)
+        const uint32_t near_mask = __shfl_sync(FULL, (d.x >= 0.0f ? (1u << sc.w8_near_bit[0]) : 0u) | (d.y >= 0.0f ? (1u << sc.w8_near_bit[1]) : 0u) |
+                                                         (d.z >= 0.0f ? (1u << sc.w8_near_bit[2]) : 0u), __ffs(members) - 1);
+        float L = EZ_INF;   // the largest per-ray limit best + best 2^-12 + slack of the members
+        int sp = 0;
+        uint32_t node = 0, g_base = 0, g_bits = 0;
+        while (true) {
+            const uint4* nd = nodes + (size_t)node * (W8_NODE_WORDS / 4);
+            const uint4 h = ldg128_u32(nd), c = ldg128_u32(nd + 1), l = ldg128_u32(nd + 2), m = ldg128_u32(nd + 3), u = ldg128_u32(nd + 4);
+            if (COUNT && lane == 0) ++*s_visits;
+            bool hit = false;
+            if (lane < 8) {
+                const float sx = __uint_as_float(W8_SCALE_BITS(h.w, 0)), sy = __uint_as_float(W8_SCALE_BITS(h.w, 1)), sz = __uint_as_float(W8_SCALE_BITS(h.w, 2));
+                const float ox = __uint_as_float(h.x), oy = __uint_as_float(h.y), oz = __uint_as_float(h.z);
+                float ex, ey, ez, xx, xy, xz;
+                w8_bundle_axis(__fadd_rd(ox, (slot_byte(c.z, c.w) - 0.25f) * sx), __fadd_ru(ox, (slot_byte(m.z, m.w) + 0.25f) * sx), signs & 3u, bnd[0], ex, xx);
+                w8_bundle_axis(__fadd_rd(oy, (slot_byte(l.x, l.y) - 0.25f) * sy), __fadd_ru(oy, (slot_byte(u.x, u.y) + 0.25f) * sy), (signs >> 2) & 3u, bnd[1], ey, xy);
+                w8_bundle_axis(__fadd_rd(oz, (slot_byte(l.z, l.w) - 0.25f) * sz), __fadd_ru(oz, (slot_byte(u.z, u.w) + 0.25f) * sz), signs >> 4, bnd[2], ez, xz);
+                hit = fmaxf(fmaxf(ex, ey), fmaxf(ez, 0.0f)) <= fminf(fminf(xx, xy), fminf(xz, L));
+            }
+            const uint32_t hits = __ballot_sync(FULL, hit) & 0xffu;
+            const uint32_t imask = h.w >> 24;
+            const uint32_t inner = hits & imask;
+            uint32_t leaf = hits & ~imask;
+            if ((g_bits >> 8) != 0u) stack[sp++] = make_uint2(g_base, g_bits);   // the rest of the group this node came from
+            g_base = c.x;
+            g_bits = imask | ((uint32_t)s_perm[near_mask * 256u + inner] << 8);
+            // triangles of the hit leaf slots (meta byte = (count << 5) | offset), every member lane its own ray, lowest first
+            uint32_t t_mask = 0u;
+            while (leaf != 0u) {
+                const int s = __ffs(leaf) - 1;
+                leaf &= leaf - 1u;
+                const uint32_t mb = ((s < 4 ? m.x : m.y) >> ((s & 3) * 8)) & 0xffu;
+                t_mask |= ((1u << (mb >> 5)) - 1u) << (mb & 31u);
+            }
+            if (t_mask != 0u) {
+                while (t_mask != 0u) {
+                    const int tri = (int)c.y + __ffs(t_mask) - 1;
+                    t_mask &= t_mask - 1u;
+                    if (member) {
+                        if (COUNT) n_tests++;
+                        float t = 0.0f;
+                        const int r = IDX ? tri_test_idx_t<true>(sc.acc_tri_geo + (size_t)tri * 2, sc.acc_tri_vert, o, d, best, t, tri_na)
+                                          : tri_test_t<true>(sc.acc_tri_geo + (size_t)tri * 4, o, d, best, t, tri_na);
+                        if (r == 2) tie = true;
+                        else if (r == 1) { best = t; best_tri = tri; tie = false; }
+                    }
+                }
+                // the per-ray limit (slack recomputed here: one register less); >= 0, so the bits order as the values
+                const float slack = sc.prune_delta * fmaxf(ez_abs(inv.x), fmaxf(ez_abs(inv.y), ez_abs(inv.z)));
+                const float lim = member ? best + (best * 0.000244140625f + slack) : 0.0f;
+                L = __uint_as_float(__reduce_max_sync(FULL, __float_as_uint(lim)));
+            }
+            // next node: from the current group, else from the stack
+            if ((g_bits >> 8) == 0u) {
+                if (sp == 0) break;
+                const uint2 e = stack[--sp];
+                g_base = e.x;
+                g_bits = e.y;
+            }
+            const int p = 23 - __clz(g_bits);
+            g_bits ^= 0x100u << p;
+            const uint32_t slot = (uint32_t)p ^ near_mask;
+            node = g_base + (uint32_t)__popc(g_bits & 0xffu & ((1u << slot) - 1u));
+        }
+        if (member) {
+            HitRec hr;
+            hr.t = best;
+            hr.tri = best_tri;
+            io.store(idx, hr, tie, o, d, inv);
+        }
+        }
+    }
+    if (COUNT) {
+        if (lane == 0) atomicAdd(counts.node_visits, (unsigned long long)*s_visits);
+        atomicAdd(counts.tri_tests, (unsigned long long)n_tests);
+    }
+}
+
+// ------------------------------------------------------------------------------------------
 // hit geometry + material for the final closest hit (tail of hitTriangle :198-214, getMaterial :110-135)
 // ------------------------------------------------------------------------------------------
 struct MaterialDev {

@@ -401,7 +401,7 @@ __global__ void __launch_bounds__(EZRT_EXTEND_MAX_THREADS, EZRT_EXTEND_LB_BLOCKS
     io.leaf_box = sc.leaf_box;
     io.defer_list = defer_list;
     io.defer_count = defer_count;
-    extend_w8<false, COUNT, IDX>(sc, n_slots, work, io, s_perm, stack_sm, counts);
+    extend_w8_bundle<COUNT, IDX>(sc, n_slots, work, io, s_perm, stack_sm, counts);
 }
 
 template <bool COUNT, bool IDX>
@@ -1196,8 +1196,10 @@ void launch_extend_camera(const SceneDev& sc, const RenderDev& rd, const TileDev
     c.node_visits = counts ? (sc.w8_nodes ? counts + 2 : counts) : nullptr;   // the 4-wide camera pass reads the 128-byte exact nodes
     c.tri_tests = counts ? counts + 1 : nullptr;
     if (sc.w8_nodes) {
+        // s_perm + one stack of W8_BUNDLE_STACK entries per warp (extend_w8_bundle)
+        auto smem_bundle = [&](const void* k) { const size_t b = 2048 + (size_t)(threads / 32) * W8_BUNDLE_STACK * sizeof(uint2); set_dynamic_smem(k, b); return b; };
 #define EZRT_LAUNCH_W8(C, I) \
-    k_extend_w8_camera<C, I><<<blocks, threads, w8_smem_for(k_extend_w8_camera<C, I>, sc), st>>>(sc, rd, tiles, batch_first_frame, n_slots, n_frames, q, work, defer_list, defer_count, c)
+    k_extend_w8_camera<C, I><<<blocks, threads, smem_bundle((const void*)k_extend_w8_camera<C, I>), st>>>(sc, rd, tiles, batch_first_frame, n_slots, n_frames, q, work, defer_list, defer_count, c)
         if (sc.acc_tri_indexed) { if (counts) EZRT_LAUNCH_W8(true, true); else EZRT_LAUNCH_W8(false, true); }
         else { if (counts) EZRT_LAUNCH_W8(true, false); else EZRT_LAUNCH_W8(false, false); }
 #undef EZRT_LAUNCH_W8

@@ -40,6 +40,24 @@
 // |inv_d| per scene from the largest per-axis scale of the tree and max|coordinate|: a power of two, at most W8_INV_LIMIT, that
 // keeps 2^15 * scale * |inv_d| and 5 * max|coordinate| * |inv_d| at or below 2^124 (the Q16 nodes: 2^23 * scale).
 //
+// Bundle bound (the camera pass, extend_w8_bundle in device_functions.cuh; the same arithmetic in tools/w8_model.cpp): one
+// interval test per slot decides for all member rays r of a (sub-)bundle at once whether one of them may reach the slot.
+//     per member ray: the float o_r, v_r = EZ_DIV(1, d_r) the per-ray decode uses (finite and non-zero: the load gate)
+//     per axis a: [omin, omax] of o_a,r and [vmin, vmax] of v_a,r over the members; the axis constrains the test only when all
+//                 members have d_a >= 0 ("pos") or all have d_a < 0 (sub-bundles always do: their v_a,r share one sign)
+//     planes, widened by W8_SLACK_STEPS and rounded outward: lo = rd(origin + (q_lo - 0.25) scale), hi = ru(origin + (q_hi + 0.25) scale)
+//                 ((q -+ 0.25) scale is exact: q has 8 bits, scale is a power of two)
+//     near plane pn = pos ? lo : hi, far plane pf = pos ? hi : lo
+//     xe = pos ? rd(pn - omax) : ru(pn - omin)          entry = rd(xe * (xe >= 0 ? vmin : vmax))
+//     xx = pos ? ru(pf - omin) : rd(pf - omax)          exit  = ru(xx * (xx >= 0 ? vmax : vmin))
+//     hit iff max(entry_x, entry_y, entry_z, 0) <= min(exit_x, exit_y, exit_z, L),   L = max over members of the per-ray limit
+// (rd / ru: round toward -inf / +inf).  For every member, (pn - o_a,r) v_a,r >= entry and (pf - o_a,r) v_a,r <= exit: the
+// product is monotonic in each factor on the box [omin, omax] x [vmin, vmax], and the chosen corner is its minimum (maximum),
+// with every rounding outward.  The per-ray decode of the same planes differs from (plane - o) v by less than 0.162 step
+// (above), less than the 0.25 step the bundle widens each plane by.  So a slot the per-ray test of any member hits, at any
+// limit <= L, is hit by the bundle test.  The bound is only as tight as [vmin, vmax]: where a component of d crosses zero
+// its 1/d spreads without bound, which is why a sub-bundle keeps each component of 1/d within a factor 2 of its leader's.
+//
 // Slot order ("octant order", after Ylitie, Karras, Laine 2017): the builder places a child in the slot whose
 // corner direction (bit a of the slot index set = towards +axis_a) matches the child's offset from the node
 // centre best; a ray visits hit slots in descending (slot ^ near_mask), near_mask bit a = 1 iff d_a >= 0, so
@@ -63,6 +81,7 @@
 #define W8_INV_MIN 8.6736173798840355e-19f   // 2^-60: ... or a smaller one (no underflow)
 
 #define W8_LOCAL_STACK 48                    // stack entries beyond the shared-memory part (local memory)
+#define W8_BUNDLE_STACK 64                   // entries of a warp's stack in the camera pass (shared memory): a lane's 16 + 48
 
 #define W8_W_ORIGIN 0
 #define W8_W_EXP_IMASK 3

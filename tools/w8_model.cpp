@@ -6,7 +6,13 @@
 // triangles pending per node visit and a warp-level replay of the kernel's schedule (serial vs cooperative triangle step).
 //   g++ -O2 -std=c++17 -fopenmp -ffp-contract=off -mfma -Iinclude -Iezrt_b200/csrc tools/w8_model.cpp \
 //       ezrt_b200/csrc/host_scene.cpp ezrt_b200/csrc/accel_w8.cpp ezrt_b200/csrc/errors.cpp -o build/w8_model
-//   build/w8_model tris.f32 n_tris rays.f32 [brute]        rays: 7-float records (o, d, kind) as oracle_set_ray_dump writes
+//   build/w8_model tris.f32 n_tris rays.f32 [brute] [bundle]   rays: 7-float records (o, d, kind) as oracle_set_ray_dump writes
+//   bundle: also walk every 32 consecutive rays as bundles (a ray joins the first pending ray's sub-bundle when each component of
+//   its 1/d has the same sign and lies within a factor 2) -- one stack, one conservative interval test per slot for all
+//   member rays, then every candidate triangle tested by every member in serial order -- and check it against the per-ray walk:
+//   equal (t, triangle, tie), and every node / triangle of the per-ray walk visited / tested by the bundle.
+//   The bundle bound and its arithmetic: w8_node.h "Bundle bound".
+#include <fenv.h>
 #include <math.h>
 #include <stdint.h>
 #include <stdio.h>
@@ -103,10 +109,30 @@ static Replay replay(const std::vector<const std::vector<uint8_t>*>& trace, bool
     return R;
 }
 
+// the bundle bound of w8_node.h with its directed roundings (the device's __fadd_rd, __fsub_ru, __fmul_rd, ...)
+static float rnd(int mode, char op, float a, float b) {
+    fesetround(mode);
+    volatile float x = a, y = b;
+    volatile float r = op == '+' ? x + y : (op == '-' ? x - y : x * y);
+    fesetround(FE_TONEAREST);
+    return r;
+}
+static void bundle_axis(float lo, float hi, int sign, float omin, float omax, float vmin, float vmax, float& entry, float& exit) {
+    if (sign == 0) { entry = -EZ_INF; exit = EZ_INF; return; }
+    const bool pos = sign == 1;
+    const float pn = pos ? lo : hi, pf = pos ? hi : lo;
+    const float xe = pos ? rnd(FE_DOWNWARD, '-', pn, omax) : rnd(FE_UPWARD, '-', pn, omin);
+    const float xx = pos ? rnd(FE_UPWARD, '-', pf, omin) : rnd(FE_DOWNWARD, '-', pf, omax);
+    entry = rnd(FE_DOWNWARD, '*', xe, xe >= 0.0f ? vmin : vmax);
+    exit = rnd(FE_UPWARD, '*', xx, xx >= 0.0f ? vmax : vmin);
+}
+struct RayResult { float t; int tri; bool tie; std::vector<int> nodes, tris; };
+
 int main(int argc, char** argv) {
     if (argc < 4) { fprintf(stderr, "usage: w8_model tris.f32 n_tris rays.f32 [brute]\n"); return 2; }
     const int n = atoi(argv[2]);
-    const bool brute = argc > 4 && !strcmp(argv[4], "brute");
+    bool brute = false, bundle = false;
+    for (int i = 4; i < argc; i++) { brute |= !strcmp(argv[i], "brute"); bundle |= !strcmp(argv[i], "bundle"); }
     std::vector<float> tris((size_t)n * 36);
     FILE* f = fopen(argv[1], "rb");
     if (!f || fread(tris.data(), 4, tris.size(), f) != tris.size()) { fprintf(stderr, "cannot read triangles\n"); return 1; }
@@ -189,6 +215,7 @@ int main(int argc, char** argv) {
     int max_sp = 0;
     std::vector<std::vector<uint8_t>> trace(NR);   // triangles pending after each node visit, for the warp replay
     std::vector<int> ray_kind(NR, -1);              // -1: left to the exact kernel
+    std::vector<RayResult> res(bundle ? NR : 0);    // bundle mode: the per-ray walk's result, nodes and triangles
 #pragma omp parallel for schedule(dynamic, 256) reduction(+ : mismatch, skipped, ties, hits) reduction(max : max_sp)
     for (int r = 0; r < NR; r++) {
         const float* R = &rays[(size_t)r * 7];
@@ -207,6 +234,7 @@ int main(int argc, char** argv) {
         for (int a = 0; a < 3; a++) if (dd[a] >= 0.0f) near_mask |= 1u << axis_bit[a];
         float best = EZ_INF;
         bool tie = false;
+        int best_tri = -1;
         struct Group { uint32_t base, bits; float tmin; uint32_t order; float ts[8]; } st[64];
         float g_ts[8] = {0, 0, 0, 0, 0, 0, 0, 0};
         const bool x_tsel = getenv("W8M_TSEL") && atoi(getenv("W8M_TSEL"));  // per-child entry distance kept with the group (ideal pop pruning)
@@ -222,6 +250,7 @@ int main(int argc, char** argv) {
             if (node >= 0) {
                 const uint32_t* w = &w8.nodes[(size_t)node * W8_NODE_WORDS];
                 my_nv += 1;
+                if (bundle) res[r].nodes.push_back(node);
                 const float limit = best + (best * 0.000244140625f + slack);
                 float A[3], B[3];
                 for (int a = 0; a < 3; a++) {
@@ -280,8 +309,9 @@ int main(int argc, char** argv) {
                 bool passed = false;
                 const int h = tri_test(rec[t_base + k], o, d, best, t, &passed);
                 my_pass += passed ? 1 : 0;
+                if (bundle) res[r].tris.push_back((int)(t_base + k));
                 if (h == 2) tie = true;
-                else if (h == 1) { best = t; tie = false; }
+                else if (h == 1) { best = t; tie = false; best_tri = (int)(t_base + k); }
             }
             bool done = false;
             while ((g_bits >> 8) == 0) {
@@ -313,6 +343,7 @@ int main(int argc, char** argv) {
             node = (int)(g_base + __builtin_popcount(g_bits & 255u & ((1u << slot) - 1u)));
         }
         if (tie) ties++;
+        if (bundle) { res[r].t = best; res[r].tri = best_tri; res[r].tie = tie; }
         // ---- check
         float want = EZ_INF;
         if (brute) {
@@ -387,6 +418,134 @@ int main(int argc, char** argv) {
             printf("%s rays, warp replay, %s triangle step (tri_w %d, refill %d): per 32 rays %.1f node steps (%.1f lanes busy), "
                    "%.1f triangle steps (%.1f lanes busy); 2 x node + triangle steps = %.1f\n", names[k], coop ? "cooperative" : "serial", coop ? tri_w : 2, refill,
                    R.node_steps * per, R.node_lanes / R.node_steps, R.tri_steps * per, R.tri_lanes / R.tri_steps, (2 * R.node_steps + R.tri_steps) * per);
+        }
+    }
+    if (bundle) {   // 32 consecutive rays, one stack, one bundle test per slot, serial triangle tests per member (see the top of the file)
+        long b_nodes = 0, b_cands = 0, b_tests = 0, r_tests = 0, n_members = 0, n_bundles = 0, bad_result = 0, bad_nodes = 0, bad_tris = 0;
+#pragma omp parallel for schedule(dynamic, 4) reduction(+ : b_nodes, b_cands, b_tests, r_tests, n_members, n_bundles, bad_result, bad_nodes, bad_tris)
+        for (int b0 = 0; b0 < NR; b0 += 32) {
+            const int nb = std::min(32, NR - b0);
+            int pend[32], np_ = 0;
+            for (int j = 0; j < nb; j++) if (ray_kind[b0 + j] >= 0) pend[np_++] = b0 + j;
+            // sub-bundles: a ray joins the first pending ray's when every component of its 1/d has the leader's sign and lies
+            // within a factor 2 of the leader's (extend_w8_bundle)
+            while (np_ > 0) {
+            int mem[32], nm = 0, rest = 0;
+            float lead[3];
+            for (int a = 0; a < 3; a++) lead[a] = EZ_DIV(1.0f, rays[(size_t)pend[0] * 7 + 3 + a]);
+            for (int k = 0; k < np_; k++) {
+                bool in = true;
+                for (int a = 0; a < 3; a++) {
+                    const float v = EZ_DIV(1.0f, rays[(size_t)pend[k] * 7 + 3 + a]), w = lead[a];
+                    in = in && (v > 0.0f) == (w > 0.0f) && fabsf(v) <= 2.0f * fabsf(w) && fabsf(w) <= 2.0f * fabsf(v);
+                }
+                if (in) mem[nm++] = pend[k]; else pend[rest++] = pend[k];
+            }
+            np_ = rest;
+            n_bundles++;
+            float bo[3][4];   // per axis: omin, omax, vmin, vmax
+            int sign[3];
+            float best[32], slack[32], inv[32][3];
+            int btri[32];
+            bool tie[32];
+            for (int a = 0; a < 3; a++) { bo[a][0] = INFINITY; bo[a][1] = -INFINITY; bo[a][2] = INFINITY; bo[a][3] = -INFINITY; }
+            int npos[3] = {0, 0, 0};
+            for (int k = 0; k < nm; k++) {
+                const float* R = &rays[(size_t)mem[k] * 7];
+                for (int a = 0; a < 3; a++) {
+                    inv[k][a] = EZ_DIV(1.0f, R[3 + a]);
+                    bo[a][0] = fminf(bo[a][0], R[a]); bo[a][1] = fmaxf(bo[a][1], R[a]);
+                    bo[a][2] = fminf(bo[a][2], inv[k][a]); bo[a][3] = fmaxf(bo[a][3], inv[k][a]);
+                    npos[a] += R[3 + a] >= 0.0f;
+                }
+                slack[k] = delta * fmaxf(fabsf(inv[k][0]), fmaxf(fabsf(inv[k][1]), fabsf(inv[k][2])));
+                best[k] = EZ_INF; btri[k] = -1; tie[k] = false;
+            }
+            for (int a = 0; a < 3; a++) sign[a] = npos[a] == nm ? 1 : (npos[a] == 0 ? 2 : 0);
+            uint32_t near_mask = 0;
+            for (int a = 0; a < 3; a++) if (rays[(size_t)mem[0] * 7 + 3 + a] >= 0.0f) near_mask |= 1u << axis_bit[a];
+            std::vector<int> vis, cand;
+            float L = EZ_INF;
+            uint32_t st_base[64], st_bits[64];
+            int sp = 0;
+            uint32_t node = 0, g_base = 0, g_bits = 0;
+            while (true) {
+                const uint32_t* w = &w8.nodes[(size_t)node * W8_NODE_WORDS];
+                vis.push_back((int)node);
+                const uint8_t* qlo = (const uint8_t*)&w[W8_W_QLO];
+                const uint8_t* qhi = (const uint8_t*)&w[W8_W_QHI];
+                const uint8_t* meta = (const uint8_t*)&w[W8_W_META];
+                uint32_t hits = 0;
+                for (int sl = 0; sl < 8; sl++) {
+                    float en[3], ex[3];
+                    for (int a = 0; a < 3; a++) {
+                        float org, sc;
+                        const uint32_t sc_bits = W8_SCALE_BITS(w[W8_W_EXP_IMASK], a);
+                        memcpy(&org, &w[W8_W_ORIGIN + a], 4);
+                        memcpy(&sc, &sc_bits, 4);
+                        const float lo = rnd(FE_DOWNWARD, '+', org, ((float)qlo[8 * a + sl] - 0.25f) * sc);
+                        const float hi = rnd(FE_UPWARD, '+', org, ((float)qhi[8 * a + sl] + 0.25f) * sc);
+                        bundle_axis(lo, hi, sign[a], bo[a][0], bo[a][1], bo[a][2], bo[a][3], en[a], ex[a]);
+                    }
+                    if (fmaxf(fmaxf(en[0], en[1]), fmaxf(en[2], 0.0f)) <= fminf(fminf(ex[0], ex[1]), fminf(ex[2], L))) hits |= 1u << sl;
+                }
+                const uint32_t imask = w[W8_W_EXP_IMASK] >> 24, inner = hits & imask;
+                uint32_t leaf = hits & ~imask, perm = 0, t_mask = 0;
+                for (int sl = 0; sl < 8; sl++) if (inner >> sl & 1) perm |= 1u << (sl ^ near_mask);
+                if (g_bits >> 8) { st_base[sp] = g_base; st_bits[sp] = g_bits; sp++; }
+                g_base = w[W8_W_CHILD_BASE];
+                g_bits = imask | (perm << 8);
+                for (int sl = 0; sl < 8; sl++) if (leaf >> sl & 1) t_mask |= ((1u << (meta[sl] >> 5)) - 1u) << (meta[sl] & 31u);
+                if (t_mask) {
+                    while (t_mask) {
+                        const int tri = (int)w[W8_W_TRI_BASE] + __builtin_ctz(t_mask);
+                        t_mask &= t_mask - 1;
+                        cand.push_back(tri);
+                        for (int k = 0; k < nm; k++) {
+                            const float* R = &rays[(size_t)mem[k] * 7];
+                            float t;
+                            const int h = tri_test(rec[tri], ez_v3(R[0], R[1], R[2]), ez_v3(R[3], R[4], R[5]), best[k], t);
+                            if (h == 2) tie[k] = true;
+                            else if (h == 1) { best[k] = t; btri[k] = tri; tie[k] = false; }
+                        }
+                    }
+                    L = 0.0f;
+                    for (int k = 0; k < nm; k++) L = fmaxf(L, best[k] + (best[k] * 0.000244140625f + slack[k]));
+                }
+                if ((g_bits >> 8) == 0) {
+                    if (sp == 0) break;
+                    --sp;
+                    g_base = st_base[sp];
+                    g_bits = st_bits[sp];
+                }
+                const int p = 31 - __builtin_clz(g_bits >> 8);
+                g_bits ^= 1u << (8 + p);
+                const uint32_t slot = (uint32_t)p ^ near_mask;
+                node = g_base + (uint32_t)__builtin_popcount(g_bits & 255u & ((1u << slot) - 1u));
+            }
+            b_nodes += (long)vis.size();
+            b_cands += (long)cand.size();
+            b_tests += (long)cand.size() * nm;
+            n_members += nm;
+            std::sort(vis.begin(), vis.end());
+            std::sort(cand.begin(), cand.end());
+            for (int k = 0; k < nm; k++) {
+                const RayResult& q = res[mem[k]];
+                r_tests += (long)q.tris.size();
+                if (memcmp(&q.t, &best[k], 4) != 0 || q.tie != tie[k] || (!q.tie && q.tri != btri[k])) bad_result++;
+                for (int x : q.nodes) if (!std::binary_search(vis.begin(), vis.end(), x)) { bad_nodes++; break; }
+                for (int x : q.tris) if (!std::binary_search(cand.begin(), cand.end(), x)) { bad_tris++; break; }
+            }
+            }
+        }
+        if (n_members > 0) {
+            const double per32 = 32.0 / n_members;
+            printf("bundle: %ld (sub-)bundles, %ld member rays; per 32 rays %.2f node visits, %.2f triangle candidates; (ray, triangle) tests per ray %.2f "
+                   "(per-ray walk %.2f); warp steps per 32 rays %.2f node + %.2f triangle\n", n_bundles, n_members, b_nodes * per32, b_cands * per32,
+                   (double)b_tests / n_members, (double)r_tests / n_members, b_nodes * per32, b_cands * per32);
+            printf("bundle checks: results differing %ld, rays with a node missing %ld, rays with a triangle missing %ld\n", bad_result, bad_nodes, bad_tris);
+            if (bad_result) return 6;
+            if (bad_nodes || bad_tris) return 5;
         }
     }
     printf("max stack depth %d, rays left to the exact kernel %ld, rays with a tie %ld\n", max_sp, skipped, ties);
