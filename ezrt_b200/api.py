@@ -18,7 +18,8 @@ MODE_DIFFUSE_P3 = 0
 MODE_DISNEY_ANISO_P4 = 1
 MODE_DISNEY_SOBOL_P5 = 2
 MODE_DISNEY_IS_MIS_P5 = 3
-MODES = {"diffuse_p3": 0, "disney_aniso_p4": 1, "disney_sobol_p5": 2, "disney_is_mis_p5": 3}
+MODE_DISNEY_LIGHTS = 4   # BRDF sampling + light sampling on the emissive triangles, MIS (DESIGN.md section 10)
+MODES = {"diffuse_p3": 0, "disney_aniso_p4": 1, "disney_sobol_p5": 2, "disney_is_mis_p5": 3, "disney_lights": 4}
 
 TRAVERSE_ACCEL = 0
 TRAVERSE_REFERENCE = 1
@@ -395,6 +396,26 @@ class Scene:
         check(lib.ezrt_trace_rays(self._h, n, _fp(o), _fp(d), int(traverse), int(bool(any_hit)), int(bool(p3_normal_fudge)),
                                   ip(hit), _fp(dist), ip(tri), ip(inside), _fp(point), _fp(normal)))
         return dict(hit=hit, distance=dist, triangle=tri, inside=inside, point=point, normal=normal)
+
+    def lights(self):
+        """The light table of MODE_DISNEY_LIGHTS (ezrt_scene_lights; built at the first call or render in that mode):
+        (triangle indices int32 [K], cdf float32 [K], W = float64 sum of the weights)."""
+        k = check(lib.ezrt_scene_lights(self._h, 0, None, None, None))
+        tri = np.zeros(k, np.int32)
+        cdf = np.zeros(k, np.float32)
+        total = C.c_double(0.0)
+        check(lib.ezrt_scene_lights(self._h, k, tri.ctypes.data_as(_lib.c_int32_p), _fp(cdf), C.byref(total)))
+        return tri, cdf, total.value
+
+    def occluded_rays(self, origins, dirs, tmax, traverse=TRAVERSE_ACCEL):
+        """ezrt_occluded_rays: 1 where nothing is accepted strictly before tmax along the ray (the render's shadow pass)."""
+        o = _f32(origins, (-1, 3))
+        d = _f32(dirs, (-1, 3))
+        n = o.shape[0]
+        t = _f32(np.broadcast_to(np.asarray(tmax, np.float32), (n,)))
+        lit = np.zeros(n, np.int32)
+        check(lib.ezrt_occluded_rays(self._h, n, _fp(o), _fp(d), _fp(t), int(traverse), lit.ctypes.data_as(_lib.c_int32_p)))
+        return lit
 
 
 def accel_build(tris, leaf_n=4, where="device", device=0):

@@ -162,6 +162,22 @@ def build_oracle_aov(force=False):
     return ORACLE_AOV_SO
 
 
+ORACLE_LIGHTS_SO = os.path.join(ROOT, "build", "libezrt_oracle_lights.so")
+
+
+def build_oracle_lights(force=False):
+    """build/libezrt_oracle_lights.so: tests/oracle_lights.cpp, the CPU restatement of the light sampling mode (light table,
+    bounded occlusion, integrator) over the oracle's functions (test infrastructure, loaded only by tests/oracle_lights.py)."""
+    src = os.path.join(ROOT, "tests", "oracle_lights.cpp")
+    deps = [src, os.path.join(ROOT, "oracle", "ezrt_oracle.cpp")] + [os.path.join(INCLUDE, f) for f in os.listdir(INCLUDE)]
+    if force or _newer(ORACLE_LIGHTS_SO, deps):
+        os.makedirs(os.path.dirname(ORACLE_LIGHTS_SO), exist_ok=True)
+        tmp = ORACLE_LIGHTS_SO + ".tmp%d" % os.getpid()
+        _run(["g++"] + HOST_FLAGS + ["-fopenmp", "-Wno-misleading-indentation", "-shared", "-I", INCLUDE, src, "-o", tmp])
+        os.replace(tmp, ORACLE_LIGHTS_SO)
+    return ORACLE_LIGHTS_SO
+
+
 def build_reference_hdrloader(force=False):
     return _oracle_recipes().build_reference_hdrloader(force)
 
@@ -222,6 +238,7 @@ def build_all(force=False, verbose=False):
     build_oracle(force=force)
     build_oracle_adaptive(force=force)
     build_oracle_aov(force=force)
+    build_oracle_lights(force=force)
     build_example(force=force)
     build_reference_hdrloader(force=force)
     build_reference_shaders(force=force)

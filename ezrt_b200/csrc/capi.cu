@@ -92,6 +92,13 @@ struct ezrt_scene {
     // feature-buffer renders: the first-hit records of a batch (32 B per sample slot); the host entry point's aov + luma2.
     // The denoiser: its ping-pong (colour, variance) images; the host entry point's device copies of its inputs
     DeviceBuffer aov_rec_buf, aov_maps_buf, denoise_buf, denoise_io_buf;
+    // the light table of the light sampling mode (build_lights, at its first use): records | cdf
+    DeviceBuffer lights_buf;
+    bool lights_built = false;
+    LightsDev lights{};
+    std::vector<int32_t> light_tri;   // the lights' triangles (caller's order)
+    std::vector<float> light_cdf;
+    double light_total = 0.0;         // W, the float64 sum of the weights
     void* hot_base = nullptr;   // accel nodes | geometry (| vertices) | shading records (L2 persisting window)
     size_t hot_bytes = 0;
     size_t l2_persist_bytes = 0;
@@ -168,7 +175,9 @@ int carve_shadow(DeviceBuffer& buf, size_t capacity, ShadowQueue& q) {
 int validate_params(const ezrt_scene* scene, const ezrt_render_params* p) {
     if (!scene || !p) return ezrt_set_error(EZRT_ERR_INVALID, "render: null argument");
     if (p->width <= 0 || p->height <= 0 || p->spp < 0) return ezrt_set_error(EZRT_ERR_INVALID, "render: bad image size/spp");
-    if (p->mode < 0 || p->mode > 3) return ezrt_set_error(EZRT_ERR_INVALID, "render: unknown mode %d", p->mode);
+    if (p->mode < 0 || p->mode > EZRT_MODE_DISNEY_LIGHTS) return ezrt_set_error(EZRT_ERR_INVALID, "render: unknown mode %d", p->mode);
+    if (p->mode == EZRT_MODE_DISNEY_LIGHTS && p->pipeline == EZRT_PIPELINE_MEGAKERNEL)
+        return ezrt_set_error(EZRT_ERR_INVALID, "render: the light sampling mode runs on the wavefront pipeline only");
     if (p->max_bounce < 0 || p->max_bounce > 64) return ezrt_set_error(EZRT_ERR_INVALID, "render: max_bounce out of range");
     if (p->out_channels != 3 && p->out_channels != 4) return ezrt_set_error(EZRT_ERR_INVALID, "render: out_channels must be 3 or 4");
     if (p->part_count < 1 || p->part_rank < 0 || p->part_rank >= p->part_count)
@@ -233,6 +242,61 @@ struct AovRun {
     float* d_aov;
     float* d_luma2;
 };
+
+// The light table of the light sampling mode (ezrt_math.h, DESIGN.md section 10), built once per scene on stream st from the
+// scene's own records: every triangle's weight, the lights kept in triangle order, their weights summed in float64 on the host,
+// the cdf and the 64-byte records uploaded.  Synchronises st.
+int build_lights(ezrt_scene* s, cudaStream_t st) {
+    if (s->lights_built) return EZRT_OK;
+    const int n = s->dev.n_triangles;
+    struct TmpBuffer : DeviceBuffer { ~TmpBuffer() { release(); } } tmp;
+    int rc = tmp.ensure(sizeof(float) * 2 * (size_t)n + sizeof(int32_t) * ((size_t)n + 4));
+    if (rc) return rc;
+    float* d_w = (float*)tmp.p;
+    float* d_wk = d_w + n;
+    int32_t* d_idx = (int32_t*)(d_wk + n);
+    int32_t* d_count = d_idx + n;
+    launch_light_weights(s->dev, d_w, st);
+    launch_light_compact(d_w, n, d_idx, d_wk, d_count, st);
+    int32_t K = 0;
+    CU_CHECK(cudaMemcpyAsync(&K, d_count, sizeof(K), cudaMemcpyDeviceToHost, st));
+    CU_CHECK(cudaStreamSynchronize(st));
+    std::vector<float> w(K);
+    std::vector<int32_t> idx(K);
+    if (K > 0) {
+        CU_CHECK(cudaMemcpyAsync(w.data(), d_wk, sizeof(float) * K, cudaMemcpyDeviceToHost, st));
+        CU_CHECK(cudaMemcpyAsync(idx.data(), d_idx, sizeof(int32_t) * K, cudaMemcpyDeviceToHost, st));
+        CU_CHECK(cudaStreamSynchronize(st));
+    }
+    double W = 0.0;
+    for (int k = 0; k < K; k++) W += (double)w[k];
+    std::vector<float> cdf(K);
+    double S = 0.0;
+    for (int k = 0; k < K; k++) {
+        S += (double)w[k];
+        cdf[k] = (float)(S / W);
+    }
+    if (K > 0) cdf[K - 1] = 1.0f;
+    LightsDev lt{};
+    if (K > 0) {
+        const size_t rec_bytes = sizeof(float4) * 4 * (size_t)K;
+        if ((rc = s->lights_buf.ensure(rec_bytes + sizeof(float) * (size_t)K))) return rc;
+        lt.rec = (const float4*)s->lights_buf.p;
+        lt.cdf = (const float*)((char*)s->lights_buf.p + rec_bytes);
+        launch_light_records(s->dev, d_idx, K, (float4*)lt.rec, st);
+        CU_CHECK(cudaMemcpyAsync((void*)lt.cdf, cdf.data(), sizeof(float) * K, cudaMemcpyHostToDevice, st));
+        CU_CHECK(cudaStreamSynchronize(st));   // cdf is pageable host memory; tmp is freed below
+    }
+    CU_CHECK(cudaGetLastError());
+    lt.n = K;
+    lt.w_total = (float)W;
+    s->lights = lt;
+    s->light_tri = idx;
+    s->light_cdf = cdf;
+    s->light_total = W;
+    s->lights_built = true;
+    return EZRT_OK;
+}
 
 RenderDev make_render_dev(const ezrt_scene* s, const ezrt_render_params* p) {
     RenderDev rd;
@@ -739,6 +803,7 @@ int ezrt_scene_destroy(ezrt_scene* s) {
     s->lo_buf.release(); s->le_buf.release(); s->counters_buf.release(); s->totals_buf.release(); s->fb_buf.release(); s->sort_buf.release();
     s->adapt_buf.release(); s->adapt_maps_buf.release();
     s->aov_rec_buf.release(); s->aov_maps_buf.release(); s->denoise_buf.release(); s->denoise_io_buf.release();
+    s->lights_buf.release();
     if (s->own_stream) cudaStreamDestroy(s->own_stream);
     if (s->copy_stream) cudaStreamDestroy(s->copy_stream);
     if (s->side_stream) cudaStreamDestroy(s->side_stream);
@@ -804,7 +869,11 @@ static int render_device_impl(ezrt_scene* s, const ezrt_render_params* p, float*
     }
 
     const size_t per_frame = (size_t)rd.n_tiles * EZRT_TILE_PIXELS;
-    const bool is_mode = (p->mode == EZRT_MODE_DISNEY_IS_MIS_P5);
+    // the modes with a shadow pass: mode 3's environment samples, the light sampling mode's bounded light samples
+    const bool lights_mode = (p->mode == EZRT_MODE_DISNEY_LIGHTS);
+    const bool is_mode = (p->mode == EZRT_MODE_DISNEY_IS_MIS_P5) || lights_mode;
+    if (lights_mode && (rc = build_lights(s, st))) return rc;
+    const LightsDev lights = lights_mode ? s->lights : LightsDev{};
     int F = p->frames_per_batch;
     if (F <= 0) F = (int)std::max<size_t>(1, ((size_t)32 << 20) / per_frame);  // ~32 M sample slots per batch (~7.5 GB of state):
                                                                               // long queues amortise the persistent kernels' ramp-up and tail
@@ -953,23 +1022,23 @@ static int render_device_impl(ezrt_scene* s, const ezrt_render_params* p, float*
                 CU_CHECK(cudaEventRecord(s->ev_fork, st));
                 CU_CHECK(cudaStreamWaitEvent(s->side_stream, s->ev_fork, 0));
                 launch_deferred_lane(s->dev, rd, d_tiles, b, batch_first, qin, defer_list, &d_ext[b], &dw_ext[b], side_hit, qout, &q_count[b + 1], sq, &s_count[b],
-                                     Lo, Le, n_fused, (uint32_t)nf, s->n_sms, s->side_stream, b == 0 ? aov_rec : nullptr);
+                                     Lo, Le, n_fused, (uint32_t)nf, s->n_sms, s->side_stream, b == 0 ? aov_rec : nullptr, lights);
                 CU_CHECK(cudaEventRecord(s->ev_join, s->side_stream));
                 s->launches += 2;
             }
             sp = s->span_begin(1, st);
             launch_shade(s->dev, rd, d_tiles, b, batch_first, qin, &q_count[b], qout, &q_count[b + 1], sq, &s_count[b], Lo, Le,
-                         n_slots, n_fused, (uint32_t)nf, s->n_sms, st, b == 0 ? aov_rec : nullptr);
+                         n_slots, n_fused, (uint32_t)nf, s->n_sms, st, b == 0 ? aov_rec : nullptr, lights);
             if (lane) CU_CHECK(cudaStreamWaitEvent(st, s->ev_join, 0));   // ... while this k_shade shades all the others; join
             s->span_end(sp, st);
             s->launches += 2;
             if (is_mode && b < p->max_bounce) {
                 sp = s->span_begin(2, st);
                 if (accel) {
-                    launch_shadow_accel(s->dev, sq, &s_count[b], &w_sh[b], Lo, defer_list, &d_sh[b], &dw_sh[b], n_slots, s->n_sms, count_ptr, st);
+                    launch_shadow_accel(s->dev, sq, &s_count[b], &w_sh[b], Lo, defer_list, &d_sh[b], &dw_sh[b], n_slots, s->n_sms, count_ptr, st, lights_mode);
                     s->launches++;
                 } else {
-                    launch_shadow(s->dev, prune, sq, &s_count[b], &w_sh[b], Lo, nullptr, n_slots, s->n_sms, st);
+                    launch_shadow(s->dev, prune, sq, &s_count[b], &w_sh[b], Lo, nullptr, n_slots, s->n_sms, st, lights_mode);
                 }
                 s->span_end(sp, st);
                 sp = s->span_begin(1, st);   // shading work: counted with k_shade
@@ -1376,6 +1445,59 @@ int ezrt_trace_rays(ezrt_scene* s, int n, const float* origins, const float* dir
     if (e == cudaSuccess) e = cudaStreamSynchronize(st);
     buf.release();
     if (e != cudaSuccess) return ezrt_set_error(EZRT_ERR_CUDA, "trace_rays: %s", cudaGetErrorString(e));
+    return EZRT_OK;
+}
+
+int ezrt_scene_lights(ezrt_scene* s, int cap, int32_t* tri_out, float* cdf_out, double* total_out) {
+    if (!s || cap < 0) return ezrt_set_error(EZRT_ERR_INVALID, "scene_lights: bad argument");
+    CU_CHECK(cudaSetDevice(s->device));
+    int rc = build_lights(s, s->own_stream);
+    if (rc) return rc;
+    const int K = (int)s->light_tri.size();
+    const int m = std::min(K, cap);
+    if (tri_out) std::copy(s->light_tri.begin(), s->light_tri.begin() + m, tri_out);
+    if (cdf_out) std::copy(s->light_cdf.begin(), s->light_cdf.begin() + m, cdf_out);
+    if (total_out) *total_out = s->light_total;
+    return K;
+}
+
+int ezrt_occluded_rays(ezrt_scene* s, int n, const float* origins, const float* dirs, const float* tmax, int traverse, int32_t* out_lit) {
+    if (!s || n < 0 || !origins || !dirs || !tmax || !out_lit) return ezrt_set_error(EZRT_ERR_INVALID, "occluded_rays: null argument");
+    if (traverse < EZRT_TRAVERSE_ACCEL || traverse > EZRT_TRAVERSE_PRUNED) return ezrt_set_error(EZRT_ERR_INVALID, "occluded_rays: bad traverse");
+    if (n == 0) return EZRT_OK;
+    CU_CHECK(cudaSetDevice(s->device));
+    // the render's shadow pass over a shadow queue of n rays (only ray_o, ray_d, nrm.w and lit are read / written)
+    const size_t N = (size_t)n;
+    std::vector<float4> ho(N), hd(N), hn(N);
+    bool bounded = false;
+    for (size_t i = 0; i < N; i++) {
+        ho[i] = make_float4(origins[3 * i], origins[3 * i + 1], origins[3 * i + 2], 0.0f);
+        hd[i] = make_float4(dirs[3 * i], dirs[3 * i + 1], dirs[3 * i + 2], 0.0f);
+        hn[i] = make_float4(0.0f, 0.0f, 0.0f, tmax[i]);
+        bounded = bounded || !(std::isinf(tmax[i]) && tmax[i] > 0.0f);
+    }
+    struct TmpBuffer : DeviceBuffer { ~TmpBuffer() { release(); } } qbuf, buf;
+    ShadowQueue sq{};
+    int rc = carve_shadow(qbuf, N, sq);
+    if (rc) return rc;
+    if ((rc = buf.ensure(sizeof(uint32_t) * (N + 8)))) return rc;
+    uint32_t* d_defer = (uint32_t*)buf.p;
+    uint32_t* d_cnt = d_defer + N;   // [0] n, [1] work, [2] deferred, [3] deferred work
+    const bool prune = s->regular_tree && traverse != EZRT_TRAVERSE_REFERENCE;
+    const bool accel = s->regular_tree && s->have_accel && traverse == EZRT_TRAVERSE_ACCEL;
+    cudaStream_t st = s->own_stream;
+    const uint32_t counters[4] = {(uint32_t)n, 0u, 0u, 0u};
+    std::vector<unsigned char> lit(N);
+    CU_CHECK(cudaMemcpyAsync(sq.ray_o, ho.data(), sizeof(float4) * N, cudaMemcpyHostToDevice, st));
+    CU_CHECK(cudaMemcpyAsync(sq.ray_d, hd.data(), sizeof(float4) * N, cudaMemcpyHostToDevice, st));
+    CU_CHECK(cudaMemcpyAsync(sq.nrm, hn.data(), sizeof(float4) * N, cudaMemcpyHostToDevice, st));
+    CU_CHECK(cudaMemcpyAsync(d_cnt, counters, sizeof(counters), cudaMemcpyHostToDevice, st));
+    if (accel) launch_shadow_accel(s->dev, sq, d_cnt, d_cnt + 1, nullptr, d_defer, d_cnt + 2, d_cnt + 3, (uint32_t)n, s->n_sms, nullptr, st, bounded);
+    else launch_shadow(s->dev, prune, sq, d_cnt, d_cnt + 1, nullptr, nullptr, (uint32_t)n, s->n_sms, st, bounded);
+    CU_CHECK(cudaGetLastError());
+    CU_CHECK(cudaMemcpyAsync(lit.data(), sq.lit, N, cudaMemcpyDeviceToHost, st));
+    CU_CHECK(cudaStreamSynchronize(st));
+    for (size_t i = 0; i < N; i++) out_lit[i] = lit[i] ? 1 : 0;
     return EZRT_OK;
 }
 

@@ -414,10 +414,11 @@ __device__ __forceinline__ bool prune_test(float t0, float best, float slack) {
 
 // hitBVH.  PRUNE: skip sub-trees whose box entry lies beyond the best hit (+ conservative slack);
 // ANYHIT: return on the first accepted triangle (shadow rays only need isHit, P5/fsh:826-829).
+// tmax: a bounded ray (light samples) starts with best = tmax, so only hits strictly closer than tmax are accepted.
 template <bool PRUNE, bool ANYHIT, bool FAST>
-__device__ __forceinline__ HitRec trace_impl(const SceneDev& sc, vec3 o, vec3 d, vec3 inv, float slack) {
+__device__ __forceinline__ HitRec trace_impl(const SceneDev& sc, vec3 o, vec3 d, vec3 inv, float slack, float tmax = EZ_INF) {
     HitRec res;
-    res.t = EZ_INF;
+    res.t = tmax;
     res.tri = -1;
     int stack[EZRT_MAX_STACK];
     float stack_t0[PRUNE ? EZRT_MAX_STACK : 1];
@@ -566,7 +567,15 @@ struct W8Counts {   // COUNT instantiations only (bench.py roofline: records fet
     unsigned long long* tri_tests;
 };
 
-template <bool PRUNE, bool ANYHIT, bool ACCEL, bool WIDE, int LL, bool COUNT, bool Q16, class RayIO>
+// BOUNDED (shadow rays of the light sampling mode): ray i starts with best = io.tmax(i) instead of EZ_INF, so a triangle occludes
+// only if it is accepted strictly before tmax.  A hit at exactly tmax is not accepted: it must not end an any-hit traversal.
+template <bool BOUNDED, class RayIO>
+__device__ __forceinline__ float ray_tmax(const RayIO& io, uint32_t i) {
+    if constexpr (BOUNDED) return io.tmax(i);
+    else return EZ_INF;
+}
+
+template <bool PRUNE, bool ANYHIT, bool ACCEL, bool WIDE, int LL, bool COUNT, bool Q16, bool BOUNDED = false, class RayIO>
 __device__ __forceinline__ void extend_persistent(const SceneDev& sc, const TreeView tree, uint32_t n, uint32_t* work, RayIO io,
                                                   const float4* smem_top, W8Counts counts = W8Counts{nullptr, nullptr}, int refill_override = 0,
                                                   int chunk_override = 0) {
@@ -638,13 +647,13 @@ __device__ __forceinline__ void extend_persistent(const SceneDev& sc, const Tree
                         ray = (int)idx;
                         ref = tree.root_ref;
                         sp = 0;
-                        best = EZ_INF;
+                        best = ray_tmax<BOUNDED>(io, idx);
                         best_tri = -1;
                         tie = false;
                     } else if (ACCEL) {  // exact kernel handles the literal ternary min/max path
                         io.defer(idx, o, d);
                     } else {  // a zero / NaN direction component: literal ternary min/max path (rare)
-                        io.store(idx, trace_impl<PRUNE, ANYHIT, false>(sc, o, d, inv, slack), false, o, d, inv);
+                        io.store(idx, trace_impl<PRUNE, ANYHIT, false>(sc, o, d, inv, slack, ray_tmax<BOUNDED>(io, idx)), false, o, d, inv);
                     }
                 }
             }
@@ -829,12 +838,13 @@ __device__ __forceinline__ void extend_persistent(const SceneDev& sc, const Tree
                     const unsigned mq = (win >> (LL * pos)) & ((1u << LL) - 1u);
                     if (mq != 0u) {
                         const float tn = __uint_as_float(res);
+                        const bool strict = !ACCEL || tn < best;
                         if (ACCEL && (__popc(mq) > 1 || tn == best)) tie = true;
-                        if (!ACCEL || tn < best) {  // ACCEL accepts t == best only to flag the tie
+                        if (strict) {  // ACCEL accepts t == best only to flag the tie
                             best = tn;
                             best_tri = leaf_first + __ffs(mq) - 1;
                         }
-                        if (ANYHIT) stop = true;
+                        if (ANYHIT && (!BOUNDED || strict)) stop = true;   // bounded: a hit at exactly tmax does not end the ray
                     }
                     leaf_first += LL;
                     leaf_cnt -= LL;
@@ -927,7 +937,7 @@ __device__ __forceinline__ int nth_set_bit(uint32_t m, int r) {
 // stack : uint2 [entries][blockDim.x] in shared memory
 // IDX: the scene's triangle records are indexed (SceneDev::acc_tri_indexed; one instantiation per layout keeps each within 64
 // registers without spilling)
-template <bool ANYHIT, bool COUNT, bool IDX, class RayIO>
+template <bool ANYHIT, bool COUNT, bool IDX, bool BOUNDED = false, class RayIO>
 __device__ __forceinline__ void extend_w8(const SceneDev& sc, uint32_t n, uint32_t* work, RayIO io, const unsigned char* s_perm, uint2* stack_sm,
                                           W8Counts counts) {
     const bool tri_na = sc.tri_l1_bypass != 0;
@@ -1012,7 +1022,7 @@ __device__ __forceinline__ void extend_w8(const SceneDev& sc, uint32_t n, uint32
                         sp = 0;
                         g_bits = 0u;
                         t_mask = 0u;
-                        best = EZ_INF;
+                        best = ray_tmax<BOUNDED>(io, idx);   // bounded: a hit at exactly tmax is a tie, which does not end the ray
                         best_tri = -1;
                         tie = false;
                     } else {  // outside the decode error bound: the exact kernel traces it
@@ -1730,6 +1740,8 @@ struct ShadowRay {
     vec3 o, d, contrib;      // contrib: DEFER_NEE = false
     vec3 N, V, history;      // DEFER_NEE = true: the inputs of nee_contrib, evaluated only if the shadow ray gets through (k_nee)
     int matId;
+    float tmax, pdf;         // light sampling mode: the shadow ray's bound and the light sample's pdf ...
+    int light_mat;           // ... and the light's material id (nee_light_contrib)
 };
 
 // Lo += a*b*c*s/p evaluated left to right as GLSL does
@@ -1760,6 +1772,26 @@ __device__ __forceinline__ vec3 nee_contrib(const SceneDev& sc, const RenderDev&
     const float mis_weight = mis_mix_weight(pdf_light, pdf_h);
     return ez_divs(ez_scale(ez_mul(ez_mul(ez_scale(history, mis_weight), color), fr_h), NdotLh), pdf_light);
 }
+// The light sampling mode's light sample (ezrt_math.h, DESIGN.md section 10), evaluated by k_nee<EZRT_MODE_DISNEY_LIGHTS> for the lit
+// rays: history * mis(pdf_l, BRDF_Pdf) * E * f_r * dot(N, L) / pdf_l, left to right as nee_contrib.
+__device__ __forceinline__ vec3 nee_light_contrib(vec3 V, vec3 N, vec3 L, const MaterialDev& mat, vec3 history, vec3 E, float pdf_l) {
+    const float NdotL = ez_dot(N, L);
+    const vec3 fr = brdf_evaluate<false>(V, N, L, mat);
+    const float pdf_b = brdf_pdf(V, N, L, mat);
+    const float mis_weight = mis_mix_weight(pdf_l, pdf_b);
+    return ez_divs(ez_scale(ez_mul(ez_mul(ez_scale(history, mis_weight), E), fr), NdotL), pdf_l);
+}
+// the three vertices of triangle `tri` in the policy's index space (flat or indexed record)
+__device__ __forceinline__ void tri_vertices(const SceneDev& sc, int tri, bool accel_space, vec3& p1, vec3& p2, vec3& p3) {
+    const float4* g = tri_geo_rec(sc, tri, accel_space);
+    const float4* v = g;
+    uint32_t i1 = 1u, i2 = 2u, i3 = 3u;
+    if (accel_space && sc.acc_tri_indexed) {
+        const uint4 qi = __ldg(reinterpret_cast<const uint4*>(g + 1));
+        v = sc.acc_tri_vert; i1 = qi.x; i2 = qi.y; i3 = qi.z;
+    }
+    p1 = f4xyz(ldg4(v + i1)); p2 = f4xyz(ldg4(v + i2)); p3 = f4xyz(ldg4(v + i3));
+}
 
 // DEFER_NEE (wavefront pipeline, IS/MIS mode): the shadow ray carries the inputs of nee_contrib instead of its value -- the
 // BRDF / environment evaluation of the light sample runs after the shadow pass, only for the rays that got through, and is
@@ -1770,10 +1802,12 @@ __device__ __forceinline__ vec3 nee_contrib(const SceneDev& sc, const RenderDev&
 template <int MODE, bool DEFER_NEE = false, bool AOV = false>
 __device__ __forceinline__ bool shade_step(const SceneDev& sc, const RenderDev& rd, int bounce, PathRegs& p, float hit_t,
                                            int hit_tri, uint32_t px, uint32_t py, float2 sob, vec3& Lo, vec3& Le,
-                                           bool& primary_miss, ShadowRay& sh, float4* aov_rec = nullptr) {
+                                           bool& primary_miss, ShadowRay& sh, float4* aov_rec = nullptr, LightsDev lights = LightsDev{}) {
     sh.valid = false;
     const int mode = (MODE < 0) ? rd.mode : MODE;
     const bool is_mode = (mode == EZRT_MODE_DISNEY_IS_MIS_P5);
+    // the light sampling mode exists only as k_shade<EZRT_MODE_DISNEY_LIGHTS> (the megakernel, MODE < 0, rejects it)
+    constexpr bool lights_mode = (MODE == EZRT_MODE_DISNEY_LIGHTS);
     if (bounce == 0) {
         Lo = splat3(0.0f);
         Le = splat3(0.0f);
@@ -1784,7 +1818,7 @@ __device__ __forceinline__ bool shade_step(const SceneDev& sc, const RenderDev& 
             return false;
         }
     } else {
-        if (is_mode && p.pdf <= 0.0f) return false;  // P5/fsh:865
+        if ((is_mode || lights_mode) && p.pdf <= 0.0f) return false;  // P5/fsh:865
         if (hit_tri < 0) {  // miss: sky contribution, then break
             vec3 sky = hdr_color(sc, rd, p.d, mode);
             if (is_mode) {  // P5/fsh:868-878
@@ -1808,7 +1842,21 @@ __device__ __forceinline__ bool shade_step(const SceneDev& sc, const RenderDev& 
             aov_rec[1] = make_float4(hit.N.x, hit.N.y, hit.N.z, 0.0f);
         }
     } else {
-        Lo = ez_add(Lo, contrib3(p.history, mat.emissive, p.f_r, p.cosine_i, p.pdf));
+        if (lights_mode) {   // a BRDF sample that hit a light: MIS against the light sampling pdf of the hit point
+            float w = 1.0f;
+            const float lum = ez_luminance(mat.emissive);
+            if (lum > 0.0f) {   // otherwise the weight area * lum is never a light
+                vec3 p1, p2, p3;
+                tri_vertices(sc, hit_tri, rd.accel_space != 0, p1, p2, p3);
+                if (ez_is_light(ez_light_weight(p1, p2, p3, mat.emissive))) {
+                    const vec3 Ng = f4xyz(ldg4(tri_geo_rec(sc, hit_tri, rd.accel_space != 0)));
+                    w = mis_mix_weight(p.pdf, ez_light_pdf(lum, lights.w_total, hit_t, ez_abs(ez_dot(Ng, p.d))));
+                }
+            }
+            Lo = ez_add(Lo, ez_divs(ez_scale(ez_mul(ez_mul(ez_scale(p.history, w), mat.emissive), p.f_r), p.cosine_i), p.pdf));
+        } else {
+            Lo = ez_add(Lo, contrib3(p.history, mat.emissive, p.f_r, p.cosine_i, p.pdf));
+        }
         p.history = ez_mul(p.history, ez_divs(ez_scale(p.f_r, p.cosine_i), p.pdf));
     }
     if (bounce >= rd.max_bounce) return false;
@@ -1816,7 +1864,43 @@ __device__ __forceinline__ bool shade_step(const SceneDev& sc, const RenderDev& 
     vec3 V = ez_neg(p.d);
     vec3 N = hit.N;
     vec3 L;
-    if (is_mode) {
+    if (lights_mode) {
+        // one light sample on the emissive triangles (ezrt_math.h, DESIGN.md section 10), then mode 3's BRDF sample.  The three
+        // draws of the light sample come first and are made whether or not the scene has a light.
+        const float r_sel = rand01(p.seed);
+        const float r_1 = rand01(p.seed);
+        const float r_2 = rand01(p.seed);
+        float xi_1 = sob.x, xi_2 = sob.y;
+        cp_rotate(xi_1, xi_2, px, py);
+        const float xi_3 = rand01(p.seed);
+        L = sample_brdf(xi_1, xi_2, xi_3, V, N, mat);
+        const float NdotL = ez_dot(N, L);
+        vec3 fr_l = splat3(0.0f);
+        float pdf_l = 0.0f;
+        if (NdotL > 0.0f) { fr_l = brdf_evaluate<false>(V, N, L, mat); pdf_l = brdf_pdf(V, N, L, mat); }
+        if (lights.n > 0) {
+            const float4* lr = lights.rec + 4 * (size_t)ez_light_select(lights.cdf, lights.n, r_sel);
+            const float4 a = ldg4(lr), b = ldg4(lr + 1), c = ldg4(lr + 2), e = ldg4(lr + 3);
+            const int self = __float_as_int(rd.accel_space ? c.w : b.w);   // the light's triangle in the hit's index space
+            const vec3 D = ez_sub(ez_triangle_point(f4xyz(a), f4xyz(b), f4xyz(c), r_1, r_2), hit.P);
+            const float dist = EZ_SQRT(ez_dot(D, D));
+            const vec3 Ll = ez_normalize(D);
+            const float cos_l = ez_abs(ez_dot(f4xyz(e), Ll));
+            if (self != hit_tri && ez_dot(N, Ll) > 0.0f && cos_l != 0.0f && dist != 0.0f) {
+                sh.valid = true;
+                sh.o = hit.P;
+                sh.d = Ll;
+                sh.N = N; sh.V = V; sh.history = p.history; sh.matId = hit.matId;
+                sh.tmax = ez_light_tmax(dist);
+                sh.pdf = ez_light_pdf(e.w, lights.w_total, dist, cos_l);
+                sh.light_mat = __float_as_int(a.w);
+            }
+        }
+        if (NdotL <= 0.0f) return false;
+        p.f_r = fr_l;
+        p.pdf = pdf_l;   // <= 0: traced, then break
+        p.cosine_i = NdotL;
+    } else if (is_mode) {
         // environment importance sample + shadow ray (P5/fsh:820-842), then the BRDF sample (:845-865).  The three
         // random numbers are drawn in the shader's order (two for SampleHdr :822, one for the lobe choice :849); the BRDF
         // value and pdf of the two directions are evaluated by ONE copy of the code (a two-trip loop that is not unrolled)

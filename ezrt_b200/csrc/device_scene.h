@@ -117,15 +117,26 @@ struct PathQueue {
     float4* fr;       // (f_r.xyz, pdf)   pdf <= 0 marks "break after trace" (P5/fsh:865)
 };
 
+// The emissive-triangle light table of mode EZRT_MODE_DISNEY_LIGHTS (ezrt_math.h, DESIGN.md section 10), built at the first
+// render in that mode.  Passed to k_shade / k_nee as a parameter of its own (not a SceneDev member, so the other kernels keep
+// their parameter layout).  Light record k (64 B): (p1, material id as bits) (p2, reference triangle index as bits)
+// (p3, accel-order triangle index as bits) (N, ez_luminance(emissive)).
+struct LightsDev {
+    const float4* rec;   // 4 float4 per light
+    const float* cdf;    // n floats, cdf[n - 1] = 1
+    int n;               // 0: no light (no light samples)
+    float w_total;       // W_f = (float) sum of the weights
+};
+
 // A shadow ray and what k_nee needs to evaluate the light sample's contribution once the ray got through (nee_contrib):
 // the BRDF / environment evaluation of the light sample is done after the shadow pass, for unoccluded rays only.
 #define EZRT_SHADOW_SLOT_BYTES (5 * 16 + 1)
 struct ShadowQueue {
     float4* ray_o;       // (origin.xyz, sample slot as bits)
     float4* ray_d;       // (direction to the light.xyz, material id as bits)
-    float4* nrm;         // (shading normal N.xyz, -)
-    float4* view;        // (V = -incoming direction.xyz, -)
-    float4* hist;        // (path history.xyz, -)
+    float4* nrm;         // (shading normal N.xyz, -; bounded rays of the light sampling mode: tmax)
+    float4* view;        // (V = -incoming direction.xyz, -; light sampling mode: pdf of the light sample)
+    float4* hist;        // (path history.xyz, -; light sampling mode: the light's material id as bits)
     unsigned char* lit;  // written by the shadow pass: 1 = nothing between the surface and the environment
 };
 

@@ -273,11 +273,14 @@ struct ShadowIO {
     }
     // every shadow ray's flag is written exactly once per pass (here, or by the exact pass over the rays an accel kernel deferred)
     __device__ __forceinline__ void mark(uint32_t j, bool lit) const { sq.lit[j] = lit ? 1 : 0; }
+    // bounded shadow rays (light sampling mode): the bound travels in nrm.w
+    __device__ __forceinline__ float tmax(uint32_t i) const { return __ldcs(sq.nrm + (perm ? perm[i] : i)).w; }
     __device__ __forceinline__ void store(uint32_t i, HitRec h, bool, vec3, vec3, vec3) const { mark(perm ? perm[i] : i, h.tri < 0); }
     __device__ __forceinline__ void defer(uint32_t, vec3, vec3) const {}
 };
 
-template <bool PRUNE>
+// BOUNDED (light sampling mode): ray j only looks for occluders strictly before sq.nrm[j].w (extend_persistent)
+template <bool PRUNE, bool BOUNDED = false>
 __global__ void __launch_bounds__(EZRT_EXTEND_MAX_THREADS, EZRT_EXTEND_LB_BLOCKS) k_shadow(SceneDev sc, ShadowQueue sq, const uint32_t* __restrict__ s_count,
                                                                 uint32_t* work, float4* __restrict__ Lo, const uint32_t* __restrict__ perm) {
     ShadowIO io;
@@ -288,7 +291,7 @@ __global__ void __launch_bounds__(EZRT_EXTEND_MAX_THREADS, EZRT_EXTEND_LB_BLOCKS
     if (blockIdx.x * blockDim.x >= n) return;
     const TreeView tree = reference_tree(sc);
     stage_top_nodes(tree);
-    extend_persistent<PRUNE, true, false, false, 8, false, false>(sc, tree, n, work, io, g_smem_top);
+    extend_persistent<PRUNE, true, false, false, 8, false, false, BOUNDED>(sc, tree, n, work, io, g_smem_top);
 }
 
 // ---- accel kernels: the device's own tree (4-wide exact boxes: extend_persistent<ACCEL, WIDE>; or W8: extend_w8 on the
@@ -427,6 +430,7 @@ struct AccelShadowIO {
     uint32_t* defer_list;
     uint32_t* defer_count;
     __device__ __forceinline__ bool load(uint32_t i, vec3& o, vec3& d) const { return base.load(i, o, d); }
+    __device__ __forceinline__ float tmax(uint32_t i) const { return base.tmax(i); }
     __device__ __forceinline__ void defer(uint32_t i, vec3, vec3) const { defer_list[atomicAdd(defer_count, 1u)] = i; }
     __device__ __forceinline__ void store(uint32_t i, HitRec h, bool, vec3 o, vec3 d, vec3 inv) const {
         if (h.tri < 0) {  // nothing accepted anywhere: the shader finds nothing either
@@ -439,7 +443,7 @@ struct AccelShadowIO {
     }
 };
 
-template <bool COUNT, bool IDX>
+template <bool COUNT, bool IDX, bool BOUNDED = false>
 __global__ void __launch_bounds__(EZRT_EXTEND_MAX_THREADS, EZRT_EXTEND_LB_BLOCKS) k_shadow_w8(SceneDev sc, ShadowQueue sq, const uint32_t* __restrict__ s_count, uint32_t* work,
                                                                    float4* __restrict__ Lo, uint32_t* defer_list, uint32_t* defer_count, W8Counts counts) {
     unsigned char* s_perm;
@@ -453,7 +457,7 @@ __global__ void __launch_bounds__(EZRT_EXTEND_MAX_THREADS, EZRT_EXTEND_LB_BLOCKS
     io.leaf_box = sc.leaf_box;
     io.defer_list = defer_list;
     io.defer_count = defer_count;
-    extend_w8<true, COUNT, IDX>(sc, *s_count, work, io, s_perm, stack_sm, counts);
+    extend_w8<true, COUNT, IDX, BOUNDED>(sc, *s_count, work, io, s_perm, stack_sm, counts);
 }
 
 // ---- the same three passes on the 4-wide exact-box tree (default form, env EZRT_ACCEL): extend_persistent<ACCEL, WIDE>
@@ -486,7 +490,7 @@ __global__ void __launch_bounds__(EZRT_EXTEND_MAX_THREADS, EZRT_EXTEND_LB_BLOCKS
     io.defer_count = defer_count;
     extend_persistent<true, false, true, true, 4, COUNT, false>(sc, accel_tree(sc), n_slots, work, io, g_smem_top, counts, sc.refill_thresh_camera, sc.work_chunk_camera);
 }
-template <bool COUNT, bool Q16>
+template <bool COUNT, bool Q16, bool BOUNDED = false>
 __global__ void __launch_bounds__(EZRT_EXTEND_MAX_THREADS, EZRT_EXTEND_LB_BLOCKS) k_shadow_accel(SceneDev sc, ShadowQueue sq, const uint32_t* __restrict__ s_count, uint32_t* work,
                                                                       float4* __restrict__ Lo, uint32_t* defer_list, uint32_t* defer_count, W8Counts counts) {
     AccelShadowIO io;
@@ -497,7 +501,7 @@ __global__ void __launch_bounds__(EZRT_EXTEND_MAX_THREADS, EZRT_EXTEND_LB_BLOCKS
     io.leaf_box = sc.leaf_box;
     io.defer_list = defer_list;
     io.defer_count = defer_count;
-    extend_persistent<true, true, true, true, 4, COUNT, Q16>(sc, accel_tree(sc), *s_count, work, io, g_smem_top, counts);
+    extend_persistent<true, true, true, true, 4, COUNT, Q16, BOUNDED>(sc, accel_tree(sc), *s_count, work, io, g_smem_top, counts);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -525,11 +529,12 @@ __global__ void __launch_bounds__(128, EZRT_SHADE_MIN_BLOCKS) k_shade(SceneDev s
                                                PathQueue qout, uint32_t* out_count, ShadowQueue sq, uint32_t* s_count,
                                                float4* __restrict__ Lo, float4* __restrict__ Le, uint32_t n_fused, uint32_t n_frames,
                                                const uint32_t* __restrict__ list, const float2* __restrict__ side_hit,
-                                               float4* __restrict__ aov_rec) {
+                                               float4* __restrict__ aov_rec, LightsDev lights) {
     // The Sobol pair of (bounce, frame) is the same for every pixel of a frame (P5/fsh:361-376: up to 2 x 32 table XORs per path): each
     // block computes the pairs of the batch's frames once into shared memory (batches of more than EZRT_SOBOL_TABLE frames compute per path).
     __shared__ float2 s_sobol[EZRT_SOBOL_TABLE];
-    const bool sobol_table = (MODE == EZRT_MODE_DISNEY_SOBOL_P5 || MODE == EZRT_MODE_DISNEY_IS_MIS_P5) && n_frames <= EZRT_SOBOL_TABLE;
+    const bool sobol_table = (MODE == EZRT_MODE_DISNEY_SOBOL_P5 || MODE == EZRT_MODE_DISNEY_IS_MIS_P5 || MODE == EZRT_MODE_DISNEY_LIGHTS) &&
+                             n_frames <= EZRT_SOBOL_TABLE;
     if (sobol_table) {
         for (uint32_t f = threadIdx.x; f < n_frames; f += blockDim.x) s_sobol[f] = sobol_pair(bounce, batch_first_frame + f);
         __syncthreads();
@@ -649,7 +654,7 @@ __global__ void __launch_bounds__(128, EZRT_SHADE_MIN_BLOCKS) k_shade(SceneDev s
 #endif
             if (LIST || __float_as_int(hit.y) != EZRT_TRI_PENDING) {   // pending: deferred by the accel kernel, shaded by the LIST pass
                 alive = shade_step<MODE, MODE == EZRT_MODE_DISNEY_IS_MIS_P5, AOV>(sc, rd, bounce, p, hit.x, __float_as_int(hit.y), px, py, sob, lo, le,
-                                                                                 pmiss, sh, AOV ? aov_rec + 2 * (size_t)slot : nullptr);
+                                                                                 pmiss, sh, AOV ? aov_rec + 2 * (size_t)slot : nullptr, lights);
                 if (bounce == 0) {
                     // Le is zero for every surface that does not emit: it is stored (and read back by k_blend) only otherwise.
                     // color = Le + Lo with Le = +-0 is Lo bit for bit, because Lo is never -0.0 (it starts at +0.0 and only grows by additions)
@@ -669,14 +674,15 @@ __global__ void __launch_bounds__(128, EZRT_SHADE_MIN_BLOCKS) k_shade(SceneDev s
             __stcs(qout.hist + pos, make_float4(p.history.x, p.history.y, p.history.z, p.cosine_i));
             __stcs(qout.fr + pos, make_float4(p.f_r.x, p.f_r.y, p.f_r.z, p.pdf));
         }
-        if (MODE == EZRT_MODE_DISNEY_IS_MIS_P5) {
+        if (MODE == EZRT_MODE_DISNEY_IS_MIS_P5 || MODE == EZRT_MODE_DISNEY_LIGHTS) {
+            constexpr bool LT = (MODE == EZRT_MODE_DISNEY_LIGHTS);   // light samples: tmax, pdf and the light's material in the .w words
             uint32_t spos = block_append(sh.valid, s_count, s_scan);
             if (sh.valid) {
                 __stcs(sq.ray_o + spos, make_float4(sh.o.x, sh.o.y, sh.o.z, __uint_as_float(slot)));
                 __stcs(sq.ray_d + spos, make_float4(sh.d.x, sh.d.y, sh.d.z, __int_as_float(sh.matId)));
-                __stcs(sq.nrm + spos, make_float4(sh.N.x, sh.N.y, sh.N.z, 0.0f));
-                __stcs(sq.view + spos, make_float4(sh.V.x, sh.V.y, sh.V.z, 0.0f));
-                __stcs(sq.hist + spos, make_float4(sh.history.x, sh.history.y, sh.history.z, 0.0f));
+                __stcs(sq.nrm + spos, make_float4(sh.N.x, sh.N.y, sh.N.z, LT ? sh.tmax : 0.0f));
+                __stcs(sq.view + spos, make_float4(sh.V.x, sh.V.y, sh.V.z, LT ? sh.pdf : 0.0f));
+                __stcs(sq.hist + spos, make_float4(sh.history.x, sh.history.y, sh.history.z, LT ? __int_as_float(sh.light_mat) : 0.0f));
             }
         }
     }
@@ -688,6 +694,8 @@ __global__ void __launch_bounds__(128, EZRT_SHADE_MIN_BLOCKS) k_shade(SceneDev s
 // the shadow pass, instead of for every light sample in k_shade.  Each block compacts the lit rays of 512 queue entries in
 // shared memory so that full warps evaluate.  One shadow ray per sample slot and bounce: no two threads touch one Lo entry.
 // ------------------------------------------------------------------------------------------
+// MODE = EZRT_MODE_DISNEY_LIGHTS: the light samples on the emissive triangles (nee_light_contrib; view.w = pdf, hist.w = the light's material).
+template <int MODE>
 __global__ void __launch_bounds__(128, 8) k_nee(SceneDev sc, RenderDev rd, ShadowQueue sq, const uint32_t* __restrict__ s_count, float4* __restrict__ Lo) {
     __shared__ uint32_t s_scan[34];
     __shared__ uint32_t s_total;
@@ -710,8 +718,13 @@ __global__ void __launch_bounds__(128, 8) k_nee(SceneDev sc, RenderDev rd, Shado
             const float4 o4 = __ldcs(sq.ray_o + j), d4 = __ldcs(sq.ray_d + j), n4 = __ldcs(sq.nrm + j), v4 = __ldcs(sq.view + j), h4 = __ldcs(sq.hist + j);
             const uint32_t slot = __float_as_uint(o4.w);
             const MaterialDev mat = load_material(sc, __float_as_int(d4.w));
-            const vec3 c = nee_contrib(sc, rd, EZRT_MODE_DISNEY_IS_MIS_P5, ez_v3(v4.x, v4.y, v4.z), ez_v3(n4.x, n4.y, n4.z), ez_v3(d4.x, d4.y, d4.z), mat,
-                                       ez_v3(h4.x, h4.y, h4.z));
+            vec3 c;
+            if (MODE == EZRT_MODE_DISNEY_LIGHTS)
+                c = nee_light_contrib(ez_v3(v4.x, v4.y, v4.z), ez_v3(n4.x, n4.y, n4.z), ez_v3(d4.x, d4.y, d4.z), mat, ez_v3(h4.x, h4.y, h4.z),
+                                      load_emissive(sc, __float_as_int(h4.w)), v4.w);
+            else
+                c = nee_contrib(sc, rd, EZRT_MODE_DISNEY_IS_MIS_P5, ez_v3(v4.x, v4.y, v4.z), ez_v3(n4.x, n4.y, n4.z), ez_v3(d4.x, d4.y, d4.z), mat,
+                                ez_v3(h4.x, h4.y, h4.z));
             float4 lo = Lo[slot];
             lo.x += c.x; lo.y += c.y; lo.z += c.z;
             Lo[slot] = lo;
@@ -1182,10 +1195,12 @@ void launch_ray_sort(const SceneDev& sc, PathQueue q, const uint32_t* q_count, u
     k_sort_scatter<<<blocks, 256, 0, st>>>(q_count, keys, bins, perm);
 }
 void launch_shadow(const SceneDev& sc, bool prune, ShadowQueue sq, const uint32_t* s_count, uint32_t* work, float4* Lo,
-                   const uint32_t* perm, uint32_t n_max, int n_sms, cudaStream_t st) {
+                   const uint32_t* perm, uint32_t n_max, int n_sms, cudaStream_t st, bool bounded) {
     const int threads = extend_threads(), blocks = persistent_blocks(n_max, n_sms);
-    if (prune) k_shadow<true><<<blocks, threads, smem_for(k_shadow<true>, sc.top_nodes), st>>>(sc, sq, s_count, work, Lo, perm);
-    else k_shadow<false><<<blocks, threads, smem_for(k_shadow<false>, sc.top_nodes), st>>>(sc, sq, s_count, work, Lo, perm);
+#define EZRT_LAUNCH_SHADOW(P, B) k_shadow<P, B><<<blocks, threads, smem_for(k_shadow<P, B>, sc.top_nodes), st>>>(sc, sq, s_count, work, Lo, perm)
+    if (bounded) { if (prune) EZRT_LAUNCH_SHADOW(true, true); else EZRT_LAUNCH_SHADOW(false, true); }
+    else { if (prune) EZRT_LAUNCH_SHADOW(true, false); else EZRT_LAUNCH_SHADOW(false, false); }
+#undef EZRT_LAUNCH_SHADOW
 }
 // camera pass of the W8 policy: rays generated in the kernel (slot i = ray i), then the exact pass over the deferred ones
 void launch_extend_camera(const SceneDev& sc, const RenderDev& rd, const TileDev* tiles, uint32_t batch_first_frame, uint32_t n_slots, uint32_t n_frames, PathQueue q,
@@ -1209,14 +1224,14 @@ void launch_extend_camera(const SceneDev& sc, const RenderDev& rd, const TileDev
     }
     launch_extend(sc, true, false, q, defer_count, defer_work, defer_list, 1, std::min<uint32_t>(n_slots, 65536u), n_sms, st, nullptr, exact_gate);
 }
-void launch_shadow_accel(const SceneDev& sc, ShadowQueue sq, const uint32_t* s_count, uint32_t* work, float4* Lo, uint32_t* defer_list,
-                         uint32_t* defer_count, uint32_t* defer_work, uint32_t n_max, int n_sms, unsigned long long* counts, cudaStream_t st) {
-    const int threads = extend_threads(), blocks = persistent_blocks(n_max, n_sms);
+template <bool B>
+static void launch_shadow_accel_t(const SceneDev& sc, ShadowQueue sq, const uint32_t* s_count, uint32_t* work, float4* Lo, uint32_t* defer_list,
+                                  uint32_t* defer_count, unsigned long long* counts, int blocks, int threads, cudaStream_t st) {
     if (sc.w8_nodes) {
         W8Counts c;
         c.node_visits = counts ? counts + 2 : nullptr;
         c.tri_tests = counts ? counts + 1 : nullptr;
-#define EZRT_LAUNCH_W8(C, I) k_shadow_w8<C, I><<<blocks, threads, w8_smem_for(k_shadow_w8<C, I>, sc), st>>>(sc, sq, s_count, work, Lo, defer_list, defer_count, c)
+#define EZRT_LAUNCH_W8(C, I) k_shadow_w8<C, I, B><<<blocks, threads, w8_smem_for(k_shadow_w8<C, I, B>, sc), st>>>(sc, sq, s_count, work, Lo, defer_list, defer_count, c)
         if (sc.acc_tri_indexed) { if (counts) EZRT_LAUNCH_W8(true, true); else EZRT_LAUNCH_W8(false, true); }
         else { if (counts) EZRT_LAUNCH_W8(true, false); else EZRT_LAUNCH_W8(false, false); }
 #undef EZRT_LAUNCH_W8
@@ -1224,30 +1239,34 @@ void launch_shadow_accel(const SceneDev& sc, ShadowQueue sq, const uint32_t* s_c
         W8Counts c;
         c.node_visits = counts ? (sc.acc_wide_q16 ? counts + 2 : counts) : nullptr;
         c.tri_tests = counts ? counts + 1 : nullptr;
-        if (sc.acc_wide_q16) {
-            if (counts) k_shadow_accel<true, true><<<blocks, threads, smem_for(k_shadow_accel<true, true>, 0), st>>>(sc, sq, s_count, work, Lo, defer_list, defer_count, c);
-            else k_shadow_accel<false, true><<<blocks, threads, smem_for(k_shadow_accel<false, true>, 0), st>>>(sc, sq, s_count, work, Lo, defer_list, defer_count, c);
-        } else {
-            if (counts) k_shadow_accel<true, false><<<blocks, threads, smem_for(k_shadow_accel<true, false>, 0), st>>>(sc, sq, s_count, work, Lo, defer_list, defer_count, c);
-            else k_shadow_accel<false, false><<<blocks, threads, smem_for(k_shadow_accel<false, false>, 0), st>>>(sc, sq, s_count, work, Lo, defer_list, defer_count, c);
-        }
+#define EZRT_LAUNCH_W4(C, Q) k_shadow_accel<C, Q, B><<<blocks, threads, smem_for(k_shadow_accel<C, Q, B>, 0), st>>>(sc, sq, s_count, work, Lo, defer_list, defer_count, c)
+        if (sc.acc_wide_q16) { if (counts) EZRT_LAUNCH_W4(true, true); else EZRT_LAUNCH_W4(false, true); }
+        else { if (counts) EZRT_LAUNCH_W4(true, false); else EZRT_LAUNCH_W4(false, false); }
+#undef EZRT_LAUNCH_W4
     }
-    launch_shadow(sc, true, sq, defer_count, defer_work, Lo, defer_list, std::min<uint32_t>(n_max, 65536u), n_sms, st);
+}
+void launch_shadow_accel(const SceneDev& sc, ShadowQueue sq, const uint32_t* s_count, uint32_t* work, float4* Lo, uint32_t* defer_list,
+                         uint32_t* defer_count, uint32_t* defer_work, uint32_t n_max, int n_sms, unsigned long long* counts, cudaStream_t st, bool bounded) {
+    const int threads = extend_threads(), blocks = persistent_blocks(n_max, n_sms);
+    if (bounded) launch_shadow_accel_t<true>(sc, sq, s_count, work, Lo, defer_list, defer_count, counts, blocks, threads, st);
+    else launch_shadow_accel_t<false>(sc, sq, s_count, work, Lo, defer_list, defer_count, counts, blocks, threads, st);
+    launch_shadow(sc, true, sq, defer_count, defer_work, Lo, defer_list, std::min<uint32_t>(n_max, 65536u), n_sms, st, bounded);
 }
 void launch_shade(const SceneDev& sc, const RenderDev& rd, const TileDev* tiles, int bounce, uint32_t batch_first_frame,
                   PathQueue qin, const uint32_t* in_count, PathQueue qout, uint32_t* out_count, ShadowQueue sq,
                   uint32_t* s_count, float4* Lo, float4* Le, uint32_t n_max, uint32_t n_fused, uint32_t n_frames, int n_sms, cudaStream_t st,
-                  float4* aov_rec) {
+                  float4* aov_rec, LightsDev lights) {
     int blocks = std::min(div_up(n_max, 128), n_sms * 4 * EZRT_SHADE_MIN_BLOCKS);
     if (blocks < 1) blocks = 1;
 #define EZRT_LAUNCH_SHADE(M)                                                                                                                  \
     if (aov_rec) k_shade<M, false, true><<<blocks, 128, 0, st>>>(sc, rd, tiles, bounce, batch_first_frame, qin, in_count, qout, out_count, sq, s_count, Lo, Le, \
-                                                                 n_fused, n_frames, nullptr, nullptr, aov_rec);                              \
-    else k_shade<M, false><<<blocks, 128, 0, st>>>(sc, rd, tiles, bounce, batch_first_frame, qin, in_count, qout, out_count, sq, s_count, Lo, Le, n_fused, n_frames, nullptr, nullptr, nullptr)
+                                                                 n_fused, n_frames, nullptr, nullptr, aov_rec, lights);                      \
+    else k_shade<M, false><<<blocks, 128, 0, st>>>(sc, rd, tiles, bounce, batch_first_frame, qin, in_count, qout, out_count, sq, s_count, Lo, Le, n_fused, n_frames, nullptr, nullptr, nullptr, lights)
     switch (rd.mode) {
         case EZRT_MODE_DIFFUSE_P3: EZRT_LAUNCH_SHADE(EZRT_MODE_DIFFUSE_P3); break;
         case EZRT_MODE_DISNEY_ANISO_P4: EZRT_LAUNCH_SHADE(EZRT_MODE_DISNEY_ANISO_P4); break;
         case EZRT_MODE_DISNEY_SOBOL_P5: EZRT_LAUNCH_SHADE(EZRT_MODE_DISNEY_SOBOL_P5); break;
+        case EZRT_MODE_DISNEY_LIGHTS: EZRT_LAUNCH_SHADE(EZRT_MODE_DISNEY_LIGHTS); break;
         default: EZRT_LAUNCH_SHADE(EZRT_MODE_DISNEY_IS_MIS_P5); break;
     }
 #undef EZRT_LAUNCH_SHADE
@@ -1258,24 +1277,81 @@ void launch_shade(const SceneDev& sc, const RenderDev& rd, const TileDev* tiles,
 void launch_deferred_lane(const SceneDev& sc, const RenderDev& rd, const TileDev* tiles, int bounce, uint32_t batch_first_frame, PathQueue qin,
                           const uint32_t* defer_list, const uint32_t* defer_count, uint32_t* defer_work, float2* side_hit, PathQueue qout,
                           uint32_t* out_count, ShadowQueue sq, uint32_t* s_count, float4* Lo, float4* Le, uint32_t n_fused, uint32_t n_frames,
-                          int n_sms, cudaStream_t st, float4* aov_rec) {
+                          int n_sms, cudaStream_t st, float4* aov_rec, LightsDev lights) {
     launch_extend(sc, true, false, qin, defer_count, defer_work, defer_list, 1, EZRT_SIDE_CAP, n_sms, st, side_hit, 1);
     const int blocks = 8;
 #define EZRT_LAUNCH_SHADE(M)                                                                                                                  \
     if (aov_rec) k_shade<M, true, true><<<blocks, 128, 0, st>>>(sc, rd, tiles, bounce, batch_first_frame, qin, defer_count, qout, out_count, sq, s_count, Lo, \
-                                                                Le, n_fused, n_frames, defer_list, side_hit, aov_rec);                         \
-    else k_shade<M, true><<<blocks, 128, 0, st>>>(sc, rd, tiles, bounce, batch_first_frame, qin, defer_count, qout, out_count, sq, s_count, Lo, Le, n_fused, n_frames, defer_list, side_hit, nullptr)
+                                                                Le, n_fused, n_frames, defer_list, side_hit, aov_rec, lights);                 \
+    else k_shade<M, true><<<blocks, 128, 0, st>>>(sc, rd, tiles, bounce, batch_first_frame, qin, defer_count, qout, out_count, sq, s_count, Lo, Le, n_fused, n_frames, defer_list, side_hit, nullptr, lights)
     switch (rd.mode) {
         case EZRT_MODE_DIFFUSE_P3: EZRT_LAUNCH_SHADE(EZRT_MODE_DIFFUSE_P3); break;
         case EZRT_MODE_DISNEY_ANISO_P4: EZRT_LAUNCH_SHADE(EZRT_MODE_DISNEY_ANISO_P4); break;
         case EZRT_MODE_DISNEY_SOBOL_P5: EZRT_LAUNCH_SHADE(EZRT_MODE_DISNEY_SOBOL_P5); break;
+        case EZRT_MODE_DISNEY_LIGHTS: EZRT_LAUNCH_SHADE(EZRT_MODE_DISNEY_LIGHTS); break;
         default: EZRT_LAUNCH_SHADE(EZRT_MODE_DISNEY_IS_MIS_P5); break;
     }
 #undef EZRT_LAUNCH_SHADE
 }
 void launch_nee(const SceneDev& sc, const RenderDev& rd, ShadowQueue sq, const uint32_t* s_count, float4* Lo, uint32_t n_max, int n_sms, cudaStream_t st) {
     const int blocks = std::max(1, std::min(div_up(n_max, 512), n_sms * 8));
-    k_nee<<<blocks, 128, 0, st>>>(sc, rd, sq, s_count, Lo);
+    if (rd.mode == EZRT_MODE_DISNEY_LIGHTS) k_nee<EZRT_MODE_DISNEY_LIGHTS><<<blocks, 128, 0, st>>>(sc, rd, sq, s_count, Lo);
+    else k_nee<EZRT_MODE_DISNEY_IS_MIS_P5><<<blocks, 128, 0, st>>>(sc, rd, sq, s_count, Lo);
+}
+
+// ------------------------------------------------------------------------------------------
+// light table of the light sampling mode (ezrt_math.h, DESIGN.md section 10): the weight of every triangle in the caller's
+// order, the lights kept in that order, then their records.  One-off, at the first render in that mode.
+// ------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256) k_light_weights(SceneDev sc, float* __restrict__ w) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= sc.n_triangles) return;
+    vec3 p1, p2, p3;
+    tri_vertices(sc, i, false, p1, p2, p3);
+    w[i] = ez_light_weight(p1, p2, p3, load_emissive(sc, tri_material(sc, i)));
+}
+// stable compaction in one block: chunks of blockDim.x triangles in order, each ranked by thread index (block_append on a
+// shared-memory counter), as k_adaptive_check's tail
+__global__ void __launch_bounds__(1024) k_light_compact(const float* __restrict__ w, int n, int32_t* __restrict__ idx_out, float* __restrict__ w_out,
+                                                        int32_t* __restrict__ count) {
+    __shared__ uint32_t s_scan[34];
+    __shared__ uint32_t s_count;
+    if (threadIdx.x == 0) s_count = 0u;
+    __syncthreads();
+    for (int i0 = 0; i0 < n; i0 += blockDim.x) {
+        const int i = i0 + threadIdx.x;
+        const float wi = (i < n) ? w[i] : 0.0f;
+        const bool keep = (i < n) && ez_is_light(wi);
+        const uint32_t pos = block_append(keep, &s_count, s_scan);
+        if (keep) { idx_out[pos] = i; w_out[pos] = wi; }
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) *count = (int32_t)s_count;
+}
+__global__ void __launch_bounds__(256) k_light_records(SceneDev sc, const int32_t* __restrict__ idx, int n, float4* __restrict__ rec) {
+    const int k = blockIdx.x * blockDim.x + threadIdx.x;
+    if (k >= n) return;
+    const int tri = idx[k];
+    vec3 p1, p2, p3;
+    tri_vertices(sc, tri, false, p1, p2, p3);
+    const int mat = tri_material(sc, tri);
+    const vec3 N = f4xyz(ldg4(tri_geo_rec(sc, tri, false)));
+    const int acc = sc.ref_to_acc ? (int)sc.ref_to_acc[tri] : tri;
+    rec[4 * k] = make_float4(p1.x, p1.y, p1.z, __int_as_float(mat));
+    rec[4 * k + 1] = make_float4(p2.x, p2.y, p2.z, __int_as_float(tri));
+    rec[4 * k + 2] = make_float4(p3.x, p3.y, p3.z, __int_as_float(acc));
+    rec[4 * k + 3] = make_float4(N.x, N.y, N.z, ez_luminance(load_emissive(sc, mat)));
+}
+void launch_light_weights(const SceneDev& sc, float* w, cudaStream_t st) {
+    if (sc.n_triangles <= 0) return;
+    k_light_weights<<<div_up(sc.n_triangles, 256), 256, 0, st>>>(sc, w);
+}
+void launch_light_compact(const float* w, int n, int32_t* idx_out, float* w_out, int32_t* count, cudaStream_t st) {
+    k_light_compact<<<1, 1024, 0, st>>>(w, n, idx_out, w_out, count);
+}
+void launch_light_records(const SceneDev& sc, const int32_t* idx, int n, float4* rec, cudaStream_t st) {
+    if (n <= 0) return;
+    k_light_records<<<div_up(n, 256), 256, 0, st>>>(sc, idx, n, rec);
 }
 void launch_blend(const RenderDev& rd, const TileDev* tiles, int nf, uint32_t batch_first_frame, const float4* Lo,
                   const float4* Le, float* fb, cudaStream_t st) {

@@ -28,22 +28,30 @@ void launch_extend_accel(const SceneDev& sc, PathQueue q, const uint32_t* q_coun
 void launch_ray_sort(const SceneDev& sc, PathQueue q, const uint32_t* q_count, uint32_t* keys, uint32_t* bins, uint32_t* perm,
                      uint32_t n_max, int n_sms, cudaStream_t st);
 void launch_shadow(const SceneDev& sc, bool prune, ShadowQueue sq, const uint32_t* s_count, uint32_t* work, float4* Lo,
-                   const uint32_t* perm, uint32_t n_max, int n_sms, cudaStream_t st);
+                   const uint32_t* perm, uint32_t n_max, int n_sms, cudaStream_t st, bool bounded = false);
+// bounded (light sampling mode): shadow ray j looks for occluders strictly before sq.nrm[j].w only
 void launch_shadow_accel(const SceneDev& sc, ShadowQueue sq, const uint32_t* s_count, uint32_t* work, float4* Lo, uint32_t* defer_list,
-                         uint32_t* defer_count, uint32_t* defer_work, uint32_t n_max, int n_sms, unsigned long long* counts, cudaStream_t st);
+                         uint32_t* defer_count, uint32_t* defer_work, uint32_t n_max, int n_sms, unsigned long long* counts, cudaStream_t st,
+                         bool bounded = false);
 void launch_shade(const SceneDev& sc, const RenderDev& rd, const TileDev* tiles, int bounce, uint32_t batch_first_frame,
                   PathQueue qin, const uint32_t* in_count, PathQueue qout, uint32_t* out_count, ShadowQueue sq,
                   uint32_t* s_count, float4* Lo, float4* Le, uint32_t n_max, uint32_t n_fused, uint32_t n_frames, int n_sms, cudaStream_t st,
-                  float4* aov_rec = nullptr);   // aov_rec: feature-buffer render, bounce 0 writes the first-hit records (k_shade<.., AOV>)
+                  float4* aov_rec = nullptr,   // aov_rec: feature-buffer render, bounce 0 writes the first-hit records (k_shade<.., AOV>)
+                  LightsDev lights = LightsDev{});   // the light table (light sampling mode)
 void launch_extend_camera(const SceneDev& sc, const RenderDev& rd, const TileDev* tiles, uint32_t batch_first_frame, uint32_t n_slots, uint32_t n_frames, PathQueue q,
                           uint32_t* work, uint32_t* defer_list, uint32_t* defer_count, uint32_t* defer_work, int n_sms, unsigned long long* counts,
                           cudaStream_t st, int exact_gate = 0);
 void launch_deferred_lane(const SceneDev& sc, const RenderDev& rd, const TileDev* tiles, int bounce, uint32_t batch_first_frame, PathQueue qin,
                           const uint32_t* defer_list, const uint32_t* defer_count, uint32_t* defer_work, float2* side_hit, PathQueue qout,
                           uint32_t* out_count, ShadowQueue sq, uint32_t* s_count, float4* Lo, float4* Le, uint32_t n_fused, uint32_t n_frames,
-                          int n_sms, cudaStream_t st, float4* aov_rec = nullptr);
+                          int n_sms, cudaStream_t st, float4* aov_rec = nullptr, LightsDev lights = LightsDev{});
 // after a shadow pass (accel or exact, including the exact pass over deferred shadow rays): contributions of the unoccluded light samples
 void launch_nee(const SceneDev& sc, const RenderDev& rd, ShadowQueue sq, const uint32_t* s_count, float4* Lo, uint32_t n_max, int n_sms, cudaStream_t st);
+// light table of the light sampling mode: every triangle's weight (w: n_triangles floats) -> the lights in triangle order
+// (idx_out, w_out: n floats each; *count = K) -> their 64-byte records (rec: 4 K float4)
+void launch_light_weights(const SceneDev& sc, float* w, cudaStream_t st);
+void launch_light_compact(const float* w, int n, int32_t* idx_out, float* w_out, int32_t* count, cudaStream_t st);
+void launch_light_records(const SceneDev& sc, const int32_t* idx, int n, float4* rec, cudaStream_t st);
 void launch_blend(const RenderDev& rd, const TileDev* tiles, int nf, uint32_t batch_first_frame, const float4* Lo,
                   const float4* Le, float* fb, cudaStream_t st);
 // adaptive sampling: k_blend<true> also keeps the running mean of the squared sample luminance and the per-pixel frame count

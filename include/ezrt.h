@@ -45,12 +45,18 @@ typedef enum ezrt_status {
     EZRT_ERR_NOMEM = -5
 } ezrt_status;
 
-/* Integrator modes = the four per-pixel loops the reference ships (SURVEY.md 8a). */
+/* Integrator modes: the four per-pixel loops the reference ships (SURVEY.md 8a), and mode 4, which adds light sampling
+ * on the scene's emissive triangles to mode 3's BRDF sampling. */
 typedef enum ezrt_mode {
     EZRT_MODE_DIFFUSE_P3 = 0,      /* P3/fsh:376-446  diffuse, uniform hemisphere, wang-hash   */
     EZRT_MODE_DISNEY_ANISO_P4 = 1, /* P4/fsh:478-550  anisotropic Disney, uniform hemisphere   */
     EZRT_MODE_DISNEY_SOBOL_P5 = 2, /* P5/fsh:762-807  Disney + Sobol/CP rotation               */
-    EZRT_MODE_DISNEY_IS_MIS_P5 = 3 /* P5/fsh:810-890  BRDF + HDR importance sampling, MIS      */
+    EZRT_MODE_DISNEY_IS_MIS_P5 = 3, /* P5/fsh:810-890  BRDF + HDR importance sampling, MIS     */
+    /* BRDF importance sampling + one light sample per bounce on the emissive triangles, balance-heuristic MIS (ezrt_math.h,
+     * DESIGN.md section 10).  With or without an HDR map: the environment is reached by BRDF samples only, at weight 1.
+     * Wavefront pipeline only.  The first render of a scene in this mode builds its light table (ezrt_scene_lights), which
+     * synchronises the render's stream once. */
+    EZRT_MODE_DISNEY_LIGHTS = 4
 } ezrt_mode;
 
 /* BVH traversal policy.  All three return bit-identical hits (tests assert it).
@@ -240,6 +246,20 @@ int ezrt_partition_scatter_host(const float* compact, float* full, int width, in
 int ezrt_trace_rays(ezrt_scene* scene, int n, const float* origins, const float* dirs, int traverse,
                     int any_hit, int p3_normal_fudge, int32_t* out_hit, float* out_distance,
                     int32_t* out_triangle, int32_t* out_inside, float* out_point, float* out_normal);
+
+/* The light table of EZRT_MODE_DISNEY_LIGHTS (ezrt_math.h; built here if no render in that mode has built it yet, which
+ * synchronises the device).  Returns K, the number of lights, or a negative status; writes min(K, cap) entries:
+ * tri_out = the lights' triangle indices (caller's order), cdf_out = their cumulative distribution (the last entry 1),
+ * and *total_out = W, the float64 sum of the weights.  Any output may be NULL. */
+int ezrt_scene_lights(ezrt_scene* scene, int cap, int32_t* tri_out, float* cdf_out, double* total_out);
+
+/* Bounded occlusion of n rays (host arrays: origins, dirs n x 3, tmax n), for parity tests beside ezrt_trace_rays: runs the
+ * shadow pass of the render for the traversal policy `traverse` -- the accel kernels with the exact pass over the rays they
+ * defer, or the exact kernel -- and writes out_lit[i] = 1 iff no triangle the shader's hitBVH would test is accepted
+ * with t < tmax[i].  When every tmax is +inf, mode 3's unbounded shadow kernels run instead (t < 114514, the shader's INF).
+ * Not a general query API: it allocates and synchronises per call. */
+int ezrt_occluded_rays(ezrt_scene* scene, int n, const float* origins, const float* dirs, const float* tmax, int traverse,
+                       int32_t* out_lit);
 
 /* Evaluate the BRDF functions on the device for n (V,N,L,material) tuples: which = 0
  * BRDF_Evaluate (P5/fsh:500-549), 1 BRDF_Evaluate aniso (P4/fsh:412-473), 2 BRDF_Pdf

@@ -348,4 +348,49 @@ EZ_HD float ez_atrous_weight(float h, float s_dist, ez_vec3 n_p, ez_vec3 n_q, fl
     return (((h * w_n) * w_z) * w_l) * w_a;
 }
 
+/* ------------------------------------------------------------------ emissive-triangle light sampling (DESIGN.md section 10)
+ * Mode EZRT_MODE_DISNEY_LIGHTS.  Light table: light k is the k-th triangle (caller's order) whose weight
+ * w = ez_light_weight(p1, p2, p3, emissive) passes ez_is_light; W = sum of the weights in float64 in triangle order,
+ * cdf_k = (float)(S_k / W) with the last entry exactly 1.0f, W_f = (float)W.
+ * Per shading point of a bounce b < max_bounce, after mode 3's emission accounting:
+ *   r_sel, r_1, r_2 = three rand01 draws (in place of mode 3's two SampleHdr draws; drawn even when there is no light), then
+ *   mode 3's Sobol pair with CP rotation, xi_3 = rand01, L = SampleBRDF(...).
+ *   k = the first entry with r_sel < cdf_k;  Q = ez_triangle_point(p1_k, p2_k, p3_k, r_1, r_2)
+ *   D = Q - P, dist = sqrt(dot(D, D)), L_l = ez_normalize(D), cos_l = |dot(N_k, L_l)| (N_k: the light's geometric normal)
+ *   pdf_l = ez_light_pdf(ez_luminance(E_k), W_f, dist, cos_l)
+ *   no sample if k is the hit triangle, dot(N, L_l) <= 0, cos_l == 0 or dist == 0; else a shadow ray P -> L_l with
+ *   tmax = ez_light_tmax(dist), lit iff no triangle is accepted with t < tmax (strict), and if lit
+ *   Lo += history * mis(pdf_l, BRDF_Pdf(V, N, L_l)) * E_k * f_r(V, N, L_l) * dot(N, L_l) / pdf_l   (left to right)
+ * A BRDF sample's emission hit at bounce >= 1 on a light T weighs mis(p.pdf, ez_light_pdf(ez_luminance(E_T), W_f, t, |dot(N_T, d)|));
+ * every other emission hit weighs 1.  mis = the balance heuristic mis_mix_weight (P5/fsh:754-757). */
+/* area = 0.5 * length(cross(p2 - p1, p3 - p1)) */
+EZ_HD float ez_triangle_area(ez_vec3 p1, ez_vec3 p2, ez_vec3 p3) {
+    const ez_vec3 c = ez_cross(ez_sub(p2, p1), ez_sub(p3, p1));
+    return 0.5f * EZ_SQRT(ez_dot(c, c));
+}
+EZ_HD float ez_light_weight(ez_vec3 p1, ez_vec3 p2, ez_vec3 p3, ez_vec3 emissive) { return ez_triangle_area(p1, p2, p3) * ez_luminance(emissive); }
+/* a light: finite weight > 0 (zero-area, black, negative and NaN emitters are not) */
+EZ_HD int ez_is_light(float w) { return ez_finite(w) && w > 0.0f; }
+/* uniform point of the triangle: s = sqrt(r_1), b0 = 1 - s, b1 = r_2 * s, Q = p1 b0 + p2 b1 + p3 (1 - b0 - b1) */
+EZ_HD ez_vec3 ez_triangle_point(ez_vec3 p1, ez_vec3 p2, ez_vec3 p3, float r_1, float r_2) {
+    const float s = EZ_SQRT(r_1);
+    const float b0 = 1.0f - s, b1 = r_2 * s;
+    const float b2 = (1.0f - b0) - b1;
+    return ez_add(ez_add(ez_scale(p1, b0), ez_scale(p2, b1)), ez_scale(p3, b2));
+}
+/* solid-angle pdf of a point at distance dist seen at cosine cos_l: ((lum / W_f) * (dist * dist)) / cos_l */
+EZ_HD float ez_light_pdf(float lum, float W_f, float dist, float cos_l) { return EZ_DIV(EZ_DIV(lum, W_f) * (dist * dist), cos_l); }
+/* the shadow ray's bound: dist * (1 - 2^-10), so that the light's own triangle and its coplanar neighbours do not occlude */
+EZ_HD float ez_light_tmax(float dist) { return dist * 0.9990234375f; }
+/* index of the selected light: the first k with r < cdf[k] (cdf non-decreasing, cdf[n - 1] = 1 > r) */
+EZ_HD int ez_light_select(const float* cdf, int n, float r) {
+    int lo = 0, hi = n - 1;
+    while (lo < hi) {
+        const int mid = (lo + hi) >> 1;
+        if (r < cdf[mid]) hi = mid;
+        else lo = mid + 1;
+    }
+    return lo;
+}
+
 #endif /* EZRT_MATH_H */
