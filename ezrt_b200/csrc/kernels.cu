@@ -759,13 +759,16 @@ __global__ void __launch_bounds__(256) k_blend(RenderDev rd, const TileDev* __re
     if (ix >= t.w || iy >= t.h) return;
     const size_t pix = fb_index(rd, t, ix, iy);
     size_t idx = pix * (size_t)rd.out_channels;
-    vec3 acc = (batch_first_frame == 0u) ? splat3(0.0f) : ez_v3(fb[idx], fb[idx + 1], fb[idx + 2]);
+    // only the first batch of a render from frame 0 starts from nothing: a later batch that starts at frame 0 because the
+    // uint32 frame counter wrapped blends onto the frames before it, as every display() call does
+    const bool fresh = (batch_first_frame == 0u) && (rd.first_frame == 0u);
+    vec3 acc = fresh ? splat3(0.0f) : ez_v3(fb[idx], fb[idx + 1], fb[idx + 2]);
     float m2 = 0.0f;
-    if (ADAPTIVE && batch_first_frame != 0u) m2 = luma2[pix];
+    if (ADAPTIVE && !fresh) m2 = luma2[pix];
     float feat[8];
     if (AOV) {
 #pragma unroll
-        for (int k = 0; k < 8; k++) feat[k] = (batch_first_frame == 0u) ? 0.0f : aov[pix * 8 + k];
+        for (int k = 0; k < 8; k++) feat[k] = fresh ? 0.0f : aov[pix * 8 + k];
     }
     for (int f = 0; f < nf; f++) {
         float4 lo = Lo[(size_t)f * per_frame + r];

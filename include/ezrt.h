@@ -85,6 +85,10 @@ typedef struct ezrt_render_params {
     int32_t width, height;   /* uniform width,height  (P5/main.cpp:922-923)                  */
     int32_t spp;             /* number of consecutive display() calls to perform             */
     uint32_t first_frame;    /* frameCounter of the first call (P5/main.cpp:719); 0 = fresh  */
+                             /* Frames count in the reference's uint arithmetic, modulo 2^32: frame 0xFFFFFFFF is
+                              * blended with weight 1/float(frame + 1u) = 1/0 = +inf, which makes every blended
+                              * value NaN (colour, features, luma2; alpha stays 1), and the frames after it (0, 1, ...)
+                              * blend into NaN and leave it NaN; its Sobol index frame + 1 is 0. */
     int32_t max_bounce;      /* literal in main(): P5/fsh:935 (2), P4/fsh:540 (4), P3 (2)    */
     int32_t mode;            /* ezrt_mode                                                    */
     float eye[3];            /* uniform eye           (P5/main.cpp:710-711, :717)            */
