@@ -76,6 +76,7 @@ SIGNATURES = {
     "ezrt_trace_rays": (C.c_int, [C.c_void_p, C.c_int, c_float_p, c_float_p, C.c_int, C.c_int, C.c_int, c_int32_p, c_float_p,
                                   c_int32_p, c_int32_p, c_float_p, c_float_p]),
     "ezrt_scene_lights": (C.c_int, [C.c_void_p, C.c_int, c_int32_p, c_float_p, C.POINTER(C.c_double)]),
+    "ezrt_scene_env_light": (C.c_int, [C.c_void_p, c_float_p, c_float_p, c_float_p, C.POINTER(C.c_double)]),
     "ezrt_occluded_rays": (C.c_int, [C.c_void_p, C.c_int, c_float_p, c_float_p, c_float_p, C.c_int, c_int32_p]),
     "ezrt_eval_brdf": (C.c_int, [C.c_int, C.c_int, C.c_int, c_float_p, c_float_p, c_float_p, c_float_p, c_float_p, c_float_p]),
     "ezrt_eval_math": (C.c_int, [C.c_int, C.c_int, C.c_int, c_float_p, c_float_p, c_float_p]),

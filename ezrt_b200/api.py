@@ -19,6 +19,8 @@ MODE_DISNEY_ANISO_P4 = 1
 MODE_DISNEY_SOBOL_P5 = 2
 MODE_DISNEY_IS_MIS_P5 = 3
 MODE_DISNEY_LIGHTS = 4   # BRDF sampling + light sampling on the emissive triangles, MIS (DESIGN.md section 10)
+PARAM_ACCUMULATE = 1   # ezrt_render_params.reserved[0] flags (include/ezrt.h)
+PARAM_ENV_LIGHT = 2
 MODES = {"diffuse_p3": 0, "disney_aniso_p4": 1, "disney_sobol_p5": 2, "disney_is_mis_p5": 3, "disney_lights": 4}
 
 TRAVERSE_ACCEL = 0
@@ -213,6 +215,7 @@ class RenderConfig:
     frames_per_batch: int = 0
     profile: int = 0
     accumulate: bool = False   # EZRT_PARAM_ACCUMULATE: counters / kernel times continue from the previous render
+    env_light: bool = False    # EZRT_PARAM_ENV_LIGHT (MODE_DISNEY_LIGHTS only): the HDR map is one more light (DESIGN.md section 11)
 
     def to_struct(self):
         p = RenderParams()
@@ -224,7 +227,7 @@ class RenderConfig:
         p.traverse, p.pipeline, p.out_channels = int(self.traverse), int(self.pipeline), int(self.out_channels)
         p.part_rank, p.part_count, p.frames_per_batch = int(self.part_rank), int(self.part_count), int(self.frames_per_batch)
         p.profile = int(self.profile)
-        p.reserved[0] = 1 if self.accumulate else 0
+        p.reserved[0] = (PARAM_ACCUMULATE if self.accumulate else 0) | (PARAM_ENV_LIGHT if self.env_light else 0)
         return p
 
 
@@ -406,6 +409,18 @@ class Scene:
         total = C.c_double(0.0)
         check(lib.ezrt_scene_lights(self._h, k, tri.ctypes.data_as(_lib.c_int32_p), _fp(cdf), C.byref(total)))
         return tri, cdf, total.value
+
+    def env_light_table(self):
+        """The environment table of RenderConfig.env_light (ezrt_scene_env_light; built at the first call or flagged render):
+        (row_cdf float32 [H], col_cdf float32 [H, W], texel_pdf float32 [H, W], T = float64 sum of the texel weights), or None
+        when the scene has no table (no map, or a black one)."""
+        total = C.c_double(0.0)
+        if not check(lib.ezrt_scene_env_light(self._h, None, None, None, C.byref(total))):
+            return None
+        h, w = self.hdr.shape[0], self.hdr.shape[1]
+        row, col, pdf = np.zeros(h, np.float32), np.zeros((h, w), np.float32), np.zeros((h, w), np.float32)
+        check(lib.ezrt_scene_env_light(self._h, _fp(row), _fp(col), _fp(pdf), None))
+        return row, col, pdf, total.value
 
     def occluded_rays(self, origins, dirs, tmax, traverse=TRAVERSE_ACCEL):
         """ezrt_occluded_rays: 1 where nothing is accepted strictly before tmax along the ray (the render's shadow pass)."""

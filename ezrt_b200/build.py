@@ -178,6 +178,24 @@ def build_oracle_lights(force=False):
     return ORACLE_LIGHTS_SO
 
 
+ORACLE_ENV_LIGHT_SO = os.path.join(ROOT, "build", "libezrt_oracle_env_light.so")
+
+
+def build_oracle_env_light(force=False):
+    """build/libezrt_oracle_env_light.so: tests/oracle_env_light.cpp, the CPU restatement of the environment map as a light
+    (table, sampler, flagged integrator) over the light sampling mode's restatement (test infrastructure, loaded only by
+    tests/oracle_env_light.py)."""
+    src = os.path.join(ROOT, "tests", "oracle_env_light.cpp")
+    deps = [src, os.path.join(ROOT, "tests", "oracle_lights.cpp"), os.path.join(ROOT, "oracle", "ezrt_oracle.cpp")] + \
+        [os.path.join(INCLUDE, f) for f in os.listdir(INCLUDE)]
+    if force or _newer(ORACLE_ENV_LIGHT_SO, deps):
+        os.makedirs(os.path.dirname(ORACLE_ENV_LIGHT_SO), exist_ok=True)
+        tmp = ORACLE_ENV_LIGHT_SO + ".tmp%d" % os.getpid()
+        _run(["g++"] + HOST_FLAGS + ["-fopenmp", "-Wno-misleading-indentation", "-shared", "-I", INCLUDE, src, "-o", tmp])
+        os.replace(tmp, ORACLE_ENV_LIGHT_SO)
+    return ORACLE_ENV_LIGHT_SO
+
+
 def build_reference_hdrloader(force=False):
     return _oracle_recipes().build_reference_hdrloader(force)
 
@@ -239,6 +257,7 @@ def build_all(force=False, verbose=False):
     build_oracle_adaptive(force=force)
     build_oracle_aov(force=force)
     build_oracle_lights(force=force)
+    build_oracle_env_light(force=force)
     build_example(force=force)
     build_reference_hdrloader(force=force)
     build_reference_shaders(force=force)

@@ -99,6 +99,11 @@ struct ezrt_scene {
     std::vector<int32_t> light_tri;   // the lights' triangles (caller's order)
     std::vector<float> light_cdf;
     double light_total = 0.0;         // W, the float64 sum of the weights
+    // the environment map's light table (build_env, at the first render with EZRT_PARAM_ENV_LIGHT): row cdf | column cdf | texel pdf
+    DeviceBuffer env_buf;
+    bool env_built = false;
+    EnvDev env{};                     // row_cdf null: the scene has no table (no map, or no texel of positive weight)
+    double env_total = 0.0;           // T, the float64 sum of the texel weights
     void* hot_base = nullptr;   // accel nodes | geometry (| vertices) | shading records (L2 persisting window)
     size_t hot_bytes = 0;
     size_t l2_persist_bytes = 0;
@@ -178,6 +183,8 @@ int validate_params(const ezrt_scene* scene, const ezrt_render_params* p) {
     if (p->mode < 0 || p->mode > EZRT_MODE_DISNEY_LIGHTS) return ezrt_set_error(EZRT_ERR_INVALID, "render: unknown mode %d", p->mode);
     if (p->mode == EZRT_MODE_DISNEY_LIGHTS && p->pipeline == EZRT_PIPELINE_MEGAKERNEL)
         return ezrt_set_error(EZRT_ERR_INVALID, "render: the light sampling mode runs on the wavefront pipeline only");
+    if ((p->reserved[0] & EZRT_PARAM_ENV_LIGHT) && p->mode != EZRT_MODE_DISNEY_LIGHTS)
+        return ezrt_set_error(EZRT_ERR_INVALID, "render: EZRT_PARAM_ENV_LIGHT needs the light sampling mode (got mode %d)", p->mode);
     if (p->max_bounce < 0 || p->max_bounce > 64) return ezrt_set_error(EZRT_ERR_INVALID, "render: max_bounce out of range");
     if (p->out_channels != 3 && p->out_channels != 4) return ezrt_set_error(EZRT_ERR_INVALID, "render: out_channels must be 3 or 4");
     if (p->part_count < 1 || p->part_rank < 0 || p->part_rank >= p->part_count)
@@ -295,6 +302,69 @@ int build_lights(ezrt_scene* s, cudaStream_t st) {
     s->light_cdf = cdf;
     s->light_total = W;
     s->lights_built = true;
+    return EZRT_OK;
+}
+
+// The environment map's light table (ezrt_math.h, DESIGN.md section 11), built once per scene on stream st from the scene's copy
+// of the map: every texel's weight on the device, the sums and cdfs in float64 on the host, the three arrays uploaded.
+// Synchronises st.  A scene without a map, or whose texels all weigh 0, has no table.
+int build_env(ezrt_scene* s, cudaStream_t st) {
+    if (s->env_built) return EZRT_OK;
+    const int W = s->dev.hdr_w, H = s->dev.hdr_h;
+    EnvDev env{};
+    double T = 0.0;
+    if (s->dev.hdr && W > 0 && H > 0) {
+        const size_t n = (size_t)W * H;
+        struct TmpBuffer : DeviceBuffer { ~TmpBuffer() { release(); } } tmp;
+        int rc = tmp.ensure(sizeof(float) * n);
+        if (rc) return rc;
+        launch_env_weights(s->dev, (float*)tmp.p, st);
+        std::vector<float> w(n);
+        CU_CHECK(cudaMemcpyAsync(w.data(), tmp.p, sizeof(float) * n, cudaMemcpyDeviceToHost, st));
+        CU_CHECK(cudaStreamSynchronize(st));
+        std::vector<double> R(H, 0.0);
+        for (int i = 0; i < H; i++) {
+            double r = 0.0;
+            for (int j = 0; j < W; j++) r += (double)w[(size_t)i * W + j];
+            R[i] = r;
+        }
+        for (int i = 0; i < H; i++) T += R[i];
+        if (std::isfinite(T) && T > 0.0) {
+            // one host array in the device layout: row cdf (H) | column cdf (H x W) | texel pdf (H x W)
+            std::vector<float> tab((size_t)H + 2 * n);
+            float* row_cdf = tab.data();
+            float* col_cdf = row_cdf + H;
+            float* texel_pdf = col_cdf + n;
+            double S = 0.0;
+            for (int i = 0; i < H; i++) {
+                S += R[i];
+                row_cdf[i] = (float)(S / T);
+                double c = 0.0;
+                for (int j = 0; j < W; j++) {
+                    const size_t k = (size_t)i * W + j;
+                    c += (double)w[k];
+                    col_cdf[k] = (R[i] > 0.0) ? (float)(c / R[i]) : 0.0f;
+                    texel_pdf[k] = (float)((double)w[k] / T);
+                }
+                if (R[i] > 0.0) col_cdf[(size_t)i * W + W - 1] = 1.0f;
+            }
+            row_cdf[H - 1] = 1.0f;
+            if ((rc = s->env_buf.ensure(sizeof(float) * tab.size()))) return rc;
+            CU_CHECK(cudaMemcpyAsync(s->env_buf.p, tab.data(), sizeof(float) * tab.size(), cudaMemcpyHostToDevice, st));
+            CU_CHECK(cudaStreamSynchronize(st));   // tab is pageable host memory
+            env.row_cdf = (const float*)s->env_buf.p;
+            env.col_cdf = env.row_cdf + H;
+            env.texel_pdf = env.col_cdf + n;
+            env.w = W;
+            env.h = H;
+        } else {
+            T = 0.0;
+        }
+    }
+    CU_CHECK(cudaGetLastError());
+    s->env = env;
+    s->env_total = T;
+    s->env_built = true;
     return EZRT_OK;
 }
 
@@ -803,7 +873,7 @@ int ezrt_scene_destroy(ezrt_scene* s) {
     s->lo_buf.release(); s->le_buf.release(); s->counters_buf.release(); s->totals_buf.release(); s->fb_buf.release(); s->sort_buf.release();
     s->adapt_buf.release(); s->adapt_maps_buf.release();
     s->aov_rec_buf.release(); s->aov_maps_buf.release(); s->denoise_buf.release(); s->denoise_io_buf.release();
-    s->lights_buf.release();
+    s->lights_buf.release(); s->env_buf.release();
     if (s->own_stream) cudaStreamDestroy(s->own_stream);
     if (s->copy_stream) cudaStreamDestroy(s->copy_stream);
     if (s->side_stream) cudaStreamDestroy(s->side_stream);
@@ -874,6 +944,16 @@ static int render_device_impl(ezrt_scene* s, const ezrt_render_params* p, float*
     const bool is_mode = (p->mode == EZRT_MODE_DISNEY_IS_MIS_P5) || lights_mode;
     if (lights_mode && (rc = build_lights(s, st))) return rc;
     const LightsDev lights = lights_mode ? s->lights : LightsDev{};
+    // EZRT_PARAM_ENV_LIGHT: the map is one more light when the scene has a table (P_env = 1/2 beside triangle lights, 1 without);
+    // without a table the render is mode 4's, and mode 4's kernels run
+    EnvDev env{};
+    if (lights_mode && (p->reserved[0] & EZRT_PARAM_ENV_LIGHT)) {
+        if ((rc = build_env(s, st))) return rc;
+        if (s->env.row_cdf) {
+            env = s->env;
+            env.p_env = (lights.n > 0) ? 0.5f : 1.0f;
+        }
+    }
     int F = p->frames_per_batch;
     if (F <= 0) F = (int)std::max<size_t>(1, ((size_t)32 << 20) / per_frame);  // ~32 M sample slots per batch (~7.5 GB of state):
                                                                               // long queues amortise the persistent kernels' ramp-up and tail
@@ -1022,13 +1102,13 @@ static int render_device_impl(ezrt_scene* s, const ezrt_render_params* p, float*
                 CU_CHECK(cudaEventRecord(s->ev_fork, st));
                 CU_CHECK(cudaStreamWaitEvent(s->side_stream, s->ev_fork, 0));
                 launch_deferred_lane(s->dev, rd, d_tiles, b, batch_first, qin, defer_list, &d_ext[b], &dw_ext[b], side_hit, qout, &q_count[b + 1], sq, &s_count[b],
-                                     Lo, Le, n_fused, (uint32_t)nf, s->n_sms, s->side_stream, b == 0 ? aov_rec : nullptr, lights);
+                                     Lo, Le, n_fused, (uint32_t)nf, s->n_sms, s->side_stream, b == 0 ? aov_rec : nullptr, lights, env);
                 CU_CHECK(cudaEventRecord(s->ev_join, s->side_stream));
                 s->launches += 2;
             }
             sp = s->span_begin(1, st);
             launch_shade(s->dev, rd, d_tiles, b, batch_first, qin, &q_count[b], qout, &q_count[b + 1], sq, &s_count[b], Lo, Le,
-                         n_slots, n_fused, (uint32_t)nf, s->n_sms, st, b == 0 ? aov_rec : nullptr, lights);
+                         n_slots, n_fused, (uint32_t)nf, s->n_sms, st, b == 0 ? aov_rec : nullptr, lights, env);
             if (lane) CU_CHECK(cudaStreamWaitEvent(st, s->ev_join, 0));   // ... while this k_shade shades all the others; join
             s->span_end(sp, st);
             s->launches += 2;
@@ -1042,7 +1122,7 @@ static int render_device_impl(ezrt_scene* s, const ezrt_render_params* p, float*
                 }
                 s->span_end(sp, st);
                 sp = s->span_begin(1, st);   // shading work: counted with k_shade
-                launch_nee(s->dev, rd, sq, &s_count[b], Lo, n_slots, s->n_sms, st);
+                launch_nee(s->dev, rd, sq, &s_count[b], Lo, n_slots, s->n_sms, st, env.row_cdf != nullptr);
                 s->span_end(sp, st);
                 s->launches += 2;
             }
@@ -1459,6 +1539,22 @@ int ezrt_scene_lights(ezrt_scene* s, int cap, int32_t* tri_out, float* cdf_out, 
     if (cdf_out) std::copy(s->light_cdf.begin(), s->light_cdf.begin() + m, cdf_out);
     if (total_out) *total_out = s->light_total;
     return K;
+}
+
+int ezrt_scene_env_light(ezrt_scene* s, float* row_cdf, float* col_cdf, float* texel_pdf, double* total) {
+    if (!s) return ezrt_set_error(EZRT_ERR_INVALID, "scene_env_light: null scene");
+    CU_CHECK(cudaSetDevice(s->device));
+    int rc = build_env(s, s->own_stream);
+    if (rc) return rc;
+    if (total) *total = s->env_total;
+    if (!s->env.row_cdf) return 0;
+    const size_t H = (size_t)s->env.h, n = (size_t)s->env.w * s->env.h;
+    cudaStream_t st = s->own_stream;
+    if (row_cdf) CU_CHECK(cudaMemcpyAsync(row_cdf, s->env.row_cdf, sizeof(float) * H, cudaMemcpyDeviceToHost, st));
+    if (col_cdf) CU_CHECK(cudaMemcpyAsync(col_cdf, s->env.col_cdf, sizeof(float) * n, cudaMemcpyDeviceToHost, st));
+    if (texel_pdf) CU_CHECK(cudaMemcpyAsync(texel_pdf, s->env.texel_pdf, sizeof(float) * n, cudaMemcpyDeviceToHost, st));
+    CU_CHECK(cudaStreamSynchronize(st));
+    return 1;
 }
 
 int ezrt_occluded_rays(ezrt_scene* s, int n, const float* origins, const float* dirs, const float* tmax, int traverse, int32_t* out_lit) {

@@ -1799,10 +1799,14 @@ __device__ __forceinline__ void tri_vertices(const SceneDev& sc, int tri, bool a
 // AOV: at bounce 0 a surface hit also writes its first-hit record to aov_rec[0..1] = (base colour, t), (shading normal as
 // surface_hit returns it, 0) -- as soon as they are known, so that they are not held through the rest of the step.  A primary
 // miss writes nothing.
-template <int MODE, bool DEFER_NEE = false, bool AOV = false>
+// ENV (light sampling mode with EZRT_PARAM_ENV_LIGHT, ezrt_math.h, DESIGN.md section 11): the map is one more light, sampled
+// with probability env.p_env from the table env; its samples travel as bounded shadow rays with tmax = EZ_INF and light
+// material -1.
+template <int MODE, bool DEFER_NEE = false, bool AOV = false, bool ENV = false>
 __device__ __forceinline__ bool shade_step(const SceneDev& sc, const RenderDev& rd, int bounce, PathRegs& p, float hit_t,
                                            int hit_tri, uint32_t px, uint32_t py, float2 sob, vec3& Lo, vec3& Le,
-                                           bool& primary_miss, ShadowRay& sh, float4* aov_rec = nullptr, LightsDev lights = LightsDev{}) {
+                                           bool& primary_miss, ShadowRay& sh, float4* aov_rec = nullptr, LightsDev lights = LightsDev{},
+                                           EnvDev env = EnvDev{}) {
     sh.valid = false;
     const int mode = (MODE < 0) ? rd.mode : MODE;
     const bool is_mode = (mode == EZRT_MODE_DISNEY_IS_MIS_P5);
@@ -1826,6 +1830,9 @@ __device__ __forceinline__ bool shade_step(const SceneDev& sc, const RenderDev& 
                 float mis_weight = mis_mix_weight(p.pdf, pdf_light);
                 vec3 c = ez_divs(ez_scale(ez_mul(ez_mul(ez_scale(p.history, mis_weight), sky), p.f_r), p.cosine_i), p.pdf);
                 Lo = ez_add(Lo, c);
+            } else if (ENV) {   // the map is a light: MIS against its sampling density, in mode 3's order
+                const float w = (env.p_env > 0.0f) ? mis_mix_weight(p.pdf, env.p_env * ez_env_pdf(env.texel_pdf, env.w, env.h, p.d)) : 1.0f;
+                Lo = ez_add(Lo, ez_divs(ez_scale(ez_mul(ez_mul(ez_scale(p.history, w), sky), p.f_r), p.cosine_i), p.pdf));
             } else {
                 Lo = ez_add(Lo, contrib3(p.history, sky, p.f_r, p.cosine_i, p.pdf));
             }
@@ -1850,7 +1857,8 @@ __device__ __forceinline__ bool shade_step(const SceneDev& sc, const RenderDev& 
                 tri_vertices(sc, hit_tri, rd.accel_space != 0, p1, p2, p3);
                 if (ez_is_light(ez_light_weight(p1, p2, p3, mat.emissive))) {
                     const vec3 Ng = f4xyz(ldg4(tri_geo_rec(sc, hit_tri, rd.accel_space != 0)));
-                    w = mis_mix_weight(p.pdf, ez_light_pdf(lum, lights.w_total, hit_t, ez_abs(ez_dot(Ng, p.d))));
+                    if constexpr (ENV) w = mis_mix_weight(p.pdf, (1.0f - env.p_env) * ez_light_pdf(lum, lights.w_total, hit_t, ez_abs(ez_dot(Ng, p.d))));
+                    else w = mis_mix_weight(p.pdf, ez_light_pdf(lum, lights.w_total, hit_t, ez_abs(ez_dot(Ng, p.d))));
                 }
             }
             Lo = ez_add(Lo, ez_divs(ez_scale(ez_mul(ez_mul(ez_scale(p.history, w), mat.emissive), p.f_r), p.cosine_i), p.pdf));
@@ -1878,8 +1886,29 @@ __device__ __forceinline__ bool shade_step(const SceneDev& sc, const RenderDev& 
         vec3 fr_l = splat3(0.0f);
         float pdf_l = 0.0f;
         if (NdotL > 0.0f) { fr_l = brdf_evaluate<false>(V, N, L, mat); pdf_l = brdf_pdf(V, N, L, mat); }
-        if (lights.n > 0) {
-            const float4* lr = lights.rec + 4 * (size_t)ez_light_select(lights.cdf, lights.n, r_sel);
+        bool env_pick = false;
+        float r_tri = r_sel;   // the triangle light's selection number
+        if constexpr (ENV) {   // the environment with probability p_env: r_sel < 0.5 beside triangle lights, always without
+            const bool half = (env.p_env == 0.5f);
+            env_pick = (env.p_env == 1.0f) || (half && r_sel < 0.5f);
+            if (half) r_tri = (r_sel - 0.5f) * 2.0f;
+            if (env_pick) {
+                int texel;
+                const vec3 Le_dir = ez_env_sample(env.row_cdf, env.col_cdf, env.w, env.h, r_1, r_2, &texel);
+                const float pdf_e = env.p_env * ez_env_pdf(env.texel_pdf, env.w, env.h, Le_dir);
+                if (ez_finite(pdf_e) && pdf_e > 0.0f && ez_dot(N, Le_dir) > 0.0f) {
+                    sh.valid = true;
+                    sh.o = hit.P;
+                    sh.d = Le_dir;
+                    sh.N = N; sh.V = V; sh.history = p.history; sh.matId = hit.matId;
+                    sh.tmax = EZ_INF;
+                    sh.pdf = pdf_e;
+                    sh.light_mat = -1;
+                }
+            }
+        }
+        if (!env_pick && lights.n > 0) {
+            const float4* lr = lights.rec + 4 * (size_t)ez_light_select(lights.cdf, lights.n, r_tri);
             const float4 a = ldg4(lr), b = ldg4(lr + 1), c = ldg4(lr + 2), e = ldg4(lr + 3);
             const int self = __float_as_int(rd.accel_space ? c.w : b.w);   // the light's triangle in the hit's index space
             const vec3 D = ez_sub(ez_triangle_point(f4xyz(a), f4xyz(b), f4xyz(c), r_1, r_2), hit.P);
@@ -1893,6 +1922,7 @@ __device__ __forceinline__ bool shade_step(const SceneDev& sc, const RenderDev& 
                 sh.N = N; sh.V = V; sh.history = p.history; sh.matId = hit.matId;
                 sh.tmax = ez_light_tmax(dist);
                 sh.pdf = ez_light_pdf(e.w, lights.w_total, dist, cos_l);
+                if constexpr (ENV) sh.pdf = sh.pdf * (1.0f - env.p_env);
                 sh.light_mat = __float_as_int(a.w);
             }
         }

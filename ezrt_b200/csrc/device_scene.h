@@ -128,15 +128,25 @@ struct LightsDev {
     float w_total;       // W_f = (float) sum of the weights
 };
 
+// The environment map's light table (EZRT_PARAM_ENV_LIGHT; ezrt_math.h, DESIGN.md section 11), built at the first flagged render
+// of a scene with a map.  Passed to the k_shade instantiations as a parameter of its own, after LightsDev.
+struct EnvDev {
+    const float* row_cdf;     // H floats, row_cdf[H - 1] = 1
+    const float* col_cdf;     // H x W floats, row-major
+    const float* texel_pdf;   // H x W floats, row-major
+    int w, h;
+    float p_env;              // the probability of an environment sample: 1/2 beside triangle lights, 1 without
+};
+
 // A shadow ray and what k_nee needs to evaluate the light sample's contribution once the ray got through (nee_contrib):
 // the BRDF / environment evaluation of the light sample is done after the shadow pass, for unoccluded rays only.
 #define EZRT_SHADOW_SLOT_BYTES (5 * 16 + 1)
 struct ShadowQueue {
     float4* ray_o;       // (origin.xyz, sample slot as bits)
     float4* ray_d;       // (direction to the light.xyz, material id as bits)
-    float4* nrm;         // (shading normal N.xyz, -; bounded rays of the light sampling mode: tmax)
+    float4* nrm;         // (shading normal N.xyz, -; bounded rays of the light sampling mode: tmax, EZ_INF for the environment)
     float4* view;        // (V = -incoming direction.xyz, -; light sampling mode: pdf of the light sample)
-    float4* hist;        // (path history.xyz, -; light sampling mode: the light's material id as bits)
+    float4* hist;        // (path history.xyz, -; light sampling mode: the light's material id as bits, -1 for the environment)
     unsigned char* lit;  // written by the shadow pass: 1 = nothing between the surface and the environment
 };
 

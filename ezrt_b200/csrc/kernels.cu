@@ -523,13 +523,14 @@ __global__ void __launch_bounds__(EZRT_EXTEND_MAX_THREADS, EZRT_EXTEND_LB_BLOCKS
 // AOV (feature-buffer renders): at bounce 0 every surface hit also writes its first-hit record, 32 bytes per sample slot:
 // aov_rec[2 slot] = (albedo, t), aov_rec[2 slot + 1] = (shading normal, 0).  A primary miss writes nothing (k_blend knows
 // it from Lo.w == 1).  The plain instantiations never touch aov_rec.
-template <int MODE, bool LIST, bool AOV = false>
+// ENV (light sampling mode with EZRT_PARAM_ENV_LIGHT): the map is one more light, sampled from the table env (shade_step).
+template <int MODE, bool LIST, bool AOV = false, bool ENV = false>
 __global__ void __launch_bounds__(128, EZRT_SHADE_MIN_BLOCKS) k_shade(SceneDev sc, RenderDev rd, const TileDev* __restrict__ tiles, int bounce,
                                                uint32_t batch_first_frame, PathQueue qin, const uint32_t* __restrict__ in_count,
                                                PathQueue qout, uint32_t* out_count, ShadowQueue sq, uint32_t* s_count,
                                                float4* __restrict__ Lo, float4* __restrict__ Le, uint32_t n_fused, uint32_t n_frames,
                                                const uint32_t* __restrict__ list, const float2* __restrict__ side_hit,
-                                               float4* __restrict__ aov_rec, LightsDev lights) {
+                                               float4* __restrict__ aov_rec, LightsDev lights, EnvDev env) {
     // The Sobol pair of (bounce, frame) is the same for every pixel of a frame (P5/fsh:361-376: up to 2 x 32 table XORs per path): each
     // block computes the pairs of the batch's frames once into shared memory (batches of more than EZRT_SOBOL_TABLE frames compute per path).
     __shared__ float2 s_sobol[EZRT_SOBOL_TABLE];
@@ -653,8 +654,8 @@ __global__ void __launch_bounds__(128, EZRT_SHADE_MIN_BLOCKS) k_shade(SceneDev s
             }
 #endif
             if (LIST || __float_as_int(hit.y) != EZRT_TRI_PENDING) {   // pending: deferred by the accel kernel, shaded by the LIST pass
-                alive = shade_step<MODE, MODE == EZRT_MODE_DISNEY_IS_MIS_P5, AOV>(sc, rd, bounce, p, hit.x, __float_as_int(hit.y), px, py, sob, lo, le,
-                                                                                 pmiss, sh, AOV ? aov_rec + 2 * (size_t)slot : nullptr, lights);
+                alive = shade_step<MODE, MODE == EZRT_MODE_DISNEY_IS_MIS_P5, AOV, ENV>(sc, rd, bounce, p, hit.x, __float_as_int(hit.y), px, py, sob, lo, le,
+                                                                                      pmiss, sh, AOV ? aov_rec + 2 * (size_t)slot : nullptr, lights, env);
                 if (bounce == 0) {
                     // Le is zero for every surface that does not emit: it is stored (and read back by k_blend) only otherwise.
                     // color = Le + Lo with Le = +-0 is Lo bit for bit, because Lo is never -0.0 (it starts at +0.0 and only grows by additions)
@@ -694,8 +695,9 @@ __global__ void __launch_bounds__(128, EZRT_SHADE_MIN_BLOCKS) k_shade(SceneDev s
 // the shadow pass, instead of for every light sample in k_shade.  Each block compacts the lit rays of 512 queue entries in
 // shared memory so that full warps evaluate.  One shadow ray per sample slot and bounce: no two threads touch one Lo entry.
 // ------------------------------------------------------------------------------------------
-// MODE = EZRT_MODE_DISNEY_LIGHTS: the light samples on the emissive triangles (nee_light_contrib; view.w = pdf, hist.w = the light's material).
-template <int MODE>
+// MODE = EZRT_MODE_DISNEY_LIGHTS: the light samples on the emissive triangles (nee_light_contrib; view.w = pdf, hist.w = the light's material);
+// ENV: and on the environment map (hist.w = -1: the light's colour is the map's in the sample's direction).
+template <int MODE, bool ENV = false>
 __global__ void __launch_bounds__(128, 8) k_nee(SceneDev sc, RenderDev rd, ShadowQueue sq, const uint32_t* __restrict__ s_count, float4* __restrict__ Lo) {
     __shared__ uint32_t s_scan[34];
     __shared__ uint32_t s_total;
@@ -719,7 +721,12 @@ __global__ void __launch_bounds__(128, 8) k_nee(SceneDev sc, RenderDev rd, Shado
             const uint32_t slot = __float_as_uint(o4.w);
             const MaterialDev mat = load_material(sc, __float_as_int(d4.w));
             vec3 c;
-            if (MODE == EZRT_MODE_DISNEY_LIGHTS)
+            if (MODE == EZRT_MODE_DISNEY_LIGHTS && ENV) {
+                const vec3 Ld = ez_v3(d4.x, d4.y, d4.z);
+                const int lm = __float_as_int(h4.w);
+                const vec3 E = (lm < 0) ? hdr_color(sc, rd, Ld, EZRT_MODE_DISNEY_LIGHTS) : load_emissive(sc, lm);
+                c = nee_light_contrib(ez_v3(v4.x, v4.y, v4.z), ez_v3(n4.x, n4.y, n4.z), Ld, mat, ez_v3(h4.x, h4.y, h4.z), E, v4.w);
+            } else if (MODE == EZRT_MODE_DISNEY_LIGHTS)
                 c = nee_light_contrib(ez_v3(v4.x, v4.y, v4.z), ez_v3(n4.x, n4.y, n4.z), ez_v3(d4.x, d4.y, d4.z), mat, ez_v3(h4.x, h4.y, h4.z),
                                       load_emissive(sc, __float_as_int(h4.w)), v4.w);
             else
@@ -1258,13 +1265,18 @@ void launch_shadow_accel(const SceneDev& sc, ShadowQueue sq, const uint32_t* s_c
 void launch_shade(const SceneDev& sc, const RenderDev& rd, const TileDev* tiles, int bounce, uint32_t batch_first_frame,
                   PathQueue qin, const uint32_t* in_count, PathQueue qout, uint32_t* out_count, ShadowQueue sq,
                   uint32_t* s_count, float4* Lo, float4* Le, uint32_t n_max, uint32_t n_fused, uint32_t n_frames, int n_sms, cudaStream_t st,
-                  float4* aov_rec, LightsDev lights) {
+                  float4* aov_rec, LightsDev lights, EnvDev env) {
     int blocks = std::min(div_up(n_max, 128), n_sms * 4 * EZRT_SHADE_MIN_BLOCKS);
     if (blocks < 1) blocks = 1;
-#define EZRT_LAUNCH_SHADE(M)                                                                                                                  \
-    if (aov_rec) k_shade<M, false, true><<<blocks, 128, 0, st>>>(sc, rd, tiles, bounce, batch_first_frame, qin, in_count, qout, out_count, sq, s_count, Lo, Le, \
-                                                                 n_fused, n_frames, nullptr, nullptr, aov_rec, lights);                      \
-    else k_shade<M, false><<<blocks, 128, 0, st>>>(sc, rd, tiles, bounce, batch_first_frame, qin, in_count, qout, out_count, sq, s_count, Lo, Le, n_fused, n_frames, nullptr, nullptr, nullptr, lights)
+#define EZRT_LAUNCH_SHADE_E(M, E)                                                                                                             \
+    if (aov_rec) k_shade<M, false, true, E><<<blocks, 128, 0, st>>>(sc, rd, tiles, bounce, batch_first_frame, qin, in_count, qout, out_count, sq, s_count, Lo, Le, \
+                                                                    n_fused, n_frames, nullptr, nullptr, aov_rec, lights, env);              \
+    else k_shade<M, false, false, E><<<blocks, 128, 0, st>>>(sc, rd, tiles, bounce, batch_first_frame, qin, in_count, qout, out_count, sq, s_count, Lo, Le, n_fused, n_frames, nullptr, nullptr, nullptr, lights, env)
+#define EZRT_LAUNCH_SHADE(M) EZRT_LAUNCH_SHADE_E(M, false)
+    if (rd.mode == EZRT_MODE_DISNEY_LIGHTS && env.row_cdf) {   // the map as a light (EZRT_PARAM_ENV_LIGHT)
+        EZRT_LAUNCH_SHADE_E(EZRT_MODE_DISNEY_LIGHTS, true);
+        return;
+    }
     switch (rd.mode) {
         case EZRT_MODE_DIFFUSE_P3: EZRT_LAUNCH_SHADE(EZRT_MODE_DIFFUSE_P3); break;
         case EZRT_MODE_DISNEY_ANISO_P4: EZRT_LAUNCH_SHADE(EZRT_MODE_DISNEY_ANISO_P4); break;
@@ -1273,6 +1285,7 @@ void launch_shade(const SceneDev& sc, const RenderDev& rd, const TileDev* tiles,
         default: EZRT_LAUNCH_SHADE(EZRT_MODE_DISNEY_IS_MIS_P5); break;
     }
 #undef EZRT_LAUNCH_SHADE
+#undef EZRT_LAUNCH_SHADE_E
 }
 // The accel policy's deferred lane (side stream, beside the main k_shade of the same bounce): exact traversal of the deferred
 // rays into side_hit, then their shading -- both do nothing if more than EZRT_SIDE_CAP rays were deferred (then
@@ -1280,13 +1293,18 @@ void launch_shade(const SceneDev& sc, const RenderDev& rd, const TileDev* tiles,
 void launch_deferred_lane(const SceneDev& sc, const RenderDev& rd, const TileDev* tiles, int bounce, uint32_t batch_first_frame, PathQueue qin,
                           const uint32_t* defer_list, const uint32_t* defer_count, uint32_t* defer_work, float2* side_hit, PathQueue qout,
                           uint32_t* out_count, ShadowQueue sq, uint32_t* s_count, float4* Lo, float4* Le, uint32_t n_fused, uint32_t n_frames,
-                          int n_sms, cudaStream_t st, float4* aov_rec, LightsDev lights) {
+                          int n_sms, cudaStream_t st, float4* aov_rec, LightsDev lights, EnvDev env) {
     launch_extend(sc, true, false, qin, defer_count, defer_work, defer_list, 1, EZRT_SIDE_CAP, n_sms, st, side_hit, 1);
     const int blocks = 8;
-#define EZRT_LAUNCH_SHADE(M)                                                                                                                  \
-    if (aov_rec) k_shade<M, true, true><<<blocks, 128, 0, st>>>(sc, rd, tiles, bounce, batch_first_frame, qin, defer_count, qout, out_count, sq, s_count, Lo, \
-                                                                Le, n_fused, n_frames, defer_list, side_hit, aov_rec, lights);                 \
-    else k_shade<M, true><<<blocks, 128, 0, st>>>(sc, rd, tiles, bounce, batch_first_frame, qin, defer_count, qout, out_count, sq, s_count, Lo, Le, n_fused, n_frames, defer_list, side_hit, nullptr, lights)
+#define EZRT_LAUNCH_SHADE_E(M, E)                                                                                                             \
+    if (aov_rec) k_shade<M, true, true, E><<<blocks, 128, 0, st>>>(sc, rd, tiles, bounce, batch_first_frame, qin, defer_count, qout, out_count, sq, s_count, Lo, \
+                                                                   Le, n_fused, n_frames, defer_list, side_hit, aov_rec, lights, env);         \
+    else k_shade<M, true, false, E><<<blocks, 128, 0, st>>>(sc, rd, tiles, bounce, batch_first_frame, qin, defer_count, qout, out_count, sq, s_count, Lo, Le, n_fused, n_frames, defer_list, side_hit, nullptr, lights, env)
+#define EZRT_LAUNCH_SHADE(M) EZRT_LAUNCH_SHADE_E(M, false)
+    if (rd.mode == EZRT_MODE_DISNEY_LIGHTS && env.row_cdf) {
+        EZRT_LAUNCH_SHADE_E(EZRT_MODE_DISNEY_LIGHTS, true);
+        return;
+    }
     switch (rd.mode) {
         case EZRT_MODE_DIFFUSE_P3: EZRT_LAUNCH_SHADE(EZRT_MODE_DIFFUSE_P3); break;
         case EZRT_MODE_DISNEY_ANISO_P4: EZRT_LAUNCH_SHADE(EZRT_MODE_DISNEY_ANISO_P4); break;
@@ -1295,10 +1313,13 @@ void launch_deferred_lane(const SceneDev& sc, const RenderDev& rd, const TileDev
         default: EZRT_LAUNCH_SHADE(EZRT_MODE_DISNEY_IS_MIS_P5); break;
     }
 #undef EZRT_LAUNCH_SHADE
+#undef EZRT_LAUNCH_SHADE_E
 }
-void launch_nee(const SceneDev& sc, const RenderDev& rd, ShadowQueue sq, const uint32_t* s_count, float4* Lo, uint32_t n_max, int n_sms, cudaStream_t st) {
+void launch_nee(const SceneDev& sc, const RenderDev& rd, ShadowQueue sq, const uint32_t* s_count, float4* Lo, uint32_t n_max, int n_sms, cudaStream_t st,
+                bool env) {
     const int blocks = std::max(1, std::min(div_up(n_max, 512), n_sms * 8));
-    if (rd.mode == EZRT_MODE_DISNEY_LIGHTS) k_nee<EZRT_MODE_DISNEY_LIGHTS><<<blocks, 128, 0, st>>>(sc, rd, sq, s_count, Lo);
+    if (rd.mode == EZRT_MODE_DISNEY_LIGHTS && env) k_nee<EZRT_MODE_DISNEY_LIGHTS, true><<<blocks, 128, 0, st>>>(sc, rd, sq, s_count, Lo);
+    else if (rd.mode == EZRT_MODE_DISNEY_LIGHTS) k_nee<EZRT_MODE_DISNEY_LIGHTS><<<blocks, 128, 0, st>>>(sc, rd, sq, s_count, Lo);
     else k_nee<EZRT_MODE_DISNEY_IS_MIS_P5><<<blocks, 128, 0, st>>>(sc, rd, sq, s_count, Lo);
 }
 
@@ -1344,6 +1365,17 @@ __global__ void __launch_bounds__(256) k_light_records(SceneDev sc, const int32_
     rec[4 * k + 1] = make_float4(p2.x, p2.y, p2.z, __int_as_float(tri));
     rec[4 * k + 2] = make_float4(p3.x, p3.y, p3.z, __int_as_float(acc));
     rec[4 * k + 3] = make_float4(N.x, N.y, N.z, ez_luminance(load_emissive(sc, mat)));
+}
+// the environment table's texel weights (ezrt_math.h, DESIGN.md section 11): w[i * W + j] = ez_env_weight(texel (i, j) of the map)
+__global__ void __launch_bounds__(256) k_env_weights(SceneDev sc, float* __restrict__ w) {
+    const int k = blockIdx.x * blockDim.x + threadIdx.x;
+    if (k >= sc.hdr_w * sc.hdr_h) return;
+    w[k] = ez_env_weight(texel3(sc.hdr, k), k / sc.hdr_w, sc.hdr_h);
+}
+void launch_env_weights(const SceneDev& sc, float* w, cudaStream_t st) {
+    const int n = sc.hdr_w * sc.hdr_h;
+    if (!sc.hdr || n <= 0) return;
+    k_env_weights<<<div_up(n, 256), 256, 0, st>>>(sc, w);
 }
 void launch_light_weights(const SceneDev& sc, float* w, cudaStream_t st) {
     if (sc.n_triangles <= 0) return;

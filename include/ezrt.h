@@ -53,9 +53,9 @@ typedef enum ezrt_mode {
     EZRT_MODE_DISNEY_SOBOL_P5 = 2, /* P5/fsh:762-807  Disney + Sobol/CP rotation               */
     EZRT_MODE_DISNEY_IS_MIS_P5 = 3, /* P5/fsh:810-890  BRDF + HDR importance sampling, MIS     */
     /* BRDF importance sampling + one light sample per bounce on the emissive triangles, balance-heuristic MIS (ezrt_math.h,
-     * DESIGN.md section 10).  With or without an HDR map: the environment is reached by BRDF samples only, at weight 1.
-     * Wavefront pipeline only.  The first render of a scene in this mode builds its light table (ezrt_scene_lights), which
-     * synchronises the render's stream once. */
+     * DESIGN.md section 10).  With or without an HDR map: the environment is reached by BRDF samples only, at weight 1,
+     * unless reserved[0] has EZRT_PARAM_ENV_LIGHT.  Wavefront pipeline only.  The first render of a scene in this mode builds
+     * its light table (ezrt_scene_lights), which synchronises the render's stream once. */
     EZRT_MODE_DISNEY_LIGHTS = 4
 } ezrt_mode;
 
@@ -111,6 +111,14 @@ typedef struct ezrt_render_params {
 /* ezrt_render_params.reserved[0]: keep counting -- ezrt_get_counters / ezrt_get_kernel_times then report the sums over all
    renders since the last one issued without this flag (a benchmark loop reads them once, without a sync per render) */
 #define EZRT_PARAM_ACCUMULATE 1
+/* ezrt_render_params.reserved[0], EZRT_MODE_DISNEY_LIGHTS only (any other mode: EZRT_ERR_INVALID): the scene's HDR map is one
+   more light.  Each shading point draws one light sample, from the map with probability 1/2 (1 when the scene has no emissive
+   triangle) by an equirectangular table proportional to luminance in solid angle, else from the triangles as in mode 4; BRDF
+   samples that leave the scene are MIS-weighted against it (ezrt_math.h, DESIGN.md section 11).  A scene without a map, or
+   whose map is black, renders as mode 4.  Accepted by ezrt_render[_device], ezrt_render_adaptive[_device] and
+   ezrt_render_aov[_device]; the first such render of a scene builds the map's table (ezrt_scene_env_light: about 8 bytes per
+   texel of device memory), which synchronises the render's stream once. */
+#define EZRT_PARAM_ENV_LIGHT 2
 
 typedef struct ezrt_counters {
     uint64_t rays;          /* hitBVH invocations: primary + bounce + shadow (SURVEY 8d)     */
@@ -256,6 +264,12 @@ int ezrt_trace_rays(ezrt_scene* scene, int n, const float* origins, const float*
  * tri_out = the lights' triangle indices (caller's order), cdf_out = their cumulative distribution (the last entry 1),
  * and *total_out = W, the float64 sum of the weights.  Any output may be NULL. */
 int ezrt_scene_lights(ezrt_scene* scene, int cap, int32_t* tri_out, float* cdf_out, double* total_out);
+
+/* The environment table of EZRT_PARAM_ENV_LIGHT (ezrt_math.h; built here if no flagged render has built it yet, which
+ * synchronises the device).  Returns 1 if the scene has a table, 0 if not (no map, or every texel weighs 0), or a negative
+ * status.  With a table of the scene's W x H map, writes row_cdf[H], col_cdf[H * W] and texel_pdf[H * W] (row-major, row 0
+ * at the top); *total = T, the float64 sum of the texel weights (0 without a table).  Any output may be NULL. */
+int ezrt_scene_env_light(ezrt_scene* scene, float* row_cdf, float* col_cdf, float* texel_pdf, double* total);
 
 /* Bounded occlusion of n rays (host arrays: origins, dirs n x 3, tmax n), for parity tests beside ezrt_trace_rays: runs the
  * shadow pass of the render for the traversal policy `traverse` -- the accel kernels with the exact pass over the rays they

@@ -393,4 +393,74 @@ EZ_HD int ez_light_select(const float* cdf, int n, float r) {
     return lo;
 }
 
+/* ------------------------------------------------------------------ the environment map as a light (DESIGN.md section 11)
+ * Mode EZRT_MODE_DISNEY_LIGHTS with EZRT_PARAM_ENV_LIGHT.  The map is W x H texels, row 0 at the top (tex2d's indexing).
+ * Table: w_ij = ez_env_weight(texel_ij, i, H); R_i = float64 sum of row i in column order, T = float64 sum of the R_i in row
+ * order; no table if T is not finite or not > 0.  Otherwise, each cast from float64 to float:
+ *   row_cdf_i = (float)((R_0 + ... + R_i) / T),  col_cdf_ij = (float)((w_i0 + ... + w_ij) / R_i) (0 where R_i = 0),
+ *   texel_pdf_ij = (float)(w_ij / T);  the last entry of row_cdf and of every row of col_cdf with R_i > 0 is exactly 1.
+ * Per shading point of a bounce b < max_bounce: P_env = 1/2 with K > 0 triangle lights, 1 with none (0 without a table:
+ * then the render is mode 4's).  The draws are mode 4's: r_sel, r_1, r_2, the Sobol pair, xi_3.  The environment is
+ * sampled if P_env == 1 or r_sel < 0.5:
+ *   L_e = ez_env_sample(r_1, r_2), pdf_e = P_env * ez_env_pdf(L_e); no sample if pdf_e is not finite or <= 0, or
+ *   dot(N, L_e) <= 0; else a shadow ray bounded at EZ_INF (mode 3's), and if lit
+ *   Lo += history * mis(pdf_e, BRDF_Pdf(V, N, L_e)) * hdrColor(L_e) * f_r(V, N, L_e) * dot(N, L_e) / pdf_e   (left to right)
+ * otherwise mode 4's triangle sample with the selection number (r_sel - 0.5) * 2 and pdf_l * (1 - P_env).
+ * A BRDF sample that leaves the scene at bounce >= 1 weighs mis(p.pdf, P_env * ez_env_pdf(d)) (mode 3's order); one that hits
+ * a light T weighs mis(p.pdf, (1 - P_env) * ez_light_pdf(...)); a camera ray that leaves the scene weighs 1. */
+/* toSphericalCoord (P5/fsh:684-690): the device's to_spherical and the oracle's toSphericalCoord are this sequence of operations */
+EZ_HD void ez_to_spherical(ez_vec3 v, float* ou, float* ov) {
+    float u = ez_atan2(v.z, v.x), w = ez_asin(v.y);
+    u = EZ_DIV(u, 2.0f * EZ_PI);
+    w = EZ_DIV(w, EZ_PI);
+    u += 0.5f;
+    w += 0.5f;
+    *ou = u;
+    *ov = 1.0f - w;
+}
+/* weight of texel (i, j) in row i of H: luminance times the cosine of the row centre's elevation (solid angle), 0 unless
+ * finite and > 0 */
+EZ_HD float ez_env_weight(ez_vec3 texel, int i, int H) {
+    const float e = EZ_PI * (0.5f - EZ_DIV((float)i + 0.5f, (float)H));
+    const float w = ez_luminance(texel) * ez_cos(e);
+    return (ez_finite(w) && w > 0.0f) ? w : 0.0f;
+}
+/* the first k with r < cdf[k] (ez_light_select) and the offset of r inside entry k, clamped below 1 */
+EZ_HD int ez_env_select(const float* cdf, int n, float r, float* offset) {
+    const int k = ez_light_select(cdf, n, r);
+    const float lo = (k > 0) ? cdf[k - 1] : 0.0f;
+    const float a = EZ_DIV(r - lo, cdf[k] - lo);
+    *offset = ez_min(a, 0.99999994f);
+    return k;
+}
+/* the direction of the sample (r_1, r_2); *texel = i * W + j, the texel it was drawn from */
+EZ_HD ez_vec3 ez_env_sample(const float* row_cdf, const float* col_cdf, int W, int H, float r_1, float r_2, int* texel) {
+    float a, b;
+    const int i = ez_env_select(row_cdf, H, r_1, &a);
+    const int j = ez_env_select(col_cdf + (size_t)i * W, W, r_2, &b);
+    *texel = i * W + j;
+    const float u = EZ_DIV((float)j + b, (float)W), v = EZ_DIV((float)i + a, (float)H);
+    const float phi = 2.0f * EZ_PI * (u - 0.5f);
+    const float e = EZ_PI * (0.5f - v);
+    const float ce = ez_cos(e);
+    return ez_v3(ce * ez_cos(phi), ez_sin(e), ce * ez_sin(phi));
+}
+/* the texel tex2d's nearest lookup reads at (u, v) */
+EZ_HD int ez_env_texel(float u, float v, int W, int H) {
+    int ix = (int)ez_floor(u * (float)W), iy = (int)ez_floor(v * (float)H);
+    ix = (ix < 0) ? 0 : ((ix > W - 1) ? W - 1 : ix);
+    iy = (iy < 0) ? 0 : ((iy > H - 1) ? H - 1 : iy);
+    return iy * W + ix;
+}
+/* solid-angle density of ez_env_sample at direction L: texel_pdf * W * H / (2 pi^2 cos e), 0 if the texel's pdf or cos e is 0 */
+EZ_HD float ez_env_pdf(const float* texel_pdf, int W, int H, ez_vec3 L) {
+    const ez_vec3 n = ez_normalize(L);
+    float u, v;
+    ez_to_spherical(n, &u, &v);
+    const float p = texel_pdf[ez_env_texel(u, v, W, H)];
+    const float ce = EZ_SQRT(n.x * n.x + n.z * n.z);
+    if (p == 0.0f || ce == 0.0f) return 0.0f;
+    return EZ_DIV(p * (float)(W * H), (2.0f * EZ_PI * EZ_PI) * ce);
+}
+
 #endif /* EZRT_MATH_H */
