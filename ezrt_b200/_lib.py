@@ -79,6 +79,7 @@ SIGNATURES = {
     "ezrt_scene_env_light": (C.c_int, [C.c_void_p, c_float_p, c_float_p, c_float_p, C.POINTER(C.c_double)]),
     "ezrt_occluded_rays": (C.c_int, [C.c_void_p, C.c_int, c_float_p, c_float_p, c_float_p, C.c_int, c_int32_p]),
     "ezrt_eval_brdf": (C.c_int, [C.c_int, C.c_int, C.c_int, c_float_p, c_float_p, c_float_p, c_float_p, c_float_p, c_float_p]),
+    "ezrt_eval_bsdf": (C.c_int, [C.c_int, C.c_int, C.c_int, c_float_p, c_float_p, c_float_p, c_float_p, c_int32_p, c_float_p, c_float_p]),
     "ezrt_eval_math": (C.c_int, [C.c_int, C.c_int, C.c_int, c_float_p, c_float_p, c_float_p]),
     "ezrt_post_tonemap": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int64, C.c_float, C.c_void_p]),
     "ezrt_write_png": (C.c_int, [C.c_char_p, c_float_p, C.c_int, C.c_int, C.c_int, C.c_int]),

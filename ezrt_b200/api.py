@@ -21,6 +21,7 @@ MODE_DISNEY_IS_MIS_P5 = 3
 MODE_DISNEY_LIGHTS = 4   # BRDF sampling + light sampling on the emissive triangles, MIS (DESIGN.md section 10)
 PARAM_ACCUMULATE = 1   # ezrt_render_params.reserved[0] flags (include/ezrt.h)
 PARAM_ENV_LIGHT = 2
+PARAM_TRANSMISSION = 4
 MODES = {"diffuse_p3": 0, "disney_aniso_p4": 1, "disney_sobol_p5": 2, "disney_is_mis_p5": 3, "disney_lights": 4}
 
 TRAVERSE_ACCEL = 0
@@ -216,6 +217,7 @@ class RenderConfig:
     profile: int = 0
     accumulate: bool = False   # EZRT_PARAM_ACCUMULATE: counters / kernel times continue from the previous render
     env_light: bool = False    # EZRT_PARAM_ENV_LIGHT (MODE_DISNEY_LIGHTS only): the HDR map is one more light (DESIGN.md section 11)
+    transmission: bool = False  # EZRT_PARAM_TRANSMISSION (MODE_DISNEY_LIGHTS only): materials' IOR and transmission (DESIGN.md section 12)
 
     def to_struct(self):
         p = RenderParams()
@@ -227,7 +229,8 @@ class RenderConfig:
         p.traverse, p.pipeline, p.out_channels = int(self.traverse), int(self.pipeline), int(self.out_channels)
         p.part_rank, p.part_count, p.frames_per_batch = int(self.part_rank), int(self.part_count), int(self.frames_per_batch)
         p.profile = int(self.profile)
-        p.reserved[0] = (PARAM_ACCUMULATE if self.accumulate else 0) | (PARAM_ENV_LIGHT if self.env_light else 0)
+        p.reserved[0] = ((PARAM_ACCUMULATE if self.accumulate else 0) | (PARAM_ENV_LIGHT if self.env_light else 0) |
+                         (PARAM_TRANSMISSION if self.transmission else 0))
         return p
 
 
@@ -477,6 +480,19 @@ def eval_brdf(which, V, N, L, xi, materials, device=0):
     out = np.zeros_like(V)
     check(lib.ezrt_eval_brdf(device, which, V.shape[0], _fp(V), _fp(N), None if L is None else _fp(L),
                              None if xi is None else _fp(xi), _fp(materials), _fp(out)))
+    return out
+
+
+def eval_bsdf(which, V, N, L, xi, inside, materials, device=0):
+    """ezrt_eval_bsdf: the transmission mixture on the device, [n, 8] float32 (which 0: f, 1: pdf, 2: sample of xi [n, 4])."""
+    V = _f32(V, (-1, 3)); N = _f32(N, (-1, 3))
+    L = None if L is None else _f32(L, (-1, 3))
+    xi = None if xi is None else _f32(xi, (-1, 4))
+    inside = np.ascontiguousarray(inside, dtype=np.int32).reshape(-1)
+    materials = _f32(materials, (-1, 18))
+    out = np.zeros((V.shape[0], 8), np.float32)
+    check(lib.ezrt_eval_bsdf(device, which, V.shape[0], _fp(V), _fp(N), None if L is None else _fp(L),
+                             None if xi is None else _fp(xi), inside.ctypes.data_as(_lib.c_int32_p), _fp(materials), _fp(out)))
     return out
 
 

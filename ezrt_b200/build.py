@@ -196,6 +196,24 @@ def build_oracle_env_light(force=False):
     return ORACLE_ENV_LIGHT_SO
 
 
+ORACLE_TRANSMISSION_SO = os.path.join(ROOT, "build", "libezrt_oracle_transmission.so")
+
+
+def build_oracle_transmission(force=False):
+    """build/libezrt_oracle_transmission.so: tests/oracle_transmission.cpp, the CPU restatement of the materials' transmission
+    (the mixture, its sampler, the flagged integrator with and without the map as a light) over the environment light's
+    restatement (test infrastructure, loaded only by tests/oracle_transmission.py)."""
+    src = os.path.join(ROOT, "tests", "oracle_transmission.cpp")
+    deps = [src, os.path.join(ROOT, "tests", "oracle_env_light.cpp"), os.path.join(ROOT, "tests", "oracle_lights.cpp"),
+            os.path.join(ROOT, "oracle", "ezrt_oracle.cpp")] + [os.path.join(INCLUDE, f) for f in os.listdir(INCLUDE)]
+    if force or _newer(ORACLE_TRANSMISSION_SO, deps):
+        os.makedirs(os.path.dirname(ORACLE_TRANSMISSION_SO), exist_ok=True)
+        tmp = ORACLE_TRANSMISSION_SO + ".tmp%d" % os.getpid()
+        _run(["g++"] + HOST_FLAGS + ["-fopenmp", "-Wno-misleading-indentation", "-shared", "-I", INCLUDE, src, "-o", tmp])
+        os.replace(tmp, ORACLE_TRANSMISSION_SO)
+    return ORACLE_TRANSMISSION_SO
+
+
 def build_reference_hdrloader(force=False):
     return _oracle_recipes().build_reference_hdrloader(force)
 
@@ -258,6 +276,7 @@ def build_all(force=False, verbose=False):
     build_oracle_aov(force=force)
     build_oracle_lights(force=force)
     build_oracle_env_light(force=force)
+    build_oracle_transmission(force=force)
     build_example(force=force)
     build_reference_hdrloader(force=force)
     build_reference_shaders(force=force)

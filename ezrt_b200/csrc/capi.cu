@@ -185,6 +185,8 @@ int validate_params(const ezrt_scene* scene, const ezrt_render_params* p) {
         return ezrt_set_error(EZRT_ERR_INVALID, "render: the light sampling mode runs on the wavefront pipeline only");
     if ((p->reserved[0] & EZRT_PARAM_ENV_LIGHT) && p->mode != EZRT_MODE_DISNEY_LIGHTS)
         return ezrt_set_error(EZRT_ERR_INVALID, "render: EZRT_PARAM_ENV_LIGHT needs the light sampling mode (got mode %d)", p->mode);
+    if ((p->reserved[0] & EZRT_PARAM_TRANSMISSION) && p->mode != EZRT_MODE_DISNEY_LIGHTS)
+        return ezrt_set_error(EZRT_ERR_INVALID, "render: EZRT_PARAM_TRANSMISSION needs the light sampling mode (got mode %d)", p->mode);
     if (p->max_bounce < 0 || p->max_bounce > 64) return ezrt_set_error(EZRT_ERR_INVALID, "render: max_bounce out of range");
     if (p->out_channels != 3 && p->out_channels != 4) return ezrt_set_error(EZRT_ERR_INVALID, "render: out_channels must be 3 or 4");
     if (p->part_count < 1 || p->part_rank < 0 || p->part_rank >= p->part_count)
@@ -954,6 +956,8 @@ static int render_device_impl(ezrt_scene* s, const ezrt_render_params* p, float*
             env.p_env = (lights.n > 0) ? 0.5f : 1.0f;
         }
     }
+    // EZRT_PARAM_TRANSMISSION: the TRANS instantiations of k_shade and k_nee
+    const bool trans = lights_mode && (p->reserved[0] & EZRT_PARAM_TRANSMISSION);
     int F = p->frames_per_batch;
     if (F <= 0) F = (int)std::max<size_t>(1, ((size_t)32 << 20) / per_frame);  // ~32 M sample slots per batch (~7.5 GB of state):
                                                                               // long queues amortise the persistent kernels' ramp-up and tail
@@ -1102,13 +1106,13 @@ static int render_device_impl(ezrt_scene* s, const ezrt_render_params* p, float*
                 CU_CHECK(cudaEventRecord(s->ev_fork, st));
                 CU_CHECK(cudaStreamWaitEvent(s->side_stream, s->ev_fork, 0));
                 launch_deferred_lane(s->dev, rd, d_tiles, b, batch_first, qin, defer_list, &d_ext[b], &dw_ext[b], side_hit, qout, &q_count[b + 1], sq, &s_count[b],
-                                     Lo, Le, n_fused, (uint32_t)nf, s->n_sms, s->side_stream, b == 0 ? aov_rec : nullptr, lights, env);
+                                     Lo, Le, n_fused, (uint32_t)nf, s->n_sms, s->side_stream, b == 0 ? aov_rec : nullptr, lights, env, trans);
                 CU_CHECK(cudaEventRecord(s->ev_join, s->side_stream));
                 s->launches += 2;
             }
             sp = s->span_begin(1, st);
             launch_shade(s->dev, rd, d_tiles, b, batch_first, qin, &q_count[b], qout, &q_count[b + 1], sq, &s_count[b], Lo, Le,
-                         n_slots, n_fused, (uint32_t)nf, s->n_sms, st, b == 0 ? aov_rec : nullptr, lights, env);
+                         n_slots, n_fused, (uint32_t)nf, s->n_sms, st, b == 0 ? aov_rec : nullptr, lights, env, trans);
             if (lane) CU_CHECK(cudaStreamWaitEvent(st, s->ev_join, 0));   // ... while this k_shade shades all the others; join
             s->span_end(sp, st);
             s->launches += 2;
@@ -1122,7 +1126,7 @@ static int render_device_impl(ezrt_scene* s, const ezrt_render_params* p, float*
                 }
                 s->span_end(sp, st);
                 sp = s->span_begin(1, st);   // shading work: counted with k_shade
-                launch_nee(s->dev, rd, sq, &s_count[b], Lo, n_slots, s->n_sms, st, env.row_cdf != nullptr);
+                launch_nee(s->dev, rd, sq, &s_count[b], Lo, n_slots, s->n_sms, st, env.row_cdf != nullptr, trans);
                 s->span_end(sp, st);
                 s->launches += 2;
             }
@@ -1626,6 +1630,40 @@ int ezrt_eval_brdf(int device, int which, int n, const float* V, const float* N,
     if (e == cudaSuccess) e = cudaMemcpy(out, dOut, f3, cudaMemcpyDeviceToHost);
     buf.release();
     if (e != cudaSuccess) return ezrt_set_error(EZRT_ERR_CUDA, "eval_brdf: %s", cudaGetErrorString(e));
+    return EZRT_OK;
+}
+
+int ezrt_eval_bsdf(int device, int which, int n, const float* V, const float* N, const float* L, const float* xi, const int32_t* inside,
+                   const float* materials, float* out) {
+    if (n < 0 || !V || !N || !inside || !materials || !out || which < 0 || which > 2) return ezrt_set_error(EZRT_ERR_INVALID, "eval_bsdf: bad argument");
+    if (which != 2 && !L) return ezrt_set_error(EZRT_ERR_INVALID, "eval_bsdf: L required");
+    if (which == 2 && !xi) return ezrt_set_error(EZRT_ERR_INVALID, "eval_bsdf: xi required");
+    if (n == 0) return EZRT_OK;
+    CU_CHECK(cudaSetDevice(device));
+    DeviceBuffer buf;
+    const size_t f3 = sizeof(float) * 3 * (size_t)n;
+    int rc = buf.ensure(f3 * 3 + sizeof(float) * (4 + 8 + 18) * (size_t)n + sizeof(int32_t) * (size_t)n + 256);
+    if (rc) return rc;
+    float* dV = (float*)buf.p;
+    float* dN = dV + 3 * (size_t)n;
+    float* dL = dN + 3 * (size_t)n;
+    float* dXi = dL + 3 * (size_t)n;
+    float* dOut = dXi + 4 * (size_t)n;
+    float* dM = dOut + 8 * (size_t)n;
+    int32_t* dIn = (int32_t*)(dM + 18 * (size_t)n);
+    cudaError_t e = cudaMemcpy(dV, V, f3, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = cudaMemcpy(dN, N, f3, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess && L) e = cudaMemcpy(dL, L, f3, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess && xi) e = cudaMemcpy(dXi, xi, sizeof(float) * 4 * (size_t)n, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = cudaMemcpy(dM, materials, sizeof(float) * 18 * (size_t)n, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = cudaMemcpy(dIn, inside, sizeof(int32_t) * (size_t)n, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) {
+        launch_eval_bsdf(which, n, dV, dN, L ? dL : nullptr, xi ? dXi : nullptr, dIn, dM, dOut, 0);
+        e = cudaGetLastError();
+    }
+    if (e == cudaSuccess) e = cudaMemcpy(out, dOut, sizeof(float) * 8 * (size_t)n, cudaMemcpyDeviceToHost);
+    buf.release();
+    if (e != cudaSuccess) return ezrt_set_error(EZRT_ERR_CUDA, "eval_bsdf: %s", cudaGetErrorString(e));
     return EZRT_OK;
 }
 

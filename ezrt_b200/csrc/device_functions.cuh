@@ -1410,6 +1410,7 @@ __device__ __forceinline__ vec3 load_emissive(const SceneDev& sc, int matId) {
 struct SurfaceHit {
     vec3 P, N;   // hitPoint, shading normal (flipped when hit from inside)
     int matId;
+    bool inside; // hit from inside: dot(Ng, d) > 0
 };
 
 // Recomputes P and the interpolated normal for (ray, t, tri).  p3fudge selects the P3/P4
@@ -1453,6 +1454,7 @@ __device__ __forceinline__ SurfaceHit surface_hit(const SceneDev& sc, vec3 o, ve
     r.P = P;
     r.N = inside ? ez_neg(Ns) : Ns;
     r.matId = __float_as_int(m0.w);
+    r.inside = inside;
     return r;
 }
 __device__ __forceinline__ int tri_material(const SceneDev& sc, int tri) {
@@ -1584,6 +1586,32 @@ __device__ __forceinline__ float mis_mix_weight(float a, float b) {  // P5/fsh:7
 }
 
 // ------------------------------------------------------------------------------------------
+// transmission (EZRT_PARAM_TRANSMISSION; ezrt_math.h, DESIGN.md section 12): the reference BRDF mixed with a rough dielectric
+// ------------------------------------------------------------------------------------------
+struct TransLobe {
+    float t, eta, alpha;   // the lobe's weight, eta_L / eta_V, the GGX alpha
+    bool matched;          // index-matched: a pass-through
+};
+// the dielectric lobe of material matId at a hit from `inside` (the record's fifth quad: IOR, transmission)
+__device__ __forceinline__ TransLobe trans_lobe(const SceneDev& sc, int matId, const MaterialDev& mat, bool inside) {
+    const float4 e = ldg4(sc.materials + (size_t)matId * 5 + 4);
+    TransLobe r;
+    r.t = ez_trans_weight(e.y, mat.metallic, e.x);
+    r.eta = ez_trans_eta(e.x, inside);
+    r.alpha = ez_max(0.001f, ez_sqr(mat.roughness));
+    r.matched = ez_trans_matched(e.x) != 0;
+    return r;
+}
+// the mixture's f at L and its pdf
+__device__ __forceinline__ vec3 bsdf_evaluate(vec3 V, vec3 N, vec3 L, const MaterialDev& mat, const TransLobe& tl, float& pdf) {
+    vec3 f_ref = splat3(0.0f), f_diel = splat3(0.0f);
+    float pdf_ref = 0.0f, pdf_diel = 0.0f;
+    if (ez_dot(N, L) > 0.0f) { f_ref = brdf_evaluate<false>(V, N, L, mat); pdf_ref = brdf_pdf(V, N, L, mat); }
+    if (!tl.matched) f_diel = ez_diel_eval(V, N, L, mat.baseColor, tl.alpha, tl.eta, &pdf_diel);
+    return ez_trans_mix(f_ref, pdf_ref, f_diel, pdf_diel, tl.t, &pdf);
+}
+
+// ------------------------------------------------------------------------------------------
 // direction samplers, P5/fsh:561-664
 // ------------------------------------------------------------------------------------------
 __device__ __forceinline__ vec3 to_normal_hemisphere(vec3 v, vec3 N) {
@@ -1637,6 +1665,27 @@ __device__ __forceinline__ vec3 sample_brdf(float xi_1, float xi_2, float xi_3, 
         return half_vector_to_L(sin_theta_h, cos_theta_h, phi_h, V, N);
     }
     return ez_v3(0.0f, 1.0f, 0.0f);
+}
+// The mixture's sample (ezrt_math.h, DESIGN.md section 12) at a hit with tl.t > 0: L, and what the path carries -- f, pdf and
+// the cosine |dot(N, L)| with the sign of dot(N, L) (< 0: below the surface).  Returns false when the path ends.  On entry L is
+// sample_brdf(xi_1, xi_2, xi_3, V, N, mat), the reference lobe's sample, which the caller has already drawn.
+__device__ __forceinline__ bool bsdf_sample(float xi_1, float xi_2, float xi_3, float r_t, vec3 V, vec3 N, const MaterialDev& mat,
+                                            const TransLobe& tl, vec3& L, vec3& f, float& pdf, float& cosine) {
+    if (r_t < tl.t) {
+        if (tl.matched) {   // pass-through: weight baseColor
+            L = ez_neg(V);
+            f = mat.baseColor;
+            pdf = 1.0f;
+            cosine = -1.0f;
+            return true;
+        }
+        if (!ez_diel_sample(xi_1, xi_2, xi_3, V, N, tl.alpha, tl.eta, &L)) return false;
+    } else if (!(ez_dot(N, L) > 0.0f)) {
+        return false;
+    }
+    f = bsdf_evaluate(V, N, L, mat, tl, pdf);
+    cosine = ez_dot(N, L);
+    return true;
 }
 
 // ------------------------------------------------------------------------------------------
@@ -1781,6 +1830,20 @@ __device__ __forceinline__ vec3 nee_light_contrib(vec3 V, vec3 N, vec3 L, const 
     const float mis_weight = mis_mix_weight(pdf_l, pdf_b);
     return ez_divs(ez_scale(ez_mul(ez_mul(ez_scale(history, mis_weight), E), fr), NdotL), pdf_l);
 }
+// ... with EZRT_PARAM_TRANSMISSION: the same product with the mixture's f and pdf, and nee_light_contrib's bits where t == 0
+__device__ __forceinline__ vec3 nee_trans_contrib(const SceneDev& sc, vec3 V, vec3 N, vec3 L, int matId, const MaterialDev& mat, bool inside,
+                                                  vec3 history, vec3 E, float pdf_l) {
+    const TransLobe tl = trans_lobe(sc, matId, mat, inside);
+    if (tl.t == 0.0f) return nee_light_contrib(V, N, L, mat, history, E, pdf_l);
+    const float NdotL = ez_dot(N, L);
+    float pdf_b;
+    const vec3 fr = bsdf_evaluate(V, N, L, mat, tl, pdf_b);
+    const float mis_weight = mis_mix_weight(pdf_l, pdf_b);
+    return ez_divs(ez_scale(ez_mul(ez_mul(ez_scale(history, mis_weight), E), fr), NdotL), pdf_l);
+}
+// the cosine a path record carries: with TRANS its sign is the bit "the BSDF sample went below the surface"
+template <bool TRANS>
+__device__ __forceinline__ float path_cos(float c) { return TRANS ? ez_abs(c) : c; }
 // the three vertices of triangle `tri` in the policy's index space (flat or indexed record)
 __device__ __forceinline__ void tri_vertices(const SceneDev& sc, int tri, bool accel_space, vec3& p1, vec3& p2, vec3& p3) {
     const float4* g = tri_geo_rec(sc, tri, accel_space);
@@ -1802,7 +1865,10 @@ __device__ __forceinline__ void tri_vertices(const SceneDev& sc, int tri, bool a
 // ENV (light sampling mode with EZRT_PARAM_ENV_LIGHT, ezrt_math.h, DESIGN.md section 11): the map is one more light, sampled
 // with probability env.p_env from the table env; its samples travel as bounded shadow rays with tmax = EZ_INF and light
 // material -1.
-template <int MODE, bool DEFER_NEE = false, bool AOV = false, bool ENV = false>
+// TRANS (light sampling mode with EZRT_PARAM_TRANSMISSION, ezrt_math.h, DESIGN.md section 12): a hit on a material with t > 0
+// samples and evaluates the mixture with the rough dielectric.  p.cosine_i keeps dot(N, L)'s sign: a BSDF sample below the
+// surface weighs 1 where it hits an emitter or leaves the scene.  The shadow ray's material id is ~matId for a hit from inside.
+template <int MODE, bool DEFER_NEE = false, bool AOV = false, bool ENV = false, bool TRANS = false>
 __device__ __forceinline__ bool shade_step(const SceneDev& sc, const RenderDev& rd, int bounce, PathRegs& p, float hit_t,
                                            int hit_tri, uint32_t px, uint32_t py, float2 sob, vec3& Lo, vec3& Le,
                                            bool& primary_miss, ShadowRay& sh, float4* aov_rec = nullptr, LightsDev lights = LightsDev{},
@@ -1812,6 +1878,7 @@ __device__ __forceinline__ bool shade_step(const SceneDev& sc, const RenderDev& 
     const bool is_mode = (mode == EZRT_MODE_DISNEY_IS_MIS_P5);
     // the light sampling mode exists only as k_shade<EZRT_MODE_DISNEY_LIGHTS> (the megakernel, MODE < 0, rejects it)
     constexpr bool lights_mode = (MODE == EZRT_MODE_DISNEY_LIGHTS);
+    const bool below = TRANS && p.cosine_i < 0.0f;   // the BSDF sample went below the surface: no light strategy reaches it
     if (bounce == 0) {
         Lo = splat3(0.0f);
         Le = splat3(0.0f);
@@ -1831,10 +1898,10 @@ __device__ __forceinline__ bool shade_step(const SceneDev& sc, const RenderDev& 
                 vec3 c = ez_divs(ez_scale(ez_mul(ez_mul(ez_scale(p.history, mis_weight), sky), p.f_r), p.cosine_i), p.pdf);
                 Lo = ez_add(Lo, c);
             } else if (ENV) {   // the map is a light: MIS against its sampling density, in mode 3's order
-                const float w = (env.p_env > 0.0f) ? mis_mix_weight(p.pdf, env.p_env * ez_env_pdf(env.texel_pdf, env.w, env.h, p.d)) : 1.0f;
-                Lo = ez_add(Lo, ez_divs(ez_scale(ez_mul(ez_mul(ez_scale(p.history, w), sky), p.f_r), p.cosine_i), p.pdf));
+                const float w = (env.p_env > 0.0f && !below) ? mis_mix_weight(p.pdf, env.p_env * ez_env_pdf(env.texel_pdf, env.w, env.h, p.d)) : 1.0f;
+                Lo = ez_add(Lo, ez_divs(ez_scale(ez_mul(ez_mul(ez_scale(p.history, w), sky), p.f_r), path_cos<TRANS>(p.cosine_i)), p.pdf));
             } else {
-                Lo = ez_add(Lo, contrib3(p.history, sky, p.f_r, p.cosine_i, p.pdf));
+                Lo = ez_add(Lo, contrib3(p.history, sky, p.f_r, path_cos<TRANS>(p.cosine_i), p.pdf));
             }
             return false;
         }
@@ -1852,7 +1919,7 @@ __device__ __forceinline__ bool shade_step(const SceneDev& sc, const RenderDev& 
         if (lights_mode) {   // a BRDF sample that hit a light: MIS against the light sampling pdf of the hit point
             float w = 1.0f;
             const float lum = ez_luminance(mat.emissive);
-            if (lum > 0.0f) {   // otherwise the weight area * lum is never a light
+            if (lum > 0.0f && !below) {   // lum <= 0: the weight area * lum is never a light; below: weight 1
                 vec3 p1, p2, p3;
                 tri_vertices(sc, hit_tri, rd.accel_space != 0, p1, p2, p3);
                 if (ez_is_light(ez_light_weight(p1, p2, p3, mat.emissive))) {
@@ -1861,11 +1928,11 @@ __device__ __forceinline__ bool shade_step(const SceneDev& sc, const RenderDev& 
                     else w = mis_mix_weight(p.pdf, ez_light_pdf(lum, lights.w_total, hit_t, ez_abs(ez_dot(Ng, p.d))));
                 }
             }
-            Lo = ez_add(Lo, ez_divs(ez_scale(ez_mul(ez_mul(ez_scale(p.history, w), mat.emissive), p.f_r), p.cosine_i), p.pdf));
+            Lo = ez_add(Lo, ez_divs(ez_scale(ez_mul(ez_mul(ez_scale(p.history, w), mat.emissive), p.f_r), path_cos<TRANS>(p.cosine_i)), p.pdf));
         } else {
             Lo = ez_add(Lo, contrib3(p.history, mat.emissive, p.f_r, p.cosine_i, p.pdf));
         }
-        p.history = ez_mul(p.history, ez_divs(ez_scale(p.f_r, p.cosine_i), p.pdf));
+        p.history = ez_mul(p.history, ez_divs(ez_scale(p.f_r, path_cos<TRANS>(p.cosine_i)), p.pdf));
     }
     if (bounce >= rd.max_bounce) return false;
 
@@ -1882,10 +1949,16 @@ __device__ __forceinline__ bool shade_step(const SceneDev& sc, const RenderDev& 
         cp_rotate(xi_1, xi_2, px, py);
         const float xi_3 = rand01(p.seed);
         L = sample_brdf(xi_1, xi_2, xi_3, V, N, mat);
-        const float NdotL = ez_dot(N, L);
+        float NdotL = ez_dot(N, L);
         vec3 fr_l = splat3(0.0f);
         float pdf_l = 0.0f;
         if (NdotL > 0.0f) { fr_l = brdf_evaluate<false>(V, N, L, mat); pdf_l = brdf_pdf(V, N, L, mat); }
+        bool go = !(NdotL <= 0.0f);   // the path continues
+        if constexpr (TRANS) {   // a material with a dielectric lobe: the mixture's sample instead, with one more draw, r_t
+            const TransLobe tl = trans_lobe(sc, hit.matId, mat, hit.inside);
+            if (tl.t != 0.0f) go = bsdf_sample(xi_1, xi_2, xi_3, rand01(p.seed), V, N, mat, tl, L, fr_l, pdf_l, NdotL);
+        }
+        const int sh_mat = (TRANS && hit.inside) ? ~hit.matId : hit.matId;   // k_nee<.., TRANS> needs the side for eta
         bool env_pick = false;
         float r_tri = r_sel;   // the triangle light's selection number
         if constexpr (ENV) {   // the environment with probability p_env: r_sel < 0.5 beside triangle lights, always without
@@ -1900,7 +1973,7 @@ __device__ __forceinline__ bool shade_step(const SceneDev& sc, const RenderDev& 
                     sh.valid = true;
                     sh.o = hit.P;
                     sh.d = Le_dir;
-                    sh.N = N; sh.V = V; sh.history = p.history; sh.matId = hit.matId;
+                    sh.N = N; sh.V = V; sh.history = p.history; sh.matId = sh_mat;
                     sh.tmax = EZ_INF;
                     sh.pdf = pdf_e;
                     sh.light_mat = -1;
@@ -1919,17 +1992,17 @@ __device__ __forceinline__ bool shade_step(const SceneDev& sc, const RenderDev& 
                 sh.valid = true;
                 sh.o = hit.P;
                 sh.d = Ll;
-                sh.N = N; sh.V = V; sh.history = p.history; sh.matId = hit.matId;
+                sh.N = N; sh.V = V; sh.history = p.history; sh.matId = sh_mat;
                 sh.tmax = ez_light_tmax(dist);
                 sh.pdf = ez_light_pdf(e.w, lights.w_total, dist, cos_l);
                 if constexpr (ENV) sh.pdf = sh.pdf * (1.0f - env.p_env);
                 sh.light_mat = __float_as_int(a.w);
             }
         }
-        if (NdotL <= 0.0f) return false;
+        if (!go) return false;
         p.f_r = fr_l;
         p.pdf = pdf_l;   // <= 0: traced, then break
-        p.cosine_i = NdotL;
+        p.cosine_i = NdotL;   // TRANS: < 0 below the surface
     } else if (is_mode) {
         // environment importance sample + shadow ray (P5/fsh:820-842), then the BRDF sample (:845-865).  The three
         // random numbers are drawn in the shader's order (two for SampleHdr :822, one for the lobe choice :849); the BRDF

@@ -524,7 +524,8 @@ __global__ void __launch_bounds__(EZRT_EXTEND_MAX_THREADS, EZRT_EXTEND_LB_BLOCKS
 // aov_rec[2 slot] = (albedo, t), aov_rec[2 slot + 1] = (shading normal, 0).  A primary miss writes nothing (k_blend knows
 // it from Lo.w == 1).  The plain instantiations never touch aov_rec.
 // ENV (light sampling mode with EZRT_PARAM_ENV_LIGHT): the map is one more light, sampled from the table env (shade_step).
-template <int MODE, bool LIST, bool AOV = false, bool ENV = false>
+// TRANS (light sampling mode with EZRT_PARAM_TRANSMISSION): materials with a dielectric lobe (shade_step).
+template <int MODE, bool LIST, bool AOV = false, bool ENV = false, bool TRANS = false>
 __global__ void __launch_bounds__(128, EZRT_SHADE_MIN_BLOCKS) k_shade(SceneDev sc, RenderDev rd, const TileDev* __restrict__ tiles, int bounce,
                                                uint32_t batch_first_frame, PathQueue qin, const uint32_t* __restrict__ in_count,
                                                PathQueue qout, uint32_t* out_count, ShadowQueue sq, uint32_t* s_count,
@@ -654,8 +655,8 @@ __global__ void __launch_bounds__(128, EZRT_SHADE_MIN_BLOCKS) k_shade(SceneDev s
             }
 #endif
             if (LIST || __float_as_int(hit.y) != EZRT_TRI_PENDING) {   // pending: deferred by the accel kernel, shaded by the LIST pass
-                alive = shade_step<MODE, MODE == EZRT_MODE_DISNEY_IS_MIS_P5, AOV, ENV>(sc, rd, bounce, p, hit.x, __float_as_int(hit.y), px, py, sob, lo, le,
-                                                                                      pmiss, sh, AOV ? aov_rec + 2 * (size_t)slot : nullptr, lights, env);
+                alive = shade_step<MODE, MODE == EZRT_MODE_DISNEY_IS_MIS_P5, AOV, ENV, TRANS>(sc, rd, bounce, p, hit.x, __float_as_int(hit.y), px, py, sob, lo, le,
+                                                                                             pmiss, sh, AOV ? aov_rec + 2 * (size_t)slot : nullptr, lights, env);
                 if (bounce == 0) {
                     // Le is zero for every surface that does not emit: it is stored (and read back by k_blend) only otherwise.
                     // color = Le + Lo with Le = +-0 is Lo bit for bit, because Lo is never -0.0 (it starts at +0.0 and only grows by additions)
@@ -697,7 +698,8 @@ __global__ void __launch_bounds__(128, EZRT_SHADE_MIN_BLOCKS) k_shade(SceneDev s
 // ------------------------------------------------------------------------------------------
 // MODE = EZRT_MODE_DISNEY_LIGHTS: the light samples on the emissive triangles (nee_light_contrib; view.w = pdf, hist.w = the light's material);
 // ENV: and on the environment map (hist.w = -1: the light's colour is the map's in the sample's direction).
-template <int MODE, bool ENV = false>
+// TRANS: evaluated with the mixture of the shading point's material (nee_trans_contrib); ray_d.w = ~matId for a hit from inside.
+template <int MODE, bool ENV = false, bool TRANS = false>
 __global__ void __launch_bounds__(128, 8) k_nee(SceneDev sc, RenderDev rd, ShadowQueue sq, const uint32_t* __restrict__ s_count, float4* __restrict__ Lo) {
     __shared__ uint32_t s_scan[34];
     __shared__ uint32_t s_total;
@@ -719,9 +721,16 @@ __global__ void __launch_bounds__(128, 8) k_nee(SceneDev sc, RenderDev rd, Shado
             const uint32_t j = s_list[q];
             const float4 o4 = __ldcs(sq.ray_o + j), d4 = __ldcs(sq.ray_d + j), n4 = __ldcs(sq.nrm + j), v4 = __ldcs(sq.view + j), h4 = __ldcs(sq.hist + j);
             const uint32_t slot = __float_as_uint(o4.w);
-            const MaterialDev mat = load_material(sc, __float_as_int(d4.w));
+            const int m_raw = __float_as_int(d4.w);
+            const int m_id = (TRANS && m_raw < 0) ? ~m_raw : m_raw;
+            const MaterialDev mat = load_material(sc, m_id);
             vec3 c;
-            if (MODE == EZRT_MODE_DISNEY_LIGHTS && ENV) {
+            if (MODE == EZRT_MODE_DISNEY_LIGHTS && TRANS) {
+                const vec3 Ld = ez_v3(d4.x, d4.y, d4.z);
+                const int lm = __float_as_int(h4.w);
+                const vec3 E = (ENV && lm < 0) ? hdr_color(sc, rd, Ld, EZRT_MODE_DISNEY_LIGHTS) : load_emissive(sc, lm);
+                c = nee_trans_contrib(sc, ez_v3(v4.x, v4.y, v4.z), ez_v3(n4.x, n4.y, n4.z), Ld, m_id, mat, m_raw < 0, ez_v3(h4.x, h4.y, h4.z), E, v4.w);
+            } else if (MODE == EZRT_MODE_DISNEY_LIGHTS && ENV) {
                 const vec3 Ld = ez_v3(d4.x, d4.y, d4.z);
                 const int lm = __float_as_int(h4.w);
                 const vec3 E = (lm < 0) ? hdr_color(sc, rd, Ld, EZRT_MODE_DISNEY_LIGHTS) : load_emissive(sc, lm);
@@ -986,6 +995,37 @@ __global__ void k_eval_brdf(int which, int n, const float* V, const float* N, co
     else if (which == 2) r.x = brdf_pdf(v, nn, l, m);
     else if (which == 3) r = sample_brdf(xi[3 * i], xi[3 * i + 1], xi[3 * i + 2], v, nn, m);
     out[3 * i] = r.x; out[3 * i + 1] = r.y; out[3 * i + 2] = r.z;
+}
+
+// ezrt_eval_bsdf: the transmission mixture (ezrt_math.h, DESIGN.md section 12), 8 floats out per tuple:
+// which 0: f (3), 1: pdf (1), 2: the sample of xi[4 i .. 4 i + 3] = (xi_1, xi_2, xi_3, r_t): L (3), f (3), pdf, signed cosine (0: the path ends)
+__global__ void k_eval_bsdf(int which, int n, const float* V, const float* N, const float* L, const float* xi, const int* inside,
+                            const float* materials, float* out) {
+    int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const vec3 v = ez_v3(V[3 * i], V[3 * i + 1], V[3 * i + 2]);
+    const vec3 nn = ez_v3(N[3 * i], N[3 * i + 1], N[3 * i + 2]);
+    const float* m18 = materials + (size_t)i * 18;
+    const MaterialDev m = material_from18(m18);
+    TransLobe tl;
+    tl.t = ez_trans_weight(m18[17], m.metallic, m18[16]);
+    tl.eta = ez_trans_eta(m18[16], inside[i]);
+    tl.alpha = ez_max(0.001f, ez_sqr(m.roughness));
+    tl.matched = ez_trans_matched(m18[16]) != 0;
+    float r[8] = {0.0f, 0.0f, 0.0f, 0.0f, 0.0f, 0.0f, 0.0f, 0.0f};
+    if (which == 0 || which == 1) {
+        float pdf;
+        const vec3 f = bsdf_evaluate(v, nn, ez_v3(L[3 * i], L[3 * i + 1], L[3 * i + 2]), m, tl, pdf);
+        if (which == 0) { r[0] = f.x; r[1] = f.y; r[2] = f.z; }
+        else r[0] = pdf;
+    } else {
+        vec3 l = sample_brdf(xi[4 * i], xi[4 * i + 1], xi[4 * i + 2], v, nn, m), f = splat3(0.0f);
+        float pdf = 0.0f, cosine = 0.0f;
+        if (bsdf_sample(xi[4 * i], xi[4 * i + 1], xi[4 * i + 2], xi[4 * i + 3], v, nn, m, tl, l, f, pdf, cosine)) {
+            r[0] = l.x; r[1] = l.y; r[2] = l.z; r[3] = f.x; r[4] = f.y; r[5] = f.z; r[6] = pdf; r[7] = cosine;
+        }
+    }
+    for (int k = 0; k < 8; k++) out[8 * (size_t)i + k] = r[k];
 }
 
 __global__ void k_eval_math(int which, int n, const float* a, const float* b, float* out) {
@@ -1265,16 +1305,21 @@ void launch_shadow_accel(const SceneDev& sc, ShadowQueue sq, const uint32_t* s_c
 void launch_shade(const SceneDev& sc, const RenderDev& rd, const TileDev* tiles, int bounce, uint32_t batch_first_frame,
                   PathQueue qin, const uint32_t* in_count, PathQueue qout, uint32_t* out_count, ShadowQueue sq,
                   uint32_t* s_count, float4* Lo, float4* Le, uint32_t n_max, uint32_t n_fused, uint32_t n_frames, int n_sms, cudaStream_t st,
-                  float4* aov_rec, LightsDev lights, EnvDev env) {
+                  float4* aov_rec, LightsDev lights, EnvDev env, bool trans) {
     int blocks = std::min(div_up(n_max, 128), n_sms * 4 * EZRT_SHADE_MIN_BLOCKS);
     if (blocks < 1) blocks = 1;
-#define EZRT_LAUNCH_SHADE_E(M, E)                                                                                                             \
-    if (aov_rec) k_shade<M, false, true, E><<<blocks, 128, 0, st>>>(sc, rd, tiles, bounce, batch_first_frame, qin, in_count, qout, out_count, sq, s_count, Lo, Le, \
-                                                                    n_fused, n_frames, nullptr, nullptr, aov_rec, lights, env);              \
-    else k_shade<M, false, false, E><<<blocks, 128, 0, st>>>(sc, rd, tiles, bounce, batch_first_frame, qin, in_count, qout, out_count, sq, s_count, Lo, Le, n_fused, n_frames, nullptr, nullptr, nullptr, lights, env)
-#define EZRT_LAUNCH_SHADE(M) EZRT_LAUNCH_SHADE_E(M, false)
+#define EZRT_LAUNCH_SHADE_E(M, E, T)                                                                                                          \
+    if (aov_rec) k_shade<M, false, true, E, T><<<blocks, 128, 0, st>>>(sc, rd, tiles, bounce, batch_first_frame, qin, in_count, qout, out_count, sq, s_count, Lo, Le, \
+                                                                       n_fused, n_frames, nullptr, nullptr, aov_rec, lights, env);           \
+    else k_shade<M, false, false, E, T><<<blocks, 128, 0, st>>>(sc, rd, tiles, bounce, batch_first_frame, qin, in_count, qout, out_count, sq, s_count, Lo, Le, n_fused, n_frames, nullptr, nullptr, nullptr, lights, env)
+#define EZRT_LAUNCH_SHADE(M) EZRT_LAUNCH_SHADE_E(M, false, false)
+    if (rd.mode == EZRT_MODE_DISNEY_LIGHTS && trans) {   // materials with a dielectric lobe (EZRT_PARAM_TRANSMISSION)
+        if (env.row_cdf) { EZRT_LAUNCH_SHADE_E(EZRT_MODE_DISNEY_LIGHTS, true, true); }
+        else { EZRT_LAUNCH_SHADE_E(EZRT_MODE_DISNEY_LIGHTS, false, true); }
+        return;
+    }
     if (rd.mode == EZRT_MODE_DISNEY_LIGHTS && env.row_cdf) {   // the map as a light (EZRT_PARAM_ENV_LIGHT)
-        EZRT_LAUNCH_SHADE_E(EZRT_MODE_DISNEY_LIGHTS, true);
+        EZRT_LAUNCH_SHADE_E(EZRT_MODE_DISNEY_LIGHTS, true, false);
         return;
     }
     switch (rd.mode) {
@@ -1293,16 +1338,21 @@ void launch_shade(const SceneDev& sc, const RenderDev& rd, const TileDev* tiles,
 void launch_deferred_lane(const SceneDev& sc, const RenderDev& rd, const TileDev* tiles, int bounce, uint32_t batch_first_frame, PathQueue qin,
                           const uint32_t* defer_list, const uint32_t* defer_count, uint32_t* defer_work, float2* side_hit, PathQueue qout,
                           uint32_t* out_count, ShadowQueue sq, uint32_t* s_count, float4* Lo, float4* Le, uint32_t n_fused, uint32_t n_frames,
-                          int n_sms, cudaStream_t st, float4* aov_rec, LightsDev lights, EnvDev env) {
+                          int n_sms, cudaStream_t st, float4* aov_rec, LightsDev lights, EnvDev env, bool trans) {
     launch_extend(sc, true, false, qin, defer_count, defer_work, defer_list, 1, EZRT_SIDE_CAP, n_sms, st, side_hit, 1);
     const int blocks = 8;
-#define EZRT_LAUNCH_SHADE_E(M, E)                                                                                                             \
-    if (aov_rec) k_shade<M, true, true, E><<<blocks, 128, 0, st>>>(sc, rd, tiles, bounce, batch_first_frame, qin, defer_count, qout, out_count, sq, s_count, Lo, \
-                                                                   Le, n_fused, n_frames, defer_list, side_hit, aov_rec, lights, env);         \
-    else k_shade<M, true, false, E><<<blocks, 128, 0, st>>>(sc, rd, tiles, bounce, batch_first_frame, qin, defer_count, qout, out_count, sq, s_count, Lo, Le, n_fused, n_frames, defer_list, side_hit, nullptr, lights, env)
-#define EZRT_LAUNCH_SHADE(M) EZRT_LAUNCH_SHADE_E(M, false)
+#define EZRT_LAUNCH_SHADE_E(M, E, T)                                                                                                          \
+    if (aov_rec) k_shade<M, true, true, E, T><<<blocks, 128, 0, st>>>(sc, rd, tiles, bounce, batch_first_frame, qin, defer_count, qout, out_count, sq, s_count, Lo, \
+                                                                      Le, n_fused, n_frames, defer_list, side_hit, aov_rec, lights, env);      \
+    else k_shade<M, true, false, E, T><<<blocks, 128, 0, st>>>(sc, rd, tiles, bounce, batch_first_frame, qin, defer_count, qout, out_count, sq, s_count, Lo, Le, n_fused, n_frames, defer_list, side_hit, nullptr, lights, env)
+#define EZRT_LAUNCH_SHADE(M) EZRT_LAUNCH_SHADE_E(M, false, false)
+    if (rd.mode == EZRT_MODE_DISNEY_LIGHTS && trans) {
+        if (env.row_cdf) { EZRT_LAUNCH_SHADE_E(EZRT_MODE_DISNEY_LIGHTS, true, true); }
+        else { EZRT_LAUNCH_SHADE_E(EZRT_MODE_DISNEY_LIGHTS, false, true); }
+        return;
+    }
     if (rd.mode == EZRT_MODE_DISNEY_LIGHTS && env.row_cdf) {
-        EZRT_LAUNCH_SHADE_E(EZRT_MODE_DISNEY_LIGHTS, true);
+        EZRT_LAUNCH_SHADE_E(EZRT_MODE_DISNEY_LIGHTS, true, false);
         return;
     }
     switch (rd.mode) {
@@ -1316,9 +1366,11 @@ void launch_deferred_lane(const SceneDev& sc, const RenderDev& rd, const TileDev
 #undef EZRT_LAUNCH_SHADE_E
 }
 void launch_nee(const SceneDev& sc, const RenderDev& rd, ShadowQueue sq, const uint32_t* s_count, float4* Lo, uint32_t n_max, int n_sms, cudaStream_t st,
-                bool env) {
+                bool env, bool trans) {
     const int blocks = std::max(1, std::min(div_up(n_max, 512), n_sms * 8));
-    if (rd.mode == EZRT_MODE_DISNEY_LIGHTS && env) k_nee<EZRT_MODE_DISNEY_LIGHTS, true><<<blocks, 128, 0, st>>>(sc, rd, sq, s_count, Lo);
+    if (rd.mode == EZRT_MODE_DISNEY_LIGHTS && trans && env) k_nee<EZRT_MODE_DISNEY_LIGHTS, true, true><<<blocks, 128, 0, st>>>(sc, rd, sq, s_count, Lo);
+    else if (rd.mode == EZRT_MODE_DISNEY_LIGHTS && trans) k_nee<EZRT_MODE_DISNEY_LIGHTS, false, true><<<blocks, 128, 0, st>>>(sc, rd, sq, s_count, Lo);
+    else if (rd.mode == EZRT_MODE_DISNEY_LIGHTS && env) k_nee<EZRT_MODE_DISNEY_LIGHTS, true><<<blocks, 128, 0, st>>>(sc, rd, sq, s_count, Lo);
     else if (rd.mode == EZRT_MODE_DISNEY_LIGHTS) k_nee<EZRT_MODE_DISNEY_LIGHTS><<<blocks, 128, 0, st>>>(sc, rd, sq, s_count, Lo);
     else k_nee<EZRT_MODE_DISNEY_IS_MIS_P5><<<blocks, 128, 0, st>>>(sc, rd, sq, s_count, Lo);
 }
@@ -1425,6 +1477,10 @@ void launch_trace_finish(const SceneDev& sc, int n, PathQueue q, int p3fudge, in
 void launch_eval_brdf(int which, int n, const float* V, const float* N, const float* L, const float* xi, const float* materials,
                       float* out, cudaStream_t st) {
     k_eval_brdf<<<div_up(n, 128), 128, 0, st>>>(which, n, V, N, L, xi, materials, out);
+}
+void launch_eval_bsdf(int which, int n, const float* V, const float* N, const float* L, const float* xi, const int* inside,
+                      const float* materials, float* out, cudaStream_t st) {
+    k_eval_bsdf<<<div_up(n, 128), 128, 0, st>>>(which, n, V, N, L, xi, inside, materials, out);
 }
 void launch_eval_math(int which, int n, const float* a, const float* b, float* out, cudaStream_t st) {
     k_eval_math<<<div_up(n, 256), 256, 0, st>>>(which, n, a, b, out);

@@ -119,6 +119,16 @@ typedef struct ezrt_render_params {
    ezrt_render_aov[_device]; the first such render of a scene builds the map's table (ezrt_scene_env_light: about 8 bytes per
    texel of device memory), which synchronises the render's stream once. */
 #define EZRT_PARAM_ENV_LIGHT 2
+/* ezrt_render_params.reserved[0], EZRT_MODE_DISNEY_LIGHTS only (any other mode: EZRT_ERR_INVALID), with or without
+   EZRT_PARAM_ENV_LIGHT: materials' IOR and transmission are rendered.  A material with t = clamp(transmission, 0, 1) *
+   (1 - metallic) > 0 scatters by (1 - t) * the reference BRDF + t * a rough dielectric (GGX, exact Fresnel; reflection
+   untinted, refraction tinted by baseColor; ezrt_math.h, DESIGN.md section 12).  The outside of every mesh is vacuum: a hit
+   from the back of a triangle (geometric normal) leaves the medium of index IOR, so transmissive meshes must be closed and
+   wound outward.  |IOR - 1| <= 2^-8 is an index-matched pass-through; IOR <= 0 or not finite is opaque.  Light samples and
+   shadow rays treat transmissive triangles as opaque: light through glass arrives by BSDF samples only.  A scene without a
+   material of t > 0 renders as without the flag, bit for bit.  Accepted by ezrt_render[_device],
+   ezrt_render_adaptive[_device] and ezrt_render_aov[_device]. */
+#define EZRT_PARAM_TRANSMISSION 4
 
 typedef struct ezrt_counters {
     uint64_t rays;          /* hitBVH invocations: primary + bounce + shadow (SURVEY 8d)     */
@@ -285,6 +295,13 @@ int ezrt_occluded_rays(ezrt_scene* scene, int n, const float* origins, const flo
 int ezrt_eval_brdf(int device, int which, int n, const float* V, const float* N, const float* L,
                    const float* xi, const float* materials, float* out);
 
+/* Evaluate the mixture of EZRT_PARAM_TRANSMISSION (ezrt_math.h, DESIGN.md section 12) on the device for n (V, N, L, inside,
+ * material) tuples (materials: 18 floats each, inside: 1 if the hit is from inside the medium).  out: 8 floats per tuple,
+ * unused ones 0.  which = 0: f (3); 1: pdf (1); 2: the BSDF sample of xi[4 i .. 4 i + 3] = (xi_1, xi_2, xi_3, r_t), L unused:
+ * L (3), the f (3), pdf and signed cosine the path carries, or 8 zeros if the path ends. */
+int ezrt_eval_bsdf(int device, int which, int n, const float* V, const float* N, const float* L, const float* xi,
+                   const int32_t* inside, const float* materials, float* out);
+
 /* Evaluate a ezrt_math.h function on the device for n inputs (parity of the arithmetic
  * definition): which = 0 sin, 1 cos, 2 log, 3 exp, 4 pow(a,b), 5 atan2(a,b), 6 asin. */
 int ezrt_eval_math(int device, int which, int n, const float* a, const float* b, float* out);
@@ -329,7 +346,8 @@ void ezrt_transform_matrix(const float rotate_deg[3], const float translate[3], 
 /* readObj (P5/main.cpp:274-392) incl. its unit-box normalisation quirk (:317-318),
  * transform, smooth-normal generation and per-mesh material (18 floats: emissive,
  * baseColor, subsurface, metallic, specular, specularTint, roughness, anisotropic, sheen,
- * sheenTint, clearcoat, clearcoatGloss, IOR, transmission). */
+ * sheenTint, clearcoat, clearcoatGloss, IOR, transmission).  IOR and transmission are read only by
+ * renders with EZRT_PARAM_TRANSMISSION. */
 int ezrt_trilist_read_obj(ezrt_trilist* list, const char* path, const float material[EZRT_MATERIAL_FLOATS],
                           const float trans[16], int smooth_normal);
 /* smooth_normal is a flag word: bit 0 = smoothNormal; EZRT_OBJ_HARDENED additionally accepts negative

@@ -463,4 +463,133 @@ EZ_HD float ez_env_pdf(const float* texel_pdf, int W, int H, ez_vec3 L) {
     return EZ_DIV(p * (float)(W * H), (2.0f * EZ_PI * EZ_PI) * ce);
 }
 
+/* ------------------------------------------------------------------ transmission (DESIGN.md section 12)
+ * Mode EZRT_MODE_DISNEY_LIGHTS with EZRT_PARAM_TRANSMISSION: a rough dielectric lobe (Walter et al. 2007) beside the reference
+ * BRDF.  At a hit: V = -d, N = the shading normal as the hit returns it (flipped towards V by the geometric test), inside = that
+ * test (dot(Ng, d) > 0: the ray leaves the medium).  The outside is vacuum; eta = eta_L / eta_V = IOR entering, 1 / IOR leaving.
+ *   t = ez_trans_weight(transmission, metallic, IOR).  t == 0: the hit is mode 4's, draws, arithmetic and bits.
+ *   BSDF  f = (1 - t) f_ref + t f_diel,  pdf = (1 - t) pdf_ref + t pdf_diel  (ez_trans_mix), f_ref / pdf_ref = the reference's
+ *         BRDF_Evaluate / BRDF_Pdf where dot(N, L) > 0 and 0 elsewhere; f_diel / pdf_diel = ez_diel_eval.
+ *   alpha = max(0.001, roughness^2); D = the reference's GTR2; G = Smith GGX G1(V) G1(L); F = exact unpolarised Fresnel (TIR: 1).
+ *   reflection (dot(N, L) > 0): h = normalize(V + L),
+ *         f_diel = F D G / (4 |N.V| |N.L|) (untinted),  pdf_diel = F D (N.h) / (4 V.h)
+ *   refraction (dot(N, L) < 0): h = normalize(-(V + eta L)) turned to the N side, den = V.h + eta L.h,
+ *         f_diel = baseColor (1 - F) D G (V.h) |L.h| / (|N.V| |N.L| den^2),  pdf_diel = (1 - F) D (N.h) eta^2 |L.h| / den^2
+ *     This is the radiance convention: f(V, L) / eta_V^2 = f(L, V) / eta_L^2, and a smooth refraction carries (1 - F) / eta^2.
+ *   f_diel = pdf_diel = 0 unless dot(N, V) > 0, N.h > 0, V.h > 0 and L.h on L's side, or where a value is not finite.
+ *   Index-matched (|IOR - 1| <= 2^-8): f_diel is a pass-through, F = 0, L = -V, weight baseColor; it adds nothing to f and pdf
+ *   at any other direction.
+ * Sampling, after mode 4's draws (r_sel, r_1, r_2, the Sobol pair, xi_3): r_t = rand01.
+ *   r_t < t: index-matched: L = d, the path carries (f, pdf, |cos|) = (baseColor, 1, 1); else L = ez_diel_sample(xi, xi_3).
+ *   otherwise: L = SampleBRDF as mode 4, the path ends unless dot(N, L) > 0.
+ *   The path then carries f and pdf of the mixture at L and |dot(N, L)|.  A failed dielectric sample ends the path.
+ * Light samples are evaluated with the mixture at L (dot(N, L) > 0) and MIS-weighted with its pdf.  A BSDF sample with
+ * dot(N, L) < 0 (a refraction or a pass-through) cannot be drawn by a light sample: the emission it hits, or the environment it
+ * leaves to, weighs 1.  The path record keeps this bit as the sign of its cosine. */
+#define EZ_TRANS_MATCHED 0.00390625f   /* 2^-8 */
+/* the weight of the dielectric lobe: clamp(transmission, 0, 1) * (1 - metallic), clamped to [0, 1]; 0 if transmission or the
+ * product is not finite, or IOR is not finite or <= 0 (opaque) */
+EZ_HD float ez_trans_weight(float transmission, float metallic, float IOR) {
+    if (!ez_finite(transmission) || !ez_finite(IOR) || !(IOR > 0.0f)) return 0.0f;
+    const float t = ez_clamp(transmission, 0.0f, 1.0f) * (1.0f - metallic);
+    return (ez_finite(t) && t > 0.0f) ? ez_min(t, 1.0f) : 0.0f;
+}
+/* eta = eta_L / eta_V of a refraction from V's side: IOR entering, 1 / IOR leaving (inside) */
+EZ_HD float ez_trans_eta(float IOR, int inside) { return inside ? EZ_DIV(1.0f, IOR) : IOR; }
+EZ_HD int ez_trans_matched(float IOR) { return ez_abs(IOR - 1.0f) <= EZ_TRANS_MATCHED; }
+/* the exact unpolarised Fresnel reflectance at cos_i = |V.h| for the relative index eta; total internal reflection gives 1 */
+EZ_HD float ez_fresnel_dielectric(float cos_i, float eta) {
+    const float c = ez_min(ez_abs(cos_i), 1.0f);
+    const float s2 = EZ_DIV(1.0f - c * c, eta * eta);
+    if (!(s2 < 1.0f)) return 1.0f;
+    const float ct = EZ_SQRT(1.0f - s2);
+    const float rs = EZ_DIV(c - eta * ct, c + eta * ct);
+    const float rp = EZ_DIV(eta * c - ct, eta * c + ct);
+    return 0.5f * (rs * rs + rp * rp);
+}
+/* the reference's GTR2 (GGX D) */
+EZ_HD float ez_ggx_D(float NdotH, float a) {
+    const float a2 = a * a;
+    const float t = 1.0f + (a2 - 1.0f) * NdotH * NdotH;
+    return EZ_DIV(a2, EZ_PI * t * t);
+}
+/* Smith GGX masking of one direction at cosine c > 0: 2 c / (c + sqrt(a^2 + c^2 - a^2 c^2)) */
+EZ_HD float ez_ggx_G1(float c, float a) {
+    const float a2 = a * a, c2 = c * c;
+    return EZ_DIV(2.0f * c, c + EZ_SQRT(a2 + c2 - a2 * c2));
+}
+/* the reference's toNormalHemisphere */
+EZ_HD ez_vec3 ez_to_normal_hemisphere(ez_vec3 v, ez_vec3 N) {
+    ez_vec3 helper = ez_v3(1.0f, 0.0f, 0.0f);
+    if (ez_abs(N.x) > 0.999f) helper = ez_v3(0.0f, 0.0f, 1.0f);
+    const ez_vec3 tangent = ez_normalize(ez_cross(N, helper));
+    const ez_vec3 bitangent = ez_normalize(ez_cross(N, tangent));
+    return ez_add(ez_add(ez_scale(tangent, v.x), ez_scale(bitangent, v.y)), ez_scale(N, v.z));
+}
+/* the reference's GTR2 half-vector law (SampleGTR2 before its reflection): density D(h) (N.h) */
+EZ_HD ez_vec3 ez_ggx_half(float xi_1, float xi_2, ez_vec3 N, float a) {
+    const float phi_h = 2.0f * EZ_PI * xi_1;
+    const float sin_phi_h = ez_sin(phi_h), cos_phi_h = ez_cos(phi_h);
+    const float cos_theta_h = EZ_SQRT(EZ_DIV(1.0f - xi_2, 1.0f + (a * a - 1.0f) * xi_2));
+    const float sin_theta_h = EZ_SQRT(ez_max(0.0f, 1.0f - cos_theta_h * cos_theta_h));
+    return ez_to_normal_hemisphere(ez_v3(sin_theta_h * cos_phi_h, sin_theta_h * sin_phi_h, cos_theta_h), N);
+}
+/* f_diel(V, L) of unit vectors (rough lobe; not for the index-matched case) and its density *pdf */
+EZ_HD ez_vec3 ez_diel_eval(ez_vec3 V, ez_vec3 N, ez_vec3 L, ez_vec3 baseColor, float a, float eta, float* pdf) {
+    const ez_vec3 zero = ez_v3(0.0f, 0.0f, 0.0f);
+    *pdf = 0.0f;
+    const float NdotV = ez_dot(N, V), NdotL = ez_dot(N, L);
+    if (!(NdotV > 0.0f) || !(NdotL != 0.0f) || !ez_finite(NdotL)) return zero;
+    const int refr = NdotL < 0.0f;
+    ez_vec3 H = ez_normalize(refr ? ez_neg(ez_add(V, ez_scale(L, eta))) : ez_add(V, L));
+    float NdotH = ez_dot(N, H);
+    if (NdotH < 0.0f) { H = ez_neg(H); NdotH = -NdotH; }
+    const float VdotH = ez_dot(V, H), LdotH = ez_dot(L, H);
+    if (!(NdotH > 0.0f) || !(VdotH > 0.0f) || (refr ? !(LdotH < 0.0f) : !(LdotH > 0.0f))) return zero;
+    const float F = ez_fresnel_dielectric(VdotH, eta);
+    const float D = ez_ggx_D(NdotH, a);
+    const float G = ez_ggx_G1(NdotV, a) * ez_ggx_G1(ez_abs(NdotL), a);
+    float f, p;
+    if (!refr) {
+        f = EZ_DIV(F * D * G, 4.0f * NdotV * NdotL);
+        p = EZ_DIV(F * D * NdotH, 4.0f * VdotH);
+    } else {
+        const float T = 1.0f - F, aL = ez_abs(LdotH);
+        const float den = VdotH + eta * LdotH;
+        const float den2 = den * den;
+        if (!(T > 0.0f) || !(den2 > 0.0f)) return zero;
+        f = EZ_DIV(T * D * G * VdotH * aL, NdotV * ez_abs(NdotL) * den2);
+        p = EZ_DIV(T * D * NdotH * (eta * eta) * aL, den2);
+    }
+    if (!ez_finite(f) || !ez_finite(p) || !(p > 0.0f)) return zero;
+    *pdf = p;
+    return refr ? ez_scale(baseColor, f) : ez_v3(f, f, f);
+}
+/* the dielectric lobe's sample: h by ez_ggx_half(xi_1, xi_2), reflect if xi_3 < F(V.h), refract otherwise.  Returns 1 with *L,
+ * or 0 (the path ends) if dot(N, V) <= 0, V.h <= 0, or L lands on the wrong side of N for its lobe */
+EZ_HD int ez_diel_sample(float xi_1, float xi_2, float xi_3, ez_vec3 V, ez_vec3 N, float a, float eta, ez_vec3* L) {
+    if (!(ez_dot(N, V) > 0.0f)) return 0;
+    const ez_vec3 H = ez_ggx_half(xi_1, xi_2, N, a);
+    const float VdotH = ez_dot(V, H);
+    if (!(VdotH > 0.0f)) return 0;
+    const float F = ez_fresnel_dielectric(VdotH, eta);
+    if (xi_3 < F) {
+        *L = ez_reflect(ez_neg(V), H);
+        return ez_dot(N, *L) > 0.0f;
+    }
+    /* F < 1: no total internal reflection, s2 < 1 as in ez_fresnel_dielectric */
+    const float c = ez_min(VdotH, 1.0f);
+    const float s2 = EZ_DIV(1.0f - c * c, eta * eta);
+    const float ct = EZ_SQRT(1.0f - s2);
+    const float ie = EZ_DIV(1.0f, eta);
+    *L = ez_normalize(ez_add(ez_scale(V, -ie), ez_scale(H, ie * c - ct)));
+    return ez_dot(N, *L) < 0.0f;
+}
+/* the mixture: f = (1 - t) f_ref + t f_diel, *pdf = (1 - t) pdf_ref + t pdf_diel */
+EZ_HD ez_vec3 ez_trans_mix(ez_vec3 f_ref, float pdf_ref, ez_vec3 f_diel, float pdf_diel, float t, float* pdf) {
+    const float s = 1.0f - t;
+    *pdf = s * pdf_ref + t * pdf_diel;
+    return ez_add(ez_scale(f_ref, s), ez_scale(f_diel, t));
+}
+
 #endif /* EZRT_MATH_H */
