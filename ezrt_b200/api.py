@@ -391,6 +391,13 @@ class Scene:
         check(lib.ezrt_get_kernel_times(self._h, ms, n))
         return {k: (ms[i], int(n[i])) for i, k in enumerate(("extend", "shade", "shadow", "other"))}
 
+    def w8_phase_cycles(self):
+        """{pass: {phase: SM cycles summed over warps}} of the last render with cfg.profile = 2 (ezrt_get_w8_phase_cycles)."""
+        c = (C.c_uint64 * 8)()
+        check(lib.ezrt_get_w8_phase_cycles(self._h, c))
+        phases = ("refill", "node", "triangle", "ray_end")
+        return {k: {ph: int(c[4 * i + j]) for j, ph in enumerate(phases)} for i, k in enumerate(("k_extend_w8", "k_shadow_w8"))}
+
     def trace_rays(self, origins, dirs, traverse=TRAVERSE_ACCEL, any_hit=False, p3_normal_fudge=False):
         """hitBVH for n rays on the device (P5/fsh:254-306)."""
         o = _f32(origins, (-1, 3))

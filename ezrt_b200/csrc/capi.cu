@@ -900,7 +900,7 @@ static int render_device_impl(ezrt_scene* s, const ezrt_render_params* p, float*
     CU_CHECK(cudaSetDevice(s->device));
     int rc = prepare_tiles(s, p, st);
     if (rc) return rc;
-    rc = s->totals_buf.ensure(sizeof(unsigned long long) * 8);
+    rc = s->totals_buf.ensure(sizeof(unsigned long long) * EZRT_TOTALS);
     if (rc) return rc;
     unsigned long long* totals = (unsigned long long*)s->totals_buf.p;
     // EZRT_PARAM_ACCUMULATE: counters, kernel spans and the device-time bracket continue from the previous render
@@ -908,7 +908,7 @@ static int render_device_impl(ezrt_scene* s, const ezrt_render_params* p, float*
     const bool accumulate = (p->reserved[0] & EZRT_PARAM_ACCUMULATE) != 0 && s->have_timing;
     if (!accumulate) {
         CU_CHECK(cudaEventRecord(s->ev_start, st));
-        CU_CHECK(cudaMemsetAsync(totals, 0, sizeof(unsigned long long) * 8, st));
+        CU_CHECK(cudaMemsetAsync(totals, 0, sizeof(unsigned long long) * EZRT_TOTALS, st));
         s->launches = 0;
         s->spans.clear();
         s->ev_used = 0;
@@ -1369,6 +1369,17 @@ int ezrt_get_counters(ezrt_scene* s, ezrt_counters* out) {
     out->samples = t[3];
     out->kernel_launches = s->launches;
     out->device_ms = ms;
+    return EZRT_OK;
+}
+
+int ezrt_get_w8_phase_cycles(ezrt_scene* s, uint64_t* out) {
+    if (!s || !out) return ezrt_set_error(EZRT_ERR_INVALID, "get_w8_phase_cycles: null argument");
+    for (int k = 0; k < 8; k++) out[k] = 0;
+    if (!s->have_timing) return EZRT_OK;
+    CU_CHECK(cudaSetDevice(s->device));
+    CU_CHECK(cudaEventSynchronize(s->ev_stop));
+    static_assert(EZRT_W8_PHASES_SHADOW == EZRT_W8_PHASES_EXTEND + 4 && 5 + EZRT_W8_PHASES_SHADOW + 4 <= EZRT_TOTALS, "totals layout");
+    CU_CHECK(cudaMemcpy(out, (unsigned long long*)s->totals_buf.p + 5 + EZRT_W8_PHASES_EXTEND, sizeof(uint64_t) * 8, cudaMemcpyDeviceToHost));
     return EZRT_OK;
 }
 

@@ -548,8 +548,8 @@ __device__ __forceinline__ bool reference_reaches_leaf(const int* __restrict__ t
     return d > 0.0f;
 }
 
-__device__ __forceinline__ bool reference_reaches_leaf_inv(const int* __restrict__ tri_leaf, const float4* __restrict__ leaf_box, int tri, vec3 o, vec3 inv) {
-    const int leaf = __ldg(tri_leaf + tri);
+// the same test on a leaf index the caller fetched earlier (tri_leaf[tri]), so that the two dependent loads need not be waited on together
+__device__ __forceinline__ bool reference_reaches_leaf_box(const float4* __restrict__ leaf_box, int leaf, vec3 o, vec3 inv) {
     const float4 a = ldg4(leaf_box + 2 * (size_t)leaf), b = ldg4(leaf_box + 2 * (size_t)leaf + 1);
     float fx = (b.x - o.x) * inv.x, fy = (b.y - o.y) * inv.y, fz = (b.z - o.z) * inv.z;
     float nx = (a.x - o.x) * inv.x, ny = (a.y - o.y) * inv.y, nz = (a.z - o.z) * inv.z;
@@ -557,6 +557,10 @@ __device__ __forceinline__ bool reference_reaches_leaf_inv(const int* __restrict
     float t0 = fmaxf(fminf(fx, nx), fmaxf(fminf(fy, ny), fminf(fz, nz)));
     float d = (t1 >= t0) ? ((t0 > 0.0f) ? t0 : t1) : -1.0f;
     return d > 0.0f;
+}
+
+__device__ __forceinline__ bool reference_reaches_leaf_inv(const int* __restrict__ tri_leaf, const float4* __restrict__ leaf_box, int tri, vec3 o, vec3 inv) {
+    return reference_reaches_leaf_box(leaf_box, __ldg(tri_leaf + tri), o, inv);
 }
 
 // ACCEL: `tree` is the device's own acceleration tree, not the reference tree: the closest hit it
@@ -933,13 +937,22 @@ __device__ __forceinline__ int nth_set_bit(uint32_t m, int r) {
     return pos + ((r >= (int)(m & 1u)) ? 1 : 0);
 }
 
+// SM clock for the phase sums of the COUNT instantiations; the memory clobber keeps the compiler from moving loads and stores across it
+__device__ __forceinline__ uint32_t w8_clock() {
+    uint32_t t;
+    asm volatile("mov.u32 %0, %%clock;" : "=r"(t) : : "memory");
+    return t;
+}
+
 // s_perm: 8 x 256 bytes in shared memory, s_perm[m * 256 + x] = the bits of x moved from position s to position s ^ m
 // stack : uint2 [entries][blockDim.x] in shared memory
 // IDX: the scene's triangle records are indexed (SceneDev::acc_tri_indexed; one instantiation per layout keeps each within 64
 // registers without spilling)
+#define W8_ENDED (-2)   // extend_w8: `node` of a lane whose ray is traced and waits for its leaf check at the next refill
+// phase_cycles (COUNT only): += the SM cycles each warp spends in [0] refill, [1] node steps, [2] triangle steps, [3] ray ends
 template <bool ANYHIT, bool COUNT, bool IDX, bool BOUNDED = false, class RayIO>
 __device__ __forceinline__ void extend_w8(const SceneDev& sc, uint32_t n, uint32_t* work, RayIO io, const unsigned char* s_perm, uint2* stack_sm,
-                                          W8Counts counts) {
+                                          W8Counts counts, unsigned long long* phase_cycles) {
     const bool tri_na = sc.tri_l1_bypass != 0;
     const int refill_thresh = sc.refill_thresh, leaf_thresh = sc.w8_tri_weight;
     const unsigned FULL = 0xffffffffu;
@@ -956,7 +969,8 @@ __device__ __forceinline__ void extend_w8(const SceneDev& sc, uint32_t n, uint32
     unsigned char* const s_owner = s_owner_all + (threadIdx.x & ~31u);
 
     int ray = -1;                 // index of the ray this lane traces, -1 = idle
-    int node = -1;                // next node to visit, -1 = none (waiting for the triangle phase, or idle)
+    int node = -1;                // next node to visit, -1 = none (waiting for the triangle phase, or idle), W8_ENDED = ray traced
+    int end_leaf = 0;             // W8_ENDED: reference leaf of best_tri, loaded at the ray's end and first read at the next refill
     int sp = 0;
     vec3 o = splat3(0.0f), d = splat3(0.0f), inv = splat3(0.0f);
     float slack = 0.0f, best = EZ_INF;
@@ -966,6 +980,8 @@ __device__ __forceinline__ void extend_w8(const SceneDev& sc, uint32_t n, uint32
     uint32_t g_base = 0, g_bits = 0;   // current group: first inner child | imask (bits 0..7), unvisited hit slots in priority positions (bits 8..15)
     uint32_t t_base = 0, t_mask = 0;   // pending triangles of the node just visited
     uint32_t n_visits = 0, n_tests = 0;   // per lane; 32 bits keep the COUNT instantiations within 64 registers
+    uint32_t cyc_refill = 0, cyc_node = 0, cyc_tri = 0, cyc_end = 0;   // COUNT: the warp's phase sums (phase_cycles)
+    uint32_t end_dt = 0, t_mark = COUNT ? w8_clock() : 0u;             // COUNT: this lane's ray-end span; end of the last phase
     bool exhausted = false;
     uint32_t chunk_pos = 0, chunk_end = 0;
     const uint32_t chunk = (uint32_t)sc.work_chunk;
@@ -973,15 +989,16 @@ __device__ __forceinline__ void extend_w8(const SceneDev& sc, uint32_t n, uint32
 #define W8_PUSH(e) do { const uint2 e__ = (e); if (sp < stack_cap) my_stack[sp * stack_stride] = e__; else stack_local[sp - stack_cap] = e__; ++sp; } while (0)
 #define W8_POP() ((--sp < stack_cap) ? my_stack[sp * stack_stride] : stack_local[sp - stack_cap])
     // next node of this lane's ray from the current group / the stack; finishes the ray when nothing is left
+    // A finished ray's leaf check (io.store) is two dependent loads.  Waited on where the ray ends, they would stall every lane of
+    // the warp in most steps; so the ray only issues the first load here and becomes W8_ENDED (no longer busy, not yet idle), and
+    // the next refill, which waits on memory anyway, finishes it with io.finish before it takes a new ray.
     auto select_next = [&]() {
         if ((g_bits >> 8) == 0u) {
             if (sp == 0) {  // ray finished
-                HitRec h;
-                h.t = best;
-                h.tri = best_tri;
-                io.store((uint32_t)ray, h, tie, o, d, inv);
-                ray = -1;
-                node = -1;
+                const uint32_t te = COUNT ? w8_clock() : 0u;
+                if (best_tri >= 0) end_leaf = io.leaf_of(best_tri);
+                if (COUNT) end_dt = w8_clock() - te;
+                node = W8_ENDED;
                 return;
             }
             const uint2 e = W8_POP();
@@ -996,11 +1013,23 @@ __device__ __forceinline__ void extend_w8(const SceneDev& sc, uint32_t n, uint32
 
     while (true) {
         // ---------------- refill idle lanes (per-warp chunks of the global work counter, as extend_persistent) ----------------
-        unsigned need = __ballot_sync(FULL, ray < 0);
+        const bool ended = node == W8_ENDED;
+        const unsigned need = __ballot_sync(FULL, ray < 0 || ended);
+        const bool claim = need != 0u && !exhausted && chunk_pos >= chunk_end;
+        uint32_t base = 0;
+        if (claim && lane == 0) base = atomicAdd(work, chunk);   // issued before the leaf checks, so that their round trips overlap
+        if (ended) {
+            HitRec h;
+            h.t = best;
+            h.tri = best_tri;
+            const uint32_t te = COUNT ? w8_clock() : 0u;
+            io.finish((uint32_t)ray, h, tie, o, d, inv, end_leaf);
+            if (COUNT) end_dt = w8_clock() - te;
+            ray = -1;
+            node = -1;
+        }
         if (need != 0u && !exhausted) {
-            if (chunk_pos >= chunk_end) {
-                uint32_t base = 0;
-                if (lane == 0) base = atomicAdd(work, chunk);
+            if (claim) {
                 base = __shfl_sync(FULL, base, 0);
                 chunk_pos = base;
                 chunk_end = (base + chunk < n) ? base + chunk : n;
@@ -1035,6 +1064,13 @@ __device__ __forceinline__ void extend_w8(const SceneDev& sc, uint32_t n, uint32
                 chunk_pos = (chunk_pos + take < chunk_end) ? chunk_pos + take : chunk_end;
             }
         }
+        if (COUNT) {
+            const uint32_t now = w8_clock(), e = __reduce_max_sync(FULL, end_dt);   // the leaf checks of the ended rays run side by side
+            end_dt = 0u;
+            cyc_end += e;
+            cyc_refill += now - t_mark - e;
+            t_mark = now;
+        }
         if (__ballot_sync(FULL, ray >= 0) == 0u) {
             if (exhausted) break;
             continue;
@@ -1053,7 +1089,8 @@ __device__ __forceinline__ void extend_w8(const SceneDev& sc, uint32_t n, uint32
             const unsigned m_node = __ballot_sync(FULL, at_node);
             const uint32_t pairs = __reduce_add_sync(FULL, (uint32_t)__popc(t_mask));
             if (m_node == 0u && pairs == 0u) { busy = 0u; break; }
-            if (m_node != 0u && tri_weight * (int)min(pairs, 32u) < __popc(m_node)) {
+            const bool node_step = m_node != 0u && tri_weight * (int)min(pairs, 32u) < __popc(m_node);
+            if (node_step) {
                 if (at_node) {
                     // the 20 words of the record (w8_node.h): h = w0..3, c = w4..7, l = w8..11, m = w12..15, u = w16..19
                     const uint4* nd = nodes + (size_t)node * (W8_NODE_WORDS / 4);
@@ -1193,7 +1230,15 @@ __device__ __forceinline__ void extend_w8(const SceneDev& sc, uint32_t n, uint32
                     if (t_mask == 0u) select_next();
                 }
             }
-            busy = __ballot_sync(FULL, ray >= 0);
+            busy = __ballot_sync(FULL, ray >= 0 && node != W8_ENDED);
+            if (COUNT) {
+                const uint32_t now = w8_clock(), e = __reduce_max_sync(FULL, end_dt);   // the ray ends of a step run side by side
+                end_dt = 0u;
+                cyc_end += e;
+                if (node_step) cyc_node += now - t_mark - e;
+                else cyc_tri += now - t_mark - e;
+                t_mark = now;
+            }
         } while (busy != 0u && (exhausted || __popc(busy) >= refill_thresh));
     }
 #undef W8_PUSH
@@ -1201,6 +1246,12 @@ __device__ __forceinline__ void extend_w8(const SceneDev& sc, uint32_t n, uint32
     if (COUNT) {
         atomicAdd(counts.node_visits, (unsigned long long)n_visits);
         atomicAdd(counts.tri_tests, (unsigned long long)n_tests);
+        if (lane == 0) {
+            atomicAdd(phase_cycles + 0, (unsigned long long)cyc_refill);
+            atomicAdd(phase_cycles + 1, (unsigned long long)cyc_node);
+            atomicAdd(phase_cycles + 2, (unsigned long long)cyc_tri);
+            atomicAdd(phase_cycles + 3, (unsigned long long)cyc_end);
+        }
     }
 }
 

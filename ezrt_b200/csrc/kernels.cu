@@ -338,6 +338,15 @@ struct AccelExtendIO {
         }
         __stcs(q.hit + (perm ? perm[i] : i), make_float2(h.t, __int_as_float(h.tri)));  // accel-order triangle index
     }
+    // store() in two halves (extend_w8): leaf_of(h.tri) when the ray ends, finish() with its result at a later refill
+    __device__ __forceinline__ int leaf_of(int tri) const { return __ldg(acc_tri_leaf + tri); }
+    __device__ __forceinline__ void finish(uint32_t i, HitRec h, bool tie, vec3 o, vec3 d, vec3 inv, int leaf) const {
+        if (h.tri >= 0 && (tie || !reference_reaches_leaf_box(leaf_box, leaf, o, inv))) {
+            defer(i, o, d);
+            return;
+        }
+        __stcs(q.hit + (perm ? perm[i] : i), make_float2(h.t, __int_as_float(h.tri)));
+    }
 };
 
 // Camera pass with the ray generation fused in (main(), P5/fsh:920-925): ray `i` IS sample slot i, generated in the
@@ -409,7 +418,8 @@ __global__ void __launch_bounds__(EZRT_EXTEND_MAX_THREADS, EZRT_EXTEND_LB_BLOCKS
 
 template <bool COUNT, bool IDX>
 __global__ void __launch_bounds__(EZRT_EXTEND_MAX_THREADS, EZRT_EXTEND_LB_BLOCKS) k_extend_w8(SceneDev sc, PathQueue q, const uint32_t* __restrict__ q_count, uint32_t* work,
-                                                                   uint32_t* defer_list, uint32_t* defer_count, W8Counts counts, const uint32_t* __restrict__ perm) {
+                                                                   uint32_t* defer_list, uint32_t* defer_count, W8Counts counts, const uint32_t* __restrict__ perm,
+                                                                   unsigned long long* phase_cycles) {
     unsigned char* s_perm;
     uint2* stack_sm;
     w8_smem_setup(s_perm, stack_sm);
@@ -420,7 +430,7 @@ __global__ void __launch_bounds__(EZRT_EXTEND_MAX_THREADS, EZRT_EXTEND_LB_BLOCKS
     io.defer_list = defer_list;
     io.defer_count = defer_count;
     io.perm = perm;
-    extend_w8<false, COUNT, IDX>(sc, *q_count, work, io, s_perm, stack_sm, counts);
+    extend_w8<false, COUNT, IDX>(sc, *q_count, work, io, s_perm, stack_sm, counts, phase_cycles);
 }
 
 struct AccelShadowIO {
@@ -441,11 +451,18 @@ struct AccelShadowIO {
         if (!reference_reaches_leaf_inv(acc_tri_leaf, leaf_box, h.tri, o, inv)) defer(i, o, d);
         else base.mark(i, false);
     }
+    __device__ __forceinline__ int leaf_of(int tri) const { return __ldg(acc_tri_leaf + tri); }
+    __device__ __forceinline__ void finish(uint32_t i, HitRec h, bool, vec3 o, vec3 d, vec3 inv, int leaf) const {
+        if (h.tri < 0) base.mark(i, true);
+        else if (!reference_reaches_leaf_box(leaf_box, leaf, o, inv)) defer(i, o, d);
+        else base.mark(i, false);
+    }
 };
 
 template <bool COUNT, bool IDX, bool BOUNDED = false>
 __global__ void __launch_bounds__(EZRT_EXTEND_MAX_THREADS, EZRT_EXTEND_LB_BLOCKS) k_shadow_w8(SceneDev sc, ShadowQueue sq, const uint32_t* __restrict__ s_count, uint32_t* work,
-                                                                   float4* __restrict__ Lo, uint32_t* defer_list, uint32_t* defer_count, W8Counts counts) {
+                                                                   float4* __restrict__ Lo, uint32_t* defer_list, uint32_t* defer_count, W8Counts counts,
+                                                                   unsigned long long* phase_cycles) {
     unsigned char* s_perm;
     uint2* stack_sm;
     w8_smem_setup(s_perm, stack_sm);
@@ -457,7 +474,7 @@ __global__ void __launch_bounds__(EZRT_EXTEND_MAX_THREADS, EZRT_EXTEND_LB_BLOCKS
     io.leaf_box = sc.leaf_box;
     io.defer_list = defer_list;
     io.defer_count = defer_count;
-    extend_w8<true, COUNT, IDX, BOUNDED>(sc, *s_count, work, io, s_perm, stack_sm, counts);
+    extend_w8<true, COUNT, IDX, BOUNDED>(sc, *s_count, work, io, s_perm, stack_sm, counts, phase_cycles);
 }
 
 // ---- the same three passes on the 4-wide exact-box tree (default form, env EZRT_ACCEL): extend_persistent<ACCEL, WIDE>
@@ -1216,7 +1233,8 @@ void launch_extend_accel(const SceneDev& sc, PathQueue q, const uint32_t* q_coun
         W8Counts c;
         c.node_visits = counts ? counts + 2 : nullptr;   // 96-byte records
         c.tri_tests = counts ? counts + 1 : nullptr;
-#define EZRT_LAUNCH_W8(C, I) k_extend_w8<C, I><<<blocks, threads, w8_smem_for(k_extend_w8<C, I>, sc), st>>>(sc, q, q_count, work, defer_list, defer_count, c, perm)
+        unsigned long long* const cyc = counts ? counts + EZRT_W8_PHASES_EXTEND : nullptr;
+#define EZRT_LAUNCH_W8(C, I) k_extend_w8<C, I><<<blocks, threads, w8_smem_for(k_extend_w8<C, I>, sc), st>>>(sc, q, q_count, work, defer_list, defer_count, c, perm, cyc)
         if (sc.acc_tri_indexed) { if (counts) EZRT_LAUNCH_W8(true, true); else EZRT_LAUNCH_W8(false, true); }
         else { if (counts) EZRT_LAUNCH_W8(true, false); else EZRT_LAUNCH_W8(false, false); }
 #undef EZRT_LAUNCH_W8
@@ -1281,7 +1299,8 @@ static void launch_shadow_accel_t(const SceneDev& sc, ShadowQueue sq, const uint
         W8Counts c;
         c.node_visits = counts ? counts + 2 : nullptr;
         c.tri_tests = counts ? counts + 1 : nullptr;
-#define EZRT_LAUNCH_W8(C, I) k_shadow_w8<C, I, B><<<blocks, threads, w8_smem_for(k_shadow_w8<C, I, B>, sc), st>>>(sc, sq, s_count, work, Lo, defer_list, defer_count, c)
+        unsigned long long* const cyc = counts ? counts + EZRT_W8_PHASES_SHADOW : nullptr;
+#define EZRT_LAUNCH_W8(C, I) k_shadow_w8<C, I, B><<<blocks, threads, w8_smem_for(k_shadow_w8<C, I, B>, sc), st>>>(sc, sq, s_count, work, Lo, defer_list, defer_count, c, cyc)
         if (sc.acc_tri_indexed) { if (counts) EZRT_LAUNCH_W8(true, true); else EZRT_LAUNCH_W8(false, true); }
         else { if (counts) EZRT_LAUNCH_W8(true, false); else EZRT_LAUNCH_W8(false, false); }
 #undef EZRT_LAUNCH_W8

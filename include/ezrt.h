@@ -248,6 +248,11 @@ int ezrt_get_counters(ezrt_scene* scene, ezrt_counters* out);
  * 2 shadow (hitBVH, any hit), 3 other (generate, blend, tally).  ms[4], launches[4]. */
 int ezrt_get_kernel_times(ezrt_scene* scene, double* ms, uint64_t* launches);
 
+/* SM cycles the 8-wide accel kernels' warps spent per phase in the most recent render with params.profile = 2 (synchronises),
+ * summed over warps: out[0..3] the bounce pass (k_extend_w8), out[4..7] the shadow pass (k_shadow_w8), each as refill, node
+ * steps, triangle steps, ray ends.  All 0 for scenes traced without the 8-wide tree.  out[8]. */
+int ezrt_get_w8_phase_cycles(ezrt_scene* scene, uint64_t* out);
+
 /* Number of pixels part `rank` of `count` owns for a width x height image. */
 int64_t ezrt_partition_pixels(int width, int height, int rank, int count);
 /* Device kernel: scatter the compact tile-major buffer of part `rank` into a full
