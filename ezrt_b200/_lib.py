@@ -81,6 +81,7 @@ SIGNATURES = {
     "ezrt_occluded_rays": (C.c_int, [C.c_void_p, C.c_int, c_float_p, c_float_p, c_float_p, C.c_int, c_int32_p]),
     "ezrt_eval_brdf": (C.c_int, [C.c_int, C.c_int, C.c_int, c_float_p, c_float_p, c_float_p, c_float_p, c_float_p, c_float_p]),
     "ezrt_eval_bsdf": (C.c_int, [C.c_int, C.c_int, C.c_int, c_float_p, c_float_p, c_float_p, c_float_p, c_int32_p, c_float_p, c_float_p]),
+    "ezrt_camera_rays": (C.c_int, [C.c_void_p, C.POINTER(RenderParams), C.c_int, c_uint32_p, c_uint32_p, c_uint32_p, c_float_p, c_float_p]),
     "ezrt_eval_math": (C.c_int, [C.c_int, C.c_int, C.c_int, c_float_p, c_float_p, c_float_p]),
     "ezrt_post_tonemap": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int64, C.c_float, C.c_void_p]),
     "ezrt_write_png": (C.c_int, [C.c_char_p, c_float_p, C.c_int, C.c_int, C.c_int, C.c_int]),
@@ -100,6 +101,7 @@ SIGNATURES = {
     "ezrt_hdr_cache": (C.c_int, [c_float_p, C.c_int, C.c_int, c_float_p]),
     "ezrt_hdr_cache_device": (C.c_int, [C.c_int, c_float_p, C.c_int, C.c_int, c_float_p, C.POINTER(C.c_double)]),
     "ezrt_camera_orbit": (None, [C.c_float, C.c_float, C.c_float, c_float_p, c_float_p]),
+    "ezrt_camera_look_at": (C.c_int, [c_float_p, c_float_p, c_float_p, C.c_float, C.c_float, c_float_p]),
 }
 
 

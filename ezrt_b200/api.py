@@ -22,6 +22,7 @@ MODE_DISNEY_LIGHTS = 4   # BRDF sampling + light sampling on the emissive triang
 PARAM_ACCUMULATE = 1   # ezrt_render_params.reserved[0] flags (include/ezrt.h)
 PARAM_ENV_LIGHT = 2
 PARAM_TRANSMISSION = 4
+PARAM_THIN_LENS = 8
 MODES = {"diffuse_p3": 0, "disney_aniso_p4": 1, "disney_sobol_p5": 2, "disney_is_mis_p5": 3, "disney_lights": 4}
 
 TRAVERSE_ACCEL = 0
@@ -86,6 +87,15 @@ def camera_orbit(rotate_angle=0.0, up_angle=0.0, r=4.0):
     cam = np.zeros(16, dtype=np.float32)
     lib.ezrt_camera_orbit(float(rotate_angle), float(up_angle), float(r), _fp(eye), _fp(cam))
     return eye, cam
+
+
+def camera_look_at(eye, target=(0.0, 0.0, 0.0), up=(0.0, 1.0, 0.0), vfov=67.38013505195957, aspect=1.0):
+    """(eye, cameraRotate) of a look-at camera with a vertical field of view vfov (degrees) and aspect = width / height
+    (ezrt_camera_look_at).  The default vfov, 2 atan(2/3), is the pinhole's own: camera_orbit's view."""
+    e = _f32(eye, (3,))
+    cam = np.zeros(16, dtype=np.float32)
+    check(lib.ezrt_camera_look_at(_fp(e), _fp(_f32(target, (3,))), _fp(_f32(up, (3,))), float(vfov), float(aspect), _fp(cam)))
+    return e.copy(), cam
 
 
 class TriangleList:
@@ -218,6 +228,8 @@ class RenderConfig:
     accumulate: bool = False   # EZRT_PARAM_ACCUMULATE: counters / kernel times continue from the previous render
     env_light: bool = False    # EZRT_PARAM_ENV_LIGHT (MODE_DISNEY_LIGHTS only): the HDR map is one more light (DESIGN.md section 11)
     transmission: bool = False  # EZRT_PARAM_TRANSMISSION (MODE_DISNEY_LIGHTS only): materials' IOR and transmission (DESIGN.md section 12)
+    lens_radius: float = 0.0    # != 0: EZRT_PARAM_THIN_LENS, a thin-lens camera of this radius (DESIGN.md section 13); must be > 0
+    focus_distance: float = None  # ... focused at this depth along the view (-column 2 of camera_rotate); required with a lens
 
     def to_struct(self):
         p = RenderParams()
@@ -231,6 +243,11 @@ class RenderConfig:
         p.profile = int(self.profile)
         p.reserved[0] = ((PARAM_ACCUMULATE if self.accumulate else 0) | (PARAM_ENV_LIGHT if self.env_light else 0) |
                          (PARAM_TRANSMISSION if self.transmission else 0))
+        if self.lens_radius != 0:   # a negative or NaN radius is set too, so that the library rejects it
+            if self.focus_distance is None:
+                raise ValueError("RenderConfig: a lens (lens_radius != 0) needs a focus_distance")
+            p.reserved[0] |= PARAM_THIN_LENS
+            p.reserved[1], p.reserved[2] = (int(x) for x in np.array([self.lens_radius, self.focus_distance], np.float32).view(np.int32))
         return p
 
 
@@ -409,6 +426,19 @@ class Scene:
         check(lib.ezrt_trace_rays(self._h, n, _fp(o), _fp(d), int(traverse), int(bool(any_hit)), int(bool(p3_normal_fudge)),
                                   ip(hit), _fp(dist), ip(tri), ip(inside), _fp(point), _fp(normal)))
         return dict(hit=hit, distance=dist, triangle=tri, inside=inside, point=point, normal=normal)
+
+    def camera_rays(self, cfg, px, py, frame):
+        """ezrt_camera_rays: the render's camera rays (pinhole, or cfg's thin lens) of the samples (px[i], py[i], frame[i]) of
+        cfg's image -> (origins [n, 3], dirs [n, 3]) float32.  For parity tests."""
+        u = lambda a: np.ascontiguousarray(a, dtype=np.uint32).reshape(-1)
+        px, py, frame = u(px), u(py), u(frame)
+        n = px.size
+        assert py.size == n and frame.size == n
+        o, d = np.zeros((n, 3), np.float32), np.zeros((n, 3), np.float32)
+        p = cfg.to_struct()
+        up = lambda a: a.ctypes.data_as(_lib.c_uint32_p)
+        check(lib.ezrt_camera_rays(self._h, C.byref(p), n, up(px), up(py), up(frame), _fp(o), _fp(d)))
+        return o, d
 
     def lights(self):
         """The light table of MODE_DISNEY_LIGHTS (ezrt_scene_lights; built at the first call or render in that mode):

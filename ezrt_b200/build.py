@@ -214,6 +214,23 @@ def build_oracle_transmission(force=False):
     return ORACLE_TRANSMISSION_SO
 
 
+ORACLE_LENS_SO = os.path.join(ROOT, "build", "libezrt_oracle_lens.so")
+
+
+def build_oracle_lens(force=False):
+    """build/libezrt_oracle_lens.so: tests/oracle_lens.cpp, the CPU restatement of the thin-lens camera (its ray, and every mode's
+    render from the lens ray's first hit) over the transmission restatement (test infrastructure, loaded only by tests/oracle_lens.py)."""
+    src = os.path.join(ROOT, "tests", "oracle_lens.cpp")
+    deps = [src] + [os.path.join(ROOT, "tests", f) for f in ("oracle_transmission.cpp", "oracle_env_light.cpp", "oracle_lights.cpp")] + \
+        [os.path.join(ROOT, "oracle", "ezrt_oracle.cpp")] + [os.path.join(INCLUDE, f) for f in os.listdir(INCLUDE)]
+    if force or _newer(ORACLE_LENS_SO, deps):
+        os.makedirs(os.path.dirname(ORACLE_LENS_SO), exist_ok=True)
+        tmp = ORACLE_LENS_SO + ".tmp%d" % os.getpid()
+        _run(["g++"] + HOST_FLAGS + ["-fopenmp", "-Wno-misleading-indentation", "-shared", "-I", INCLUDE, src, "-o", tmp])
+        os.replace(tmp, ORACLE_LENS_SO)
+    return ORACLE_LENS_SO
+
+
 def build_reference_hdrloader(force=False):
     return _oracle_recipes().build_reference_hdrloader(force)
 
@@ -277,6 +294,7 @@ def build_all(force=False, verbose=False):
     build_oracle_lights(force=force)
     build_oracle_env_light(force=force)
     build_oracle_transmission(force=force)
+    build_oracle_lens(force=force)
     build_example(force=force)
     build_reference_hdrloader(force=force)
     build_reference_shaders(force=force)

@@ -177,6 +177,15 @@ int carve_shadow(DeviceBuffer& buf, size_t capacity, ShadowQueue& q) {
     return EZRT_OK;
 }
 
+// EZRT_PARAM_THIN_LENS: true with the lens in *lens when the flag is set and its parameters are valid (ez_lens_setup)
+bool thin_lens(const ezrt_render_params* p, LensDev* lens) {
+    if (!(p->reserved[0] & EZRT_PARAM_THIN_LENS)) return false;
+    float R, f;
+    memcpy(&R, &p->reserved[1], sizeof(float));
+    memcpy(&f, &p->reserved[2], sizeof(float));
+    return ez_lens_setup(p->eye, p->camera_rotate, R, f, lens) != 0;
+}
+
 int validate_params(const ezrt_scene* scene, const ezrt_render_params* p) {
     if (!scene || !p) return ezrt_set_error(EZRT_ERR_INVALID, "render: null argument");
     if (p->width <= 0 || p->height <= 0 || p->spp < 0) return ezrt_set_error(EZRT_ERR_INVALID, "render: bad image size/spp");
@@ -187,6 +196,10 @@ int validate_params(const ezrt_scene* scene, const ezrt_render_params* p) {
         return ezrt_set_error(EZRT_ERR_INVALID, "render: EZRT_PARAM_ENV_LIGHT needs the light sampling mode (got mode %d)", p->mode);
     if ((p->reserved[0] & EZRT_PARAM_TRANSMISSION) && p->mode != EZRT_MODE_DISNEY_LIGHTS)
         return ezrt_set_error(EZRT_ERR_INVALID, "render: EZRT_PARAM_TRANSMISSION needs the light sampling mode (got mode %d)", p->mode);
+    LensDev lens;
+    if (!thin_lens(p, &lens) && (p->reserved[0] & EZRT_PARAM_THIN_LENS))
+        return ezrt_set_error(EZRT_ERR_INVALID, "render: EZRT_PARAM_THIN_LENS needs a finite lens radius and focus distance > 0 and columns 0-2 "
+                                                "of camera_rotate of finite, non-zero length");
     if (p->max_bounce < 0 || p->max_bounce > 64) return ezrt_set_error(EZRT_ERR_INVALID, "render: max_bounce out of range");
     if (p->out_channels != 3 && p->out_channels != 4) return ezrt_set_error(EZRT_ERR_INVALID, "render: out_channels must be 3 or 4");
     if (p->part_count < 1 || p->part_rank < 0 || p->part_rank >= p->part_count)
@@ -919,6 +932,8 @@ static int render_device_impl(ezrt_scene* s, const ezrt_render_params* p, float*
     const TileDev* d_tiles = (const TileDev*)s->tiles_buf.p;
     const bool prune = s->regular_tree && (p->traverse != EZRT_TRAVERSE_REFERENCE);
     const bool accel = s->regular_tree && s->have_accel && (p->traverse == EZRT_TRAVERSE_ACCEL);
+    LensDev lens_v;
+    const LensDev* lens = thin_lens(p, &lens_v) ? &lens_v : nullptr;   // EZRT_PARAM_THIN_LENS (validated)
     if (rd.n_tiles == 0 || p->spp == 0) {
         CU_CHECK(cudaEventRecord(s->ev_stop, st));
         s->have_timing = true;
@@ -931,7 +946,7 @@ static int render_device_impl(ezrt_scene* s, const ezrt_render_params* p, float*
             s->fb_wait = nullptr;
         }
         int sp = s->span_begin(0, st);
-        launch_megakernel(s->dev, rd, d_tiles, prune, p->spp, d_fb, totals, st);
+        launch_megakernel(s->dev, rd, d_tiles, prune, p->spp, d_fb, totals, st, lens);
         s->span_end(sp, st);
         s->launches++;
         CU_CHECK(cudaGetLastError());
@@ -1069,11 +1084,14 @@ static int render_device_impl(ezrt_scene* s, const ezrt_render_params* p, float*
         const uint32_t n_slots = (uint32_t)((size_t)rd.n_tiles * EZRT_TILE_PIXELS * (size_t)nf);
         const uint32_t batch_first = p->first_frame + (uint32_t)done;
         CU_CHECK(cudaMemsetAsync(cnt, 0, sizeof(uint32_t) * n_counters, st));
-        const bool fused_camera = accel;   // accel policy: camera rays are generated inside the first extend kernel
+        // accel policy: camera rays are generated inside the first extend kernel.  Thin-lens camera rays do not share an origin:
+        // k_generate<true> queues them and bounce 0 takes the unfused form under every policy (the accel policy's per-ray kernels,
+        // k_shade reading the rays back from queue 0)
+        const bool fused_camera = accel && !lens;
         int sp = -1;
         if (!fused_camera) {
             sp = s->span_begin(3, st);
-            launch_generate(rd, d_tiles, n_slots, batch_first, q[0], &q_count[0], s->n_sms, st);
+            launch_generate(rd, d_tiles, n_slots, batch_first, q[0], &q_count[0], s->n_sms, st, lens);
             s->span_end(sp, st);
             s->launches++;
         }
@@ -1641,6 +1659,41 @@ int ezrt_eval_brdf(int device, int which, int n, const float* V, const float* N,
     if (e == cudaSuccess) e = cudaMemcpy(out, dOut, f3, cudaMemcpyDeviceToHost);
     buf.release();
     if (e != cudaSuccess) return ezrt_set_error(EZRT_ERR_CUDA, "eval_brdf: %s", cudaGetErrorString(e));
+    return EZRT_OK;
+}
+
+int ezrt_camera_rays(ezrt_scene* s, const ezrt_render_params* p, int n, const uint32_t* px, const uint32_t* py, const uint32_t* frame,
+                     float* origins_out, float* dirs_out) {
+    int rc = validate_params(s, p);
+    if (rc) return rc;
+    if (n < 0 || !px || !py || !frame || !origins_out || !dirs_out) return ezrt_set_error(EZRT_ERR_INVALID, "camera_rays: bad argument");
+    if (n == 0) return EZRT_OK;
+    CU_CHECK(cudaSetDevice(s->device));
+    RenderDev rd{};
+    rd.width = p->width; rd.height = p->height;
+    memcpy(rd.eye, p->eye, sizeof(rd.eye));
+    memcpy(rd.cam, p->camera_rotate, sizeof(rd.cam));
+    LensDev lens_v;
+    const LensDev* lens = thin_lens(p, &lens_v) ? &lens_v : nullptr;
+    DeviceBuffer buf;
+    const size_t u1 = sizeof(uint32_t) * (size_t)n, f3 = sizeof(float) * 3 * (size_t)n;
+    if ((rc = buf.ensure(3 * u1 + 2 * f3 + 256))) return rc;
+    uint32_t* dPx = (uint32_t*)buf.p;
+    uint32_t* dPy = dPx + n;
+    uint32_t* dFr = dPy + n;
+    float* dO = (float*)(dFr + n);
+    float* dD = dO + 3 * (size_t)n;
+    cudaError_t e = cudaMemcpy(dPx, px, u1, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = cudaMemcpy(dPy, py, u1, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = cudaMemcpy(dFr, frame, u1, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) {
+        launch_camera_rays(rd, lens, n, dPx, dPy, dFr, dO, dD, 0);
+        e = cudaGetLastError();
+    }
+    if (e == cudaSuccess) e = cudaMemcpy(origins_out, dO, f3, cudaMemcpyDeviceToHost);
+    if (e == cudaSuccess) e = cudaMemcpy(dirs_out, dD, f3, cudaMemcpyDeviceToHost);
+    buf.release();
+    if (e != cudaSuccess) return ezrt_set_error(EZRT_ERR_CUDA, "camera_rays: %s", cudaGetErrorString(e));
     return EZRT_OK;
 }
 

@@ -1810,8 +1810,8 @@ __device__ __forceinline__ float hdr_pdf(const SceneDev& sc, vec3 L) {
 // ------------------------------------------------------------------------------------------
 // camera ray, main() P5/fsh:920-925
 // ------------------------------------------------------------------------------------------
-__device__ __forceinline__ void primary_ray(const RenderDev& rd, uint32_t px, uint32_t py, uint32_t frame, uint32_t& seed,
-                                            vec3& o, vec3& d) {
+// the pinhole direction M (vx, vy, -1.5, 0) before normalisation; seed leaves with the two jitter draws taken
+__device__ __forceinline__ vec3 pinhole_dir(const RenderDev& rd, uint32_t px, uint32_t py, uint32_t frame, uint32_t& seed) {
     seed = pixel_seed(px, py, frame);
     float pixx = EZ_DIV((float)px + 0.5f, (float)rd.width) * 2.0f - 1.0f;
     float pixy = EZ_DIV((float)py + 0.5f, (float)rd.height) * 2.0f - 1.0f;
@@ -1819,11 +1819,31 @@ __device__ __forceinline__ void primary_ray(const RenderDev& rd, uint32_t px, ui
     float aay = EZ_DIV(rand01(seed) - 0.5f, (float)rd.height);
     float vx = pixx + aax, vy = pixy + aay, vz = -1.5f, vw = 0.0f;
     const float* m = rd.cam;
-    vec3 dir = ez_v3(((m[0] * vx + m[4] * vy) + m[8] * vz) + m[12] * vw,
-                     ((m[1] * vx + m[5] * vy) + m[9] * vz) + m[13] * vw,
-                     ((m[2] * vx + m[6] * vy) + m[10] * vz) + m[14] * vw);
+    return ez_v3(((m[0] * vx + m[4] * vy) + m[8] * vz) + m[12] * vw,
+                 ((m[1] * vx + m[5] * vy) + m[9] * vz) + m[13] * vw,
+                 ((m[2] * vx + m[6] * vy) + m[10] * vz) + m[14] * vw);
+}
+__device__ __forceinline__ void primary_ray(const RenderDev& rd, uint32_t px, uint32_t py, uint32_t frame, uint32_t& seed,
+                                            vec3& o, vec3& d) {
+    const vec3 dir = pinhole_dir(rd, px, py, frame, seed);
     o = ez_v3(rd.eye[0], rd.eye[1], rd.eye[2]);
     d = ez_normalize(dir);
+}
+// the thin-lens camera ray (EZRT_PARAM_THIN_LENS; ezrt_math.h, DESIGN.md section 13): the pinhole's seed, jitter and direction,
+// then the lens point from the lens stream; seed leaves as primary_ray leaves it
+__device__ __forceinline__ void lens_ray(const RenderDev& rd, const LensDev& lens, uint32_t px, uint32_t py, uint32_t frame, uint32_t& seed,
+                                         vec3& o, vec3& d) {
+    const vec3 dir = pinhole_dir(rd, px, py, frame, seed);
+    float r_a, r_b;
+    ez_lens_draws(px, py, frame, &r_a, &r_b);
+    ez_lens_ray(&lens, dir, r_a, r_b, &o, &d);
+}
+// the camera ray of a render: the pinhole's, or the thin lens's (LENS)
+template <bool LENS>
+__device__ __forceinline__ void camera_ray(const RenderDev& rd, const LensDev& lens, uint32_t px, uint32_t py, uint32_t frame, uint32_t& seed,
+                                           vec3& o, vec3& d) {
+    if (LENS) lens_ray(rd, lens, px, py, frame, seed, o, d);
+    else primary_ray(rd, px, py, frame, seed, o, d);
 }
 
 // ------------------------------------------------------------------------------------------

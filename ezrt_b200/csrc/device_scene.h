@@ -27,6 +27,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "ezrt_math.h"
+
 #define EZRT_MAX_STACK 256       // >= validated tree depth + 1: the shader's own bound, int stack[256] (P5/fsh:260)
 #define EZRT_LEAF_FLAG 0x80000000u
 #define EZRT_LEAF_MAX_N 127
@@ -137,6 +139,11 @@ struct EnvDev {
     int w, h;
     float p_env;              // the probability of an environment sample: 1/2 beside triangle lights, 1 without
 };
+
+// The thin lens of EZRT_PARAM_THIN_LENS (ez_lens_setup, ezrt_math.h; DESIGN.md section 13): eye, the unit axes of the lens,
+// the focus scale and the radius.  Passed to the lens instantiations (k_generate<true>, k_megakernel<.., true>) as a parameter
+// of their own, after the others, so that no other kernel's parameter layout moves.
+typedef ez_lens LensDev;
 
 // A shadow ray and what k_nee needs to evaluate the light sample's contribution once the ray got through (nee_contrib):
 // the BRDF / environment evaluation of the light sample is done after the shadow pass, for unoccluded rays only.

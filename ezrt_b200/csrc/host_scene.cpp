@@ -1139,4 +1139,25 @@ void ezrt_camera_orbit(float rotatAngle, float upAngle, float r, float eye_out[3
     memcpy(camera_rotate, inv.c, sizeof(float) * 16);
 }
 
+// ---- look-at camera with field of view and aspect: inverse(lookAt) has columns (s, u, -f, eye) (mat_look_at's basis)
+int ezrt_camera_look_at(const float eye[3], const float target[3], const float up[3], float vfov_deg, float aspect, float cam_out[16]) {
+    if (!eye || !target || !up || !cam_out) return ezrt_set_error(EZRT_ERR_INVALID, "camera_look_at: null argument");
+    if (!(vfov_deg > 0.0f && vfov_deg < 180.0f) || !(aspect > 0.0f) || !ez_finite(aspect))
+        return ezrt_set_error(EZRT_ERR_INVALID, "camera_look_at: need 0 < vfov_deg < 180 and a finite aspect > 0");
+    const ez_vec3 e = ez_v3(eye[0], eye[1], eye[2]);
+    const ez_vec3 d = ez_sub(ez_v3(target[0], target[1], target[2]), e);
+    const ez_vec3 c = ez_cross(ez_normalize(d), ez_v3(up[0], up[1], up[2]));
+    const float dd = ez_dot(d, d), cc = ez_dot(c, c);
+    if (!(dd > 0.0f) || !ez_finite(dd) || !(cc > 0.0f) || !ez_finite(cc) || !ez_finite(e.x) || !ez_finite(e.y) || !ez_finite(e.z))
+        return ezrt_set_error(EZRT_ERR_INVALID, "camera_look_at: degenerate view (eye == target, up parallel to the view, or not finite)");
+    const ez_vec3 f = ez_normalize(d);
+    const ez_vec3 s = ez_normalize(ez_cross(f, ez_v3(up[0], up[1], up[2])));
+    const ez_vec3 u = ez_cross(s, f);
+    const double t = tan(0.5 * (double)vfov_deg * 0.017453292519943295769);
+    const float sy = (float)(t * 1.5), sx = (float)((double)aspect * t * 1.5);
+    const float m[16] = {s.x * sx, s.y * sx, s.z * sx, 0.0f, u.x * sy, u.y * sy, u.z * sy, 0.0f, -f.x, -f.y, -f.z, 0.0f, e.x, e.y, e.z, 1.0f};
+    memcpy(cam_out, m, sizeof(m));
+    return EZRT_OK;
+}
+
 }  // extern "C"

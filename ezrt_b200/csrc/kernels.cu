@@ -75,8 +75,11 @@ __device__ __forceinline__ uint32_t block_append(bool valid, uint32_t* counter, 
 }
 
 // ------------------------------------------------------------------------------------------
+// LENS (EZRT_PARAM_THIN_LENS): the thin-lens camera rays of `lens`, written to the same records; every policy traces them from
+// the queue at bounce 0
+template <bool LENS>
 __global__ void __launch_bounds__(256) k_generate(RenderDev rd, const TileDev* __restrict__ tiles, uint32_t n_slots,
-                                                  uint32_t batch_first_frame, PathQueue q, uint32_t* q_count) {
+                                                  uint32_t batch_first_frame, PathQueue q, uint32_t* q_count, LensDev lens) {
     __shared__ uint32_t s_scan[34];
     uint32_t stride = gridDim.x * blockDim.x;
     uint32_t n_round = ((n_slots + blockDim.x - 1u) / blockDim.x) * blockDim.x;
@@ -87,7 +90,7 @@ __global__ void __launch_bounds__(256) k_generate(RenderDev rd, const TileDev* _
         if (!valid) continue;
         uint32_t seed;
         vec3 o, d;
-        primary_ray(rd, px, py, batch_first_frame + fib, seed, o, d);
+        camera_ray<LENS>(rd, lens, px, py, batch_first_frame + fib, seed, o, d);
         __stcs(q.ray_o + pos, make_float4(o.x, o.y, o.z, __uint_as_float(seed)));
         __stcs(q.ray_d + pos, make_float4(d.x, d.y, d.z, __uint_as_float(slot)));
     }
@@ -911,9 +914,10 @@ __global__ void k_tally(const uint32_t* __restrict__ q_counts, const uint32_t* _
 // ------------------------------------------------------------------------------------------
 // megakernel: one thread = one pixel, all frames and bounces in registers (cross-check pipeline)
 // ------------------------------------------------------------------------------------------
-template <bool PRUNE>
+// LENS (EZRT_PARAM_THIN_LENS): the camera rays are the thin lens's
+template <bool PRUNE, bool LENS>
 __global__ void __launch_bounds__(128) k_megakernel(SceneDev sc, RenderDev rd, const TileDev* __restrict__ tiles, int spp,
-                                                    float* __restrict__ fb, unsigned long long* totals) {
+                                                    float* __restrict__ fb, unsigned long long* totals, LensDev lens) {
     uint32_t per_frame = (uint32_t)rd.n_tiles * EZRT_TILE_PIXELS;
     uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
     if (r >= per_frame) return;
@@ -928,7 +932,7 @@ __global__ void __launch_bounds__(128) k_megakernel(SceneDev sc, RenderDev rd, c
     for (int s = 0; s < spp; s++) {
         uint32_t frame = rd.first_frame + (uint32_t)s;
         PathRegs p;
-        primary_ray(rd, px, py, frame, p.seed, p.o, p.d);
+        camera_ray<LENS>(rd, lens, px, py, frame, p.seed, p.o, p.d);
         p.history = splat3(1.0f);
         p.f_r = splat3(0.0f);
         p.cosine_i = 0.0f;
@@ -1043,6 +1047,20 @@ __global__ void k_eval_bsdf(int which, int n, const float* V, const float* N, co
         }
     }
     for (int k = 0; k < 8; k++) out[8 * (size_t)i + k] = r[k];
+}
+
+// ezrt_camera_rays: the camera ray of sample (px[i], py[i], frame[i]), pinhole or thin lens (lens_on)
+__global__ void k_camera_rays(RenderDev rd, int lens_on, int n, const uint32_t* px, const uint32_t* py, const uint32_t* frame, float* o_out,
+                              float* d_out, LensDev lens) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    uint32_t seed;
+    vec3 o, d;
+    if (lens_on) camera_ray<true>(rd, lens, px[i], py[i], frame[i], seed, o, d);
+    else camera_ray<false>(rd, lens, px[i], py[i], frame[i], seed, o, d);
+    const size_t k = 3 * (size_t)i;
+    o_out[k] = o.x; o_out[k + 1] = o.y; o_out[k + 2] = o.z;
+    d_out[k] = d.x; d_out[k + 1] = d.y; d_out[k + 2] = d.z;
 }
 
 __global__ void k_eval_math(int which, int n, const float* a, const float* b, float* out) {
@@ -1176,9 +1194,10 @@ static int extend_blocks_per_sm() {
     return v;
 }
 void launch_generate(const RenderDev& rd, const TileDev* tiles, uint32_t n_slots, uint32_t batch_first_frame, PathQueue q,
-                     uint32_t* q_count, int n_sms, cudaStream_t st) {
+                     uint32_t* q_count, int n_sms, cudaStream_t st, const LensDev* lens) {
     int blocks = std::min(div_up(n_slots, 256), n_sms * 8);
-    k_generate<<<blocks, 256, 0, st>>>(rd, tiles, n_slots, batch_first_frame, q, q_count);
+    if (lens) k_generate<true><<<blocks, 256, 0, st>>>(rd, tiles, n_slots, batch_first_frame, q, q_count, *lens);
+    else k_generate<false><<<blocks, 256, 0, st>>>(rd, tiles, n_slots, batch_first_frame, q, q_count, LensDev{});
 }
 // cudaFuncSetAttribute once per (kernel, size): the launchers run for every bounce of every batch
 static void set_dynamic_smem(const void* kernel, size_t bytes) {
@@ -1484,10 +1503,18 @@ void launch_tally(const uint32_t* q_counts, const uint32_t* s_counts, const uint
     k_tally<<<1, 32, 0, st>>>(q_counts, s_counts, d_ext, d_sh, n_stages, totals, n_primary);
 }
 void launch_megakernel(const SceneDev& sc, const RenderDev& rd, const TileDev* tiles, bool prune, int spp, float* fb,
-                       unsigned long long* totals, cudaStream_t st) {
+                       unsigned long long* totals, cudaStream_t st, const LensDev* lens) {
     uint32_t per_frame = (uint32_t)rd.n_tiles * EZRT_TILE_PIXELS;
-    if (prune) k_megakernel<true><<<div_up(per_frame, 128), 128, 0, st>>>(sc, rd, tiles, spp, fb, totals);
-    else k_megakernel<false><<<div_up(per_frame, 128), 128, 0, st>>>(sc, rd, tiles, spp, fb, totals);
+    const LensDev l = lens ? *lens : LensDev{};
+#define EZRT_LAUNCH_MEGA(P, L) k_megakernel<P, L><<<div_up(per_frame, 128), 128, 0, st>>>(sc, rd, tiles, spp, fb, totals, l)
+    if (lens) { if (prune) EZRT_LAUNCH_MEGA(true, true); else EZRT_LAUNCH_MEGA(false, true); }
+    else { if (prune) EZRT_LAUNCH_MEGA(true, false); else EZRT_LAUNCH_MEGA(false, false); }
+#undef EZRT_LAUNCH_MEGA
+}
+void launch_camera_rays(const RenderDev& rd, const LensDev* lens, int n, const uint32_t* px, const uint32_t* py, const uint32_t* frame,
+                        float* o, float* d, cudaStream_t st) {
+    if (n <= 0) return;
+    k_camera_rays<<<div_up(n, 128), 128, 0, st>>>(rd, lens ? 1 : 0, n, px, py, frame, o, d, lens ? *lens : LensDev{});
 }
 void launch_trace_finish(const SceneDev& sc, int n, PathQueue q, int p3fudge, int accel_space, int* hit, float* dist, int* tri, int* inside,
                          float* point, float* normal, cudaStream_t st) {

@@ -16,8 +16,9 @@
 #endif
 #define EZRT_EXTEND_BLOCKS_PER_SM 1
 
+// lens (EZRT_PARAM_THIN_LENS): the thin-lens camera rays (k_generate<true>); null: the pinhole's
 void launch_generate(const RenderDev& rd, const TileDev* tiles, uint32_t n_slots, uint32_t batch_first_frame, PathQueue q,
-                     uint32_t* q_count, int n_sms, cudaStream_t st);
+                     uint32_t* q_count, int n_sms, cudaStream_t st, const LensDev* lens = nullptr);
 void launch_extend(const SceneDev& sc, bool prune, bool anyhit, PathQueue q, const uint32_t* q_count, uint32_t* work,
                    const uint32_t* perm, int to_accel, uint32_t n_max, int n_sms, cudaStream_t st, float2* side_hit = nullptr, int gate = 0);
 // counts (params.profile = 2): [0] 128-byte node visits, [1] triangle tests, [2] quantised node visits, then the W8 kernels' phase
@@ -79,7 +80,10 @@ void launch_adaptive_check(const RenderDev& rd, const TileDev* tiles_in, int n_f
 void launch_tally(const uint32_t* q_counts, const uint32_t* s_counts, const uint32_t* d_ext, const uint32_t* d_sh, int n_stages,
                   unsigned long long* totals, uint32_t n_primary, cudaStream_t st);
 void launch_megakernel(const SceneDev& sc, const RenderDev& rd, const TileDev* tiles, bool prune, int spp, float* fb,
-                       unsigned long long* totals, cudaStream_t st);
+                       unsigned long long* totals, cudaStream_t st, const LensDev* lens = nullptr);
+// ezrt_camera_rays: n camera rays (device arrays) -> origins, dirs (n x 3 floats each); lens null: the pinhole's
+void launch_camera_rays(const RenderDev& rd, const LensDev* lens, int n, const uint32_t* px, const uint32_t* py, const uint32_t* frame,
+                        float* o, float* d, cudaStream_t st);
 void launch_trace_finish(const SceneDev& sc, int n, PathQueue q, int p3fudge, int accel_space, int* hit, float* dist, int* tri, int* inside,
                          float* point, float* normal, cudaStream_t st);
 void launch_eval_brdf(int which, int n, const float* V, const float* N, const float* L, const float* xi, const float* materials,

@@ -105,7 +105,8 @@ typedef struct ezrt_render_params {
     int32_t profile;          /* 1: bracket every kernel with CUDA events (ezrt_get_kernel_times);
                                  2: count the records the accel traversal fetches (ezrt_counters.node_visits / tri_tests;
                                     a slower instantiation of the same kernels -- never inside a timed region) */
-    int32_t reserved[3];      /* [0]: flags, EZRT_PARAM_*; [1], [2]: 0 */
+    int32_t reserved[3];      /* [0]: flags, EZRT_PARAM_*; [1], [2]: with EZRT_PARAM_THIN_LENS the lens radius and the focus
+                                 distance as IEEE-754 float bits, ignored otherwise */
 } ezrt_render_params;
 
 /* ezrt_render_params.reserved[0]: keep counting -- ezrt_get_counters / ezrt_get_kernel_times then report the sums over all
@@ -129,6 +130,15 @@ typedef struct ezrt_render_params {
    material of t > 0 renders as without the flag, bit for bit.  Accepted by ezrt_render[_device],
    ezrt_render_adaptive[_device] and ezrt_render_aov[_device]. */
 #define EZRT_PARAM_TRANSMISSION 4
+/* ezrt_render_params.reserved[0], any mode, policy and pipeline: a thin-lens camera (depth of field).  reserved[1] holds the
+   bits of the lens radius R, reserved[2] those of the focus distance f (memcpy a float into each).  Each camera ray starts at a
+   point of the disk of radius R around eye spanned by columns 0 and 1 of camera_rotate (normalised), and passes through the
+   point the pinhole ray of the same pixel jitter reaches at depth f along -column 2; ezrt_math.h and DESIGN.md section 13 give
+   the arithmetic.  The lens point is drawn from a random stream of its own, so the rest of every path draws what the pinhole
+   render draws.  Invalid (EZRT_ERR_INVALID) unless R and f are finite and > 0 and columns 0, 1 and 2 have finite, non-zero
+   length.  Accepted by ezrt_render[_device], ezrt_render_adaptive[_device] and ezrt_render_aov[_device]; a feature-buffer
+   render's depth is the first hit's distance from the lens point. */
+#define EZRT_PARAM_THIN_LENS 8
 
 typedef struct ezrt_counters {
     uint64_t rays;          /* hitBVH invocations: primary + bounce + shadow (SURVEY 8d)     */
@@ -307,6 +317,12 @@ int ezrt_eval_brdf(int device, int which, int n, const float* V, const float* N,
 int ezrt_eval_bsdf(int device, int which, int n, const float* V, const float* N, const float* L, const float* xi,
                    const int32_t* inside, const float* materials, float* out);
 
+/* The camera rays of n samples (pixel px[i], py[i] of params' image, frame[i]; host arrays) as the render's kernels generate
+ * them: the pinhole ray, or the thin-lens ray with EZRT_PARAM_THIN_LENS (validated as a render validates it).  origins_out,
+ * dirs_out: n x 3 floats.  For parity tests, like ezrt_eval_bsdf: it allocates and synchronises per call. */
+int ezrt_camera_rays(ezrt_scene* scene, const ezrt_render_params* params, int n, const uint32_t* px, const uint32_t* py,
+                     const uint32_t* frame, float* origins_out, float* dirs_out);
+
 /* Evaluate a ezrt_math.h function on the device for n inputs (parity of the arithmetic
  * definition): which = 0 sin, 1 cos, 2 log, 3 exp, 4 pow(a,b), 5 atan2(a,b), 6 asin. */
 int ezrt_eval_math(int device, int which, int n, const float* a, const float* b, float* out);
@@ -411,6 +427,14 @@ int ezrt_hdr_cache_device(int device, const float* hdr, int width, int height, f
  * eye, cameraRotate = inverse(lookAt(eye, 0, +y)), column-major. */
 void ezrt_camera_orbit(float rotate_angle_deg, float up_angle_deg, float r, float eye[3],
                        float camera_rotate[16]);
+/* A look-at camera with a vertical field of view (degrees, 0 < vfov_deg < 180) and an aspect ratio (width / height): the
+ * cameraRotate whose columns are the orthonormal right, up and back vectors of lookAt(eye, target, up) (as camera_orbit's
+ * inverse(lookAt)), column 0 scaled by aspect * tan(vfov/2) * 1.5 and column 1 by tan(vfov/2) * 1.5, column 3 = (eye, 1).
+ * The pinhole kernels then render that field of view and aspect (they map the image to [-1, 1]^2 at depth 1.5).  Returns
+ * EZRT_ERR_INVALID for a degenerate view (eye == target, up parallel to the view), vfov_deg outside (0, 180) or
+ * aspect <= 0 or not finite. */
+int ezrt_camera_look_at(const float eye[3], const float target[3], const float up[3], float vfov_deg, float aspect,
+                        float cam_out[16]);
 
 #ifdef __cplusplus
 }

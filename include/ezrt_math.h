@@ -592,4 +592,71 @@ EZ_HD ez_vec3 ez_trans_mix(ez_vec3 f_ref, float pdf_ref, ez_vec3 f_diel, float p
     return ez_add(ez_scale(f_ref, s), ez_scale(f_diel, t));
 }
 
+/* ------------------------------------------------------------------ thin-lens camera (DESIGN.md section 13)
+ * EZRT_PARAM_THIN_LENS, any mode: lens radius R = reserved[1], focus distance f = reserved[2] (IEEE-754 bits of floats).
+ * M = camera_rotate (column-major), c_i = column i, eye = params.eye.  Per sample (px, py, frame):
+ *   the pinhole's seed, jitter draws, vx, vy and dir_pin = M (vx, vy, -1.5, 0), bit for bit (primary_ray, P5/fsh:915-925);
+ *   F = eye + dir_pin * k,  k = f / (1.5 |c2|)        the point at depth f along -c2 (ez_lens_setup: k, u0, u1)
+ *   (lx, ly) = ez_concentric_disk(r_a, r_b),  (r_a, r_b) = ez_lens_draws(px, py, frame)
+ *   o = eye + (lx u0 + ly u1) R,  u0 = c0 / |c0|, u1 = c1 / |c1|;   d = normalize(F - o)
+ * |c| = sqrt(dot(c, c)).  The lens draws come from a stream of their own, so every draw of the path after the jitter is the
+ * pinhole render's.  The flag is valid iff R and f are finite and > 0, |c0|, |c1|, |c2| are finite and > 0, and k is finite. */
+#define EZRT_LENS_SALT 0x4c454e53u   /* "LENS" */
+/* wang_hash / rand (P5/fsh:320-331) */
+EZ_HD uint32_t ez_wang_hash(uint32_t* seed) {
+    uint32_t s = *seed;
+    s = (s ^ 61u) ^ (s >> 16);
+    s *= 9u;
+    s = s ^ (s >> 4);
+    s *= 0x27d4eb2du;
+    s = s ^ (s >> 15);
+    *seed = s;
+    return s;
+}
+EZ_HD float ez_rand01(uint32_t* seed) { return ez_u32_to_float(ez_wang_hash(seed)) * 2.3283064365386963e-10f; }
+/* the lens stream: two rand draws from the pixel seed (P5/fsh:315-318) XOR EZRT_LENS_SALT; a function of (px, py, frame) only */
+EZ_HD void ez_lens_draws(uint32_t px, uint32_t py, uint32_t frame, float* r_a, float* r_b) {
+    uint32_t s = ((px * 1973u + py * 9277u + frame * 26699u) | 1u) ^ EZRT_LENS_SALT;
+    *r_a = ez_rand01(&s);
+    *r_b = ez_rand01(&s);
+}
+/* Shirley-Chiu concentric map of [0, 1]^2 onto the unit disk (uniform in area) */
+EZ_HD void ez_concentric_disk(float u1, float u2, float* x, float* y) {
+    const float a = 2.0f * u1 - 1.0f, b = 2.0f * u2 - 1.0f;
+    if (a == 0.0f && b == 0.0f) { *x = 0.0f; *y = 0.0f; return; }
+    float r, phi;
+    if (ez_abs(a) > ez_abs(b)) { r = a; phi = EZ_PIO4 * EZ_DIV(b, a); }
+    else { r = b; phi = EZ_PIO2 - EZ_PIO4 * EZ_DIV(a, b); }
+    *x = r * ez_cos(phi);
+    *y = r * ez_sin(phi);
+}
+struct ez_lens {
+    ez_vec3 eye, u0, u1;   /* the lens centre and its unit axes */
+    float k, R;            /* focus scale f / (1.5 |c2|), lens radius */
+};
+typedef struct ez_lens ez_lens;
+/* the lens of (eye, camera_rotate, R, f); returns 0 (and leaves *L unset) if the flag's parameters are invalid */
+EZ_HD int ez_lens_setup(const float eye[3], const float cam[16], float R, float f, ez_lens* L) {
+    const ez_vec3 c0 = ez_v3(cam[0], cam[1], cam[2]), c1 = ez_v3(cam[4], cam[5], cam[6]), c2 = ez_v3(cam[8], cam[9], cam[10]);
+    const float n0 = EZ_SQRT(ez_dot(c0, c0)), n1 = EZ_SQRT(ez_dot(c1, c1)), n2 = EZ_SQRT(ez_dot(c2, c2));
+    if (!(ez_finite(R) && R > 0.0f && ez_finite(f) && f > 0.0f)) return 0;
+    if (!(ez_finite(n0) && n0 > 0.0f && ez_finite(n1) && n1 > 0.0f && ez_finite(n2) && n2 > 0.0f)) return 0;
+    const float k = EZ_DIV(f, 1.5f * n2);
+    if (!ez_finite(k)) return 0;
+    L->eye = ez_v3(eye[0], eye[1], eye[2]);
+    L->u0 = ez_divs(c0, n0);
+    L->u1 = ez_divs(c1, n1);
+    L->k = k;
+    L->R = R;
+    return 1;
+}
+/* the lens ray through the pinhole direction dir_pin with the lens draws (r_a, r_b) */
+EZ_HD void ez_lens_ray(const ez_lens* L, ez_vec3 dir_pin, float r_a, float r_b, ez_vec3* o, ez_vec3* d) {
+    const ez_vec3 F = ez_add(L->eye, ez_scale(dir_pin, L->k));
+    float lx, ly;
+    ez_concentric_disk(r_a, r_b, &lx, &ly);
+    *o = ez_add(L->eye, ez_scale(ez_add(ez_scale(L->u0, lx), ez_scale(L->u1, ly)), L->R));
+    *d = ez_normalize(ez_sub(F, *o));
+}
+
 #endif /* EZRT_MATH_H */
