@@ -37,6 +37,12 @@ class DenoiseParams(C.Structure):
                 ("reserved", C.c_int32)]
 
 
+class Medium(C.Structure):
+    """struct ezrt_medium (include/ezrt.h)."""
+    _fields_ = [("sigma_t", C.c_float), ("albedo", C.c_float * 3), ("g", C.c_float), ("box_min", C.c_float * 3), ("box_max", C.c_float * 3),
+                ("reserved", C.c_int32)]
+
+
 class Counters(C.Structure):
     """struct ezrt_counters (include/ezrt.h)."""
     _fields_ = [
@@ -54,6 +60,7 @@ SIGNATURES = {
     "ezrt_scene_create": (C.c_int, [C.c_int, c_float_p, C.c_int, c_float_p, C.c_int, c_float_p, c_float_p, C.c_int, C.c_int,
                                     C.c_int, C.POINTER(C.c_void_p)]),
     "ezrt_scene_destroy": (C.c_int, [C.c_void_p]),
+    "ezrt_scene_set_medium": (C.c_int, [C.c_void_p, C.POINTER(Medium)]),
     "ezrt_render": (C.c_int, [C.c_void_p, C.POINTER(RenderParams), c_float_p]),
     "ezrt_render_device": (C.c_int, [C.c_void_p, C.POINTER(RenderParams), C.c_void_p, C.c_void_p]),
     "ezrt_render_adaptive_device": (C.c_int, [C.c_void_p, C.POINTER(RenderParams), C.POINTER(AdaptiveParams), C.c_void_p, C.c_void_p,

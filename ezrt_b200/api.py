@@ -12,7 +12,7 @@ from dataclasses import dataclass, field
 import numpy as np
 
 from . import _lib
-from ._lib import AdaptiveParams, Counters, DenoiseParams, EzrtError, RenderParams, check, lib
+from ._lib import AdaptiveParams, Counters, DenoiseParams, EzrtError, Medium, RenderParams, check, lib
 
 MODE_DIFFUSE_P3 = 0
 MODE_DISNEY_ANISO_P4 = 1
@@ -23,6 +23,7 @@ PARAM_ACCUMULATE = 1   # ezrt_render_params.reserved[0] flags (include/ezrt.h)
 PARAM_ENV_LIGHT = 2
 PARAM_TRANSMISSION = 4
 PARAM_THIN_LENS = 8
+PARAM_MEDIUM = 16
 MODES = {"diffuse_p3": 0, "disney_aniso_p4": 1, "disney_sobol_p5": 2, "disney_is_mis_p5": 3, "disney_lights": 4}
 
 TRAVERSE_ACCEL = 0
@@ -230,6 +231,7 @@ class RenderConfig:
     transmission: bool = False  # EZRT_PARAM_TRANSMISSION (MODE_DISNEY_LIGHTS only): materials' IOR and transmission (DESIGN.md section 12)
     lens_radius: float = 0.0    # != 0: EZRT_PARAM_THIN_LENS, a thin-lens camera of this radius (DESIGN.md section 13); must be > 0
     focus_distance: float = None  # ... focused at this depth along the view (-column 2 of camera_rotate); required with a lens
+    medium: bool = False        # EZRT_PARAM_MEDIUM (MODE_DISNEY_LIGHTS only): the scene's homogeneous medium (Scene.set_medium, DESIGN.md section 14)
 
     def to_struct(self):
         p = RenderParams()
@@ -242,7 +244,7 @@ class RenderConfig:
         p.part_rank, p.part_count, p.frames_per_batch = int(self.part_rank), int(self.part_count), int(self.frames_per_batch)
         p.profile = int(self.profile)
         p.reserved[0] = ((PARAM_ACCUMULATE if self.accumulate else 0) | (PARAM_ENV_LIGHT if self.env_light else 0) |
-                         (PARAM_TRANSMISSION if self.transmission else 0))
+                         (PARAM_TRANSMISSION if self.transmission else 0) | (PARAM_MEDIUM if self.medium else 0))
         if self.lens_radius != 0:   # a negative or NaN radius is set too, so that the library rejects it
             if self.focus_distance is None:
                 raise ValueError("RenderConfig: a lens (lens_radius != 0) needs a focus_distance")
@@ -297,6 +299,22 @@ class Scene:
             lib.ezrt_scene_destroy(h)
 
     __del__ = close
+
+    def set_medium(self, sigma_t, albedo=(1.0, 1.0, 1.0), g=0.0, box_min=None, box_max=None):
+        """ezrt_scene_set_medium: the homogeneous medium RenderConfig.medium renders -- grey extinction sigma_t, RGB albedo,
+        Henyey-Greenstein g, filling the box [box_min, box_max] (DESIGN.md section 14; both corners required).  set_medium(None)
+        clears it.  Renders already enqueued keep the medium they were enqueued with."""
+        if sigma_t is None:
+            check(lib.ezrt_scene_set_medium(self._h, None))
+            return
+        if box_min is None or box_max is None:
+            raise ValueError("Scene.set_medium: box_min and box_max are required (the medium fills that box)")
+        m = Medium()
+        m.sigma_t, m.g, m.reserved = float(sigma_t), float(g), 0
+        m.albedo[:] = [float(x) for x in albedo]
+        m.box_min[:] = [float(x) for x in box_min]
+        m.box_max[:] = [float(x) for x in box_max]
+        check(lib.ezrt_scene_set_medium(self._h, C.byref(m)))
 
     def render(self, cfg, framebuffer=None):
         """render(width, height, spp) -> framebuffer: `spp` display() calls through HOST buffers

@@ -231,6 +231,24 @@ def build_oracle_lens(force=False):
     return ORACLE_LENS_SO
 
 
+ORACLE_MEDIUM_SO = os.path.join(ROOT, "build", "libezrt_oracle_medium.so")
+
+
+def build_oracle_medium(force=False):
+    """build/libezrt_oracle_medium.so: tests/oracle_medium.cpp, the CPU restatement of the homogeneous medium (free flight, the
+    phase function, the light samples' transmittance, the flagged render) over the lens restatement (test infrastructure, loaded only
+    by tests/oracle_medium.py)."""
+    src = os.path.join(ROOT, "tests", "oracle_medium.cpp")
+    deps = [src] + [os.path.join(ROOT, "tests", f) for f in ("oracle_lens.cpp", "oracle_transmission.cpp", "oracle_env_light.cpp", "oracle_lights.cpp")] + \
+        [os.path.join(ROOT, "oracle", "ezrt_oracle.cpp")] + [os.path.join(INCLUDE, f) for f in os.listdir(INCLUDE)]
+    if force or _newer(ORACLE_MEDIUM_SO, deps):
+        os.makedirs(os.path.dirname(ORACLE_MEDIUM_SO), exist_ok=True)
+        tmp = ORACLE_MEDIUM_SO + ".tmp%d" % os.getpid()
+        _run(["g++"] + HOST_FLAGS + ["-fopenmp", "-Wno-misleading-indentation", "-shared", "-I", INCLUDE, src, "-o", tmp])
+        os.replace(tmp, ORACLE_MEDIUM_SO)
+    return ORACLE_MEDIUM_SO
+
+
 def build_reference_hdrloader(force=False):
     return _oracle_recipes().build_reference_hdrloader(force)
 
@@ -295,6 +313,7 @@ def build_all(force=False, verbose=False):
     build_oracle_env_light(force=force)
     build_oracle_transmission(force=force)
     build_oracle_lens(force=force)
+    build_oracle_medium(force=force)
     build_example(force=force)
     build_reference_hdrloader(force=force)
     build_reference_shaders(force=force)

@@ -104,6 +104,9 @@ struct ezrt_scene {
     bool env_built = false;
     EnvDev env{};                     // row_cdf null: the scene has no table (no map, or no texel of positive weight)
     double env_total = 0.0;           // T, the float64 sum of the texel weights
+    // the homogeneous medium of EZRT_PARAM_MEDIUM (ezrt_scene_set_medium), copied into the kernels' parameters at every render
+    bool has_medium = false;
+    MediumDev medium{};
     void* hot_base = nullptr;   // accel nodes | geometry (| vertices) | shading records (L2 persisting window)
     size_t hot_bytes = 0;
     size_t l2_persist_bytes = 0;
@@ -200,6 +203,13 @@ int validate_params(const ezrt_scene* scene, const ezrt_render_params* p) {
     if (!thin_lens(p, &lens) && (p->reserved[0] & EZRT_PARAM_THIN_LENS))
         return ezrt_set_error(EZRT_ERR_INVALID, "render: EZRT_PARAM_THIN_LENS needs a finite lens radius and focus distance > 0 and columns 0-2 "
                                                 "of camera_rotate of finite, non-zero length");
+    if (p->reserved[0] & EZRT_PARAM_MEDIUM) {
+        if (p->mode != EZRT_MODE_DISNEY_LIGHTS)
+            return ezrt_set_error(EZRT_ERR_INVALID, "render: EZRT_PARAM_MEDIUM needs the light sampling mode (got mode %d)", p->mode);
+        if (p->reserved[0] & EZRT_PARAM_TRANSMISSION)
+            return ezrt_set_error(EZRT_ERR_INVALID, "render: EZRT_PARAM_MEDIUM is not rendered with EZRT_PARAM_TRANSMISSION (glass is defined with vacuum outside)");
+        if (!scene->has_medium) return ezrt_set_error(EZRT_ERR_INVALID, "render: EZRT_PARAM_MEDIUM needs a medium (ezrt_scene_set_medium)");
+    }
     if (p->max_bounce < 0 || p->max_bounce > 64) return ezrt_set_error(EZRT_ERR_INVALID, "render: max_bounce out of range");
     if (p->out_channels != 3 && p->out_channels != 4) return ezrt_set_error(EZRT_ERR_INVALID, "render: out_channels must be 3 or 4");
     if (p->part_count < 1 || p->part_rank < 0 || p->part_rank >= p->part_count)
@@ -877,6 +887,32 @@ int ezrt_scene_create(int device, const float* tris, int n_triangles, const floa
     return EZRT_OK;
 }
 
+int ezrt_scene_set_medium(ezrt_scene* s, const ezrt_medium* m) {
+    if (!s) return ezrt_set_error(EZRT_ERR_INVALID, "scene_set_medium: null scene");
+    if (!m) {
+        s->has_medium = false;
+        s->medium = MediumDev{};
+        return EZRT_OK;
+    }
+    if (!(ez_finite(m->sigma_t) && m->sigma_t >= 0.0f)) return ezrt_set_error(EZRT_ERR_INVALID, "scene_set_medium: sigma_t must be finite and >= 0");
+    for (int k = 0; k < 3; k++) {
+        if (!(m->albedo[k] >= 0.0f && m->albedo[k] <= 1.0f)) return ezrt_set_error(EZRT_ERR_INVALID, "scene_set_medium: albedo must lie in [0, 1]");
+        if (!(ez_finite(m->box_min[k]) && ez_finite(m->box_max[k]))) return ezrt_set_error(EZRT_ERR_INVALID, "scene_set_medium: the box must be finite");
+        if (m->box_min[k] > m->box_max[k]) return ezrt_set_error(EZRT_ERR_INVALID, "scene_set_medium: box_min > box_max on axis %d", k);
+    }
+    if (!(m->g > -1.0f && m->g < 1.0f)) return ezrt_set_error(EZRT_ERR_INVALID, "scene_set_medium: g must lie in (-1, 1)");
+    if (m->reserved != 0) return ezrt_set_error(EZRT_ERR_INVALID, "scene_set_medium: reserved must be 0");
+    MediumDev d;
+    d.sigma_t = m->sigma_t;
+    d.albedo = ez_v3(m->albedo[0], m->albedo[1], m->albedo[2]);
+    d.g = m->g;
+    d.bmin = ez_v3(m->box_min[0], m->box_min[1], m->box_min[2]);
+    d.bmax = ez_v3(m->box_max[0], m->box_max[1], m->box_max[2]);
+    s->medium = d;
+    s->has_medium = true;
+    return EZRT_OK;
+}
+
 int ezrt_scene_destroy(ezrt_scene* s) {
     if (!s) return EZRT_OK;
     cudaSetDevice(s->device);
@@ -973,6 +1009,9 @@ static int render_device_impl(ezrt_scene* s, const ezrt_render_params* p, float*
     }
     // EZRT_PARAM_TRANSMISSION: the TRANS instantiations of k_shade and k_nee
     const bool trans = lights_mode && (p->reserved[0] & EZRT_PARAM_TRANSMISSION);
+    // EZRT_PARAM_MEDIUM (validated: a medium is set): the MEDIUM instantiations, by value; sigma_t == 0 is mode 4 and runs its kernels
+    const MediumDev medium_v = s->medium;
+    const MediumDev* med = (lights_mode && (p->reserved[0] & EZRT_PARAM_MEDIUM) && medium_v.sigma_t > 0.0f) ? &medium_v : nullptr;
     int F = p->frames_per_batch;
     if (F <= 0) F = (int)std::max<size_t>(1, ((size_t)32 << 20) / per_frame);  // ~32 M sample slots per batch (~7.5 GB of state):
                                                                               // long queues amortise the persistent kernels' ramp-up and tail
@@ -1124,13 +1163,13 @@ static int render_device_impl(ezrt_scene* s, const ezrt_render_params* p, float*
                 CU_CHECK(cudaEventRecord(s->ev_fork, st));
                 CU_CHECK(cudaStreamWaitEvent(s->side_stream, s->ev_fork, 0));
                 launch_deferred_lane(s->dev, rd, d_tiles, b, batch_first, qin, defer_list, &d_ext[b], &dw_ext[b], side_hit, qout, &q_count[b + 1], sq, &s_count[b],
-                                     Lo, Le, n_fused, (uint32_t)nf, s->n_sms, s->side_stream, b == 0 ? aov_rec : nullptr, lights, env, trans);
+                                     Lo, Le, n_fused, (uint32_t)nf, s->n_sms, s->side_stream, b == 0 ? aov_rec : nullptr, lights, env, trans, med);
                 CU_CHECK(cudaEventRecord(s->ev_join, s->side_stream));
                 s->launches += 2;
             }
             sp = s->span_begin(1, st);
             launch_shade(s->dev, rd, d_tiles, b, batch_first, qin, &q_count[b], qout, &q_count[b + 1], sq, &s_count[b], Lo, Le,
-                         n_slots, n_fused, (uint32_t)nf, s->n_sms, st, b == 0 ? aov_rec : nullptr, lights, env, trans);
+                         n_slots, n_fused, (uint32_t)nf, s->n_sms, st, b == 0 ? aov_rec : nullptr, lights, env, trans, med);
             if (lane) CU_CHECK(cudaStreamWaitEvent(st, s->ev_join, 0));   // ... while this k_shade shades all the others; join
             s->span_end(sp, st);
             s->launches += 2;
@@ -1144,7 +1183,7 @@ static int render_device_impl(ezrt_scene* s, const ezrt_render_params* p, float*
                 }
                 s->span_end(sp, st);
                 sp = s->span_begin(1, st);   // shading work: counted with k_shade
-                launch_nee(s->dev, rd, sq, &s_count[b], Lo, n_slots, s->n_sms, st, env.row_cdf != nullptr, trans);
+                launch_nee(s->dev, rd, sq, &s_count[b], Lo, n_slots, s->n_sms, st, env.row_cdf != nullptr, trans, med);
                 s->span_end(sp, st);
                 s->launches += 2;
             }

@@ -1912,6 +1912,13 @@ __device__ __forceinline__ vec3 nee_trans_contrib(const SceneDev& sc, vec3 V, ve
     const float mis_weight = mis_mix_weight(pdf_l, pdf_b);
     return ez_divs(ez_scale(ez_mul(ez_mul(ez_scale(history, mis_weight), E), fr), NdotL), pdf_l);
 }
+// ... at a medium vertex (EZRT_PARAM_MEDIUM; ezrt_math.h, DESIGN.md section 14), before the shadow ray's transmittance: the phase
+// function in place of f_r and the cosine 1; d = the path's propagation direction at the vertex
+__device__ __forceinline__ vec3 nee_medium_contrib(vec3 d, vec3 L, float g, vec3 history, vec3 E, float pdf_l) {
+    const float p = ez_hg_pdf(d, L, g);
+    const float mis_weight = mis_mix_weight(pdf_l, p);
+    return ez_divs(ez_scale(ez_mul(ez_mul(ez_scale(history, mis_weight), E), splat3(p)), 1.0f), pdf_l);
+}
 // the cosine a path record carries: with TRANS its sign is the bit "the BSDF sample went below the surface"
 template <bool TRANS>
 __device__ __forceinline__ float path_cos(float c) { return TRANS ? ez_abs(c) : c; }
@@ -1927,6 +1934,84 @@ __device__ __forceinline__ void tri_vertices(const SceneDev& sc, int tri, bool a
     p1 = f4xyz(ldg4(v + i1)); p2 = f4xyz(ldg4(v + i2)); p3 = f4xyz(ldg4(v + i3));
 }
 
+// A medium vertex (EZRT_PARAM_MEDIUM; ezrt_math.h, DESIGN.md section 14): p's segment scattered at t_s before its hit (hit_t,
+// hit_tri) or its miss.  The weights of the segment (bounce >= 1) and the albedo enter the history; then, below max_bounce, one light
+// sample from P as at a surface but without the hemisphere test and the self exclusion (its shadow ray carries EZRT_MEDIUM_VERTEX
+// and d), and the phase function's sample as the next ray with the record (splat(p), p, 1).  Returns false when the path ends.
+template <bool AOV, bool ENV>
+__device__ __forceinline__ bool medium_step(const SceneDev& sc, const RenderDev& rd, int bounce, PathRegs& p, float t_s, float hit_t,
+                                            int hit_tri, vec3& Lo, vec3& Le, bool& primary_miss, ShadowRay& sh, float4* aov_rec,
+                                            const LightsDev& lights, const EnvDev& env, const MediumDev& med) {
+    if (bounce == 0) {
+        Lo = splat3(0.0f);
+        Le = splat3(0.0f);
+        primary_miss = hit_tri < 0;   // k_blend: a camera ray that left the scene, its colour the Lo of its medium vertices
+        if (AOV && hit_tri >= 0) {    // the feature buffers describe the first surface behind the medium
+            const SurfaceHit hit = surface_hit(sc, p.o, p.d, hit_t, hit_tri, false, rd.accel_space != 0);
+            const MaterialDev mat = load_material(sc, hit.matId);
+            aov_rec[0] = make_float4(mat.baseColor.x, mat.baseColor.y, mat.baseColor.z, hit_t);
+            aov_rec[1] = make_float4(hit.N.x, hit.N.y, hit.N.z, 0.0f);
+        }
+    } else {
+        p.history = ez_mul(p.history, ez_divs(ez_scale(p.f_r, p.cosine_i), p.pdf));
+    }
+    p.history = ez_mul(p.history, med.albedo);
+    if (bounce >= rd.max_bounce) return false;
+    const vec3 P = ez_add(p.o, ez_scale(p.d, t_s));
+    const float r_sel = rand01(p.seed);
+    const float r_1 = rand01(p.seed);
+    const float r_2 = rand01(p.seed);
+    bool env_pick = false;
+    float r_tri = r_sel;
+    if constexpr (ENV) {
+        const bool half = (env.p_env == 0.5f);
+        env_pick = (env.p_env == 1.0f) || (half && r_sel < 0.5f);
+        if (half) r_tri = (r_sel - 0.5f) * 2.0f;
+        if (env_pick) {
+            int texel;
+            const vec3 Le_dir = ez_env_sample(env.row_cdf, env.col_cdf, env.w, env.h, r_1, r_2, &texel);
+            const float pdf_e = env.p_env * ez_env_pdf(env.texel_pdf, env.w, env.h, Le_dir);
+            if (ez_finite(pdf_e) && pdf_e > 0.0f) {
+                sh.valid = true;
+                sh.d = Le_dir;
+                sh.tmax = EZ_INF;
+                sh.pdf = pdf_e;
+                sh.light_mat = -1;
+            }
+        }
+    }
+    if (!env_pick && lights.n > 0) {
+        const float4* lr = lights.rec + 4 * (size_t)ez_light_select(lights.cdf, lights.n, r_tri);
+        const float4 a = ldg4(lr), b = ldg4(lr + 1), c = ldg4(lr + 2), e = ldg4(lr + 3);
+        const vec3 D = ez_sub(ez_triangle_point(f4xyz(a), f4xyz(b), f4xyz(c), r_1, r_2), P);
+        const float dist = EZ_SQRT(ez_dot(D, D));
+        const vec3 Ll = ez_normalize(D);
+        const float cos_l = ez_abs(ez_dot(f4xyz(e), Ll));
+        if (cos_l != 0.0f && dist != 0.0f) {
+            sh.valid = true;
+            sh.d = Ll;
+            sh.tmax = ez_light_tmax(dist);
+            sh.pdf = ez_light_pdf(e.w, lights.w_total, dist, cos_l);
+            if constexpr (ENV) sh.pdf = sh.pdf * (1.0f - env.p_env);
+            sh.light_mat = __float_as_int(a.w);
+        }
+    }
+    if (sh.valid) {
+        sh.o = P;
+        sh.N = splat3(0.0f); sh.V = p.d; sh.history = p.history; sh.matId = EZRT_MEDIUM_VERTEX;
+    }
+    const float h_1 = rand01(p.seed);
+    const float h_2 = rand01(p.seed);
+    const vec3 L = ez_hg_sample(p.d, med.g, h_1, h_2);
+    const float pdf = ez_hg_pdf(p.d, L, med.g);
+    p.f_r = splat3(pdf);
+    p.pdf = pdf;
+    p.cosine_i = 1.0f;
+    p.o = P;
+    p.d = L;
+    return true;
+}
+
 // DEFER_NEE (wavefront pipeline, IS/MIS mode): the shadow ray carries the inputs of nee_contrib instead of its value -- the
 // BRDF / environment evaluation of the light sample runs after the shadow pass, only for the rays that got through, and is
 // no longer part of k_shade (5104 instructions, instruction-fetch bound).
@@ -1939,17 +2024,27 @@ __device__ __forceinline__ void tri_vertices(const SceneDev& sc, int tri, bool a
 // TRANS (light sampling mode with EZRT_PARAM_TRANSMISSION, ezrt_math.h, DESIGN.md section 12): a hit on a material with t > 0
 // samples and evaluates the mixture with the rough dielectric.  p.cosine_i keeps dot(N, L)'s sign: a BSDF sample below the
 // surface weighs 1 where it hits an emitter or leaves the scene.  The shadow ray's material id is ~matId for a hit from inside.
-template <int MODE, bool DEFER_NEE = false, bool AOV = false, bool ENV = false, bool TRANS = false>
+// MEDIUM (light sampling mode with EZRT_PARAM_MEDIUM, ezrt_math.h, DESIGN.md section 14; not with TRANS): the free flight of the
+// traced segment comes first; a path that scatters takes a medium vertex (medium_step) instead of its hit or miss.
+template <int MODE, bool DEFER_NEE = false, bool AOV = false, bool ENV = false, bool TRANS = false, bool MEDIUM = false>
 __device__ __forceinline__ bool shade_step(const SceneDev& sc, const RenderDev& rd, int bounce, PathRegs& p, float hit_t,
                                            int hit_tri, uint32_t px, uint32_t py, float2 sob, vec3& Lo, vec3& Le,
                                            bool& primary_miss, ShadowRay& sh, float4* aov_rec = nullptr, LightsDev lights = LightsDev{},
-                                           EnvDev env = EnvDev{}) {
+                                           EnvDev env = EnvDev{}, MediumDev med = MediumDev{}) {
     sh.valid = false;
     const int mode = (MODE < 0) ? rd.mode : MODE;
     const bool is_mode = (mode == EZRT_MODE_DISNEY_IS_MIS_P5);
     // the light sampling mode exists only as k_shade<EZRT_MODE_DISNEY_LIGHTS> (the megakernel, MODE < 0, rejects it)
     constexpr bool lights_mode = (MODE == EZRT_MODE_DISNEY_LIGHTS);
     const bool below = TRANS && p.cosine_i < 0.0f;   // the BSDF sample went below the surface: no light strategy reaches it
+    if constexpr (MEDIUM) {
+        static_assert(lights_mode && !TRANS, "the medium is rendered in the light sampling mode, without transmission");
+        if (bounce > 0 && p.pdf <= 0.0f) return false;   // P5/fsh:865, before the free flight's draw
+        float t_s;
+        const float t_end = (hit_tri < 0) ? __int_as_float(0x7f800000) : hit_t;
+        if (ez_medium_flight(&med, p.o, p.d, t_end, &p.seed, &t_s))
+            return medium_step<AOV, ENV>(sc, rd, bounce, p, t_s, hit_t, hit_tri, Lo, Le, primary_miss, sh, aov_rec, lights, env, med);
+    }
     if (bounce == 0) {
         Lo = splat3(0.0f);
         Le = splat3(0.0f);

@@ -145,6 +145,13 @@ struct EnvDev {
 // of their own, after the others, so that no other kernel's parameter layout moves.
 typedef ez_lens LensDev;
 
+// The homogeneous medium of EZRT_PARAM_MEDIUM (ezrt_math.h, DESIGN.md section 14): sigma_t, albedo, g and the box, copied from the
+// scene when the render is enqueued.  Passed to the medium instantiations (k_shade<.., MEDIUM>, k_nee<.., MEDIUM>) as a parameter of
+// their own, after the others.  A medium vertex's shadow ray carries EZRT_MEDIUM_VERTEX as its material id (ShadowQueue::ray_d.w;
+// no ~matId there, as EZRT_PARAM_TRANSMISSION is excluded) and its propagation direction d in place of V.
+typedef ez_medium MediumDev;
+#define EZRT_MEDIUM_VERTEX (-1)
+
 // A shadow ray and what k_nee needs to evaluate the light sample's contribution once the ray got through (nee_contrib):
 // the BRDF / environment evaluation of the light sample is done after the shadow pass, for unoccluded rays only.
 #define EZRT_SHADOW_SLOT_BYTES (5 * 16 + 1)

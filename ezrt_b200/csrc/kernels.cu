@@ -545,13 +545,14 @@ __global__ void __launch_bounds__(EZRT_EXTEND_MAX_THREADS, EZRT_EXTEND_LB_BLOCKS
 // it from Lo.w == 1).  The plain instantiations never touch aov_rec.
 // ENV (light sampling mode with EZRT_PARAM_ENV_LIGHT): the map is one more light, sampled from the table env (shade_step).
 // TRANS (light sampling mode with EZRT_PARAM_TRANSMISSION): materials with a dielectric lobe (shade_step).
-template <int MODE, bool LIST, bool AOV = false, bool ENV = false, bool TRANS = false>
+// MEDIUM (light sampling mode with EZRT_PARAM_MEDIUM): the homogeneous medium med (shade_step, medium_step).
+template <int MODE, bool LIST, bool AOV = false, bool ENV = false, bool TRANS = false, bool MEDIUM = false>
 __global__ void __launch_bounds__(128, EZRT_SHADE_MIN_BLOCKS) k_shade(SceneDev sc, RenderDev rd, const TileDev* __restrict__ tiles, int bounce,
                                                uint32_t batch_first_frame, PathQueue qin, const uint32_t* __restrict__ in_count,
                                                PathQueue qout, uint32_t* out_count, ShadowQueue sq, uint32_t* s_count,
                                                float4* __restrict__ Lo, float4* __restrict__ Le, uint32_t n_fused, uint32_t n_frames,
                                                const uint32_t* __restrict__ list, const float2* __restrict__ side_hit,
-                                               float4* __restrict__ aov_rec, LightsDev lights, EnvDev env) {
+                                               float4* __restrict__ aov_rec, LightsDev lights, EnvDev env, MediumDev med) {
     // The Sobol pair of (bounce, frame) is the same for every pixel of a frame (P5/fsh:361-376: up to 2 x 32 table XORs per path): each
     // block computes the pairs of the batch's frames once into shared memory (batches of more than EZRT_SOBOL_TABLE frames compute per path).
     __shared__ float2 s_sobol[EZRT_SOBOL_TABLE];
@@ -675,8 +676,9 @@ __global__ void __launch_bounds__(128, EZRT_SHADE_MIN_BLOCKS) k_shade(SceneDev s
             }
 #endif
             if (LIST || __float_as_int(hit.y) != EZRT_TRI_PENDING) {   // pending: deferred by the accel kernel, shaded by the LIST pass
-                alive = shade_step<MODE, MODE == EZRT_MODE_DISNEY_IS_MIS_P5, AOV, ENV, TRANS>(sc, rd, bounce, p, hit.x, __float_as_int(hit.y), px, py, sob, lo, le,
-                                                                                             pmiss, sh, AOV ? aov_rec + 2 * (size_t)slot : nullptr, lights, env);
+                alive = shade_step<MODE, MODE == EZRT_MODE_DISNEY_IS_MIS_P5, AOV, ENV, TRANS, MEDIUM>(sc, rd, bounce, p, hit.x, __float_as_int(hit.y), px, py, sob,
+                                                                                                     lo, le, pmiss, sh, AOV ? aov_rec + 2 * (size_t)slot : nullptr,
+                                                                                                     lights, env, med);
                 if (bounce == 0) {
                     // Le is zero for every surface that does not emit: it is stored (and read back by k_blend) only otherwise.
                     // color = Le + Lo with Le = +-0 is Lo bit for bit, because Lo is never -0.0 (it starts at +0.0 and only grows by additions)
@@ -719,8 +721,11 @@ __global__ void __launch_bounds__(128, EZRT_SHADE_MIN_BLOCKS) k_shade(SceneDev s
 // MODE = EZRT_MODE_DISNEY_LIGHTS: the light samples on the emissive triangles (nee_light_contrib; view.w = pdf, hist.w = the light's material);
 // ENV: and on the environment map (hist.w = -1: the light's colour is the map's in the sample's direction).
 // TRANS: evaluated with the mixture of the shading point's material (nee_trans_contrib); ray_d.w = ~matId for a hit from inside.
-template <int MODE, bool ENV = false, bool TRANS = false>
-__global__ void __launch_bounds__(128, 8) k_nee(SceneDev sc, RenderDev rd, ShadowQueue sq, const uint32_t* __restrict__ s_count, float4* __restrict__ Lo) {
+// MEDIUM: every contribution times the shadow ray's transmittance through the medium med; a medium vertex's (ray_d.w =
+// EZRT_MEDIUM_VERTEX, view = d) is evaluated with the phase function (nee_medium_contrib).
+template <int MODE, bool ENV = false, bool TRANS = false, bool MEDIUM = false>
+__global__ void __launch_bounds__(128, 8) k_nee(SceneDev sc, RenderDev rd, ShadowQueue sq, const uint32_t* __restrict__ s_count, float4* __restrict__ Lo,
+                                                MediumDev med) {
     __shared__ uint32_t s_scan[34];
     __shared__ uint32_t s_total;
     __shared__ uint32_t s_list[512];
@@ -742,9 +747,22 @@ __global__ void __launch_bounds__(128, 8) k_nee(SceneDev sc, RenderDev rd, Shado
             const float4 o4 = __ldcs(sq.ray_o + j), d4 = __ldcs(sq.ray_d + j), n4 = __ldcs(sq.nrm + j), v4 = __ldcs(sq.view + j), h4 = __ldcs(sq.hist + j);
             const uint32_t slot = __float_as_uint(o4.w);
             const int m_raw = __float_as_int(d4.w);
+            vec3 c;
+            if constexpr (MEDIUM) {
+                static_assert(MODE == EZRT_MODE_DISNEY_LIGHTS && !TRANS, "the medium is rendered in the light sampling mode, without transmission");
+                const vec3 Ld = ez_v3(d4.x, d4.y, d4.z);
+                const int lm = __float_as_int(h4.w);
+                const vec3 E = (ENV && lm < 0) ? hdr_color(sc, rd, Ld, EZRT_MODE_DISNEY_LIGHTS) : load_emissive(sc, lm);
+                if (m_raw == EZRT_MEDIUM_VERTEX) c = nee_medium_contrib(ez_v3(v4.x, v4.y, v4.z), Ld, med.g, ez_v3(h4.x, h4.y, h4.z), E, v4.w);
+                else c = nee_light_contrib(ez_v3(v4.x, v4.y, v4.z), ez_v3(n4.x, n4.y, n4.z), Ld, load_material(sc, m_raw), ez_v3(h4.x, h4.y, h4.z), E, v4.w);
+                c = ez_scale(c, ez_medium_transmittance(&med, ez_v3(o4.x, o4.y, o4.z), Ld, ez_medium_light_dist(n4.w, ENV && lm < 0)));
+                float4 lo = Lo[slot];
+                lo.x += c.x; lo.y += c.y; lo.z += c.z;
+                Lo[slot] = lo;
+                continue;
+            }
             const int m_id = (TRANS && m_raw < 0) ? ~m_raw : m_raw;
             const MaterialDev mat = load_material(sc, m_id);
-            vec3 c;
             if (MODE == EZRT_MODE_DISNEY_LIGHTS && TRANS) {
                 const vec3 Ld = ez_v3(d4.x, d4.y, d4.z);
                 const int lm = __float_as_int(h4.w);
@@ -1343,14 +1361,21 @@ void launch_shadow_accel(const SceneDev& sc, ShadowQueue sq, const uint32_t* s_c
 void launch_shade(const SceneDev& sc, const RenderDev& rd, const TileDev* tiles, int bounce, uint32_t batch_first_frame,
                   PathQueue qin, const uint32_t* in_count, PathQueue qout, uint32_t* out_count, ShadowQueue sq,
                   uint32_t* s_count, float4* Lo, float4* Le, uint32_t n_max, uint32_t n_fused, uint32_t n_frames, int n_sms, cudaStream_t st,
-                  float4* aov_rec, LightsDev lights, EnvDev env, bool trans) {
+                  float4* aov_rec, LightsDev lights, EnvDev env, bool trans, const MediumDev* med) {
     int blocks = std::min(div_up(n_max, 128), n_sms * 4 * EZRT_SHADE_MIN_BLOCKS);
     if (blocks < 1) blocks = 1;
-#define EZRT_LAUNCH_SHADE_E(M, E, T)                                                                                                          \
-    if (aov_rec) k_shade<M, false, true, E, T><<<blocks, 128, 0, st>>>(sc, rd, tiles, bounce, batch_first_frame, qin, in_count, qout, out_count, sq, s_count, Lo, Le, \
-                                                                       n_fused, n_frames, nullptr, nullptr, aov_rec, lights, env);           \
-    else k_shade<M, false, false, E, T><<<blocks, 128, 0, st>>>(sc, rd, tiles, bounce, batch_first_frame, qin, in_count, qout, out_count, sq, s_count, Lo, Le, n_fused, n_frames, nullptr, nullptr, nullptr, lights, env)
+    const MediumDev m = med ? *med : MediumDev{};
+#define EZRT_LAUNCH_SHADE_X(M, E, T, X)                                                                                                       \
+    if (aov_rec) k_shade<M, false, true, E, T, X><<<blocks, 128, 0, st>>>(sc, rd, tiles, bounce, batch_first_frame, qin, in_count, qout, out_count, sq, s_count, Lo, \
+                                                                          Le, n_fused, n_frames, nullptr, nullptr, aov_rec, lights, env, m);   \
+    else k_shade<M, false, false, E, T, X><<<blocks, 128, 0, st>>>(sc, rd, tiles, bounce, batch_first_frame, qin, in_count, qout, out_count, sq, s_count, Lo, Le, n_fused, n_frames, nullptr, nullptr, nullptr, lights, env, m)
+#define EZRT_LAUNCH_SHADE_E(M, E, T) EZRT_LAUNCH_SHADE_X(M, E, T, false)
 #define EZRT_LAUNCH_SHADE(M) EZRT_LAUNCH_SHADE_E(M, false, false)
+    if (rd.mode == EZRT_MODE_DISNEY_LIGHTS && med) {   // the homogeneous medium (EZRT_PARAM_MEDIUM; never with trans)
+        if (env.row_cdf) { EZRT_LAUNCH_SHADE_X(EZRT_MODE_DISNEY_LIGHTS, true, false, true); }
+        else { EZRT_LAUNCH_SHADE_X(EZRT_MODE_DISNEY_LIGHTS, false, false, true); }
+        return;
+    }
     if (rd.mode == EZRT_MODE_DISNEY_LIGHTS && trans) {   // materials with a dielectric lobe (EZRT_PARAM_TRANSMISSION)
         if (env.row_cdf) { EZRT_LAUNCH_SHADE_E(EZRT_MODE_DISNEY_LIGHTS, true, true); }
         else { EZRT_LAUNCH_SHADE_E(EZRT_MODE_DISNEY_LIGHTS, false, true); }
@@ -1369,6 +1394,7 @@ void launch_shade(const SceneDev& sc, const RenderDev& rd, const TileDev* tiles,
     }
 #undef EZRT_LAUNCH_SHADE
 #undef EZRT_LAUNCH_SHADE_E
+#undef EZRT_LAUNCH_SHADE_X
 }
 // The accel policy's deferred lane (side stream, beside the main k_shade of the same bounce): exact traversal of the deferred
 // rays into side_hit, then their shading -- both do nothing if more than EZRT_SIDE_CAP rays were deferred (then
@@ -1376,14 +1402,21 @@ void launch_shade(const SceneDev& sc, const RenderDev& rd, const TileDev* tiles,
 void launch_deferred_lane(const SceneDev& sc, const RenderDev& rd, const TileDev* tiles, int bounce, uint32_t batch_first_frame, PathQueue qin,
                           const uint32_t* defer_list, const uint32_t* defer_count, uint32_t* defer_work, float2* side_hit, PathQueue qout,
                           uint32_t* out_count, ShadowQueue sq, uint32_t* s_count, float4* Lo, float4* Le, uint32_t n_fused, uint32_t n_frames,
-                          int n_sms, cudaStream_t st, float4* aov_rec, LightsDev lights, EnvDev env, bool trans) {
+                          int n_sms, cudaStream_t st, float4* aov_rec, LightsDev lights, EnvDev env, bool trans, const MediumDev* med) {
     launch_extend(sc, true, false, qin, defer_count, defer_work, defer_list, 1, EZRT_SIDE_CAP, n_sms, st, side_hit, 1);
     const int blocks = 8;
-#define EZRT_LAUNCH_SHADE_E(M, E, T)                                                                                                          \
-    if (aov_rec) k_shade<M, true, true, E, T><<<blocks, 128, 0, st>>>(sc, rd, tiles, bounce, batch_first_frame, qin, defer_count, qout, out_count, sq, s_count, Lo, \
-                                                                      Le, n_fused, n_frames, defer_list, side_hit, aov_rec, lights, env);      \
-    else k_shade<M, true, false, E, T><<<blocks, 128, 0, st>>>(sc, rd, tiles, bounce, batch_first_frame, qin, defer_count, qout, out_count, sq, s_count, Lo, Le, n_fused, n_frames, defer_list, side_hit, nullptr, lights, env)
+    const MediumDev m = med ? *med : MediumDev{};
+#define EZRT_LAUNCH_SHADE_X(M, E, T, X)                                                                                                       \
+    if (aov_rec) k_shade<M, true, true, E, T, X><<<blocks, 128, 0, st>>>(sc, rd, tiles, bounce, batch_first_frame, qin, defer_count, qout, out_count, sq, s_count, Lo, \
+                                                                         Le, n_fused, n_frames, defer_list, side_hit, aov_rec, lights, env, m);   \
+    else k_shade<M, true, false, E, T, X><<<blocks, 128, 0, st>>>(sc, rd, tiles, bounce, batch_first_frame, qin, defer_count, qout, out_count, sq, s_count, Lo, Le, n_fused, n_frames, defer_list, side_hit, nullptr, lights, env, m)
+#define EZRT_LAUNCH_SHADE_E(M, E, T) EZRT_LAUNCH_SHADE_X(M, E, T, false)
 #define EZRT_LAUNCH_SHADE(M) EZRT_LAUNCH_SHADE_E(M, false, false)
+    if (rd.mode == EZRT_MODE_DISNEY_LIGHTS && med) {
+        if (env.row_cdf) { EZRT_LAUNCH_SHADE_X(EZRT_MODE_DISNEY_LIGHTS, true, false, true); }
+        else { EZRT_LAUNCH_SHADE_X(EZRT_MODE_DISNEY_LIGHTS, false, false, true); }
+        return;
+    }
     if (rd.mode == EZRT_MODE_DISNEY_LIGHTS && trans) {
         if (env.row_cdf) { EZRT_LAUNCH_SHADE_E(EZRT_MODE_DISNEY_LIGHTS, true, true); }
         else { EZRT_LAUNCH_SHADE_E(EZRT_MODE_DISNEY_LIGHTS, false, true); }
@@ -1402,15 +1435,19 @@ void launch_deferred_lane(const SceneDev& sc, const RenderDev& rd, const TileDev
     }
 #undef EZRT_LAUNCH_SHADE
 #undef EZRT_LAUNCH_SHADE_E
+#undef EZRT_LAUNCH_SHADE_X
 }
 void launch_nee(const SceneDev& sc, const RenderDev& rd, ShadowQueue sq, const uint32_t* s_count, float4* Lo, uint32_t n_max, int n_sms, cudaStream_t st,
-                bool env, bool trans) {
+                bool env, bool trans, const MediumDev* med) {
     const int blocks = std::max(1, std::min(div_up(n_max, 512), n_sms * 8));
-    if (rd.mode == EZRT_MODE_DISNEY_LIGHTS && trans && env) k_nee<EZRT_MODE_DISNEY_LIGHTS, true, true><<<blocks, 128, 0, st>>>(sc, rd, sq, s_count, Lo);
-    else if (rd.mode == EZRT_MODE_DISNEY_LIGHTS && trans) k_nee<EZRT_MODE_DISNEY_LIGHTS, false, true><<<blocks, 128, 0, st>>>(sc, rd, sq, s_count, Lo);
-    else if (rd.mode == EZRT_MODE_DISNEY_LIGHTS && env) k_nee<EZRT_MODE_DISNEY_LIGHTS, true><<<blocks, 128, 0, st>>>(sc, rd, sq, s_count, Lo);
-    else if (rd.mode == EZRT_MODE_DISNEY_LIGHTS) k_nee<EZRT_MODE_DISNEY_LIGHTS><<<blocks, 128, 0, st>>>(sc, rd, sq, s_count, Lo);
-    else k_nee<EZRT_MODE_DISNEY_IS_MIS_P5><<<blocks, 128, 0, st>>>(sc, rd, sq, s_count, Lo);
+    const MediumDev m = med ? *med : MediumDev{};
+    if (rd.mode == EZRT_MODE_DISNEY_LIGHTS && med && env) k_nee<EZRT_MODE_DISNEY_LIGHTS, true, false, true><<<blocks, 128, 0, st>>>(sc, rd, sq, s_count, Lo, m);
+    else if (rd.mode == EZRT_MODE_DISNEY_LIGHTS && med) k_nee<EZRT_MODE_DISNEY_LIGHTS, false, false, true><<<blocks, 128, 0, st>>>(sc, rd, sq, s_count, Lo, m);
+    else if (rd.mode == EZRT_MODE_DISNEY_LIGHTS && trans && env) k_nee<EZRT_MODE_DISNEY_LIGHTS, true, true><<<blocks, 128, 0, st>>>(sc, rd, sq, s_count, Lo, m);
+    else if (rd.mode == EZRT_MODE_DISNEY_LIGHTS && trans) k_nee<EZRT_MODE_DISNEY_LIGHTS, false, true><<<blocks, 128, 0, st>>>(sc, rd, sq, s_count, Lo, m);
+    else if (rd.mode == EZRT_MODE_DISNEY_LIGHTS && env) k_nee<EZRT_MODE_DISNEY_LIGHTS, true><<<blocks, 128, 0, st>>>(sc, rd, sq, s_count, Lo, m);
+    else if (rd.mode == EZRT_MODE_DISNEY_LIGHTS) k_nee<EZRT_MODE_DISNEY_LIGHTS><<<blocks, 128, 0, st>>>(sc, rd, sq, s_count, Lo, m);
+    else k_nee<EZRT_MODE_DISNEY_IS_MIS_P5><<<blocks, 128, 0, st>>>(sc, rd, sq, s_count, Lo, m);
 }
 
 // ------------------------------------------------------------------------------------------

@@ -45,7 +45,8 @@ void launch_shade(const SceneDev& sc, const RenderDev& rd, const TileDev* tiles,
                   float4* aov_rec = nullptr,   // aov_rec: feature-buffer render, bounce 0 writes the first-hit records (k_shade<.., AOV>)
                   LightsDev lights = LightsDev{},    // the light table (light sampling mode)
                   EnvDev env = EnvDev{},             // the environment table (light sampling mode with EZRT_PARAM_ENV_LIGHT; row_cdf null: none)
-                  bool trans = false);               // light sampling mode with EZRT_PARAM_TRANSMISSION (k_shade<.., TRANS>)
+                  bool trans = false,                // light sampling mode with EZRT_PARAM_TRANSMISSION (k_shade<.., TRANS>)
+                  const MediumDev* med = nullptr);   // light sampling mode with EZRT_PARAM_MEDIUM and sigma_t > 0 (k_shade<.., MEDIUM>)
 void launch_extend_camera(const SceneDev& sc, const RenderDev& rd, const TileDev* tiles, uint32_t batch_first_frame, uint32_t n_slots, uint32_t n_frames, PathQueue q,
                           uint32_t* work, uint32_t* defer_list, uint32_t* defer_count, uint32_t* defer_work, int n_sms, unsigned long long* counts,
                           cudaStream_t st, int exact_gate = 0);
@@ -53,11 +54,12 @@ void launch_deferred_lane(const SceneDev& sc, const RenderDev& rd, const TileDev
                           const uint32_t* defer_list, const uint32_t* defer_count, uint32_t* defer_work, float2* side_hit, PathQueue qout,
                           uint32_t* out_count, ShadowQueue sq, uint32_t* s_count, float4* Lo, float4* Le, uint32_t n_fused, uint32_t n_frames,
                           int n_sms, cudaStream_t st, float4* aov_rec = nullptr, LightsDev lights = LightsDev{}, EnvDev env = EnvDev{},
-                          bool trans = false);
+                          bool trans = false, const MediumDev* med = nullptr);
 // after a shadow pass (accel or exact, including the exact pass over deferred shadow rays): contributions of the unoccluded light samples
-// env: the light sampling mode's queue also holds environment samples (hist.w = -1); trans: EZRT_PARAM_TRANSMISSION (k_nee<.., TRANS>)
+// env: the light sampling mode's queue also holds environment samples (hist.w = -1); trans: EZRT_PARAM_TRANSMISSION (k_nee<.., TRANS>);
+// med: EZRT_PARAM_MEDIUM (k_nee<.., MEDIUM>: the shadow rays' transmittance, the medium vertices' phase function)
 void launch_nee(const SceneDev& sc, const RenderDev& rd, ShadowQueue sq, const uint32_t* s_count, float4* Lo, uint32_t n_max, int n_sms, cudaStream_t st,
-                bool env = false, bool trans = false);
+                bool env = false, bool trans = false, const MediumDev* med = nullptr);
 // light table of the light sampling mode: every triangle's weight (w: n_triangles floats) -> the lights in triangle order
 // (idx_out, w_out: n floats each; *count = K) -> their 64-byte records (rec: 4 K float4)
 void launch_light_weights(const SceneDev& sc, float* w, cudaStream_t st);

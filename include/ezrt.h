@@ -125,7 +125,7 @@ typedef struct ezrt_render_params {
    (1 - metallic) > 0 scatters by (1 - t) * the reference BRDF + t * a rough dielectric (GGX, exact Fresnel; reflection
    untinted, refraction tinted by baseColor; ezrt_math.h, DESIGN.md section 12).  The outside of every mesh is vacuum: a hit
    from the back of a triangle (geometric normal) leaves the medium of index IOR, so transmissive meshes must be closed and
-   wound outward.  |IOR - 1| <= 2^-8 is an index-matched pass-through; IOR <= 0 or not finite is opaque.  Light samples and
+   wound outward (so EZRT_PARAM_MEDIUM is rejected beside this flag).  |IOR - 1| <= 2^-8 is an index-matched pass-through; IOR <= 0 or not finite is opaque.  Light samples and
    shadow rays treat transmissive triangles as opaque: light through glass arrives by BSDF samples only.  A scene without a
    material of t > 0 renders as without the flag, bit for bit.  Accepted by ezrt_render[_device],
    ezrt_render_adaptive[_device] and ezrt_render_aov[_device]. */
@@ -139,6 +139,28 @@ typedef struct ezrt_render_params {
    length.  Accepted by ezrt_render[_device], ezrt_render_adaptive[_device] and ezrt_render_aov[_device]; a feature-buffer
    render's depth is the first hit's distance from the lens point. */
 #define EZRT_PARAM_THIN_LENS 8
+/* ezrt_render_params.reserved[0], EZRT_MODE_DISNEY_LIGHTS on the wavefront pipeline only, with or without EZRT_PARAM_ENV_LIGHT and
+   EZRT_PARAM_THIN_LENS: the scene's homogeneous medium (ezrt_scene_set_medium) is rendered.  Every traced segment that overlaps the
+   medium's box draws a free-flight distance; a path that scatters there takes a medium vertex (one bounce): a light sample evaluated
+   with the Henyey-Greenstein phase function and a phase-function sample of the next direction.  Every light sample's contribution
+   (from surfaces too) is multiplied by the transmittance of its shadow ray.  Opaque objects in the box stay surfaces; the feature
+   buffers still describe the first surface along the camera ray.  ezrt_math.h and DESIGN.md section 14 give the arithmetic.
+   Invalid (EZRT_ERR_INVALID) without a medium set on the scene, in another mode, with the megakernel, and with
+   EZRT_PARAM_TRANSMISSION (glass is defined with vacuum outside; a medium around it would need a medium stack).  Accepted by
+   ezrt_render[_device], ezrt_render_adaptive[_device] and ezrt_render_aov[_device]. */
+#define EZRT_PARAM_MEDIUM 16
+
+/* The homogeneous medium of EZRT_PARAM_MEDIUM: a grey extinction, an RGB single-scattering albedo and a Henyey-Greenstein
+   asymmetry g (> 0: forward scattering), filling the axis-aligned box [box_min, box_max] (a box of zero extent on an axis holds
+   no medium). */
+typedef struct ezrt_medium {
+    float sigma_t;     /* extinction per unit length, finite and >= 0 (0: the flagged render is mode 4's) */
+    float albedo[3];   /* single-scattering albedo, each in [0, 1] */
+    float g;           /* Henyey-Greenstein asymmetry, -1 < g < 1 */
+    float box_min[3];  /* finite, box_min <= box_max on every axis */
+    float box_max[3];
+    int32_t reserved;  /* 0 */
+} ezrt_medium;
 
 typedef struct ezrt_counters {
     uint64_t rays;          /* hitBVH invocations: primary + bounce + shadow (SURVEY 8d)     */
@@ -174,6 +196,11 @@ int ezrt_scene_create(int device, const float* tris, int n_triangles, const floa
                       const float* hdr, const float* hdr_cache, int hdr_w, int hdr_h,
                       int hdr_filter_linear, ezrt_scene** out_scene);
 int ezrt_scene_destroy(ezrt_scene* scene);
+/* Sets the scene's homogeneous medium (a copy of *medium), or clears it (medium NULL).  Returns EZRT_ERR_INVALID, and keeps the
+ * previous medium, for a non-finite or negative sigma_t, an albedo component outside [0, 1] or NaN, |g| >= 1 or NaN, a non-finite
+ * box corner, box_min > box_max on an axis, or reserved != 0.  The medium travels to the kernels by value when a render is
+ * enqueued: changing it afterwards does not affect renders already enqueued. */
+int ezrt_scene_set_medium(ezrt_scene* scene, const ezrt_medium* medium);
 
 /* render(width,height,spp) -> framebuffer: equals `spp` consecutive display() calls
  * (P5/main.cpp:697-748) each drawing pass1 (P5/fsh:894-949) and copying to lastFrame.

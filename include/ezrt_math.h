@@ -659,4 +659,102 @@ EZ_HD void ez_lens_ray(const ez_lens* L, ez_vec3 dir_pin, float r_a, float r_b, 
     *d = ez_normalize(ez_sub(F, *o));
 }
 
+/* ------------------------------------------------------------------ homogeneous medium (DESIGN.md section 14)
+ * Mode EZRT_MODE_DISNEY_LIGHTS with EZRT_PARAM_MEDIUM: grey extinction sigma_t, albedo, Henyey-Greenstein g, box [bmin, bmax].
+ * Free flight, on every traced segment (origin o, direction d, hit distance t_hit, or a miss) of a path, camera rays included:
+ *   t_end = t_hit, or +inf for a miss.  At the start of the shading step (at bounce >= 1 after the check of the previous sample's
+ *   pdf), ez_medium_flight: if sigma_t > 0 and ez_box_overlap(o, d, bmin, bmax, t_end) = [t0, t1] with t0 < t1, one draw
+ *   r_m = rand01 and t_s = t0 + ez_free_flight(r_m, sigma_t); the path scatters iff t_s < t1.  A segment without overlap draws
+ *   nothing.  A path that does not scatter reaches its hit, or leaves the scene, exactly as in mode 4.
+ * Medium vertex (the path scatters) at bounce b, P = o + d t_s:
+ *   b == 0: Lo = 0, no emission; a camera ray that missed is a primary miss (its colour is Lo), one that hit keeps its first-hit
+ *   features.  b >= 1: history *= f_r cos / pdf as at a surface.  Then history *= albedo; b >= max_bounce: the path ends.
+ *   Draws: r_sel, r_1, r_2, then h_1, h_2 (rand01 each).  The light sample is the surface's (sections 10, 11: the map with P_env,
+ *   else the triangles) at P with neither the hemisphere test nor the self exclusion: a triangle sample needs cos_l != 0 and
+ *   dist != 0, a map sample a finite pdf_e > 0.  If its shadow ray is lit (p = ez_hg_pdf(d, L_l, g)):
+ *     Lo += ((history * mis(pdf_l, p) * E * splat(p)) * 1 / pdf_l) * T   (left to right; T = ez_medium_transmittance)
+ *   L = ez_hg_sample(d, g, h_1, h_2); the path record is (f_r, pdf, cos) = (splat(p), p, 1) with p = ez_hg_pdf(d, L, g), so that the
+ *   emission and environment it reaches are MIS-weighted by mode 4's code unchanged.
+ * Every lit light sample (surface or medium vertex) is multiplied by T = ez_medium_transmittance(o, L_l, ez_medium_light_dist(tmax,
+ * map)) of its shadow ray after its mode-4 value: the contribution times T, with T = 1 when the ray does not overlap the box.
+ * Limit: rays from a medium vertex are traced like every other ray, so a triangle closer than the traversal's minimum hit distance
+ * (0.0005, the reference's hitTriangle) is not seen by them.  A vertex within 0.0005 of a surface can send its phase sample or its
+ * shadow ray through that surface: with a mean free path near or below 0.0005 (sigma_t >~ 2000) light leaks into and past opaque
+ * objects.  The definition is what the kernels compute either way; it is the physics that degrades there. */
+struct ez_medium {
+    float sigma_t;
+    ez_vec3 albedo;
+    float g;
+    ez_vec3 bmin, bmax;
+};
+typedef struct ez_medium ez_medium;
+/* the overlap [*t0, *t1] of the segment o + t d, 0 <= t <= t_end, with the box; 1 iff it has positive length (t0 < t1) and the box
+ * has positive extent on every axis.  Per axis a: d_a == 0: no overlap if o_a < bmin_a or o_a > bmax_a, else no bound; otherwise
+ * ta = (bmin_a - o_a) / d_a, tb = (bmax_a - o_a) / d_a, t0 = max(t0, min(ta, tb)), t1 = min(t1, max(ta, tb)) (from 0, t_end) */
+EZ_HD int ez_box_overlap(ez_vec3 o, ez_vec3 d, ez_vec3 bmin, ez_vec3 bmax, float t_end, float* t0, float* t1) {
+    const float oo[3] = {o.x, o.y, o.z}, dd[3] = {d.x, d.y, d.z};
+    const float lo[3] = {bmin.x, bmin.y, bmin.z}, hi[3] = {bmax.x, bmax.y, bmax.z};
+    float a = 0.0f, b = t_end;
+    for (int k = 0; k < 3; k++) {
+        if (!(lo[k] < hi[k])) return 0;
+        if (dd[k] == 0.0f) {
+            if (oo[k] < lo[k] || oo[k] > hi[k]) return 0;
+            continue;
+        }
+        const float ta = EZ_DIV(lo[k] - oo[k], dd[k]), tb = EZ_DIV(hi[k] - oo[k], dd[k]);
+        a = ez_max(a, ez_min(ta, tb));
+        b = ez_min(b, ez_max(ta, tb));
+    }
+    *t0 = a;
+    *t1 = b;
+    return a < b;
+}
+/* the free-flight distance of the draw r: -log(1 - r) / sigma_t */
+EZ_HD float ez_free_flight(float r, float sigma_t) { return EZ_DIV(-ez_log(1.0f - r), sigma_t); }
+/* the free flight of a segment (t_end: the hit distance, +inf for a miss): 1 with *t_s if the path scatters.  Draws r_m from *seed
+ * only when the segment overlaps the medium. */
+EZ_HD int ez_medium_flight(const ez_medium* m, ez_vec3 o, ez_vec3 d, float t_end, uint32_t* seed, float* t_s) {
+    float t0, t1;
+    if (!(m->sigma_t > 0.0f) || !ez_box_overlap(o, d, m->bmin, m->bmax, t_end, &t0, &t1)) return 0;
+    const float t = t0 + ez_free_flight(ez_rand01(seed), m->sigma_t);
+    *t_s = t;
+    return t < t1;
+}
+/* the transmittance of the shadow ray o + t d, 0 <= t <= L: exp(-sigma_t |[0, L] & box|), exactly 1 without overlap */
+EZ_HD float ez_medium_transmittance(const ez_medium* m, ez_vec3 o, ez_vec3 d, float L) {
+    float t0, t1;
+    if (!(m->sigma_t > 0.0f) || !ez_box_overlap(o, d, m->bmin, m->bmax, L, &t0, &t1)) return 1.0f;
+    return ez_exp(-(m->sigma_t * (t1 - t0)));
+}
+/* L of a light sample's shadow ray: the light's distance recovered from the bound tmax = ez_light_tmax(dist), or +inf for the map
+ * (the box exit) */
+EZ_HD float ez_medium_light_dist(float tmax, int map) { return map ? ez_u2f(0x7f800000u) : EZ_DIV(tmax, 0.9990234375f); }
+/* Henyey-Greenstein density (per steradian) of the direction L after propagation along d (unit vectors; cos = their angle's cosine):
+ * (1 - g^2) / (4 pi den^1.5), den = 1 + g^2 - 2 g cos, evaluated without cancellation as (1 - g)^2 + g |d - L|^2 for g >= 0 and
+ * (1 + g)^2 - g |d + L|^2 for g < 0 (|d -+ L|^2 = 2 (1 -+ cos)) */
+EZ_HD float ez_hg_pdf(ez_vec3 d, ez_vec3 L, float g) {
+    float den;
+    if (g >= 0.0f) {
+        const ez_vec3 v = ez_sub(d, L);
+        den = (1.0f - g) * (1.0f - g) + g * ez_dot(v, v);
+    } else {
+        const ez_vec3 v = ez_add(d, L);
+        den = (1.0f + g) * (1.0f + g) - g * ez_dot(v, v);
+    }
+    return EZ_DIV((1.0f - g) * (1.0f + g), (4.0f * EZ_PI) * (den * EZ_SQRT(den)));
+}
+/* the exact inversion of the Henyey-Greenstein law of cos (h_1 = its cdf) and phi = 2 pi h_2, in the frame of d
+ * (ez_to_normal_hemisphere).  With a = 1 - g + 2 g h_1 (> 0):  1 - cos = 2 (1 - g)^2 (1 - h_1) (1 + g h_1) / a^2,
+ * 1 + cos = 2 (1 + g)^2 h_1 (1 - g + g h_1) / a^2;  cos from the smaller of the two, sin = sqrt((1 - cos)(1 + cos)) */
+EZ_HD ez_vec3 ez_hg_sample(ez_vec3 d, float g, float h_1, float h_2) {
+    const float a = (1.0f - g) + (2.0f * g) * h_1;
+    const float a2 = a * a;
+    const float qm = EZ_DIV((2.0f * ((1.0f - g) * (1.0f - g))) * ((1.0f - h_1) * (1.0f + g * h_1)), a2);
+    const float qp = EZ_DIV((2.0f * ((1.0f + g) * (1.0f + g))) * (h_1 * ((1.0f - g) + g * h_1)), a2);
+    const float c = (qm < qp) ? 1.0f - qm : qp - 1.0f;
+    const float s = EZ_SQRT(qm * qp);
+    const float phi = 2.0f * EZ_PI * h_2;
+    return ez_to_normal_hemisphere(ez_v3(s * ez_cos(phi), s * ez_sin(phi), c), d);
+}
+
 #endif /* EZRT_MATH_H */
