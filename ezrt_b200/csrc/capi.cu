@@ -942,6 +942,33 @@ int ezrt_scene_destroy(ezrt_scene* s) {
 // ------------------------------------------------------------------------------------------
 // render
 // ------------------------------------------------------------------------------------------
+// The light sampling mode's options of a render (LightOptions, kernels.h) from the validated params: builds the light table, and the
+// environment table when the map is a light, at the first render that needs them.
+static int light_options(ezrt_scene* s, const ezrt_render_params* p, cudaStream_t st, LightOptions& o) {
+    o = LightOptions{};
+    if (p->mode != EZRT_MODE_DISNEY_LIGHTS) return EZRT_OK;
+    int rc = build_lights(s, st);
+    if (rc) return rc;
+    o.lights = s->lights;
+    // EZRT_PARAM_ENV_LIGHT: the map is one more light when the scene has a table (P_env = 1/2 beside triangle lights, 1 without);
+    // without a table the render is mode 4's, and mode 4's kernels run
+    if (p->reserved[0] & EZRT_PARAM_ENV_LIGHT) {
+        if ((rc = build_env(s, st))) return rc;
+        if (s->env.row_cdf) {
+            o.env = s->env;
+            o.env.p_env = (o.lights.n > 0) ? 0.5f : 1.0f;
+            o.env_on = true;
+        }
+    }
+    o.trans_on = (p->reserved[0] & EZRT_PARAM_TRANSMISSION) != 0;
+    // EZRT_PARAM_MEDIUM (validated: a medium is set, no transmission); sigma_t == 0 is mode 4 and runs its kernels
+    if ((p->reserved[0] & EZRT_PARAM_MEDIUM) && s->medium.sigma_t > 0.0f) {
+        o.med = s->medium;
+        o.medium_on = true;
+    }
+    return EZRT_OK;
+}
+
 // The render of ezrt_render_device (ad == av == nullptr), ezrt_render_adaptive_device (ad) and ezrt_render_aov_device (av): the
 // arguments are validated.
 static int render_device_impl(ezrt_scene* s, const ezrt_render_params* p, float* d_fb, cudaStream_t st, const AdaptiveRun* ad,
@@ -995,23 +1022,8 @@ static int render_device_impl(ezrt_scene* s, const ezrt_render_params* p, float*
     // the modes with a shadow pass: mode 3's environment samples, the light sampling mode's bounded light samples
     const bool lights_mode = (p->mode == EZRT_MODE_DISNEY_LIGHTS);
     const bool is_mode = (p->mode == EZRT_MODE_DISNEY_IS_MIS_P5) || lights_mode;
-    if (lights_mode && (rc = build_lights(s, st))) return rc;
-    const LightsDev lights = lights_mode ? s->lights : LightsDev{};
-    // EZRT_PARAM_ENV_LIGHT: the map is one more light when the scene has a table (P_env = 1/2 beside triangle lights, 1 without);
-    // without a table the render is mode 4's, and mode 4's kernels run
-    EnvDev env{};
-    if (lights_mode && (p->reserved[0] & EZRT_PARAM_ENV_LIGHT)) {
-        if ((rc = build_env(s, st))) return rc;
-        if (s->env.row_cdf) {
-            env = s->env;
-            env.p_env = (lights.n > 0) ? 0.5f : 1.0f;
-        }
-    }
-    // EZRT_PARAM_TRANSMISSION: the TRANS instantiations of k_shade and k_nee
-    const bool trans = lights_mode && (p->reserved[0] & EZRT_PARAM_TRANSMISSION);
-    // EZRT_PARAM_MEDIUM (validated: a medium is set): the MEDIUM instantiations, by value; sigma_t == 0 is mode 4 and runs its kernels
-    const MediumDev medium_v = s->medium;
-    const MediumDev* med = (lights_mode && (p->reserved[0] & EZRT_PARAM_MEDIUM) && medium_v.sigma_t > 0.0f) ? &medium_v : nullptr;
+    LightOptions lopt;
+    if ((rc = light_options(s, p, st, lopt))) return rc;
     int F = p->frames_per_batch;
     if (F <= 0) F = (int)std::max<size_t>(1, ((size_t)32 << 20) / per_frame);  // ~32 M sample slots per batch (~7.5 GB of state):
                                                                               // long queues amortise the persistent kernels' ramp-up and tail
@@ -1163,13 +1175,13 @@ static int render_device_impl(ezrt_scene* s, const ezrt_render_params* p, float*
                 CU_CHECK(cudaEventRecord(s->ev_fork, st));
                 CU_CHECK(cudaStreamWaitEvent(s->side_stream, s->ev_fork, 0));
                 launch_deferred_lane(s->dev, rd, d_tiles, b, batch_first, qin, defer_list, &d_ext[b], &dw_ext[b], side_hit, qout, &q_count[b + 1], sq, &s_count[b],
-                                     Lo, Le, n_fused, (uint32_t)nf, s->n_sms, s->side_stream, b == 0 ? aov_rec : nullptr, lights, env, trans, med);
+                                     Lo, Le, n_fused, (uint32_t)nf, s->n_sms, s->side_stream, b == 0 ? aov_rec : nullptr, lopt);
                 CU_CHECK(cudaEventRecord(s->ev_join, s->side_stream));
                 s->launches += 2;
             }
             sp = s->span_begin(1, st);
             launch_shade(s->dev, rd, d_tiles, b, batch_first, qin, &q_count[b], qout, &q_count[b + 1], sq, &s_count[b], Lo, Le,
-                         n_slots, n_fused, (uint32_t)nf, s->n_sms, st, b == 0 ? aov_rec : nullptr, lights, env, trans, med);
+                         n_slots, n_fused, (uint32_t)nf, s->n_sms, st, b == 0 ? aov_rec : nullptr, lopt);
             if (lane) CU_CHECK(cudaStreamWaitEvent(st, s->ev_join, 0));   // ... while this k_shade shades all the others; join
             s->span_end(sp, st);
             s->launches += 2;
@@ -1183,7 +1195,7 @@ static int render_device_impl(ezrt_scene* s, const ezrt_render_params* p, float*
                 }
                 s->span_end(sp, st);
                 sp = s->span_begin(1, st);   // shading work: counted with k_shade
-                launch_nee(s->dev, rd, sq, &s_count[b], Lo, n_slots, s->n_sms, st, env.row_cdf != nullptr, trans, med);
+                launch_nee(s->dev, rd, sq, &s_count[b], Lo, n_slots, s->n_sms, st, lopt);
                 s->span_end(sp, st);
                 s->launches += 2;
             }
@@ -1193,9 +1205,8 @@ static int render_device_impl(ezrt_scene* s, const ezrt_render_params* p, float*
             CU_CHECK(cudaStreamWaitEvent(st, s->fb_wait, 0));
             s->fb_wait = nullptr;
         }
-        if (av) launch_blend_aov(rd, d_tiles, nf, batch_first, Lo, Le, aov_rec, d_fb, av->d_aov, av->d_luma2, st);
-        else if (ad) launch_blend_adaptive(rd, d_tiles, nf, batch_first, Lo, Le, d_fb, ad->d_luma2, ad->d_spp, st);
-        else launch_blend(rd, d_tiles, nf, batch_first, Lo, Le, d_fb, st);
+        launch_blend(rd, d_tiles, nf, batch_first, Lo, Le, d_fb, av ? av->d_luma2 : ad ? ad->d_luma2 : nullptr, ad ? ad->d_spp : nullptr, aov_rec,
+                     av ? av->d_aov : nullptr, st);
         launch_tally(q_count, s_count, d_ext, d_sh, p->max_bounce + 1, totals, fused_camera ? (uint32_t)(active_pixels * (size_t)nf) : 0u, st);
         s->span_end(sp, st);
         s->launches += 2;

@@ -21,6 +21,7 @@
 #include <cstdlib>
 #include <map>
 #include <mutex>
+#include <type_traits>
 
 #include "device_functions.cuh"
 
@@ -726,6 +727,8 @@ __global__ void __launch_bounds__(128, EZRT_SHADE_MIN_BLOCKS) k_shade(SceneDev s
 template <int MODE, bool ENV = false, bool TRANS = false, bool MEDIUM = false>
 __global__ void __launch_bounds__(128, 8) k_nee(SceneDev sc, RenderDev rd, ShadowQueue sq, const uint32_t* __restrict__ s_count, float4* __restrict__ Lo,
                                                 MediumDev med) {
+    static_assert(MODE == EZRT_MODE_DISNEY_LIGHTS || !(ENV || TRANS || MEDIUM), "the options exist in the light sampling mode");
+    static_assert(!(TRANS && MEDIUM), "the medium is rendered without transmission");
     __shared__ uint32_t s_scan[34];
     __shared__ uint32_t s_total;
     __shared__ uint32_t s_list[512];
@@ -747,38 +750,25 @@ __global__ void __launch_bounds__(128, 8) k_nee(SceneDev sc, RenderDev rd, Shado
             const float4 o4 = __ldcs(sq.ray_o + j), d4 = __ldcs(sq.ray_d + j), n4 = __ldcs(sq.nrm + j), v4 = __ldcs(sq.view + j), h4 = __ldcs(sq.hist + j);
             const uint32_t slot = __float_as_uint(o4.w);
             const int m_raw = __float_as_int(d4.w);
+            const vec3 V = ez_v3(v4.x, v4.y, v4.z), N = ez_v3(n4.x, n4.y, n4.z), Ld = ez_v3(d4.x, d4.y, d4.z), hist = ez_v3(h4.x, h4.y, h4.z);
             vec3 c;
-            if constexpr (MEDIUM) {
-                static_assert(MODE == EZRT_MODE_DISNEY_LIGHTS && !TRANS, "the medium is rendered in the light sampling mode, without transmission");
-                const vec3 Ld = ez_v3(d4.x, d4.y, d4.z);
-                const int lm = __float_as_int(h4.w);
-                const vec3 E = (ENV && lm < 0) ? hdr_color(sc, rd, Ld, EZRT_MODE_DISNEY_LIGHTS) : load_emissive(sc, lm);
-                if (m_raw == EZRT_MEDIUM_VERTEX) c = nee_medium_contrib(ez_v3(v4.x, v4.y, v4.z), Ld, med.g, ez_v3(h4.x, h4.y, h4.z), E, v4.w);
-                else c = nee_light_contrib(ez_v3(v4.x, v4.y, v4.z), ez_v3(n4.x, n4.y, n4.z), Ld, load_material(sc, m_raw), ez_v3(h4.x, h4.y, h4.z), E, v4.w);
-                c = ez_scale(c, ez_medium_transmittance(&med, ez_v3(o4.x, o4.y, o4.z), Ld, ez_medium_light_dist(n4.w, ENV && lm < 0)));
-                float4 lo = Lo[slot];
-                lo.x += c.x; lo.y += c.y; lo.z += c.z;
-                Lo[slot] = lo;
-                continue;
+            if constexpr (MODE == EZRT_MODE_DISNEY_LIGHTS) {
+                const int lm = __float_as_int(h4.w);   // the light's material; -1: an environment sample
+                const auto light_color = [&] { return (ENV && lm < 0) ? hdr_color(sc, rd, Ld, EZRT_MODE_DISNEY_LIGHTS) : load_emissive(sc, lm); };
+                if constexpr (MEDIUM) {   // a medium vertex loads no material
+                    const vec3 E = light_color();
+                    if (m_raw == EZRT_MEDIUM_VERTEX) c = nee_medium_contrib(V, Ld, med.g, hist, E, v4.w);
+                    else c = nee_light_contrib(V, N, Ld, load_material(sc, m_raw), hist, E, v4.w);
+                    c = ez_scale(c, ez_medium_transmittance(&med, ez_v3(o4.x, o4.y, o4.z), Ld, ez_medium_light_dist(n4.w, ENV && lm < 0)));
+                } else {
+                    const int m_id = (TRANS && m_raw < 0) ? ~m_raw : m_raw;
+                    const MaterialDev mat = load_material(sc, m_id);
+                    if constexpr (TRANS) c = nee_trans_contrib(sc, V, N, Ld, m_id, mat, m_raw < 0, hist, light_color(), v4.w);
+                    else c = nee_light_contrib(V, N, Ld, mat, hist, light_color(), v4.w);
+                }
+            } else {
+                c = nee_contrib(sc, rd, EZRT_MODE_DISNEY_IS_MIS_P5, V, N, Ld, load_material(sc, m_raw), hist);
             }
-            const int m_id = (TRANS && m_raw < 0) ? ~m_raw : m_raw;
-            const MaterialDev mat = load_material(sc, m_id);
-            if (MODE == EZRT_MODE_DISNEY_LIGHTS && TRANS) {
-                const vec3 Ld = ez_v3(d4.x, d4.y, d4.z);
-                const int lm = __float_as_int(h4.w);
-                const vec3 E = (ENV && lm < 0) ? hdr_color(sc, rd, Ld, EZRT_MODE_DISNEY_LIGHTS) : load_emissive(sc, lm);
-                c = nee_trans_contrib(sc, ez_v3(v4.x, v4.y, v4.z), ez_v3(n4.x, n4.y, n4.z), Ld, m_id, mat, m_raw < 0, ez_v3(h4.x, h4.y, h4.z), E, v4.w);
-            } else if (MODE == EZRT_MODE_DISNEY_LIGHTS && ENV) {
-                const vec3 Ld = ez_v3(d4.x, d4.y, d4.z);
-                const int lm = __float_as_int(h4.w);
-                const vec3 E = (lm < 0) ? hdr_color(sc, rd, Ld, EZRT_MODE_DISNEY_LIGHTS) : load_emissive(sc, lm);
-                c = nee_light_contrib(ez_v3(v4.x, v4.y, v4.z), ez_v3(n4.x, n4.y, n4.z), Ld, mat, ez_v3(h4.x, h4.y, h4.z), E, v4.w);
-            } else if (MODE == EZRT_MODE_DISNEY_LIGHTS)
-                c = nee_light_contrib(ez_v3(v4.x, v4.y, v4.z), ez_v3(n4.x, n4.y, n4.z), ez_v3(d4.x, d4.y, d4.z), mat, ez_v3(h4.x, h4.y, h4.z),
-                                      load_emissive(sc, __float_as_int(h4.w)), v4.w);
-            else
-                c = nee_contrib(sc, rd, EZRT_MODE_DISNEY_IS_MIS_P5, ez_v3(v4.x, v4.y, v4.z), ez_v3(n4.x, n4.y, n4.z), ez_v3(d4.x, d4.y, d4.z), mat,
-                                ez_v3(h4.x, h4.y, h4.z));
             float4 lo = Lo[slot];
             lo.x += c.x; lo.y += c.y; lo.z += c.z;
             Lo[slot] = lo;
@@ -1193,6 +1183,14 @@ __global__ void __launch_bounds__(256) k_atrous(int width, int height, int step,
 // ------------------------------------------------------------------------------------------
 static inline int div_up(long long a, long long b) { return (int)((a + b - 1) / b); }
 
+// run-time options -> template arguments: f(std::integral_constant<bool, b>...) for the bools b in order, so that each launcher
+// names its kernel's instantiation once (combinations that are never instantiated are excluded by `if constexpr` inside f)
+template <class F> static void with_bools(F&& f) { f(); }
+template <class F, class... B> static void with_bools(F&& f, bool b, B... rest) {
+    if (b) with_bools([&](auto... t) { f(std::true_type{}, t...); }, rest...);
+    else with_bools([&](auto... t) { f(std::false_type{}, t...); }, rest...);
+}
+
 // persistent extend/shadow kernels: block size and resident blocks per SM (each block stages its own
 // copy of the top tree levels in shared memory); env EZRT_EXTEND_THREADS / EZRT_EXTEND_BPS override
 static int extend_threads() {
@@ -1214,8 +1212,8 @@ static int extend_blocks_per_sm() {
 void launch_generate(const RenderDev& rd, const TileDev* tiles, uint32_t n_slots, uint32_t batch_first_frame, PathQueue q,
                      uint32_t* q_count, int n_sms, cudaStream_t st, const LensDev* lens) {
     int blocks = std::min(div_up(n_slots, 256), n_sms * 8);
-    if (lens) k_generate<true><<<blocks, 256, 0, st>>>(rd, tiles, n_slots, batch_first_frame, q, q_count, *lens);
-    else k_generate<false><<<blocks, 256, 0, st>>>(rd, tiles, n_slots, batch_first_frame, q, q_count, LensDev{});
+    const LensDev l = lens ? *lens : LensDev{};
+    with_bools([&](auto L) { k_generate<L><<<blocks, 256, 0, st>>>(rd, tiles, n_slots, batch_first_frame, q, q_count, l); }, lens != nullptr);
 }
 // cudaFuncSetAttribute once per (kernel, size): the launchers run for every bounce of every batch
 static void set_dynamic_smem(const void* kernel, size_t bytes) {
@@ -1249,10 +1247,9 @@ void launch_extend(const SceneDev& sc, bool prune, bool anyhit, PathQueue q, con
         blocks = std::max(1, std::min(div_up(n_max, threads), 64));
         top = 0;
     }
-    if (prune && anyhit) k_extend<true, true><<<blocks, threads, smem_for(k_extend<true, true>, top), st>>>(sc, q, q_count, work, perm, to_accel, side_hit, gate);
-    else if (prune) k_extend<true, false><<<blocks, threads, smem_for(k_extend<true, false>, top), st>>>(sc, q, q_count, work, perm, to_accel, side_hit, gate);
-    else if (anyhit) k_extend<false, true><<<blocks, threads, smem_for(k_extend<false, true>, top), st>>>(sc, q, q_count, work, perm, to_accel, side_hit, gate);
-    else k_extend<false, false><<<blocks, threads, smem_for(k_extend<false, false>, top), st>>>(sc, q, q_count, work, perm, to_accel, side_hit, gate);
+    with_bools([&](auto P, auto A) {
+        k_extend<P, A><<<blocks, threads, smem_for(k_extend<P, A>, top), st>>>(sc, q, q_count, work, perm, to_accel, side_hit, gate);
+    }, prune, anyhit);
 }
 template <class K>
 static size_t w8_smem_for(K kernel, const SceneDev& sc) {
@@ -1260,33 +1257,31 @@ static size_t w8_smem_for(K kernel, const SceneDev& sc) {
     set_dynamic_smem((const void*)kernel, bytes);
     return bytes;
 }
+// the counters of the counting instantiations (counts != null, params.profile = 2): node visits to counts[2] when the kernel reads
+// quantised nodes (W8, or the 4-wide tree's 96-byte form), to counts[0] when it reads the 128-byte exact nodes; triangle tests to counts[1]
+static W8Counts w8_counts(unsigned long long* counts, bool quantised) {
+    W8Counts c;
+    c.node_visits = counts ? (quantised ? counts + 2 : counts) : nullptr;
+    c.tri_tests = counts ? counts + 1 : nullptr;
+    return c;
+}
 // accel policy: acceleration-tree pass (W8, or the round-1 4-wide kernel when the scene carries no W8 tree), then the
 // exact pass over whatever it deferred.  counts != null selects the counting instantiation (params.profile = 2).
 void launch_extend_accel(const SceneDev& sc, PathQueue q, const uint32_t* q_count, uint32_t* work, uint32_t* defer_list,
                          uint32_t* defer_count, uint32_t* defer_work, uint32_t n_max, int n_sms, unsigned long long* counts, const uint32_t* perm,
                          cudaStream_t st, int exact_gate) {
     const int threads = extend_threads(), blocks = persistent_blocks(n_max, n_sms);
+    // incoherent rays on the 4-wide tree: the 96-byte quantised form of the nodes when the scene carries it (env EZRT_ACCEL_Q16=0: exact nodes)
+    const W8Counts c = w8_counts(counts, sc.w8_nodes || sc.acc_wide_q16);
     if (sc.w8_nodes) {
-        W8Counts c;
-        c.node_visits = counts ? counts + 2 : nullptr;   // 96-byte records
-        c.tri_tests = counts ? counts + 1 : nullptr;
         unsigned long long* const cyc = counts ? counts + EZRT_W8_PHASES_EXTEND : nullptr;
-#define EZRT_LAUNCH_W8(C, I) k_extend_w8<C, I><<<blocks, threads, w8_smem_for(k_extend_w8<C, I>, sc), st>>>(sc, q, q_count, work, defer_list, defer_count, c, perm, cyc)
-        if (sc.acc_tri_indexed) { if (counts) EZRT_LAUNCH_W8(true, true); else EZRT_LAUNCH_W8(false, true); }
-        else { if (counts) EZRT_LAUNCH_W8(true, false); else EZRT_LAUNCH_W8(false, false); }
-#undef EZRT_LAUNCH_W8
+        with_bools([&](auto C, auto I) {
+            k_extend_w8<C, I><<<blocks, threads, w8_smem_for(k_extend_w8<C, I>, sc), st>>>(sc, q, q_count, work, defer_list, defer_count, c, perm, cyc);
+        }, counts != nullptr, sc.acc_tri_indexed != 0);
     } else {
-        W8Counts c;
-        c.node_visits = counts ? (sc.acc_wide_q16 ? counts + 2 : counts) : nullptr;   // counts[2]: 96-byte records, counts[0]: 128-byte records
-        c.tri_tests = counts ? counts + 1 : nullptr;
-        // incoherent rays: the 96-byte quantised form of the nodes when the scene carries it (env EZRT_ACCEL_Q16=0: exact nodes)
-        if (sc.acc_wide_q16) {
-            if (counts) k_extend_accel<true, true><<<blocks, threads, smem_for(k_extend_accel<true, true>, 0), st>>>(sc, q, q_count, work, defer_list, defer_count, c, perm);
-            else k_extend_accel<false, true><<<blocks, threads, smem_for(k_extend_accel<false, true>, 0), st>>>(sc, q, q_count, work, defer_list, defer_count, c, perm);
-        } else {
-            if (counts) k_extend_accel<true, false><<<blocks, threads, smem_for(k_extend_accel<true, false>, 0), st>>>(sc, q, q_count, work, defer_list, defer_count, c, perm);
-            else k_extend_accel<false, false><<<blocks, threads, smem_for(k_extend_accel<false, false>, 0), st>>>(sc, q, q_count, work, defer_list, defer_count, c, perm);
-        }
+        with_bools([&](auto C, auto Q) {
+            k_extend_accel<C, Q><<<blocks, threads, smem_for(k_extend_accel<C, Q>, 0), st>>>(sc, q, q_count, work, defer_list, defer_count, c, perm);
+        }, counts != nullptr, sc.acc_wide_q16 != 0);
     }
     launch_extend(sc, true, false, q, defer_count, defer_work, defer_list, 1, std::min<uint32_t>(n_max, 65536u), n_sms, st, nullptr, exact_gate);
 }
@@ -1302,99 +1297,75 @@ void launch_ray_sort(const SceneDev& sc, PathQueue q, const uint32_t* q_count, u
 void launch_shadow(const SceneDev& sc, bool prune, ShadowQueue sq, const uint32_t* s_count, uint32_t* work, float4* Lo,
                    const uint32_t* perm, uint32_t n_max, int n_sms, cudaStream_t st, bool bounded) {
     const int threads = extend_threads(), blocks = persistent_blocks(n_max, n_sms);
-#define EZRT_LAUNCH_SHADOW(P, B) k_shadow<P, B><<<blocks, threads, smem_for(k_shadow<P, B>, sc.top_nodes), st>>>(sc, sq, s_count, work, Lo, perm)
-    if (bounded) { if (prune) EZRT_LAUNCH_SHADOW(true, true); else EZRT_LAUNCH_SHADOW(false, true); }
-    else { if (prune) EZRT_LAUNCH_SHADOW(true, false); else EZRT_LAUNCH_SHADOW(false, false); }
-#undef EZRT_LAUNCH_SHADOW
+    with_bools([&](auto P, auto B) {
+        k_shadow<P, B><<<blocks, threads, smem_for(k_shadow<P, B>, sc.top_nodes), st>>>(sc, sq, s_count, work, Lo, perm);
+    }, prune, bounded);
 }
 // camera pass of the W8 policy: rays generated in the kernel (slot i = ray i), then the exact pass over the deferred ones
 void launch_extend_camera(const SceneDev& sc, const RenderDev& rd, const TileDev* tiles, uint32_t batch_first_frame, uint32_t n_slots, uint32_t n_frames, PathQueue q,
                           uint32_t* work, uint32_t* defer_list, uint32_t* defer_count, uint32_t* defer_work, int n_sms, unsigned long long* counts,
                           cudaStream_t st, int exact_gate) {
     const int threads = extend_threads(), blocks = persistent_blocks(n_slots, n_sms);
-    W8Counts c;
-    c.node_visits = counts ? (sc.w8_nodes ? counts + 2 : counts) : nullptr;   // the 4-wide camera pass reads the 128-byte exact nodes
-    c.tri_tests = counts ? counts + 1 : nullptr;
+    const W8Counts c = w8_counts(counts, sc.w8_nodes != nullptr);   // the 4-wide camera pass reads the 128-byte exact nodes
     if (sc.w8_nodes) {
         // s_perm + one stack of W8_BUNDLE_STACK entries per warp (extend_w8_bundle)
-        auto smem_bundle = [&](const void* k) { const size_t b = 2048 + (size_t)(threads / 32) * W8_BUNDLE_STACK * sizeof(uint2); set_dynamic_smem(k, b); return b; };
-#define EZRT_LAUNCH_W8(C, I) \
-    k_extend_w8_camera<C, I><<<blocks, threads, smem_bundle((const void*)k_extend_w8_camera<C, I>), st>>>(sc, rd, tiles, batch_first_frame, n_slots, n_frames, q, work, defer_list, defer_count, c)
-        if (sc.acc_tri_indexed) { if (counts) EZRT_LAUNCH_W8(true, true); else EZRT_LAUNCH_W8(false, true); }
-        else { if (counts) EZRT_LAUNCH_W8(true, false); else EZRT_LAUNCH_W8(false, false); }
-#undef EZRT_LAUNCH_W8
+        const size_t smem = 2048 + (size_t)(threads / 32) * W8_BUNDLE_STACK * sizeof(uint2);
+        with_bools([&](auto C, auto I) {
+            set_dynamic_smem((const void*)k_extend_w8_camera<C, I>, smem);
+            k_extend_w8_camera<C, I><<<blocks, threads, smem, st>>>(sc, rd, tiles, batch_first_frame, n_slots, n_frames, q, work, defer_list, defer_count, c);
+        }, counts != nullptr, sc.acc_tri_indexed != 0);
     } else {
-        if (counts) k_extend_accel_camera<true><<<blocks, threads, smem_for(k_extend_accel_camera<true>, 0), st>>>(sc, rd, tiles, batch_first_frame, n_slots, n_frames, q, work, defer_list, defer_count, c);
-        else k_extend_accel_camera<false><<<blocks, threads, smem_for(k_extend_accel_camera<false>, 0), st>>>(sc, rd, tiles, batch_first_frame, n_slots, n_frames, q, work, defer_list, defer_count, c);
+        with_bools([&](auto C) {
+            k_extend_accel_camera<C><<<blocks, threads, smem_for(k_extend_accel_camera<C>, 0), st>>>(sc, rd, tiles, batch_first_frame, n_slots, n_frames, q, work, defer_list, defer_count, c);
+        }, counts != nullptr);
     }
     launch_extend(sc, true, false, q, defer_count, defer_work, defer_list, 1, std::min<uint32_t>(n_slots, 65536u), n_sms, st, nullptr, exact_gate);
-}
-template <bool B>
-static void launch_shadow_accel_t(const SceneDev& sc, ShadowQueue sq, const uint32_t* s_count, uint32_t* work, float4* Lo, uint32_t* defer_list,
-                                  uint32_t* defer_count, unsigned long long* counts, int blocks, int threads, cudaStream_t st) {
-    if (sc.w8_nodes) {
-        W8Counts c;
-        c.node_visits = counts ? counts + 2 : nullptr;
-        c.tri_tests = counts ? counts + 1 : nullptr;
-        unsigned long long* const cyc = counts ? counts + EZRT_W8_PHASES_SHADOW : nullptr;
-#define EZRT_LAUNCH_W8(C, I) k_shadow_w8<C, I, B><<<blocks, threads, w8_smem_for(k_shadow_w8<C, I, B>, sc), st>>>(sc, sq, s_count, work, Lo, defer_list, defer_count, c, cyc)
-        if (sc.acc_tri_indexed) { if (counts) EZRT_LAUNCH_W8(true, true); else EZRT_LAUNCH_W8(false, true); }
-        else { if (counts) EZRT_LAUNCH_W8(true, false); else EZRT_LAUNCH_W8(false, false); }
-#undef EZRT_LAUNCH_W8
-    } else {
-        W8Counts c;
-        c.node_visits = counts ? (sc.acc_wide_q16 ? counts + 2 : counts) : nullptr;
-        c.tri_tests = counts ? counts + 1 : nullptr;
-#define EZRT_LAUNCH_W4(C, Q) k_shadow_accel<C, Q, B><<<blocks, threads, smem_for(k_shadow_accel<C, Q, B>, 0), st>>>(sc, sq, s_count, work, Lo, defer_list, defer_count, c)
-        if (sc.acc_wide_q16) { if (counts) EZRT_LAUNCH_W4(true, true); else EZRT_LAUNCH_W4(false, true); }
-        else { if (counts) EZRT_LAUNCH_W4(true, false); else EZRT_LAUNCH_W4(false, false); }
-#undef EZRT_LAUNCH_W4
-    }
 }
 void launch_shadow_accel(const SceneDev& sc, ShadowQueue sq, const uint32_t* s_count, uint32_t* work, float4* Lo, uint32_t* defer_list,
                          uint32_t* defer_count, uint32_t* defer_work, uint32_t n_max, int n_sms, unsigned long long* counts, cudaStream_t st, bool bounded) {
     const int threads = extend_threads(), blocks = persistent_blocks(n_max, n_sms);
-    if (bounded) launch_shadow_accel_t<true>(sc, sq, s_count, work, Lo, defer_list, defer_count, counts, blocks, threads, st);
-    else launch_shadow_accel_t<false>(sc, sq, s_count, work, Lo, defer_list, defer_count, counts, blocks, threads, st);
+    const W8Counts c = w8_counts(counts, sc.w8_nodes || sc.acc_wide_q16);
+    if (sc.w8_nodes) {
+        unsigned long long* const cyc = counts ? counts + EZRT_W8_PHASES_SHADOW : nullptr;
+        with_bools([&](auto C, auto I, auto B) {
+            k_shadow_w8<C, I, B><<<blocks, threads, w8_smem_for(k_shadow_w8<C, I, B>, sc), st>>>(sc, sq, s_count, work, Lo, defer_list, defer_count, c, cyc);
+        }, counts != nullptr, sc.acc_tri_indexed != 0, bounded);
+    } else {
+        with_bools([&](auto C, auto Q, auto B) {
+            k_shadow_accel<C, Q, B><<<blocks, threads, smem_for(k_shadow_accel<C, Q, B>, 0), st>>>(sc, sq, s_count, work, Lo, defer_list, defer_count, c);
+        }, counts != nullptr, sc.acc_wide_q16 != nullptr, bounded);
+    }
     launch_shadow(sc, true, sq, defer_count, defer_work, Lo, defer_list, std::min<uint32_t>(n_max, 65536u), n_sms, st, bounded);
+}
+// k_shade over the queue, or (LIST) over the deferred lane's list with its hits in side_hit.  The instantiation follows the mode,
+// aov_rec (non-null: AOV) and the light sampling mode's options; MODE = k_shade's mode template argument for rd.mode.
+template <bool LIST>
+static void launch_shade_t(int blocks, const SceneDev& sc, const RenderDev& rd, const TileDev* tiles, int bounce, uint32_t batch_first_frame,
+                           PathQueue qin, const uint32_t* in_count, PathQueue qout, uint32_t* out_count, ShadowQueue sq, uint32_t* s_count,
+                           float4* Lo, float4* Le, uint32_t n_fused, uint32_t n_frames, const uint32_t* list, const float2* side_hit,
+                           float4* aov_rec, const LightOptions& o, cudaStream_t st) {
+    auto launch = [&](auto M) {
+        with_bools([&](auto A, auto E, auto T, auto X) {
+            if constexpr ((M == EZRT_MODE_DISNEY_LIGHTS || !(E || T || X)) && !(T && X))   // the options exist in the light sampling mode
+                k_shade<M, LIST, A, E, T, X><<<blocks, 128, 0, st>>>(sc, rd, tiles, bounce, batch_first_frame, qin, in_count, qout, out_count, sq,
+                                                                     s_count, Lo, Le, n_fused, n_frames, list, side_hit, aov_rec, o.lights, o.env, o.med);
+        }, aov_rec != nullptr, o.env_on, o.trans_on, o.medium_on);
+    };
+    switch (rd.mode) {
+        case EZRT_MODE_DIFFUSE_P3: launch(std::integral_constant<int, EZRT_MODE_DIFFUSE_P3>{}); break;
+        case EZRT_MODE_DISNEY_ANISO_P4: launch(std::integral_constant<int, EZRT_MODE_DISNEY_ANISO_P4>{}); break;
+        case EZRT_MODE_DISNEY_SOBOL_P5: launch(std::integral_constant<int, EZRT_MODE_DISNEY_SOBOL_P5>{}); break;
+        case EZRT_MODE_DISNEY_LIGHTS: launch(std::integral_constant<int, EZRT_MODE_DISNEY_LIGHTS>{}); break;
+        default: launch(std::integral_constant<int, EZRT_MODE_DISNEY_IS_MIS_P5>{}); break;
+    }
 }
 void launch_shade(const SceneDev& sc, const RenderDev& rd, const TileDev* tiles, int bounce, uint32_t batch_first_frame,
                   PathQueue qin, const uint32_t* in_count, PathQueue qout, uint32_t* out_count, ShadowQueue sq,
                   uint32_t* s_count, float4* Lo, float4* Le, uint32_t n_max, uint32_t n_fused, uint32_t n_frames, int n_sms, cudaStream_t st,
-                  float4* aov_rec, LightsDev lights, EnvDev env, bool trans, const MediumDev* med) {
-    int blocks = std::min(div_up(n_max, 128), n_sms * 4 * EZRT_SHADE_MIN_BLOCKS);
-    if (blocks < 1) blocks = 1;
-    const MediumDev m = med ? *med : MediumDev{};
-#define EZRT_LAUNCH_SHADE_X(M, E, T, X)                                                                                                       \
-    if (aov_rec) k_shade<M, false, true, E, T, X><<<blocks, 128, 0, st>>>(sc, rd, tiles, bounce, batch_first_frame, qin, in_count, qout, out_count, sq, s_count, Lo, \
-                                                                          Le, n_fused, n_frames, nullptr, nullptr, aov_rec, lights, env, m);   \
-    else k_shade<M, false, false, E, T, X><<<blocks, 128, 0, st>>>(sc, rd, tiles, bounce, batch_first_frame, qin, in_count, qout, out_count, sq, s_count, Lo, Le, n_fused, n_frames, nullptr, nullptr, nullptr, lights, env, m)
-#define EZRT_LAUNCH_SHADE_E(M, E, T) EZRT_LAUNCH_SHADE_X(M, E, T, false)
-#define EZRT_LAUNCH_SHADE(M) EZRT_LAUNCH_SHADE_E(M, false, false)
-    if (rd.mode == EZRT_MODE_DISNEY_LIGHTS && med) {   // the homogeneous medium (EZRT_PARAM_MEDIUM; never with trans)
-        if (env.row_cdf) { EZRT_LAUNCH_SHADE_X(EZRT_MODE_DISNEY_LIGHTS, true, false, true); }
-        else { EZRT_LAUNCH_SHADE_X(EZRT_MODE_DISNEY_LIGHTS, false, false, true); }
-        return;
-    }
-    if (rd.mode == EZRT_MODE_DISNEY_LIGHTS && trans) {   // materials with a dielectric lobe (EZRT_PARAM_TRANSMISSION)
-        if (env.row_cdf) { EZRT_LAUNCH_SHADE_E(EZRT_MODE_DISNEY_LIGHTS, true, true); }
-        else { EZRT_LAUNCH_SHADE_E(EZRT_MODE_DISNEY_LIGHTS, false, true); }
-        return;
-    }
-    if (rd.mode == EZRT_MODE_DISNEY_LIGHTS && env.row_cdf) {   // the map as a light (EZRT_PARAM_ENV_LIGHT)
-        EZRT_LAUNCH_SHADE_E(EZRT_MODE_DISNEY_LIGHTS, true, false);
-        return;
-    }
-    switch (rd.mode) {
-        case EZRT_MODE_DIFFUSE_P3: EZRT_LAUNCH_SHADE(EZRT_MODE_DIFFUSE_P3); break;
-        case EZRT_MODE_DISNEY_ANISO_P4: EZRT_LAUNCH_SHADE(EZRT_MODE_DISNEY_ANISO_P4); break;
-        case EZRT_MODE_DISNEY_SOBOL_P5: EZRT_LAUNCH_SHADE(EZRT_MODE_DISNEY_SOBOL_P5); break;
-        case EZRT_MODE_DISNEY_LIGHTS: EZRT_LAUNCH_SHADE(EZRT_MODE_DISNEY_LIGHTS); break;
-        default: EZRT_LAUNCH_SHADE(EZRT_MODE_DISNEY_IS_MIS_P5); break;
-    }
-#undef EZRT_LAUNCH_SHADE
-#undef EZRT_LAUNCH_SHADE_E
-#undef EZRT_LAUNCH_SHADE_X
+                  float4* aov_rec, const LightOptions& o) {
+    const int blocks = std::max(1, std::min(div_up(n_max, 128), n_sms * 4 * EZRT_SHADE_MIN_BLOCKS));
+    launch_shade_t<false>(blocks, sc, rd, tiles, bounce, batch_first_frame, qin, in_count, qout, out_count, sq, s_count, Lo, Le, n_fused, n_frames,
+                          nullptr, nullptr, aov_rec, o, st);
 }
 // The accel policy's deferred lane (side stream, beside the main k_shade of the same bounce): exact traversal of the deferred
 // rays into side_hit, then their shading -- both do nothing if more than EZRT_SIDE_CAP rays were deferred (then
@@ -1402,52 +1373,18 @@ void launch_shade(const SceneDev& sc, const RenderDev& rd, const TileDev* tiles,
 void launch_deferred_lane(const SceneDev& sc, const RenderDev& rd, const TileDev* tiles, int bounce, uint32_t batch_first_frame, PathQueue qin,
                           const uint32_t* defer_list, const uint32_t* defer_count, uint32_t* defer_work, float2* side_hit, PathQueue qout,
                           uint32_t* out_count, ShadowQueue sq, uint32_t* s_count, float4* Lo, float4* Le, uint32_t n_fused, uint32_t n_frames,
-                          int n_sms, cudaStream_t st, float4* aov_rec, LightsDev lights, EnvDev env, bool trans, const MediumDev* med) {
+                          int n_sms, cudaStream_t st, float4* aov_rec, const LightOptions& o) {
     launch_extend(sc, true, false, qin, defer_count, defer_work, defer_list, 1, EZRT_SIDE_CAP, n_sms, st, side_hit, 1);
-    const int blocks = 8;
-    const MediumDev m = med ? *med : MediumDev{};
-#define EZRT_LAUNCH_SHADE_X(M, E, T, X)                                                                                                       \
-    if (aov_rec) k_shade<M, true, true, E, T, X><<<blocks, 128, 0, st>>>(sc, rd, tiles, bounce, batch_first_frame, qin, defer_count, qout, out_count, sq, s_count, Lo, \
-                                                                         Le, n_fused, n_frames, defer_list, side_hit, aov_rec, lights, env, m);   \
-    else k_shade<M, true, false, E, T, X><<<blocks, 128, 0, st>>>(sc, rd, tiles, bounce, batch_first_frame, qin, defer_count, qout, out_count, sq, s_count, Lo, Le, n_fused, n_frames, defer_list, side_hit, nullptr, lights, env, m)
-#define EZRT_LAUNCH_SHADE_E(M, E, T) EZRT_LAUNCH_SHADE_X(M, E, T, false)
-#define EZRT_LAUNCH_SHADE(M) EZRT_LAUNCH_SHADE_E(M, false, false)
-    if (rd.mode == EZRT_MODE_DISNEY_LIGHTS && med) {
-        if (env.row_cdf) { EZRT_LAUNCH_SHADE_X(EZRT_MODE_DISNEY_LIGHTS, true, false, true); }
-        else { EZRT_LAUNCH_SHADE_X(EZRT_MODE_DISNEY_LIGHTS, false, false, true); }
-        return;
-    }
-    if (rd.mode == EZRT_MODE_DISNEY_LIGHTS && trans) {
-        if (env.row_cdf) { EZRT_LAUNCH_SHADE_E(EZRT_MODE_DISNEY_LIGHTS, true, true); }
-        else { EZRT_LAUNCH_SHADE_E(EZRT_MODE_DISNEY_LIGHTS, false, true); }
-        return;
-    }
-    if (rd.mode == EZRT_MODE_DISNEY_LIGHTS && env.row_cdf) {
-        EZRT_LAUNCH_SHADE_E(EZRT_MODE_DISNEY_LIGHTS, true, false);
-        return;
-    }
-    switch (rd.mode) {
-        case EZRT_MODE_DIFFUSE_P3: EZRT_LAUNCH_SHADE(EZRT_MODE_DIFFUSE_P3); break;
-        case EZRT_MODE_DISNEY_ANISO_P4: EZRT_LAUNCH_SHADE(EZRT_MODE_DISNEY_ANISO_P4); break;
-        case EZRT_MODE_DISNEY_SOBOL_P5: EZRT_LAUNCH_SHADE(EZRT_MODE_DISNEY_SOBOL_P5); break;
-        case EZRT_MODE_DISNEY_LIGHTS: EZRT_LAUNCH_SHADE(EZRT_MODE_DISNEY_LIGHTS); break;
-        default: EZRT_LAUNCH_SHADE(EZRT_MODE_DISNEY_IS_MIS_P5); break;
-    }
-#undef EZRT_LAUNCH_SHADE
-#undef EZRT_LAUNCH_SHADE_E
-#undef EZRT_LAUNCH_SHADE_X
+    launch_shade_t<true>(8, sc, rd, tiles, bounce, batch_first_frame, qin, defer_count, qout, out_count, sq, s_count, Lo, Le, n_fused, n_frames,
+                         defer_list, side_hit, aov_rec, o, st);
 }
 void launch_nee(const SceneDev& sc, const RenderDev& rd, ShadowQueue sq, const uint32_t* s_count, float4* Lo, uint32_t n_max, int n_sms, cudaStream_t st,
-                bool env, bool trans, const MediumDev* med) {
+                const LightOptions& o) {
     const int blocks = std::max(1, std::min(div_up(n_max, 512), n_sms * 8));
-    const MediumDev m = med ? *med : MediumDev{};
-    if (rd.mode == EZRT_MODE_DISNEY_LIGHTS && med && env) k_nee<EZRT_MODE_DISNEY_LIGHTS, true, false, true><<<blocks, 128, 0, st>>>(sc, rd, sq, s_count, Lo, m);
-    else if (rd.mode == EZRT_MODE_DISNEY_LIGHTS && med) k_nee<EZRT_MODE_DISNEY_LIGHTS, false, false, true><<<blocks, 128, 0, st>>>(sc, rd, sq, s_count, Lo, m);
-    else if (rd.mode == EZRT_MODE_DISNEY_LIGHTS && trans && env) k_nee<EZRT_MODE_DISNEY_LIGHTS, true, true><<<blocks, 128, 0, st>>>(sc, rd, sq, s_count, Lo, m);
-    else if (rd.mode == EZRT_MODE_DISNEY_LIGHTS && trans) k_nee<EZRT_MODE_DISNEY_LIGHTS, false, true><<<blocks, 128, 0, st>>>(sc, rd, sq, s_count, Lo, m);
-    else if (rd.mode == EZRT_MODE_DISNEY_LIGHTS && env) k_nee<EZRT_MODE_DISNEY_LIGHTS, true><<<blocks, 128, 0, st>>>(sc, rd, sq, s_count, Lo, m);
-    else if (rd.mode == EZRT_MODE_DISNEY_LIGHTS) k_nee<EZRT_MODE_DISNEY_LIGHTS><<<blocks, 128, 0, st>>>(sc, rd, sq, s_count, Lo, m);
-    else k_nee<EZRT_MODE_DISNEY_IS_MIS_P5><<<blocks, 128, 0, st>>>(sc, rd, sq, s_count, Lo, m);
+    with_bools([&](auto L, auto E, auto T, auto X) {
+        if constexpr ((L || !(E || T || X)) && !(T && X))   // the options exist in the light sampling mode; the other mode here is mode 3
+            k_nee<L ? EZRT_MODE_DISNEY_LIGHTS : EZRT_MODE_DISNEY_IS_MIS_P5, E, T, X><<<blocks, 128, 0, st>>>(sc, rd, sq, s_count, Lo, o.med);
+    }, rd.mode == EZRT_MODE_DISNEY_LIGHTS, o.env_on, o.trans_on, o.medium_on);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -1515,20 +1452,13 @@ void launch_light_records(const SceneDev& sc, const int32_t* idx, int n, float4*
     if (n <= 0) return;
     k_light_records<<<div_up(n, 256), 256, 0, st>>>(sc, idx, n, rec);
 }
-void launch_blend(const RenderDev& rd, const TileDev* tiles, int nf, uint32_t batch_first_frame, const float4* Lo,
-                  const float4* Le, float* fb, cudaStream_t st) {
+void launch_blend(const RenderDev& rd, const TileDev* tiles, int nf, uint32_t batch_first_frame, const float4* Lo, const float4* Le,
+                  float* fb, float* luma2, int32_t* spp_map, const float4* aov_rec, float* aov, cudaStream_t st) {
     uint32_t per_frame = (uint32_t)rd.n_tiles * EZRT_TILE_PIXELS;
-    k_blend<false><<<div_up(per_frame, 256), 256, 0, st>>>(rd, tiles, nf, batch_first_frame, Lo, Le, fb, nullptr, nullptr, nullptr, nullptr);
-}
-void launch_blend_aov(const RenderDev& rd, const TileDev* tiles, int nf, uint32_t batch_first_frame, const float4* Lo, const float4* Le,
-                      const float4* aov_rec, float* fb, float* aov, float* luma2, cudaStream_t st) {
-    uint32_t per_frame = (uint32_t)rd.n_tiles * EZRT_TILE_PIXELS;
-    k_blend<true, true><<<div_up(per_frame, 256), 256, 0, st>>>(rd, tiles, nf, batch_first_frame, Lo, Le, fb, luma2, nullptr, aov_rec, aov);
-}
-void launch_blend_adaptive(const RenderDev& rd, const TileDev* tiles, int nf, uint32_t batch_first_frame, const float4* Lo,
-                           const float4* Le, float* fb, float* luma2, int32_t* spp_map, cudaStream_t st) {
-    uint32_t per_frame = (uint32_t)rd.n_tiles * EZRT_TILE_PIXELS;
-    k_blend<true><<<div_up(per_frame, 256), 256, 0, st>>>(rd, tiles, nf, batch_first_frame, Lo, Le, fb, luma2, spp_map, nullptr, nullptr);
+    with_bools([&](auto ADAPTIVE, auto AOV) {
+        if constexpr (ADAPTIVE || !AOV)   // the feature buffers keep luma2
+            k_blend<ADAPTIVE, AOV><<<div_up(per_frame, 256), 256, 0, st>>>(rd, tiles, nf, batch_first_frame, Lo, Le, fb, luma2, spp_map, aov_rec, aov);
+    }, luma2 != nullptr, aov != nullptr);
 }
 void launch_adaptive_check(const RenderDev& rd, const TileDev* tiles_in, int n_frames, float threshold, const float* fb, const float* luma2,
                            unsigned char* keep, unsigned int* blocks_done, TileDev* tiles_out, int32_t* counts, cudaStream_t st) {
@@ -1543,10 +1473,8 @@ void launch_megakernel(const SceneDev& sc, const RenderDev& rd, const TileDev* t
                        unsigned long long* totals, cudaStream_t st, const LensDev* lens) {
     uint32_t per_frame = (uint32_t)rd.n_tiles * EZRT_TILE_PIXELS;
     const LensDev l = lens ? *lens : LensDev{};
-#define EZRT_LAUNCH_MEGA(P, L) k_megakernel<P, L><<<div_up(per_frame, 128), 128, 0, st>>>(sc, rd, tiles, spp, fb, totals, l)
-    if (lens) { if (prune) EZRT_LAUNCH_MEGA(true, true); else EZRT_LAUNCH_MEGA(false, true); }
-    else { if (prune) EZRT_LAUNCH_MEGA(true, false); else EZRT_LAUNCH_MEGA(false, false); }
-#undef EZRT_LAUNCH_MEGA
+    with_bools([&](auto P, auto L) { k_megakernel<P, L><<<div_up(per_frame, 128), 128, 0, st>>>(sc, rd, tiles, spp, fb, totals, l); },
+               prune, lens != nullptr);
 }
 void launch_camera_rays(const RenderDev& rd, const LensDev* lens, int n, const uint32_t* px, const uint32_t* py, const uint32_t* frame,
                         float* o, float* d, cudaStream_t st) {

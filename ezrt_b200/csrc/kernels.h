@@ -16,6 +16,19 @@
 #endif
 #define EZRT_EXTEND_BLOCKS_PER_SM 1
 
+// The light sampling mode's options of a render (capi.cu light_options), passed as one value to launch_shade, launch_deferred_lane
+// and launch_nee, which pick the k_shade / k_nee instantiation from them:
+//   env_on    EZRT_PARAM_ENV_LIGHT and the scene has an environment table: the map is one more light (<.., ENV>)
+//   trans_on  EZRT_PARAM_TRANSMISSION: materials with a dielectric lobe (<.., TRANS>)
+//   medium_on EZRT_PARAM_MEDIUM with sigma_t > 0: the homogeneous medium med (<.., MEDIUM>); never with trans_on
+// All off outside the light sampling mode; the tables are zero where unused, as the kernels' parameters.
+struct LightOptions {
+    LightsDev lights{};   // the light table (light sampling mode)
+    EnvDev env{};         // the environment table (env_on)
+    MediumDev med{};      // the medium (medium_on)
+    bool env_on = false, trans_on = false, medium_on = false;
+};
+
 // lens (EZRT_PARAM_THIN_LENS): the thin-lens camera rays (k_generate<true>); null: the pinhole's
 void launch_generate(const RenderDev& rd, const TileDev* tiles, uint32_t n_slots, uint32_t batch_first_frame, PathQueue q,
                      uint32_t* q_count, int n_sms, cudaStream_t st, const LensDev* lens = nullptr);
@@ -42,24 +55,18 @@ void launch_shadow_accel(const SceneDev& sc, ShadowQueue sq, const uint32_t* s_c
 void launch_shade(const SceneDev& sc, const RenderDev& rd, const TileDev* tiles, int bounce, uint32_t batch_first_frame,
                   PathQueue qin, const uint32_t* in_count, PathQueue qout, uint32_t* out_count, ShadowQueue sq,
                   uint32_t* s_count, float4* Lo, float4* Le, uint32_t n_max, uint32_t n_fused, uint32_t n_frames, int n_sms, cudaStream_t st,
-                  float4* aov_rec = nullptr,   // aov_rec: feature-buffer render, bounce 0 writes the first-hit records (k_shade<.., AOV>)
-                  LightsDev lights = LightsDev{},    // the light table (light sampling mode)
-                  EnvDev env = EnvDev{},             // the environment table (light sampling mode with EZRT_PARAM_ENV_LIGHT; row_cdf null: none)
-                  bool trans = false,                // light sampling mode with EZRT_PARAM_TRANSMISSION (k_shade<.., TRANS>)
-                  const MediumDev* med = nullptr);   // light sampling mode with EZRT_PARAM_MEDIUM and sigma_t > 0 (k_shade<.., MEDIUM>)
+                  float4* aov_rec,   // feature-buffer render, bounce 0 writes the first-hit records (k_shade<.., AOV>); else null
+                  const LightOptions& o);
 void launch_extend_camera(const SceneDev& sc, const RenderDev& rd, const TileDev* tiles, uint32_t batch_first_frame, uint32_t n_slots, uint32_t n_frames, PathQueue q,
                           uint32_t* work, uint32_t* defer_list, uint32_t* defer_count, uint32_t* defer_work, int n_sms, unsigned long long* counts,
                           cudaStream_t st, int exact_gate = 0);
 void launch_deferred_lane(const SceneDev& sc, const RenderDev& rd, const TileDev* tiles, int bounce, uint32_t batch_first_frame, PathQueue qin,
                           const uint32_t* defer_list, const uint32_t* defer_count, uint32_t* defer_work, float2* side_hit, PathQueue qout,
                           uint32_t* out_count, ShadowQueue sq, uint32_t* s_count, float4* Lo, float4* Le, uint32_t n_fused, uint32_t n_frames,
-                          int n_sms, cudaStream_t st, float4* aov_rec = nullptr, LightsDev lights = LightsDev{}, EnvDev env = EnvDev{},
-                          bool trans = false, const MediumDev* med = nullptr);
+                          int n_sms, cudaStream_t st, float4* aov_rec, const LightOptions& o);
 // after a shadow pass (accel or exact, including the exact pass over deferred shadow rays): contributions of the unoccluded light samples
-// env: the light sampling mode's queue also holds environment samples (hist.w = -1); trans: EZRT_PARAM_TRANSMISSION (k_nee<.., TRANS>);
-// med: EZRT_PARAM_MEDIUM (k_nee<.., MEDIUM>: the shadow rays' transmittance, the medium vertices' phase function)
 void launch_nee(const SceneDev& sc, const RenderDev& rd, ShadowQueue sq, const uint32_t* s_count, float4* Lo, uint32_t n_max, int n_sms, cudaStream_t st,
-                bool env = false, bool trans = false, const MediumDev* med = nullptr);
+                const LightOptions& o);
 // light table of the light sampling mode: every triangle's weight (w: n_triangles floats) -> the lights in triangle order
 // (idx_out, w_out: n floats each; *count = K) -> their 64-byte records (rec: 4 K float4)
 void launch_light_weights(const SceneDev& sc, float* w, cudaStream_t st);
@@ -67,14 +74,11 @@ void launch_light_weights(const SceneDev& sc, float* w, cudaStream_t st);
 void launch_env_weights(const SceneDev& sc, float* w, cudaStream_t st);
 void launch_light_compact(const float* w, int n, int32_t* idx_out, float* w_out, int32_t* count, cudaStream_t st);
 void launch_light_records(const SceneDev& sc, const int32_t* idx, int n, float4* rec, cudaStream_t st);
-void launch_blend(const RenderDev& rd, const TileDev* tiles, int nf, uint32_t batch_first_frame, const float4* Lo,
-                  const float4* Le, float* fb, cudaStream_t st);
-// adaptive sampling: k_blend<true> also keeps the running mean of the squared sample luminance and the per-pixel frame count
-void launch_blend_adaptive(const RenderDev& rd, const TileDev* tiles, int nf, uint32_t batch_first_frame, const float4* Lo,
-                           const float4* Le, float* fb, float* luma2, int32_t* spp_map, cudaStream_t st);
-// feature-buffer render: k_blend<true, true> also blends the first-hit records of aov_rec into aov (8 floats per pixel) and keeps luma2
-void launch_blend_aov(const RenderDev& rd, const TileDev* tiles, int nf, uint32_t batch_first_frame, const float4* Lo, const float4* Le,
-                      const float4* aov_rec, float* fb, float* aov, float* luma2, cudaStream_t st);
+// running mean of the batch's frames into fb (k_blend).  Adaptive sampling (luma2, spp_map): k_blend<true> also keeps the running mean of
+// the squared sample luminance and the per-pixel frame count; the feature-buffer render (luma2, aov_rec, aov; spp_map null):
+// k_blend<true, true> also blends the first-hit records of aov_rec into aov (8 floats per pixel).  Null pointers: the plain blend.
+void launch_blend(const RenderDev& rd, const TileDev* tiles, int nf, uint32_t batch_first_frame, const float4* Lo, const float4* Le,
+                  float* fb, float* luma2, int32_t* spp_map, const float4* aov_rec, float* aov, cudaStream_t st);
 // convergence test of the rd.n_tiles tiles of tiles_in after n_frames frames: the surviving tiles -> tiles_out (input order),
 // counts[0] = surviving tiles, counts[1] = their in-image pixels; keep holds rd.n_tiles bytes, *blocks_done must be 0 (left 0)
 void launch_adaptive_check(const RenderDev& rd, const TileDev* tiles_in, int n_frames, float threshold, const float* fb, const float* luma2,
