@@ -75,6 +75,7 @@ SIGNATURES = {
     "ezrt_get_counters": (C.c_int, [C.c_void_p, C.POINTER(Counters)]),
     "ezrt_get_kernel_times": (C.c_int, [C.c_void_p, C.POINTER(C.c_double), C.POINTER(C.c_uint64)]),
     "ezrt_get_w8_phase_cycles": (C.c_int, [C.c_void_p, C.POINTER(C.c_uint64)]),
+    "ezrt_get_w8_step_counts": (C.c_int, [C.c_void_p, C.POINTER(C.c_uint64)]),
     "ezrt_partition_pixels": (C.c_int64, [C.c_int, C.c_int, C.c_int, C.c_int]),
     "ezrt_partition_scatter": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]),
     "ezrt_partition_cache_clear": (C.c_int, [C.c_int]),

@@ -433,6 +433,14 @@ class Scene:
         phases = ("refill", "node", "triangle", "ray_end")
         return {k: {ph: int(c[4 * i + j]) for j, ph in enumerate(phases)} for i, k in enumerate(("k_extend_w8", "k_shadow_w8"))}
 
+    def w8_step_counts(self):
+        """{pass: {count: n}} of the same render: the warps' node and triangle steps, the rays' node visits and triangle tests
+        (ezrt_get_w8_step_counts)."""
+        c = (C.c_uint64 * 8)()
+        check(lib.ezrt_get_w8_step_counts(self._h, c))
+        names = ("node_steps", "triangle_steps", "node_visits", "triangle_tests")
+        return {k: {nm: int(c[4 * i + j]) for j, nm in enumerate(names)} for i, k in enumerate(("k_extend_w8", "k_shadow_w8"))}
+
     def trace_rays(self, origins, dirs, traverse=TRAVERSE_ACCEL, any_hit=False, p3_normal_fudge=False):
         """hitBVH for n rays on the device (P5/fsh:254-306)."""
         o = _f32(origins, (-1, 3))

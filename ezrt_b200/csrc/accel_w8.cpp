@@ -89,7 +89,7 @@ float ezrt_q16_max_scale(const uint32_t* nodes, size_t n_nodes) {
 // heuristic, after Ylitie et al. 2017 section 3.1; children have larger indices than their parent):
 //   C(n,1) = min(cost of n as ONE leaf (<= max_leaf triangles, consecutive), area(n) * cost_node + best split of n into <= width roots)
 //   C(n,i) = min(C(n,i-1), min_k C(left,k) + C(right,i-k))          i = 2..width-1: n's sub-tree represented by <= i roots
-// Visiting a wide node costs cost_node, testing one triangle cost_tri (ratio of the kernels' instruction counts).
+// Visiting a wide node costs cost_node, testing one triangle cost_tri (the 8-wide form's prices: w8_node.h, W8_COST_TRI).
 // ------------------------------------------------------------------------------------------
 int EzrtCollapse::build(const std::vector<EzrtAccelNode>& an_, int width_, int max_leaf, double cost_node, double cost_tri, int threads) {
     an = &an_;
@@ -215,11 +215,8 @@ int EzrtCollapse::children(int b, int* ch) const {
     return cnt;
 }
 
-#define W8_COST_NODE 1.0
-#define W8_COST_TRI 0.4
-
 int ezrt_build_w8(const std::vector<EzrtAccelNode>& an, const std::vector<uint32_t>& order_in, float pad, float max_abs_coord,
-                  const int axis_bit[3], EzrtW8Tree& out) {
+                  const int axis_bit[3], double cost_tri, int threads, EzrtW8Tree& out) {
     out.nodes.clear();
     out.tri_order.clear();
     out.leaf_first.assign(an.size(), -1);
@@ -230,7 +227,7 @@ int ezrt_build_w8(const std::vector<EzrtAccelNode>& an, const std::vector<uint32
     const int NB = (int)an.size();
     const double min_step = (double)max_abs_coord * (double)W8_MIN_STEP_REL;
     EzrtCollapse col;
-    const int crc = col.build(an, 8, W8_MAX_LEAF_TRIS, W8_COST_NODE, W8_COST_TRI);
+    const int crc = col.build(an, 8, W8_MAX_LEAF_TRIS, 1.0, cost_tri, threads);
     if (crc) return crc;
     const std::vector<int>& first = col.first;
     const std::vector<int>& count = col.count;

@@ -631,38 +631,42 @@ int ezrt_scene_create(int device, const float* tris, int n_triangles, const floa
     int acc_depth = 0, w8_depth = 0, w8_near_bit[3] = {0, 1, 2};
     bool have_accel = true;
     {
-        std::vector<EzrtAccelNode> an;
-        std::vector<uint32_t> order_bin;
-        // on the GPU (accel_build.cu; the same tree node for node); env EZRT_BUILD=host: the host builder (host_scene.cpp)
-        const char* be = getenv("EZRT_BUILD");
-        if (be && !strcmp(be, "host")) {
-            ezrt_build_accel(tris, n_triangles, W8_MAX_LEAF_TRIS, an, order_bin);
-            lap("acceleration tree: binary SAH build (host)");
-        } else {
-            const int brc = ezrt_build_accel_device((const float*)raw.p, n_triangles, W8_MAX_LEAF_TRIS, an, order_bin, nullptr);
-            if (brc < 0) return brc;
-            lap("acceleration tree: binary SAH build (device)");
-        }
-        // boxes inflated by 2*delta: a hit hitTriangle accepts lies within delta of its triangle's box, so
-        // the inflated boxes of the whole ancestor chain are entered no later than the hit distance
-        const float pad = 2.0f * prune_delta;
         // Which form of the tree the accel kernels walk, chosen by scene size (env EZRT_ACCEL=4 / 8 forces one):
         //   8: 8-wide nodes with 8-bit quantised boxes in octant order (k_extend_w8): 96-byte records, fewer L1 wavefronts per
         //      ray, more instructions.  On an H100 SXM it measured 2258 vs 1773 Mrays/s on C3 and 1956 vs 1546 on C4 (1 M
         //      triangles) against the 4-wide form (bench.py, 700 W)
         //   4: 4-wide nodes with exact fp32 boxes, children sorted by entry distance (k_extend_accel): 10841-10883 vs
         //      10476-10513 Mrays/s on C2 (5,300 triangles, whose tree stays in L1; bench.py, 400 W)
-        // The threshold lies between the two measured sizes.
+        // The threshold lies between the two measured sizes.  A scene of at most W8_MAX_LEAF_TRIS triangles is one leaf of the
+        // 4-wide form's binary tree, which the 4-wide builder does not take: the W8 builder handles it.
         int accel_form = (n_triangles >= (1 << 16)) ? 8 : 4;
         if (const char* we = getenv("EZRT_ACCEL")) {
             const int v = atoi(we);
             if (v == 4 || v == 8) accel_form = v;
         }
-        if (an[0].n > 0) accel_form = 8;   // a single-leaf tree: the W8 builder handles it
+        if (n_triangles <= W8_MAX_LEAF_TRIS) accel_form = 8;
+        // the binary tree's leaves: the 4-wide form keeps ranges of <= 4 triangles as leaves; the W8 form builds down to
+        // W8_BINARY_LEAF_TRIS and leaves the choice of its leaves to the collapse (w8_node.h)
+        const int leaf_n = (accel_form == 8) ? W8_BINARY_LEAF_TRIS : W8_MAX_LEAF_TRIS;
+        std::vector<EzrtAccelNode> an;
+        std::vector<uint32_t> order_bin;
+        // on the GPU (accel_build.cu; the same tree node for node); env EZRT_BUILD=host: the host builder (host_scene.cpp)
+        const char* be = getenv("EZRT_BUILD");
+        if (be && !strcmp(be, "host")) {
+            ezrt_build_accel(tris, n_triangles, leaf_n, an, order_bin);
+            lap("acceleration tree: binary SAH build (host)");
+        } else {
+            const int brc = ezrt_build_accel_device((const float*)raw.p, n_triangles, leaf_n, an, order_bin, nullptr);
+            if (brc < 0) return brc;
+            lap("acceleration tree: binary SAH build (device)");
+        }
+        // boxes inflated by 2*delta: a hit hitTriangle accepts lies within delta of its triangle's box, so
+        // the inflated boxes of the whole ancestor chain are entered no later than the hit distance
+        const float pad = 2.0f * prune_delta;
         EzrtW8Tree w8;
         ezrt_w8_axis_bits(bmin, bmax, w8_near_bit);
         if (accel_form == 8) {
-            const int wrc = ezrt_build_w8(an, order_bin, pad, max_abs, w8_near_bit, w8);
+            const int wrc = ezrt_build_w8(an, order_bin, pad, max_abs, w8_near_bit, W8_COST_TRI, ezrt_host_threads(), w8);
             if (wrc != 0 || w8.depth > EZRT_W8_SMEM_STACK + W8_LOCAL_STACK) {
                 have_accel = false;
             } else {
@@ -1440,15 +1444,30 @@ int ezrt_get_counters(ezrt_scene* s, ezrt_counters* out) {
     return EZRT_OK;
 }
 
-int ezrt_get_w8_phase_cycles(ezrt_scene* s, uint64_t* out) {
-    if (!s || !out) return ezrt_set_error(EZRT_ERR_INVALID, "get_w8_phase_cycles: null argument");
+// words [first, first + 4) of the bounce and the shadow pass's blocks of the totals (kernels.h) -> out[0..3], out[4..7]
+static int w8_pass_words(ezrt_scene* s, int first, uint64_t* out) {
     for (int k = 0; k < 8; k++) out[k] = 0;
     if (!s->have_timing) return EZRT_OK;
     CU_CHECK(cudaSetDevice(s->device));
     CU_CHECK(cudaEventSynchronize(s->ev_stop));
-    static_assert(EZRT_W8_PHASES_SHADOW == EZRT_W8_PHASES_EXTEND + 4 && 5 + EZRT_W8_PHASES_SHADOW + 4 <= EZRT_TOTALS, "totals layout");
-    CU_CHECK(cudaMemcpy(out, (unsigned long long*)s->totals_buf.p + 5 + EZRT_W8_PHASES_EXTEND, sizeof(uint64_t) * 8, cudaMemcpyDeviceToHost));
+    static_assert(5 + EZRT_W8_PHASES_SHADOW + EZRT_W8_PASS_WORDS <= EZRT_TOTALS, "totals layout");
+    unsigned long long t[EZRT_TOTALS];
+    CU_CHECK(cudaMemcpy(t, s->totals_buf.p, sizeof(t), cudaMemcpyDeviceToHost));
+    for (int k = 0; k < 4; k++) {
+        out[k] = t[5 + EZRT_W8_PHASES_EXTEND + first + k];
+        out[4 + k] = t[5 + EZRT_W8_PHASES_SHADOW + first + k];
+    }
     return EZRT_OK;
+}
+
+int ezrt_get_w8_phase_cycles(ezrt_scene* s, uint64_t* out) {
+    if (!s || !out) return ezrt_set_error(EZRT_ERR_INVALID, "get_w8_phase_cycles: null argument");
+    return w8_pass_words(s, 0, out);
+}
+
+int ezrt_get_w8_step_counts(ezrt_scene* s, uint64_t* out) {
+    if (!s || !out) return ezrt_set_error(EZRT_ERR_INVALID, "get_w8_step_counts: null argument");
+    return w8_pass_words(s, 4, out);
 }
 
 int ezrt_get_kernel_times(ezrt_scene* s, double* ms, uint64_t* launches) {

@@ -949,7 +949,8 @@ __device__ __forceinline__ uint32_t w8_clock() {
 // IDX: the scene's triangle records are indexed (SceneDev::acc_tri_indexed; one instantiation per layout keeps each within 64
 // registers without spilling)
 #define W8_ENDED (-2)   // extend_w8: `node` of a lane whose ray is traced and waits for its leaf check at the next refill
-// phase_cycles (COUNT only): += the SM cycles each warp spends in [0] refill, [1] node steps, [2] triangle steps, [3] ray ends
+// phase_cycles (COUNT only): += the SM cycles each warp spends in [0] refill, [1] node steps, [2] triangle steps, [3] ray ends,
+// then the warp's [4] node steps and [5] triangle steps and its lanes' [6] node visits and [7] triangle tests
 template <bool ANYHIT, bool COUNT, bool IDX, bool BOUNDED = false, class RayIO>
 __device__ __forceinline__ void extend_w8(const SceneDev& sc, uint32_t n, uint32_t* work, RayIO io, const unsigned char* s_perm, uint2* stack_sm,
                                           W8Counts counts, unsigned long long* phase_cycles) {
@@ -981,6 +982,7 @@ __device__ __forceinline__ void extend_w8(const SceneDev& sc, uint32_t n, uint32
     uint32_t t_base = 0, t_mask = 0;   // pending triangles of the node just visited
     uint32_t n_visits = 0, n_tests = 0;   // per lane; 32 bits keep the COUNT instantiations within 64 registers
     uint32_t cyc_refill = 0, cyc_node = 0, cyc_tri = 0, cyc_end = 0;   // COUNT: the warp's phase sums (phase_cycles)
+    uint32_t n_node_steps = 0, n_tri_steps = 0;                        // COUNT: the warp's steps of each kind
     uint32_t end_dt = 0, t_mark = COUNT ? w8_clock() : 0u;             // COUNT: this lane's ray-end span; end of the last phase
     bool exhausted = false;
     uint32_t chunk_pos = 0, chunk_end = 0;
@@ -1235,8 +1237,8 @@ __device__ __forceinline__ void extend_w8(const SceneDev& sc, uint32_t n, uint32
                 const uint32_t now = w8_clock(), e = __reduce_max_sync(FULL, end_dt);   // the ray ends of a step run side by side
                 end_dt = 0u;
                 cyc_end += e;
-                if (node_step) cyc_node += now - t_mark - e;
-                else cyc_tri += now - t_mark - e;
+                if (node_step) { cyc_node += now - t_mark - e; n_node_steps++; }
+                else { cyc_tri += now - t_mark - e; n_tri_steps++; }
                 t_mark = now;
             }
         } while (busy != 0u && (exhausted || __popc(busy) >= refill_thresh));
@@ -1246,11 +1248,15 @@ __device__ __forceinline__ void extend_w8(const SceneDev& sc, uint32_t n, uint32
     if (COUNT) {
         atomicAdd(counts.node_visits, (unsigned long long)n_visits);
         atomicAdd(counts.tri_tests, (unsigned long long)n_tests);
+        atomicAdd(phase_cycles + 6, (unsigned long long)n_visits);
+        atomicAdd(phase_cycles + 7, (unsigned long long)n_tests);
         if (lane == 0) {
             atomicAdd(phase_cycles + 0, (unsigned long long)cyc_refill);
             atomicAdd(phase_cycles + 1, (unsigned long long)cyc_node);
             atomicAdd(phase_cycles + 2, (unsigned long long)cyc_tri);
             atomicAdd(phase_cycles + 3, (unsigned long long)cyc_end);
+            atomicAdd(phase_cycles + 4, (unsigned long long)n_node_steps);
+            atomicAdd(phase_cycles + 5, (unsigned long long)n_tri_steps);
         }
     }
 }

@@ -134,10 +134,12 @@ struct EzrtW8Tree {
     long long n_children;              // occupied slots over all nodes (fill statistics)
 };
 // `order_in`: triangle order of the binary tree (ezrt_build_accel); `pad`: box inflation (2 * prune_delta);
-// axis_bit[a]: significance (0..2) of axis a in the slot index (largest scene extent -> bit 2).  Returns 0 or < 0.
+// axis_bit[a]: significance (0..2) of axis a in the slot index (largest scene extent -> bit 2); cost_tri: the collapse's price
+// of a triangle test, a node visit costing 1 (the product's: W8_COST_TRI); threads: the collapse's (the result does not
+// depend on them).  Returns 0 or < 0.
 void ezrt_w8_axis_bits(const float bmin[3], const float bmax[3], int axis_bit[3]);
 int ezrt_build_w8(const std::vector<EzrtAccelNode>& an, const std::vector<uint32_t>& order_in, float pad, float max_abs_coord,
-                  const int axis_bit[3], EzrtW8Tree& out);
+                  const int axis_bit[3], double cost_tri, int threads, EzrtW8Tree& out);
 
 // accel_w8.cpp: the largest |1/d_a| a quantised tree may be walked with (w8_node.h, "decode range"): a power of two, at most
 // W8_INV_LIMIT, small enough that the decode's terms bias * scale * |1/d_a| and 5 * max|coordinate| * |1/d_a| stay finite for

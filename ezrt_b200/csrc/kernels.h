@@ -35,10 +35,12 @@ void launch_generate(const RenderDev& rd, const TileDev* tiles, uint32_t n_slots
 void launch_extend(const SceneDev& sc, bool prune, bool anyhit, PathQueue q, const uint32_t* q_count, uint32_t* work,
                    const uint32_t* perm, int to_accel, uint32_t n_max, int n_sms, cudaStream_t st, float2* side_hit = nullptr, int gate = 0);
 // counts (params.profile = 2): [0] 128-byte node visits, [1] triangle tests, [2] quantised node visits, then the W8 kernels' phase
-// cycles (extend_w8: refill, node steps, triangle steps, ray ends) from [EZRT_W8_PHASES_EXTEND] (bounce) and [EZRT_W8_PHASES_SHADOW]
+// cycles (extend_w8: refill, node steps, triangle steps, ray ends) and their step, visit and test counts (node steps, triangle
+// steps, node visits, triangle tests), EZRT_W8_PASS_WORDS from [EZRT_W8_PHASES_EXTEND] (bounce) and from [EZRT_W8_PHASES_SHADOW]
+#define EZRT_W8_PASS_WORDS 8
 #define EZRT_W8_PHASES_EXTEND 3
-#define EZRT_W8_PHASES_SHADOW 7
-#define EZRT_TOTALS 16   // the render's 64-bit totals: rays, samples, deferred rays, then counts at [5]
+#define EZRT_W8_PHASES_SHADOW (EZRT_W8_PHASES_EXTEND + EZRT_W8_PASS_WORDS)
+#define EZRT_TOTALS 24   // the render's 64-bit totals: rays, samples, deferred rays, then counts at [5]
 // exact_gate: the exact pass over the deferred rays that follows the accel kernel -- 0: always (in line); 2: only when more than
 // EZRT_SIDE_CAP rays were deferred (the caller runs launch_deferred_lane on a side stream for the usual handful)
 void launch_extend_accel(const SceneDev& sc, PathQueue q, const uint32_t* q_count, uint32_t* work, uint32_t* defer_list,

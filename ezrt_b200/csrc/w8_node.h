@@ -72,6 +72,13 @@
 #define W8_NODE_BYTES 80
 #define W8_MAX_LEAF_TRIS 4            // triangles per leaf slot (meta count field)
 #define W8_MAX_NODE_TRIS 32           // triangles of all leaf slots of one node (bits of the triangle mask)
+// The tree the collapse starts from and what it weighs (accel_w8.cpp, capi.cu): the binary SAH tree is built down to
+// W8_BINARY_LEAF_TRIS triangles per leaf, so that the collapse, not the binary builder, decides every leaf slot (Ylitie et al.
+// 2017); a triangle test is priced at W8_COST_TRI node visits.  Measured on an H100 (700 W), a test costs 1.16 visits in the
+// bounce kernel; on single-triangle leaves, prices from 0.4 to 1.6 predict bounce-kernel cycles within 1.5 % of each other
+// (tools/w8_model.cpp sweep), and 0.4 keeps the larger leaf slots that load the cooperative triangle step.  DESIGN.md section 6.
+#define W8_BINARY_LEAF_TRIS 1
+#define W8_COST_TRI 0.4
 #define W8_SLACK_STEPS 0.25                  // outward slack of the stored planes, in quantisation steps
 #define W8_DECODE_BIAS 32768.0f              // 2^15: f = as_float(W8_DECODE_BITS | q << 8) = 2^15 + q
 #define W8_DECODE_BITS 0x47000000u

@@ -289,6 +289,9 @@ int ezrt_get_kernel_times(ezrt_scene* scene, double* ms, uint64_t* launches);
  * summed over warps: out[0..3] the bounce pass (k_extend_w8), out[4..7] the shadow pass (k_shadow_w8), each as refill, node
  * steps, triangle steps, ray ends.  All 0 for scenes traced without the 8-wide tree.  out[8]. */
 int ezrt_get_w8_phase_cycles(ezrt_scene* scene, uint64_t* out);
+/* Work of the same kernels in the same render: out[0..3] the bounce pass, out[4..7] the shadow pass, each as warp node steps,
+ * warp triangle steps, node visits (per ray, summed) and triangle tests (per ray, summed).  All 0 as above.  out[8]. */
+int ezrt_get_w8_step_counts(ezrt_scene* scene, uint64_t* out);
 
 /* Number of pixels part `rank` of `count` owns for a width x height image. */
 int64_t ezrt_partition_pixels(int width, int height, int rank, int count);

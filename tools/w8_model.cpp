@@ -6,7 +6,11 @@
 // triangles pending per node visit and a warp-level replay of the kernel's schedule (serial vs cooperative triangle step).
 //   g++ -O2 -std=c++17 -fopenmp -ffp-contract=off -mfma -Iinclude -Iezrt_b200/csrc tools/w8_model.cpp \
 //       ezrt_b200/csrc/host_scene.cpp ezrt_b200/csrc/accel_w8.cpp ezrt_b200/csrc/errors.cpp -o build/w8_model
-//   build/w8_model tris.f32 n_tris rays.f32 [brute] [bundle]   rays: 7-float records (o, d, kind) as oracle_set_ray_dump writes
+//   build/w8_model tris.f32 n_tris rays.f32 [brute] [bundle] [sweep] [prices=N,T]   rays: 7-float records (o, d, kind) as oracle_set_ray_dump writes
+//   The tree is the product's (binary leaves of W8_BINARY_LEAF_TRIS, triangle price W8_COST_TRI); sweep: the same walk on every tree of
+//   binary leaf size 1, 2, 4 times collapse triangle price 0.4, 0.7, 1.0, 1.3, 1.6, then one summary line per tree.  prices=N,T: the
+//   bounce kernel's measured warp cycles per node step and per triangle step (tools/bench_extend_phases.py), which turn the warp
+//   replay's steps into predicted cycles per 32 bounce rays.
 //   bundle: also walk every 32 consecutive rays as bundles (a ray joins the first pending ray's sub-bundle when each component of
 //   its 1/d has the same sign and lies within a factor 2) -- one stack, one conservative interval test per slot for all
 //   member rays, then every candidate triangle tested by every member in serial order -- and check it against the per-ray walk:
@@ -128,11 +132,28 @@ static void bundle_axis(float lo, float hi, int sign, float omin, float omax, fl
 }
 struct RayResult { float t; int tri; bool tie; std::vector<int> nodes, tris; };
 
+// what one tree's walk of the rays costs (the sweep's summary)
+struct TreeStats {
+    int depth = 0, n_nodes = 0, max_sp = 0;
+    double nv = 0, nt = 0, npass = 0, node_steps = 0, tri_steps = 0;   // bounce rays: per ray; warp replay (cooperative step): per 32 rays
+    double cam_nodes = 0, cam_cands = 0;                                // bundle mode: camera bundles' node visits, triangle candidates per 32 rays
+    float inv_limit = 0.0f;
+};
+
+static int model(const std::vector<float>& tris, int n, const std::vector<float>& rays, bool brute, bool bundle, int leaf_n, double cost_tri,
+                 TreeStats& S);
+
 int main(int argc, char** argv) {
-    if (argc < 4) { fprintf(stderr, "usage: w8_model tris.f32 n_tris rays.f32 [brute]\n"); return 2; }
+    if (argc < 4) { fprintf(stderr, "usage: w8_model tris.f32 n_tris rays.f32 [brute] [bundle] [sweep] [prices=N,T]\n"); return 2; }
     const int n = atoi(argv[2]);
-    bool brute = false, bundle = false;
-    for (int i = 4; i < argc; i++) { brute |= !strcmp(argv[i], "brute"); bundle |= !strcmp(argv[i], "bundle"); }
+    bool brute = false, bundle = false, sweep = false;
+    double price_node = 0.0, price_tri = 0.0;
+    for (int i = 4; i < argc; i++) {
+        brute |= !strcmp(argv[i], "brute");
+        bundle |= !strcmp(argv[i], "bundle");
+        sweep |= !strcmp(argv[i], "sweep");
+        if (!strncmp(argv[i], "prices=", 7) && sscanf(argv[i] + 7, "%lf,%lf", &price_node, &price_tri) != 2) { fprintf(stderr, "prices=N,T\n"); return 2; }
+    }
     std::vector<float> tris((size_t)n * 36);
     FILE* f = fopen(argv[1], "rb");
     if (!f || fread(tris.data(), 4, tris.size(), f) != tris.size()) { fprintf(stderr, "cannot read triangles\n"); return 1; }
@@ -144,6 +165,32 @@ int main(int argc, char** argv) {
         while (rf && fread(r, 4, 7, rf) == 7) rays.insert(rays.end(), r, r + 7);
         if (rf) fclose(rf);
     }
+    if (!sweep) {
+        TreeStats S;
+        return model(tris, n, rays, brute, bundle, W8_BINARY_LEAF_TRIS, W8_COST_TRI, S);
+    }
+    struct Row { int leaf; double cost; TreeStats S; };
+    std::vector<Row> rows;
+    for (int leaf : {1, 2, 4})
+        for (double cost : {0.4, 0.7, 1.0, 1.3, 1.6}) {
+            printf("==== binary leaves <= %d, collapse triangle price %.1f\n", leaf, cost);
+            Row r{leaf, cost, TreeStats()};
+            const int rc = model(tris, n, rays, brute, bundle, leaf, cost, r.S);
+            if (rc) return rc;
+            rows.push_back(r);
+        }
+    printf("sweep: leaf, price, W8 depth, nodes, max stack, decode range; bounce rays per ray: node visits, triangle tests, distance-check "
+           "passes; per 32 bounce rays: node steps, triangle steps, predicted warp cycles (prices %.1f, %.1f); camera bundles per 32 rays: "
+           "node visits, triangle candidates\n", price_node, price_tri);
+    for (const Row& r : rows)
+        printf("sweep %d %.1f | %d %d %d %g | %.3f %.3f %.3f | %.2f %.2f %.0f | %.2f %.2f\n", r.leaf, r.cost, r.S.depth, r.S.n_nodes, r.S.max_sp,
+               r.S.inv_limit, r.S.nv, r.S.nt, r.S.npass, r.S.node_steps, r.S.tri_steps, r.S.node_steps * price_node + r.S.tri_steps * price_tri,
+               r.S.cam_nodes, r.S.cam_cands);
+    return 0;
+}
+
+static int model(const std::vector<float>& tris, int n, const std::vector<float>& rays, bool brute, bool bundle, int leaf_n, double cost_tri,
+                 TreeStats& S) {
     const int NR = (int)(rays.size() / 7);
     float maxc = 0, bmin[3] = {3e38f, 3e38f, 3e38f}, bmax[3] = {-3e38f, -3e38f, -3e38f};
     for (int i = 0; i < n; i++)
@@ -159,9 +206,9 @@ int main(int argc, char** argv) {
 
     std::vector<EzrtAccelNode> an;
     std::vector<uint32_t> order;
-    ezrt_build_accel(tris.data(), n, 4, an, order);
+    ezrt_build_accel(tris.data(), n, leaf_n, an, order);
     EzrtW8Tree w8;
-    const int rc = ezrt_build_w8(an, order, pad, maxc, axis_bit, w8);
+    const int rc = ezrt_build_w8(an, order, pad, maxc, axis_bit, cost_tri, ezrt_host_threads(), w8);
     if (rc) { fprintf(stderr, "ezrt_build_w8 failed: %d\n", rc); return 1; }
     printf("binary nodes %zu, 8-wide nodes %d (%.1f MB), depth %d, mean fill %.2f, axis bits x%d y%d z%d\n", an.size(), w8.n_nodes,
            w8.n_nodes * (double)W8_NODE_BYTES / 1e6, w8.depth, (double)w8.n_children / w8.n_nodes, axis_bit[0], axis_bit[1], axis_bit[2]);
@@ -169,6 +216,9 @@ int main(int argc, char** argv) {
     const float max_scale = ezrt_w8_max_scale(w8.nodes.data(), (size_t)w8.n_nodes);
     const float inv_limit = ezrt_quant_inv_limit(max_scale, W8_DECODE_BIAS, maxc);
     printf("largest node scale %g, decode range |1/d| <= %g\n", max_scale, inv_limit);
+    S.depth = w8.depth;
+    S.n_nodes = w8.n_nodes;
+    S.inv_limit = inv_limit;
     {   // the 4-wide collapse the default kernel uses (same dynamic programme, width 4): every triangle in exactly one leaf of <= 4
         EzrtCollapse c4;
         if (c4.build(an, 4, W8_MAX_LEAF_TRIS, 1.0, 0.3) != 0) { fprintf(stderr, "4-wide collapse failed\n"); return 1; }
@@ -383,6 +433,8 @@ int main(int argc, char** argv) {
         { nv[kind] += my_nv; nt[kind] += my_nt; npass[kind] += my_pass; npush[kind] += my_push; cntk[kind] += 1; }
     }
     const char* names[3] = {"camera", "bounce", "shadow"};
+    if (cntk[1] > 0) { S.nv = nv[1] / cntk[1]; S.nt = nt[1] / cntk[1]; S.npass = npass[1] / cntk[1]; }
+    S.max_sp = max_sp;
     for (int k = 0; k < 3; k++)
         if (cntk[k] > 0)
             printf("%s rays %.0f: %.2f node visits, %.2f triangle tests, %.2f pushes per ray; %.3f of the tests pass the distance checks\n", names[k], cntk[k],
@@ -415,6 +467,7 @@ int main(int argc, char** argv) {
         for (int coop = 0; coop < 2; coop++) {
             const Replay R = replay(q, coop != 0, coop ? tri_w : 2, refill, 32);
             const double per = 32.0 / q.size();
+            if (k == 1 && coop) { S.node_steps = R.node_steps * per; S.tri_steps = R.tri_steps * per; }
             printf("%s rays, warp replay, %s triangle step (tri_w %d, refill %d): per 32 rays %.1f node steps (%.1f lanes busy), "
                    "%.1f triangle steps (%.1f lanes busy); 2 x node + triangle steps = %.1f\n", names[k], coop ? "cooperative" : "serial", coop ? tri_w : 2, refill,
                    R.node_steps * per, R.node_lanes / R.node_steps, R.tri_steps * per, R.tri_lanes / R.tri_steps, (2 * R.node_steps + R.tri_steps) * per);
@@ -540,6 +593,8 @@ int main(int argc, char** argv) {
         }
         if (n_members > 0) {
             const double per32 = 32.0 / n_members;
+            S.cam_nodes = b_nodes * per32;
+            S.cam_cands = b_cands * per32;
             printf("bundle: %ld (sub-)bundles, %ld member rays; per 32 rays %.2f node visits, %.2f triangle candidates; (ray, triangle) tests per ray %.2f "
                    "(per-ray walk %.2f); warp steps per 32 rays %.2f node + %.2f triangle\n", n_bundles, n_members, b_nodes * per32, b_cands * per32,
                    (double)b_tests / n_members, (double)r_tests / n_members, b_nodes * per32, b_cands * per32);
