@@ -33,6 +33,8 @@ _o.oracle_sobol.argtypes = [C.c_uint32, C.c_uint32]
 _o.oracle_cp_rotation.restype = None
 _o.oracle_cp_rotation.argtypes = [_fp, C.c_uint32, C.c_uint32]
 _o.oracle_pi.restype = C.c_float
+_o.oracle_set_ray_dump.restype = C.c_uint64
+_o.oracle_set_ray_dump.argtypes = [_fp, C.c_uint64]
 
 COUNTER_NAMES = ["rays_primary", "rays_bounce", "rays_shadow", "n_node", "n_tri", "hits", "hdr_lookups", "samples", "max_stack"]
 
@@ -65,6 +67,23 @@ def render(tris, nodes, cfg, hdr=None, hdr_cache=None, hdr_linear=True, framebuf
     c = {k: int(v) for k, v in zip(COUNTER_NAMES, cnt)}
     c["rays"] = c["rays_primary"] + c["rays_bounce"] + c["rays_shadow"]
     return fb, c
+
+
+def render_rays(tris, nodes, cfg, hdr=None, hdr_cache=None, hdr_linear=True, window=None):
+    """render() that also returns the rays the render traced: (image, counters, rays [n, 7] float32), every ray's origin,
+    direction and kind (0 camera, 1 bounce, 2 shadow; oracle_set_ray_dump).  The oracle renders on many threads, so the
+    rows come in no fixed order: compare sums over rays only."""
+    x0, y0, x1, y1 = (0, 0, cfg.width, cfg.height) if window is None else window
+    cap = (x1 - x0) * (y1 - y0) * cfg.spp * (2 * cfg.max_bounce + 3)   # a camera ray, then a bounce and a shadow ray per bounce
+    buf = np.zeros((cap, 7), np.float32)
+    _o.oracle_set_ray_dump(_f(buf), cap)
+    try:
+        img, c = render(tris, nodes, cfg, hdr=hdr, hdr_cache=hdr_cache, hdr_linear=hdr_linear, window=window)
+    finally:
+        seen = int(_o.oracle_set_ray_dump(None, 0))
+    if seen > cap or seen != c["rays"]:
+        raise RuntimeError("oracle ray dump: %d rays seen, %d counted, room for %d" % (seen, c["rays"], cap))
+    return img, c, buf[:seen]
 
 
 def trace_rays(tris, nodes, origins, dirs, traverse=0, p3_fudge=False, brute=False):

@@ -6,16 +6,17 @@ import re
 import subprocess
 
 import numpy as np
+import pytest
 
 from ezrt_b200 import build, scenes
 
 
-def _run_model(tmp_path, tris, rays, brute):
+def _run_model(tmp_path, tris, rays, brute, *flags):
     exe = build.build_w8_model()
     tf, rf = os.path.join(tmp_path, "tris.f32"), os.path.join(tmp_path, "rays.f32")
     np.ascontiguousarray(tris, np.float32).tofile(tf)
     np.ascontiguousarray(rays, np.float32).tofile(rf)
-    r = subprocess.run([exe, tf, str(tris.shape[0]), rf] + (["brute"] if brute else []), stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True, timeout=600)
+    r = subprocess.run([exe, tf, str(tris.shape[0]), rf] + (["brute"] if brute else []) + list(flags), stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True, timeout=600)
     assert r.returncode == 0, r.stdout
     assert "differing from" in r.stdout and ": 0 of" in r.stdout, r.stdout
     assert "violations 0" in r.stdout, r.stdout        # the 4-wide collapse covers every triangle exactly once, leaves <= 4
@@ -173,3 +174,101 @@ def test_w4_builder_is_thread_count_independent_and_well_formed(tmp_path):
     soup[:, :9] = (c + rng.uniform(-0.05, 0.05, (70000, 3, 3))).reshape(-1, 9).astype(np.float32)
     soup[:300, :9] = soup[0, :9]                 # coincident triangles
     _run_w4_check(str(tmp_path), soup)
+
+
+_TOTALS = r"^totals %s rays (\d+) gate (\d+) ties (\d+) visits (\d+) tests (\d+) tests_max (\d+)$"
+
+
+def _totals(out, kind):
+    return dict(zip(("rays", "gate", "ties", "visits", "tests", "tests_max"), map(int, _model_stat(out, re.compile(_TOTALS % kind, re.M)).groups())))
+
+
+def _as_kind(rays, kind):
+    r = rays.copy()
+    r[:, 6] = kind
+    return r
+
+
+def _any_hit_against_brute_force(tmp_path, tris, rays):
+    """Shadow rays (kind 2) walked any-hit: hit exactly where brute force finds a hit (the model's own check, brute), min <=
+    max, and on rays that miss everything both equal the closest-hit walk's count, and so do the node visits."""
+    out = _run_model(tmp_path, tris, _as_kind(rays, 2), brute=True)
+    s = _totals(out, "shadow")
+    assert s["rays"] > 0 and s["tests"] <= s["tests_max"]
+    assert s["tests"] < s["tests_max"]          # some first hits leave triangles of their node untested in the serial order
+    hits = int(_model_stat(out, r"\((\d+) of them hit\)").group(1))
+    assert 0 < hits < s["rays"]
+    b = _totals(_run_model(tmp_path, tris, _as_kind(rays, 1), brute=True), "bounce")
+    assert s["visits"] < b["visits"] and s["tests"] < b["tests"]   # the first hit ends a shadow ray early
+    # per ray: a ray that misses walks the same nodes and tests the same triangles either way
+    both = np.concatenate([_as_kind(rays, 1), _as_kind(rays, 2)])
+    per = {}
+    for r, kind, v, t, tm, hit in (map(int, m.groups()) for m in re.finditer(r"^ray (\d+) (\d) (\d+) (\d+) (\d+) (\d)$", _run_model(tmp_path, tris, both, True, "per_ray"), re.M)):
+        per[(kind, r % len(rays))] = (v, t, tm, hit)
+    misses = [r for (kind, r), x in per.items() if kind == 2 and not x[3]]
+    assert len(misses) > 100
+    for r in misses:
+        v, t, tm, _ = per[(2, r)]
+        assert t == tm and (v, t, t) == per[(1, r)][:3], (r, per[(1, r)], per[(2, r)])
+    assert all(per[(1, r)][3] == per[(2, r)][3] for kind, r in per if kind == 2)
+
+
+def test_w8_any_hit_walk_on_the_bunny_scene(tmp_path):
+    tris, _, _, _ = scenes.s_p3_bunny()
+    _any_hit_against_brute_force(str(tmp_path), tris, _rays(tris, 20000, 4))
+
+
+def test_w8_any_hit_walk_on_a_degenerate_soup(tmp_path):
+    rng = np.random.default_rng(6)
+    n = 3000
+    tris = np.zeros((n, 36), np.float32)
+    p = rng.uniform(-1, 1, (n, 3, 3)).astype(np.float32) * rng.choice([1e-3, 0.1, 1.0], (n, 1, 1)).astype(np.float32)
+    p += rng.uniform(-2, 2, (n, 1, 3)).astype(np.float32)
+    p[:200] = p[0]                      # 200 coincident triangles
+    p[200:260, 2] = p[200:260, 1]       # zero-area
+    tris[:, :9] = p.reshape(n, 9)
+    tris[:, 21:24] = 1.0
+    _any_hit_against_brute_force(str(tmp_path), tris, _rays(tris, 6000, 7))
+
+
+def test_w8_totals_agree_with_the_per_ray_averages(tmp_path):
+    """The integer totals line and the per-ray summary line describe the same walk."""
+    tris, _, _, _ = scenes.s_p3_bunny()
+    rays = _rays(tris, 20000, 1)
+    rays[1::3, 6] = 2
+    out = _run_model(str(tmp_path), tris, rays, brute=True)
+    gate = 0
+    for kind in ("bounce", "shadow"):
+        t = _totals(out, kind)
+        m = _model_stat(out, r"%s rays (\d+): (\S+) node visits, (\S+) triangle tests" % kind)
+        assert int(m.group(1)) == t["rays"]
+        assert float(m.group(2)) == pytest.approx(t["visits"] / t["rays"], abs=0.005)
+        assert float(m.group(3)) == pytest.approx(t["tests"] / t["rays"], abs=0.005)
+        gate += t["gate"]
+        assert t["rays"] + t["gate"] == (rays[:, 6] == (1 if kind == "bounce" else 2)).sum()
+    assert gate == int(_model_stat(out, r"rays left to the exact kernel (\d+)").group(1)) > 0
+    assert _totals(out, "bounce")["ties"] + _totals(out, "shadow")["ties"] == _ties(out)
+
+
+def _run_threads(tmp_path, tris, threads="1,2,5,16"):
+    exe = build.build_w8_model()
+    tf, rf = os.path.join(tmp_path, "tris_t.f32"), os.path.join(tmp_path, "rays_t.f32")
+    np.ascontiguousarray(tris, np.float32).tofile(tf)
+    _rays(tris, 64, 9).tofile(rf)
+    r = subprocess.run([exe, tf, str(tris.shape[0]), rf, "threads=" + threads], stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True, timeout=600)
+    assert r.returncode == 0, r.stdout
+    for t in threads.split(","):
+        assert "threads %s: identical" % t in r.stdout, r.stdout
+
+
+def test_w8_builder_is_thread_count_independent(tmp_path):
+    """ezrt_build_w8's collapse runs on ezrt_host_threads() threads: the same node words, tri_order and leaf_first for 1, 2, 5
+    and 16 threads, on the bunny and on 70,000 triangles with coincident ones (> 65,536 binary nodes)."""
+    tris, _, _, _ = scenes.s_p3_bunny()
+    _run_threads(str(tmp_path), tris)
+    rng = np.random.default_rng(11)
+    soup = np.zeros((70000, 36), np.float32)
+    c = rng.uniform(-5, 5, (70000, 1, 3))
+    soup[:, :9] = (c + rng.uniform(-0.05, 0.05, (70000, 3, 3))).reshape(-1, 9).astype(np.float32)
+    soup[:300, :9] = soup[0, :9]
+    _run_threads(str(tmp_path), soup)

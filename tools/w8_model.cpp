@@ -15,7 +15,22 @@
 //   its 1/d has the same sign and lies within a factor 2) -- one stack, one conservative interval test per slot for all
 //   member rays, then every candidate triangle tested by every member in serial order -- and check it against the per-ray walk:
 //   equal (t, triangle, tie), and every node / triangle of the per-ray walk visited / tested by the bundle.
-//   The bundle bound and its arithmetic: w8_node.h "Bundle bound".
+//   The bundle bound and its arithmetic: w8_node.h "Bundle bound".  Kind-2 (shadow) rays stay out of the bundles: the camera
+//   pass never traces them.
+//   Kind-2 rays are walked any-hit, as extend_w8<ANYHIT = true> (k_shadow_w8) walks them: unbounded (P5's shadow rays), the first
+//   strict hit ends the ray after the node it was found in, and the check is hit / miss against brute force (or the exact
+//   boxes).  Their triangle tests have two totals: min, the serial order's (up to and including the first strict hit), and
+//   max, every triangle pending at that node.  The kernel's cooperative step tests an owner's run of pairs at once and where
+//   the run splits depends on the rays sharing the warp, so its count lies between the two; node visits are exact.
+//   Machine-readable lines after the summary (integers; test_w8_tree.py, test_gpu_w8_counts.py parse them):
+//     totals <camera|bounce|shadow> rays R gate G ties T visits V tests N tests_max M   (per kind: rays walked, rays left to the
+//       exact kernel, rays with a tie, node visits, triangle tests; tests_max = tests except for shadow rays)
+//     bundle totals bundles B members K visits V tests N   (bundle mode: (sub-)bundle node visits, member x candidate tests --
+//       what extend_w8_bundle counts: one visit per warp per node, one test per member lane per candidate triangle)
+//   per_ray: also "ray <index> <kind> <visits> <tests> <tests_max> <hit>" for every walked ray and (bundle mode) "bundle_at <first
+//     record> <visits> <tests>" for every 32 records holding a bundle, in record order.
+//   threads=a,b,...: rebuild the 8-wide tree with ezrt_build_w8 on each thread count and check that the node words, tri_order and
+//     leaf_first equal those of the ezrt_host_threads() build ("threads <t>: identical" / "differs"; exit 7 if any differs).
 #include <fenv.h>
 #include <math.h>
 #include <stdint.h>
@@ -140,19 +155,30 @@ struct TreeStats {
     float inv_limit = 0.0f;
 };
 
-static int model(const std::vector<float>& tris, int n, const std::vector<float>& rays, bool brute, bool bundle, int leaf_n, double cost_tri,
+struct Options { bool brute = false, bundle = false, per_ray = false; std::vector<int> threads; };
+static int model(const std::vector<float>& tris, int n, const std::vector<float>& rays, const Options& opt, int leaf_n, double cost_tri,
                  TreeStats& S);
 
 int main(int argc, char** argv) {
-    if (argc < 4) { fprintf(stderr, "usage: w8_model tris.f32 n_tris rays.f32 [brute] [bundle] [sweep] [prices=N,T]\n"); return 2; }
+    if (argc < 4) { fprintf(stderr, "usage: w8_model tris.f32 n_tris rays.f32 [brute] [bundle] [sweep] [per_ray] [prices=N,T] [threads=a,b,...]\n"); return 2; }
     const int n = atoi(argv[2]);
-    bool brute = false, bundle = false, sweep = false;
+    Options opt;
+    bool sweep = false;
     double price_node = 0.0, price_tri = 0.0;
     for (int i = 4; i < argc; i++) {
-        brute |= !strcmp(argv[i], "brute");
-        bundle |= !strcmp(argv[i], "bundle");
+        opt.brute |= !strcmp(argv[i], "brute");
+        opt.bundle |= !strcmp(argv[i], "bundle");
+        opt.per_ray |= !strcmp(argv[i], "per_ray");
         sweep |= !strcmp(argv[i], "sweep");
         if (!strncmp(argv[i], "prices=", 7) && sscanf(argv[i] + 7, "%lf,%lf", &price_node, &price_tri) != 2) { fprintf(stderr, "prices=N,T\n"); return 2; }
+        if (!strncmp(argv[i], "threads=", 8))
+            for (const char* c = argv[i] + 8; *c;) {
+                char* e;
+                const long t = strtol(c, &e, 10);
+                if (e == c || t < 1) { fprintf(stderr, "threads=a,b,...\n"); return 2; }
+                opt.threads.push_back((int)t);
+                c = *e == ',' ? e + 1 : e;
+            }
     }
     std::vector<float> tris((size_t)n * 36);
     FILE* f = fopen(argv[1], "rb");
@@ -167,7 +193,7 @@ int main(int argc, char** argv) {
     }
     if (!sweep) {
         TreeStats S;
-        return model(tris, n, rays, brute, bundle, W8_BINARY_LEAF_TRIS, W8_COST_TRI, S);
+        return model(tris, n, rays, opt, W8_BINARY_LEAF_TRIS, W8_COST_TRI, S);
     }
     struct Row { int leaf; double cost; TreeStats S; };
     std::vector<Row> rows;
@@ -175,7 +201,7 @@ int main(int argc, char** argv) {
         for (double cost : {0.4, 0.7, 1.0, 1.3, 1.6}) {
             printf("==== binary leaves <= %d, collapse triangle price %.1f\n", leaf, cost);
             Row r{leaf, cost, TreeStats()};
-            const int rc = model(tris, n, rays, brute, bundle, leaf, cost, r.S);
+            const int rc = model(tris, n, rays, opt, leaf, cost, r.S);
             if (rc) return rc;
             rows.push_back(r);
         }
@@ -189,8 +215,9 @@ int main(int argc, char** argv) {
     return 0;
 }
 
-static int model(const std::vector<float>& tris, int n, const std::vector<float>& rays, bool brute, bool bundle, int leaf_n, double cost_tri,
+static int model(const std::vector<float>& tris, int n, const std::vector<float>& rays, const Options& opt, int leaf_n, double cost_tri,
                  TreeStats& S) {
+    const bool brute = opt.brute, bundle = opt.bundle;
     const int NR = (int)(rays.size() / 7);
     float maxc = 0, bmin[3] = {3e38f, 3e38f, 3e38f}, bmax[3] = {-3e38f, -3e38f, -3e38f};
     for (int i = 0; i < n; i++)
@@ -216,6 +243,14 @@ static int model(const std::vector<float>& tris, int n, const std::vector<float>
     const float max_scale = ezrt_w8_max_scale(w8.nodes.data(), (size_t)w8.n_nodes);
     const float inv_limit = ezrt_quant_inv_limit(max_scale, W8_DECODE_BIAS, maxc);
     printf("largest node scale %g, decode range |1/d| <= %g\n", max_scale, inv_limit);
+    bool threads_differ = false;
+    for (int t : opt.threads) {   // the collapse's result must not depend on its thread count
+        EzrtW8Tree w;
+        if (ezrt_build_w8(an, order, pad, maxc, axis_bit, cost_tri, t, w)) { fprintf(stderr, "ezrt_build_w8 failed on %d threads\n", t); return 1; }
+        const bool same = w.n_nodes == w8.n_nodes && w.depth == w8.depth && w.nodes == w8.nodes && w.tri_order == w8.tri_order && w.leaf_first == w8.leaf_first;
+        printf("threads %d: %s\n", t, same ? "identical" : "differs");
+        threads_differ |= !same;
+    }
     S.depth = w8.depth;
     S.n_nodes = w8.n_nodes;
     S.inv_limit = inv_limit;
@@ -261,6 +296,9 @@ static int model(const std::vector<float>& tris, int n, const std::vector<float>
     // W8M_EXACT=1 exact child boxes instead of the quantised ones (how much the 8-bit planes cost)
     const bool x_sort = getenv("W8M_SORT") && atoi(getenv("W8M_SORT")), x_gmin = getenv("W8M_GMIN") && atoi(getenv("W8M_GMIN"));
     double nv[3] = {0, 0, 0}, nt[3] = {0, 0, 0}, npass[3] = {0, 0, 0}, npush[3] = {0, 0, 0}, cntk[3] = {0, 0, 0};
+    long long tot_rays[3] = {0, 0, 0}, tot_gate[3] = {0, 0, 0}, tot_ties[3] = {0, 0, 0}, tot_nv[3] = {0, 0, 0}, tot_nt[3] = {0, 0, 0}, tot_nt_max[3] = {0, 0, 0};
+    std::vector<long long> ray_nv(opt.per_ray ? NR : 0), ray_nt(opt.per_ray ? NR : 0), ray_nt_max(opt.per_ray ? NR : 0);
+    std::vector<char> ray_hit(opt.per_ray ? NR : 0);
     long mismatch = 0, skipped = 0, ties = 0, hits = 0;
     int max_sp = 0;
     std::vector<std::vector<uint8_t>> trace(NR);   // triangles pending after each node visit, for the warp replay
@@ -276,9 +314,13 @@ static int model(const std::vector<float>& tris, int n, const std::vector<float>
         const float olim = W8_ORIGIN_LIMIT_REL * maxc;
         if (!(ax <= inv_limit && ay <= inv_limit && az <= inv_limit && ax >= W8_INV_MIN && ay >= W8_INV_MIN && az >= W8_INV_MIN) || !(fabsf(oo[0]) <= olim && fabsf(oo[1]) <= olim && fabsf(oo[2]) <= olim)) {
             skipped++;  // the kernel hands these to the exact traversal
+#pragma omp atomic
+            tot_gate[kind]++;
             continue;
         }
         ray_kind[r] = kind;
+        const bool anyhit = kind == 2;
+        long long my_nt_max = -1;   // any-hit: tests up to the end of the node of the first strict hit (-1: no hit yet)
         const float slack = delta * fmaxf(ax, fmaxf(ay, az));
         uint32_t near_mask = 0;
         for (int a = 0; a < 3; a++) if (dd[a] >= 0.0f) near_mask |= 1u << axis_bit[a];
@@ -351,6 +393,7 @@ static int model(const std::vector<float>& tris, int n, const std::vector<float>
                     g_bits = imask | (inner << 8);
                 }
             }
+            const long long node_end = (long long)my_nt + __builtin_popcount(t_mask);
             while (t_mask) {  // the node's triangles, lowest offset first
                 const int k = __builtin_ctz(t_mask);
                 t_mask &= t_mask - 1;
@@ -362,7 +405,9 @@ static int model(const std::vector<float>& tris, int n, const std::vector<float>
                 if (bundle) res[r].tris.push_back((int)(t_base + k));
                 if (h == 2) tie = true;
                 else if (h == 1) { best = t; tie = false; best_tri = (int)(t_base + k); }
+                if (anyhit && h == 1) { my_nt_max = node_end; break; }   // the first strict hit ends a shadow ray
             }
+            if (my_nt_max >= 0) break;
             bool done = false;
             while ((g_bits >> 8) == 0) {
                 if (sp == 0) { done = true; break; }
@@ -427,10 +472,15 @@ static int model(const std::vector<float>& tris, int n, const std::vector<float>
                 cur = stk[--sp2];
             }
         }
-        if (memcmp(&want, &best, 4) != 0) mismatch++;
+        if (anyhit ? (want < EZ_INF) != (best < EZ_INF) : memcmp(&want, &best, 4) != 0) mismatch++;
         if (want < EZ_INF) hits++;
+        if (my_nt_max < 0) my_nt_max = (long long)my_nt;
+        if (opt.per_ray) { ray_nv[r] = (long long)my_nv; ray_nt[r] = (long long)my_nt; ray_nt_max[r] = my_nt_max; ray_hit[r] = best < EZ_INF; }
 #pragma omp critical
-        { nv[kind] += my_nv; nt[kind] += my_nt; npass[kind] += my_pass; npush[kind] += my_push; cntk[kind] += 1; }
+        {
+            nv[kind] += my_nv; nt[kind] += my_nt; npass[kind] += my_pass; npush[kind] += my_push; cntk[kind] += 1;
+            tot_rays[kind]++; tot_ties[kind] += tie; tot_nv[kind] += (long long)my_nv; tot_nt[kind] += (long long)my_nt; tot_nt_max[kind] += my_nt_max;
+        }
     }
     const char* names[3] = {"camera", "bounce", "shadow"};
     if (cntk[1] > 0) { S.nv = nv[1] / cntk[1]; S.nt = nt[1] / cntk[1]; S.npass = npass[1] / cntk[1]; }
@@ -475,11 +525,12 @@ static int model(const std::vector<float>& tris, int n, const std::vector<float>
     }
     if (bundle) {   // 32 consecutive rays, one stack, one bundle test per slot, serial triangle tests per member (see the top of the file)
         long b_nodes = 0, b_cands = 0, b_tests = 0, r_tests = 0, n_members = 0, n_bundles = 0, bad_result = 0, bad_nodes = 0, bad_tris = 0;
+        std::vector<long long> at_nv(opt.per_ray ? (NR + 31) / 32 : 0), at_nt(at_nv.size());   // per_ray: per 32 records
 #pragma omp parallel for schedule(dynamic, 4) reduction(+ : b_nodes, b_cands, b_tests, r_tests, n_members, n_bundles, bad_result, bad_nodes, bad_tris)
         for (int b0 = 0; b0 < NR; b0 += 32) {
             const int nb = std::min(32, NR - b0);
             int pend[32], np_ = 0;
-            for (int j = 0; j < nb; j++) if (ray_kind[b0 + j] >= 0) pend[np_++] = b0 + j;
+            for (int j = 0; j < nb; j++) if (ray_kind[b0 + j] >= 0 && ray_kind[b0 + j] != 2) pend[np_++] = b0 + j;
             // sub-bundles: a ray joins the first pending ray's when every component of its 1/d has the leader's sign and lies
             // within a factor 2 of the leader's (extend_w8_bundle)
             while (np_ > 0) {
@@ -579,6 +630,7 @@ static int model(const std::vector<float>& tris, int n, const std::vector<float>
             b_nodes += (long)vis.size();
             b_cands += (long)cand.size();
             b_tests += (long)cand.size() * nm;
+            if (opt.per_ray) { at_nv[b0 / 32] += (long long)vis.size(); at_nt[b0 / 32] += (long long)cand.size() * nm; }
             n_members += nm;
             std::sort(vis.begin(), vis.end());
             std::sort(cand.begin(), cand.end());
@@ -599,11 +651,23 @@ static int model(const std::vector<float>& tris, int n, const std::vector<float>
                    "(per-ray walk %.2f); warp steps per 32 rays %.2f node + %.2f triangle\n", n_bundles, n_members, b_nodes * per32, b_cands * per32,
                    (double)b_tests / n_members, (double)r_tests / n_members, b_nodes * per32, b_cands * per32);
             printf("bundle checks: results differing %ld, rays with a node missing %ld, rays with a triangle missing %ld\n", bad_result, bad_nodes, bad_tris);
+        }
+        printf("bundle totals bundles %ld members %ld visits %ld tests %ld\n", n_bundles, n_members, b_nodes, b_tests);
+        for (size_t b = 0; b < at_nv.size(); b++)
+            if (at_nv[b]) printf("bundle_at %zu %lld %lld\n", 32 * b, at_nv[b], at_nt[b]);
+        if (n_members > 0) {
             if (bad_result) return 6;
             if (bad_nodes || bad_tris) return 5;
         }
     }
     printf("max stack depth %d, rays left to the exact kernel %ld, rays with a tie %ld\n", max_sp, skipped, ties);
     printf("closest-hit distances differing from %s: %ld of %d rays (%ld of them hit)\n", brute ? "brute force" : "the exact-box traversal", mismatch, NR, hits);
-    return mismatch == 0 ? 0 : 3;
+    for (int k = 0; k < 3; k++)
+        printf("totals %s rays %lld gate %lld ties %lld visits %lld tests %lld tests_max %lld\n", names[k], tot_rays[k], tot_gate[k], tot_ties[k], tot_nv[k],
+               tot_nt[k], tot_nt_max[k]);
+    if (opt.per_ray)
+        for (int r = 0; r < NR; r++)
+            if (ray_kind[r] >= 0) printf("ray %d %d %lld %lld %lld %d\n", r, ray_kind[r], ray_nv[r], ray_nt[r], ray_nt_max[r], (int)ray_hit[r]);
+    if (mismatch) return 3;
+    return threads_differ ? 7 : 0;
 }
