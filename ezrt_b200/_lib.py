@@ -43,6 +43,11 @@ class Medium(C.Structure):
                 ("reserved", C.c_int32)]
 
 
+class Texture(C.Structure):
+    """struct ezrt_texture (include/ezrt.h)."""
+    _fields_ = [("width", C.c_int32), ("height", C.c_int32), ("rgba", C.c_void_p), ("reserved", C.c_int32)]
+
+
 class Counters(C.Structure):
     """struct ezrt_counters (include/ezrt.h)."""
     _fields_ = [
@@ -61,6 +66,8 @@ SIGNATURES = {
                                     C.c_int, C.POINTER(C.c_void_p)]),
     "ezrt_scene_destroy": (C.c_int, [C.c_void_p]),
     "ezrt_scene_set_medium": (C.c_int, [C.c_void_p, C.POINTER(Medium)]),
+    "ezrt_scene_set_textures": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(Texture), c_float_p, c_int32_p]),
+    "ezrt_scene_sample_textures": (C.c_int, [C.c_void_p, C.c_int, c_int32_p, c_float_p, c_float_p, c_float_p]),
     "ezrt_render": (C.c_int, [C.c_void_p, C.POINTER(RenderParams), c_float_p]),
     "ezrt_render_device": (C.c_int, [C.c_void_p, C.POINTER(RenderParams), C.c_void_p, C.c_void_p]),
     "ezrt_render_adaptive_device": (C.c_int, [C.c_void_p, C.POINTER(RenderParams), C.POINTER(AdaptiveParams), C.c_void_p, C.c_void_p,
@@ -100,6 +107,9 @@ SIGNATURES = {
     "ezrt_trilist_read_obj": (C.c_int, [C.c_void_p, C.c_char_p, c_float_p, c_float_p, C.c_int]),
     "ezrt_trilist_read_obj_text": (C.c_int, [C.c_void_p, C.c_char_p, C.c_size_t, c_float_p, c_float_p, C.c_int]),
     "ezrt_trilist_append_encoded": (C.c_int, [C.c_void_p, c_float_p, C.c_int]),
+    "ezrt_trilist_read_obj_textured": (C.c_int, [C.c_void_p, C.c_char_p, c_float_p, c_float_p, C.c_int, C.c_int32]),
+    "ezrt_trilist_read_obj_textured_text": (C.c_int, [C.c_void_p, C.c_char_p, C.c_size_t, c_float_p, c_float_p, C.c_int, C.c_int32]),
+    "ezrt_trilist_encode_texcoords": (C.c_int, [C.c_void_p, c_float_p, c_int32_p]),
     "ezrt_trilist_build_bvh": (C.c_int, [C.c_void_p, C.c_int, C.c_int]),
     "ezrt_trilist_node_count": (C.c_int, [C.c_void_p]),
     "ezrt_trilist_encode_triangles": (C.c_int, [C.c_void_p, c_float_p]),

@@ -249,6 +249,24 @@ def build_oracle_medium(force=False):
     return ORACLE_MEDIUM_SO
 
 
+ORACLE_TEXTURES_SO = os.path.join(ROOT, "build", "libezrt_oracle_textures.so")
+
+
+def build_oracle_textures(force=False):
+    """build/libezrt_oracle_textures.so: tests/oracle_textures.cpp, the CPU restatement of base-colour textures (the barycentrics, the
+    filter, the flagged render) over the medium restatement (test infrastructure, loaded only by tests/oracle_textures.py)."""
+    src = os.path.join(ROOT, "tests", "oracle_textures.cpp")
+    deps = [src] + [os.path.join(ROOT, "tests", f) for f in ("oracle_medium.cpp", "oracle_lens.cpp", "oracle_transmission.cpp", "oracle_env_light.cpp",
+                                                              "oracle_lights.cpp")] + \
+        [os.path.join(ROOT, "oracle", "ezrt_oracle.cpp")] + [os.path.join(INCLUDE, f) for f in os.listdir(INCLUDE)]
+    if force or _newer(ORACLE_TEXTURES_SO, deps):
+        os.makedirs(os.path.dirname(ORACLE_TEXTURES_SO), exist_ok=True)
+        tmp = ORACLE_TEXTURES_SO + ".tmp%d" % os.getpid()
+        _run(["g++"] + HOST_FLAGS + ["-fopenmp", "-Wno-misleading-indentation", "-shared", "-I", INCLUDE, src, "-o", tmp])
+        os.replace(tmp, ORACLE_TEXTURES_SO)
+    return ORACLE_TEXTURES_SO
+
+
 def build_reference_hdrloader(force=False):
     return _oracle_recipes().build_reference_hdrloader(force)
 
@@ -314,6 +332,7 @@ def build_all(force=False, verbose=False):
     build_oracle_transmission(force=force)
     build_oracle_lens(force=force)
     build_oracle_medium(force=force)
+    build_oracle_textures(force=force)
     build_example(force=force)
     build_reference_hdrloader(force=force)
     build_reference_shaders(force=force)

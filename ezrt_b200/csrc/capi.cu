@@ -107,6 +107,11 @@ struct ezrt_scene {
     // the homogeneous medium of EZRT_PARAM_MEDIUM (ezrt_scene_set_medium), copied into the kernels' parameters at every render
     bool has_medium = false;
     MediumDev medium{};
+    // the base-colour textures of EZRT_PARAM_TEXTURES (ezrt_scene_set_textures): sRGB table | texture table | texels, and the texcoord
+    // records in reference | accel order; tex.sh_base is set per render
+    DeviceBuffer tex_buf, tex_rec_buf;
+    bool has_textures = false;
+    TexDev tex{};
     void* hot_base = nullptr;   // accel nodes | geometry (| vertices) | shading records (L2 persisting window)
     size_t hot_bytes = 0;
     size_t l2_persist_bytes = 0;
@@ -209,6 +214,11 @@ int validate_params(const ezrt_scene* scene, const ezrt_render_params* p) {
         if (p->reserved[0] & EZRT_PARAM_TRANSMISSION)
             return ezrt_set_error(EZRT_ERR_INVALID, "render: EZRT_PARAM_MEDIUM is not rendered with EZRT_PARAM_TRANSMISSION (glass is defined with vacuum outside)");
         if (!scene->has_medium) return ezrt_set_error(EZRT_ERR_INVALID, "render: EZRT_PARAM_MEDIUM needs a medium (ezrt_scene_set_medium)");
+    }
+    if (p->reserved[0] & EZRT_PARAM_TEXTURES) {
+        if (p->mode != EZRT_MODE_DISNEY_LIGHTS)
+            return ezrt_set_error(EZRT_ERR_INVALID, "render: EZRT_PARAM_TEXTURES needs the light sampling mode (got mode %d)", p->mode);
+        if (!scene->has_textures) return ezrt_set_error(EZRT_ERR_INVALID, "render: EZRT_PARAM_TEXTURES needs textures (ezrt_scene_set_textures)");
     }
     if (p->max_bounce < 0 || p->max_bounce > 64) return ezrt_set_error(EZRT_ERR_INVALID, "render: max_bounce out of range");
     if (p->out_channels != 3 && p->out_channels != 4) return ezrt_set_error(EZRT_ERR_INVALID, "render: out_channels must be 3 or 4");
@@ -917,6 +927,115 @@ int ezrt_scene_set_medium(ezrt_scene* s, const ezrt_medium* m) {
     return EZRT_OK;
 }
 
+int ezrt_scene_set_textures(ezrt_scene* s, int n_textures, const ezrt_texture* textures, const float* texcoords, const int32_t* texture_id) {
+    if (!s) return ezrt_set_error(EZRT_ERR_INVALID, "scene_set_textures: null scene");
+    CU_CHECK(cudaSetDevice(s->device));
+    if (!textures) {
+        CU_CHECK(cudaDeviceSynchronize());   // renders already enqueued still read the buffers
+        s->tex_buf.release(); s->tex_rec_buf.release();
+        s->has_textures = false;
+        s->tex = TexDev{};
+        return EZRT_OK;
+    }
+    const int n_tri = s->dev.n_triangles;
+    if (n_textures < 1 || !texcoords || !texture_id) return ezrt_set_error(EZRT_ERR_INVALID, "scene_set_textures: bad argument");
+    size_t n_texels = 0;
+    for (int k = 0; k < n_textures; k++) {
+        const ezrt_texture& t = textures[k];
+        if (t.width < 1 || t.width > 16384 || t.height < 1 || t.height > 16384)
+            return ezrt_set_error(EZRT_ERR_INVALID, "scene_set_textures: texture %d is %dx%d (each side 1 to 16384)", k, t.width, t.height);
+        if (!t.rgba || t.reserved != 0) return ezrt_set_error(EZRT_ERR_INVALID, "scene_set_textures: texture %d has no texels or reserved != 0", k);
+        n_texels += (size_t)t.width * t.height;
+    }
+    for (int i = 0; i < n_tri; i++)
+        if (texture_id[i] < -1 || texture_id[i] >= n_textures)
+            return ezrt_set_error(EZRT_ERR_INVALID, "scene_set_textures: triangle %d has texture id %d (valid: -1 to %d)", i, texture_id[i], n_textures - 1);
+    // host staging: sRGB table | texture table | texels; reference-order records.  The new buffers are filled before the previous
+    // ones are released, so that a failure leaves the scene's textures as they were.
+    const size_t lut_bytes = 256 * sizeof(float), table_bytes = ((sizeof(int4) * (size_t)n_textures + 255) / 256) * 256;
+    if (n_texels > (size_t)INT32_MAX) return ezrt_set_error(EZRT_ERR_INVALID, "scene_set_textures: more than 2^31 texels");
+    std::vector<unsigned char> host;
+    std::vector<float4> rec;
+    try {
+        host.resize(lut_bytes + table_bytes + 4 * n_texels);
+        rec.resize(2 * (size_t)n_tri);
+    } catch (const std::bad_alloc&) {
+        return ezrt_set_error(EZRT_ERR_NOMEM, "scene_set_textures: host staging of %zu texels", n_texels);
+    }
+    memcpy(host.data(), ez_srgb_table, lut_bytes);
+    int4* table = (int4*)(host.data() + lut_bytes);
+    size_t off = 0;
+    for (int k = 0; k < n_textures; k++) {
+        const size_t n = (size_t)textures[k].width * textures[k].height;
+        table[k] = make_int4((int)off, textures[k].width, textures[k].height, 0);
+        memcpy(host.data() + lut_bytes + table_bytes + 4 * off, textures[k].rgba, 4 * n);
+        off += n;
+    }
+    for (int i = 0; i < n_tri; i++) {
+        const float* c = texcoords + 6 * (size_t)i;
+        int32_t id = texture_id[i];
+        float idf;
+        memcpy(&idf, &id, 4);
+        rec[2 * (size_t)i] = make_float4(c[0], c[1], c[2], c[3]);
+        rec[2 * (size_t)i + 1] = make_float4(c[4], c[5], idf, 0.0f);
+    }
+    DeviceBuffer nbuf, nrec;
+    int rc = nbuf.ensure(host.size());
+    if (!rc) rc = nrec.ensure(2 * sizeof(float4) * 2 * (size_t)std::max(n_tri, 1));
+    if (rc) { nbuf.release(); nrec.release(); return rc; }
+    float4* d_rec = (float4*)nrec.p;
+    float4* d_acc = d_rec + 2 * (size_t)n_tri;
+    cudaError_t e = cudaMemcpy(nbuf.p, host.data(), host.size(), cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = cudaMemcpy(d_rec, rec.data(), sizeof(float4) * rec.size(), cudaMemcpyHostToDevice);
+    if (e == cudaSuccess && s->dev.acc_tri_ref && n_tri > 0) {
+        launch_tex_gather(d_rec, s->dev.acc_tri_ref, n_tri, d_acc, 0);
+        e = cudaGetLastError();
+    }
+    if (e == cudaSuccess) e = cudaDeviceSynchronize();   // also: renders already enqueued still read the previous buffers
+    if (e != cudaSuccess) {
+        nbuf.release(); nrec.release();
+        return ezrt_set_error(EZRT_ERR_CUDA, "scene_set_textures: %s", cudaGetErrorString(e));
+    }
+    s->tex_buf.release(); s->tex_rec_buf.release();
+    s->tex_buf = nbuf; s->tex_rec_buf = nrec;   // DeviceBuffer frees only on release(): the pointers move to the scene
+    TexDev t{};
+    t.rec = d_rec;
+    t.acc_rec = d_acc;
+    t.lut = (const float*)s->tex_buf.p;
+    t.table = (const int4*)((const char*)s->tex_buf.p + lut_bytes);
+    t.texels = (const uint32_t*)((const char*)s->tex_buf.p + lut_bytes + table_bytes);
+    s->tex = t;
+    s->has_textures = true;
+    return EZRT_OK;
+}
+
+int ezrt_scene_sample_textures(ezrt_scene* s, int n, const int32_t* tri, const float* points, float* uv_out, float* rgb_out) {
+    if (!s || n < 0 || (n > 0 && (!tri || !points || !uv_out || !rgb_out))) return ezrt_set_error(EZRT_ERR_INVALID, "scene_sample_textures: bad argument");
+    if (!s->has_textures) return ezrt_set_error(EZRT_ERR_INVALID, "scene_sample_textures: no textures (ezrt_scene_set_textures)");
+    for (int i = 0; i < n; i++)
+        if (tri[i] < 0 || tri[i] >= s->dev.n_triangles) return ezrt_set_error(EZRT_ERR_INVALID, "scene_sample_textures: triangle %d out of range", tri[i]);
+    if (n == 0) return EZRT_OK;
+    CU_CHECK(cudaSetDevice(s->device));
+    DeviceBuffer buf;
+    int rc = buf.ensure(sizeof(float) * 9 * (size_t)n + 256);
+    if (rc) return rc;
+    int32_t* d_tri = (int32_t*)buf.p;
+    float* d_p = (float*)(d_tri + n);
+    float* d_uv = d_p + 3 * (size_t)n;
+    float* d_rgb = d_uv + 2 * (size_t)n;
+    cudaError_t e = cudaMemcpy(d_tri, tri, sizeof(int32_t) * (size_t)n, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = cudaMemcpy(d_p, points, sizeof(float) * 3 * (size_t)n, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) {
+        launch_sample_textures(s->dev, s->tex, n, d_tri, d_p, d_uv, d_rgb, 0);
+        e = cudaGetLastError();
+    }
+    if (e == cudaSuccess) e = cudaMemcpy(uv_out, d_uv, sizeof(float) * 2 * (size_t)n, cudaMemcpyDeviceToHost);
+    if (e == cudaSuccess) e = cudaMemcpy(rgb_out, d_rgb, sizeof(float) * 3 * (size_t)n, cudaMemcpyDeviceToHost);
+    buf.release();
+    if (e != cudaSuccess) return ezrt_set_error(EZRT_ERR_CUDA, "scene_sample_textures: %s", cudaGetErrorString(e));
+    return EZRT_OK;
+}
+
 int ezrt_scene_destroy(ezrt_scene* s) {
     if (!s) return EZRT_OK;
     cudaSetDevice(s->device);
@@ -928,7 +1047,7 @@ int ezrt_scene_destroy(ezrt_scene* s) {
     s->lo_buf.release(); s->le_buf.release(); s->counters_buf.release(); s->totals_buf.release(); s->fb_buf.release(); s->sort_buf.release();
     s->adapt_buf.release(); s->adapt_maps_buf.release();
     s->aov_rec_buf.release(); s->aov_maps_buf.release(); s->denoise_buf.release(); s->denoise_io_buf.release();
-    s->lights_buf.release(); s->env_buf.release();
+    s->lights_buf.release(); s->env_buf.release(); s->tex_buf.release(); s->tex_rec_buf.release();
     if (s->own_stream) cudaStreamDestroy(s->own_stream);
     if (s->copy_stream) cudaStreamDestroy(s->copy_stream);
     if (s->side_stream) cudaStreamDestroy(s->side_stream);
@@ -969,6 +1088,11 @@ static int light_options(ezrt_scene* s, const ezrt_render_params* p, cudaStream_
     if ((p->reserved[0] & EZRT_PARAM_MEDIUM) && s->medium.sigma_t > 0.0f) {
         o.med = s->medium;
         o.medium_on = true;
+    }
+    // EZRT_PARAM_TEXTURES (validated: textures are set); tex.sh_base is carved with the shadow queue
+    if (p->reserved[0] & EZRT_PARAM_TEXTURES) {
+        o.tex = s->tex;
+        o.tex_on = true;
     }
     return EZRT_OK;
 }
@@ -1035,7 +1159,7 @@ static int render_device_impl(ezrt_scene* s, const ezrt_render_params* p, float*
     {   // bound the batch by the memory that is actually there (scratch already held by this scene counts as available);
         // asked once per (slots per frame, integrator): cudaMemGetInfo is a driver round trip, the render path is launch-only
         const size_t per_slot = 2 * (sizeof(float4) * 4 + sizeof(float2)) + 2 * sizeof(float4) + sizeof(uint32_t) +
-                                (is_mode ? (size_t)EZRT_SHADOW_SLOT_BYTES : 0) + (s->sort_rays ? 2 * sizeof(uint32_t) : 0) +
+                                (is_mode ? (size_t)EZRT_SHADOW_SLOT_BYTES : 0) + (lopt.tex_on ? sizeof(float4) : 0) + (s->sort_rays ? 2 * sizeof(uint32_t) : 0) +
                                 (av ? 2 * sizeof(float4) : 0);
         if (s->fmax_key[0] != per_frame || s->fmax_key[1] != per_slot) {
             size_t free_b = 0, total_b = 0;
@@ -1061,6 +1185,11 @@ static int render_device_impl(ezrt_scene* s, const ezrt_render_params* p, float*
     if ((rc = carve_shadow(s->shadow_buf, is_mode ? capacity : 1, sq))) return rc;
     if ((rc = s->lo_buf.ensure(sizeof(float4) * capacity))) return rc;
     if ((rc = s->le_buf.ensure(sizeof(float4) * capacity))) return rc;
+    if (lopt.tex_on) {   // the shadow slots' textured base colours, after the 81-byte slots (the plain renders' slots stay as they are)
+        if ((rc = s->shadow_buf.ensure(((size_t)EZRT_SHADOW_SLOT_BYTES + sizeof(float4)) * capacity + 512))) return rc;
+        if ((rc = carve_shadow(s->shadow_buf, capacity, sq))) return rc;
+        lopt.tex.sh_base = (float4*)((((uintptr_t)sq.lit + capacity) + 255) & ~(uintptr_t)255);
+    }
     float4* aov_rec = nullptr;   // feature-buffer render only: the first-hit record of every sample slot
     if (av) {
         if ((rc = s->aov_rec_buf.ensure(2 * sizeof(float4) * capacity))) return rc;

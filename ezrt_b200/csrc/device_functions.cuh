@@ -1939,22 +1939,43 @@ __device__ __forceinline__ void tri_vertices(const SceneDev& sc, int tri, bool a
     }
     p1 = f4xyz(ldg4(v + i1)); p2 = f4xyz(ldg4(v + i2)); p3 = f4xyz(ldg4(v + i3));
 }
+// EZRT_PARAM_TEXTURES (ezrt_math.h, DESIGN.md section 15): the base colour `base` of the hit at P on triangle `tri` (the policy's index
+// space) times its texture's filtered colour at the hit's UV; `base` itself for texture id -1.  One 32-byte texcoord record as two
+// 128-bit loads, the triangle's records again (L1 hits after surface_hit), four texel words and twelve table reads through L1.
+__device__ __forceinline__ vec3 tex_base_color(const SceneDev& sc, const TexDev& tex, int tri, bool accel_space, vec3 P, vec3 base, float* uv_out = nullptr) {
+    const float4* r = (accel_space ? tex.acc_rec : tex.rec) + (size_t)tri * 2;
+    const float4 a = ldg4(r), b = ldg4(r + 1);
+    const int id = __float_as_int(b.z);
+    vec3 p1, p2, p3;
+    tri_vertices(sc, tri, accel_space, p1, p2, p3);
+    const vec3 Ng = f4xyz(ldg4(tri_geo_rec(sc, tri, accel_space)));
+    float w1, w2, w3, u, v;
+    ez_tri_bary(P, p1, p2, p3, Ng, &w1, &w2, &w3);
+    const float uv6[6] = {a.x, a.y, a.z, a.w, b.x, b.y};
+    ez_tex_uv(w1, w2, w3, uv6, &u, &v);
+    if (uv_out) { uv_out[0] = u; uv_out[1] = v; }
+    if (id < 0) return base;
+    const int4 t = __ldg(tex.table + id);
+    return ez_mul(base, ez_tex_sample(tex.texels + t.x, t.y, t.z, u, v, tex.lut));
+}
 
 // A medium vertex (EZRT_PARAM_MEDIUM; ezrt_math.h, DESIGN.md section 14): p's segment scattered at t_s before its hit (hit_t,
 // hit_tri) or its miss.  The weights of the segment (bounce >= 1) and the albedo enter the history; then, below max_bounce, one light
 // sample from P as at a surface but without the hemisphere test and the self exclusion (its shadow ray carries EZRT_MEDIUM_VERTEX
 // and d), and the phase function's sample as the next ray with the record (splat(p), p, 1).  Returns false when the path ends.
-template <bool AOV, bool ENV>
+// TEX: the first-hit record's albedo is the textured base colour.
+template <bool AOV, bool ENV, bool TEX = false>
 __device__ __forceinline__ bool medium_step(const SceneDev& sc, const RenderDev& rd, int bounce, PathRegs& p, float t_s, float hit_t,
                                             int hit_tri, vec3& Lo, vec3& Le, bool& primary_miss, ShadowRay& sh, float4* aov_rec,
-                                            const LightsDev& lights, const EnvDev& env, const MediumDev& med) {
+                                            const LightsDev& lights, const EnvDev& env, const MediumDev& med, const TexDev& tex = TexDev{}) {
     if (bounce == 0) {
         Lo = splat3(0.0f);
         Le = splat3(0.0f);
         primary_miss = hit_tri < 0;   // k_blend: a camera ray that left the scene, its colour the Lo of its medium vertices
         if (AOV && hit_tri >= 0) {    // the feature buffers describe the first surface behind the medium
             const SurfaceHit hit = surface_hit(sc, p.o, p.d, hit_t, hit_tri, false, rd.accel_space != 0);
-            const MaterialDev mat = load_material(sc, hit.matId);
+            MaterialDev mat = load_material(sc, hit.matId);
+            if constexpr (TEX) mat.baseColor = tex_base_color(sc, tex, hit_tri, rd.accel_space != 0, hit.P, mat.baseColor);
             aov_rec[0] = make_float4(mat.baseColor.x, mat.baseColor.y, mat.baseColor.z, hit_t);
             aov_rec[1] = make_float4(hit.N.x, hit.N.y, hit.N.z, 0.0f);
         }
@@ -2032,24 +2053,28 @@ __device__ __forceinline__ bool medium_step(const SceneDev& sc, const RenderDev&
 // surface weighs 1 where it hits an emitter or leaves the scene.  The shadow ray's material id is ~matId for a hit from inside.
 // MEDIUM (light sampling mode with EZRT_PARAM_MEDIUM, ezrt_math.h, DESIGN.md section 14; not with TRANS): the free flight of the
 // traced segment comes first; a path that scatters takes a medium vertex (medium_step) instead of its hit or miss.
-template <int MODE, bool DEFER_NEE = false, bool AOV = false, bool ENV = false, bool TRANS = false, bool MEDIUM = false>
+// TEX (light sampling mode with EZRT_PARAM_TEXTURES, ezrt_math.h, DESIGN.md section 15): every use of the hit's base colour -- the
+// BRDF / mixture's evaluation, sampling and pdf, the first-hit record -- takes the textured one (tex_base_color); a light sample's
+// shadow ray carries it out through *sh_base, for k_nee.
+template <int MODE, bool DEFER_NEE = false, bool AOV = false, bool ENV = false, bool TRANS = false, bool MEDIUM = false, bool TEX = false>
 __device__ __forceinline__ bool shade_step(const SceneDev& sc, const RenderDev& rd, int bounce, PathRegs& p, float hit_t,
                                            int hit_tri, uint32_t px, uint32_t py, float2 sob, vec3& Lo, vec3& Le,
                                            bool& primary_miss, ShadowRay& sh, float4* aov_rec = nullptr, LightsDev lights = LightsDev{},
-                                           EnvDev env = EnvDev{}, MediumDev med = MediumDev{}) {
+                                           EnvDev env = EnvDev{}, MediumDev med = MediumDev{}, TexDev tex = TexDev{}, vec3* sh_base = nullptr) {
     sh.valid = false;
     const int mode = (MODE < 0) ? rd.mode : MODE;
     const bool is_mode = (mode == EZRT_MODE_DISNEY_IS_MIS_P5);
     // the light sampling mode exists only as k_shade<EZRT_MODE_DISNEY_LIGHTS> (the megakernel, MODE < 0, rejects it)
     constexpr bool lights_mode = (MODE == EZRT_MODE_DISNEY_LIGHTS);
     const bool below = TRANS && p.cosine_i < 0.0f;   // the BSDF sample went below the surface: no light strategy reaches it
+    static_assert(lights_mode || !TEX, "textures are rendered in the light sampling mode");
     if constexpr (MEDIUM) {
         static_assert(lights_mode && !TRANS, "the medium is rendered in the light sampling mode, without transmission");
         if (bounce > 0 && p.pdf <= 0.0f) return false;   // P5/fsh:865, before the free flight's draw
         float t_s;
         const float t_end = (hit_tri < 0) ? __int_as_float(0x7f800000) : hit_t;
         if (ez_medium_flight(&med, p.o, p.d, t_end, &p.seed, &t_s))
-            return medium_step<AOV, ENV>(sc, rd, bounce, p, t_s, hit_t, hit_tri, Lo, Le, primary_miss, sh, aov_rec, lights, env, med);
+            return medium_step<AOV, ENV, TEX>(sc, rd, bounce, p, t_s, hit_t, hit_tri, Lo, Le, primary_miss, sh, aov_rec, lights, env, med, tex);
     }
     if (bounce == 0) {
         Lo = splat3(0.0f);
@@ -2081,6 +2106,12 @@ __device__ __forceinline__ bool shade_step(const SceneDev& sc, const RenderDev& 
     const bool fudge = (mode == EZRT_MODE_DIFFUSE_P3 || mode == EZRT_MODE_DISNEY_ANISO_P4);
     SurfaceHit hit = surface_hit(sc, p.o, p.d, hit_t, hit_tri, fudge, rd.accel_space != 0);
     MaterialDev mat = load_material(sc, hit.matId);
+    if constexpr (TEX) {   // not at the last vertex, where only the emission is read
+        if ((AOV && bounce == 0) || bounce < rd.max_bounce) {
+            mat.baseColor = tex_base_color(sc, tex, hit_tri, rd.accel_space != 0, hit.P, mat.baseColor);
+            *sh_base = mat.baseColor;
+        }
+    }
     if (bounce == 0) {
         Le = mat.emissive;  // P5/fsh:936
         if (AOV) {

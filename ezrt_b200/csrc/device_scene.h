@@ -152,6 +152,22 @@ typedef ez_lens LensDev;
 typedef ez_medium MediumDev;
 #define EZRT_MEDIUM_VERTEX (-1)
 
+// The base-colour textures of EZRT_PARAM_TEXTURES (ezrt_math.h, DESIGN.md section 15), set by ezrt_scene_set_textures.  Passed to the
+// textured instantiations (k_shade<.., TEX>, k_nee<.., TEX>) as a parameter of their own, after the others.
+//   rec / acc_rec: 32 bytes per triangle, (u1, v1, u2, v2) (u3, v3, texture id as bits, 0), in reference and in accel order (hit
+//       records hold either index, RenderDev::accel_space)
+//   table: per texture (offset of its first texel in texels, W, H, 0); texels: RGBA8 words; lut: ez_srgb_table, read through L1
+//   sh_base: the textured base colour of every shadow slot's shading point (16 B per slot, carved beside the shadow queue for the
+//       flagged renders only), read back by k_nee, which reloads the material from its id
+struct TexDev {
+    const float4* rec;
+    const float4* acc_rec;
+    const int4* table;
+    const uint32_t* texels;
+    const float* lut;
+    float4* sh_base;
+};
+
 // A shadow ray and what k_nee needs to evaluate the light sample's contribution once the ray got through (nee_contrib):
 // the BRDF / environment evaluation of the light sample is done after the shadow pass, for unoccluded rays only.
 #define EZRT_SHADOW_SLOT_BYTES (5 * 16 + 1)

@@ -34,6 +34,10 @@ struct Tri {
     ez_vec3 p1, p2, p3;
     ez_vec3 n1, n2, n3;
     float material[EZRT_MATERIAL_FLOATS];
+    // base-colour texture (ezrt_trilist_read_obj_textured): (u1, v1, u2, v2, u3, v3) and the texture id, -1 = untextured.  Carried
+    // through every builder: the builders' permutations depend only on comparison outcomes, never on these
+    float uv[6] = {0.0f, 0.0f, 0.0f, 0.0f, 0.0f, 0.0f};
+    int32_t tex_id = -1;
 };
 struct Node {
     int left, right, n, index;
@@ -186,10 +190,14 @@ Mat4 mat_look_at(ez_vec3 eye, ez_vec3 center, ez_vec3 up) {
 // ------------------------------------------------------------------------------------------
 // readObj, P5/main.cpp:274-392
 // ------------------------------------------------------------------------------------------
+// textured (ezrt_trilist_read_obj_textured): also the "vt u v [w]" lines and each face vertex's vt index; a triangle whose three
+// vertices all carry one gets (its UVs, texture_id), any other -1.  Positions, normals and materials are read_obj's.
 int read_obj_stream(std::istream& fin, std::vector<Tri>& triangles, const float material[EZRT_MATERIAL_FLOATS],
-                    const Mat4& trans, bool smoothNormal, bool hardened = false) {
+                    const Mat4& trans, bool smoothNormal, bool hardened = false, bool textured = false, int texture_id = -1) {
     std::vector<ez_vec3> vertices;
     std::vector<unsigned> indices;
+    std::vector<float> texcoords;   // textured: 2 floats per vt line
+    std::vector<int> tri_vt;        // textured: 3 vt indices (0-based) per triangle, or -1 when a vertex has none
 
     float maxx = -11451419.19f, maxy = -11451419.19f, maxz = -11451419.19f;
     float minx = 11451419.19f, miny = 11451419.19f, minz = 11451419.19f;
@@ -207,32 +215,56 @@ int read_obj_stream(std::istream& fin, std::vector<Tri>& triangles, const float 
             maxx = ez_max(maxx, x); maxy = ez_max(maxx, y); maxz = ez_max(maxx, z);
             minx = ez_min(minx, x); miny = ez_min(minx, y); minz = ez_min(minx, z);
         }
+        if (textured && type == "vt") {   // a third component is ignored
+            float u = 0, v = 0;
+            sin >> u >> v;
+            texcoords.push_back(u);
+            texcoords.push_back(v);
+        }
         if (type == "f") {
             // "v", "v/vt", "v/vt/vn" (and, hardened, "v//vn"): the leading integer of each
             // of the first three vertex tokens; extra vertices are ignored as in the reference.
             // Hardened mode (EZRT_OBJ_HARDENED): negative (relative) indices, and polygons are
             // triangulated as a fan instead of being cut to their first three vertices.
-            std::vector<int> fv;
+            std::vector<int> fv, fvt;
             std::string tok;
             while (sin >> tok) {
-                int idx = (int)std::strtol(tok.c_str(), nullptr, 10);
+                char* end = nullptr;
+                int idx = (int)std::strtol(tok.c_str(), &end, 10);
                 if (hardened && idx < 0) idx = (int)vertices.size() + 1 + idx;
                 fv.push_back(idx);
+                if (textured) {   // "v/vt[/vn]": the integer after the first '/', if any (0 = none)
+                    int vt = 0;
+                    if (*end == '/' && end[1] != '/' && end[1] != '\0') {
+                        vt = (int)std::strtol(end + 1, nullptr, 10);
+                        if (hardened && vt < 0) vt = (int)(texcoords.size() / 2) + 1 + vt;
+                        if (vt < 1) return EZRT_ERR_IO;
+                    }
+                    fvt.push_back(vt);
+                }
                 if (!hardened && fv.size() == 3) break;
             }
             if (fv.size() < 3) return EZRT_ERR_IO;
             for (int idx : fv)
                 if (idx < 1) return EZRT_ERR_IO;   // upper bound: after the whole file is read (a face may precede its vertices)
+            const bool face_vt = textured && std::find(fvt.begin(), fvt.end(), 0) == fvt.end();
             for (size_t k = 2; k < fv.size(); k++) {
                 indices.push_back((unsigned)(fv[0] - 1));
                 indices.push_back((unsigned)(fv[k - 1] - 1));
                 indices.push_back((unsigned)(fv[k] - 1));
+                if (textured) {
+                    tri_vt.push_back(face_vt ? fvt[0] - 1 : -1);
+                    tri_vt.push_back(face_vt ? fvt[k - 1] - 1 : -1);
+                    tri_vt.push_back(face_vt ? fvt[k] - 1 : -1);
+                }
             }
         }
     }
 
     for (unsigned idx : indices)   // the reference resolves indices after reading the whole file (P5/main.cpp:344-362)
         if ((size_t)idx >= vertices.size()) return EZRT_ERR_IO;
+    for (int vt : tri_vt)
+        if (vt >= 0 && (size_t)vt >= texcoords.size() / 2) return EZRT_ERR_IO;
 
     float lenx = maxx - minx, leny = maxy - miny, lenz = maxz - minz;
     float maxaxis = ez_max(lenx, ez_max(leny, lenz));
@@ -270,6 +302,13 @@ int read_obj_stream(std::istream& fin, std::vector<Tri>& triangles, const float 
             t.n3 = ez_normalize(normals[indices[i + 2]]);
         }
         memcpy(t.material, material, sizeof(t.material));
+        if (textured && tri_vt[i] >= 0) {
+            for (int c = 0; c < 3; c++) {
+                t.uv[2 * c] = texcoords[2 * (size_t)tri_vt[i + c]];
+                t.uv[2 * c + 1] = texcoords[2 * (size_t)tri_vt[i + c] + 1];
+            }
+            t.tex_id = texture_id;
+        }
     }
     return EZRT_OK;
 }
@@ -681,6 +720,38 @@ int ezrt_trilist_read_obj_text(ezrt_trilist* list, const char* text, size_t len,
     memcpy(m.c, trans, sizeof(float) * 16);
     int rc = read_obj_stream(fin, list->tris, material, m, (smooth_normal & 1) != 0, (smooth_normal & EZRT_OBJ_HARDENED) != 0);
     if (rc) return ezrt_set_error(rc, "read_obj_text: malformed face");
+    return EZRT_OK;
+}
+
+int ezrt_trilist_read_obj_textured(ezrt_trilist* list, const char* path, const float material[EZRT_MATERIAL_FLOATS],
+                                   const float trans[16], int smooth_normal, int32_t texture_id) {
+    if (!list || !path || !material || !trans || texture_id < -1) return ezrt_set_error(EZRT_ERR_INVALID, "read_obj_textured: bad argument");
+    std::ifstream fin(path);
+    if (!fin.is_open()) return ezrt_set_error(EZRT_ERR_IO, "read_obj_textured: cannot open %s", path);
+    Mat4 m;
+    memcpy(m.c, trans, sizeof(float) * 16);
+    int rc = read_obj_stream(fin, list->tris, material, m, (smooth_normal & 1) != 0, (smooth_normal & EZRT_OBJ_HARDENED) != 0, true, texture_id);
+    if (rc) return ezrt_set_error(rc, "read_obj_textured: malformed face or texture index in %s", path);
+    return EZRT_OK;
+}
+
+int ezrt_trilist_read_obj_textured_text(ezrt_trilist* list, const char* text, size_t len, const float material[EZRT_MATERIAL_FLOATS],
+                                        const float trans[16], int smooth_normal, int32_t texture_id) {
+    if (!list || !text || !material || !trans || texture_id < -1) return ezrt_set_error(EZRT_ERR_INVALID, "read_obj_textured_text: bad argument");
+    std::istringstream fin(std::string(text, len));
+    Mat4 m;
+    memcpy(m.c, trans, sizeof(float) * 16);
+    int rc = read_obj_stream(fin, list->tris, material, m, (smooth_normal & 1) != 0, (smooth_normal & EZRT_OBJ_HARDENED) != 0, true, texture_id);
+    if (rc) return ezrt_set_error(rc, "read_obj_textured_text: malformed face or texture index");
+    return EZRT_OK;
+}
+
+int ezrt_trilist_encode_texcoords(const ezrt_trilist* list, float* uv_out, int32_t* id_out) {
+    if (!list || !uv_out || !id_out) return ezrt_set_error(EZRT_ERR_INVALID, "encode_texcoords: null argument");
+    for (size_t i = 0; i < list->tris.size(); i++) {
+        memcpy(uv_out + 6 * i, list->tris[i].uv, sizeof(float) * 6);
+        id_out[i] = list->tris[i].tex_id;
+    }
     return EZRT_OK;
 }
 

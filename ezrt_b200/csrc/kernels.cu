@@ -547,13 +547,15 @@ __global__ void __launch_bounds__(EZRT_EXTEND_MAX_THREADS, EZRT_EXTEND_LB_BLOCKS
 // ENV (light sampling mode with EZRT_PARAM_ENV_LIGHT): the map is one more light, sampled from the table env (shade_step).
 // TRANS (light sampling mode with EZRT_PARAM_TRANSMISSION): materials with a dielectric lobe (shade_step).
 // MEDIUM (light sampling mode with EZRT_PARAM_MEDIUM): the homogeneous medium med (shade_step, medium_step).
-template <int MODE, bool LIST, bool AOV = false, bool ENV = false, bool TRANS = false, bool MEDIUM = false>
+// TEX (light sampling mode with EZRT_PARAM_TEXTURES): the base-colour textures tex (shade_step); every shadow slot also gets its
+// shading point's textured base colour, tex.sh_base[spos].
+template <int MODE, bool LIST, bool AOV = false, bool ENV = false, bool TRANS = false, bool MEDIUM = false, bool TEX = false>
 __global__ void __launch_bounds__(128, EZRT_SHADE_MIN_BLOCKS) k_shade(SceneDev sc, RenderDev rd, const TileDev* __restrict__ tiles, int bounce,
                                                uint32_t batch_first_frame, PathQueue qin, const uint32_t* __restrict__ in_count,
                                                PathQueue qout, uint32_t* out_count, ShadowQueue sq, uint32_t* s_count,
                                                float4* __restrict__ Lo, float4* __restrict__ Le, uint32_t n_fused, uint32_t n_frames,
                                                const uint32_t* __restrict__ list, const float2* __restrict__ side_hit,
-                                               float4* __restrict__ aov_rec, LightsDev lights, EnvDev env, MediumDev med) {
+                                               float4* __restrict__ aov_rec, LightsDev lights, EnvDev env, MediumDev med, TexDev tex) {
     // The Sobol pair of (bounce, frame) is the same for every pixel of a frame (P5/fsh:361-376: up to 2 x 32 table XORs per path): each
     // block computes the pairs of the batch's frames once into shared memory (batches of more than EZRT_SOBOL_TABLE frames compute per path).
     __shared__ float2 s_sobol[EZRT_SOBOL_TABLE];
@@ -590,6 +592,7 @@ __global__ void __launch_bounds__(128, EZRT_SHADE_MIN_BLOCKS) k_shade(SceneDev s
         PathRegs p;
         ShadowRay sh;
         sh.valid = false;
+        vec3 sh_base;   // TEX: the shading point's textured base colour
         uint32_t slot = 0;
         uint32_t px = 0, py = 0, fib = 0;
         bool present = i < n;
@@ -677,9 +680,9 @@ __global__ void __launch_bounds__(128, EZRT_SHADE_MIN_BLOCKS) k_shade(SceneDev s
             }
 #endif
             if (LIST || __float_as_int(hit.y) != EZRT_TRI_PENDING) {   // pending: deferred by the accel kernel, shaded by the LIST pass
-                alive = shade_step<MODE, MODE == EZRT_MODE_DISNEY_IS_MIS_P5, AOV, ENV, TRANS, MEDIUM>(sc, rd, bounce, p, hit.x, __float_as_int(hit.y), px, py, sob,
-                                                                                                     lo, le, pmiss, sh, AOV ? aov_rec + 2 * (size_t)slot : nullptr,
-                                                                                                     lights, env, med);
+                alive = shade_step<MODE, MODE == EZRT_MODE_DISNEY_IS_MIS_P5, AOV, ENV, TRANS, MEDIUM, TEX>(sc, rd, bounce, p, hit.x, __float_as_int(hit.y), px, py,
+                                                                                                          sob, lo, le, pmiss, sh, AOV ? aov_rec + 2 * (size_t)slot : nullptr,
+                                                                                                          lights, env, med, tex, &sh_base);
                 if (bounce == 0) {
                     // Le is zero for every surface that does not emit: it is stored (and read back by k_blend) only otherwise.
                     // color = Le + Lo with Le = +-0 is Lo bit for bit, because Lo is never -0.0 (it starts at +0.0 and only grows by additions)
@@ -708,6 +711,9 @@ __global__ void __launch_bounds__(128, EZRT_SHADE_MIN_BLOCKS) k_shade(SceneDev s
                 __stcs(sq.nrm + spos, make_float4(sh.N.x, sh.N.y, sh.N.z, LT ? sh.tmax : 0.0f));
                 __stcs(sq.view + spos, make_float4(sh.V.x, sh.V.y, sh.V.z, LT ? sh.pdf : 0.0f));
                 __stcs(sq.hist + spos, make_float4(sh.history.x, sh.history.y, sh.history.z, LT ? __int_as_float(sh.light_mat) : 0.0f));
+                if constexpr (TEX) {   // a medium vertex's slot has no shading point: its entry is never read
+                    if (sh.matId != EZRT_MEDIUM_VERTEX || !MEDIUM) __stcs(tex.sh_base + spos, make_float4(sh_base.x, sh_base.y, sh_base.z, 0.0f));
+                }
             }
         }
     }
@@ -724,9 +730,10 @@ __global__ void __launch_bounds__(128, EZRT_SHADE_MIN_BLOCKS) k_shade(SceneDev s
 // TRANS: evaluated with the mixture of the shading point's material (nee_trans_contrib); ray_d.w = ~matId for a hit from inside.
 // MEDIUM: every contribution times the shadow ray's transmittance through the medium med; a medium vertex's (ray_d.w =
 // EZRT_MEDIUM_VERTEX, view = d) is evaluated with the phase function (nee_medium_contrib).
-template <int MODE, bool ENV = false, bool TRANS = false, bool MEDIUM = false>
+// TEX: the shading point's material with the textured base colour k_shade left in tex.sh_base[j].
+template <int MODE, bool ENV = false, bool TRANS = false, bool MEDIUM = false, bool TEX = false>
 __global__ void __launch_bounds__(128, 8) k_nee(SceneDev sc, RenderDev rd, ShadowQueue sq, const uint32_t* __restrict__ s_count, float4* __restrict__ Lo,
-                                                MediumDev med) {
+                                                MediumDev med, TexDev tex) {
     static_assert(MODE == EZRT_MODE_DISNEY_LIGHTS || !(ENV || TRANS || MEDIUM), "the options exist in the light sampling mode");
     static_assert(!(TRANS && MEDIUM), "the medium is rendered without transmission");
     __shared__ uint32_t s_scan[34];
@@ -750,6 +757,11 @@ __global__ void __launch_bounds__(128, 8) k_nee(SceneDev sc, RenderDev rd, Shado
             const float4 o4 = __ldcs(sq.ray_o + j), d4 = __ldcs(sq.ray_d + j), n4 = __ldcs(sq.nrm + j), v4 = __ldcs(sq.view + j), h4 = __ldcs(sq.hist + j);
             const uint32_t slot = __float_as_uint(o4.w);
             const int m_raw = __float_as_int(d4.w);
+            const auto material = [&](int m_id) {
+                MaterialDev m = load_material(sc, m_id);
+                if constexpr (TEX) m.baseColor = f4xyz(__ldcs(tex.sh_base + j));
+                return m;
+            };
             const vec3 V = ez_v3(v4.x, v4.y, v4.z), N = ez_v3(n4.x, n4.y, n4.z), Ld = ez_v3(d4.x, d4.y, d4.z), hist = ez_v3(h4.x, h4.y, h4.z);
             vec3 c;
             if constexpr (MODE == EZRT_MODE_DISNEY_LIGHTS) {
@@ -758,11 +770,11 @@ __global__ void __launch_bounds__(128, 8) k_nee(SceneDev sc, RenderDev rd, Shado
                 if constexpr (MEDIUM) {   // a medium vertex loads no material
                     const vec3 E = light_color();
                     if (m_raw == EZRT_MEDIUM_VERTEX) c = nee_medium_contrib(V, Ld, med.g, hist, E, v4.w);
-                    else c = nee_light_contrib(V, N, Ld, load_material(sc, m_raw), hist, E, v4.w);
+                    else c = nee_light_contrib(V, N, Ld, material(m_raw), hist, E, v4.w);
                     c = ez_scale(c, ez_medium_transmittance(&med, ez_v3(o4.x, o4.y, o4.z), Ld, ez_medium_light_dist(n4.w, ENV && lm < 0)));
                 } else {
                     const int m_id = (TRANS && m_raw < 0) ? ~m_raw : m_raw;
-                    const MaterialDev mat = load_material(sc, m_id);
+                    const MaterialDev mat = material(m_id);
                     if constexpr (TRANS) c = nee_trans_contrib(sc, V, N, Ld, m_id, mat, m_raw < 0, hist, light_color(), v4.w);
                     else c = nee_light_contrib(V, N, Ld, mat, hist, light_color(), v4.w);
                 }
@@ -1345,11 +1357,12 @@ static void launch_shade_t(int blocks, const SceneDev& sc, const RenderDev& rd, 
                            float4* Lo, float4* Le, uint32_t n_fused, uint32_t n_frames, const uint32_t* list, const float2* side_hit,
                            float4* aov_rec, const LightOptions& o, cudaStream_t st) {
     auto launch = [&](auto M) {
-        with_bools([&](auto A, auto E, auto T, auto X) {
-            if constexpr ((M == EZRT_MODE_DISNEY_LIGHTS || !(E || T || X)) && !(T && X))   // the options exist in the light sampling mode
-                k_shade<M, LIST, A, E, T, X><<<blocks, 128, 0, st>>>(sc, rd, tiles, bounce, batch_first_frame, qin, in_count, qout, out_count, sq,
-                                                                     s_count, Lo, Le, n_fused, n_frames, list, side_hit, aov_rec, o.lights, o.env, o.med);
-        }, aov_rec != nullptr, o.env_on, o.trans_on, o.medium_on);
+        with_bools([&](auto A, auto E, auto T, auto X, auto TX) {
+            if constexpr ((M == EZRT_MODE_DISNEY_LIGHTS || !(E || T || X || TX)) && !(T && X))   // the options exist in the light sampling mode
+                k_shade<M, LIST, A, E, T, X, TX><<<blocks, 128, 0, st>>>(sc, rd, tiles, bounce, batch_first_frame, qin, in_count, qout, out_count, sq,
+                                                                         s_count, Lo, Le, n_fused, n_frames, list, side_hit, aov_rec, o.lights, o.env, o.med,
+                                                                         o.tex);
+        }, aov_rec != nullptr, o.env_on, o.trans_on, o.medium_on, o.tex_on);
     };
     switch (rd.mode) {
         case EZRT_MODE_DIFFUSE_P3: launch(std::integral_constant<int, EZRT_MODE_DIFFUSE_P3>{}); break;
@@ -1381,10 +1394,10 @@ void launch_deferred_lane(const SceneDev& sc, const RenderDev& rd, const TileDev
 void launch_nee(const SceneDev& sc, const RenderDev& rd, ShadowQueue sq, const uint32_t* s_count, float4* Lo, uint32_t n_max, int n_sms, cudaStream_t st,
                 const LightOptions& o) {
     const int blocks = std::max(1, std::min(div_up(n_max, 512), n_sms * 8));
-    with_bools([&](auto L, auto E, auto T, auto X) {
-        if constexpr ((L || !(E || T || X)) && !(T && X))   // the options exist in the light sampling mode; the other mode here is mode 3
-            k_nee<L ? EZRT_MODE_DISNEY_LIGHTS : EZRT_MODE_DISNEY_IS_MIS_P5, E, T, X><<<blocks, 128, 0, st>>>(sc, rd, sq, s_count, Lo, o.med);
-    }, rd.mode == EZRT_MODE_DISNEY_LIGHTS, o.env_on, o.trans_on, o.medium_on);
+    with_bools([&](auto L, auto E, auto T, auto X, auto TX) {
+        if constexpr ((L || !(E || T || X || TX)) && !(T && X))   // the options exist in the light sampling mode; the other mode here is mode 3
+            k_nee<L ? EZRT_MODE_DISNEY_LIGHTS : EZRT_MODE_DISNEY_IS_MIS_P5, E, T, X, TX><<<blocks, 128, 0, st>>>(sc, rd, sq, s_count, Lo, o.med, o.tex);
+    }, rd.mode == EZRT_MODE_DISNEY_LIGHTS, o.env_on, o.trans_on, o.medium_on, o.tex_on);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -1492,6 +1505,30 @@ void launch_eval_brdf(int which, int n, const float* V, const float* N, const fl
 void launch_eval_bsdf(int which, int n, const float* V, const float* N, const float* L, const float* xi, const int* inside,
                       const float* materials, float* out, cudaStream_t st) {
     k_eval_bsdf<<<div_up(n, 128), 128, 0, st>>>(which, n, V, N, L, xi, inside, materials, out);
+}
+__global__ void k_tex_gather(const float4* __restrict__ rec, const uint32_t* __restrict__ acc_tri_ref, int n, float4* __restrict__ acc_rec) {
+    const int a = blockIdx.x * blockDim.x + threadIdx.x;
+    if (a >= n) return;
+    const uint32_t r = acc_tri_ref[a];
+    acc_rec[2 * (size_t)a] = rec[2 * (size_t)r];
+    acc_rec[2 * (size_t)a + 1] = rec[2 * (size_t)r + 1];
+}
+void launch_tex_gather(const float4* rec, const uint32_t* acc_tri_ref, int n, float4* acc_rec, cudaStream_t st) {
+    k_tex_gather<<<div_up(n, 256), 256, 0, st>>>(rec, acc_tri_ref, n, acc_rec);
+}
+// the textured base colour of the hits shade_step<.., TEX> computes, at the points of reference triangles (ezrt_scene_sample_textures)
+__global__ void k_sample_textures(SceneDev sc, TexDev tex, int n, const int32_t* __restrict__ tri, const float* __restrict__ points,
+                                  float* __restrict__ uv, float* __restrict__ rgb) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const int t = tri[i];
+    const vec3 P = ez_v3(points[3 * i], points[3 * i + 1], points[3 * i + 2]);
+    const vec3 c = tex_base_color(sc, tex, t, false, P, load_material(sc, tri_material(sc, t)).baseColor, uv + 2 * (size_t)i);
+    rgb[3 * i] = c.x; rgb[3 * i + 1] = c.y; rgb[3 * i + 2] = c.z;
+}
+void launch_sample_textures(const SceneDev& sc, const TexDev& tex, int n, const int32_t* tri, const float* points, float* uv, float* rgb,
+                            cudaStream_t st) {
+    k_sample_textures<<<div_up(n, 128), 128, 0, st>>>(sc, tex, n, tri, points, uv, rgb);
 }
 void launch_eval_math(int which, int n, const float* a, const float* b, float* out, cudaStream_t st) {
     k_eval_math<<<div_up(n, 256), 256, 0, st>>>(which, n, a, b, out);

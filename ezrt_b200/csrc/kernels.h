@@ -21,12 +21,14 @@
 //   env_on    EZRT_PARAM_ENV_LIGHT and the scene has an environment table: the map is one more light (<.., ENV>)
 //   trans_on  EZRT_PARAM_TRANSMISSION: materials with a dielectric lobe (<.., TRANS>)
 //   medium_on EZRT_PARAM_MEDIUM with sigma_t > 0: the homogeneous medium med (<.., MEDIUM>); never with trans_on
+//   tex_on    EZRT_PARAM_TEXTURES: the scene's base-colour textures tex (<.., TEX>)
 // All off outside the light sampling mode; the tables are zero where unused, as the kernels' parameters.
 struct LightOptions {
     LightsDev lights{};   // the light table (light sampling mode)
     EnvDev env{};         // the environment table (env_on)
     MediumDev med{};      // the medium (medium_on)
-    bool env_on = false, trans_on = false, medium_on = false;
+    TexDev tex{};         // the textures and the shadow slots' base colours (tex_on)
+    bool env_on = false, trans_on = false, medium_on = false, tex_on = false;
 };
 
 // lens (EZRT_PARAM_THIN_LENS): the thin-lens camera rays (k_generate<true>); null: the pinhole's
@@ -99,6 +101,11 @@ void launch_eval_brdf(int which, int n, const float* V, const float* N, const fl
 // the transmission mixture for ezrt_eval_bsdf (8 floats out per tuple)
 void launch_eval_bsdf(int which, int n, const float* V, const float* N, const float* L, const float* xi, const int* inside,
                       const float* materials, float* out, cudaStream_t st);
+// the texcoord records of the accel order: acc_rec[a] = rec[acc_tri_ref[a]] (2 float4 each, n triangles)
+void launch_tex_gather(const float4* rec, const uint32_t* acc_tri_ref, int n, float4* acc_rec, cudaStream_t st);
+// ezrt_scene_sample_textures: n (reference triangle, point) pairs -> uv (2 floats) and the textured base colour (3 floats) each
+void launch_sample_textures(const SceneDev& sc, const TexDev& tex, int n, const int32_t* tri, const float* points, float* uv, float* rgb,
+                            cudaStream_t st);
 void launch_eval_math(int which, int n, const float* a, const float* b, float* out, cudaStream_t st);
 void launch_tonemap(const float* in, int channels, float* out, long long n, float limit, cudaStream_t st);
 void launch_partition_scatter(const float* compact, float* full, const TileDev* tiles, int n_tiles, int width, int channels,

@@ -269,3 +269,85 @@ def synth_hdr(width=512, height=256, seed=3, n_lamps=16):
         img[:, :, 1] += lamp * 0.9
         img[:, :, 2] += lamp * 0.7
     return img.astype(np.float32)
+
+
+def procedural_textures(n=2, seed=11):
+    """n seeded sRGB textures for EZRT_PARAM_TEXTURES, uint8 [H, W, 3] each: even indices an 8x8 checker of two colours (256 x 256),
+    odd indices bilinear value noise on a 16x16 lattice (128 x 192)."""
+    out = []
+    for k in range(n):
+        h, w = (256, 256) if k % 2 == 0 else (128, 192)
+        r = _unit_randoms(seed * 7919 + k, 6 + 17 * 17 * 3)
+        ys, xs = np.meshgrid(np.arange(h), np.arange(w), indexing="ij")
+        if k % 2 == 0:
+            c0, c1 = np.array(r[0:3]) * 255.0, np.array(r[3:6]) * 255.0
+            on = ((ys * 8 // h) + (xs * 8 // w)) % 2 == 1
+            img = np.where(on[:, :, None], c1, c0)
+        else:
+            lat = np.array(r[6:]).reshape(17, 17, 3)
+            fy, fx = ys * 16.0 / h, xs * 16.0 / w
+            iy, ix = fy.astype(int), fx.astype(int)
+            ty, tx = (fy - iy)[:, :, None], (fx - ix)[:, :, None]
+            a = lat[iy, ix] * (1 - tx) + lat[iy, ix + 1] * tx
+            b = lat[iy + 1, ix] * (1 - tx) + lat[iy + 1, ix + 1] * tx
+            img = (a * (1 - ty) + b * ty) * 255.0
+        out.append(np.clip(np.rint(img), 0, 255).astype(np.uint8))
+    return out
+
+
+
+def obj_with_vt(text, projection):
+    """OBJ text with a vt line per vertex and every face as "f a/a b/b c/c": projection "spherical" (u = 2 x longitude, v = latitude
+    about the mesh's bounding-box centre) or "planar" (u, v = x, z over the mesh's extent, 8 repeats)."""
+    lines = text.splitlines()
+    v = np.array([[float(x) for x in l.split()[1:4]] for l in lines if l.startswith("v ")], np.float64)
+    lo, hi = v.min(0), v.max(0)
+    d = v - (lo + hi) / 2
+    if projection == "spherical":
+        u = np.arctan2(d[:, 2], d[:, 0]) / np.pi + 1.0
+        w = np.arcsin(np.clip(d[:, 1] / np.maximum(np.linalg.norm(d, axis=1), 1e-12), -1, 1)) / np.pi + 0.5
+    else:
+        ext = np.maximum(hi - lo, 1e-12)
+        u, w = 8.0 * (v[:, 0] - lo[0]) / ext[0], 8.0 * (v[:, 2] - lo[2]) / ext[2]
+    out = [l for l in lines if l.startswith("v ")] + ["vt %.9g %.9g" % (a, b) for a, b in zip(u, w)]
+    for l in lines:
+        if l.startswith("f "):
+            out.append("f " + " ".join("%s/%s" % (t, t) for t in l.split()[1:]))
+    return "\n".join(out) + "\n"
+
+
+def _textured_list(meshes, n_textures):
+    """meshes of p3_bunny_meshes / grid_meshes read as textured OBJ text: emissive meshes untextured, flat boxes planar with the last
+    texture id, the other meshes spherical with ids cycling over the others"""
+    tl = TriangleList()
+    k = 0
+    for text, m, trans, smooth in meshes:
+        if any(c > 0 for c in m.emissive):
+            tl.read_obj_text(text, m, trans, smooth)
+        elif text == box_obj():
+            tl.read_obj_text(obj_with_vt(text, "planar"), m, trans, smooth, texture_id=n_textures - 1)
+        else:
+            tl.read_obj_text(obj_with_vt(text, "spherical"), m, trans, smooth, texture_id=k % max(1, n_textures - 1))
+            k += 1
+    return tl
+
+
+def s_p3_bunny_textured(n_textures=2, builder=api.BVH_SAH_FAST):
+    """s_p3_bunny with texture coordinates read from OBJ vt lines (the bunny spherical, the floor planar, the light untextured) and
+    seeded procedural textures.  Returns (tris, nodes, eye, cam, textures, texcoords [N, 3, 2], texture_id [N]); the geometry is
+    s_p3_bunny's byte for byte."""
+    tl = _textured_list(p3_bunny_meshes(), n_textures)
+    tris, nodes = tl.build_bvh(8, builder)
+    uv, ids = tl.encode_texcoords()
+    eye, cam = api.camera_orbit(0.0, 0.0, 4.0)
+    return tris, nodes, eye, cam, procedural_textures(n_textures), uv, ids
+
+
+def s_1m_bunny_textured(n_textures=2, builder=api.BVH_SAH_FAST):
+    """s_1m_bunny with texture coordinates read from OBJ vt lines, as s_p3_bunny_textured (the bunnies' ids cycle over all textures
+    but the last, the floor's)."""
+    tl = _textured_list(grid_meshes(15, 14, 4, 1.2, "bunny", 201), n_textures)
+    tris, nodes = tl.build_bvh(8, builder)
+    uv, ids = tl.encode_texcoords()
+    eye, cam = api.camera_orbit(30.0, 25.0, 0.62 * max(15 * 1.2, 14 * 1.2) + 3.0)
+    return tris, nodes, eye, cam, procedural_textures(n_textures), uv, ids

@@ -149,6 +149,23 @@ typedef struct ezrt_render_params {
    EZRT_PARAM_TRANSMISSION (glass is defined with vacuum outside; a medium around it would need a medium stack).  Accepted by
    ezrt_render[_device], ezrt_render_adaptive[_device] and ezrt_render_aov[_device]. */
 #define EZRT_PARAM_MEDIUM 16
+/* ezrt_render_params.reserved[0], EZRT_MODE_DISNEY_LIGHTS on the wavefront pipeline only, with or without EZRT_PARAM_ENV_LIGHT,
+   EZRT_PARAM_TRANSMISSION, EZRT_PARAM_THIN_LENS and EZRT_PARAM_MEDIUM: the scene's base-colour textures (ezrt_scene_set_textures)
+   are rendered.  Wherever the render reads the base colour of a surface hit -- the BRDF and the transmission mixture (evaluation,
+   sampling, pdf), the light samples evaluated after the shadow pass, the feature buffers' albedo -- it uses the material's baseColor
+   times the filtered linear colour of the triangle's texture at the hit's UV: barycentrics on the triangle's dominant plane, wrap
+   addressing, RGBA8 texels decoded by the sRGB EOTF (alpha ignored), bilinear filtering (ezrt_math.h, DESIGN.md section 15).
+   Emission is not textured, and no random number is drawn, so a render whose textures are all 1x1 white is the unflagged render's
+   bit for bit.  Invalid (EZRT_ERR_INVALID) without textures set on the scene and in another mode.  Accepted by ezrt_render[_device],
+   ezrt_render_adaptive[_device] and ezrt_render_aov[_device]; each shadow slot of a flagged render takes 16 bytes more. */
+#define EZRT_PARAM_TEXTURES 32
+
+/* One texture of ezrt_scene_set_textures: width x height RGBA8 texels (4 bytes each, R first), row 0 the image's top row */
+typedef struct ezrt_texture {
+    int32_t width, height;   /* each in [1, 16384] */
+    const uint8_t* rgba;     /* width * height * 4 bytes, sRGB-encoded colour; alpha is ignored */
+    int32_t reserved;        /* 0 */
+} ezrt_texture;
 
 /* The homogeneous medium of EZRT_PARAM_MEDIUM: a grey extinction, an RGB single-scattering albedo and a Henyey-Greenstein
    asymmetry g (> 0: forward scattering), filling the axis-aligned box [box_min, box_max] (a box of zero extent on an axis holds
@@ -201,6 +218,18 @@ int ezrt_scene_destroy(ezrt_scene* scene);
  * box corner, box_min > box_max on an axis, or reserved != 0.  The medium travels to the kernels by value when a render is
  * enqueued: changing it afterwards does not affect renders already enqueued. */
 int ezrt_scene_set_medium(ezrt_scene* scene, const ezrt_medium* medium);
+/* Sets the scene's base-colour textures (EZRT_PARAM_TEXTURES): n_textures textures (copied), and per triangle, in the order of the
+ * `tris` array given to ezrt_scene_create, 6 floats of texcoords (u1, v1, u2, v2, u3, v3: OBJ's convention, v = 0 at the image's
+ * bottom) and a texture id in [-1, n_textures) (-1: the material's base colour).  textures NULL clears them.  Returns
+ * EZRT_ERR_INVALID for a side outside [1, 16384], a null rgba, reserved != 0, an id out of range, more than 2^31 texels, or
+ * n_textures < 1 with textures set; EZRT_ERR_NOMEM / EZRT_ERR_CUDA when the copies cannot be made.  On every error the previous
+ * textures are kept.  The call first waits for every render already enqueued on the scene's device (it frees the
+ * previous buffers those renders read), then uploads synchronously. */
+int ezrt_scene_set_textures(ezrt_scene* scene, int n_textures, const ezrt_texture* textures, const float* texcoords, const int32_t* texture_id);
+/* The textured base colour the kernels compute at n hit points: points[3 i..] on reference triangle tri[i] -> uv_out[2 i..] (the
+ * interpolated UV) and rgb_out[3 i..] (the material's baseColor times the filtered texture; baseColor for texture id -1).  Host
+ * arrays; synchronous.  EZRT_ERR_INVALID without textures set or for a triangle index out of range. */
+int ezrt_scene_sample_textures(ezrt_scene* scene, int n, const int32_t* tri, const float* points, float* uv_out, float* rgb_out);
 
 /* render(width,height,spp) -> framebuffer: equals `spp` consecutive display() calls
  * (P5/main.cpp:697-748) each drawing pass1 (P5/fsh:894-949) and copying to lastFrame.
@@ -409,8 +438,19 @@ int ezrt_trilist_read_obj(ezrt_trilist* list, const char* path, const float mate
 int ezrt_trilist_read_obj_text(ezrt_trilist* list, const char* text, size_t len,
                                const float material[EZRT_MATERIAL_FLOATS], const float trans[16],
                                int smooth_normal);
-/* Append already-built triangles in Triangle_encoded layout. */
+/* ezrt_trilist_read_obj[_text] that also reads the mesh's texture coordinates, for EZRT_PARAM_TEXTURES: the "vt u v [w]" lines
+ * (w ignored) and each face vertex's vt index ("v/vt" and "v/vt/vn"; with EZRT_OBJ_HARDENED also negative, relative ones, and the
+ * UVs follow the fan).  A triangle whose three vertices all carry a vt gets their UVs and texture_id (>= 0, or -1), any other
+ * texture id -1.  A vt index out of range is EZRT_ERR_IO.  Positions, normals and materials are exactly read_obj's. */
+int ezrt_trilist_read_obj_textured(ezrt_trilist* list, const char* path, const float material[EZRT_MATERIAL_FLOATS],
+                                   const float trans[16], int smooth_normal, int32_t texture_id);
+int ezrt_trilist_read_obj_textured_text(ezrt_trilist* list, const char* text, size_t len, const float material[EZRT_MATERIAL_FLOATS],
+                                        const float trans[16], int smooth_normal, int32_t texture_id);
+/* Append already-built triangles in Triangle_encoded layout (texture id -1; also read_obj's triangles). */
 int ezrt_trilist_append_encoded(ezrt_trilist* list, const float* tris, int n);
+/* The texcoords (6 floats: u1, v1, u2, v2, u3, v3) and texture id of every triangle, in the list's current order: after
+ * ezrt_trilist_build_bvh, the order of the encoded triangles, i.e. what ezrt_scene_set_textures takes. */
+int ezrt_trilist_encode_texcoords(const ezrt_trilist* list, float* uv_out, int32_t* id_out);
 
 typedef enum ezrt_bvh_builder {
     EZRT_BVH_SAH_FAST = 0,    /* same tree as SAH_LITERAL, keys pre-computed, subtrees in parallel */

@@ -757,4 +757,73 @@ EZ_HD ez_vec3 ez_hg_sample(ez_vec3 d, float g, float h_1, float h_2) {
     return ez_to_normal_hemisphere(ez_v3(s * ez_cos(phi), s * ez_sin(phi), c), d);
 }
 
+/* ------------------------------------------------------------------ base-colour textures (EZRT_PARAM_TEXTURES, DESIGN.md section 15)
+ * A textured triangle carries three UVs and a texture index; the base colour of a hit on it is mat.baseColor * the texture's filtered
+ * linear colour at the hit's UV, per channel.  Texture index -1: the material's base colour.  No random number is drawn.
+ * Barycentrics (ez_tri_bary): drop the axis k of the largest |Ng_k| (the first on ties), 2D edge functions on the axes (k+1, k+2) mod 3:
+ *   w1 = e(p2, p3, P) / A, w2 = e(p3, p1, P) / A, w3 = (1 - w1) - w2 with A = e(p1, p2, p3); A == 0 or not finite: 1/3 each.
+ *   (surface_hit's weights are the reference's xy-projected ones, which collapse on triangles of degenerate xy projection.)
+ *   uv = (w1 uv1 + w2 uv2) + w3 uv3.
+ * Filter (ez_tex_sample): wrap in both axes, s = u - floor(u), t = v - floor(v); x = s W - 0.5, y = (1 - t) H - 0.5 (texel row 0 is
+ *   the image's top row, OBJ's v = 0 its bottom); x0 = floor(x), weight x - x0, x0 and x0 + 1 reduced modulo W (s may round to
+ *   1.0); the same for y.  Texels are RGBA8 (alpha ignored), each channel decoded by ez_srgb_table (the sRGB EOTF in float64, rounded
+ *   to fp32), then filtered bilinearly with lerp(a, b, f) = a + (b - a) f, so that four equal texels give that texel exactly.  A
+ *   non-finite u or v gives exactly (1, 1, 1). */
+static const float ez_srgb_table[256] = {
+#include "ezrt_srgb_table.inc"
+};
+EZ_HD float ez_tex_axis(const ez_vec3 v, int a) { return a == 0 ? v.x : (a == 1 ? v.y : v.z); }
+/* the 2D edge function of (p, q) at r on the axes (a, b) */
+EZ_HD float ez_tex_edge(ez_vec3 p, ez_vec3 q, ez_vec3 r, int a, int b) {
+    return (ez_tex_axis(q, a) - ez_tex_axis(p, a)) * (ez_tex_axis(r, b) - ez_tex_axis(p, b)) -
+           (ez_tex_axis(q, b) - ez_tex_axis(p, b)) * (ez_tex_axis(r, a) - ez_tex_axis(p, a));
+}
+EZ_HD void ez_tri_bary(ez_vec3 P, ez_vec3 p1, ez_vec3 p2, ez_vec3 p3, ez_vec3 Ng, float* w1, float* w2, float* w3) {
+    int k = 0;
+    float m = ez_abs(Ng.x);
+    if (ez_abs(Ng.y) > m) { k = 1; m = ez_abs(Ng.y); }
+    if (ez_abs(Ng.z) > m) k = 2;
+    const int a = (k + 1) % 3, b = (k + 2) % 3;
+    const float A = ez_tex_edge(p1, p2, p3, a, b);
+    if (A == 0.0f || !ez_finite(A)) {
+        *w1 = *w2 = *w3 = 1.0f / 3.0f;
+        return;
+    }
+    *w1 = EZ_DIV(ez_tex_edge(p2, p3, P, a, b), A);
+    *w2 = EZ_DIV(ez_tex_edge(p3, p1, P, a, b), A);
+    *w3 = (1.0f - *w1) - *w2;
+}
+EZ_HD float ez_tex_lerp(float a, float b, float f) { return a + (b - a) * f; }
+/* i in [-1, n] reduced modulo n */
+EZ_HD int ez_tex_wrap(int i, int n) { return i < 0 ? i + n : (i >= n ? i - n : i); }
+EZ_HD ez_vec3 ez_tex_texel(const uint32_t* texels, int idx, const float* lut) {
+#if defined(__CUDA_ARCH__)
+    const uint32_t c = __ldg(texels + idx);
+    return ez_v3(__ldg(lut + (c & 255u)), __ldg(lut + ((c >> 8) & 255u)), __ldg(lut + ((c >> 16) & 255u)));
+#else
+    const uint32_t c = texels[idx];
+    return ez_v3(lut[c & 255u], lut[(c >> 8) & 255u], lut[(c >> 16) & 255u]);
+#endif
+}
+/* the filtered linear colour of the W x H texture `texels` (RGBA8 as little-endian words, row 0 on top) at (u, v); lut = ez_srgb_table */
+EZ_HD ez_vec3 ez_tex_sample(const uint32_t* texels, int W, int H, float u, float v, const float* lut) {
+    if (!ez_finite(u) || !ez_finite(v)) return ez_v3(1.0f, 1.0f, 1.0f);
+    const float s = u - ez_floor(u), t = v - ez_floor(v);
+    const float x = s * (float)W - 0.5f, y = (1.0f - t) * (float)H - 0.5f;
+    const float fx0 = ez_floor(x), fy0 = ez_floor(y);
+    const float ax = x - fx0, ay = y - fy0;
+    const int x0 = ez_tex_wrap((int)fx0, W), x1 = ez_tex_wrap((int)fx0 + 1, W);
+    const int y0 = ez_tex_wrap((int)fy0, H), y1 = ez_tex_wrap((int)fy0 + 1, H);
+    const ez_vec3 t00 = ez_tex_texel(texels, y0 * W + x0, lut), t10 = ez_tex_texel(texels, y0 * W + x1, lut);
+    const ez_vec3 t01 = ez_tex_texel(texels, y1 * W + x0, lut), t11 = ez_tex_texel(texels, y1 * W + x1, lut);
+    const ez_vec3 top = ez_v3(ez_tex_lerp(t00.x, t10.x, ax), ez_tex_lerp(t00.y, t10.y, ax), ez_tex_lerp(t00.z, t10.z, ax));
+    const ez_vec3 bot = ez_v3(ez_tex_lerp(t01.x, t11.x, ax), ez_tex_lerp(t01.y, t11.y, ax), ez_tex_lerp(t01.z, t11.z, ax));
+    return ez_v3(ez_tex_lerp(top.x, bot.x, ay), ez_tex_lerp(top.y, bot.y, ay), ez_tex_lerp(top.z, bot.z, ay));
+}
+/* the interpolated UV of barycentrics (w1, w2, w3) over the triangle's (u1, v1, u2, v2) (u3, v3) */
+EZ_HD void ez_tex_uv(float w1, float w2, float w3, const float* uv6, float* u, float* v) {
+    *u = (w1 * uv6[0] + w2 * uv6[2]) + w3 * uv6[4];
+    *v = (w1 * uv6[1] + w2 * uv6[3]) + w3 * uv6[5];
+}
+
 #endif /* EZRT_MATH_H */
