@@ -68,6 +68,8 @@ SIGNATURES = {
     "ezrt_scene_set_medium": (C.c_int, [C.c_void_p, C.POINTER(Medium)]),
     "ezrt_scene_set_textures": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(Texture), c_float_p, c_int32_p]),
     "ezrt_scene_sample_textures": (C.c_int, [C.c_void_p, C.c_int, c_int32_p, c_float_p, c_float_p, c_float_p]),
+    "ezrt_scene_set_material_maps": (C.c_int, [C.c_void_p, c_int32_p, c_int32_p]),
+    "ezrt_scene_sample_materials": (C.c_int, [C.c_void_p, C.c_int, c_int32_p, c_float_p, c_float_p]),
     "ezrt_render": (C.c_int, [C.c_void_p, C.POINTER(RenderParams), c_float_p]),
     "ezrt_render_device": (C.c_int, [C.c_void_p, C.POINTER(RenderParams), C.c_void_p, C.c_void_p]),
     "ezrt_render_adaptive_device": (C.c_int, [C.c_void_p, C.POINTER(RenderParams), C.POINTER(AdaptiveParams), C.c_void_p, C.c_void_p,

@@ -25,6 +25,7 @@ PARAM_TRANSMISSION = 4
 PARAM_THIN_LENS = 8
 PARAM_MEDIUM = 16
 PARAM_TEXTURES = 32
+PARAM_MATERIAL_MAPS = 64
 MODES = {"diffuse_p3": 0, "disney_aniso_p4": 1, "disney_sobol_p5": 2, "disney_is_mis_p5": 3, "disney_lights": 4}
 
 TRAVERSE_ACCEL = 0
@@ -250,6 +251,7 @@ class RenderConfig:
     focus_distance: float = None  # ... focused at this depth along the view (-column 2 of camera_rotate); required with a lens
     medium: bool = False        # EZRT_PARAM_MEDIUM (MODE_DISNEY_LIGHTS only): the scene's homogeneous medium (Scene.set_medium, DESIGN.md section 14)
     textures: bool = False      # EZRT_PARAM_TEXTURES (MODE_DISNEY_LIGHTS only): the scene's base-colour textures (Scene.set_textures, DESIGN.md section 15)
+    material_maps: bool = False  # EZRT_PARAM_MATERIAL_MAPS (with textures): the scene's material maps (Scene.set_material_maps, DESIGN.md section 16)
 
     def to_struct(self):
         p = RenderParams()
@@ -263,7 +265,7 @@ class RenderConfig:
         p.profile = int(self.profile)
         p.reserved[0] = ((PARAM_ACCUMULATE if self.accumulate else 0) | (PARAM_ENV_LIGHT if self.env_light else 0) |
                          (PARAM_TRANSMISSION if self.transmission else 0) | (PARAM_MEDIUM if self.medium else 0) |
-                         (PARAM_TEXTURES if self.textures else 0))
+                         (PARAM_TEXTURES if self.textures else 0) | (PARAM_MATERIAL_MAPS if self.material_maps else 0))
         if self.lens_radius != 0:   # a negative or NaN radius is set too, so that the library rejects it
             if self.focus_distance is None:
                 raise ValueError("RenderConfig: a lens (lens_radius != 0) needs a focus_distance")
@@ -369,6 +371,31 @@ class Scene:
         rgb = np.zeros((tri.shape[0], 3), np.float32)
         check(lib.ezrt_scene_sample_textures(self._h, tri.shape[0], tri.ctypes.data_as(C.POINTER(C.c_int32)), _fp(pts), _fp(uv), _fp(rgb)))
         return uv, rgb
+
+    def set_material_maps(self, metal_rough_id, normal_id=None):
+        """ezrt_scene_set_material_maps: the material maps RenderConfig.material_maps renders (DESIGN.md section 16).  metal_rough_id and
+        normal_id [N] int: per triangle (in the order of the scene's triangles) the ids of its metallic-roughness and normal maps among
+        the textures of set_textures (-1: no map).  set_material_maps(None) clears them.  set_textures clears them too."""
+        if metal_rough_id is None:
+            check(lib.ezrt_scene_set_material_maps(self._h, None, None))
+            return
+        if normal_id is None:
+            raise ValueError("Scene.set_material_maps: normal_id is required with metal_rough_id")
+        n = self.tris.shape[0]
+        mr = np.ascontiguousarray(np.asarray(metal_rough_id, np.int32).reshape(n))
+        nm = np.ascontiguousarray(np.asarray(normal_id, np.int32).reshape(n))
+        check(lib.ezrt_scene_set_material_maps(self._h, mr.ctypes.data_as(C.POINTER(C.c_int32)), nm.ctypes.data_as(C.POINTER(C.c_int32))))
+
+    def sample_materials(self, tri, o, d, t):
+        """ezrt_scene_sample_materials: what the maps renders compute at hits of reference triangles tri ([n]) by rays (o [n, 3], d [n, 3],
+        t [n]): a dict of uv [n, 2], base_color [n, 3], roughness [n], metallic [n] and normal [n, 3] (the final shading normal)."""
+        tri = np.ascontiguousarray(np.asarray(tri, np.int32).reshape(-1))
+        n = tri.shape[0]
+        hits = np.ascontiguousarray(np.concatenate([np.asarray(o, np.float32).reshape(n, 3), np.asarray(d, np.float32).reshape(n, 3),
+                                                    np.asarray(t, np.float32).reshape(n, 1)], axis=1))
+        out = np.zeros((n, 10), np.float32)
+        check(lib.ezrt_scene_sample_materials(self._h, n, tri.ctypes.data_as(C.POINTER(C.c_int32)), _fp(hits), _fp(out)))
+        return dict(uv=out[:, 0:2], base_color=out[:, 2:5], roughness=out[:, 5], metallic=out[:, 6], normal=out[:, 7:10])
 
     def render(self, cfg, framebuffer=None):
         """render(width, height, spp) -> framebuffer: `spp` display() calls through HOST buffers

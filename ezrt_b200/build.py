@@ -267,6 +267,25 @@ def build_oracle_textures(force=False):
     return ORACLE_TEXTURES_SO
 
 
+ORACLE_MATERIAL_MAPS_SO = os.path.join(ROOT, "build", "libezrt_oracle_material_maps.so")
+
+
+def build_oracle_material_maps(force=False):
+    """build/libezrt_oracle_material_maps.so: tests/oracle_material_maps.cpp, the CPU restatement of the material maps (the table, the
+    tangent frame, the mapped normal, the flagged render's medium and transmission loops) over the textures' restatement (test
+    infrastructure, loaded only by tests/oracle_material_maps.py)."""
+    src = os.path.join(ROOT, "tests", "oracle_material_maps.cpp")
+    deps = [src] + [os.path.join(ROOT, "tests", f) for f in ("oracle_textures.cpp", "oracle_medium.cpp", "oracle_lens.cpp", "oracle_transmission.cpp",
+                                                              "oracle_env_light.cpp", "oracle_lights.cpp")] + \
+        [os.path.join(ROOT, "oracle", "ezrt_oracle.cpp")] + [os.path.join(INCLUDE, f) for f in os.listdir(INCLUDE)]
+    if force or _newer(ORACLE_MATERIAL_MAPS_SO, deps):
+        os.makedirs(os.path.dirname(ORACLE_MATERIAL_MAPS_SO), exist_ok=True)
+        tmp = ORACLE_MATERIAL_MAPS_SO + ".tmp%d" % os.getpid()
+        _run(["g++"] + HOST_FLAGS + ["-fopenmp", "-Wno-misleading-indentation", "-shared", "-I", INCLUDE, src, "-o", tmp])
+        os.replace(tmp, ORACLE_MATERIAL_MAPS_SO)
+    return ORACLE_MATERIAL_MAPS_SO
+
+
 def build_reference_hdrloader(force=False):
     return _oracle_recipes().build_reference_hdrloader(force)
 
@@ -333,6 +352,7 @@ def build_all(force=False, verbose=False):
     build_oracle_lens(force=force)
     build_oracle_medium(force=force)
     build_oracle_textures(force=force)
+    build_oracle_material_maps(force=force)
     build_example(force=force)
     build_reference_hdrloader(force=force)
     build_reference_shaders(force=force)

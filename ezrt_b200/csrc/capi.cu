@@ -111,7 +111,11 @@ struct ezrt_scene {
     // records in reference | accel order; tex.sh_base is set per render
     DeviceBuffer tex_buf, tex_rec_buf;
     bool has_textures = false;
+    // the material maps of EZRT_PARAM_MATERIAL_MAPS (ezrt_scene_set_material_maps): their ids live in the texcoord records' fourth word
+    bool has_maps = false;
+    int n_textures = 0;
     TexDev tex{};
+    MapsDev maps{};   // maps.sh_metal is set per render
     void* hot_base = nullptr;   // accel nodes | geometry (| vertices) | shading records (L2 persisting window)
     size_t hot_bytes = 0;
     size_t l2_persist_bytes = 0;
@@ -219,6 +223,11 @@ int validate_params(const ezrt_scene* scene, const ezrt_render_params* p) {
         if (p->mode != EZRT_MODE_DISNEY_LIGHTS)
             return ezrt_set_error(EZRT_ERR_INVALID, "render: EZRT_PARAM_TEXTURES needs the light sampling mode (got mode %d)", p->mode);
         if (!scene->has_textures) return ezrt_set_error(EZRT_ERR_INVALID, "render: EZRT_PARAM_TEXTURES needs textures (ezrt_scene_set_textures)");
+    }
+    if (p->reserved[0] & EZRT_PARAM_MATERIAL_MAPS) {
+        if (!(p->reserved[0] & EZRT_PARAM_TEXTURES))
+            return ezrt_set_error(EZRT_ERR_INVALID, "render: EZRT_PARAM_MATERIAL_MAPS needs EZRT_PARAM_TEXTURES");
+        if (!scene->has_maps) return ezrt_set_error(EZRT_ERR_INVALID, "render: EZRT_PARAM_MATERIAL_MAPS needs maps (ezrt_scene_set_material_maps)");
     }
     if (p->max_bounce < 0 || p->max_bounce > 64) return ezrt_set_error(EZRT_ERR_INVALID, "render: max_bounce out of range");
     if (p->out_channels != 3 && p->out_channels != 4) return ezrt_set_error(EZRT_ERR_INVALID, "render: out_channels must be 3 or 4");
@@ -934,7 +943,10 @@ int ezrt_scene_set_textures(ezrt_scene* s, int n_textures, const ezrt_texture* t
         CU_CHECK(cudaDeviceSynchronize());   // renders already enqueued still read the buffers
         s->tex_buf.release(); s->tex_rec_buf.release();
         s->has_textures = false;
+        s->has_maps = false;
+        s->n_textures = 0;
         s->tex = TexDev{};
+        s->maps = MapsDev{};
         return EZRT_OK;
     }
     const int n_tri = s->dev.n_triangles;
@@ -952,7 +964,7 @@ int ezrt_scene_set_textures(ezrt_scene* s, int n_textures, const ezrt_texture* t
             return ezrt_set_error(EZRT_ERR_INVALID, "scene_set_textures: triangle %d has texture id %d (valid: -1 to %d)", i, texture_id[i], n_textures - 1);
     // host staging: sRGB table | texture table | texels; reference-order records.  The new buffers are filled before the previous
     // ones are released, so that a failure leaves the scene's textures as they were.
-    const size_t lut_bytes = 256 * sizeof(float), table_bytes = ((sizeof(int4) * (size_t)n_textures + 255) / 256) * 256;
+    const size_t lut_bytes = 2 * 256 * sizeof(float), table_bytes = ((sizeof(int4) * (size_t)n_textures + 255) / 256) * 256;
     if (n_texels > (size_t)INT32_MAX) return ezrt_set_error(EZRT_ERR_INVALID, "scene_set_textures: more than 2^31 texels");
     std::vector<unsigned char> host;
     std::vector<float4> rec;
@@ -962,7 +974,8 @@ int ezrt_scene_set_textures(ezrt_scene* s, int n_textures, const ezrt_texture* t
     } catch (const std::bad_alloc&) {
         return ezrt_set_error(EZRT_ERR_NOMEM, "scene_set_textures: host staging of %zu texels", n_texels);
     }
-    memcpy(host.data(), ez_srgb_table, lut_bytes);
+    memcpy(host.data(), ez_srgb_table, sizeof(ez_srgb_table));   // then ez_unorm8_table, for the material maps
+    memcpy(host.data() + sizeof(ez_srgb_table), ez_unorm8_table, sizeof(ez_unorm8_table));
     int4* table = (int4*)(host.data() + lut_bytes);
     size_t off = 0;
     for (int k = 0; k < n_textures; k++) {
@@ -1002,10 +1015,78 @@ int ezrt_scene_set_textures(ezrt_scene* s, int n_textures, const ezrt_texture* t
     t.rec = d_rec;
     t.acc_rec = d_acc;
     t.lut = (const float*)s->tex_buf.p;
+    s->maps.unorm = t.lut + 256;
     t.table = (const int4*)((const char*)s->tex_buf.p + lut_bytes);
     t.texels = (const uint32_t*)((const char*)s->tex_buf.p + lut_bytes + table_bytes);
     s->tex = t;
     s->has_textures = true;
+    s->n_textures = n_textures;
+    s->has_maps = false;   // the new records' fourth words are 0: the maps' ids referred to the previous textures
+    return EZRT_OK;
+}
+
+int ezrt_scene_set_material_maps(ezrt_scene* s, const int32_t* metal_rough_id, const int32_t* normal_id) {
+    if (!s) return ezrt_set_error(EZRT_ERR_INVALID, "scene_set_material_maps: null scene");
+    if (!s->has_textures) return ezrt_set_error(EZRT_ERR_INVALID, "scene_set_material_maps: no textures (ezrt_scene_set_textures)");
+    if ((metal_rough_id == nullptr) != (normal_id == nullptr)) return ezrt_set_error(EZRT_ERR_INVALID, "scene_set_material_maps: bad argument");
+    const int n_tri = s->dev.n_triangles;
+    const int n_tex = s->n_textures;
+    std::vector<uint32_t> words;
+    try {
+        words.assign((size_t)n_tri, 0u);
+    } catch (const std::bad_alloc&) {
+        return ezrt_set_error(EZRT_ERR_NOMEM, "scene_set_material_maps: host staging");
+    }
+    if (metal_rough_id) {
+        for (int i = 0; i < n_tri; i++) {
+            const int32_t a = metal_rough_id[i], b = normal_id[i];
+            if (a < -1 || a >= n_tex || a >= 65535 || b < -1 || b >= n_tex || b >= 65535)
+                return ezrt_set_error(EZRT_ERR_INVALID, "scene_set_material_maps: triangle %d has map ids (%d, %d) (valid: -1 to %d)", i, a, b,
+                                      std::min(n_tex, 65535) - 1);
+            words[i] = (uint32_t)(a + 1) | ((uint32_t)(b + 1) << 16);
+        }
+    }
+    CU_CHECK(cudaSetDevice(s->device));
+    if (n_tri > 0) {
+        DeviceBuffer buf;
+        int rc = buf.ensure(sizeof(uint32_t) * (size_t)n_tri);
+        if (rc) return rc;
+        cudaError_t e = cudaDeviceSynchronize();   // renders already enqueued still read the records
+        if (e == cudaSuccess) e = cudaMemcpy(buf.p, words.data(), sizeof(uint32_t) * (size_t)n_tri, cudaMemcpyHostToDevice);
+        if (e == cudaSuccess) {
+            launch_maps_set((const uint32_t*)buf.p, s->dev.acc_tri_ref, n_tri, (float4*)s->tex.rec, (float4*)s->tex.acc_rec, 0);
+            e = cudaGetLastError();
+        }
+        if (e == cudaSuccess) e = cudaDeviceSynchronize();
+        buf.release();
+        if (e != cudaSuccess) return ezrt_set_error(EZRT_ERR_CUDA, "scene_set_material_maps: %s", cudaGetErrorString(e));
+    }
+    s->has_maps = metal_rough_id != nullptr;
+    return EZRT_OK;
+}
+
+int ezrt_scene_sample_materials(ezrt_scene* s, int n, const int32_t* tri, const float* hits, float* out) {
+    if (!s || n < 0 || (n > 0 && (!tri || !hits || !out))) return ezrt_set_error(EZRT_ERR_INVALID, "scene_sample_materials: bad argument");
+    if (!s->has_textures) return ezrt_set_error(EZRT_ERR_INVALID, "scene_sample_materials: no textures (ezrt_scene_set_textures)");
+    for (int i = 0; i < n; i++)
+        if (tri[i] < 0 || tri[i] >= s->dev.n_triangles) return ezrt_set_error(EZRT_ERR_INVALID, "scene_sample_materials: triangle %d out of range", tri[i]);
+    if (n == 0) return EZRT_OK;
+    CU_CHECK(cudaSetDevice(s->device));
+    DeviceBuffer buf;
+    int rc = buf.ensure(sizeof(float) * 18 * (size_t)n + 256);
+    if (rc) return rc;
+    int32_t* d_tri = (int32_t*)buf.p;
+    float* d_h = (float*)(d_tri + n);
+    float* d_out = d_h + 7 * (size_t)n;
+    cudaError_t e = cudaMemcpy(d_tri, tri, sizeof(int32_t) * (size_t)n, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = cudaMemcpy(d_h, hits, sizeof(float) * 7 * (size_t)n, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) {
+        launch_sample_materials(s->dev, s->tex, s->maps, n, d_tri, d_h, d_out, 0);
+        e = cudaGetLastError();
+    }
+    if (e == cudaSuccess) e = cudaMemcpy(out, d_out, sizeof(float) * 10 * (size_t)n, cudaMemcpyDeviceToHost);
+    buf.release();
+    if (e != cudaSuccess) return ezrt_set_error(EZRT_ERR_CUDA, "scene_sample_materials: %s", cudaGetErrorString(e));
     return EZRT_OK;
 }
 
@@ -1093,6 +1174,8 @@ static int light_options(ezrt_scene* s, const ezrt_render_params* p, cudaStream_
     if (p->reserved[0] & EZRT_PARAM_TEXTURES) {
         o.tex = s->tex;
         o.tex_on = true;
+        o.maps = s->maps;
+        o.maps_on = (p->reserved[0] & EZRT_PARAM_MATERIAL_MAPS) != 0;   // validated: with the textures, and maps are set
     }
     return EZRT_OK;
 }
@@ -1159,7 +1242,7 @@ static int render_device_impl(ezrt_scene* s, const ezrt_render_params* p, float*
     {   // bound the batch by the memory that is actually there (scratch already held by this scene counts as available);
         // asked once per (slots per frame, integrator): cudaMemGetInfo is a driver round trip, the render path is launch-only
         const size_t per_slot = 2 * (sizeof(float4) * 4 + sizeof(float2)) + 2 * sizeof(float4) + sizeof(uint32_t) +
-                                (is_mode ? (size_t)EZRT_SHADOW_SLOT_BYTES : 0) + (lopt.tex_on ? sizeof(float4) : 0) + (s->sort_rays ? 2 * sizeof(uint32_t) : 0) +
+                                (is_mode ? (size_t)EZRT_SHADOW_SLOT_BYTES : 0) + (lopt.tex_on ? sizeof(float4) : 0) + (lopt.maps_on ? sizeof(float) : 0) + (s->sort_rays ? 2 * sizeof(uint32_t) : 0) +
                                 (av ? 2 * sizeof(float4) : 0);
         if (s->fmax_key[0] != per_frame || s->fmax_key[1] != per_slot) {
             size_t free_b = 0, total_b = 0;
@@ -1189,6 +1272,12 @@ static int render_device_impl(ezrt_scene* s, const ezrt_render_params* p, float*
         if ((rc = s->shadow_buf.ensure(((size_t)EZRT_SHADOW_SLOT_BYTES + sizeof(float4)) * capacity + 512))) return rc;
         if ((rc = carve_shadow(s->shadow_buf, capacity, sq))) return rc;
         lopt.tex.sh_base = (float4*)((((uintptr_t)sq.lit + capacity) + 255) & ~(uintptr_t)255);
+    }
+    if (lopt.maps_on) {   // ... and their mapped metallic after those (the roughness rides in sh_base's fourth word)
+        if ((rc = s->shadow_buf.ensure(((size_t)EZRT_SHADOW_SLOT_BYTES + sizeof(float4) + sizeof(float)) * capacity + 768))) return rc;
+        if ((rc = carve_shadow(s->shadow_buf, capacity, sq))) return rc;
+        lopt.tex.sh_base = (float4*)((((uintptr_t)sq.lit + capacity) + 255) & ~(uintptr_t)255);
+        lopt.maps.sh_metal = (float*)((((uintptr_t)(lopt.tex.sh_base + capacity)) + 255) & ~(uintptr_t)255);
     }
     float4* aov_rec = nullptr;   // feature-buffer render only: the first-hit record of every sample slot
     if (av) {

@@ -1958,24 +1958,57 @@ __device__ __forceinline__ vec3 tex_base_color(const SceneDev& sc, const TexDev&
     const int4 t = __ldg(tex.table + id);
     return ez_mul(base, ez_tex_sample(tex.texels + t.x, t.y, t.z, u, v, tex.lut));
 }
+// EZRT_PARAM_MATERIAL_MAPS (ezrt_math.h, DESIGN.md section 16): the whole lookup of a hit in one place -- mat's base colour textured
+// as tex_base_color's, its roughness and metallic by the metallic-roughness map, and N (surface_hit's, for a hit from `inside`,
+// viewed from V) replaced by the normal map's.  The same loads as tex_base_color, plus four texel words per map.
+__device__ __forceinline__ void tex_material(const SceneDev& sc, const TexDev& tex, const MapsDev& maps_dev, int tri, bool accel_space, vec3 P, vec3 V, bool inside,
+                                             MaterialDev& mat, vec3& N, float* uv_out = nullptr) {
+    const float4* r = (accel_space ? tex.acc_rec : tex.rec) + (size_t)tri * 2;
+    const float4 a = ldg4(r), b = ldg4(r + 1);
+    const int id = __float_as_int(b.z);
+    const uint32_t maps = __float_as_uint(b.w);
+    vec3 p1, p2, p3;
+    tri_vertices(sc, tri, accel_space, p1, p2, p3);
+    const vec3 Ng = f4xyz(ldg4(tri_geo_rec(sc, tri, accel_space)));
+    float w1, w2, w3, u, v;
+    ez_tri_bary(P, p1, p2, p3, Ng, &w1, &w2, &w3);
+    const float uv6[6] = {a.x, a.y, a.z, a.w, b.x, b.y};
+    ez_tex_uv(w1, w2, w3, uv6, &u, &v);
+    if (uv_out) { uv_out[0] = u; uv_out[1] = v; }
+    if (id >= 0) {
+        const int4 t = __ldg(tex.table + id);
+        mat.baseColor = ez_mul(mat.baseColor, ez_tex_sample(tex.texels + t.x, t.y, t.z, u, v, tex.lut));
+    }
+    const int mr = ez_maps_mr_id(maps), nm = ez_maps_normal_id(maps);
+    if (mr >= 0) {
+        const int4 t = __ldg(tex.table + mr);
+        ez_mr_apply(ez_tex_sample(tex.texels + t.x, t.y, t.z, u, v, maps_dev.unorm), &mat.roughness, &mat.metallic);
+    }
+    if (nm >= 0) {
+        const int4 t = __ldg(tex.table + nm);
+        N = ez_normal_map(p1, p2, p3, uv6, u, v, ez_tex_sample(tex.texels + t.x, t.y, t.z, u, v, maps_dev.unorm), N, inside, V);
+    }
+}
 
 // A medium vertex (EZRT_PARAM_MEDIUM; ezrt_math.h, DESIGN.md section 14): p's segment scattered at t_s before its hit (hit_t,
 // hit_tri) or its miss.  The weights of the segment (bounce >= 1) and the albedo enter the history; then, below max_bounce, one light
 // sample from P as at a surface but without the hemisphere test and the self exclusion (its shadow ray carries EZRT_MEDIUM_VERTEX
 // and d), and the phase function's sample as the next ray with the record (splat(p), p, 1).  Returns false when the path ends.
-// TEX: the first-hit record's albedo is the textured base colour.
-template <bool AOV, bool ENV, bool TEX = false>
+// TEX: the first-hit record's albedo is the textured base colour.  MAPS: ... and its normal the mapped one.
+template <bool AOV, bool ENV, bool TEX = false, bool MAPS = false>
 __device__ __forceinline__ bool medium_step(const SceneDev& sc, const RenderDev& rd, int bounce, PathRegs& p, float t_s, float hit_t,
                                             int hit_tri, vec3& Lo, vec3& Le, bool& primary_miss, ShadowRay& sh, float4* aov_rec,
-                                            const LightsDev& lights, const EnvDev& env, const MediumDev& med, const TexDev& tex = TexDev{}) {
+                                            const LightsDev& lights, const EnvDev& env, const MediumDev& med, const TexDev& tex = TexDev{},
+                                            const MapsDev& maps = MapsDev{}) {
     if (bounce == 0) {
         Lo = splat3(0.0f);
         Le = splat3(0.0f);
         primary_miss = hit_tri < 0;   // k_blend: a camera ray that left the scene, its colour the Lo of its medium vertices
         if (AOV && hit_tri >= 0) {    // the feature buffers describe the first surface behind the medium
-            const SurfaceHit hit = surface_hit(sc, p.o, p.d, hit_t, hit_tri, false, rd.accel_space != 0);
+            SurfaceHit hit = surface_hit(sc, p.o, p.d, hit_t, hit_tri, false, rd.accel_space != 0);
             MaterialDev mat = load_material(sc, hit.matId);
-            if constexpr (TEX) mat.baseColor = tex_base_color(sc, tex, hit_tri, rd.accel_space != 0, hit.P, mat.baseColor);
+            if constexpr (MAPS) tex_material(sc, tex, maps, hit_tri, rd.accel_space != 0, hit.P, ez_neg(p.d), hit.inside, mat, hit.N);
+            else if constexpr (TEX) mat.baseColor = tex_base_color(sc, tex, hit_tri, rd.accel_space != 0, hit.P, mat.baseColor);
             aov_rec[0] = make_float4(mat.baseColor.x, mat.baseColor.y, mat.baseColor.z, hit_t);
             aov_rec[1] = make_float4(hit.N.x, hit.N.y, hit.N.z, 0.0f);
         }
@@ -2056,11 +2089,17 @@ __device__ __forceinline__ bool medium_step(const SceneDev& sc, const RenderDev&
 // TEX (light sampling mode with EZRT_PARAM_TEXTURES, ezrt_math.h, DESIGN.md section 15): every use of the hit's base colour -- the
 // BRDF / mixture's evaluation, sampling and pdf, the first-hit record -- takes the textured one (tex_base_color); a light sample's
 // shadow ray carries it out through *sh_base, for k_nee.
-template <int MODE, bool DEFER_NEE = false, bool AOV = false, bool ENV = false, bool TRANS = false, bool MEDIUM = false, bool TEX = false>
+// MAPS (with TEX; EZRT_PARAM_MATERIAL_MAPS, ezrt_math.h, DESIGN.md section 16): the hit's roughness and metallic are the
+// metallic-roughness map's and its shading normal N the normal map's (tex_material), everywhere N and the material are read after
+// the lookup: the BSDF, the lobe weights, the light samples' hemisphere tests, the path record's cosine, the shadow ray's N and the
+// first-hit record; the emission's MIS and the inside test keep the geometric normal.  *sh_rm carries (roughness, metallic) to k_nee.
+template <int MODE, bool DEFER_NEE = false, bool AOV = false, bool ENV = false, bool TRANS = false, bool MEDIUM = false, bool TEX = false,
+          bool MAPS = false>
 __device__ __forceinline__ bool shade_step(const SceneDev& sc, const RenderDev& rd, int bounce, PathRegs& p, float hit_t,
                                            int hit_tri, uint32_t px, uint32_t py, float2 sob, vec3& Lo, vec3& Le,
                                            bool& primary_miss, ShadowRay& sh, float4* aov_rec = nullptr, LightsDev lights = LightsDev{},
-                                           EnvDev env = EnvDev{}, MediumDev med = MediumDev{}, TexDev tex = TexDev{}, vec3* sh_base = nullptr) {
+                                           EnvDev env = EnvDev{}, MediumDev med = MediumDev{}, TexDev tex = TexDev{}, vec3* sh_base = nullptr,
+                                           float2* sh_rm = nullptr, MapsDev maps = MapsDev{}) {
     sh.valid = false;
     const int mode = (MODE < 0) ? rd.mode : MODE;
     const bool is_mode = (mode == EZRT_MODE_DISNEY_IS_MIS_P5);
@@ -2068,13 +2107,14 @@ __device__ __forceinline__ bool shade_step(const SceneDev& sc, const RenderDev& 
     constexpr bool lights_mode = (MODE == EZRT_MODE_DISNEY_LIGHTS);
     const bool below = TRANS && p.cosine_i < 0.0f;   // the BSDF sample went below the surface: no light strategy reaches it
     static_assert(lights_mode || !TEX, "textures are rendered in the light sampling mode");
+    static_assert(TEX || !MAPS, "material maps are rendered with the textures");
     if constexpr (MEDIUM) {
         static_assert(lights_mode && !TRANS, "the medium is rendered in the light sampling mode, without transmission");
         if (bounce > 0 && p.pdf <= 0.0f) return false;   // P5/fsh:865, before the free flight's draw
         float t_s;
         const float t_end = (hit_tri < 0) ? __int_as_float(0x7f800000) : hit_t;
         if (ez_medium_flight(&med, p.o, p.d, t_end, &p.seed, &t_s))
-            return medium_step<AOV, ENV, TEX>(sc, rd, bounce, p, t_s, hit_t, hit_tri, Lo, Le, primary_miss, sh, aov_rec, lights, env, med, tex);
+            return medium_step<AOV, ENV, TEX, MAPS>(sc, rd, bounce, p, t_s, hit_t, hit_tri, Lo, Le, primary_miss, sh, aov_rec, lights, env, med, tex, maps);
     }
     if (bounce == 0) {
         Lo = splat3(0.0f);
@@ -2108,7 +2148,12 @@ __device__ __forceinline__ bool shade_step(const SceneDev& sc, const RenderDev& 
     MaterialDev mat = load_material(sc, hit.matId);
     if constexpr (TEX) {   // not at the last vertex, where only the emission is read
         if ((AOV && bounce == 0) || bounce < rd.max_bounce) {
-            mat.baseColor = tex_base_color(sc, tex, hit_tri, rd.accel_space != 0, hit.P, mat.baseColor);
+            if constexpr (MAPS) {
+                tex_material(sc, tex, maps, hit_tri, rd.accel_space != 0, hit.P, ez_neg(p.d), hit.inside, mat, hit.N);
+                *sh_rm = make_float2(mat.roughness, mat.metallic);
+            } else {
+                mat.baseColor = tex_base_color(sc, tex, hit_tri, rd.accel_space != 0, hit.P, mat.baseColor);
+            }
             *sh_base = mat.baseColor;
         }
     }

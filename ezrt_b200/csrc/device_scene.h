@@ -167,6 +167,16 @@ struct TexDev {
     const float* lut;
     float4* sh_base;
 };
+// The material maps of EZRT_PARAM_MATERIAL_MAPS (ezrt_math.h, DESIGN.md section 16), set by ezrt_scene_set_material_maps: their ids
+// are the fourth word of TexDev's records, (metal_rough_id + 1) | (normal_id + 1) << 16 (0: no maps).  Passed to the maps
+// instantiations (k_shade<.., TEX, MAPS>, k_nee<.., TEX, MAPS>) as one more parameter, after TexDev.
+//   unorm: ez_unorm8_table, read through L1
+//   sh_metal: the mapped metallic of every shadow slot's shading point (4 B per slot, after TexDev::sh_base, maps renders only); the
+//       mapped roughness rides in sh_base[j].w
+struct MapsDev {
+    const float* unorm;
+    float* sh_metal;
+};
 
 // A shadow ray and what k_nee needs to evaluate the light sample's contribution once the ray got through (nee_contrib):
 // the BRDF / environment evaluation of the light sample is done after the shadow pass, for unoccluded rays only.

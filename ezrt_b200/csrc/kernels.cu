@@ -549,13 +549,17 @@ __global__ void __launch_bounds__(EZRT_EXTEND_MAX_THREADS, EZRT_EXTEND_LB_BLOCKS
 // MEDIUM (light sampling mode with EZRT_PARAM_MEDIUM): the homogeneous medium med (shade_step, medium_step).
 // TEX (light sampling mode with EZRT_PARAM_TEXTURES): the base-colour textures tex (shade_step); every shadow slot also gets its
 // shading point's textured base colour, tex.sh_base[spos].
-template <int MODE, bool LIST, bool AOV = false, bool ENV = false, bool TRANS = false, bool MEDIUM = false, bool TEX = false>
+// MAPS (with TEX; EZRT_PARAM_MATERIAL_MAPS): the material maps (shade_step); the slot also gets the mapped roughness in
+// tex.sh_base[spos].w and the mapped metallic in maps.sh_metal[spos].
+template <int MODE, bool LIST, bool AOV = false, bool ENV = false, bool TRANS = false, bool MEDIUM = false, bool TEX = false,
+          bool MAPS = false>
 __global__ void __launch_bounds__(128, EZRT_SHADE_MIN_BLOCKS) k_shade(SceneDev sc, RenderDev rd, const TileDev* __restrict__ tiles, int bounce,
                                                uint32_t batch_first_frame, PathQueue qin, const uint32_t* __restrict__ in_count,
                                                PathQueue qout, uint32_t* out_count, ShadowQueue sq, uint32_t* s_count,
                                                float4* __restrict__ Lo, float4* __restrict__ Le, uint32_t n_fused, uint32_t n_frames,
                                                const uint32_t* __restrict__ list, const float2* __restrict__ side_hit,
-                                               float4* __restrict__ aov_rec, LightsDev lights, EnvDev env, MediumDev med, TexDev tex) {
+                                               float4* __restrict__ aov_rec, LightsDev lights, EnvDev env, MediumDev med, TexDev tex,
+                                               MapsDev maps) {
     // The Sobol pair of (bounce, frame) is the same for every pixel of a frame (P5/fsh:361-376: up to 2 x 32 table XORs per path): each
     // block computes the pairs of the batch's frames once into shared memory (batches of more than EZRT_SOBOL_TABLE frames compute per path).
     __shared__ float2 s_sobol[EZRT_SOBOL_TABLE];
@@ -593,6 +597,7 @@ __global__ void __launch_bounds__(128, EZRT_SHADE_MIN_BLOCKS) k_shade(SceneDev s
         ShadowRay sh;
         sh.valid = false;
         vec3 sh_base;   // TEX: the shading point's textured base colour
+        float2 sh_rm;   // MAPS: its mapped roughness and metallic
         uint32_t slot = 0;
         uint32_t px = 0, py = 0, fib = 0;
         bool present = i < n;
@@ -680,9 +685,9 @@ __global__ void __launch_bounds__(128, EZRT_SHADE_MIN_BLOCKS) k_shade(SceneDev s
             }
 #endif
             if (LIST || __float_as_int(hit.y) != EZRT_TRI_PENDING) {   // pending: deferred by the accel kernel, shaded by the LIST pass
-                alive = shade_step<MODE, MODE == EZRT_MODE_DISNEY_IS_MIS_P5, AOV, ENV, TRANS, MEDIUM, TEX>(sc, rd, bounce, p, hit.x, __float_as_int(hit.y), px, py,
+                alive = shade_step<MODE, MODE == EZRT_MODE_DISNEY_IS_MIS_P5, AOV, ENV, TRANS, MEDIUM, TEX, MAPS>(sc, rd, bounce, p, hit.x, __float_as_int(hit.y), px, py,
                                                                                                           sob, lo, le, pmiss, sh, AOV ? aov_rec + 2 * (size_t)slot : nullptr,
-                                                                                                          lights, env, med, tex, &sh_base);
+                                                                                                          lights, env, med, tex, &sh_base, &sh_rm, maps);
                 if (bounce == 0) {
                     // Le is zero for every surface that does not emit: it is stored (and read back by k_blend) only otherwise.
                     // color = Le + Lo with Le = +-0 is Lo bit for bit, because Lo is never -0.0 (it starts at +0.0 and only grows by additions)
@@ -712,7 +717,10 @@ __global__ void __launch_bounds__(128, EZRT_SHADE_MIN_BLOCKS) k_shade(SceneDev s
                 __stcs(sq.view + spos, make_float4(sh.V.x, sh.V.y, sh.V.z, LT ? sh.pdf : 0.0f));
                 __stcs(sq.hist + spos, make_float4(sh.history.x, sh.history.y, sh.history.z, LT ? __int_as_float(sh.light_mat) : 0.0f));
                 if constexpr (TEX) {   // a medium vertex's slot has no shading point: its entry is never read
-                    if (sh.matId != EZRT_MEDIUM_VERTEX || !MEDIUM) __stcs(tex.sh_base + spos, make_float4(sh_base.x, sh_base.y, sh_base.z, 0.0f));
+                    if (sh.matId != EZRT_MEDIUM_VERTEX || !MEDIUM) {
+                        __stcs(tex.sh_base + spos, make_float4(sh_base.x, sh_base.y, sh_base.z, MAPS ? sh_rm.x : 0.0f));
+                        if constexpr (MAPS) __stcs(maps.sh_metal + spos, sh_rm.y);
+                    }
                 }
             }
         }
@@ -731,9 +739,10 @@ __global__ void __launch_bounds__(128, EZRT_SHADE_MIN_BLOCKS) k_shade(SceneDev s
 // MEDIUM: every contribution times the shadow ray's transmittance through the medium med; a medium vertex's (ray_d.w =
 // EZRT_MEDIUM_VERTEX, view = d) is evaluated with the phase function (nee_medium_contrib).
 // TEX: the shading point's material with the textured base colour k_shade left in tex.sh_base[j].
-template <int MODE, bool ENV = false, bool TRANS = false, bool MEDIUM = false, bool TEX = false>
+// MAPS: ... and the mapped roughness and metallic, tex.sh_base[j].w and maps.sh_metal[j]; the slot's N is already the mapped normal.
+template <int MODE, bool ENV = false, bool TRANS = false, bool MEDIUM = false, bool TEX = false, bool MAPS = false>
 __global__ void __launch_bounds__(128, 8) k_nee(SceneDev sc, RenderDev rd, ShadowQueue sq, const uint32_t* __restrict__ s_count, float4* __restrict__ Lo,
-                                                MediumDev med, TexDev tex) {
+                                                MediumDev med, TexDev tex, MapsDev maps) {
     static_assert(MODE == EZRT_MODE_DISNEY_LIGHTS || !(ENV || TRANS || MEDIUM), "the options exist in the light sampling mode");
     static_assert(!(TRANS && MEDIUM), "the medium is rendered without transmission");
     __shared__ uint32_t s_scan[34];
@@ -759,7 +768,14 @@ __global__ void __launch_bounds__(128, 8) k_nee(SceneDev sc, RenderDev rd, Shado
             const int m_raw = __float_as_int(d4.w);
             const auto material = [&](int m_id) {
                 MaterialDev m = load_material(sc, m_id);
-                if constexpr (TEX) m.baseColor = f4xyz(__ldcs(tex.sh_base + j));
+                if constexpr (MAPS) {
+                    const float4 b = __ldcs(tex.sh_base + j);
+                    m.baseColor = f4xyz(b);
+                    m.roughness = b.w;
+                    m.metallic = __ldcs(maps.sh_metal + j);
+                } else if constexpr (TEX) {
+                    m.baseColor = f4xyz(__ldcs(tex.sh_base + j));
+                }
                 return m;
             };
             const vec3 V = ez_v3(v4.x, v4.y, v4.z), N = ez_v3(n4.x, n4.y, n4.z), Ld = ez_v3(d4.x, d4.y, d4.z), hist = ez_v3(h4.x, h4.y, h4.z);
@@ -1357,12 +1373,13 @@ static void launch_shade_t(int blocks, const SceneDev& sc, const RenderDev& rd, 
                            float4* Lo, float4* Le, uint32_t n_fused, uint32_t n_frames, const uint32_t* list, const float2* side_hit,
                            float4* aov_rec, const LightOptions& o, cudaStream_t st) {
     auto launch = [&](auto M) {
-        with_bools([&](auto A, auto E, auto T, auto X, auto TX) {
-            if constexpr ((M == EZRT_MODE_DISNEY_LIGHTS || !(E || T || X || TX)) && !(T && X))   // the options exist in the light sampling mode
-                k_shade<M, LIST, A, E, T, X, TX><<<blocks, 128, 0, st>>>(sc, rd, tiles, bounce, batch_first_frame, qin, in_count, qout, out_count, sq,
-                                                                         s_count, Lo, Le, n_fused, n_frames, list, side_hit, aov_rec, o.lights, o.env, o.med,
-                                                                         o.tex);
-        }, aov_rec != nullptr, o.env_on, o.trans_on, o.medium_on, o.tex_on);
+        with_bools([&](auto A, auto E, auto T, auto X, auto TX, auto MP) {
+            // the options exist in the light sampling mode; the maps with the textures
+            if constexpr ((M == EZRT_MODE_DISNEY_LIGHTS || !(E || T || X || TX)) && !(T && X) && (TX || !MP))
+                k_shade<M, LIST, A, E, T, X, TX, MP><<<blocks, 128, 0, st>>>(sc, rd, tiles, bounce, batch_first_frame, qin, in_count, qout, out_count, sq,
+                                                                             s_count, Lo, Le, n_fused, n_frames, list, side_hit, aov_rec, o.lights, o.env,
+                                                                             o.med, o.tex, o.maps);
+        }, aov_rec != nullptr, o.env_on, o.trans_on, o.medium_on, o.tex_on, o.maps_on);
     };
     switch (rd.mode) {
         case EZRT_MODE_DIFFUSE_P3: launch(std::integral_constant<int, EZRT_MODE_DIFFUSE_P3>{}); break;
@@ -1394,10 +1411,11 @@ void launch_deferred_lane(const SceneDev& sc, const RenderDev& rd, const TileDev
 void launch_nee(const SceneDev& sc, const RenderDev& rd, ShadowQueue sq, const uint32_t* s_count, float4* Lo, uint32_t n_max, int n_sms, cudaStream_t st,
                 const LightOptions& o) {
     const int blocks = std::max(1, std::min(div_up(n_max, 512), n_sms * 8));
-    with_bools([&](auto L, auto E, auto T, auto X, auto TX) {
-        if constexpr ((L || !(E || T || X || TX)) && !(T && X))   // the options exist in the light sampling mode; the other mode here is mode 3
-            k_nee<L ? EZRT_MODE_DISNEY_LIGHTS : EZRT_MODE_DISNEY_IS_MIS_P5, E, T, X, TX><<<blocks, 128, 0, st>>>(sc, rd, sq, s_count, Lo, o.med, o.tex);
-    }, rd.mode == EZRT_MODE_DISNEY_LIGHTS, o.env_on, o.trans_on, o.medium_on, o.tex_on);
+    with_bools([&](auto L, auto E, auto T, auto X, auto TX, auto MP) {
+        // the options exist in the light sampling mode (the other mode here is mode 3); the maps with the textures
+        if constexpr ((L || !(E || T || X || TX)) && !(T && X) && (TX || !MP))
+            k_nee<L ? EZRT_MODE_DISNEY_LIGHTS : EZRT_MODE_DISNEY_IS_MIS_P5, E, T, X, TX, MP><<<blocks, 128, 0, st>>>(sc, rd, sq, s_count, Lo, o.med, o.tex, o.maps);
+    }, rd.mode == EZRT_MODE_DISNEY_LIGHTS, o.env_on, o.trans_on, o.medium_on, o.tex_on, o.maps_on);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -1529,6 +1547,37 @@ __global__ void k_sample_textures(SceneDev sc, TexDev tex, int n, const int32_t*
 void launch_sample_textures(const SceneDev& sc, const TexDev& tex, int n, const int32_t* tri, const float* points, float* uv, float* rgb,
                             cudaStream_t st) {
     k_sample_textures<<<div_up(n, 128), 128, 0, st>>>(sc, tex, n, tri, points, uv, rgb);
+}
+// what shade_step<.., TEX, MAPS> computes at hits (reference triangle, o, d, t) (ezrt_scene_sample_materials): the UV, the textured
+// base colour, the mapped roughness and metallic and the final shading normal, 10 floats per hit
+__global__ void k_sample_materials(SceneDev sc, TexDev tex, MapsDev maps, int n, const int32_t* __restrict__ tri, const float* __restrict__ odt,
+                                   float* __restrict__ out) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const int t = tri[i];
+    const float* r = odt + 7 * (size_t)i;
+    const vec3 o = ez_v3(r[0], r[1], r[2]), d = ez_v3(r[3], r[4], r[5]);
+    SurfaceHit hit = surface_hit(sc, o, d, r[6], t, false, false);
+    MaterialDev mat = load_material(sc, hit.matId);
+    float* w = out + 10 * (size_t)i;
+    tex_material(sc, tex, maps, t, false, hit.P, ez_neg(d), hit.inside, mat, hit.N, w);
+    w[2] = mat.baseColor.x; w[3] = mat.baseColor.y; w[4] = mat.baseColor.z;
+    w[5] = mat.roughness; w[6] = mat.metallic;
+    w[7] = hit.N.x; w[8] = hit.N.y; w[9] = hit.N.z;
+}
+void launch_sample_materials(const SceneDev& sc, const TexDev& tex, const MapsDev& maps, int n, const int32_t* tri, const float* odt, float* out,
+                             cudaStream_t st) {
+    k_sample_materials<<<div_up(n, 128), 128, 0, st>>>(sc, tex, maps, n, tri, odt, out);
+}
+// the maps' words of n triangles (reference order) into the fourth word of both texcoord record copies (ezrt_scene_set_material_maps)
+__global__ void k_maps_set(const uint32_t* __restrict__ words, const uint32_t* __restrict__ acc_tri_ref, int n, float4* rec, float4* acc_rec) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    rec[2 * (size_t)i + 1].w = __uint_as_float(words[i]);
+    if (acc_tri_ref) acc_rec[2 * (size_t)i + 1].w = __uint_as_float(words[acc_tri_ref[i]]);
+}
+void launch_maps_set(const uint32_t* words, const uint32_t* acc_tri_ref, int n, float4* rec, float4* acc_rec, cudaStream_t st) {
+    k_maps_set<<<div_up(n, 256), 256, 0, st>>>(words, acc_tri_ref, n, rec, acc_rec);
 }
 void launch_eval_math(int which, int n, const float* a, const float* b, float* out, cudaStream_t st) {
     k_eval_math<<<div_up(n, 256), 256, 0, st>>>(which, n, a, b, out);

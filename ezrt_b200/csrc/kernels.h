@@ -22,13 +22,15 @@
 //   trans_on  EZRT_PARAM_TRANSMISSION: materials with a dielectric lobe (<.., TRANS>)
 //   medium_on EZRT_PARAM_MEDIUM with sigma_t > 0: the homogeneous medium med (<.., MEDIUM>); never with trans_on
 //   tex_on    EZRT_PARAM_TEXTURES: the scene's base-colour textures tex (<.., TEX>)
+//   maps_on   EZRT_PARAM_MATERIAL_MAPS (with tex_on): the material maps of tex (<.., TEX, MAPS>)
 // All off outside the light sampling mode; the tables are zero where unused, as the kernels' parameters.
 struct LightOptions {
     LightsDev lights{};   // the light table (light sampling mode)
     EnvDev env{};         // the environment table (env_on)
     MediumDev med{};      // the medium (medium_on)
     TexDev tex{};         // the textures and the shadow slots' base colours (tex_on)
-    bool env_on = false, trans_on = false, medium_on = false, tex_on = false;
+    MapsDev maps{};       // the maps' table and the shadow slots' metallic (maps_on)
+    bool env_on = false, trans_on = false, medium_on = false, tex_on = false, maps_on = false;
 };
 
 // lens (EZRT_PARAM_THIN_LENS): the thin-lens camera rays (k_generate<true>); null: the pinhole's
@@ -106,6 +108,11 @@ void launch_tex_gather(const float4* rec, const uint32_t* acc_tri_ref, int n, fl
 // ezrt_scene_sample_textures: n (reference triangle, point) pairs -> uv (2 floats) and the textured base colour (3 floats) each
 void launch_sample_textures(const SceneDev& sc, const TexDev& tex, int n, const int32_t* tri, const float* points, float* uv, float* rgb,
                             cudaStream_t st);
+// ezrt_scene_sample_materials: n hits (reference triangle, o, d, t as 7 floats) -> 10 floats each (uv, base colour, roughness,
+// metallic, shading normal)
+void launch_sample_materials(const SceneDev& sc, const TexDev& tex, const MapsDev& maps, int n, const int32_t* tri, const float* odt, float* out, cudaStream_t st);
+// the maps' words (n, reference order) into the fourth word of rec[2 i + 1] and, with acc_tri_ref, of acc_rec[2 a + 1]
+void launch_maps_set(const uint32_t* words, const uint32_t* acc_tri_ref, int n, float4* rec, float4* acc_rec, cudaStream_t st);
 void launch_eval_math(int which, int n, const float* a, const float* b, float* out, cudaStream_t st);
 void launch_tonemap(const float* in, int channels, float* out, long long n, float limit, cudaStream_t st);
 void launch_partition_scatter(const float* compact, float* full, const TileDev* tiles, int n_tiles, int width, int channels,

@@ -351,3 +351,63 @@ def s_1m_bunny_textured(n_textures=2, builder=api.BVH_SAH_FAST):
     uv, ids = tl.encode_texcoords()
     eye, cam = api.camera_orbit(30.0, 25.0, 0.62 * max(15 * 1.2, 14 * 1.2) + 3.0)
     return tris, nodes, eye, cam, procedural_textures(n_textures), uv, ids
+
+
+def height_normal_map(seed=21, size=128, cells=8, strength=2.0):
+    """a tangent-space normal map for EZRT_PARAM_MATERIAL_MAPS (uint8 [size, size, 4], OpenGL +Y, linear): the finite differences of a
+    seeded periodic value-noise height field, so that the map tiles under wrap addressing"""
+    lat = np.random.default_rng(seed).uniform(0, 1, (cells + 1, cells + 1))
+    lat[-1, :], lat[:, -1] = lat[0, :], lat[:, 0]
+    ys, xs = np.meshgrid(np.arange(size) * cells / size, np.arange(size) * cells / size, indexing="ij")
+    iy, ix = ys.astype(int), xs.astype(int)
+    ty, tx = ys - iy, xs - ix
+    h = (lat[iy, ix] * (1 - tx) + lat[iy, ix + 1] * tx) * (1 - ty) + (lat[iy + 1, ix] * (1 - tx) + lat[iy + 1, ix + 1] * tx) * ty
+    dx = (np.roll(h, -1, axis=1) - np.roll(h, 1, axis=1)) * 0.5 * strength
+    dy = (np.roll(h, 1, axis=0) - np.roll(h, -1, axis=0)) * 0.5 * strength   # row 0 is the image's top: +v is -row
+    n = np.stack([-dx, -dy, np.ones_like(h)], axis=2)
+    n /= np.linalg.norm(n, axis=2, keepdims=True)
+    out = np.empty((size, size, 4), np.uint8)
+    out[:, :, :3] = np.clip(np.rint((n * 0.5 + 0.5) * 255.0), 0, 255)
+    out[:, :, 3] = 255
+    return out
+
+
+def noise_mr_map(seed=22, size=64, cells=4):
+    """a metallic-roughness map for EZRT_PARAM_MATERIAL_MAPS (uint8 [size, size, 4], linear, glTF's channels): R 0, G (the roughness
+    factor) and B (the metallic factor) seeded value noise"""
+    rng = np.random.default_rng(seed)
+    out = np.zeros((size, size, 4), np.uint8)
+    ys, xs = np.meshgrid(np.arange(size) * cells / size, np.arange(size) * cells / size, indexing="ij")
+    iy, ix = ys.astype(int), xs.astype(int)
+    ty, tx = ys - iy, xs - ix
+    for c in (1, 2):
+        lat = rng.uniform(0, 1, (cells + 1, cells + 1))
+        v = (lat[iy, ix] * (1 - tx) + lat[iy, ix + 1] * tx) * (1 - ty) + (lat[iy + 1, ix] * (1 - tx) + lat[iy + 1, ix + 1] * tx) * ty
+        out[:, :, c] = np.clip(np.rint(v * 255.0), 0, 255)
+    out[:, :, 3] = 255
+    return out
+
+
+def _with_maps(textured):
+    """a textured scene (s_*_textured's tuple) plus the two procedural maps appended to its textures and their ids: every textured
+    triangle takes both maps, except every 7th (no metallic-roughness map) and every 11th (no normal map); untextured ones (the
+    lights) none"""
+    tris, nodes, eye, cam, tex, uv, ids = textured
+    n = len(tex)
+    k = np.arange(len(ids))
+    on = ids >= 0
+    mr = np.where(on & (k % 7 != 0), n, -1).astype(np.int32)
+    nm = np.where(on & (k % 11 != 0), n + 1, -1).astype(np.int32)
+    return tris, nodes, eye, cam, tex + [noise_mr_map(), height_normal_map()], uv, ids, mr, nm
+
+
+def s_p3_bunny_mapped(n_textures=2, builder=api.BVH_SAH_FAST):
+    """s_p3_bunny_textured plus a seeded metallic-roughness map and a tangent-space normal map (EZRT_PARAM_MATERIAL_MAPS).  Returns
+    (tris, nodes, eye, cam, textures, texcoords, texture_id, metal_rough_id, normal_id); the geometry is s_p3_bunny_textured's byte for
+    byte, and the maps are the last two textures."""
+    return _with_maps(s_p3_bunny_textured(n_textures, builder))
+
+
+def s_1m_bunny_mapped(n_textures=2, builder=api.BVH_SAH_FAST):
+    """s_1m_bunny_textured plus the maps of s_p3_bunny_mapped"""
+    return _with_maps(s_1m_bunny_textured(n_textures, builder))

@@ -159,6 +159,18 @@ typedef struct ezrt_render_params {
    bit for bit.  Invalid (EZRT_ERR_INVALID) without textures set on the scene and in another mode.  Accepted by ezrt_render[_device],
    ezrt_render_adaptive[_device] and ezrt_render_aov[_device]; each shadow slot of a flagged render takes 16 bytes more. */
 #define EZRT_PARAM_TEXTURES 32
+/* ezrt_render_params.reserved[0], with EZRT_PARAM_TEXTURES (so in EZRT_MODE_DISNEY_LIGHTS on the wavefront pipeline only, with or
+   without EZRT_PARAM_ENV_LIGHT, EZRT_PARAM_TRANSMISSION, EZRT_PARAM_THIN_LENS and EZRT_PARAM_MEDIUM): the scene's material maps
+   (ezrt_scene_set_material_maps) are rendered.  At every surface hit but the last vertex, the metallic-roughness map (linear, glTF's
+   channels) scales the material's roughness by its G and its metallic by its B, and the tangent-space normal map (linear, OpenGL's +Y)
+   replaces the shading normal, in a per-triangle tangent frame from the triangle's edges and UV deltas (ezrt_math.h, DESIGN.md
+   section 16).  The mapped values are used wherever the render reads them: the BRDF and the transmission mixture (evaluation,
+   sampling, pdf, the lobe weights), the light samples' hemisphere tests and their evaluation after the shadow pass, the path's
+   cosine, and the feature buffers' normal.  The emission's MIS and the inside test keep the geometric normal.  No random number is
+   drawn.  Invalid (EZRT_ERR_INVALID) without EZRT_PARAM_TEXTURES or without maps set.  Accepted by ezrt_render[_device],
+   ezrt_render_adaptive[_device] and ezrt_render_aov[_device].  Each shadow slot of a render takes 81 bytes, 97 with
+   EZRT_PARAM_TEXTURES, 101 with EZRT_PARAM_MATERIAL_MAPS too. */
+#define EZRT_PARAM_MATERIAL_MAPS 64
 
 /* One texture of ezrt_scene_set_textures: width x height RGBA8 texels (4 bytes each, R first), row 0 the image's top row */
 typedef struct ezrt_texture {
@@ -230,6 +242,17 @@ int ezrt_scene_set_textures(ezrt_scene* scene, int n_textures, const ezrt_textur
  * interpolated UV) and rgb_out[3 i..] (the material's baseColor times the filtered texture; baseColor for texture id -1).  Host
  * arrays; synchronous.  EZRT_ERR_INVALID without textures set or for a triangle index out of range. */
 int ezrt_scene_sample_textures(ezrt_scene* scene, int n, const int32_t* tri, const float* points, float* uv_out, float* rgb_out);
+/* Sets the scene's material maps (EZRT_PARAM_MATERIAL_MAPS): per triangle, in the order of the `tris` array given to
+ * ezrt_scene_create, the id of its metallic-roughness map and of its normal map among the textures of ezrt_scene_set_textures (-1: no
+ * map).  Both NULL clears them.  Returns EZRT_ERR_INVALID without textures set, for exactly one NULL array, or for an id outside
+ * [-1, n_textures) or of 65535 or more; on every error the previous maps are kept.  ezrt_scene_set_textures (also clearing) clears the
+ * maps.  The call first waits for every render already enqueued on the scene's device, then writes the ids synchronously. */
+int ezrt_scene_set_material_maps(ezrt_scene* scene, const int32_t* metal_rough_id, const int32_t* normal_id);
+/* What the maps renders compute at n surface hits: reference triangle tri[i] hit by the ray hits[7 i..] = (o, d, t) -> out[10 i..] =
+ * (u, v, the textured base colour (3), the mapped roughness, the mapped metallic, the final shading normal (3), flipped for a hit from
+ * inside).  The maps set on the scene are used (none: the material's values and surface_hit's normal).  Host arrays; synchronous.
+ * EZRT_ERR_INVALID without textures set or for a triangle index out of range. */
+int ezrt_scene_sample_materials(ezrt_scene* scene, int n, const int32_t* tri, const float* hits, float* out);
 
 /* render(width,height,spp) -> framebuffer: equals `spp` consecutive display() calls
  * (P5/main.cpp:697-748) each drawing pass1 (P5/fsh:894-949) and copying to lastFrame.

@@ -826,4 +826,65 @@ EZ_HD void ez_tex_uv(float w1, float w2, float w3, const float* uv6, float* u, f
     *v = (w1 * uv6[1] + w2 * uv6[3]) + w3 * uv6[5];
 }
 
+/* ------------------------------------------------------------------ material maps (EZRT_PARAM_MATERIAL_MAPS, DESIGN.md section 16)
+ * Two more per-triangle texture ids into the textures of EZRT_PARAM_TEXTURES, looked up at the same UV as the base colour with
+ * ez_tex_sample(..., ez_unorm8_table): the maps are linear data (c / 255 in float64, rounded to fp32), not sRGB.  Id -1: no map.
+ * Metallic-roughness map (glTF's channels): roughness = mat.roughness * G, metallic = mat.metallic * B (ez_mr_apply).
+ * Normal map (tangent space, OpenGL +Y), ez_normal_map; N is surface_hit's shading normal, No = N, negated for a hit from inside:
+ *   e1 = p2 - p1, e2 = p3 - p1, (du1, dv1) = uv2 - uv1, (du2, dv2) = uv3 - uv1, det = du1 dv2 - du2 dv1;
+ *   T = (dv2 e1 - dv1 e2) / det, B_uv = (du1 e2 - du2 e1) / det (each component: (a x - b y) / det);
+ *   T' = normalize(T - dot(No, T) No), B = cross(No, T'), negated when dot(B, B_uv) < 0;
+ *   n_t = 2 f - 1 per channel of the filtered colour f; n = normalize((n_t.x T' + n_t.y B) + n_t.z No), negated for a hit from inside.
+ *   N itself, bit for bit, when u or v is not finite, det is 0 or not finite, dot(T - dot(No, T) No, itself) is 0 or not finite,
+ *   dot(B, B_uv) is 0 or not finite, n is not finite, or dot(n, V) <= 0 (the view stays on the shading side) -- in that order.
+ * The tangent is per triangle (not MikkTSpace): maps baked against smooth per-vertex tangents show faint seams between facets. */
+static const float ez_unorm8_table[256] = {
+#include "ezrt_unorm8_table.inc"
+};
+/* the metallic-roughness map's filtered colour f applied to a material's roughness and metallic */
+EZ_HD void ez_mr_apply(ez_vec3 f, float* roughness, float* metallic) {
+    *roughness = *roughness * f.y;
+    *metallic = *metallic * f.z;
+}
+EZ_HD int ez_finite3(ez_vec3 v) { return ez_finite(v.x) && ez_finite(v.y) && ez_finite(v.z); }
+/* (a x - b y) / det per component */
+EZ_HD ez_vec3 ez_tangent_comb(float a, ez_vec3 x, float b, ez_vec3 y, float det) {
+    return ez_divs(ez_sub(ez_scale(x, a), ez_scale(y, b)), det);
+}
+/* the triangle's tangent frame (T', B) about the unflipped shading normal No; 0 when it falls back */
+EZ_HD int ez_tangent_frame(ez_vec3 p1, ez_vec3 p2, ez_vec3 p3, const float* uv6, ez_vec3 No, ez_vec3* T, ez_vec3* B) {
+    const ez_vec3 e1 = ez_sub(p2, p1), e2 = ez_sub(p3, p1);
+    const float du1 = uv6[2] - uv6[0], dv1 = uv6[3] - uv6[1], du2 = uv6[4] - uv6[0], dv2 = uv6[5] - uv6[1];
+    const float det = du1 * dv2 - du2 * dv1;
+    if (det == 0.0f || !ez_finite(det)) return 0;
+    const ez_vec3 Tu = ez_tangent_comb(dv2, e1, dv1, e2, det);
+    const ez_vec3 Bu = ez_tangent_comb(du1, e2, du2, e1, det);
+    const ez_vec3 Tp = ez_sub(Tu, ez_scale(No, ez_dot(No, Tu)));
+    const float l2 = ez_dot(Tp, Tp);
+    if (l2 == 0.0f || !ez_finite(l2)) return 0;
+    *T = ez_normalize(Tp);
+    ez_vec3 b = ez_cross(No, *T);
+    const float s = ez_dot(b, Bu);
+    if (s == 0.0f || !ez_finite(s)) return 0;
+    *B = (s < 0.0f) ? ez_neg(b) : b;
+    return 1;
+}
+/* the mapped shading normal of a hit at (u, v) on (p1, p2, p3) with the triangle's UVs uv6: f the normal map's filtered colour, N
+ * surface_hit's shading normal, inside the hit's side, V = -d */
+EZ_HD ez_vec3 ez_normal_map(ez_vec3 p1, ez_vec3 p2, ez_vec3 p3, const float* uv6, float u, float v, ez_vec3 f, ez_vec3 N, int inside, ez_vec3 V) {
+    if (!ez_finite(u) || !ez_finite(v)) return N;
+    const ez_vec3 No = inside ? ez_neg(N) : N;
+    ez_vec3 T, B;
+    if (!ez_tangent_frame(p1, p2, p3, uv6, No, &T, &B)) return N;
+    const float tx = 2.0f * f.x - 1.0f, ty = 2.0f * f.y - 1.0f, tz = 2.0f * f.z - 1.0f;
+    ez_vec3 n = ez_normalize(ez_add(ez_add(ez_scale(T, tx), ez_scale(B, ty)), ez_scale(No, tz)));
+    if (!ez_finite3(n)) return N;
+    if (inside) n = ez_neg(n);
+    if (!(ez_dot(n, V) > 0.0f)) return N;
+    return n;
+}
+/* the material-maps word of a texcoord record (its fourth float's bits): (metal_rough_id + 1) | (normal_id + 1) << 16 */
+EZ_HD int ez_maps_mr_id(uint32_t w) { return (int)(w & 0xffffu) - 1; }
+EZ_HD int ez_maps_normal_id(uint32_t w) { return (int)(w >> 16) - 1; }
+
 #endif /* EZRT_MATH_H */
