@@ -2055,7 +2055,7 @@ int ezrt_accel_build(int device, const float* tris, int n_triangles, int leaf_n,
 }
 
 int ezrt_eval_math(int device, int which, int n, const float* a, const float* b, float* out) {
-    if (n < 0 || !a || !out || which < 0 || which > 6) return ezrt_set_error(EZRT_ERR_INVALID, "eval_math: bad argument");
+    if (n < 0 || !a || !out || which < 0 || which > 7) return ezrt_set_error(EZRT_ERR_INVALID, "eval_math: bad argument");
     if (n == 0) return EZRT_OK;
     CU_CHECK(cudaSetDevice(device));
     DeviceBuffer buf;

@@ -1752,19 +1752,14 @@ __device__ __forceinline__ vec3 texel3(const float* img, int idx) {
     const float* p = img + (size_t)idx * 3;
     return ez_v3(__ldg(p), __ldg(p + 1), __ldg(p + 2));
 }
-__device__ __forceinline__ int clampi(int v, int hi) { return v < 0 ? 0 : (v > hi ? hi : v); }
 __device__ __forceinline__ vec3 tex2d(const float* img, int W, int H, float u, float v, int linear) {
-    if (!linear) {
-        int ix = clampi((int)ez_floor(u * (float)W), W - 1), iy = clampi((int)ez_floor(v * (float)H), H - 1);
-        return texel3(img, iy * W + ix);
-    }
+    if (!linear) return texel3(img, ez_env_texel(u, v, W, H));
     float x = u * (float)W - 0.5f, y = v * (float)H - 0.5f;
     float fx0 = ez_floor(x), fy0 = ez_floor(y);
     float ax = x - fx0, ay = y - fy0;
-    int x0 = (int)fx0, y0 = (int)fy0;
-    int x1 = clampi(x0 + 1, W - 1), y1 = clampi(y0 + 1, H - 1);
-    x0 = clampi(x0, W - 1);
-    y0 = clampi(y0, H - 1);
+    // indices clamped in float: a NaN coordinate reads texel 0 and weighs it by NaN
+    const int x0 = ez_texel_clamp(fx0, W), x1 = ez_texel_clamp(fx0 + 1.0f, W);
+    const int y0 = ez_texel_clamp(fy0, H), y1 = ez_texel_clamp(fy0 + 1.0f, H);
     vec3 t00 = texel3(img, y0 * W + x0), t10 = texel3(img, y0 * W + x1);
     vec3 t01 = texel3(img, y1 * W + x0), t11 = texel3(img, y1 * W + x1);
     return ez_vmix(ez_vmix(t00, t10, ax), ez_vmix(t01, t11, ax), ay);

@@ -1111,6 +1111,7 @@ __global__ void k_eval_math(int which, int n, const float* a, const float* b, fl
         case 4: r = ez_pow(x, y); break;
         case 5: r = ez_atan2(x, y); break;
         case 6: r = ez_asin(x); break;
+        case 7: r = ez_floor(x); break;
     }
     out[i] = r;
 }

@@ -406,7 +406,7 @@ int ezrt_camera_rays(ezrt_scene* scene, const ezrt_render_params* params, int n,
                      const uint32_t* frame, float* origins_out, float* dirs_out);
 
 /* Evaluate a ezrt_math.h function on the device for n inputs (parity of the arithmetic
- * definition): which = 0 sin, 1 cos, 2 log, 3 exp, 4 pow(a,b), 5 atan2(a,b), 6 asin. */
+ * definition): which = 0 sin, 1 cos, 2 log, 3 exp, 4 pow(a,b), 5 atan2(a,b), 6 asin, 7 floor. */
 int ezrt_eval_math(int device, int which, int n, const float* a, const float* b, float* out);
 
 /* The binary SAH tree ezrt_scene_create derives its acceleration tree from (NOT the reference's tree: the same

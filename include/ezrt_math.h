@@ -72,10 +72,18 @@ EZ_HD float ez_clamp(float x, float lo, float hi) { return ez_min(ez_max(x, lo),
 /* GLSL mix(x,y,a) = x*(1-a) + y*a */
 EZ_HD float ez_mix(float x, float y, float a) { return x * (1.0f - a) + y * a; }
 EZ_HD float ez_sqr(float x) { return x * x; }
-/* floor for |x| < 2^31 */
+/* floor, exact for every input: NaN, +-inf and every |x| >= 2^23 are whole already and return themselves (no conversion to int
+ * out of its range, which the host leaves undefined and the device saturates); floor(-0) = +0 */
 EZ_HD float ez_floor(float x) {
+    if (!(ez_abs(x) < 8388608.0f)) return x;
     float t = (float)(int)x;
     return (t > x) ? (t - 1.0f) : t;
+}
+/* a texel index in [0, n): f a whole number (ez_floor's result) or NaN, clamped in float before the conversion, so that NaN and
+ * f < 0 give 0 and f > n - 1 gives n - 1 for every f */
+EZ_HD int ez_texel_clamp(float f, int n) {
+    const int i = (f > 0.0f) ? (int)ez_min(f, 2147483520.0f) : 0;
+    return (i > n - 1) ? n - 1 : i;
 }
 /* uint -> float, round to nearest even (GLSL float(uint)) */
 EZ_HD float ez_u32_to_float(uint32_t u) {
@@ -447,10 +455,7 @@ EZ_HD ez_vec3 ez_env_sample(const float* row_cdf, const float* col_cdf, int W, i
 }
 /* the texel tex2d's nearest lookup reads at (u, v) */
 EZ_HD int ez_env_texel(float u, float v, int W, int H) {
-    int ix = (int)ez_floor(u * (float)W), iy = (int)ez_floor(v * (float)H);
-    ix = (ix < 0) ? 0 : ((ix > W - 1) ? W - 1 : ix);
-    iy = (iy < 0) ? 0 : ((iy > H - 1) ? H - 1 : iy);
-    return iy * W + ix;
+    return ez_texel_clamp(ez_floor(v * (float)H), H) * W + ez_texel_clamp(ez_floor(u * (float)W), W);
 }
 /* solid-angle density of ez_env_sample at direction L: texel_pdf * W * H / (2 pi^2 cos e), 0 if the texel's pdf or cos e is 0 */
 EZ_HD float ez_env_pdf(const float* texel_pdf, int W, int H, ez_vec3 L) {
@@ -768,7 +773,7 @@ EZ_HD ez_vec3 ez_hg_sample(ez_vec3 d, float g, float h_1, float h_2) {
  *   the image's top row, OBJ's v = 0 its bottom); x0 = floor(x), weight x - x0, x0 and x0 + 1 reduced modulo W (s may round to
  *   1.0); the same for y.  Texels are RGBA8 (alpha ignored), each channel decoded by ez_srgb_table (the sRGB EOTF in float64, rounded
  *   to fp32), then filtered bilinearly with lerp(a, b, f) = a + (b - a) f, so that four equal texels give that texel exactly.  A
- *   non-finite u or v gives exactly (1, 1, 1). */
+ *   non-finite u or v gives exactly (1, 1, 1); every finite |u| >= 2^23 is whole, so s = 0 there and the texel indices stay in range. */
 static const float ez_srgb_table[256] = {
 #include "ezrt_srgb_table.inc"
 };

@@ -555,20 +555,13 @@ inline float misMixWeight(float a, float b) {
 // ---------------------------------------------------------------- textures
 // texture2D on an RGB32F W x H image with CLAMP_TO_EDGE; row 0 <-> v = 0.
 vec3 tex2D(const float* img, int W, int H, float u, float v, bool linear) {
-    if (!linear) {  // GL_NEAREST
-        int ix = (int)ez_floor(u * (float)W), iy = (int)ez_floor(v * (float)H);
-        if (ix < 0) ix = 0; if (ix > W - 1) ix = W - 1;
-        if (iy < 0) iy = 0; if (iy > H - 1) iy = H - 1;
-        return texel(img, iy * W + ix);
-    }
+    if (!linear) return texel(img, ez_env_texel(u, v, W, H));  // GL_NEAREST
     float x = u * (float)W - 0.5f, y = v * (float)H - 0.5f;
     float fx0 = ez_floor(x), fy0 = ez_floor(y);
     float ax = x - fx0, ay = y - fy0;
-    int x0 = (int)fx0, y0 = (int)fy0, x1 = x0 + 1, y1 = y0 + 1;
-    if (x0 < 0) x0 = 0; if (x0 > W - 1) x0 = W - 1;
-    if (x1 < 0) x1 = 0; if (x1 > W - 1) x1 = W - 1;
-    if (y0 < 0) y0 = 0; if (y0 > H - 1) y0 = H - 1;
-    if (y1 < 0) y1 = 0; if (y1 > H - 1) y1 = H - 1;
+    // indices clamped in float: a NaN coordinate reads texel 0 and weighs it by NaN
+    const int x0 = ez_texel_clamp(fx0, W), x1 = ez_texel_clamp(fx0 + 1.0f, W);
+    const int y0 = ez_texel_clamp(fy0, H), y1 = ez_texel_clamp(fy0 + 1.0f, H);
     vec3 t00 = texel(img, y0 * W + x0), t10 = texel(img, y0 * W + x1);
     vec3 t01 = texel(img, y1 * W + x0), t11 = texel(img, y1 * W + x1);
     return ez_vmix(ez_vmix(t00, t10, ax), ez_vmix(t01, t11, ax), ay);
@@ -934,7 +927,7 @@ int oracle_eval_brdf(int which, int n, const float* Vv, const float* Nn, const f
     return 0;
 }
 
-// which: 0 sin, 1 cos, 2 log, 3 exp, 4 pow, 5 atan2, 6 asin
+// which: 0 sin, 1 cos, 2 log, 3 exp, 4 pow, 5 atan2, 6 asin, 7 floor
 int oracle_eval_math(int which, int n, const float* a, const float* b, float* out) {
     for (int i = 0; i < n; i++) {
         float x = a[i], y = b ? b[i] : 0.0f, r;
@@ -946,6 +939,7 @@ int oracle_eval_math(int which, int n, const float* a, const float* b, float* ou
             case 4: r = ez_pow(x, y); break;
             case 5: r = ez_atan2(x, y); break;
             case 6: r = ez_asin(x); break;
+            case 7: r = ez_floor(x); break;
             default: return -1;
         }
         out[i] = r;

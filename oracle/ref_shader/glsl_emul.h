@@ -140,18 +140,17 @@ inline vec3 texel2D(const sampler2D& s, int ix, int iy) {
     const float* p = s.img + ((long long)iy * s.w + ix) * s.channels;
     return vec3(p[0], p[1], p[2]);
 }
-inline int clampi(int v, int hi) { return v < 0 ? 0 : (v > hi ? hi : v); }
 inline vec4 texture2D(const sampler2D& s, vec2 uv) {
     if (s.filter == 0) {
-        int ix = clampi((int)ez_floor(uv.x * (float)s.w), s.w - 1);
-        int iy = clampi((int)ez_floor(uv.y * (float)s.h), s.h - 1);
+        int ix = ez_texel_clamp(ez_floor(uv.x * (float)s.w), s.w);
+        int iy = ez_texel_clamp(ez_floor(uv.y * (float)s.h), s.h);
         return vec4(texel2D(s, ix, iy), 1.0f);
     }
     float x = uv.x * (float)s.w - 0.5f, y = uv.y * (float)s.h - 0.5f;
     float fx0 = ez_floor(x), fy0 = ez_floor(y);
     float ax = x - fx0, ay = y - fy0;
-    int x0 = clampi((int)fx0, s.w - 1), x1 = clampi((int)fx0 + 1, s.w - 1);
-    int y0 = clampi((int)fy0, s.h - 1), y1 = clampi((int)fy0 + 1, s.h - 1);
+    int x0 = ez_texel_clamp(fx0, s.w), x1 = ez_texel_clamp(fx0 + 1.0f, s.w);
+    int y0 = ez_texel_clamp(fy0, s.h), y1 = ez_texel_clamp(fy0 + 1.0f, s.h);
     vec3 t00 = texel2D(s, x0, y0), t10 = texel2D(s, x1, y0), t01 = texel2D(s, x0, y1), t11 = texel2D(s, x1, y1);
     return vec4(mix(mix(t00, t10, ax), mix(t01, t11, ax), ay), 1.0f);
 }

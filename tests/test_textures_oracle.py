@@ -62,11 +62,14 @@ def test_c_table_equals_the_committed_one():
 def test_c_filter_matches_the_float64_model():
     from tests import oracle_textures as ot
     rng = np.random.default_rng(4)
-    for h, w in ((1, 1), (1, 9), (7, 1), (3, 5), (17, 13), (64, 64)):
+    # beyond 2^23 every float is a whole number: s = t = 0 up to FLT_MAX, past 2^31 and int's range included
+    huge = np.array([2.0 ** 31 - 128, 2.0 ** 31, -2.0 ** 31, 3e9, -3e9, 2.0 ** 40, -2.0 ** 40, 3.4028235e38, -3.4028235e38, 0.25], np.float32)
+    for h, w in ((1, 1), (1, 9), (7, 1), (3, 5), (17, 13), (64, 64), (1, 16384)):
         t = rng.integers(0, 256, (h, w, 4)).astype(np.uint8)
         uv = np.concatenate([rng.uniform(-5, 5, (300, 2)),
                              np.array([[0, 0], [1, 1], [-1e-9, 1 - 1e-8], [-0.5, 2.5], [8388608, -8388609], [3e7, -3e7], [0.9999999, 1e-30],
-                                       [-1e-30, -0.9999999]])]).astype(np.float32)
+                                       [-1e-30, -0.9999999]]),
+                             np.stack(np.meshgrid(huge, huge), axis=-1).reshape(-1, 2)]).astype(np.float32)
         got = ot.tex_sample(t, uv)
         want = np.array([sample64(t, u, v) for u, v in uv])
         assert np.allclose(got, want, rtol=1e-5, atol=max(w, h) * 1e-6), (h, w)
