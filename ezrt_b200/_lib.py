@@ -48,6 +48,12 @@ class Texture(C.Structure):
     _fields_ = [("width", C.c_int32), ("height", C.c_int32), ("rgba", C.c_void_p), ("reserved", C.c_int32)]
 
 
+class PunctualLight(C.Structure):
+    """struct ezrt_punctual_light (include/ezrt.h)."""
+    _fields_ = [("type", C.c_int32), ("position", C.c_float * 3), ("direction", C.c_float * 3), ("color", C.c_float * 3),
+                ("intensity", C.c_float), ("inner_cone", C.c_float), ("outer_cone", C.c_float), ("reserved", C.c_int32)]
+
+
 class Counters(C.Structure):
     """struct ezrt_counters (include/ezrt.h)."""
     _fields_ = [
@@ -70,6 +76,8 @@ SIGNATURES = {
     "ezrt_scene_sample_textures": (C.c_int, [C.c_void_p, C.c_int, c_int32_p, c_float_p, c_float_p, c_float_p]),
     "ezrt_scene_set_material_maps": (C.c_int, [C.c_void_p, c_int32_p, c_int32_p]),
     "ezrt_scene_sample_materials": (C.c_int, [C.c_void_p, C.c_int, c_int32_p, c_float_p, c_float_p]),
+    "ezrt_scene_set_punctual_lights": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(PunctualLight)]),
+    "ezrt_scene_punctual_lights": (C.c_int, [C.c_void_p, C.c_int, c_int32_p, c_float_p, c_float_p, C.POINTER(C.c_double)]),
     "ezrt_render": (C.c_int, [C.c_void_p, C.POINTER(RenderParams), c_float_p]),
     "ezrt_render_device": (C.c_int, [C.c_void_p, C.POINTER(RenderParams), C.c_void_p, C.c_void_p]),
     "ezrt_render_adaptive_device": (C.c_int, [C.c_void_p, C.POINTER(RenderParams), C.POINTER(AdaptiveParams), C.c_void_p, C.c_void_p,

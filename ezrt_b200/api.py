@@ -26,6 +26,8 @@ PARAM_THIN_LENS = 8
 PARAM_MEDIUM = 16
 PARAM_TEXTURES = 32
 PARAM_MATERIAL_MAPS = 64
+PARAM_PUNCTUAL_LIGHTS = 128
+PUNCTUAL_POINT, PUNCTUAL_SPOT, PUNCTUAL_DIRECTIONAL = 0, 1, 2   # ezrt_punctual_light.type
 MODES = {"diffuse_p3": 0, "disney_aniso_p4": 1, "disney_sobol_p5": 2, "disney_is_mis_p5": 3, "disney_lights": 4}
 
 TRAVERSE_ACCEL = 0
@@ -252,6 +254,7 @@ class RenderConfig:
     medium: bool = False        # EZRT_PARAM_MEDIUM (MODE_DISNEY_LIGHTS only): the scene's homogeneous medium (Scene.set_medium, DESIGN.md section 14)
     textures: bool = False      # EZRT_PARAM_TEXTURES (MODE_DISNEY_LIGHTS only): the scene's base-colour textures (Scene.set_textures, DESIGN.md section 15)
     material_maps: bool = False  # EZRT_PARAM_MATERIAL_MAPS (with textures): the scene's material maps (Scene.set_material_maps, DESIGN.md section 16)
+    punctual_lights: bool = False  # EZRT_PARAM_PUNCTUAL_LIGHTS (MODE_DISNEY_LIGHTS only): the scene's punctual lights (Scene.set_punctual_lights, DESIGN.md section 17)
 
     def to_struct(self):
         p = RenderParams()
@@ -265,13 +268,49 @@ class RenderConfig:
         p.profile = int(self.profile)
         p.reserved[0] = ((PARAM_ACCUMULATE if self.accumulate else 0) | (PARAM_ENV_LIGHT if self.env_light else 0) |
                          (PARAM_TRANSMISSION if self.transmission else 0) | (PARAM_MEDIUM if self.medium else 0) |
-                         (PARAM_TEXTURES if self.textures else 0) | (PARAM_MATERIAL_MAPS if self.material_maps else 0))
+                         (PARAM_TEXTURES if self.textures else 0) | (PARAM_MATERIAL_MAPS if self.material_maps else 0) |
+                         (PARAM_PUNCTUAL_LIGHTS if self.punctual_lights else 0))
         if self.lens_radius != 0:   # a negative or NaN radius is set too, so that the library rejects it
             if self.focus_distance is None:
                 raise ValueError("RenderConfig: a lens (lens_radius != 0) needs a focus_distance")
             p.reserved[0] |= PARAM_THIN_LENS
             p.reserved[1], p.reserved[2] = (int(x) for x in np.array([self.lens_radius, self.focus_distance], np.float32).view(np.int32))
         return p
+
+
+def _punctual(type_, position=(0.0, 0.0, 0.0), direction=(0.0, 0.0, 0.0), color=(1.0, 1.0, 1.0), intensity=1.0, inner_cone=0.0,
+              outer_cone=0.0):
+    l = _lib.PunctualLight()
+    l.type, l.intensity, l.inner_cone, l.outer_cone, l.reserved = int(type_), float(intensity), float(inner_cone), float(outer_cone), 0
+    l.position[:] = [float(x) for x in position]
+    l.direction[:] = [float(x) for x in direction]
+    l.color[:] = [float(x) for x in color]
+    return l
+
+
+def point_light(position, color=(1.0, 1.0, 1.0), intensity=1.0):
+    """A point light of Scene.set_punctual_lights (struct ezrt_punctual_light): intensity is radiant intensity in the render's units."""
+    return _punctual(PUNCTUAL_POINT, position=position, color=color, intensity=intensity)
+
+
+def spot_light(position, direction, color=(1.0, 1.0, 1.0), intensity=1.0, inner_cone=0.0, outer_cone=np.pi / 4):
+    """A spot light pointing along direction, with glTF's falloff between the cones (radians, 0 <= inner < outer <= pi/2)."""
+    return _punctual(PUNCTUAL_SPOT, position=position, direction=direction, color=color, intensity=intensity, inner_cone=inner_cone,
+                     outer_cone=outer_cone)
+
+
+def directional_light(direction, color=(1.0, 1.0, 1.0), intensity=1.0):
+    """A directional (sun) light travelling along direction; intensity is irradiance in the render's units."""
+    return _punctual(PUNCTUAL_DIRECTIONAL, direction=direction, color=color, intensity=intensity)
+
+
+def punctual_array(lights):
+    """struct ezrt_punctual_light[len(lights)] of a sequence of point_light / spot_light / directional_light values"""
+    lights = list(lights)
+    arr = (_lib.PunctualLight * max(1, len(lights)))()
+    for k, l in enumerate(lights):
+        arr[k] = l
+    return arr, len(lights)
 
 
 def adaptive_params(threshold, min_spp, check_interval):
@@ -385,6 +424,25 @@ class Scene:
         mr = np.ascontiguousarray(np.asarray(metal_rough_id, np.int32).reshape(n))
         nm = np.ascontiguousarray(np.asarray(normal_id, np.int32).reshape(n))
         check(lib.ezrt_scene_set_material_maps(self._h, mr.ctypes.data_as(C.POINTER(C.c_int32)), nm.ctypes.data_as(C.POINTER(C.c_int32))))
+
+    def set_punctual_lights(self, lights):
+        """ezrt_scene_set_punctual_lights: the punctual lights RenderConfig.punctual_lights renders (DESIGN.md section 17), a sequence of
+        point_light / spot_light / directional_light values.  set_punctual_lights(None) clears them.  The call waits for the renders
+        already enqueued on the device."""
+        if lights is None:
+            check(lib.ezrt_scene_set_punctual_lights(self._h, 0, None))
+            return
+        arr, n = punctual_array(lights)
+        check(lib.ezrt_scene_set_punctual_lights(self._h, n, arr))
+
+    def punctual_light_table(self):
+        """The punctual lights' table (ezrt_scene_punctual_lights): (each light's index among the lights set int32 [J], cdf float32 [J],
+        selection probabilities q float32 [J], W = float64 sum of the weights)."""
+        j = check(lib.ezrt_scene_punctual_lights(self._h, 0, None, None, None, None))
+        idx, cdf, q = np.zeros(j, np.int32), np.zeros(j, np.float32), np.zeros(j, np.float32)
+        total = C.c_double(0.0)
+        check(lib.ezrt_scene_punctual_lights(self._h, j, idx.ctypes.data_as(_lib.c_int32_p), _fp(cdf), _fp(q), C.byref(total)))
+        return idx, cdf, q, total.value
 
     def sample_materials(self, tri, o, d, t):
         """ezrt_scene_sample_materials: what the maps renders compute at hits of reference triangles tri ([n]) by rays (o [n, 3], d [n, 3],

@@ -286,6 +286,25 @@ def build_oracle_material_maps(force=False):
     return ORACLE_MATERIAL_MAPS_SO
 
 
+ORACLE_PUNCTUAL_SO = os.path.join(ROOT, "build", "libezrt_oracle_punctual.so")
+
+
+def build_oracle_punctual(force=False):
+    """build/libezrt_oracle_punctual.so: tests/oracle_punctual.cpp, the CPU restatement of the punctual lights (the table, the sample,
+    the flagged render's medium and transmission loops with the category split) over the material maps' restatement (test
+    infrastructure, loaded only by tests/oracle_punctual.py)."""
+    src = os.path.join(ROOT, "tests", "oracle_punctual.cpp")
+    deps = [src] + [os.path.join(ROOT, "tests", f) for f in ("oracle_material_maps.cpp", "oracle_textures.cpp", "oracle_medium.cpp", "oracle_lens.cpp",
+                                                              "oracle_transmission.cpp", "oracle_env_light.cpp", "oracle_lights.cpp")] + \
+        [os.path.join(ROOT, "oracle", "ezrt_oracle.cpp")] + [os.path.join(INCLUDE, f) for f in os.listdir(INCLUDE)]
+    if force or _newer(ORACLE_PUNCTUAL_SO, deps):
+        os.makedirs(os.path.dirname(ORACLE_PUNCTUAL_SO), exist_ok=True)
+        tmp = ORACLE_PUNCTUAL_SO + ".tmp%d" % os.getpid()
+        _run(["g++"] + HOST_FLAGS + ["-fopenmp", "-Wno-misleading-indentation", "-shared", "-I", INCLUDE, src, "-o", tmp])
+        os.replace(tmp, ORACLE_PUNCTUAL_SO)
+    return ORACLE_PUNCTUAL_SO
+
+
 def build_reference_hdrloader(force=False):
     return _oracle_recipes().build_reference_hdrloader(force)
 
@@ -353,6 +372,7 @@ def build_all(force=False, verbose=False):
     build_oracle_medium(force=force)
     build_oracle_textures(force=force)
     build_oracle_material_maps(force=force)
+    build_oracle_punctual(force=force)
     build_example(force=force)
     build_reference_hdrloader(force=force)
     build_reference_shaders(force=force)

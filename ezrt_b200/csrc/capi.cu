@@ -21,6 +21,7 @@
 #include "ezrt.h"
 #include "ezrt_internal.h"
 #include "ezrt_math.h"
+#include "ezrt_punctual.h"
 #include "kernels.h"
 #include "w8_node.h"
 
@@ -116,6 +117,13 @@ struct ezrt_scene {
     int n_textures = 0;
     TexDev tex{};
     MapsDev maps{};   // maps.sh_metal is set per render
+    // the punctual lights of EZRT_PARAM_PUNCTUAL_LIGHTS (ezrt_scene_set_punctual_lights): the table (ezrt_punctual.h) and its device
+    // copy, records | cdf; punct.p_p is set per render
+    bool has_punct = false;
+    EzPunctTable punct_table;
+    DeviceBuffer punct_buf;
+    PunctDev punct{};
+    float vbox_min[3] = {0, 0, 0}, vbox_max[3] = {0, 0, 0};   // the triangles' vertex box (the directional lights' weight)
     void* hot_base = nullptr;   // accel nodes | geometry (| vertices) | shading records (L2 persisting window)
     size_t hot_bytes = 0;
     size_t l2_persist_bytes = 0;
@@ -228,6 +236,12 @@ int validate_params(const ezrt_scene* scene, const ezrt_render_params* p) {
         if (!(p->reserved[0] & EZRT_PARAM_TEXTURES))
             return ezrt_set_error(EZRT_ERR_INVALID, "render: EZRT_PARAM_MATERIAL_MAPS needs EZRT_PARAM_TEXTURES");
         if (!scene->has_maps) return ezrt_set_error(EZRT_ERR_INVALID, "render: EZRT_PARAM_MATERIAL_MAPS needs maps (ezrt_scene_set_material_maps)");
+    }
+    if (p->reserved[0] & EZRT_PARAM_PUNCTUAL_LIGHTS) {
+        if (p->mode != EZRT_MODE_DISNEY_LIGHTS)
+            return ezrt_set_error(EZRT_ERR_INVALID, "render: EZRT_PARAM_PUNCTUAL_LIGHTS needs the light sampling mode (got mode %d)", p->mode);
+        if (!scene->has_punct)
+            return ezrt_set_error(EZRT_ERR_INVALID, "render: EZRT_PARAM_PUNCTUAL_LIGHTS needs punctual lights (ezrt_scene_set_punctual_lights)");
     }
     if (p->max_bounce < 0 || p->max_bounce > 64) return ezrt_set_error(EZRT_ERR_INVALID, "render: max_bounce out of range");
     if (p->out_channels != 3 && p->out_channels != 4) return ezrt_set_error(EZRT_ERR_INVALID, "render: out_channels must be 3 or 4");
@@ -878,6 +892,8 @@ int ezrt_scene_create(int device, const float* tris, int n_triangles, const floa
     }
     d.prune_delta = prune_delta;  // 2^-16 * scene extent (DESIGN.md "pruning")
     for (int k = 0; k < 3; k++) {
+        sc->vbox_min[k] = bmin[k];
+        sc->vbox_max[k] = bmax[k];
         d.bmin[k] = bmin[k];
         float ext = bmax[k] - bmin[k];
         d.cell_scale[k] = (ext > 0.0f) ? 32.0f / ext : 0.0f;
@@ -1025,6 +1041,67 @@ int ezrt_scene_set_textures(ezrt_scene* s, int n_textures, const ezrt_texture* t
     return EZRT_OK;
 }
 
+int ezrt_scene_set_punctual_lights(ezrt_scene* s, int n, const ezrt_punctual_light* lights) {
+    if (!s) return ezrt_set_error(EZRT_ERR_INVALID, "scene_set_punctual_lights: null scene");
+    CU_CHECK(cudaSetDevice(s->device));
+    if (!lights) {
+        CU_CHECK(cudaDeviceSynchronize());   // renders already enqueued still read the buffer
+        s->punct_buf.release();
+        s->has_punct = false;
+        s->punct_table = EzPunctTable{};
+        s->punct = PunctDev{};
+        return EZRT_OK;
+    }
+    if (n < 0) return ezrt_set_error(EZRT_ERR_INVALID, "scene_set_punctual_lights: n = %d", n);
+    EzPunctTable t;
+    const char* why = "";
+    try {
+        const int bad = ez_punct_build(n, lights, s->vbox_min, s->vbox_max, &t, &why);
+        if (bad >= 0) return ezrt_set_error(EZRT_ERR_INVALID, "scene_set_punctual_lights: light %d has %s", bad, why);
+    } catch (const std::bad_alloc&) {
+        return ezrt_set_error(EZRT_ERR_NOMEM, "scene_set_punctual_lights: host staging of %d lights", n);
+    }
+    const int J = (int)t.index.size();
+    // the new buffer is filled before the previous one is released, so that a failure keeps the previous lights
+    DeviceBuffer nbuf;
+    PunctDev d{};
+    if (J > 0) {
+        const size_t rec_bytes = sizeof(float) * t.rec.size();
+        int rc = nbuf.ensure(rec_bytes + sizeof(float) * (size_t)J);
+        if (rc) return rc;
+        cudaError_t e = cudaDeviceSynchronize();   // renders already enqueued still read the previous buffer
+        if (e == cudaSuccess) e = cudaMemcpy(nbuf.p, t.rec.data(), rec_bytes, cudaMemcpyHostToDevice);
+        if (e == cudaSuccess) e = cudaMemcpy((char*)nbuf.p + rec_bytes, t.cdf.data(), sizeof(float) * (size_t)J, cudaMemcpyHostToDevice);
+        if (e != cudaSuccess) {
+            nbuf.release();
+            return ezrt_set_error(EZRT_ERR_CUDA, "scene_set_punctual_lights: %s", cudaGetErrorString(e));
+        }
+        d.rec = (const float4*)nbuf.p;
+        d.cdf = (const float*)((const char*)nbuf.p + rec_bytes);
+        d.n = J;
+    } else {
+        CU_CHECK(cudaDeviceSynchronize());
+    }
+    s->punct_buf.release();
+    s->punct_buf = nbuf;   // DeviceBuffer frees only on release(): the pointer moves to the scene
+    s->punct = d;
+    s->punct_table = t;
+    s->has_punct = true;
+    return EZRT_OK;
+}
+
+int ezrt_scene_punctual_lights(ezrt_scene* s, int cap, int32_t* index_out, float* cdf_out, float* q_out, double* total_out) {
+    if (!s || cap < 0) return ezrt_set_error(EZRT_ERR_INVALID, "scene_punctual_lights: bad argument");
+    const EzPunctTable& t = s->punct_table;
+    const int J = (int)t.index.size();
+    const int m = std::min(J, cap);
+    if (index_out) std::copy(t.index.begin(), t.index.begin() + m, index_out);
+    if (cdf_out) std::copy(t.cdf.begin(), t.cdf.begin() + m, cdf_out);
+    if (q_out) std::copy(t.q.begin(), t.q.begin() + m, q_out);
+    if (total_out) *total_out = t.W;
+    return J;
+}
+
 int ezrt_scene_set_material_maps(ezrt_scene* s, const int32_t* metal_rough_id, const int32_t* normal_id) {
     if (!s) return ezrt_set_error(EZRT_ERR_INVALID, "scene_set_material_maps: null scene");
     if (!s->has_textures) return ezrt_set_error(EZRT_ERR_INVALID, "scene_set_material_maps: no textures (ezrt_scene_set_textures)");
@@ -1128,7 +1205,7 @@ int ezrt_scene_destroy(ezrt_scene* s) {
     s->lo_buf.release(); s->le_buf.release(); s->counters_buf.release(); s->totals_buf.release(); s->fb_buf.release(); s->sort_buf.release();
     s->adapt_buf.release(); s->adapt_maps_buf.release();
     s->aov_rec_buf.release(); s->aov_maps_buf.release(); s->denoise_buf.release(); s->denoise_io_buf.release();
-    s->lights_buf.release(); s->env_buf.release(); s->tex_buf.release(); s->tex_rec_buf.release();
+    s->lights_buf.release(); s->env_buf.release(); s->tex_buf.release(); s->tex_rec_buf.release(); s->punct_buf.release();
     if (s->own_stream) cudaStreamDestroy(s->own_stream);
     if (s->copy_stream) cudaStreamDestroy(s->copy_stream);
     if (s->side_stream) cudaStreamDestroy(s->side_stream);
@@ -1176,6 +1253,13 @@ static int light_options(ezrt_scene* s, const ezrt_render_params* p, cudaStream_
         o.tex_on = true;
         o.maps = s->maps;
         o.maps_on = (p->reserved[0] & EZRT_PARAM_MATERIAL_MAPS) != 0;   // validated: with the textures, and maps are set
+    }
+    // EZRT_PARAM_PUNCTUAL_LIGHTS (validated: lights are set); a table of J = 0 is mode 4 and runs its kernels.  P_p = 1 when the render
+    // has neither triangle lights nor the map's table, 1/2 otherwise
+    if ((p->reserved[0] & EZRT_PARAM_PUNCTUAL_LIGHTS) && s->punct.n > 0) {
+        o.punct = s->punct;
+        o.punct.p_p = (o.lights.n > 0 || o.env_on) ? 0.5f : 1.0f;
+        o.punct_on = true;
     }
     return EZRT_OK;
 }

@@ -1985,16 +1985,40 @@ __device__ __forceinline__ void tex_material(const SceneDev& sc, const TexDev& t
     }
 }
 
+// EZRT_PARAM_PUNCTUAL_LIGHTS (ezrt_math.h, DESIGN.md section 17): the category split of a light sample's selection number r_sel --
+// true (punctual) with *r_p its number in the table; false with *r_rest the number the map-or-triangle rule takes
+__device__ __forceinline__ bool punct_pick(const PunctDev& punct, float r_sel, float* r_p, float* r_rest) {
+    const bool half = (punct.p_p == 0.5f);
+    if (!half || r_sel < 0.5f) {
+        *r_p = half ? r_sel * 2.0f : r_sel;
+        return true;
+    }
+    *r_rest = (r_sel - 0.5f) * 2.0f;
+    return false;
+}
+// ... and the sample of light ez_light_select(cdf, n, r_p) at P: sh.d, sh.tmax, sh.pdf = the scale s, sh.light_mat = -2 - j; false
+// when there is none (medium: a medium vertex, no hemisphere test)
+__device__ __forceinline__ bool punct_sample(const PunctDev& punct, float r_p, vec3 P, vec3 N, bool medium, ShadowRay& sh) {
+    const int j = ez_light_select(punct.cdf, punct.n, r_p);
+    const float4* rp = punct.rec + 4 * (size_t)j;
+    const float4 a = ldg4(rp), b = ldg4(rp + 1), c = ldg4(rp + 2), e = ldg4(rp + 3);
+    const float r[16] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w, c.x, c.y, c.z, c.w, e.x, e.y, e.z, e.w};
+    if (!ez_punct_sample(r, punct.p_p * e.x, P, N, medium ? 1 : 0, &sh.d, &sh.tmax, &sh.pdf)) return false;
+    sh.light_mat = -2 - j;
+    return true;
+}
+
 // A medium vertex (EZRT_PARAM_MEDIUM; ezrt_math.h, DESIGN.md section 14): p's segment scattered at t_s before its hit (hit_t,
 // hit_tri) or its miss.  The weights of the segment (bounce >= 1) and the albedo enter the history; then, below max_bounce, one light
 // sample from P as at a surface but without the hemisphere test and the self exclusion (its shadow ray carries EZRT_MEDIUM_VERTEX
 // and d), and the phase function's sample as the next ray with the record (splat(p), p, 1).  Returns false when the path ends.
 // TEX: the first-hit record's albedo is the textured base colour.  MAPS: ... and its normal the mapped one.
-template <bool AOV, bool ENV, bool TEX = false, bool MAPS = false>
+// PUNCT: the light sample is punctual with probability punct.p_p (punct_pick, punct_sample).
+template <bool AOV, bool ENV, bool TEX = false, bool MAPS = false, bool PUNCT = false>
 __device__ __forceinline__ bool medium_step(const SceneDev& sc, const RenderDev& rd, int bounce, PathRegs& p, float t_s, float hit_t,
                                             int hit_tri, vec3& Lo, vec3& Le, bool& primary_miss, ShadowRay& sh, float4* aov_rec,
                                             const LightsDev& lights, const EnvDev& env, const MediumDev& med, const TexDev& tex = TexDev{},
-                                            const MapsDev& maps = MapsDev{}) {
+                                            const MapsDev& maps = MapsDev{}, const PunctDev& punct = PunctDev{}) {
     if (bounce == 0) {
         Lo = splat3(0.0f);
         Le = splat3(0.0f);
@@ -2016,12 +2040,19 @@ __device__ __forceinline__ bool medium_step(const SceneDev& sc, const RenderDev&
     const float r_sel = rand01(p.seed);
     const float r_1 = rand01(p.seed);
     const float r_2 = rand01(p.seed);
+    bool punct_on = false;   // PUNCT: the sample is punctual
+    float r_env = r_sel;     // the map-or-triangle rule's selection number
+    if constexpr (PUNCT) {
+        float r_p;
+        punct_on = punct_pick(punct, r_sel, &r_p, &r_env);
+        if (punct_on) sh.valid = punct_sample(punct, r_p, P, splat3(0.0f), true, sh);
+    }
     bool env_pick = false;
-    float r_tri = r_sel;
+    float r_tri = r_env;
     if constexpr (ENV) {
         const bool half = (env.p_env == 0.5f);
-        env_pick = (env.p_env == 1.0f) || (half && r_sel < 0.5f);
-        if (half) r_tri = (r_sel - 0.5f) * 2.0f;
+        env_pick = !punct_on && ((env.p_env == 1.0f) || (half && r_env < 0.5f));
+        if (half) r_tri = (r_env - 0.5f) * 2.0f;
         if (env_pick) {
             int texel;
             const vec3 Le_dir = ez_env_sample(env.row_cdf, env.col_cdf, env.w, env.h, r_1, r_2, &texel);
@@ -2031,11 +2062,12 @@ __device__ __forceinline__ bool medium_step(const SceneDev& sc, const RenderDev&
                 sh.d = Le_dir;
                 sh.tmax = EZ_INF;
                 sh.pdf = pdf_e;
+                if constexpr (PUNCT) sh.pdf = sh.pdf * (1.0f - punct.p_p);
                 sh.light_mat = -1;
             }
         }
     }
-    if (!env_pick && lights.n > 0) {
+    if (!punct_on && !env_pick && lights.n > 0) {
         const float4* lr = lights.rec + 4 * (size_t)ez_light_select(lights.cdf, lights.n, r_tri);
         const float4 a = ldg4(lr), b = ldg4(lr + 1), c = ldg4(lr + 2), e = ldg4(lr + 3);
         const vec3 D = ez_sub(ez_triangle_point(f4xyz(a), f4xyz(b), f4xyz(c), r_1, r_2), P);
@@ -2048,6 +2080,7 @@ __device__ __forceinline__ bool medium_step(const SceneDev& sc, const RenderDev&
             sh.tmax = ez_light_tmax(dist);
             sh.pdf = ez_light_pdf(e.w, lights.w_total, dist, cos_l);
             if constexpr (ENV) sh.pdf = sh.pdf * (1.0f - env.p_env);
+            if constexpr (PUNCT) sh.pdf = sh.pdf * (1.0f - punct.p_p);
             sh.light_mat = __float_as_int(a.w);
         }
     }
@@ -2088,13 +2121,16 @@ __device__ __forceinline__ bool medium_step(const SceneDev& sc, const RenderDev&
 // metallic-roughness map's and its shading normal N the normal map's (tex_material), everywhere N and the material are read after
 // the lookup: the BSDF, the lobe weights, the light samples' hemisphere tests, the path record's cosine, the shadow ray's N and the
 // first-hit record; the emission's MIS and the inside test keep the geometric normal.  *sh_rm carries (roughness, metallic) to k_nee.
+// PUNCT (light sampling mode with EZRT_PARAM_PUNCTUAL_LIGHTS, ezrt_math.h, DESIGN.md section 17): the light sample is punctual with
+// probability punct.p_p (punct_pick, punct_sample); the triangle and map samples' pdfs and the MIS weights of BSDF samples that reach
+// those lights take the factor 1 - p_p.
 template <int MODE, bool DEFER_NEE = false, bool AOV = false, bool ENV = false, bool TRANS = false, bool MEDIUM = false, bool TEX = false,
-          bool MAPS = false>
+          bool MAPS = false, bool PUNCT = false>
 __device__ __forceinline__ bool shade_step(const SceneDev& sc, const RenderDev& rd, int bounce, PathRegs& p, float hit_t,
                                            int hit_tri, uint32_t px, uint32_t py, float2 sob, vec3& Lo, vec3& Le,
                                            bool& primary_miss, ShadowRay& sh, float4* aov_rec = nullptr, LightsDev lights = LightsDev{},
                                            EnvDev env = EnvDev{}, MediumDev med = MediumDev{}, TexDev tex = TexDev{}, vec3* sh_base = nullptr,
-                                           float2* sh_rm = nullptr, MapsDev maps = MapsDev{}) {
+                                           float2* sh_rm = nullptr, MapsDev maps = MapsDev{}, PunctDev punct = PunctDev{}) {
     sh.valid = false;
     const int mode = (MODE < 0) ? rd.mode : MODE;
     const bool is_mode = (mode == EZRT_MODE_DISNEY_IS_MIS_P5);
@@ -2109,7 +2145,8 @@ __device__ __forceinline__ bool shade_step(const SceneDev& sc, const RenderDev& 
         float t_s;
         const float t_end = (hit_tri < 0) ? __int_as_float(0x7f800000) : hit_t;
         if (ez_medium_flight(&med, p.o, p.d, t_end, &p.seed, &t_s))
-            return medium_step<AOV, ENV, TEX, MAPS>(sc, rd, bounce, p, t_s, hit_t, hit_tri, Lo, Le, primary_miss, sh, aov_rec, lights, env, med, tex, maps);
+            return medium_step<AOV, ENV, TEX, MAPS, PUNCT>(sc, rd, bounce, p, t_s, hit_t, hit_tri, Lo, Le, primary_miss, sh, aov_rec, lights, env, med, tex,
+                                                           maps, punct);
     }
     if (bounce == 0) {
         Lo = splat3(0.0f);
@@ -2130,7 +2167,12 @@ __device__ __forceinline__ bool shade_step(const SceneDev& sc, const RenderDev& 
                 vec3 c = ez_divs(ez_scale(ez_mul(ez_mul(ez_scale(p.history, mis_weight), sky), p.f_r), p.cosine_i), p.pdf);
                 Lo = ez_add(Lo, c);
             } else if (ENV) {   // the map is a light: MIS against its sampling density, in mode 3's order
-                const float w = (env.p_env > 0.0f && !below) ? mis_mix_weight(p.pdf, env.p_env * ez_env_pdf(env.texel_pdf, env.w, env.h, p.d)) : 1.0f;
+                float w;
+                if constexpr (PUNCT)
+                    w = (env.p_env > 0.0f && !below) ? mis_mix_weight(p.pdf, (1.0f - punct.p_p) * (env.p_env * ez_env_pdf(env.texel_pdf, env.w, env.h, p.d)))
+                                                     : 1.0f;
+                else
+                    w = (env.p_env > 0.0f && !below) ? mis_mix_weight(p.pdf, env.p_env * ez_env_pdf(env.texel_pdf, env.w, env.h, p.d)) : 1.0f;
                 Lo = ez_add(Lo, ez_divs(ez_scale(ez_mul(ez_mul(ez_scale(p.history, w), sky), p.f_r), path_cos<TRANS>(p.cosine_i)), p.pdf));
             } else {
                 Lo = ez_add(Lo, contrib3(p.history, sky, p.f_r, path_cos<TRANS>(p.cosine_i), p.pdf));
@@ -2167,8 +2209,15 @@ __device__ __forceinline__ bool shade_step(const SceneDev& sc, const RenderDev& 
                 tri_vertices(sc, hit_tri, rd.accel_space != 0, p1, p2, p3);
                 if (ez_is_light(ez_light_weight(p1, p2, p3, mat.emissive))) {
                     const vec3 Ng = f4xyz(ldg4(tri_geo_rec(sc, hit_tri, rd.accel_space != 0)));
-                    if constexpr (ENV) w = mis_mix_weight(p.pdf, (1.0f - env.p_env) * ez_light_pdf(lum, lights.w_total, hit_t, ez_abs(ez_dot(Ng, p.d))));
-                    else w = mis_mix_weight(p.pdf, ez_light_pdf(lum, lights.w_total, hit_t, ez_abs(ez_dot(Ng, p.d))));
+                    if constexpr (PUNCT) {
+                        float pl = ez_light_pdf(lum, lights.w_total, hit_t, ez_abs(ez_dot(Ng, p.d)));
+                        if constexpr (ENV) pl = (1.0f - env.p_env) * pl;
+                        w = mis_mix_weight(p.pdf, (1.0f - punct.p_p) * pl);
+                    } else if constexpr (ENV) {
+                        w = mis_mix_weight(p.pdf, (1.0f - env.p_env) * ez_light_pdf(lum, lights.w_total, hit_t, ez_abs(ez_dot(Ng, p.d))));
+                    } else {
+                        w = mis_mix_weight(p.pdf, ez_light_pdf(lum, lights.w_total, hit_t, ez_abs(ez_dot(Ng, p.d))));
+                    }
                 }
             }
             Lo = ez_add(Lo, ez_divs(ez_scale(ez_mul(ez_mul(ez_scale(p.history, w), mat.emissive), p.f_r), path_cos<TRANS>(p.cosine_i)), p.pdf));
@@ -2202,12 +2251,23 @@ __device__ __forceinline__ bool shade_step(const SceneDev& sc, const RenderDev& 
             if (tl.t != 0.0f) go = bsdf_sample(xi_1, xi_2, xi_3, rand01(p.seed), V, N, mat, tl, L, fr_l, pdf_l, NdotL);
         }
         const int sh_mat = (TRANS && hit.inside) ? ~hit.matId : hit.matId;   // k_nee<.., TRANS> needs the side for eta
+        bool punct_on = false;   // PUNCT: the sample is punctual
+        float r_env = r_sel;     // the map-or-triangle rule's selection number
+        if constexpr (PUNCT) {
+            float r_p;
+            punct_on = punct_pick(punct, r_sel, &r_p, &r_env);
+            if (punct_on && punct_sample(punct, r_p, hit.P, N, false, sh)) {
+                sh.valid = true;
+                sh.o = hit.P;
+                sh.N = N; sh.V = V; sh.history = p.history; sh.matId = sh_mat;
+            }
+        }
         bool env_pick = false;
-        float r_tri = r_sel;   // the triangle light's selection number
+        float r_tri = r_env;   // the triangle light's selection number
         if constexpr (ENV) {   // the environment with probability p_env: r_sel < 0.5 beside triangle lights, always without
             const bool half = (env.p_env == 0.5f);
-            env_pick = (env.p_env == 1.0f) || (half && r_sel < 0.5f);
-            if (half) r_tri = (r_sel - 0.5f) * 2.0f;
+            env_pick = !punct_on && ((env.p_env == 1.0f) || (half && r_env < 0.5f));
+            if (half) r_tri = (r_env - 0.5f) * 2.0f;
             if (env_pick) {
                 int texel;
                 const vec3 Le_dir = ez_env_sample(env.row_cdf, env.col_cdf, env.w, env.h, r_1, r_2, &texel);
@@ -2219,11 +2279,12 @@ __device__ __forceinline__ bool shade_step(const SceneDev& sc, const RenderDev& 
                     sh.N = N; sh.V = V; sh.history = p.history; sh.matId = sh_mat;
                     sh.tmax = EZ_INF;
                     sh.pdf = pdf_e;
+                    if constexpr (PUNCT) sh.pdf = sh.pdf * (1.0f - punct.p_p);
                     sh.light_mat = -1;
                 }
             }
         }
-        if (!env_pick && lights.n > 0) {
+        if (!punct_on && !env_pick && lights.n > 0) {
             const float4* lr = lights.rec + 4 * (size_t)ez_light_select(lights.cdf, lights.n, r_tri);
             const float4 a = ldg4(lr), b = ldg4(lr + 1), c = ldg4(lr + 2), e = ldg4(lr + 3);
             const int self = __float_as_int(rd.accel_space ? c.w : b.w);   // the light's triangle in the hit's index space
@@ -2239,6 +2300,7 @@ __device__ __forceinline__ bool shade_step(const SceneDev& sc, const RenderDev& 
                 sh.tmax = ez_light_tmax(dist);
                 sh.pdf = ez_light_pdf(e.w, lights.w_total, dist, cos_l);
                 if constexpr (ENV) sh.pdf = sh.pdf * (1.0f - env.p_env);
+                if constexpr (PUNCT) sh.pdf = sh.pdf * (1.0f - punct.p_p);
                 sh.light_mat = __float_as_int(a.w);
             }
         }

@@ -178,6 +178,18 @@ struct MapsDev {
     float* sh_metal;
 };
 
+// The punctual lights of EZRT_PARAM_PUNCTUAL_LIGHTS (ezrt_math.h, DESIGN.md section 17), set by ezrt_scene_set_punctual_lights.
+// Passed to every k_shade / k_nee instantiation as their last parameter, after MapsDev, so that no other parameter moves; read by
+// the punctual instantiations (<.., PUNCT>) only.  A punctual sample's shadow slot carries hist.w = -2 - j (the light's index in the
+// table, beside -1 for the map) and view.w = its scale ez_punct_sample's s in place of a pdf.
+//   rec: 4 float4 per light (ezrt_math.h's 16 floats); cdf: n floats, cdf[n - 1] = 1; p_p: P_p (1/2 or 1)
+struct PunctDev {
+    const float4* rec;
+    const float* cdf;
+    int n;
+    float p_p;
+};
+
 // A shadow ray and what k_nee needs to evaluate the light sample's contribution once the ray got through (nee_contrib):
 // the BRDF / environment evaluation of the light sample is done after the shadow pass, for unoccluded rays only.
 #define EZRT_SHADOW_SLOT_BYTES (5 * 16 + 1)

@@ -551,15 +551,17 @@ __global__ void __launch_bounds__(EZRT_EXTEND_MAX_THREADS, EZRT_EXTEND_LB_BLOCKS
 // shading point's textured base colour, tex.sh_base[spos].
 // MAPS (with TEX; EZRT_PARAM_MATERIAL_MAPS): the material maps (shade_step); the slot also gets the mapped roughness in
 // tex.sh_base[spos].w and the mapped metallic in maps.sh_metal[spos].
+// PUNCT (light sampling mode with EZRT_PARAM_PUNCTUAL_LIGHTS): the punctual lights punct are one more category of light samples
+// (shade_step); a punctual sample's slot carries hist.w = -2 - j and its scale in view.w.
 template <int MODE, bool LIST, bool AOV = false, bool ENV = false, bool TRANS = false, bool MEDIUM = false, bool TEX = false,
-          bool MAPS = false>
+          bool MAPS = false, bool PUNCT = false>
 __global__ void __launch_bounds__(128, EZRT_SHADE_MIN_BLOCKS) k_shade(SceneDev sc, RenderDev rd, const TileDev* __restrict__ tiles, int bounce,
                                                uint32_t batch_first_frame, PathQueue qin, const uint32_t* __restrict__ in_count,
                                                PathQueue qout, uint32_t* out_count, ShadowQueue sq, uint32_t* s_count,
                                                float4* __restrict__ Lo, float4* __restrict__ Le, uint32_t n_fused, uint32_t n_frames,
                                                const uint32_t* __restrict__ list, const float2* __restrict__ side_hit,
                                                float4* __restrict__ aov_rec, LightsDev lights, EnvDev env, MediumDev med, TexDev tex,
-                                               MapsDev maps) {
+                                               MapsDev maps, PunctDev punct) {
     // The Sobol pair of (bounce, frame) is the same for every pixel of a frame (P5/fsh:361-376: up to 2 x 32 table XORs per path): each
     // block computes the pairs of the batch's frames once into shared memory (batches of more than EZRT_SOBOL_TABLE frames compute per path).
     __shared__ float2 s_sobol[EZRT_SOBOL_TABLE];
@@ -685,9 +687,9 @@ __global__ void __launch_bounds__(128, EZRT_SHADE_MIN_BLOCKS) k_shade(SceneDev s
             }
 #endif
             if (LIST || __float_as_int(hit.y) != EZRT_TRI_PENDING) {   // pending: deferred by the accel kernel, shaded by the LIST pass
-                alive = shade_step<MODE, MODE == EZRT_MODE_DISNEY_IS_MIS_P5, AOV, ENV, TRANS, MEDIUM, TEX, MAPS>(sc, rd, bounce, p, hit.x, __float_as_int(hit.y), px, py,
+                alive = shade_step<MODE, MODE == EZRT_MODE_DISNEY_IS_MIS_P5, AOV, ENV, TRANS, MEDIUM, TEX, MAPS, PUNCT>(sc, rd, bounce, p, hit.x, __float_as_int(hit.y), px, py,
                                                                                                           sob, lo, le, pmiss, sh, AOV ? aov_rec + 2 * (size_t)slot : nullptr,
-                                                                                                          lights, env, med, tex, &sh_base, &sh_rm, maps);
+                                                                                                          lights, env, med, tex, &sh_base, &sh_rm, maps, punct);
                 if (bounce == 0) {
                     // Le is zero for every surface that does not emit: it is stored (and read back by k_blend) only otherwise.
                     // color = Le + Lo with Le = +-0 is Lo bit for bit, because Lo is never -0.0 (it starts at +0.0 and only grows by additions)
@@ -740,9 +742,11 @@ __global__ void __launch_bounds__(128, EZRT_SHADE_MIN_BLOCKS) k_shade(SceneDev s
 // EZRT_MEDIUM_VERTEX, view = d) is evaluated with the phase function (nee_medium_contrib).
 // TEX: the shading point's material with the textured base colour k_shade left in tex.sh_base[j].
 // MAPS: ... and the mapped roughness and metallic, tex.sh_base[j].w and maps.sh_metal[j]; the slot's N is already the mapped normal.
-template <int MODE, bool ENV = false, bool TRANS = false, bool MEDIUM = false, bool TEX = false, bool MAPS = false>
+// PUNCT: and the punctual samples (hist.w = -2 - j): ez_punct_contrib of the shading point's f (the BSDF or mixture at a surface, the
+// phase function at a medium vertex) with light j's intensity * color and the scale in view.w, without a MIS weight.
+template <int MODE, bool ENV = false, bool TRANS = false, bool MEDIUM = false, bool TEX = false, bool MAPS = false, bool PUNCT = false>
 __global__ void __launch_bounds__(128, 8) k_nee(SceneDev sc, RenderDev rd, ShadowQueue sq, const uint32_t* __restrict__ s_count, float4* __restrict__ Lo,
-                                                MediumDev med, TexDev tex, MapsDev maps) {
+                                                MediumDev med, TexDev tex, MapsDev maps, PunctDev punct) {
     static_assert(MODE == EZRT_MODE_DISNEY_LIGHTS || !(ENV || TRANS || MEDIUM), "the options exist in the light sampling mode");
     static_assert(!(TRANS && MEDIUM), "the medium is rendered without transmission");
     __shared__ uint32_t s_scan[34];
@@ -781,9 +785,30 @@ __global__ void __launch_bounds__(128, 8) k_nee(SceneDev sc, RenderDev rd, Shado
             const vec3 V = ez_v3(v4.x, v4.y, v4.z), N = ez_v3(n4.x, n4.y, n4.z), Ld = ez_v3(d4.x, d4.y, d4.z), hist = ez_v3(h4.x, h4.y, h4.z);
             vec3 c;
             if constexpr (MODE == EZRT_MODE_DISNEY_LIGHTS) {
-                const int lm = __float_as_int(h4.w);   // the light's material; -1: an environment sample
+                const int lm = __float_as_int(h4.w);   // the light's material; -1: an environment sample; PUNCT: <= -2 a punctual one
                 const auto light_color = [&] { return (ENV && lm < 0) ? hdr_color(sc, rd, Ld, EZRT_MODE_DISNEY_LIGHTS) : load_emissive(sc, lm); };
-                if constexpr (MEDIUM) {   // a medium vertex loads no material
+                if (PUNCT && lm < -1) {
+                    const float4* r = punct.rec + 4 * (size_t)(-2 - lm);
+                    vec3 f;
+                    float cosine = 1.0f;
+                    if (MEDIUM && m_raw == EZRT_MEDIUM_VERTEX) {
+                        f = splat3(ez_hg_pdf(V, Ld, med.g));
+                    } else {
+                        const int m_id = (TRANS && m_raw < 0) ? ~m_raw : m_raw;
+                        const MaterialDev mat = material(m_id);
+                        if constexpr (TRANS) {   // the mixture where t > 0, the reference BRDF's bits where t == 0
+                            const TransLobe tl = trans_lobe(sc, m_id, mat, m_raw < 0);
+                            float pdf_unused;
+                            f = (tl.t == 0.0f) ? brdf_evaluate<false>(V, N, Ld, mat) : bsdf_evaluate(V, N, Ld, mat, tl, pdf_unused);
+                        } else {
+                            f = brdf_evaluate<false>(V, N, Ld, mat);
+                        }
+                        cosine = ez_dot(N, Ld);
+                    }
+                    c = ez_punct_contrib(hist, f, cosine, f4xyz(ldg4(r + 2)), v4.w);
+                    if constexpr (MEDIUM)
+                        c = ez_scale(c, ez_medium_transmittance(&med, ez_v3(o4.x, o4.y, o4.z), Ld, ez_medium_light_dist(n4.w, ldg4(r).w == 2.0f)));
+                } else if constexpr (MEDIUM) {   // a medium vertex loads no material
                     const vec3 E = light_color();
                     if (m_raw == EZRT_MEDIUM_VERTEX) c = nee_medium_contrib(V, Ld, med.g, hist, E, v4.w);
                     else c = nee_light_contrib(V, N, Ld, material(m_raw), hist, E, v4.w);
@@ -1374,13 +1399,13 @@ static void launch_shade_t(int blocks, const SceneDev& sc, const RenderDev& rd, 
                            float4* Lo, float4* Le, uint32_t n_fused, uint32_t n_frames, const uint32_t* list, const float2* side_hit,
                            float4* aov_rec, const LightOptions& o, cudaStream_t st) {
     auto launch = [&](auto M) {
-        with_bools([&](auto A, auto E, auto T, auto X, auto TX, auto MP) {
+        with_bools([&](auto A, auto E, auto T, auto X, auto TX, auto MP, auto P) {
             // the options exist in the light sampling mode; the maps with the textures
-            if constexpr ((M == EZRT_MODE_DISNEY_LIGHTS || !(E || T || X || TX)) && !(T && X) && (TX || !MP))
-                k_shade<M, LIST, A, E, T, X, TX, MP><<<blocks, 128, 0, st>>>(sc, rd, tiles, bounce, batch_first_frame, qin, in_count, qout, out_count, sq,
-                                                                             s_count, Lo, Le, n_fused, n_frames, list, side_hit, aov_rec, o.lights, o.env,
-                                                                             o.med, o.tex, o.maps);
-        }, aov_rec != nullptr, o.env_on, o.trans_on, o.medium_on, o.tex_on, o.maps_on);
+            if constexpr ((M == EZRT_MODE_DISNEY_LIGHTS || !(E || T || X || TX || P)) && !(T && X) && (TX || !MP))
+                k_shade<M, LIST, A, E, T, X, TX, MP, P><<<blocks, 128, 0, st>>>(sc, rd, tiles, bounce, batch_first_frame, qin, in_count, qout, out_count, sq,
+                                                                                s_count, Lo, Le, n_fused, n_frames, list, side_hit, aov_rec, o.lights, o.env,
+                                                                                o.med, o.tex, o.maps, o.punct);
+        }, aov_rec != nullptr, o.env_on, o.trans_on, o.medium_on, o.tex_on, o.maps_on, o.punct_on);
     };
     switch (rd.mode) {
         case EZRT_MODE_DIFFUSE_P3: launch(std::integral_constant<int, EZRT_MODE_DIFFUSE_P3>{}); break;
@@ -1412,11 +1437,12 @@ void launch_deferred_lane(const SceneDev& sc, const RenderDev& rd, const TileDev
 void launch_nee(const SceneDev& sc, const RenderDev& rd, ShadowQueue sq, const uint32_t* s_count, float4* Lo, uint32_t n_max, int n_sms, cudaStream_t st,
                 const LightOptions& o) {
     const int blocks = std::max(1, std::min(div_up(n_max, 512), n_sms * 8));
-    with_bools([&](auto L, auto E, auto T, auto X, auto TX, auto MP) {
+    with_bools([&](auto L, auto E, auto T, auto X, auto TX, auto MP, auto P) {
         // the options exist in the light sampling mode (the other mode here is mode 3); the maps with the textures
-        if constexpr ((L || !(E || T || X || TX)) && !(T && X) && (TX || !MP))
-            k_nee<L ? EZRT_MODE_DISNEY_LIGHTS : EZRT_MODE_DISNEY_IS_MIS_P5, E, T, X, TX, MP><<<blocks, 128, 0, st>>>(sc, rd, sq, s_count, Lo, o.med, o.tex, o.maps);
-    }, rd.mode == EZRT_MODE_DISNEY_LIGHTS, o.env_on, o.trans_on, o.medium_on, o.tex_on, o.maps_on);
+        if constexpr ((L || !(E || T || X || TX || P)) && !(T && X) && (TX || !MP))
+            k_nee<L ? EZRT_MODE_DISNEY_LIGHTS : EZRT_MODE_DISNEY_IS_MIS_P5, E, T, X, TX, MP, P><<<blocks, 128, 0, st>>>(sc, rd, sq, s_count, Lo, o.med, o.tex, o.maps,
+                                                                                                                    o.punct);
+    }, rd.mode == EZRT_MODE_DISNEY_LIGHTS, o.env_on, o.trans_on, o.medium_on, o.tex_on, o.maps_on, o.punct_on);
 }
 
 // ------------------------------------------------------------------------------------------

@@ -23,6 +23,7 @@
 //   medium_on EZRT_PARAM_MEDIUM with sigma_t > 0: the homogeneous medium med (<.., MEDIUM>); never with trans_on
 //   tex_on    EZRT_PARAM_TEXTURES: the scene's base-colour textures tex (<.., TEX>)
 //   maps_on   EZRT_PARAM_MATERIAL_MAPS (with tex_on): the material maps of tex (<.., TEX, MAPS>)
+//   punct_on  EZRT_PARAM_PUNCTUAL_LIGHTS and the scene's punctual table has J > 0 lights: punct (<.., PUNCT>)
 // All off outside the light sampling mode; the tables are zero where unused, as the kernels' parameters.
 struct LightOptions {
     LightsDev lights{};   // the light table (light sampling mode)
@@ -30,7 +31,8 @@ struct LightOptions {
     MediumDev med{};      // the medium (medium_on)
     TexDev tex{};         // the textures and the shadow slots' base colours (tex_on)
     MapsDev maps{};       // the maps' table and the shadow slots' metallic (maps_on)
-    bool env_on = false, trans_on = false, medium_on = false, tex_on = false, maps_on = false;
+    PunctDev punct{};     // the punctual lights' table and P_p (punct_on)
+    bool env_on = false, trans_on = false, medium_on = false, tex_on = false, maps_on = false, punct_on = false;
 };
 
 // lens (EZRT_PARAM_THIN_LENS): the thin-lens camera rays (k_generate<true>); null: the pinhole's

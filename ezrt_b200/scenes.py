@@ -411,3 +411,24 @@ def s_p3_bunny_mapped(n_textures=2, builder=api.BVH_SAH_FAST):
 def s_1m_bunny_mapped(n_textures=2, builder=api.BVH_SAH_FAST):
     """s_1m_bunny_textured plus the maps of s_p3_bunny_mapped"""
     return _with_maps(s_1m_bunny_textured(n_textures, builder))
+
+
+def punctual_rig(tris, seed=0, n_points=3, power=1.0):
+    """A seeded rig of punctual lights for RenderConfig.punctual_lights (Scene.set_punctual_lights), placed from the triangles' bounds:
+    a sun from above at a seeded slant, a key spot above and in front of the centre aimed at it, and n_points coloured point lights
+    around the scene.  power scales every intensity (the units are the render's; the scene's extent sets the point lights' scale)."""
+    v = np.asarray(tris, np.float32).reshape(-1, 36)[:, :9].reshape(-1, 3).astype(np.float64)
+    lo, hi = v.min(axis=0), v.max(axis=0)
+    c, r = 0.5 * (lo + hi), 0.5 * float(np.linalg.norm(hi - lo))
+    rng = np.random.default_rng(seed)
+    a = rng.uniform(0, 2 * np.pi)
+    sun_dir = (0.4 * np.cos(a), -1.0, 0.4 * np.sin(a))
+    lights = [api.directional_light(sun_dir, color=(1.0, 0.95, 0.85), intensity=1.5 * power)]
+    key = c + np.array([0.3 * r, 1.2 * r, 1.2 * r])
+    lights.append(api.spot_light(key, c - key, color=(1.0, 0.9, 0.8), intensity=4.0 * r * r * power, inner_cone=0.25, outer_cone=0.6))
+    for k in range(n_points):
+        phi = 2 * np.pi * (k + rng.uniform()) / max(1, n_points)
+        pos = c + r * np.array([1.1 * np.cos(phi), rng.uniform(0.2, 0.9), 1.1 * np.sin(phi)])
+        col = rng.uniform(0.3, 1.0, 3)
+        lights.append(api.point_light(pos, color=tuple(col), intensity=float(rng.uniform(0.5, 1.5) * r * r * power)))
+    return lights

@@ -171,6 +171,34 @@ typedef struct ezrt_render_params {
    ezrt_render_adaptive[_device] and ezrt_render_aov[_device].  Each shadow slot of a render takes 81 bytes, 97 with
    EZRT_PARAM_TEXTURES, 101 with EZRT_PARAM_MATERIAL_MAPS too. */
 #define EZRT_PARAM_MATERIAL_MAPS 64
+/* ezrt_render_params.reserved[0], EZRT_MODE_DISNEY_LIGHTS on the wavefront pipeline only, with or without every other flag of that
+   mode: the scene's punctual lights (ezrt_scene_set_punctual_lights; glTF's KHR_lights_punctual point, spot and directional lights)
+   are one more category of light samples.  With a table of J > 0 lights, a light sample is punctual with probability P_p = 1 when
+   the render has neither triangle lights nor the map as a light (EZRT_PARAM_ENV_LIGHT with a table), 1/2 otherwise: r_sel < 1/2 picks
+   it with r_p = 2 r_sel, and (r_sel - 1/2) 2 goes into the map-or-triangle rule; no draw is added.  Light j of the table is chosen by
+   its cdf and sampled at the shading point with one shadow ray (bounded at ez_light_tmax(dist) for point and spot lights, at EZ_INF for
+   directional ones); a lit sample adds history * f * cos * (intensity * color) * falloff / (P_p q_j dist^2) (no dist^2 for
+   directional lights) and no MIS weight, as no BSDF sample reaches a delta light.  The triangle and map samples' pdfs and the MIS
+   weights of BSDF samples that hit them take the factor 1 - P_p (ezrt_math.h, DESIGN.md section 17).  A table of J = 0 (no lights,
+   or all of weight 0) renders mode 4's image with mode 4's kernels.  Invalid (EZRT_ERR_INVALID) in another mode, with the
+   megakernel, or without lights set.  Accepted by ezrt_render[_device], ezrt_render_adaptive[_device] and ezrt_render_aov[_device];
+   the shadow slots keep their sizes. */
+#define EZRT_PARAM_PUNCTUAL_LIGHTS 128
+
+/* One punctual light of ezrt_scene_set_punctual_lights (glTF's KHR_lights_punctual, in the render's units: no photometric
+   conversion; the caller scales glTF's candela and lux) */
+#define EZRT_PUNCTUAL_POINT 0
+#define EZRT_PUNCTUAL_SPOT 1
+#define EZRT_PUNCTUAL_DIRECTIONAL 2
+typedef struct ezrt_punctual_light {
+    int32_t type;                   /* EZRT_PUNCTUAL_POINT, _SPOT or _DIRECTIONAL */
+    float position[3];              /* point and spot */
+    float direction[3];             /* spot: where the cone points; directional: where the light travels (non-zero length; normalised) */
+    float color[3];                 /* linear RGB, each >= 0 */
+    float intensity;                /* >= 0: radiant intensity (point, spot) or irradiance (directional) */
+    float inner_cone, outer_cone;   /* spot only, radians: 0 <= inner < outer <= pi/2 (rounded to fp32) */
+    int32_t reserved;               /* 0 */
+} ezrt_punctual_light;
 
 /* One texture of ezrt_scene_set_textures: width x height RGBA8 texels (4 bytes each, R first), row 0 the image's top row */
 typedef struct ezrt_texture {
@@ -253,6 +281,17 @@ int ezrt_scene_set_material_maps(ezrt_scene* scene, const int32_t* metal_rough_i
  * inside).  The maps set on the scene are used (none: the material's values and surface_hit's normal).  Host arrays; synchronous.
  * EZRT_ERR_INVALID without textures set or for a triangle index out of range. */
 int ezrt_scene_sample_materials(ezrt_scene* scene, int n, const int32_t* tri, const float* hits, float* out);
+/* Sets the scene's punctual lights (EZRT_PARAM_PUNCTUAL_LIGHTS): n lights, copied; lights NULL clears them.  Builds their table on
+ * the host in float64 (ezrt_math.h, DESIGN.md section 17: the lights of weight > 0 in the caller's order, their cdf and selection
+ * probabilities) and uploads it.  Returns EZRT_ERR_INVALID, and keeps the previous lights, for n < 0, an unknown type, a non-finite
+ * field, a zero-length direction on a spot or directional light, a negative colour channel or intensity, spot cones outside
+ * 0 <= inner < outer <= pi/2, reserved != 0, or a weight (or their sum) that is not finite.  The call first waits for every render
+ * already enqueued on the scene's device, then uploads synchronously. */
+int ezrt_scene_set_punctual_lights(ezrt_scene* scene, int n, const ezrt_punctual_light* lights);
+/* The table of ezrt_scene_set_punctual_lights: returns J, the number of lights of weight > 0 (0 without lights), or a negative
+ * status; writes min(J, cap) entries: index_out = each light's index among the caller's lights, cdf_out = the cdf (the last entry 1),
+ * q_out = the selection probabilities (float)(w_j / W), and *total_out = W, the float64 sum of the weights.  Any output may be NULL. */
+int ezrt_scene_punctual_lights(ezrt_scene* scene, int cap, int32_t* index_out, float* cdf_out, float* q_out, double* total_out);
 
 /* render(width,height,spp) -> framebuffer: equals `spp` consecutive display() calls
  * (P5/main.cpp:697-748) each drawing pass1 (P5/fsh:894-949) and copying to lastFrame.

@@ -892,4 +892,55 @@ EZ_HD ez_vec3 ez_normal_map(ez_vec3 p1, ez_vec3 p2, ez_vec3 p3, const float* uv6
 EZ_HD int ez_maps_mr_id(uint32_t w) { return (int)(w & 0xffffu) - 1; }
 EZ_HD int ez_maps_normal_id(uint32_t w) { return (int)(w >> 16) - 1; }
 
+/* ------------------------------------------------------------------ punctual lights (EZRT_PARAM_PUNCTUAL_LIGHTS, DESIGN.md section 17)
+ * The table (ezrt_punctual.h, float64 on the host): light j's record is 16 floats,
+ *   [0..2] position, [3] type (0 point, 1 spot, 2 directional, as a float), [4..6] unit direction (float64-normalised), [7] cos_o,
+ *   [8..10] intensity * color (fp32 products), [11] cos_i, [12] q_j, [13..15] 0;  cos_i, cos_o = (float)cos((double)cone).
+ * Per shading point P (shading normal N) of a light sample: P_p = 1 without triangle lights and map table, else 1/2.
+ *   punctual iff P_p == 1 or r_sel < 0.5; then r_p = r_sel (P_p = 1) or r_sel * 2, j = ez_light_select(cdf, J, r_p), and
+ *   ez_punct_sample below with pq = P_p * q_j; otherwise (r_sel - 0.5) * 2 goes into the map-or-triangle rule, and the pdf of a
+ *   triangle or map sample is pdf * (1 - P_p) (after its own factors).  A lit punctual sample adds
+ *   ez_punct_contrib(history, f(V, N, L), cos, intensity * color, s), cos = dot(N, L) at a surface and 1 with f = splat(phase) at a
+ *   medium vertex; in fog times ez_medium_transmittance over ez_medium_light_dist(tmax, directional).
+ * A BSDF sample's MIS weight at an emission hit of a triangle light: mis(p.pdf, (1 - P_p) * pdf_l) with pdf_l as without punctual
+ * lights (including its (1 - P_env)); at an environment miss: mis(p.pdf, (1 - P_p) * (P_env * env_pdf)). */
+/* glTF's spot falloff of the light direction L (shading point to light) under the cone about dir: clamp(cd s - cos_o s, 0, 1)^2 with
+ * cd = dot(dir, -L), s = 1 / max(0.001, cos_i - cos_o) */
+EZ_HD float ez_spot_falloff(ez_vec3 dir, ez_vec3 L, float cos_i, float cos_o) {
+    const float cd = ez_dot(dir, ez_neg(L));
+    const float s = EZ_DIV(1.0f, ez_max(0.001f, cos_i - cos_o));
+    const float t = ez_clamp(cd * s - cos_o * s, 0.0f, 1.0f);
+    return t * t;
+}
+/* The sample of the light with record r (16 floats) at P, chosen with probability pq = P_p * q_j: 1 with the direction *L, the shadow
+ * ray's bound *tmax and the contribution's scale *s, or 0 for no sample.  medium != 0 (a medium vertex): no hemisphere test.
+ *   point / spot: D = pos - P, d2 = dot(D, D), dist = sqrt(d2); none if dist == 0 or not finite; L = normalize(D); none if
+ *     dot(N, L) <= 0; a = ez_spot_falloff (spot) or 1 (point); none if a == 0; tmax = ez_light_tmax(dist), s = a / (pq * d2)
+ *   directional: L = -dir; none if dot(N, L) <= 0; tmax = EZ_INF, s = 1 / pq */
+EZ_HD int ez_punct_sample(const float* r, float pq, ez_vec3 P, ez_vec3 N, int medium, ez_vec3* L, float* tmax, float* s) {
+    const ez_vec3 dir = ez_v3(r[4], r[5], r[6]);
+    if (r[3] == 2.0f) {
+        *L = ez_neg(dir);
+        if (!medium && !(ez_dot(N, *L) > 0.0f)) return 0;
+        *tmax = EZ_INF;
+        *s = EZ_DIV(1.0f, pq);
+        return 1;
+    }
+    const ez_vec3 D = ez_sub(ez_v3(r[0], r[1], r[2]), P);
+    const float d2 = ez_dot(D, D);
+    const float dist = EZ_SQRT(d2);
+    if (dist == 0.0f || !ez_finite(dist)) return 0;
+    *L = ez_normalize(D);
+    if (!medium && !(ez_dot(N, *L) > 0.0f)) return 0;
+    const float a = (r[3] == 1.0f) ? ez_spot_falloff(dir, *L, r[11], r[7]) : 1.0f;
+    if (a == 0.0f) return 0;
+    *tmax = ez_light_tmax(dist);
+    *s = EZ_DIV(a, pq * d2);
+    return 1;
+}
+/* a lit punctual sample's contribution: ((history * f) * cos) * E * s, left to right (E = intensity * color) */
+EZ_HD ez_vec3 ez_punct_contrib(ez_vec3 history, ez_vec3 f, float cosine, ez_vec3 E, float s) {
+    return ez_scale(ez_mul(ez_scale(ez_mul(history, f), cosine), E), s);
+}
+
 #endif /* EZRT_MATH_H */
