@@ -27,6 +27,7 @@ PARAM_MEDIUM = 16
 PARAM_TEXTURES = 32
 PARAM_MATERIAL_MAPS = 64
 PARAM_PUNCTUAL_LIGHTS = 128
+PARAM_EMISSION_MAPS = 256
 PUNCTUAL_POINT, PUNCTUAL_SPOT, PUNCTUAL_DIRECTIONAL = 0, 1, 2   # ezrt_punctual_light.type
 MODES = {"diffuse_p3": 0, "disney_aniso_p4": 1, "disney_sobol_p5": 2, "disney_is_mis_p5": 3, "disney_lights": 4}
 
@@ -255,6 +256,7 @@ class RenderConfig:
     textures: bool = False      # EZRT_PARAM_TEXTURES (MODE_DISNEY_LIGHTS only): the scene's base-colour textures (Scene.set_textures, DESIGN.md section 15)
     material_maps: bool = False  # EZRT_PARAM_MATERIAL_MAPS (with textures): the scene's material maps (Scene.set_material_maps, DESIGN.md section 16)
     punctual_lights: bool = False  # EZRT_PARAM_PUNCTUAL_LIGHTS (MODE_DISNEY_LIGHTS only): the scene's punctual lights (Scene.set_punctual_lights, DESIGN.md section 17)
+    emission_maps: bool = False  # EZRT_PARAM_EMISSION_MAPS (with textures): the scene's emission maps (Scene.set_emission_maps, DESIGN.md section 18)
 
     def to_struct(self):
         p = RenderParams()
@@ -269,7 +271,7 @@ class RenderConfig:
         p.reserved[0] = ((PARAM_ACCUMULATE if self.accumulate else 0) | (PARAM_ENV_LIGHT if self.env_light else 0) |
                          (PARAM_TRANSMISSION if self.transmission else 0) | (PARAM_MEDIUM if self.medium else 0) |
                          (PARAM_TEXTURES if self.textures else 0) | (PARAM_MATERIAL_MAPS if self.material_maps else 0) |
-                         (PARAM_PUNCTUAL_LIGHTS if self.punctual_lights else 0))
+                         (PARAM_PUNCTUAL_LIGHTS if self.punctual_lights else 0) | (PARAM_EMISSION_MAPS if self.emission_maps else 0))
         if self.lens_radius != 0:   # a negative or NaN radius is set too, so that the library rejects it
             if self.focus_distance is None:
                 raise ValueError("RenderConfig: a lens (lens_radius != 0) needs a focus_distance")
@@ -424,6 +426,34 @@ class Scene:
         mr = np.ascontiguousarray(np.asarray(metal_rough_id, np.int32).reshape(n))
         nm = np.ascontiguousarray(np.asarray(normal_id, np.int32).reshape(n))
         check(lib.ezrt_scene_set_material_maps(self._h, mr.ctypes.data_as(C.POINTER(C.c_int32)), nm.ctypes.data_as(C.POINTER(C.c_int32))))
+
+    def set_emission_maps(self, emission_id):
+        """ezrt_scene_set_emission_maps: the emission maps RenderConfig.emission_maps renders (DESIGN.md section 18).  emission_id [N] int:
+        per triangle (in the order of the scene's triangles) the id of its emission texture among the textures of set_textures (-1: no
+        map).  Builds the emission table.  set_emission_maps(None) clears them; set_textures clears them too."""
+        if emission_id is None:
+            check(lib.ezrt_scene_set_emission_maps(self._h, None))
+            return
+        ids = np.ascontiguousarray(np.asarray(emission_id, np.int32).reshape(self.tris.shape[0]))
+        check(lib.ezrt_scene_set_emission_maps(self._h, ids.ctypes.data_as(C.POINTER(C.c_int32))))
+
+    def emission_light_table(self):
+        """The emission table (ezrt_scene_emission_lights): (triangle indices int32 [K], cdf float32 [K], lum_eff float32 [K], W = float64
+        sum of the weights).  Scene.lights() stays mode 4's table."""
+        k = check(lib.ezrt_scene_emission_lights(self._h, 0, None, None, None, None))
+        tri, cdf, lum = np.zeros(k, np.int32), np.zeros(k, np.float32), np.zeros(k, np.float32)
+        total = C.c_double(0.0)
+        check(lib.ezrt_scene_emission_lights(self._h, k, tri.ctypes.data_as(_lib.c_int32_p), _fp(cdf), _fp(lum), C.byref(total)))
+        return tri, cdf, lum, total.value
+
+    def sample_emission(self, tri, points):
+        """ezrt_scene_sample_emission: the emission E(Q) ([n, 3]) the emission-map renders read at points ([n, 3]) on reference triangles."""
+        tri = np.ascontiguousarray(np.asarray(tri, np.int32).reshape(-1))
+        pts = np.ascontiguousarray(np.asarray(points, np.float32).reshape(-1, 3))
+        assert pts.shape[0] == tri.shape[0]
+        rgb = np.zeros((tri.shape[0], 3), np.float32)
+        check(lib.ezrt_scene_sample_emission(self._h, tri.shape[0], tri.ctypes.data_as(C.POINTER(C.c_int32)), _fp(pts), _fp(rgb)))
+        return rgb
 
     def set_punctual_lights(self, lights):
         """ezrt_scene_set_punctual_lights: the punctual lights RenderConfig.punctual_lights renders (DESIGN.md section 17), a sequence of

@@ -124,6 +124,15 @@ struct ezrt_scene {
     DeviceBuffer punct_buf;
     PunctDev punct{};
     float vbox_min[3] = {0, 0, 0}, vbox_max[3] = {0, 0, 0};   // the triangles' vertex box (the directional lights' weight)
+    // the emission maps of EZRT_PARAM_EMISSION_MAPS (ezrt_scene_set_emission_maps): the per-triangle records in reference | accel
+    // order, and the emission table (records | cdf) with its host copy; emit.sh_emit is set per render
+    bool has_emit = false;
+    DeviceBuffer emit_buf, emit_lights_buf;
+    EmitDev emit{};
+    LightsDev emit_lights{};
+    std::vector<int32_t> emit_tri;
+    std::vector<float> emit_cdf, emit_lum;
+    double emit_total = 0.0;
     void* hot_base = nullptr;   // accel nodes | geometry (| vertices) | shading records (L2 persisting window)
     size_t hot_bytes = 0;
     size_t l2_persist_bytes = 0;
@@ -237,6 +246,11 @@ int validate_params(const ezrt_scene* scene, const ezrt_render_params* p) {
             return ezrt_set_error(EZRT_ERR_INVALID, "render: EZRT_PARAM_MATERIAL_MAPS needs EZRT_PARAM_TEXTURES");
         if (!scene->has_maps) return ezrt_set_error(EZRT_ERR_INVALID, "render: EZRT_PARAM_MATERIAL_MAPS needs maps (ezrt_scene_set_material_maps)");
     }
+    if (p->reserved[0] & EZRT_PARAM_EMISSION_MAPS) {
+        if (!(p->reserved[0] & EZRT_PARAM_TEXTURES))
+            return ezrt_set_error(EZRT_ERR_INVALID, "render: EZRT_PARAM_EMISSION_MAPS needs EZRT_PARAM_TEXTURES");
+        if (!scene->has_emit) return ezrt_set_error(EZRT_ERR_INVALID, "render: EZRT_PARAM_EMISSION_MAPS needs emission maps (ezrt_scene_set_emission_maps)");
+    }
     if (p->reserved[0] & EZRT_PARAM_PUNCTUAL_LIGHTS) {
         if (p->mode != EZRT_MODE_DISNEY_LIGHTS)
             return ezrt_set_error(EZRT_ERR_INVALID, "render: EZRT_PARAM_PUNCTUAL_LIGHTS needs the light sampling mode (got mode %d)", p->mode);
@@ -308,20 +322,21 @@ struct AovRun {
     float* d_luma2;
 };
 
-// The light table of the light sampling mode (ezrt_math.h, DESIGN.md section 10), built once per scene on stream st from the
-// scene's own records: every triangle's weight, the lights kept in triangle order, their weights summed in float64 on the host,
-// the cdf and the 64-byte records uploaded.  Synchronises st.
-int build_lights(ezrt_scene* s, cudaStream_t st) {
-    if (s->lights_built) return EZRT_OK;
+// A light table of the light sampling mode (ezrt_math.h, DESIGN.md section 10) from every triangle's weight d_w (n floats in
+// tmp, reference order; tmp holds 2 n floats and n + 4 ints): the lights kept in triangle order, their weights summed in float64 on
+// the host, the cdf and the 64-byte records uploaded into buf; with emit_rec (an emission table, section 18) the records' fourth
+// word is each light's lum_eff, also returned in *lum.  Synchronises st.  buf is written only once the table is known.
+struct LightTable {
+    LightsDev dev{};
+    std::vector<int32_t> tri;   // the lights' triangles (caller's order)
+    std::vector<float> cdf, lum;
+    double total = 0.0;         // W, the float64 sum of the weights
+};
+int light_table(ezrt_scene* s, float* d_w, const float2* emit_rec, DeviceBuffer& buf, LightTable& out, cudaStream_t st) {
     const int n = s->dev.n_triangles;
-    struct TmpBuffer : DeviceBuffer { ~TmpBuffer() { release(); } } tmp;
-    int rc = tmp.ensure(sizeof(float) * 2 * (size_t)n + sizeof(int32_t) * ((size_t)n + 4));
-    if (rc) return rc;
-    float* d_w = (float*)tmp.p;
     float* d_wk = d_w + n;
     int32_t* d_idx = (int32_t*)(d_wk + n);
     int32_t* d_count = d_idx + n;
-    launch_light_weights(s->dev, d_w, st);
     launch_light_compact(d_w, n, d_idx, d_wk, d_count, st);
     int32_t K = 0;
     CU_CHECK(cudaMemcpyAsync(&K, d_count, sizeof(K), cudaMemcpyDeviceToHost, st));
@@ -335,7 +350,7 @@ int build_lights(ezrt_scene* s, cudaStream_t st) {
     }
     double W = 0.0;
     for (int k = 0; k < K; k++) W += (double)w[k];
-    std::vector<float> cdf(K);
+    std::vector<float> cdf(K), lum;
     double S = 0.0;
     for (int k = 0; k < K; k++) {
         S += (double)w[k];
@@ -345,20 +360,45 @@ int build_lights(ezrt_scene* s, cudaStream_t st) {
     LightsDev lt{};
     if (K > 0) {
         const size_t rec_bytes = sizeof(float4) * 4 * (size_t)K;
-        if ((rc = s->lights_buf.ensure(rec_bytes + sizeof(float) * (size_t)K))) return rc;
-        lt.rec = (const float4*)s->lights_buf.p;
-        lt.cdf = (const float*)((char*)s->lights_buf.p + rec_bytes);
+        int rc = buf.ensure(rec_bytes + sizeof(float) * (size_t)K);
+        if (rc) return rc;
+        lt.rec = (const float4*)buf.p;
+        lt.cdf = (const float*)((char*)buf.p + rec_bytes);
         launch_light_records(s->dev, d_idx, K, (float4*)lt.rec, st);
+        if (emit_rec) {
+            launch_emit_records(emit_rec, d_idx, K, (float4*)lt.rec, st);
+            lum.resize(K);
+            CU_CHECK(cudaMemcpy2DAsync(lum.data(), sizeof(float), (const char*)lt.rec + 60, 64, sizeof(float), K, cudaMemcpyDeviceToHost, st));
+        }
         CU_CHECK(cudaMemcpyAsync((void*)lt.cdf, cdf.data(), sizeof(float) * K, cudaMemcpyHostToDevice, st));
-        CU_CHECK(cudaStreamSynchronize(st));   // cdf is pageable host memory; tmp is freed below
+        CU_CHECK(cudaStreamSynchronize(st));   // cdf is pageable host memory; tmp is freed by the caller
     }
     CU_CHECK(cudaGetLastError());
     lt.n = K;
     lt.w_total = (float)W;
-    s->lights = lt;
-    s->light_tri = idx;
-    s->light_cdf = cdf;
-    s->light_total = W;
+    out.dev = lt;
+    out.tri = idx;
+    out.cdf = cdf;
+    out.lum = lum;
+    out.total = W;
+    return EZRT_OK;
+}
+
+// The light table of the light sampling mode, built once per scene on stream st from the scene's own records (light_table over
+// every triangle's weight).  Synchronises st.
+int build_lights(ezrt_scene* s, cudaStream_t st) {
+    if (s->lights_built) return EZRT_OK;
+    const int n = s->dev.n_triangles;
+    struct TmpBuffer : DeviceBuffer { ~TmpBuffer() { release(); } } tmp;
+    int rc = tmp.ensure(sizeof(float) * 2 * (size_t)n + sizeof(int32_t) * ((size_t)n + 4));
+    if (rc) return rc;
+    launch_light_weights(s->dev, (float*)tmp.p, st);
+    LightTable t;
+    if ((rc = light_table(s, (float*)tmp.p, nullptr, s->lights_buf, t, st))) return rc;
+    s->lights = t.dev;
+    s->light_tri = t.tri;
+    s->light_cdf = t.cdf;
+    s->light_total = t.total;
     s->lights_built = true;
     return EZRT_OK;
 }
@@ -424,6 +464,19 @@ int build_env(ezrt_scene* s, cudaStream_t st) {
     s->env_total = T;
     s->env_built = true;
     return EZRT_OK;
+}
+
+// drops the scene's emission maps (the caller has waited for the renders that read them)
+void clear_emission_maps(ezrt_scene* s) {
+    s->emit_buf.release();
+    s->emit_lights_buf.release();
+    s->has_emit = false;
+    s->emit = EmitDev{};
+    s->emit_lights = LightsDev{};
+    s->emit_tri.clear();
+    s->emit_cdf.clear();
+    s->emit_lum.clear();
+    s->emit_total = 0.0;
 }
 
 RenderDev make_render_dev(const ezrt_scene* s, const ezrt_render_params* p) {
@@ -960,6 +1013,7 @@ int ezrt_scene_set_textures(ezrt_scene* s, int n_textures, const ezrt_texture* t
         s->tex_buf.release(); s->tex_rec_buf.release();
         s->has_textures = false;
         s->has_maps = false;
+        clear_emission_maps(s);
         s->n_textures = 0;
         s->tex = TexDev{};
         s->maps = MapsDev{};
@@ -1038,6 +1092,102 @@ int ezrt_scene_set_textures(ezrt_scene* s, int n_textures, const ezrt_texture* t
     s->has_textures = true;
     s->n_textures = n_textures;
     s->has_maps = false;   // the new records' fourth words are 0: the maps' ids referred to the previous textures
+    clear_emission_maps(s);   // ... and so did the emission maps' (the synchronisation above covers their buffers)
+    return EZRT_OK;
+}
+
+int ezrt_scene_set_emission_maps(ezrt_scene* s, const int32_t* emission_id) {
+    if (!s) return ezrt_set_error(EZRT_ERR_INVALID, "scene_set_emission_maps: null scene");
+    CU_CHECK(cudaSetDevice(s->device));
+    if (!emission_id) {
+        CU_CHECK(cudaDeviceSynchronize());   // renders already enqueued still read the buffers
+        clear_emission_maps(s);
+        return EZRT_OK;
+    }
+    if (!s->has_textures) return ezrt_set_error(EZRT_ERR_INVALID, "scene_set_emission_maps: no textures (ezrt_scene_set_textures)");
+    const int n = s->dev.n_triangles;
+    for (int i = 0; i < n; i++)
+        if (emission_id[i] < -1 || emission_id[i] >= s->n_textures)
+            return ezrt_set_error(EZRT_ERR_INVALID, "scene_set_emission_maps: triangle %d has emission id %d (valid: -1 to %d)", i, emission_id[i],
+                                  s->n_textures - 1);
+    // the new buffers are filled before the previous ones are released, so that a failure keeps the previous maps
+    cudaStream_t st = s->own_stream;
+    struct TmpBuffer : DeviceBuffer { ~TmpBuffer() { release(); } } tmp;
+    DeviceBuffer nrec, nlights;
+    int rc = tmp.ensure(sizeof(float) * 2 * (size_t)n + sizeof(int32_t) * (2 * (size_t)n + 4));
+    if (!rc) rc = nrec.ensure(2 * sizeof(float2) * (size_t)n);
+    if (rc) { nrec.release(); return rc; }
+    float* d_w = (float*)tmp.p;
+    int32_t* d_ids = (int32_t*)(d_w + 2 * (size_t)n) + n + 4;
+    float2* d_rec = (float2*)nrec.p;
+    float2* d_acc = d_rec + n;
+    LightTable t;
+    cudaError_t e = cudaMemcpyAsync(d_ids, emission_id, sizeof(int32_t) * (size_t)n, cudaMemcpyHostToDevice, st);
+    if (e == cudaSuccess) {
+        launch_emit_weights(s->dev, s->tex, d_ids, s->dev.acc_tri_ref, d_rec, d_acc, d_w, st);
+        e = cudaGetLastError();
+    }
+    if (e != cudaSuccess) {
+        nrec.release();
+        return ezrt_set_error(EZRT_ERR_CUDA, "scene_set_emission_maps: %s", cudaGetErrorString(e));
+    }
+    if ((rc = light_table(s, d_w, d_rec, nlights, t, st))) {
+        nrec.release(); nlights.release();
+        return rc;
+    }
+    e = cudaDeviceSynchronize();   // renders already enqueued still read the previous buffers
+    if (e != cudaSuccess) {
+        nrec.release(); nlights.release();
+        return ezrt_set_error(EZRT_ERR_CUDA, "scene_set_emission_maps: %s", cudaGetErrorString(e));
+    }
+    clear_emission_maps(s);
+    s->emit_buf = nrec;   // DeviceBuffer frees only on release(): the pointers move to the scene
+    s->emit_lights_buf = nlights;
+    s->emit.rec = d_rec;
+    s->emit.acc_rec = s->dev.acc_tri_ref ? d_acc : d_rec;
+    s->emit_lights = t.dev;
+    s->emit_tri = t.tri;
+    s->emit_cdf = t.cdf;
+    s->emit_lum = t.lum;
+    s->emit_total = t.total;
+    s->has_emit = true;
+    return EZRT_OK;
+}
+
+int ezrt_scene_emission_lights(ezrt_scene* s, int cap, int32_t* tri_out, float* cdf_out, float* lum_out, double* total_out) {
+    if (!s || cap < 0) return ezrt_set_error(EZRT_ERR_INVALID, "scene_emission_lights: bad argument");
+    if (!s->has_emit) return ezrt_set_error(EZRT_ERR_INVALID, "scene_emission_lights: no emission maps (ezrt_scene_set_emission_maps)");
+    const int K = (int)s->emit_tri.size();
+    const int m = std::min(K, cap);
+    if (tri_out) std::copy(s->emit_tri.begin(), s->emit_tri.begin() + m, tri_out);
+    if (cdf_out) std::copy(s->emit_cdf.begin(), s->emit_cdf.begin() + m, cdf_out);
+    if (lum_out) std::copy(s->emit_lum.begin(), s->emit_lum.begin() + m, lum_out);
+    if (total_out) *total_out = s->emit_total;
+    return K;
+}
+
+int ezrt_scene_sample_emission(ezrt_scene* s, int n, const int32_t* tri, const float* points, float* rgb_out) {
+    if (!s || n < 0 || (n > 0 && (!tri || !points || !rgb_out))) return ezrt_set_error(EZRT_ERR_INVALID, "scene_sample_emission: bad argument");
+    if (!s->has_textures) return ezrt_set_error(EZRT_ERR_INVALID, "scene_sample_emission: no textures (ezrt_scene_set_textures)");
+    for (int i = 0; i < n; i++)
+        if (tri[i] < 0 || tri[i] >= s->dev.n_triangles) return ezrt_set_error(EZRT_ERR_INVALID, "scene_sample_emission: triangle %d out of range", tri[i]);
+    if (n == 0) return EZRT_OK;
+    CU_CHECK(cudaSetDevice(s->device));
+    DeviceBuffer buf;
+    int rc = buf.ensure(sizeof(float) * 7 * (size_t)n + 256);
+    if (rc) return rc;
+    int32_t* d_tri = (int32_t*)buf.p;
+    float* d_p = (float*)(d_tri + n);
+    float* d_rgb = d_p + 3 * (size_t)n;
+    cudaError_t e = cudaMemcpy(d_tri, tri, sizeof(int32_t) * (size_t)n, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = cudaMemcpy(d_p, points, sizeof(float) * 3 * (size_t)n, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) {
+        launch_sample_emission(s->dev, s->tex, s->has_emit ? s->emit : EmitDev{}, n, d_tri, d_p, d_rgb, 0);
+        e = cudaGetLastError();
+    }
+    if (e == cudaSuccess) e = cudaMemcpy(rgb_out, d_rgb, sizeof(float) * 3 * (size_t)n, cudaMemcpyDeviceToHost);
+    buf.release();
+    if (e != cudaSuccess) return ezrt_set_error(EZRT_ERR_CUDA, "scene_sample_emission: %s", cudaGetErrorString(e));
     return EZRT_OK;
 }
 
@@ -1206,6 +1356,7 @@ int ezrt_scene_destroy(ezrt_scene* s) {
     s->adapt_buf.release(); s->adapt_maps_buf.release();
     s->aov_rec_buf.release(); s->aov_maps_buf.release(); s->denoise_buf.release(); s->denoise_io_buf.release();
     s->lights_buf.release(); s->env_buf.release(); s->tex_buf.release(); s->tex_rec_buf.release(); s->punct_buf.release();
+    s->emit_buf.release(); s->emit_lights_buf.release();
     if (s->own_stream) cudaStreamDestroy(s->own_stream);
     if (s->copy_stream) cudaStreamDestroy(s->copy_stream);
     if (s->side_stream) cudaStreamDestroy(s->side_stream);
@@ -1231,6 +1382,13 @@ static int light_options(ezrt_scene* s, const ezrt_render_params* p, cudaStream_
     int rc = build_lights(s, st);
     if (rc) return rc;
     o.lights = s->lights;
+    // EZRT_PARAM_EMISSION_MAPS (validated: with the textures, and maps are set): the emission table is the render's light table, from
+    // which P_env and P_p below follow; emit.sh_emit is carved with the shadow queue
+    if (p->reserved[0] & EZRT_PARAM_EMISSION_MAPS) {
+        o.lights = s->emit_lights;
+        o.emit = s->emit;
+        o.emap_on = true;
+    }
     // EZRT_PARAM_ENV_LIGHT: the map is one more light when the scene has a table (P_env = 1/2 beside triangle lights, 1 without);
     // without a table the render is mode 4's, and mode 4's kernels run
     if (p->reserved[0] & EZRT_PARAM_ENV_LIGHT) {
@@ -1326,7 +1484,7 @@ static int render_device_impl(ezrt_scene* s, const ezrt_render_params* p, float*
     {   // bound the batch by the memory that is actually there (scratch already held by this scene counts as available);
         // asked once per (slots per frame, integrator): cudaMemGetInfo is a driver round trip, the render path is launch-only
         const size_t per_slot = 2 * (sizeof(float4) * 4 + sizeof(float2)) + 2 * sizeof(float4) + sizeof(uint32_t) +
-                                (is_mode ? (size_t)EZRT_SHADOW_SLOT_BYTES : 0) + (lopt.tex_on ? sizeof(float4) : 0) + (lopt.maps_on ? sizeof(float) : 0) + (s->sort_rays ? 2 * sizeof(uint32_t) : 0) +
+                                (is_mode ? (size_t)EZRT_SHADOW_SLOT_BYTES : 0) + (lopt.tex_on ? sizeof(float4) : 0) + (lopt.maps_on ? sizeof(float) : 0) + (lopt.emap_on ? sizeof(float4) : 0) + (s->sort_rays ? 2 * sizeof(uint32_t) : 0) +
                                 (av ? 2 * sizeof(float4) : 0);
         if (s->fmax_key[0] != per_frame || s->fmax_key[1] != per_slot) {
             size_t free_b = 0, total_b = 0;
@@ -1362,6 +1520,17 @@ static int render_device_impl(ezrt_scene* s, const ezrt_render_params* p, float*
         if ((rc = carve_shadow(s->shadow_buf, capacity, sq))) return rc;
         lopt.tex.sh_base = (float4*)((((uintptr_t)sq.lit + capacity) + 255) & ~(uintptr_t)255);
         lopt.maps.sh_metal = (float*)((((uintptr_t)(lopt.tex.sh_base + capacity)) + 255) & ~(uintptr_t)255);
+    }
+    if (lopt.emap_on) {   // ... and the triangle light samples' E(Q) after all of those
+        if ((rc = s->shadow_buf.ensure(((size_t)EZRT_SHADOW_SLOT_BYTES + 2 * sizeof(float4) + sizeof(float)) * capacity + 1024))) return rc;
+        if ((rc = carve_shadow(s->shadow_buf, capacity, sq))) return rc;
+        lopt.tex.sh_base = (float4*)((((uintptr_t)sq.lit + capacity) + 255) & ~(uintptr_t)255);
+        uintptr_t end = (uintptr_t)(lopt.tex.sh_base + capacity);
+        if (lopt.maps_on) {
+            lopt.maps.sh_metal = (float*)((end + 255) & ~(uintptr_t)255);
+            end = (uintptr_t)(lopt.maps.sh_metal + capacity);
+        }
+        lopt.emit.sh_emit = (float4*)((end + 255) & ~(uintptr_t)255);
     }
     float4* aov_rec = nullptr;   // feature-buffer render only: the first-hit record of every sample slot
     if (av) {

@@ -2008,17 +2008,54 @@ __device__ __forceinline__ bool punct_sample(const PunctDev& punct, float r_p, v
     return true;
 }
 
+// EZRT_PARAM_EMISSION_MAPS (ezrt_math.h, DESIGN.md section 18): E at Q of triangle `tri` (the index space of accel_space) with
+// vertices p1..p3, geometric normal Ng and emission texture `id`: ez_emit_eval over the texcoord record, four texels through L1
+__device__ __forceinline__ vec3 emit_tex(const TexDev& tex, int id, int tri, bool accel_space, vec3 Q, vec3 p1, vec3 p2, vec3 p3, vec3 Ng, vec3 E) {
+    const float4* r = (accel_space ? tex.acc_rec : tex.rec) + (size_t)tri * 2;
+    const float4 a = ldg4(r), b = ldg4(r + 1);
+    const float uv6[6] = {a.x, a.y, a.z, a.w, b.x, b.y};
+    const int4 t = __ldg(tex.table + id);
+    return ez_emit_eval(E, Q, p1, p2, p3, Ng, uv6, tex.texels + t.x, t.y, t.z, tex.lut);
+}
+// ... of a hit at Q on triangle `tri` whose emission E has lum(E) > 0: true with E = E(Q), lum_eff and the vertices when the triangle
+// is mapped; false, E unchanged, for emission id -1 (one 8-byte record read)
+__device__ __forceinline__ bool emit_hit(const SceneDev& sc, const TexDev& tex, const EmitDev& emit, int tri, bool accel_space, vec3 Q, vec3& E,
+                                         float& lum_eff, vec3& p1, vec3& p2, vec3& p3) {
+    const float2 er = __ldg((accel_space ? emit.acc_rec : emit.rec) + tri);
+    const int id = __float_as_int(er.x);
+    if (id < 0) return false;
+    lum_eff = er.y;
+    tri_vertices(sc, tri, accel_space, p1, p2, p3);
+    E = emit_tex(tex, id, tri, accel_space, Q, p1, p2, p3, f4xyz(ldg4(tri_geo_rec(sc, tri, accel_space))), E);
+    return true;
+}
+// ... of the triangle light sample with record (a, b, c, e) at ez_triangle_point(r_1, r_2): the light's material's emission, textured
+// when the light is mapped (reference index space, the record's vertices and geometric normal)
+__device__ __forceinline__ vec3 emit_light(const SceneDev& sc, const TexDev& tex, const EmitDev& emit, float4 a, float4 b, float4 c, float4 e,
+                                           float r_1, float r_2) {
+    const vec3 E = load_emissive(sc, __float_as_int(a.w));
+    const int ref = __float_as_int(b.w);
+    const int id = __float_as_int(__ldg(emit.rec + ref).x);
+    if (id < 0) return E;
+    const vec3 Q = ez_triangle_point(f4xyz(a), f4xyz(b), f4xyz(c), r_1, r_2);
+    return emit_tex(tex, id, ref, false, Q, f4xyz(a), f4xyz(b), f4xyz(c), f4xyz(e), E);
+}
+// a light sample whose E(Q) is 0 in every channel is no sample
+__device__ __forceinline__ bool emit_black(vec3 E) { return E.x == 0.0f && E.y == 0.0f && E.z == 0.0f; }
+
 // A medium vertex (EZRT_PARAM_MEDIUM; ezrt_math.h, DESIGN.md section 14): p's segment scattered at t_s before its hit (hit_t,
 // hit_tri) or its miss.  The weights of the segment (bounce >= 1) and the albedo enter the history; then, below max_bounce, one light
 // sample from P as at a surface but without the hemisphere test and the self exclusion (its shadow ray carries EZRT_MEDIUM_VERTEX
 // and d), and the phase function's sample as the next ray with the record (splat(p), p, 1).  Returns false when the path ends.
 // TEX: the first-hit record's albedo is the textured base colour.  MAPS: ... and its normal the mapped one.
 // PUNCT: the light sample is punctual with probability punct.p_p (punct_pick, punct_sample).
-template <bool AOV, bool ENV, bool TEX = false, bool MAPS = false, bool PUNCT = false>
+// EMAP: a triangle light sample's emission is E(Q) (emit_light), out through *sh_E; none where it is black.
+template <bool AOV, bool ENV, bool TEX = false, bool MAPS = false, bool PUNCT = false, bool EMAP = false>
 __device__ __forceinline__ bool medium_step(const SceneDev& sc, const RenderDev& rd, int bounce, PathRegs& p, float t_s, float hit_t,
                                             int hit_tri, vec3& Lo, vec3& Le, bool& primary_miss, ShadowRay& sh, float4* aov_rec,
                                             const LightsDev& lights, const EnvDev& env, const MediumDev& med, const TexDev& tex = TexDev{},
-                                            const MapsDev& maps = MapsDev{}, const PunctDev& punct = PunctDev{}) {
+                                            const MapsDev& maps = MapsDev{}, const PunctDev& punct = PunctDev{}, const EmitDev& emit = EmitDev{},
+                                            vec3* sh_E = nullptr) {
     if (bounce == 0) {
         Lo = splat3(0.0f);
         Le = splat3(0.0f);
@@ -2074,7 +2111,14 @@ __device__ __forceinline__ bool medium_step(const SceneDev& sc, const RenderDev&
         const float dist = EZ_SQRT(ez_dot(D, D));
         const vec3 Ll = ez_normalize(D);
         const float cos_l = ez_abs(ez_dot(f4xyz(e), Ll));
-        if (cos_l != 0.0f && dist != 0.0f) {
+        bool emits = true;
+        if constexpr (EMAP) {
+            if (cos_l != 0.0f && dist != 0.0f) {
+                *sh_E = emit_light(sc, tex, emit, a, b, c, e, r_1, r_2);
+                emits = !emit_black(*sh_E);
+            }
+        }
+        if (cos_l != 0.0f && dist != 0.0f && emits) {
             sh.valid = true;
             sh.d = Ll;
             sh.tmax = ez_light_tmax(dist);
@@ -2124,13 +2168,17 @@ __device__ __forceinline__ bool medium_step(const SceneDev& sc, const RenderDev&
 // PUNCT (light sampling mode with EZRT_PARAM_PUNCTUAL_LIGHTS, ezrt_math.h, DESIGN.md section 17): the light sample is punctual with
 // probability punct.p_p (punct_pick, punct_sample); the triangle and map samples' pdfs and the MIS weights of BSDF samples that reach
 // those lights take the factor 1 - p_p.
+// EMAP (with TEX; EZRT_PARAM_EMISSION_MAPS, ezrt_math.h, DESIGN.md section 18): a mapped emitter's emission is E(Q) at the camera
+// ray's hit and at BSDF-sample emission hits (emit_hit), whose MIS uses the triangle's lum_eff and the emission table `lights`; a
+// triangle light sample's emission is E(Q) (emit_light), out through *sh_E for k_nee, and a black one is no sample.
 template <int MODE, bool DEFER_NEE = false, bool AOV = false, bool ENV = false, bool TRANS = false, bool MEDIUM = false, bool TEX = false,
-          bool MAPS = false, bool PUNCT = false>
+          bool MAPS = false, bool PUNCT = false, bool EMAP = false>
 __device__ __forceinline__ bool shade_step(const SceneDev& sc, const RenderDev& rd, int bounce, PathRegs& p, float hit_t,
                                            int hit_tri, uint32_t px, uint32_t py, float2 sob, vec3& Lo, vec3& Le,
                                            bool& primary_miss, ShadowRay& sh, float4* aov_rec = nullptr, LightsDev lights = LightsDev{},
                                            EnvDev env = EnvDev{}, MediumDev med = MediumDev{}, TexDev tex = TexDev{}, vec3* sh_base = nullptr,
-                                           float2* sh_rm = nullptr, MapsDev maps = MapsDev{}, PunctDev punct = PunctDev{}) {
+                                           float2* sh_rm = nullptr, MapsDev maps = MapsDev{}, PunctDev punct = PunctDev{}, EmitDev emit = EmitDev{},
+                                           vec3* sh_E = nullptr) {
     sh.valid = false;
     const int mode = (MODE < 0) ? rd.mode : MODE;
     const bool is_mode = (mode == EZRT_MODE_DISNEY_IS_MIS_P5);
@@ -2139,14 +2187,15 @@ __device__ __forceinline__ bool shade_step(const SceneDev& sc, const RenderDev& 
     const bool below = TRANS && p.cosine_i < 0.0f;   // the BSDF sample went below the surface: no light strategy reaches it
     static_assert(lights_mode || !TEX, "textures are rendered in the light sampling mode");
     static_assert(TEX || !MAPS, "material maps are rendered with the textures");
+    static_assert(TEX || !EMAP, "emission maps are rendered with the textures");
     if constexpr (MEDIUM) {
         static_assert(lights_mode && !TRANS, "the medium is rendered in the light sampling mode, without transmission");
         if (bounce > 0 && p.pdf <= 0.0f) return false;   // P5/fsh:865, before the free flight's draw
         float t_s;
         const float t_end = (hit_tri < 0) ? __int_as_float(0x7f800000) : hit_t;
         if (ez_medium_flight(&med, p.o, p.d, t_end, &p.seed, &t_s))
-            return medium_step<AOV, ENV, TEX, MAPS, PUNCT>(sc, rd, bounce, p, t_s, hit_t, hit_tri, Lo, Le, primary_miss, sh, aov_rec, lights, env, med, tex,
-                                                           maps, punct);
+            return medium_step<AOV, ENV, TEX, MAPS, PUNCT, EMAP>(sc, rd, bounce, p, t_s, hit_t, hit_tri, Lo, Le, primary_miss, sh, aov_rec, lights, env, med,
+                                                                 tex, maps, punct, emit, sh_E);
     }
     if (bounce == 0) {
         Lo = splat3(0.0f);
@@ -2196,12 +2245,39 @@ __device__ __forceinline__ bool shade_step(const SceneDev& sc, const RenderDev& 
     }
     if (bounce == 0) {
         Le = mat.emissive;  // P5/fsh:936
+        if constexpr (EMAP) {
+            if (ez_luminance(Le) > 0.0f) {
+                float lum_eff;
+                vec3 p1, p2, p3;
+                emit_hit(sc, tex, emit, hit_tri, rd.accel_space != 0, hit.P, Le, lum_eff, p1, p2, p3);
+            }
+        }
         if (AOV) {
             aov_rec[0] = make_float4(mat.baseColor.x, mat.baseColor.y, mat.baseColor.z, hit_t);
             aov_rec[1] = make_float4(hit.N.x, hit.N.y, hit.N.z, 0.0f);
         }
     } else {
-        if (lights_mode) {   // a BRDF sample that hit a light: MIS against the light sampling pdf of the hit point
+        if (EMAP && lights_mode) {   // ... with the emission maps: E(Q), and a mapped light's lum_eff
+            float w = 1.0f;
+            vec3 E = mat.emissive;
+            const float lum = ez_luminance(E);
+            if (lum > 0.0f) {
+                vec3 p1, p2, p3;
+                float lum_eff;
+                const bool mapped = emit_hit(sc, tex, emit, hit_tri, rd.accel_space != 0, hit.P, E, lum_eff, p1, p2, p3);
+                if (!below) {
+                    if (!mapped) tri_vertices(sc, hit_tri, rd.accel_space != 0, p1, p2, p3);
+                    if (ez_is_light(mapped ? ez_triangle_area(p1, p2, p3) * lum_eff : ez_light_weight(p1, p2, p3, mat.emissive))) {
+                        const vec3 Ng = f4xyz(ldg4(tri_geo_rec(sc, hit_tri, rd.accel_space != 0)));
+                        float pl = ez_light_pdf(mapped ? lum_eff : lum, lights.w_total, hit_t, ez_abs(ez_dot(Ng, p.d)));
+                        if constexpr (ENV) pl = (1.0f - env.p_env) * pl;
+                        if constexpr (PUNCT) pl = (1.0f - punct.p_p) * pl;
+                        w = mis_mix_weight(p.pdf, pl);
+                    }
+                }
+            }
+            Lo = ez_add(Lo, ez_divs(ez_scale(ez_mul(ez_mul(ez_scale(p.history, w), E), p.f_r), path_cos<TRANS>(p.cosine_i)), p.pdf));
+        } else if (lights_mode) {   // a BRDF sample that hit a light: MIS against the light sampling pdf of the hit point
             float w = 1.0f;
             const float lum = ez_luminance(mat.emissive);
             if (lum > 0.0f && !below) {   // lum <= 0: the weight area * lum is never a light; below: weight 1
@@ -2292,7 +2368,14 @@ __device__ __forceinline__ bool shade_step(const SceneDev& sc, const RenderDev& 
             const float dist = EZ_SQRT(ez_dot(D, D));
             const vec3 Ll = ez_normalize(D);
             const float cos_l = ez_abs(ez_dot(f4xyz(e), Ll));
-            if (self != hit_tri && ez_dot(N, Ll) > 0.0f && cos_l != 0.0f && dist != 0.0f) {
+            bool emits = true;
+            if constexpr (EMAP) {
+                if (self != hit_tri && ez_dot(N, Ll) > 0.0f && cos_l != 0.0f && dist != 0.0f) {
+                    *sh_E = emit_light(sc, tex, emit, a, b, c, e, r_1, r_2);
+                    emits = !emit_black(*sh_E);
+                }
+            }
+            if (self != hit_tri && ez_dot(N, Ll) > 0.0f && cos_l != 0.0f && dist != 0.0f && emits) {
                 sh.valid = true;
                 sh.o = hit.P;
                 sh.d = Ll;

@@ -190,6 +190,20 @@ struct PunctDev {
     float p_p;
 };
 
+// The emission maps of EZRT_PARAM_EMISSION_MAPS (ezrt_math.h, DESIGN.md section 18), set by ezrt_scene_set_emission_maps.  Passed to
+// every k_shade / k_nee instantiation as their last parameter, after PunctDev, so that no other parameter moves; read by the
+// emission-map instantiations (<.., EMAP>) only.  Their light table is the emission table (LightsDev, the records' fourth word
+// lum_eff), passed in place of mode 4's.
+//   rec / acc_rec: 8 bytes per triangle, (emission id as bits, lum_eff), in reference and in accel order; read only for triangles
+//       with lum(E_T) > 0
+//   sh_emit: E(Q) of every shadow slot's triangle light sample (16 B per slot, carved after the other per-slot arrays for the
+//       flagged renders only), read back by k_nee
+struct EmitDev {
+    const float2* rec;
+    const float2* acc_rec;
+    float4* sh_emit;
+};
+
 // A shadow ray and what k_nee needs to evaluate the light sample's contribution once the ray got through (nee_contrib):
 // the BRDF / environment evaluation of the light sample is done after the shadow pass, for unoccluded rays only.
 #define EZRT_SHADOW_SLOT_BYTES (5 * 16 + 1)

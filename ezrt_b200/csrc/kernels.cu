@@ -553,15 +553,17 @@ __global__ void __launch_bounds__(EZRT_EXTEND_MAX_THREADS, EZRT_EXTEND_LB_BLOCKS
 // tex.sh_base[spos].w and the mapped metallic in maps.sh_metal[spos].
 // PUNCT (light sampling mode with EZRT_PARAM_PUNCTUAL_LIGHTS): the punctual lights punct are one more category of light samples
 // (shade_step); a punctual sample's slot carries hist.w = -2 - j and its scale in view.w.
+// EMAP (with TEX; EZRT_PARAM_EMISSION_MAPS): the emission maps emit, and lights is the emission table (shade_step); a triangle light
+// sample's slot also gets its E(Q) in emit.sh_emit[spos].
 template <int MODE, bool LIST, bool AOV = false, bool ENV = false, bool TRANS = false, bool MEDIUM = false, bool TEX = false,
-          bool MAPS = false, bool PUNCT = false>
+          bool MAPS = false, bool PUNCT = false, bool EMAP = false>
 __global__ void __launch_bounds__(128, EZRT_SHADE_MIN_BLOCKS) k_shade(SceneDev sc, RenderDev rd, const TileDev* __restrict__ tiles, int bounce,
                                                uint32_t batch_first_frame, PathQueue qin, const uint32_t* __restrict__ in_count,
                                                PathQueue qout, uint32_t* out_count, ShadowQueue sq, uint32_t* s_count,
                                                float4* __restrict__ Lo, float4* __restrict__ Le, uint32_t n_fused, uint32_t n_frames,
                                                const uint32_t* __restrict__ list, const float2* __restrict__ side_hit,
                                                float4* __restrict__ aov_rec, LightsDev lights, EnvDev env, MediumDev med, TexDev tex,
-                                               MapsDev maps, PunctDev punct) {
+                                               MapsDev maps, PunctDev punct, EmitDev emit) {
     // The Sobol pair of (bounce, frame) is the same for every pixel of a frame (P5/fsh:361-376: up to 2 x 32 table XORs per path): each
     // block computes the pairs of the batch's frames once into shared memory (batches of more than EZRT_SOBOL_TABLE frames compute per path).
     __shared__ float2 s_sobol[EZRT_SOBOL_TABLE];
@@ -600,6 +602,7 @@ __global__ void __launch_bounds__(128, EZRT_SHADE_MIN_BLOCKS) k_shade(SceneDev s
         sh.valid = false;
         vec3 sh_base;   // TEX: the shading point's textured base colour
         float2 sh_rm;   // MAPS: its mapped roughness and metallic
+        vec3 sh_E;      // EMAP: the triangle light sample's E(Q)
         uint32_t slot = 0;
         uint32_t px = 0, py = 0, fib = 0;
         bool present = i < n;
@@ -687,9 +690,9 @@ __global__ void __launch_bounds__(128, EZRT_SHADE_MIN_BLOCKS) k_shade(SceneDev s
             }
 #endif
             if (LIST || __float_as_int(hit.y) != EZRT_TRI_PENDING) {   // pending: deferred by the accel kernel, shaded by the LIST pass
-                alive = shade_step<MODE, MODE == EZRT_MODE_DISNEY_IS_MIS_P5, AOV, ENV, TRANS, MEDIUM, TEX, MAPS, PUNCT>(sc, rd, bounce, p, hit.x, __float_as_int(hit.y), px, py,
+                alive = shade_step<MODE, MODE == EZRT_MODE_DISNEY_IS_MIS_P5, AOV, ENV, TRANS, MEDIUM, TEX, MAPS, PUNCT, EMAP>(sc, rd, bounce, p, hit.x, __float_as_int(hit.y), px, py,
                                                                                                           sob, lo, le, pmiss, sh, AOV ? aov_rec + 2 * (size_t)slot : nullptr,
-                                                                                                          lights, env, med, tex, &sh_base, &sh_rm, maps, punct);
+                                                                                                          lights, env, med, tex, &sh_base, &sh_rm, maps, punct, emit, &sh_E);
                 if (bounce == 0) {
                     // Le is zero for every surface that does not emit: it is stored (and read back by k_blend) only otherwise.
                     // color = Le + Lo with Le = +-0 is Lo bit for bit, because Lo is never -0.0 (it starts at +0.0 and only grows by additions)
@@ -724,6 +727,9 @@ __global__ void __launch_bounds__(128, EZRT_SHADE_MIN_BLOCKS) k_shade(SceneDev s
                         if constexpr (MAPS) __stcs(maps.sh_metal + spos, sh_rm.y);
                     }
                 }
+                if constexpr (EMAP) {
+                    if (sh.light_mat >= 0) __stcs(emit.sh_emit + spos, make_float4(sh_E.x, sh_E.y, sh_E.z, 0.0f));
+                }
             }
         }
     }
@@ -744,9 +750,11 @@ __global__ void __launch_bounds__(128, EZRT_SHADE_MIN_BLOCKS) k_shade(SceneDev s
 // MAPS: ... and the mapped roughness and metallic, tex.sh_base[j].w and maps.sh_metal[j]; the slot's N is already the mapped normal.
 // PUNCT: and the punctual samples (hist.w = -2 - j): ez_punct_contrib of the shading point's f (the BSDF or mixture at a surface, the
 // phase function at a medium vertex) with light j's intensity * color and the scale in view.w, without a MIS weight.
-template <int MODE, bool ENV = false, bool TRANS = false, bool MEDIUM = false, bool TEX = false, bool MAPS = false, bool PUNCT = false>
+// EMAP: a triangle light sample's emission is the E(Q) k_shade left in emit.sh_emit[j].
+template <int MODE, bool ENV = false, bool TRANS = false, bool MEDIUM = false, bool TEX = false, bool MAPS = false, bool PUNCT = false,
+          bool EMAP = false>
 __global__ void __launch_bounds__(128, 8) k_nee(SceneDev sc, RenderDev rd, ShadowQueue sq, const uint32_t* __restrict__ s_count, float4* __restrict__ Lo,
-                                                MediumDev med, TexDev tex, MapsDev maps, PunctDev punct) {
+                                                MediumDev med, TexDev tex, MapsDev maps, PunctDev punct, EmitDev emit) {
     static_assert(MODE == EZRT_MODE_DISNEY_LIGHTS || !(ENV || TRANS || MEDIUM), "the options exist in the light sampling mode");
     static_assert(!(TRANS && MEDIUM), "the medium is rendered without transmission");
     __shared__ uint32_t s_scan[34];
@@ -786,7 +794,12 @@ __global__ void __launch_bounds__(128, 8) k_nee(SceneDev sc, RenderDev rd, Shado
             vec3 c;
             if constexpr (MODE == EZRT_MODE_DISNEY_LIGHTS) {
                 const int lm = __float_as_int(h4.w);   // the light's material; -1: an environment sample; PUNCT: <= -2 a punctual one
-                const auto light_color = [&] { return (ENV && lm < 0) ? hdr_color(sc, rd, Ld, EZRT_MODE_DISNEY_LIGHTS) : load_emissive(sc, lm); };
+                const auto light_color = [&] {
+                    if constexpr (EMAP) {
+                        if (lm >= 0) return f4xyz(__ldcs(emit.sh_emit + j));
+                    }
+                    return (ENV && lm < 0) ? hdr_color(sc, rd, Ld, EZRT_MODE_DISNEY_LIGHTS) : load_emissive(sc, lm);
+                };
                 if (PUNCT && lm < -1) {
                     const float4* r = punct.rec + 4 * (size_t)(-2 - lm);
                     vec3 f;
@@ -1399,13 +1412,13 @@ static void launch_shade_t(int blocks, const SceneDev& sc, const RenderDev& rd, 
                            float4* Lo, float4* Le, uint32_t n_fused, uint32_t n_frames, const uint32_t* list, const float2* side_hit,
                            float4* aov_rec, const LightOptions& o, cudaStream_t st) {
     auto launch = [&](auto M) {
-        with_bools([&](auto A, auto E, auto T, auto X, auto TX, auto MP, auto P) {
+        with_bools([&](auto A, auto E, auto T, auto X, auto TX, auto MP, auto P, auto EM) {
             // the options exist in the light sampling mode; the maps with the textures
-            if constexpr ((M == EZRT_MODE_DISNEY_LIGHTS || !(E || T || X || TX || P)) && !(T && X) && (TX || !MP))
-                k_shade<M, LIST, A, E, T, X, TX, MP, P><<<blocks, 128, 0, st>>>(sc, rd, tiles, bounce, batch_first_frame, qin, in_count, qout, out_count, sq,
-                                                                                s_count, Lo, Le, n_fused, n_frames, list, side_hit, aov_rec, o.lights, o.env,
-                                                                                o.med, o.tex, o.maps, o.punct);
-        }, aov_rec != nullptr, o.env_on, o.trans_on, o.medium_on, o.tex_on, o.maps_on, o.punct_on);
+            if constexpr ((M == EZRT_MODE_DISNEY_LIGHTS || !(E || T || X || TX || P)) && !(T && X) && (TX || !MP) && (TX || !EM))
+                k_shade<M, LIST, A, E, T, X, TX, MP, P, EM><<<blocks, 128, 0, st>>>(sc, rd, tiles, bounce, batch_first_frame, qin, in_count, qout, out_count, sq,
+                                                                                    s_count, Lo, Le, n_fused, n_frames, list, side_hit, aov_rec, o.lights, o.env,
+                                                                                    o.med, o.tex, o.maps, o.punct, o.emit);
+        }, aov_rec != nullptr, o.env_on, o.trans_on, o.medium_on, o.tex_on, o.maps_on, o.punct_on, o.emap_on);
     };
     switch (rd.mode) {
         case EZRT_MODE_DIFFUSE_P3: launch(std::integral_constant<int, EZRT_MODE_DIFFUSE_P3>{}); break;
@@ -1437,12 +1450,12 @@ void launch_deferred_lane(const SceneDev& sc, const RenderDev& rd, const TileDev
 void launch_nee(const SceneDev& sc, const RenderDev& rd, ShadowQueue sq, const uint32_t* s_count, float4* Lo, uint32_t n_max, int n_sms, cudaStream_t st,
                 const LightOptions& o) {
     const int blocks = std::max(1, std::min(div_up(n_max, 512), n_sms * 8));
-    with_bools([&](auto L, auto E, auto T, auto X, auto TX, auto MP, auto P) {
+    with_bools([&](auto L, auto E, auto T, auto X, auto TX, auto MP, auto P, auto EM) {
         // the options exist in the light sampling mode (the other mode here is mode 3); the maps with the textures
-        if constexpr ((L || !(E || T || X || TX || P)) && !(T && X) && (TX || !MP))
-            k_nee<L ? EZRT_MODE_DISNEY_LIGHTS : EZRT_MODE_DISNEY_IS_MIS_P5, E, T, X, TX, MP, P><<<blocks, 128, 0, st>>>(sc, rd, sq, s_count, Lo, o.med, o.tex, o.maps,
-                                                                                                                    o.punct);
-    }, rd.mode == EZRT_MODE_DISNEY_LIGHTS, o.env_on, o.trans_on, o.medium_on, o.tex_on, o.maps_on, o.punct_on);
+        if constexpr ((L || !(E || T || X || TX || P)) && !(T && X) && (TX || !MP) && (TX || !EM))
+            k_nee<L ? EZRT_MODE_DISNEY_LIGHTS : EZRT_MODE_DISNEY_IS_MIS_P5, E, T, X, TX, MP, P, EM><<<blocks, 128, 0, st>>>(sc, rd, sq, s_count, Lo, o.med, o.tex,
+                                                                                                                        o.maps, o.punct, o.emit);
+    }, rd.mode == EZRT_MODE_DISNEY_LIGHTS, o.env_on, o.trans_on, o.medium_on, o.tex_on, o.maps_on, o.punct_on, o.emap_on);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -1605,6 +1618,66 @@ __global__ void k_maps_set(const uint32_t* __restrict__ words, const uint32_t* _
 }
 void launch_maps_set(const uint32_t* words, const uint32_t* acc_tri_ref, int n, float4* rec, float4* acc_rec, cudaStream_t st) {
     k_maps_set<<<div_up(n, 256), 256, 0, st>>>(words, acc_tri_ref, n, rec, acc_rec);
+}
+// the emission maps' records and emission-table weights (ezrt_scene_set_emission_maps; ezrt_math.h, DESIGN.md section 18): per
+// triangle i (reference order), lum_eff = ez_emit_lum_eff for a mapped emitter (lum(E) > 0, id >= 0), else lum(E); w[i] = area *
+// lum_eff for a mapped emitter, k_light_weights' weight otherwise.  Then the accel order's copy of the records.
+__global__ void __launch_bounds__(256) k_emit_weights(SceneDev sc, TexDev tex, const int32_t* __restrict__ ids, float2* __restrict__ rec,
+                                                      float* __restrict__ w) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= sc.n_triangles) return;
+    vec3 p1, p2, p3;
+    tri_vertices(sc, i, false, p1, p2, p3);
+    const vec3 E = load_emissive(sc, tri_material(sc, i));
+    const int id = ids[i];
+    float lum_eff = ez_luminance(E);
+    if (id >= 0 && lum_eff > 0.0f) {
+        const float4 a = ldg4(tex.rec + 2 * (size_t)i), b = ldg4(tex.rec + 2 * (size_t)i + 1);
+        const float uv6[6] = {a.x, a.y, a.z, a.w, b.x, b.y};
+        const int4 t = __ldg(tex.table + id);
+        lum_eff = ez_emit_lum_eff(E, uv6, tex.texels + t.x, t.y, t.z, tex.lut);
+        w[i] = ez_triangle_area(p1, p2, p3) * lum_eff;
+    } else {
+        w[i] = ez_light_weight(p1, p2, p3, E);
+    }
+    rec[i] = make_float2(__int_as_float(id), lum_eff);
+}
+__global__ void k_emit_gather(const float2* __restrict__ rec, const uint32_t* __restrict__ acc_tri_ref, int n, float2* __restrict__ acc_rec) {
+    const int a = blockIdx.x * blockDim.x + threadIdx.x;
+    if (a < n) acc_rec[a] = rec[acc_tri_ref[a]];
+}
+void launch_emit_weights(const SceneDev& sc, const TexDev& tex, const int32_t* ids, const uint32_t* acc_tri_ref, float2* rec, float2* acc_rec,
+                         float* w, cudaStream_t st) {
+    const int n = sc.n_triangles;
+    if (n <= 0) return;
+    k_emit_weights<<<div_up(n, 256), 256, 0, st>>>(sc, tex, ids, rec, w);
+    if (acc_tri_ref) k_emit_gather<<<div_up(n, 256), 256, 0, st>>>(rec, acc_tri_ref, n, acc_rec);
+}
+__global__ void __launch_bounds__(256) k_emit_records(const float2* __restrict__ emit_rec, const int32_t* __restrict__ idx, int n, float4* __restrict__ rec) {
+    const int k = blockIdx.x * blockDim.x + threadIdx.x;
+    if (k < n) rec[4 * k + 3].w = emit_rec[idx[k]].y;
+}
+void launch_emit_records(const float2* emit_rec, const int32_t* idx, int n, float4* rec, cudaStream_t st) {
+    if (n <= 0) return;
+    k_emit_records<<<div_up(n, 256), 256, 0, st>>>(emit_rec, idx, n, rec);
+}
+// the emission shade_step<.., EMAP> reads at the points of reference triangles (ezrt_scene_sample_emission)
+__global__ void k_sample_emission(SceneDev sc, TexDev tex, EmitDev emit, int n, const int32_t* __restrict__ tri, const float* __restrict__ points,
+                                  float* __restrict__ rgb) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const int t = tri[i];
+    vec3 E = load_emissive(sc, tri_material(sc, t));
+    if (emit.rec && ez_luminance(E) > 0.0f) {
+        float lum_eff;
+        vec3 p1, p2, p3;
+        emit_hit(sc, tex, emit, t, false, ez_v3(points[3 * i], points[3 * i + 1], points[3 * i + 2]), E, lum_eff, p1, p2, p3);
+    }
+    rgb[3 * i] = E.x; rgb[3 * i + 1] = E.y; rgb[3 * i + 2] = E.z;
+}
+void launch_sample_emission(const SceneDev& sc, const TexDev& tex, const EmitDev& emit, int n, const int32_t* tri, const float* points, float* rgb,
+                            cudaStream_t st) {
+    k_sample_emission<<<div_up(n, 128), 128, 0, st>>>(sc, tex, emit, n, tri, points, rgb);
 }
 void launch_eval_math(int which, int n, const float* a, const float* b, float* out, cudaStream_t st) {
     k_eval_math<<<div_up(n, 256), 256, 0, st>>>(which, n, a, b, out);

@@ -24,6 +24,7 @@
 //   tex_on    EZRT_PARAM_TEXTURES: the scene's base-colour textures tex (<.., TEX>)
 //   maps_on   EZRT_PARAM_MATERIAL_MAPS (with tex_on): the material maps of tex (<.., TEX, MAPS>)
 //   punct_on  EZRT_PARAM_PUNCTUAL_LIGHTS and the scene's punctual table has J > 0 lights: punct (<.., PUNCT>)
+//   emap_on   EZRT_PARAM_EMISSION_MAPS (with tex_on): the emission maps emit, and lights is the emission table (<.., TEX, .., EMAP>)
 // All off outside the light sampling mode; the tables are zero where unused, as the kernels' parameters.
 struct LightOptions {
     LightsDev lights{};   // the light table (light sampling mode)
@@ -32,7 +33,8 @@ struct LightOptions {
     TexDev tex{};         // the textures and the shadow slots' base colours (tex_on)
     MapsDev maps{};       // the maps' table and the shadow slots' metallic (maps_on)
     PunctDev punct{};     // the punctual lights' table and P_p (punct_on)
-    bool env_on = false, trans_on = false, medium_on = false, tex_on = false, maps_on = false, punct_on = false;
+    EmitDev emit{};       // the emission maps' records and the shadow slots' E(Q) (emap_on)
+    bool env_on = false, trans_on = false, medium_on = false, tex_on = false, maps_on = false, punct_on = false, emap_on = false;
 };
 
 // lens (EZRT_PARAM_THIN_LENS): the thin-lens camera rays (k_generate<true>); null: the pinhole's
@@ -115,6 +117,15 @@ void launch_sample_textures(const SceneDev& sc, const TexDev& tex, int n, const 
 void launch_sample_materials(const SceneDev& sc, const TexDev& tex, const MapsDev& maps, int n, const int32_t* tri, const float* odt, float* out, cudaStream_t st);
 // the maps' words (n, reference order) into the fourth word of rec[2 i + 1] and, with acc_tri_ref, of acc_rec[2 a + 1]
 void launch_maps_set(const uint32_t* words, const uint32_t* acc_tri_ref, int n, float4* rec, float4* acc_rec, cudaStream_t st);
+// the emission maps' per-triangle records (ids: n emission ids, reference order; rec, acc_rec: n float2 each, acc_rec with
+// acc_tri_ref only) and every triangle's emission-table weight w (n floats), 64 filtered lookups per mapped emitter
+void launch_emit_weights(const SceneDev& sc, const TexDev& tex, const int32_t* ids, const uint32_t* acc_tri_ref, float2* rec, float2* acc_rec,
+                         float* w, cudaStream_t st);
+// the light records of an emission table (launch_light_records' rec, lights idx) take lum_eff from rec in their fourth word
+void launch_emit_records(const float2* emit_rec, const int32_t* idx, int n, float4* rec, cudaStream_t st);
+// ezrt_scene_sample_emission: n (reference triangle, point) pairs -> E(Q) (3 floats each); emit.rec null: no maps
+void launch_sample_emission(const SceneDev& sc, const TexDev& tex, const EmitDev& emit, int n, const int32_t* tri, const float* points, float* rgb,
+                            cudaStream_t st);
 void launch_eval_math(int which, int n, const float* a, const float* b, float* out, cudaStream_t st);
 void launch_tonemap(const float* in, int channels, float* out, long long n, float limit, cudaStream_t st);
 void launch_partition_scatter(const float* compact, float* full, const TileDev* tiles, int n_tiles, int width, int channels,

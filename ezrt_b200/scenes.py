@@ -316,14 +316,17 @@ def obj_with_vt(text, projection):
     return "\n".join(out) + "\n"
 
 
-def _textured_list(meshes, n_textures):
-    """meshes of p3_bunny_meshes / grid_meshes read as textured OBJ text: emissive meshes untextured, flat boxes planar with the last
-    texture id, the other meshes spherical with ids cycling over the others"""
+def _textured_list(meshes, n_textures, emissive_uv=False):
+    """meshes of p3_bunny_meshes / grid_meshes read as textured OBJ text: emissive meshes untextured (emissive_uv: with spherical UVs
+    for their emission maps), flat boxes planar with the last texture id, the other meshes spherical with ids cycling over the others"""
     tl = TriangleList()
     k = 0
     for text, m, trans, smooth in meshes:
         if any(c > 0 for c in m.emissive):
-            tl.read_obj_text(text, m, trans, smooth)
+            if emissive_uv:
+                tl.read_obj_text(obj_with_vt(text, "spherical"), m, trans, smooth, texture_id=-1)
+            else:
+                tl.read_obj_text(text, m, trans, smooth)
         elif text == box_obj():
             tl.read_obj_text(obj_with_vt(text, "planar"), m, trans, smooth, texture_id=n_textures - 1)
         else:
@@ -432,3 +435,85 @@ def punctual_rig(tris, seed=0, n_points=3, power=1.0):
         col = rng.uniform(0.3, 1.0, 3)
         lights.append(api.point_light(pos, color=tuple(col), intensity=float(rng.uniform(0.5, 1.5) * r * r * power)))
     return lights
+
+
+def emission_bands(seed=31, size=(64, 128)):
+    """a high-contrast emission texture for EZRT_PARAM_EMISSION_MAPS (uint8 [H, W, 3], sRGB): seeded bright coloured bands across u on
+    black, wide enough gaps that some triangles of a mapped sphere are black at all 64 points of their table weight"""
+    h, w = size
+    rng = np.random.default_rng(seed)
+    img = np.zeros((h, w, 3), np.uint8)
+    x = int(rng.integers(0, 8))
+    while x < w:
+        on, off = int(rng.integers(3, 10)), int(rng.integers(10, 26))
+        img[:, x:x + on] = rng.integers(150, 256, 3)
+        x += on + off
+    return img
+
+
+def _emission_mapped(textured_list, n_textures, builder):
+    tris, nodes = textured_list.build_bvh(8, builder)
+    uv, ids = textured_list.encode_texcoords()
+    emissive = np.asarray(tris, np.float32).reshape(-1, 36)[:, 18:21]
+    eid = np.where((emissive > 0).any(axis=1), n_textures, -1).astype(np.int32)
+    return tris, nodes, uv, ids, eid
+
+
+def s_p3_bunny_emission_mapped(n_textures=2, builder=api.BVH_SAH_FAST):
+    """s_p3_bunny_textured with the emissive sphere read with spherical UVs and mapped by emission_bands (EZRT_PARAM_EMISSION_MAPS).
+    Returns (tris, nodes, eye, cam, textures, texcoords, texture_id, emission_id); the geometry is s_p3_bunny's byte for byte, and the
+    emission texture is the last one."""
+    tris, nodes, uv, ids, eid = _emission_mapped(_textured_list(p3_bunny_meshes(), n_textures, emissive_uv=True), n_textures, builder)
+    eye, cam = api.camera_orbit(0.0, 0.0, 4.0)
+    return tris, nodes, eye, cam, procedural_textures(n_textures) + [emission_bands()], uv, ids, eid
+
+
+def s_1m_bunny_emission_mapped(n_textures=2, builder=api.BVH_SAH_FAST):
+    """s_1m_bunny_textured with its four emissive spheres mapped as s_p3_bunny_emission_mapped's; the geometry is s_1m_bunny's"""
+    tl = _textured_list(grid_meshes(15, 14, 4, 1.2, "bunny", 201), n_textures, emissive_uv=True)
+    tris, nodes, uv, ids, eid = _emission_mapped(tl, n_textures, builder)
+    eye, cam = api.camera_orbit(30.0, 25.0, 0.62 * max(15 * 1.2, 14 * 1.2) + 3.0)
+    return tris, nodes, eye, cam, procedural_textures(n_textures) + [emission_bands()], uv, ids, eid
+
+
+def screen_image(seed=41, size=(72, 128)):
+    """an image-like emission texture (uint8 [H, W, 3], sRGB): a seeded colour gradient with dark window bars and a few bright discs"""
+    h, w = size
+    rng = np.random.default_rng(seed)
+    ys, xs = np.meshgrid(np.arange(h) / h, np.arange(w) / w, indexing="ij")
+    c0, c1 = rng.uniform(0.2, 1.0, 3), rng.uniform(0.2, 1.0, 3)
+    img = c0 * (1 - xs[..., None]) + c1 * xs[..., None]
+    img *= (1.0 - 0.8 * ((ys * 6) % 1.0 < 0.15))[..., None]
+    for _ in range(4):
+        cy, cx, r = rng.uniform(0, 1), rng.uniform(0, 1), rng.uniform(0.05, 0.15)
+        img[(ys - cy) ** 2 + ((xs - cx) * w / h) ** 2 < r * r] = rng.uniform(0.7, 1.0, 3)
+    return np.clip(np.rint(img * 255.0), 0, 255).astype(np.uint8)
+
+
+def screen_obj(width=3.0, height=1.8):
+    """a quad in the z = 0 plane facing +z, centred at the origin, with UVs 0..1 (v = 0 at its bottom), as OBJ text"""
+    x, y = width / 2.0, height / 2.0
+    return ("v %r %r 0\nv %r %r 0\nv %r %r 0\nv %r %r 0\nvt 0 0\nvt 1 0\nvt 1 1\nvt 0 1\nf 1/1 2/2 3/3\nf 1/1 3/3 4/4\n"
+            % (-x, -y, x, -y, x, y, -x, y))
+
+
+def s_screen(bunny=True, builder=api.BVH_SAH_FAST, emission=(6.0, 6.0, 6.0)):
+    """a "screen": a 3 x 1.8 quad emitter standing at the back edge of a floor, facing +z, mapped with screen_image, and the bunny
+    (bunny=True) on the floor in front of it, lit by it and shadowing the floor in front.  readObj normalises every mesh to its unit
+    box, so the meshes' sizes are set by their transforms' scales.
+    Returns (tris, nodes, eye, cam, textures [screen_image()], texcoords, texture_id (all -1), emission_id (the quad 0, others -1))."""
+    tl = TriangleList()
+    top = -1.395   # the floor's top face
+    # the floor ends at the screen's plane, so that no surface sees the screen's back
+    floor = (box_obj(), Material(baseColor=(0.725, 0.71, 0.68)), transform_matrix((0, 0, 0), (0, -1.4, 1.8), (8.0, 0.01, 6.0)), False)
+    meshes = [floor]
+    if bunny:
+        text, m, _, smooth = p3_bunny_meshes()[0]
+        meshes.append((text, m, transform_matrix((0, 0, 0), (0.3, top - 1.5 * _unit_ymin(text), -0.2), (1.5, 1.5, 1.5)), smooth))
+    for text, m, trans, smooth in meshes:
+        tl.read_obj_text(obj_with_vt(text, "planar"), m, trans, smooth, texture_id=-1)
+    tl.read_obj_text(screen_obj(), Material(baseColor=(0, 0, 0), emissive=tuple(emission)),
+                     transform_matrix((0, 0, 0), (0.0, top + 0.95, -1.2), (3.0, 3.0, 3.0)), False, texture_id=-1)
+    tris, nodes, uv, ids, eid = _emission_mapped(tl, 0, builder)
+    eye, cam = api.camera_orbit(0.0, 15.0, 4.0)
+    return tris, nodes, eye, cam, [screen_image()], uv, ids, eid

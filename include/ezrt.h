@@ -184,6 +184,16 @@ typedef struct ezrt_render_params {
    megakernel, or without lights set.  Accepted by ezrt_render[_device], ezrt_render_adaptive[_device] and ezrt_render_aov[_device];
    the shadow slots keep their sizes. */
 #define EZRT_PARAM_PUNCTUAL_LIGHTS 128
+/* ezrt_render_params.reserved[0], with EZRT_PARAM_TEXTURES (so in EZRT_MODE_DISNEY_LIGHTS on the wavefront pipeline) and emission maps
+   set (ezrt_scene_set_emission_maps; glTF's emissiveTexture): a triangle T with emission E_T, lum(E_T) > 0 and emission id m >= 0
+   emits E(Q) = E_T * the filtered sRGB colour of texture m at the UV of Q (ezrt_math.h, DESIGN.md section 18) -- at the camera ray's
+   hit, at BSDF-sample emission hits and in the triangle light samples.  The render's light table is the emission table, in which
+   a mapped emitter weighs area * lum_eff, the mean luminance of E over 64 fixed points of T; a light sample's pdf and the MIS weight
+   of a hit on a mapped light use lum_eff.  A light sample whose E(Q) is black traces no shadow ray.  No draw is added.  Combines
+   with every other flag of the mode and every traversal policy.  Invalid (EZRT_ERR_INVALID) without EZRT_PARAM_TEXTURES or without
+   emission maps set.  Accepted by ezrt_render[_device], ezrt_render_adaptive[_device] and ezrt_render_aov[_device]; each shadow
+   slot takes 16 more bytes. */
+#define EZRT_PARAM_EMISSION_MAPS 256
 
 /* One punctual light of ezrt_scene_set_punctual_lights (glTF's KHR_lights_punctual, in the render's units: no photometric
    conversion; the caller scales glTF's candela and lux) */
@@ -292,6 +302,21 @@ int ezrt_scene_set_punctual_lights(ezrt_scene* scene, int n, const ezrt_punctual
  * status; writes min(J, cap) entries: index_out = each light's index among the caller's lights, cdf_out = the cdf (the last entry 1),
  * q_out = the selection probabilities (float)(w_j / W), and *total_out = W, the float64 sum of the weights.  Any output may be NULL. */
 int ezrt_scene_punctual_lights(ezrt_scene* scene, int cap, int32_t* index_out, float* cdf_out, float* q_out, double* total_out);
+/* Sets the scene's emission maps (EZRT_PARAM_EMISSION_MAPS): emission_id = one id per triangle (tris order) into the textures of
+ * ezrt_scene_set_textures, -1 for none; NULL clears them, and so does ezrt_scene_set_textures (including a clear), as the ids refer
+ * to its list.  Builds the emission table on the device (64 filtered lookups per mapped emitter, then the weights summed in float64 on
+ * the host).  Returns EZRT_ERR_INVALID, and keeps the previous maps, without textures set or for an id outside -1 to the texture count
+ * - 1; keeps them too on every other error.  Waits for every render already enqueued on the scene's device. */
+int ezrt_scene_set_emission_maps(ezrt_scene* scene, const int32_t* emission_id);
+/* The emission table of ezrt_scene_set_emission_maps, as ezrt_scene_lights returns mode 4's: returns K, the number of lights, or a
+ * negative status (EZRT_ERR_INVALID without emission maps); writes min(K, cap) entries of tri_out (the lights' triangles), cdf_out (the
+ * last entry 1) and lum_out (each light's lum_eff, the records' fourth word), and *total_out = W, the float64 sum of the weights.  Any
+ * output may be NULL. */
+int ezrt_scene_emission_lights(ezrt_scene* scene, int cap, int32_t* tri_out, float* cdf_out, float* lum_out, double* total_out);
+/* What the emission-map renders read as the emission at n points (points: 3 floats each) of reference triangles tri: rgb_out (3 floats
+ * each) = E(Q) with the scene's emission maps (none set: each triangle's material emission).  Host arrays; synchronous.
+ * EZRT_ERR_INVALID without textures set or for a triangle index out of range. */
+int ezrt_scene_sample_emission(ezrt_scene* scene, int n, const int32_t* tri, const float* points, float* rgb_out);
 
 /* render(width,height,spp) -> framebuffer: equals `spp` consecutive display() calls
  * (P5/main.cpp:697-748) each drawing pass1 (P5/fsh:894-949) and copying to lastFrame.

@@ -892,6 +892,48 @@ EZ_HD ez_vec3 ez_normal_map(ez_vec3 p1, ez_vec3 p2, ez_vec3 p3, const float* uv6
 EZ_HD int ez_maps_mr_id(uint32_t w) { return (int)(w & 0xffffu) - 1; }
 EZ_HD int ez_maps_normal_id(uint32_t w) { return (int)(w >> 16) - 1; }
 
+/* ------------------------------------------------------------------ emission maps (EZRT_PARAM_EMISSION_MAPS, DESIGN.md section 18)
+ * One more per-triangle texture id m (glTF's emissiveTexture, sRGB: decoded by ez_srgb_table) into the textures of EZRT_PARAM_TEXTURES.
+ * Emission at a point Q of triangle T with emission E_T (ez_emit_eval):
+ *   E(Q) = E_T * ez_tex_sample(texture m, uv(Q), ez_srgb_table) per channel when m >= 0 and lum(E_T) > 0; E_T otherwise.
+ *   uv(Q) is section 15's: ez_tri_bary with T's geometric normal, then ez_tex_uv.  Read wherever mode 4 reads emission: the camera
+ *   ray's Le, BSDF-sample emission hits and the triangle light samples.  No random number is drawn.
+ * Table: a triangle with lum(E_T) > 0 and m >= 0 weighs area * lum_eff with lum_eff = ez_emit_lum_eff, the mean of
+ *   lum(E_T * t(uv_j)) over the 64 centroids of T's 8-fold subdivision (barycentrics (a / 24, b / 24, rest), ez_emit_lum_eff's
+ *   order), reduced by pairwise midpoints mid(x, y) = x + (y - x) * 0.5 in a fixed tree (terms 2i and 2i + 1, then their midpoints
+ *   likewise): 64 equal finite terms give that term exactly, subnormal or near FLT_MAX (scaling by 1/64 first rounds subnormals;
+ *   dividing the sum at the end overflows above FLT_MAX / 64).  Every other triangle weighs ez_light_weight.  Membership (ez_is_light),
+ *   W, the cdf and the 64-byte records are section 10's; the record's fourth word is lum_eff in place of lum(E).
+ * Light sample: Q as section 10; E(Q) with the light's geometric normal; none if E(Q) is 0 in every channel; pdf_l =
+ *   ez_light_pdf(lum_eff, W_f, dist, cos_l) with the factors of section 11 and 17.  Emission hit on a mapped triangle (lum(E_T) > 0,
+ *   m >= 0): a light iff ez_is_light(area * lum_eff), and its MIS pdf uses lum_eff; unmapped triangles are section 10's. */
+EZ_HD ez_vec3 ez_emit_eval(ez_vec3 E, ez_vec3 Q, ez_vec3 p1, ez_vec3 p2, ez_vec3 p3, ez_vec3 Ng, const float* uv6, const uint32_t* texels, int W,
+                           int H, const float* lut) {
+    float w1, w2, w3, u, v;
+    ez_tri_bary(Q, p1, p2, p3, Ng, &w1, &w2, &w3);
+    ez_tex_uv(w1, w2, w3, uv6, &u, &v);
+    return ez_mul(E, ez_tex_sample(texels, W, H, u, v, lut));
+}
+EZ_HD float ez_emit_mid(float x, float y) { return x + (y - x) * 0.5f; }
+/* lum_eff of a triangle with emission E, UVs uv6 and emission texture (texels, W, H): rows i = 0..7 of the subdivision, in each the
+ * upward cells j = 0..7-i (a, b) = (3i + 1, 3j + 1), then the downward cells j = 0..6-i (3i + 2, 3j + 2) */
+EZ_HD float ez_emit_lum_eff(ez_vec3 E, const float* uv6, const uint32_t* texels, int W, int H, const float* lut) {
+    float t[64];
+    int k = 0;
+    for (int i = 0; i < 8; i++)
+        for (int down = 0; down < 2; down++)
+            for (int j = 0; j < 8 - i - down; j++) {
+                const float w1 = EZ_DIV((float)(3 * i + 1 + down), 24.0f), w2 = EZ_DIV((float)(3 * j + 1 + down), 24.0f);
+                const float w3 = (1.0f - w1) - w2;
+                float u, v;
+                ez_tex_uv(w1, w2, w3, uv6, &u, &v);
+                t[k++] = ez_luminance(ez_mul(E, ez_tex_sample(texels, W, H, u, v, lut)));
+            }
+    for (int n = 32; n >= 1; n >>= 1)
+        for (int j = 0; j < n; j++) t[j] = ez_emit_mid(t[2 * j], t[2 * j + 1]);
+    return t[0];
+}
+
 /* ------------------------------------------------------------------ punctual lights (EZRT_PARAM_PUNCTUAL_LIGHTS, DESIGN.md section 17)
  * The table (ezrt_punctual.h, float64 on the host): light j's record is 16 floats,
  *   [0..2] position, [3] type (0 point, 1 spot, 2 directional, as a float), [4..6] unit direction (float64-normalised), [7] cos_o,
