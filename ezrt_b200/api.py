@@ -28,6 +28,7 @@ PARAM_TEXTURES = 32
 PARAM_MATERIAL_MAPS = 64
 PARAM_PUNCTUAL_LIGHTS = 128
 PARAM_EMISSION_MAPS = 256
+PARAM_LIGHT_TREE = 512
 PUNCTUAL_POINT, PUNCTUAL_SPOT, PUNCTUAL_DIRECTIONAL = 0, 1, 2   # ezrt_punctual_light.type
 MODES = {"diffuse_p3": 0, "disney_aniso_p4": 1, "disney_sobol_p5": 2, "disney_is_mis_p5": 3, "disney_lights": 4}
 
@@ -257,6 +258,7 @@ class RenderConfig:
     material_maps: bool = False  # EZRT_PARAM_MATERIAL_MAPS (with textures): the scene's material maps (Scene.set_material_maps, DESIGN.md section 16)
     punctual_lights: bool = False  # EZRT_PARAM_PUNCTUAL_LIGHTS (MODE_DISNEY_LIGHTS only): the scene's punctual lights (Scene.set_punctual_lights, DESIGN.md section 17)
     emission_maps: bool = False  # EZRT_PARAM_EMISSION_MAPS (with textures): the scene's emission maps (Scene.set_emission_maps, DESIGN.md section 18)
+    light_tree: bool = False    # EZRT_PARAM_LIGHT_TREE (MODE_DISNEY_LIGHTS only): triangle lights chosen by a light tree (Scene.light_tree, DESIGN.md section 19)
 
     def to_struct(self):
         p = RenderParams()
@@ -271,7 +273,8 @@ class RenderConfig:
         p.reserved[0] = ((PARAM_ACCUMULATE if self.accumulate else 0) | (PARAM_ENV_LIGHT if self.env_light else 0) |
                          (PARAM_TRANSMISSION if self.transmission else 0) | (PARAM_MEDIUM if self.medium else 0) |
                          (PARAM_TEXTURES if self.textures else 0) | (PARAM_MATERIAL_MAPS if self.material_maps else 0) |
-                         (PARAM_PUNCTUAL_LIGHTS if self.punctual_lights else 0) | (PARAM_EMISSION_MAPS if self.emission_maps else 0))
+                         (PARAM_PUNCTUAL_LIGHTS if self.punctual_lights else 0) | (PARAM_EMISSION_MAPS if self.emission_maps else 0) |
+                         (PARAM_LIGHT_TREE if self.light_tree else 0))
         if self.lens_radius != 0:   # a negative or NaN radius is set too, so that the library rejects it
             if self.focus_distance is None:
                 raise ValueError("RenderConfig: a lens (lens_radius != 0) needs a focus_distance")
@@ -333,6 +336,29 @@ def denoise_params(iterations=5, sigma_l=4.0, sigma_n=128.0, sigma_z=1.0, sigma_
     d.iterations, d.sigma_l, d.sigma_n, d.sigma_z, d.sigma_a, d.reserved = int(iterations), float(sigma_l), float(sigma_n), float(sigma_z), \
         float(sigma_a), 0
     return d
+
+
+def light_tree_arrays(nodes, paths):
+    """The dict of Scene.light_tree from the raw node records [M, 12] float32 and path records [K, 4] uint32"""
+    nodes = np.asarray(nodes, np.float32).reshape(-1, 12)
+    paths = np.asarray(paths, np.uint32).reshape(-1, 4)
+    return {"lo": nodes[:, 0:3].copy(), "phi": nodes[:, 3].copy(), "hi": nodes[:, 4:7].copy(), "cos_o": nodes[:, 7].copy(),
+            "axis": nodes[:, 8:11].copy(), "child": nodes[:, 11].copy().view(np.int32),
+            "path": paths[:, 0].astype(np.uint64) | (paths[:, 1].astype(np.uint64) << np.uint64(32)), "depth": paths[:, 2].astype(np.int32),
+            "area": paths[:, 3].copy().view(np.float32), "nodes": nodes.copy(), "paths": paths.copy()}
+
+
+def build_light_tree(verts, weights):
+    """ezrt_light_tree_build on the host (no device needed): verts [K, 3, 3] (each light's vertices), weights [K] (table weights) -> the
+    dict of Scene.light_tree"""
+    v = np.ascontiguousarray(np.asarray(verts, np.float32).reshape(-1, 9))
+    w = np.ascontiguousarray(np.asarray(weights, np.float32).reshape(-1))
+    assert v.shape[0] == w.shape[0]
+    m = check(lib.ezrt_light_tree_build(w.shape[0], _fp(v), _fp(w), 0, None, None))
+    nodes = np.zeros((m, 12), np.float32)
+    paths = np.zeros((w.shape[0], 4), np.uint32)
+    check(lib.ezrt_light_tree_build(w.shape[0], _fp(v), _fp(w), m, _fp(nodes), paths.ctypes.data_as(_lib.c_uint32_p)))
+    return light_tree_arrays(nodes, paths)
 
 
 class Scene:
@@ -454,6 +480,37 @@ class Scene:
         rgb = np.zeros((tri.shape[0], 3), np.float32)
         check(lib.ezrt_scene_sample_emission(self._h, tri.shape[0], tri.ctypes.data_as(C.POINTER(C.c_int32)), _fp(pts), _fp(rgb)))
         return rgb
+
+    def light_tree(self, emission=False):
+        """The light tree RenderConfig.light_tree renders with (ezrt_scene_light_tree; DESIGN.md section 19) over mode 4's table, or the
+        emission table with emission=True: a dict of numpy arrays, per node lo, hi [M, 3], phi, cos_o [M], axis [M, 3], child [M] (>= 0 the
+        left child, the right one follows; < 0 the leaf of light ~child), and per light (table order) path (uint64), depth and area [K]."""
+        m = check(lib.ezrt_scene_light_tree(self._h, int(bool(emission)), 0, None, None))
+        nodes = np.zeros((m, 12), np.float32)
+        k = (m + 1) // 2
+        paths = np.zeros((k, 4), np.uint32)
+        check(lib.ezrt_scene_light_tree(self._h, int(bool(emission)), m, _fp(nodes), paths.ctypes.data_as(_lib.c_uint32_p)))
+        return light_tree_arrays(nodes, paths)
+
+    def sample_light_tree(self, P, r, emission=False):
+        """The device's descent (ezrt_scene_light_tree_eval, which 0): points P [n, 3] and selection numbers r [n] -> (light index in
+        table order int32 [n], -1 for no sample; P_sel float32 [n])."""
+        P = np.ascontiguousarray(np.asarray(P, np.float32).reshape(-1, 3))
+        r = np.ascontiguousarray(np.asarray(r, np.float32).reshape(-1))
+        assert r.shape[0] == P.shape[0]
+        k = np.zeros(P.shape[0], np.int32)
+        p = np.zeros(P.shape[0], np.float32)
+        check(lib.ezrt_scene_light_tree_eval(self._h, int(bool(emission)), 0, P.shape[0], _fp(P), _fp(r), None, k.ctypes.data_as(_lib.c_int32_p), _fp(p)))
+        return k, p
+
+    def light_tree_prob(self, P, light, emission=False):
+        """The device's hit-side walk (ezrt_scene_light_tree_eval, which 1): P_sel float32 [n] of lights light [n] at points P [n, 3]."""
+        P = np.ascontiguousarray(np.asarray(P, np.float32).reshape(-1, 3))
+        light = np.ascontiguousarray(np.asarray(light, np.int32).reshape(-1))
+        assert light.shape[0] == P.shape[0]
+        p = np.zeros(P.shape[0], np.float32)
+        check(lib.ezrt_scene_light_tree_eval(self._h, int(bool(emission)), 1, P.shape[0], _fp(P), None, light.ctypes.data_as(_lib.c_int32_p), None, _fp(p)))
+        return p
 
     def set_punctual_lights(self, lights):
         """ezrt_scene_set_punctual_lights: the punctual lights RenderConfig.punctual_lights renders (DESIGN.md section 17), a sequence of

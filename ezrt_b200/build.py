@@ -99,18 +99,22 @@ def build_product(force=False, verbose=False, variant=None, defines=()):
 
 def _build_product_locked(nvcc, target, cu, cpp, objdir, defines, verbose):
     dflags = ["-D" + d for d in defines]
-    objs = []
+    jobs = []   # (command, object, ptxas log); compiled concurrently: the translation units are independent
     for src in cu:
         obj = os.path.join(objdir, os.path.basename(src) + ".o")
-        out = _run([nvcc] + NVCC_FLAGS + dflags + ["-I", INCLUDE, "-I", CSRC, "-c", src, "-o", obj],
-                   log=os.path.join(objdir, os.path.basename(src) + ".ptxas.log"))
-        if verbose:
-            print(out)
-        objs.append(obj)
+        jobs.append(([nvcc] + NVCC_FLAGS + dflags + ["-I", INCLUDE, "-I", CSRC, "-c", src, "-o", obj], obj,
+                     os.path.join(objdir, os.path.basename(src) + ".ptxas.log")))
     for src in cpp:
         obj = os.path.join(objdir, os.path.basename(src) + ".o")
-        _run(["g++"] + HOST_FLAGS + dflags + ["-pthread", "-I", INCLUDE, "-I", CSRC, "-c", src, "-o", obj])
-        objs.append(obj)
+        jobs.append((["g++"] + HOST_FLAGS + dflags + ["-pthread", "-I", INCLUDE, "-I", CSRC, "-c", src, "-o", obj], obj, None))
+    from concurrent.futures import ThreadPoolExecutor
+    with ThreadPoolExecutor(max_workers=max(1, min(len(jobs), os.cpu_count() or 1))) as pool:
+        outs = list(pool.map(lambda j: _run(j[0], log=j[2]), jobs))
+    if verbose:
+        for (cmd, _, log), out in zip(jobs, outs):
+            if log:
+                print(out)
+    objs = [obj for _, obj, _ in jobs]
     tmp = target + ".tmp%d" % os.getpid()
     _run([nvcc, "-shared", "-o", tmp] + objs + ["-Xcompiler", "-pthread", "-cudart", "static"])
     os.replace(tmp, target)  # atomic: a concurrent import never sees a half-written library
@@ -324,6 +328,26 @@ def build_oracle_emission_maps(force=False):
     return ORACLE_EMISSION_MAPS_SO
 
 
+ORACLE_LIGHT_TREE_SO = os.path.join(ROOT, "build", "libezrt_oracle_light_tree.so")
+
+
+def build_oracle_light_tree(force=False):
+    """build/libezrt_oracle_light_tree.so: tests/oracle_light_tree.cpp, the CPU restatement of the light tree (the descent, the
+    hit-side walk, the flagged render's medium and transmission loops) over the emission maps' restatement (test infrastructure,
+    loaded only by tests/oracle_light_tree.py)."""
+    src = os.path.join(ROOT, "tests", "oracle_light_tree.cpp")
+    deps = [src] + [os.path.join(ROOT, "tests", f) for f in ("oracle_emission_maps.cpp", "oracle_punctual.cpp", "oracle_material_maps.cpp",
+                                                              "oracle_textures.cpp", "oracle_medium.cpp", "oracle_lens.cpp", "oracle_transmission.cpp",
+                                                              "oracle_env_light.cpp", "oracle_lights.cpp")] + \
+        [os.path.join(ROOT, "oracle", "ezrt_oracle.cpp")] + [os.path.join(INCLUDE, f) for f in os.listdir(INCLUDE)]
+    if force or _newer(ORACLE_LIGHT_TREE_SO, deps):
+        os.makedirs(os.path.dirname(ORACLE_LIGHT_TREE_SO), exist_ok=True)
+        tmp = ORACLE_LIGHT_TREE_SO + ".tmp%d" % os.getpid()
+        _run(["g++"] + HOST_FLAGS + ["-fopenmp", "-Wno-misleading-indentation", "-shared", "-I", INCLUDE, src, "-o", tmp])
+        os.replace(tmp, ORACLE_LIGHT_TREE_SO)
+    return ORACLE_LIGHT_TREE_SO
+
+
 def build_reference_hdrloader(force=False):
     return _oracle_recipes().build_reference_hdrloader(force)
 
@@ -393,6 +417,7 @@ def build_all(force=False, verbose=False):
     build_oracle_material_maps(force=force)
     build_oracle_punctual(force=force)
     build_oracle_emission_maps(force=force)
+    build_oracle_light_tree(force=force)
     build_example(force=force)
     build_reference_hdrloader(force=force)
     build_reference_shaders(force=force)

@@ -99,6 +99,7 @@ struct ezrt_scene {
     LightsDev lights{};
     std::vector<int32_t> light_tri;   // the lights' triangles (caller's order)
     std::vector<float> light_cdf;
+    std::vector<float> light_w;       // the lights' weights
     double light_total = 0.0;         // W, the float64 sum of the weights
     // the environment map's light table (build_env, at the first render with EZRT_PARAM_ENV_LIGHT): row cdf | column cdf | texel pdf
     DeviceBuffer env_buf;
@@ -131,8 +132,17 @@ struct ezrt_scene {
     EmitDev emit{};
     LightsDev emit_lights{};
     std::vector<int32_t> emit_tri;
-    std::vector<float> emit_cdf, emit_lum;
+    std::vector<float> emit_cdf, emit_lum, emit_w;
     double emit_total = 0.0;
+    // the light trees of EZRT_PARAM_LIGHT_TREE (build_light_tree, at their first use) over mode 4's table [0] and the emission table [1]:
+    // nodes | paths | light ids (reference order) | light ids (accel order), and the host copies of the builder's output
+    struct LightTree {
+        bool built = false;
+        DeviceBuffer buf;
+        LightTreeDev dev{};
+        std::vector<float> nodes;
+        std::vector<uint32_t> paths;
+    } ltree[2];
     void* hot_base = nullptr;   // accel nodes | geometry (| vertices) | shading records (L2 persisting window)
     size_t hot_bytes = 0;
     size_t l2_persist_bytes = 0;
@@ -257,6 +267,8 @@ int validate_params(const ezrt_scene* scene, const ezrt_render_params* p) {
         if (!scene->has_punct)
             return ezrt_set_error(EZRT_ERR_INVALID, "render: EZRT_PARAM_PUNCTUAL_LIGHTS needs punctual lights (ezrt_scene_set_punctual_lights)");
     }
+    if ((p->reserved[0] & EZRT_PARAM_LIGHT_TREE) && p->mode != EZRT_MODE_DISNEY_LIGHTS)
+        return ezrt_set_error(EZRT_ERR_INVALID, "render: EZRT_PARAM_LIGHT_TREE needs the light sampling mode (got mode %d)", p->mode);
     if (p->max_bounce < 0 || p->max_bounce > 64) return ezrt_set_error(EZRT_ERR_INVALID, "render: max_bounce out of range");
     if (p->out_channels != 3 && p->out_channels != 4) return ezrt_set_error(EZRT_ERR_INVALID, "render: out_channels must be 3 or 4");
     if (p->part_count < 1 || p->part_rank < 0 || p->part_rank >= p->part_count)
@@ -330,6 +342,7 @@ struct LightTable {
     LightsDev dev{};
     std::vector<int32_t> tri;   // the lights' triangles (caller's order)
     std::vector<float> cdf, lum;
+    std::vector<float> w;       // the lights' weights
     double total = 0.0;         // W, the float64 sum of the weights
 };
 int light_table(ezrt_scene* s, float* d_w, const float2* emit_rec, DeviceBuffer& buf, LightTable& out, cudaStream_t st) {
@@ -378,6 +391,7 @@ int light_table(ezrt_scene* s, float* d_w, const float2* emit_rec, DeviceBuffer&
     lt.w_total = (float)W;
     out.dev = lt;
     out.tri = idx;
+    out.w = w;
     out.cdf = cdf;
     out.lum = lum;
     out.total = W;
@@ -398,8 +412,49 @@ int build_lights(ezrt_scene* s, cudaStream_t st) {
     s->lights = t.dev;
     s->light_tri = t.tri;
     s->light_cdf = t.cdf;
+    s->light_w = t.w;
     s->light_total = t.total;
     s->lights_built = true;
+    return EZRT_OK;
+}
+
+// The light tree of EZRT_PARAM_LIGHT_TREE over mode 4's table (which = 0, built) or the emission table (which = 1), once per table: the
+// lights' vertices read back from their records (one synchronisation of st), ezrt_light_tree_build on the host, the nodes and paths
+// uploaded and every triangle's light index scattered on st.  A table without lights has no tree.
+int build_light_tree(ezrt_scene* s, int which, cudaStream_t st) {
+    ezrt_scene::LightTree& t = s->ltree[which];
+    if (t.built) return EZRT_OK;
+    const LightsDev& lt = which ? s->emit_lights : s->lights;
+    const std::vector<float>& w = which ? s->emit_w : s->light_w;
+    const int K = lt.n, n = s->dev.n_triangles;
+    if (K > 0) {
+        const int M = 2 * K - 1;
+        const size_t node_bytes = 3 * sizeof(float4) * (size_t)M, path_bytes = sizeof(uint4) * (size_t)K;
+        int rc = t.buf.ensure(node_bytes + path_bytes + 2 * sizeof(int32_t) * (size_t)n);
+        if (rc) return rc;
+        std::vector<float4> rec(4 * (size_t)K);
+        CU_CHECK(cudaMemcpyAsync(rec.data(), lt.rec, sizeof(float4) * rec.size(), cudaMemcpyDeviceToHost, st));
+        CU_CHECK(cudaStreamSynchronize(st));
+        std::vector<float> verts(9 * (size_t)K);
+        for (int k = 0; k < K; k++)
+            for (int v = 0; v < 3; v++) {
+                const float4 q = rec[4 * (size_t)k + v];
+                verts[9 * (size_t)k + 3 * v] = q.x; verts[9 * (size_t)k + 3 * v + 1] = q.y; verts[9 * (size_t)k + 3 * v + 2] = q.z;
+            }
+        t.nodes.assign(12 * (size_t)M, 0.0f);
+        t.paths.assign(4 * (size_t)K, 0u);
+        if ((rc = ezrt_light_tree_build(K, verts.data(), w.data(), M, t.nodes.data(), t.paths.data())) != M) return rc < 0 ? rc : EZRT_ERR_INVALID;
+        t.dev.nodes = (const float4*)t.buf.p;
+        t.dev.path = (const uint4*)((char*)t.buf.p + node_bytes);
+        t.dev.light = (const int32_t*)((char*)t.buf.p + node_bytes + path_bytes);
+        t.dev.acc_light = t.dev.light + n;
+        // t.nodes and t.paths stay with the scene, so the copies need no synchronisation
+        CU_CHECK(cudaMemcpyAsync((void*)t.dev.nodes, t.nodes.data(), node_bytes, cudaMemcpyHostToDevice, st));
+        CU_CHECK(cudaMemcpyAsync((void*)t.dev.path, t.paths.data(), path_bytes, cudaMemcpyHostToDevice, st));
+        launch_ltree_ids(lt.rec, K, n, (int32_t*)t.dev.light, (int32_t*)t.dev.acc_light, st);
+        CU_CHECK(cudaGetLastError());
+    }
+    t.built = true;
     return EZRT_OK;
 }
 
@@ -476,7 +531,10 @@ void clear_emission_maps(ezrt_scene* s) {
     s->emit_tri.clear();
     s->emit_cdf.clear();
     s->emit_lum.clear();
+    s->emit_w.clear();
     s->emit_total = 0.0;
+    s->ltree[1].buf.release();   // the emission table's tree goes with the table
+    s->ltree[1] = ezrt_scene::LightTree{};
 }
 
 RenderDev make_render_dev(const ezrt_scene* s, const ezrt_render_params* p) {
@@ -1149,6 +1207,7 @@ int ezrt_scene_set_emission_maps(ezrt_scene* s, const int32_t* emission_id) {
     s->emit_tri = t.tri;
     s->emit_cdf = t.cdf;
     s->emit_lum = t.lum;
+    s->emit_w = t.w;
     s->emit_total = t.total;
     s->has_emit = true;
     return EZRT_OK;
@@ -1357,6 +1416,7 @@ int ezrt_scene_destroy(ezrt_scene* s) {
     s->aov_rec_buf.release(); s->aov_maps_buf.release(); s->denoise_buf.release(); s->denoise_io_buf.release();
     s->lights_buf.release(); s->env_buf.release(); s->tex_buf.release(); s->tex_rec_buf.release(); s->punct_buf.release();
     s->emit_buf.release(); s->emit_lights_buf.release();
+    s->ltree[0].buf.release(); s->ltree[1].buf.release();
     if (s->own_stream) cudaStreamDestroy(s->own_stream);
     if (s->copy_stream) cudaStreamDestroy(s->copy_stream);
     if (s->side_stream) cudaStreamDestroy(s->side_stream);
@@ -1418,6 +1478,13 @@ static int light_options(ezrt_scene* s, const ezrt_render_params* p, cudaStream_
         o.punct = s->punct;
         o.punct.p_p = (o.lights.n > 0 || o.env_on) ? 0.5f : 1.0f;
         o.punct_on = true;
+    }
+    // EZRT_PARAM_LIGHT_TREE: the tree over the render's table; a table of K = 0 is mode 4 and runs its kernels
+    if ((p->reserved[0] & EZRT_PARAM_LIGHT_TREE) && o.lights.n > 0) {
+        const int which = o.emap_on ? 1 : 0;
+        if ((rc = build_light_tree(s, which, st))) return rc;
+        o.tree = s->ltree[which].dev;
+        o.tree_on = true;
     }
     return EZRT_OK;
 }
@@ -2112,6 +2179,66 @@ int ezrt_scene_lights(ezrt_scene* s, int cap, int32_t* tri_out, float* cdf_out, 
     if (cdf_out) std::copy(s->light_cdf.begin(), s->light_cdf.begin() + m, cdf_out);
     if (total_out) *total_out = s->light_total;
     return K;
+}
+
+// the table of ezrt_scene_light_tree(s, emission) and its tree, built on the scene's own stream and complete on return
+static int scene_light_tree(ezrt_scene* s, int emission, const char* what, int* which) {
+    if (!s) return ezrt_set_error(EZRT_ERR_INVALID, "%s: null scene", what);
+    if (emission && !s->has_emit) return ezrt_set_error(EZRT_ERR_INVALID, "%s: no emission maps (ezrt_scene_set_emission_maps)", what);
+    CU_CHECK(cudaSetDevice(s->device));
+    int rc = build_lights(s, s->own_stream);
+    if (rc) return rc;
+    *which = emission ? 1 : 0;
+    if ((rc = build_light_tree(s, *which, s->own_stream))) return rc;
+    CU_CHECK(cudaStreamSynchronize(s->own_stream));
+    return EZRT_OK;
+}
+
+int ezrt_scene_light_tree(ezrt_scene* s, int emission, int cap, float* nodes_out, uint32_t* paths_out) {
+    int which;
+    if (cap < 0) return ezrt_set_error(EZRT_ERR_INVALID, "scene_light_tree: bad argument");
+    int rc = scene_light_tree(s, emission, "scene_light_tree", &which);
+    if (rc) return rc;
+    const ezrt_scene::LightTree& t = s->ltree[which];
+    const int M = (int)(t.nodes.size() / 12);
+    if (nodes_out) std::copy(t.nodes.begin(), t.nodes.begin() + 12 * (size_t)std::min(M, cap), nodes_out);
+    if (paths_out && cap >= M) std::copy(t.paths.begin(), t.paths.end(), paths_out);
+    return M;
+}
+
+int ezrt_scene_light_tree_eval(ezrt_scene* s, int emission, int which, int n, const float* P, const float* r, const int32_t* light_in,
+                               int32_t* light_out, float* p_out) {
+    if (n < 0 || (which != 0 && which != 1) || (n > 0 && (!P || !p_out || (which == 0 && (!r || !light_out)) || (which == 1 && !light_in))))
+        return ezrt_set_error(EZRT_ERR_INVALID, "scene_light_tree_eval: bad argument");
+    int t;
+    int rc = scene_light_tree(s, emission, "scene_light_tree_eval", &t);
+    if (rc) return rc;
+    const int K = (emission ? s->emit_lights : s->lights).n;
+    if (K == 0) return ezrt_set_error(EZRT_ERR_INVALID, "scene_light_tree_eval: the table has no lights");
+    if (which == 1)
+        for (int i = 0; i < n; i++)
+            if (light_in[i] < 0 || light_in[i] >= K) return ezrt_set_error(EZRT_ERR_INVALID, "scene_light_tree_eval: light %d out of range", light_in[i]);
+    if (n == 0) return EZRT_OK;
+    DeviceBuffer buf;
+    rc = buf.ensure(sizeof(float) * 7 * (size_t)n + 256);   // P (3 n) | r | light_in | light_out | P_sel
+    if (rc) return rc;
+    float* d_P = (float*)buf.p;
+    float* d_r = d_P + 3 * (size_t)n;
+    int32_t* d_in = (int32_t*)(d_r + n);
+    int32_t* d_out = d_in + n;
+    float* d_p = (float*)(d_out + n);
+    cudaError_t e = cudaMemcpy(d_P, P, sizeof(float) * 3 * (size_t)n, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = (which == 0) ? cudaMemcpy(d_r, r, sizeof(float) * n, cudaMemcpyHostToDevice)
+                                           : cudaMemcpy(d_in, light_in, sizeof(int32_t) * n, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) {
+        launch_ltree_eval(s->ltree[t].dev, which, n, d_P, d_r, d_in, d_out, d_p, 0);
+        e = cudaGetLastError();
+    }
+    if (e == cudaSuccess && which == 0) e = cudaMemcpy(light_out, d_out, sizeof(int32_t) * n, cudaMemcpyDeviceToHost);
+    if (e == cudaSuccess) e = cudaMemcpy(p_out, d_p, sizeof(float) * n, cudaMemcpyDeviceToHost);
+    buf.release();
+    if (e != cudaSuccess) return ezrt_set_error(EZRT_ERR_CUDA, "scene_light_tree_eval: %s", cudaGetErrorString(e));
+    return EZRT_OK;
 }
 
 int ezrt_scene_env_light(ezrt_scene* s, float* row_cdf, float* col_cdf, float* texel_pdf, double* total) {

@@ -2043,6 +2043,56 @@ __device__ __forceinline__ vec3 emit_light(const SceneDev& sc, const TexDev& tex
 // a light sample whose E(Q) is 0 in every channel is no sample
 __device__ __forceinline__ bool emit_black(vec3 E) { return E.x == 0.0f && E.y == 0.0f && E.z == 0.0f; }
 
+// EZRT_PARAM_LIGHT_TREE (ezrt_math.h, DESIGN.md section 19): node i of the tree, three 128-bit loads
+__device__ __forceinline__ ez_ltree_node ltree_node(const LightTreeDev& t, int i) {
+    const float4 a = ldg4(t.nodes + 3 * (size_t)i), b = ldg4(t.nodes + 3 * (size_t)i + 1), c = ldg4(t.nodes + 3 * (size_t)i + 2);
+    ez_ltree_node n;
+    n.lo = f4xyz(a); n.phi = a.w;
+    n.hi = f4xyz(b); n.cos_o = b.w;
+    n.axis = f4xyz(c); n.child = __float_as_int(c.w);
+    return n;
+}
+// ... the descent from P with r (ez_ltree_descend): the light's index in the table, with p_sel = its P_sel; -1 for no sample
+__device__ __forceinline__ int ltree_descend(const LightTreeDev& t, vec3 P, float r, float& p_sel) {
+    float q = 1.0f;
+    r = ez_min(r, 0.99999994f);
+    int c = __float_as_int(ldg4(t.nodes + 2).w);
+    while (c >= 0) {
+        const ez_ltree_node L = ltree_node(t, c), R = ltree_node(t, c + 1);
+        const int s = ez_ltree_step(ez_ltree_p_left(&L, &R, P), &r, &q);
+        if (s < 0) return -1;
+        c = s ? R.child : L.child;
+    }
+    p_sel = q;
+    return ~c;
+}
+// ... P_sel of light k at P along its stored path (ez_ltree_prob); *area = the light's area, the path record's fourth word
+__device__ __forceinline__ float ltree_prob(const LightTreeDev& t, vec3 P, int k, float* area) {
+    const uint4 pa = __ldg(t.path + k);
+    const uint64_t path = ((uint64_t)pa.y << 32) | pa.x;
+    *area = __uint_as_float(pa.w);
+    float q = 1.0f;
+    int c = __float_as_int(ldg4(t.nodes + 2).w);
+    for (int j = 0; j < (int)pa.z; j++) {
+        const ez_ltree_node L = ltree_node(t, c), R = ltree_node(t, c + 1);
+        const float pl = ez_ltree_p_left(&L, &R, P);
+        const bool right = (path >> j) & 1u;
+        q = q * (right ? 1.0f - pl : pl);
+        c = right ? R.child : L.child;
+    }
+    return q;
+}
+// ... the MIS pdf of a BSDF sample from P that hits triangle `tri` (the index space of accel_space) at distance t, seen at cos_l; false
+// when the triangle is no light of the table
+__device__ __forceinline__ bool ltree_hit_pdf(const LightTreeDev& t, int tri, bool accel_space, vec3 P, float dist, float cos_l, float& pdf) {
+    const int k = __ldg((accel_space ? t.acc_light : t.light) + tri);
+    if (k < 0) return false;
+    float area;
+    const float q = ltree_prob(t, P, k, &area);
+    pdf = ez_ltree_pdf(q, area, dist, cos_l);
+    return true;
+}
+
 // A medium vertex (EZRT_PARAM_MEDIUM; ezrt_math.h, DESIGN.md section 14): p's segment scattered at t_s before its hit (hit_t,
 // hit_tri) or its miss.  The weights of the segment (bounce >= 1) and the albedo enter the history; then, below max_bounce, one light
 // sample from P as at a surface but without the hemisphere test and the self exclusion (its shadow ray carries EZRT_MEDIUM_VERTEX
@@ -2050,12 +2100,13 @@ __device__ __forceinline__ bool emit_black(vec3 E) { return E.x == 0.0f && E.y =
 // TEX: the first-hit record's albedo is the textured base colour.  MAPS: ... and its normal the mapped one.
 // PUNCT: the light sample is punctual with probability punct.p_p (punct_pick, punct_sample).
 // EMAP: a triangle light sample's emission is E(Q) (emit_light), out through *sh_E; none where it is black.
-template <bool AOV, bool ENV, bool TEX = false, bool MAPS = false, bool PUNCT = false, bool EMAP = false>
+// LTREE: the triangle light is chosen by the light tree's descent from P (ltree_descend), its pdf ez_ltree_pdf.
+template <bool AOV, bool ENV, bool TEX = false, bool MAPS = false, bool PUNCT = false, bool EMAP = false, bool LTREE = false>
 __device__ __forceinline__ bool medium_step(const SceneDev& sc, const RenderDev& rd, int bounce, PathRegs& p, float t_s, float hit_t,
                                             int hit_tri, vec3& Lo, vec3& Le, bool& primary_miss, ShadowRay& sh, float4* aov_rec,
                                             const LightsDev& lights, const EnvDev& env, const MediumDev& med, const TexDev& tex = TexDev{},
                                             const MapsDev& maps = MapsDev{}, const PunctDev& punct = PunctDev{}, const EmitDev& emit = EmitDev{},
-                                            vec3* sh_E = nullptr) {
+                                            vec3* sh_E = nullptr, const LightTreeDev& tree = LightTreeDev{}) {
     if (bounce == 0) {
         Lo = splat3(0.0f);
         Le = splat3(0.0f);
@@ -2105,7 +2156,9 @@ __device__ __forceinline__ bool medium_step(const SceneDev& sc, const RenderDev&
         }
     }
     if (!punct_on && !env_pick && lights.n > 0) {
-        const float4* lr = lights.rec + 4 * (size_t)ez_light_select(lights.cdf, lights.n, r_tri);
+        float p_sel = 0.0f;   // LTREE: the light's P_sel; k < 0: no sample
+        const int k = LTREE ? ltree_descend(tree, P, r_tri, p_sel) : ez_light_select(lights.cdf, lights.n, r_tri);
+        const float4* lr = lights.rec + 4 * (size_t)(LTREE ? (k < 0 ? 0 : k) : k);
         const float4 a = ldg4(lr), b = ldg4(lr + 1), c = ldg4(lr + 2), e = ldg4(lr + 3);
         const vec3 D = ez_sub(ez_triangle_point(f4xyz(a), f4xyz(b), f4xyz(c), r_1, r_2), P);
         const float dist = EZ_SQRT(ez_dot(D, D));
@@ -2113,16 +2166,17 @@ __device__ __forceinline__ bool medium_step(const SceneDev& sc, const RenderDev&
         const float cos_l = ez_abs(ez_dot(f4xyz(e), Ll));
         bool emits = true;
         if constexpr (EMAP) {
-            if (cos_l != 0.0f && dist != 0.0f) {
+            if ((!LTREE || k >= 0) && cos_l != 0.0f && dist != 0.0f) {
                 *sh_E = emit_light(sc, tex, emit, a, b, c, e, r_1, r_2);
                 emits = !emit_black(*sh_E);
             }
         }
-        if (cos_l != 0.0f && dist != 0.0f && emits) {
+        if ((!LTREE || k >= 0) && cos_l != 0.0f && dist != 0.0f && emits) {
             sh.valid = true;
             sh.d = Ll;
             sh.tmax = ez_light_tmax(dist);
-            sh.pdf = ez_light_pdf(e.w, lights.w_total, dist, cos_l);
+            if constexpr (LTREE) sh.pdf = ez_ltree_pdf(p_sel, ez_triangle_area(f4xyz(a), f4xyz(b), f4xyz(c)), dist, cos_l);
+            else sh.pdf = ez_light_pdf(e.w, lights.w_total, dist, cos_l);
             if constexpr (ENV) sh.pdf = sh.pdf * (1.0f - env.p_env);
             if constexpr (PUNCT) sh.pdf = sh.pdf * (1.0f - punct.p_p);
             sh.light_mat = __float_as_int(a.w);
@@ -2171,14 +2225,17 @@ __device__ __forceinline__ bool medium_step(const SceneDev& sc, const RenderDev&
 // EMAP (with TEX; EZRT_PARAM_EMISSION_MAPS, ezrt_math.h, DESIGN.md section 18): a mapped emitter's emission is E(Q) at the camera
 // ray's hit and at BSDF-sample emission hits (emit_hit), whose MIS uses the triangle's lum_eff and the emission table `lights`; a
 // triangle light sample's emission is E(Q) (emit_light), out through *sh_E for k_nee, and a black one is no sample.
+// LTREE (light sampling mode with EZRT_PARAM_LIGHT_TREE, ezrt_math.h, DESIGN.md section 19): the triangle light sample's light is
+// chosen by the descent of the tree over `lights` from the shading point (ltree_descend), and its pdf and the MIS pdf of a BSDF sample
+// that hits a light of the table are ez_ltree_pdf with P_sel recomputed from the path's previous vertex p.o (ltree_hit_pdf).
 template <int MODE, bool DEFER_NEE = false, bool AOV = false, bool ENV = false, bool TRANS = false, bool MEDIUM = false, bool TEX = false,
-          bool MAPS = false, bool PUNCT = false, bool EMAP = false>
+          bool MAPS = false, bool PUNCT = false, bool EMAP = false, bool LTREE = false>
 __device__ __forceinline__ bool shade_step(const SceneDev& sc, const RenderDev& rd, int bounce, PathRegs& p, float hit_t,
                                            int hit_tri, uint32_t px, uint32_t py, float2 sob, vec3& Lo, vec3& Le,
                                            bool& primary_miss, ShadowRay& sh, float4* aov_rec = nullptr, LightsDev lights = LightsDev{},
                                            EnvDev env = EnvDev{}, MediumDev med = MediumDev{}, TexDev tex = TexDev{}, vec3* sh_base = nullptr,
                                            float2* sh_rm = nullptr, MapsDev maps = MapsDev{}, PunctDev punct = PunctDev{}, EmitDev emit = EmitDev{},
-                                           vec3* sh_E = nullptr) {
+                                           vec3* sh_E = nullptr, LightTreeDev tree = LightTreeDev{}) {
     sh.valid = false;
     const int mode = (MODE < 0) ? rd.mode : MODE;
     const bool is_mode = (mode == EZRT_MODE_DISNEY_IS_MIS_P5);
@@ -2188,14 +2245,15 @@ __device__ __forceinline__ bool shade_step(const SceneDev& sc, const RenderDev& 
     static_assert(lights_mode || !TEX, "textures are rendered in the light sampling mode");
     static_assert(TEX || !MAPS, "material maps are rendered with the textures");
     static_assert(TEX || !EMAP, "emission maps are rendered with the textures");
+    static_assert(lights_mode || !LTREE, "the light tree is rendered in the light sampling mode");
     if constexpr (MEDIUM) {
         static_assert(lights_mode && !TRANS, "the medium is rendered in the light sampling mode, without transmission");
         if (bounce > 0 && p.pdf <= 0.0f) return false;   // P5/fsh:865, before the free flight's draw
         float t_s;
         const float t_end = (hit_tri < 0) ? __int_as_float(0x7f800000) : hit_t;
         if (ez_medium_flight(&med, p.o, p.d, t_end, &p.seed, &t_s))
-            return medium_step<AOV, ENV, TEX, MAPS, PUNCT, EMAP>(sc, rd, bounce, p, t_s, hit_t, hit_tri, Lo, Le, primary_miss, sh, aov_rec, lights, env, med,
-                                                                 tex, maps, punct, emit, sh_E);
+            return medium_step<AOV, ENV, TEX, MAPS, PUNCT, EMAP, LTREE>(sc, rd, bounce, p, t_s, hit_t, hit_tri, Lo, Le, primary_miss, sh, aov_rec, lights,
+                                                                        env, med, tex, maps, punct, emit, sh_E, tree);
     }
     if (bounce == 0) {
         Lo = splat3(0.0f);
@@ -2265,7 +2323,15 @@ __device__ __forceinline__ bool shade_step(const SceneDev& sc, const RenderDev& 
                 vec3 p1, p2, p3;
                 float lum_eff;
                 const bool mapped = emit_hit(sc, tex, emit, hit_tri, rd.accel_space != 0, hit.P, E, lum_eff, p1, p2, p3);
-                if (!below) {
+                if (LTREE && !below) {
+                    const vec3 Ng = f4xyz(ldg4(tri_geo_rec(sc, hit_tri, rd.accel_space != 0)));
+                    float pl;
+                    if (ltree_hit_pdf(tree, hit_tri, rd.accel_space != 0, p.o, hit_t, ez_abs(ez_dot(Ng, p.d)), pl)) {
+                        if constexpr (ENV) pl = (1.0f - env.p_env) * pl;
+                        if constexpr (PUNCT) pl = (1.0f - punct.p_p) * pl;
+                        w = mis_mix_weight(p.pdf, pl);
+                    }
+                } else if (!below) {
                     if (!mapped) tri_vertices(sc, hit_tri, rd.accel_space != 0, p1, p2, p3);
                     if (ez_is_light(mapped ? ez_triangle_area(p1, p2, p3) * lum_eff : ez_light_weight(p1, p2, p3, mat.emissive))) {
                         const vec3 Ng = f4xyz(ldg4(tri_geo_rec(sc, hit_tri, rd.accel_space != 0)));
@@ -2280,7 +2346,15 @@ __device__ __forceinline__ bool shade_step(const SceneDev& sc, const RenderDev& 
         } else if (lights_mode) {   // a BRDF sample that hit a light: MIS against the light sampling pdf of the hit point
             float w = 1.0f;
             const float lum = ez_luminance(mat.emissive);
-            if (lum > 0.0f && !below) {   // lum <= 0: the weight area * lum is never a light; below: weight 1
+            if (LTREE && lum > 0.0f && !below) {   // ... the tree's P_sel from the previous vertex
+                const vec3 Ng = f4xyz(ldg4(tri_geo_rec(sc, hit_tri, rd.accel_space != 0)));
+                float pl;
+                if (ltree_hit_pdf(tree, hit_tri, rd.accel_space != 0, p.o, hit_t, ez_abs(ez_dot(Ng, p.d)), pl)) {
+                    if constexpr (ENV) pl = (1.0f - env.p_env) * pl;
+                    if constexpr (PUNCT) pl = (1.0f - punct.p_p) * pl;
+                    w = mis_mix_weight(p.pdf, pl);
+                }
+            } else if (lum > 0.0f && !below) {   // lum <= 0: the weight area * lum is never a light; below: weight 1
                 vec3 p1, p2, p3;
                 tri_vertices(sc, hit_tri, rd.accel_space != 0, p1, p2, p3);
                 if (ez_is_light(ez_light_weight(p1, p2, p3, mat.emissive))) {
@@ -2361,7 +2435,9 @@ __device__ __forceinline__ bool shade_step(const SceneDev& sc, const RenderDev& 
             }
         }
         if (!punct_on && !env_pick && lights.n > 0) {
-            const float4* lr = lights.rec + 4 * (size_t)ez_light_select(lights.cdf, lights.n, r_tri);
+            float p_sel = 0.0f;   // LTREE: the light's P_sel; k < 0: no sample
+            const int k = LTREE ? ltree_descend(tree, hit.P, r_tri, p_sel) : ez_light_select(lights.cdf, lights.n, r_tri);
+            const float4* lr = lights.rec + 4 * (size_t)(LTREE ? (k < 0 ? 0 : k) : k);
             const float4 a = ldg4(lr), b = ldg4(lr + 1), c = ldg4(lr + 2), e = ldg4(lr + 3);
             const int self = __float_as_int(rd.accel_space ? c.w : b.w);   // the light's triangle in the hit's index space
             const vec3 D = ez_sub(ez_triangle_point(f4xyz(a), f4xyz(b), f4xyz(c), r_1, r_2), hit.P);
@@ -2370,18 +2446,19 @@ __device__ __forceinline__ bool shade_step(const SceneDev& sc, const RenderDev& 
             const float cos_l = ez_abs(ez_dot(f4xyz(e), Ll));
             bool emits = true;
             if constexpr (EMAP) {
-                if (self != hit_tri && ez_dot(N, Ll) > 0.0f && cos_l != 0.0f && dist != 0.0f) {
+                if ((!LTREE || k >= 0) && self != hit_tri && ez_dot(N, Ll) > 0.0f && cos_l != 0.0f && dist != 0.0f) {
                     *sh_E = emit_light(sc, tex, emit, a, b, c, e, r_1, r_2);
                     emits = !emit_black(*sh_E);
                 }
             }
-            if (self != hit_tri && ez_dot(N, Ll) > 0.0f && cos_l != 0.0f && dist != 0.0f && emits) {
+            if ((!LTREE || k >= 0) && self != hit_tri && ez_dot(N, Ll) > 0.0f && cos_l != 0.0f && dist != 0.0f && emits) {
                 sh.valid = true;
                 sh.o = hit.P;
                 sh.d = Ll;
                 sh.N = N; sh.V = V; sh.history = p.history; sh.matId = sh_mat;
                 sh.tmax = ez_light_tmax(dist);
-                sh.pdf = ez_light_pdf(e.w, lights.w_total, dist, cos_l);
+                if constexpr (LTREE) sh.pdf = ez_ltree_pdf(p_sel, ez_triangle_area(f4xyz(a), f4xyz(b), f4xyz(c)), dist, cos_l);
+                else sh.pdf = ez_light_pdf(e.w, lights.w_total, dist, cos_l);
                 if constexpr (ENV) sh.pdf = sh.pdf * (1.0f - env.p_env);
                 if constexpr (PUNCT) sh.pdf = sh.pdf * (1.0f - punct.p_p);
                 sh.light_mat = __float_as_int(a.w);

@@ -204,6 +204,19 @@ struct EmitDev {
     float4* sh_emit;
 };
 
+// The light tree of EZRT_PARAM_LIGHT_TREE (ezrt_math.h, DESIGN.md section 19) over the render's light table (mode 4's, or the emission
+// table with EZRT_PARAM_EMISSION_MAPS), built by ezrt_light_tree_build at the first flagged render.  Passed to every k_shade
+// instantiation as its last parameter, after EmitDev; read by the light-tree instantiations (<.., LTREE>) only.
+//   nodes: 3 float4 per node, (lo, phi), (hi, cos_o), (axis, child word as bits), two children adjacent, the root at 0
+//   path: per light (table order), (path bits low, high, depth, area bits)
+//   light / acc_light: per triangle, its light index in the table or -1, in reference and in accel order
+struct LightTreeDev {
+    const float4* nodes;
+    const uint4* path;
+    const int32_t* light;
+    const int32_t* acc_light;
+};
+
 // A shadow ray and what k_nee needs to evaluate the light sample's contribution once the ray got through (nee_contrib):
 // the BRDF / environment evaluation of the light sample is done after the shadow pass, for unoccluded rays only.
 #define EZRT_SHADOW_SLOT_BYTES (5 * 16 + 1)

@@ -75,6 +75,7 @@ __device__ __forceinline__ uint32_t block_append(bool valid, uint32_t* counter, 
     return pos;
 }
 
+#ifndef EZRT_KERNELS_LTREE   // kernels_ltree.cu compiles only the light-tree instantiations of k_shade from this file
 // ------------------------------------------------------------------------------------------
 // LENS (EZRT_PARAM_THIN_LENS): the thin-lens camera rays of `lens`, written to the same records; every policy traces them from
 // the queue at bounce 0
@@ -525,6 +526,8 @@ __global__ void __launch_bounds__(EZRT_EXTEND_MAX_THREADS, EZRT_EXTEND_LB_BLOCKS
     extend_persistent<true, true, true, true, 4, COUNT, Q16, BOUNDED>(sc, accel_tree(sc), *s_count, work, io, g_smem_top, counts);
 }
 
+#endif
+
 // ------------------------------------------------------------------------------------------
 #ifndef EZRT_SHADE_REGROUP
 #define EZRT_SHADE_REGROUP 0      // k_shade, bounces > 0: 1 = each block shades its 128 paths in the order hits | misses (exchange through shared
@@ -555,15 +558,17 @@ __global__ void __launch_bounds__(EZRT_EXTEND_MAX_THREADS, EZRT_EXTEND_LB_BLOCKS
 // (shade_step); a punctual sample's slot carries hist.w = -2 - j and its scale in view.w.
 // EMAP (with TEX; EZRT_PARAM_EMISSION_MAPS): the emission maps emit, and lights is the emission table (shade_step); a triangle light
 // sample's slot also gets its E(Q) in emit.sh_emit[spos].
+// LTREE (EZRT_PARAM_LIGHT_TREE): the triangle light samples choose their light by the light tree `tree` over `lights`, and the
+// MIS weights of emission hits use its P_sel (shade_step).
 template <int MODE, bool LIST, bool AOV = false, bool ENV = false, bool TRANS = false, bool MEDIUM = false, bool TEX = false,
-          bool MAPS = false, bool PUNCT = false, bool EMAP = false>
+          bool MAPS = false, bool PUNCT = false, bool EMAP = false, bool LTREE = false>
 __global__ void __launch_bounds__(128, EZRT_SHADE_MIN_BLOCKS) k_shade(SceneDev sc, RenderDev rd, const TileDev* __restrict__ tiles, int bounce,
                                                uint32_t batch_first_frame, PathQueue qin, const uint32_t* __restrict__ in_count,
                                                PathQueue qout, uint32_t* out_count, ShadowQueue sq, uint32_t* s_count,
                                                float4* __restrict__ Lo, float4* __restrict__ Le, uint32_t n_fused, uint32_t n_frames,
                                                const uint32_t* __restrict__ list, const float2* __restrict__ side_hit,
                                                float4* __restrict__ aov_rec, LightsDev lights, EnvDev env, MediumDev med, TexDev tex,
-                                               MapsDev maps, PunctDev punct, EmitDev emit) {
+                                               MapsDev maps, PunctDev punct, EmitDev emit, LightTreeDev tree) {
     // The Sobol pair of (bounce, frame) is the same for every pixel of a frame (P5/fsh:361-376: up to 2 x 32 table XORs per path): each
     // block computes the pairs of the batch's frames once into shared memory (batches of more than EZRT_SOBOL_TABLE frames compute per path).
     __shared__ float2 s_sobol[EZRT_SOBOL_TABLE];
@@ -690,9 +695,9 @@ __global__ void __launch_bounds__(128, EZRT_SHADE_MIN_BLOCKS) k_shade(SceneDev s
             }
 #endif
             if (LIST || __float_as_int(hit.y) != EZRT_TRI_PENDING) {   // pending: deferred by the accel kernel, shaded by the LIST pass
-                alive = shade_step<MODE, MODE == EZRT_MODE_DISNEY_IS_MIS_P5, AOV, ENV, TRANS, MEDIUM, TEX, MAPS, PUNCT, EMAP>(sc, rd, bounce, p, hit.x, __float_as_int(hit.y), px, py,
+                alive = shade_step<MODE, MODE == EZRT_MODE_DISNEY_IS_MIS_P5, AOV, ENV, TRANS, MEDIUM, TEX, MAPS, PUNCT, EMAP, LTREE>(sc, rd, bounce, p, hit.x, __float_as_int(hit.y), px, py,
                                                                                                           sob, lo, le, pmiss, sh, AOV ? aov_rec + 2 * (size_t)slot : nullptr,
-                                                                                                          lights, env, med, tex, &sh_base, &sh_rm, maps, punct, emit, &sh_E);
+                                                                                                          lights, env, med, tex, &sh_base, &sh_rm, maps, punct, emit, &sh_E, tree);
                 if (bounce == 0) {
                     // Le is zero for every surface that does not emit: it is stored (and read back by k_blend) only otherwise.
                     // color = Le + Lo with Le = +-0 is Lo bit for bit, because Lo is never -0.0 (it starts at +0.0 and only grows by additions)
@@ -735,6 +740,7 @@ __global__ void __launch_bounds__(128, EZRT_SHADE_MIN_BLOCKS) k_shade(SceneDev s
     }
 }
 
+#ifndef EZRT_KERNELS_LTREE
 // ------------------------------------------------------------------------------------------
 // k_nee: the light samples whose shadow ray got through (sq.lit) add their contribution to Lo -- the BRDF value and pdf of the
 // light direction, the environment colour and pdf and the MIS weight (nee_contrib, P5/fsh:829-841) are evaluated here, after
@@ -1245,6 +1251,8 @@ __global__ void __launch_bounds__(256) k_atrous(int width, int height, int step,
     }
 }
 
+#endif
+
 // ------------------------------------------------------------------------------------------
 // launchers
 // ------------------------------------------------------------------------------------------
@@ -1257,6 +1265,8 @@ template <class F, class... B> static void with_bools(F&& f, bool b, B... rest) 
     if (b) with_bools([&](auto... t) { f(std::true_type{}, t...); }, rest...);
     else with_bools([&](auto... t) { f(std::false_type{}, t...); }, rest...);
 }
+
+#ifndef EZRT_KERNELS_LTREE
 
 // persistent extend/shadow kernels: block size and resident blocks per SM (each block stages its own
 // copy of the top tree levels in shared memory); env EZRT_EXTEND_THREADS / EZRT_EXTEND_BPS override
@@ -1417,9 +1427,14 @@ static void launch_shade_t(int blocks, const SceneDev& sc, const RenderDev& rd, 
             if constexpr ((M == EZRT_MODE_DISNEY_LIGHTS || !(E || T || X || TX || P)) && !(T && X) && (TX || !MP) && (TX || !EM))
                 k_shade<M, LIST, A, E, T, X, TX, MP, P, EM><<<blocks, 128, 0, st>>>(sc, rd, tiles, bounce, batch_first_frame, qin, in_count, qout, out_count, sq,
                                                                                     s_count, Lo, Le, n_fused, n_frames, list, side_hit, aov_rec, o.lights, o.env,
-                                                                                    o.med, o.tex, o.maps, o.punct, o.emit);
+                                                                                    o.med, o.tex, o.maps, o.punct, o.emit, o.tree);
         }, aov_rec != nullptr, o.env_on, o.trans_on, o.medium_on, o.tex_on, o.maps_on, o.punct_on, o.emap_on);
     };
+    if (o.tree_on) {   // the light-tree instantiations (light sampling mode only) are kernels_ltree.cu's
+        launch_shade_ltree(LIST, blocks, sc, rd, tiles, bounce, batch_first_frame, qin, in_count, qout, out_count, sq, s_count, Lo, Le, n_fused, n_frames,
+                           list, side_hit, aov_rec, o, st);
+        return;
+    }
     switch (rd.mode) {
         case EZRT_MODE_DIFFUSE_P3: launch(std::integral_constant<int, EZRT_MODE_DIFFUSE_P3>{}); break;
         case EZRT_MODE_DISNEY_ANISO_P4: launch(std::integral_constant<int, EZRT_MODE_DISNEY_ANISO_P4>{}); break;
@@ -1679,6 +1694,38 @@ void launch_sample_emission(const SceneDev& sc, const TexDev& tex, const EmitDev
                             cudaStream_t st) {
     k_sample_emission<<<div_up(n, 128), 128, 0, st>>>(sc, tex, emit, n, tri, points, rgb);
 }
+__global__ void k_ltree_ids(const float4* __restrict__ rec, int K, int32_t* __restrict__ light, int32_t* __restrict__ acc_light) {
+    const int k = blockIdx.x * blockDim.x + threadIdx.x;
+    if (k >= K) return;
+    light[__float_as_int(rec[4 * (size_t)k + 1].w)] = k;
+    acc_light[__float_as_int(rec[4 * (size_t)k + 2].w)] = k;
+}
+void launch_ltree_ids(const float4* rec, int K, int n_tri, int32_t* light, int32_t* acc_light, cudaStream_t st) {
+    cudaMemsetAsync(light, 0xff, sizeof(int32_t) * (size_t)n_tri, st);
+    cudaMemsetAsync(acc_light, 0xff, sizeof(int32_t) * (size_t)n_tri, st);
+    if (K > 0) k_ltree_ids<<<div_up(K, 256), 256, 0, st>>>(rec, K, light, acc_light);
+}
+// the light tree's device code on n inputs (ezrt_scene_light_tree_eval): which 0, ltree_descend (P, r) -> (light, P_sel; -1 and 0 for
+// no sample); which 1, ltree_prob (P, light) -> P_sel
+__global__ void k_ltree_eval(LightTreeDev tree, int which, int n, const float* __restrict__ P, const float* __restrict__ r,
+                             const int32_t* __restrict__ light_in, int32_t* __restrict__ light_out, float* __restrict__ p_out) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const vec3 Pi = ez_v3(P[3 * i], P[3 * i + 1], P[3 * i + 2]);
+    if (which == 0) {
+        float q = 0.0f;
+        light_out[i] = ltree_descend(tree, Pi, r[i], q);
+        p_out[i] = q;
+    } else {
+        float area;
+        p_out[i] = ltree_prob(tree, Pi, light_in[i], &area);
+    }
+}
+void launch_ltree_eval(const LightTreeDev& tree, int which, int n, const float* P, const float* r, const int32_t* light_in, int32_t* light_out,
+                       float* p_out, cudaStream_t st) {
+    if (n <= 0) return;
+    k_ltree_eval<<<div_up(n, 128), 128, 0, st>>>(tree, which, n, P, r, light_in, light_out, p_out);
+}
 void launch_eval_math(int which, int n, const float* a, const float* b, float* out, cudaStream_t st) {
     k_eval_math<<<div_up(n, 256), 256, 0, st>>>(which, n, a, b, out);
 }
@@ -1703,3 +1750,5 @@ void launch_denoise(const float* color, int channels, const float* aov, const fl
                                          (k & 1) ? cv0 : cv1, color, last ? out : nullptr, channels);
     }
 }
+
+#endif  // EZRT_KERNELS_LTREE

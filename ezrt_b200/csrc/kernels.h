@@ -25,6 +25,7 @@
 //   maps_on   EZRT_PARAM_MATERIAL_MAPS (with tex_on): the material maps of tex (<.., TEX, MAPS>)
 //   punct_on  EZRT_PARAM_PUNCTUAL_LIGHTS and the scene's punctual table has J > 0 lights: punct (<.., PUNCT>)
 //   emap_on   EZRT_PARAM_EMISSION_MAPS (with tex_on): the emission maps emit, and lights is the emission table (<.., TEX, .., EMAP>)
+//   tree_on   EZRT_PARAM_LIGHT_TREE and the render's table has K > 0 lights: the tree over lights, tree (k_shade<.., LTREE>)
 // All off outside the light sampling mode; the tables are zero where unused, as the kernels' parameters.
 struct LightOptions {
     LightsDev lights{};   // the light table (light sampling mode)
@@ -34,7 +35,8 @@ struct LightOptions {
     MapsDev maps{};       // the maps' table and the shadow slots' metallic (maps_on)
     PunctDev punct{};     // the punctual lights' table and P_p (punct_on)
     EmitDev emit{};       // the emission maps' records and the shadow slots' E(Q) (emap_on)
-    bool env_on = false, trans_on = false, medium_on = false, tex_on = false, maps_on = false, punct_on = false, emap_on = false;
+    LightTreeDev tree{};  // the light tree over lights (tree_on)
+    bool env_on = false, trans_on = false, medium_on = false, tex_on = false, maps_on = false, punct_on = false, emap_on = false, tree_on = false;
 };
 
 // lens (EZRT_PARAM_THIN_LENS): the thin-lens camera rays (k_generate<true>); null: the pinhole's
@@ -126,6 +128,18 @@ void launch_emit_records(const float2* emit_rec, const int32_t* idx, int n, floa
 // ezrt_scene_sample_emission: n (reference triangle, point) pairs -> E(Q) (3 floats each); emit.rec null: no maps
 void launch_sample_emission(const SceneDev& sc, const TexDev& tex, const EmitDev& emit, int n, const int32_t* tri, const float* points, float* rgb,
                             cudaStream_t st);
+// the light tree's per-triangle light indices (LightTreeDev): light and acc_light (n_tri each) -1, then k at light k's triangle in
+// reference order (its record's b.w) and in accel order (c.w), for the K records rec of the tree's table
+void launch_ltree_ids(const float4* rec, int K, int n_tri, int32_t* light, int32_t* acc_light, cudaStream_t st);
+// launch_shade's light-tree renders (o.tree_on, light sampling mode): k_shade<EZRT_MODE_DISNEY_LIGHTS, list, .., LTREE = true>, compiled
+// in kernels_ltree.cu so that its instantiations compile beside kernels.cu's
+void launch_shade_ltree(bool list, int blocks, const SceneDev& sc, const RenderDev& rd, const TileDev* tiles, int bounce, uint32_t batch_first_frame,
+                        PathQueue qin, const uint32_t* in_count, PathQueue qout, uint32_t* out_count, ShadowQueue sq, uint32_t* s_count, float4* Lo,
+                        float4* Le, uint32_t n_fused, uint32_t n_frames, const uint32_t* list_idx, const float2* side_hit, float4* aov_rec,
+                        const LightOptions& o, cudaStream_t st);
+// ezrt_scene_light_tree_eval: which 0, the descent (P, r) -> (light, P_sel); which 1, the hit side (P, light) -> P_sel (n inputs)
+void launch_ltree_eval(const LightTreeDev& tree, int which, int n, const float* P, const float* r, const int32_t* light_in, int32_t* light_out,
+                       float* p_out, cudaStream_t st);
 void launch_eval_math(int which, int n, const float* a, const float* b, float* out, cudaStream_t st);
 void launch_tonemap(const float* in, int channels, float* out, long long n, float limit, cudaStream_t st);
 void launch_partition_scatter(const float* compact, float* full, const TileDev* tiles, int n_tiles, int width, int channels,

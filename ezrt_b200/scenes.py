@@ -227,6 +227,45 @@ def s_1m_bunny(builder=api.BVH_SAH_FAST):
     return s_grid(15, 14, 4, builder, mesh="bunny", count=201)
 
 
+def lamps_meshes(nx, nz, pitch=1.2, mesh="blob", count=None, rough=False, seed=5):
+    """grid_meshes(nx, nz, 0, ...) with a small emissive sphere (320 triangles, scale 0.2) at y = 0.4 over each instance, in place of
+    the four big ones.  Lamp i's colour is 0.4 + 0.6 u (per channel) and its intensity 2 * 100^u' (2 to 200), from
+    seeded uniforms; rough=True sets every instance's roughness to at least 0.5 and its metallic to at most 0.5."""
+    out = grid_meshes(nx, nz, 0, pitch, mesh, count)
+    floor = out.pop()
+    if rough:
+        out = [(t, Material(**{**m.__dict__, "roughness": max(m.roughness, 0.5), "metallic": min(m.metallic, 0.5)}), tr, sm)
+               for t, m, tr, sm in out]
+    n = len(out)
+    u = np.array(_unit_randoms(seed * 7919 + 3, 4 * n)).reshape(n, 4)
+    sph = sphere_obj()
+    for i in range(n):
+        ix, iz = i % nx, i // nx
+        x = (ix - (nx - 1) / 2.0) * pitch
+        z = (iz - (nz - 1) / 2.0) * pitch
+        E = (0.4 + 0.6 * u[i, :3]) * (2.0 * 100.0 ** u[i, 3])
+        out.append((sph, Material(baseColor=(1, 1, 1), emissive=tuple(float(e) for e in E)),
+                    transform_matrix((0, 0, 0), (x, 0.4, z), (0.2, 0.2, 0.2)), False))
+    out.append(floor)
+    return out
+
+
+def s_lamps(nx, nz, builder=api.BVH_SAH_FAST, pitch=1.2, mesh="blob", count=None, rough=False, seed=5):
+    """lamps_meshes() built with the default leaf size, camera as s_grid.  Returns (tris, nodes, eye, cam)."""
+    tl = TriangleList()
+    for text, m, trans, smooth in lamps_meshes(nx, nz, pitch, mesh, count, rough, seed):
+        tl.read_obj_text(text, m, trans, smooth)
+    tris, nodes = tl.build_bvh(8, builder)
+    r = 0.62 * max(nx * pitch, nz * pitch) + 3.0
+    eye, cam = api.camera_orbit(30.0, 25.0, r)
+    return tris, nodes, eye, cam
+
+
+def s_1m_lamps(builder=api.BVH_SAH_FAST):
+    """S-1M's 201 bunnies with a lamp over each (s_lamps): 201 * 4968 + 201 * 320 + 12 = 1,062,900 triangles, 64,320 of them lights."""
+    return s_lamps(15, 14, builder, mesh="bunny", count=201)
+
+
 def p3_bunny_meshes():
     """P3's scene block (P3/main.cpp:690-701) with the real bunny."""
     return [

@@ -194,6 +194,18 @@ typedef struct ezrt_render_params {
    emission maps set.  Accepted by ezrt_render[_device], ezrt_render_adaptive[_device] and ezrt_render_aov[_device]; each shadow
    slot takes 16 more bytes. */
 #define EZRT_PARAM_EMISSION_MAPS 256
+/* ezrt_render_params.reserved[0], EZRT_MODE_DISNEY_LIGHTS on the wavefront pipeline only, with or without every other flag of that
+   mode: a triangle light sample picks its light from a light tree over the render's table (mode 4's, or the emission table with
+   EZRT_PARAM_EMISSION_MAPS) instead of by power alone.  The tree is descended from the shading point with the selection number the
+   table search would use, each step choosing a child by its power, distance and orientation from the point (no receiver normal), and
+   the light sample's pdf and the MIS weight of a BSDF sample that hits a light use the product of the chosen probabilities, recomputed
+   from the path's previous vertex (ezrt_math.h, DESIGN.md section 19).  No draw is added; the estimator stays unbiased because both
+   strategies' pdfs are the same function.  A scene without triangle lights renders mode 4's image.  The first such render of a scene
+   builds the tree on the host beside the table (ezrt_light_tree_build; device memory: 48 bytes per node of 2K - 1, 16 per light and
+   8 per triangle), which synchronises the render's stream once.  Invalid (EZRT_ERR_INVALID) in another mode and with the
+   megakernel.  Accepted by ezrt_render[_device], ezrt_render_adaptive[_device] and ezrt_render_aov[_device]; the shadow slots keep
+   their sizes. */
+#define EZRT_PARAM_LIGHT_TREE 512
 
 /* One punctual light of ezrt_scene_set_punctual_lights (glTF's KHR_lights_punctual, in the render's units: no photometric
    conversion; the caller scales glTF's candela and lux) */
@@ -317,6 +329,25 @@ int ezrt_scene_emission_lights(ezrt_scene* scene, int cap, int32_t* tri_out, flo
  * each) = E(Q) with the scene's emission maps (none set: each triangle's material emission).  Host arrays; synchronous.
  * EZRT_ERR_INVALID without textures set or for a triangle index out of range. */
 int ezrt_scene_sample_emission(ezrt_scene* scene, int n, const int32_t* tri, const float* points, float* rgb_out);
+/* The light tree of EZRT_PARAM_LIGHT_TREE over n lights (ezrt_math.h, DESIGN.md section 19), on the host, without a device: verts
+ * = each light's three vertices (9 floats), weights = its table weight (finite and > 0).  Returns M = 2n - 1 nodes (0 for n = 0), or
+ * EZRT_ERR_INVALID for a bad weight, a vertex that is not finite or a null array with n > 0.  With cap >= M and both outputs given,
+ * writes nodes_out (12 floats per node, ezrt_math.h's record) and paths_out (4 words per light: its path from the root as 64 bits,
+ * low word first -- bit j set where step j goes right -- its depth, and the bits of its area ez_triangle_area(p1, p2, p3)); otherwise
+ * writes nothing.  Deterministic. */
+int ezrt_light_tree_build(int n, const float* verts, const float* weights, int cap, float* nodes_out, uint32_t* paths_out);
+/* The light tree the EZRT_PARAM_LIGHT_TREE renders use over mode 4's table (emission = 0) or the emission table (emission != 0;
+ * EZRT_ERR_INVALID without emission maps), built on the first call or flagged render: ezrt_light_tree_build's output over the table's
+ * lights in table order.  Returns M, the number of nodes, or a negative status; writes min(M, cap) node records into nodes_out and,
+ * with cap >= M, the K paths into paths_out.  Either output may be NULL.  Synchronises the scene's device once, to build. */
+int ezrt_scene_light_tree(ezrt_scene* scene, int emission, int cap, float* nodes_out, uint32_t* paths_out);
+/* The device's tree code on n inputs (host arrays; synchronous), over the tree of ezrt_scene_light_tree(scene, emission):
+ * which = 0, the descent: P (3 floats each) and r (1 float each) -> light_out (the light index in table order, -1 for no sample) and
+ *   p_out (P_sel; 0 for no sample);
+ * which = 1, the hit side: P and light_in (light indices) -> p_out (P_sel of that light at P), r and light_out unused.
+ * EZRT_ERR_INVALID for another which, a light index out of range, or a table without lights. */
+int ezrt_scene_light_tree_eval(ezrt_scene* scene, int emission, int which, int n, const float* P, const float* r, const int32_t* light_in,
+                               int32_t* light_out, float* p_out);
 
 /* render(width,height,spp) -> framebuffer: equals `spp` consecutive display() calls
  * (P5/main.cpp:697-748) each drawing pass1 (P5/fsh:894-949) and copying to lastFrame.

@@ -985,4 +985,104 @@ EZ_HD ez_vec3 ez_punct_contrib(ez_vec3 history, ez_vec3 f, float cosine, ez_vec3
     return ez_scale(ez_mul(ez_scale(ez_mul(history, f), cosine), E), s);
 }
 
+/* ------------------------------------------------------------------ the light tree (EZRT_PARAM_LIGHT_TREE, DESIGN.md section 19)
+ * A binary tree over the K lights of the render's table (ezrt_light_tree_build, 2K - 1 nodes, the root node 0, two children adjacent).
+ * Node record, 12 floats: [0..2] lo, [3] phi, [4..6] hi, [7] cos_o, [8..10] axis a, [11] the child word as int bits: c >= 0 the left
+ * child's index (the right one is c + 1), c < 0 the leaf of light ~c.  [lo, hi] contains every vertex of the node's lights, phi is the
+ * (float) of the float64 sum of their table weights, and |dot(N_k, a)| >= cos_o for each light's geometric normal (emission is
+ * two-sided, so the cone bounds the normals' lines).
+ * Importance of a node at a point P (no receiver normal): c = lo / 2 + hi / 2, r^2 = |hi - lo|^2 / 4, D = P - c, d^2 = max(|D|^2, r^2);
+ *   theta_w = the angle of P - c to the line of a, in [0, pi/2]; theta_o = acos(cos_o); theta_b = asin(r / |D|) (pi/2 for |D|^2 <= r^2);
+ *   I = phi * cos(max(0, theta_w - theta_o - theta_b)) / d^2, and 0 where that cosine is not > 0 (differences of angles as cosines and
+ *   sines, ez_ltree_importance's order).
+ * Child probability p_L = I_L / (I_L + I_R), p_R = 1 - p_L; where I_L + I_R is not finite or not > 0, p_L = phi_L / (phi_L + phi_R).
+ * Descent (light sample, r = r_tri): r = min(r, 1 - 2^-24); at each interior node left iff r < p_L, r = r / p_L, else
+ *   r = (r - p_L) / (1 - p_L), then r = min(r, 1 - 2^-24); P_sel = the product of the taken probabilities, root to leaf; a taken
+ *   probability that is not > 0 is no sample.  Hit side (an emission hit on light k from the path's previous vertex P): the same
+ *   products along k's path.  pdf = ez_ltree_pdf(P_sel, area_k, dist, cos_l) in place of ez_light_pdf, with the factors of sections 11
+ *   and 17. */
+typedef struct ez_ltree_node {
+    ez_vec3 lo;
+    float phi;
+    ez_vec3 hi;
+    float cos_o;
+    ez_vec3 axis;
+    int child;
+} ez_ltree_node;
+EZ_HD ez_ltree_node ez_ltree_load(const float* nd) {
+    ez_ltree_node n;
+    n.lo = ez_v3(nd[0], nd[1], nd[2]); n.phi = nd[3];
+    n.hi = ez_v3(nd[4], nd[5], nd[6]); n.cos_o = nd[7];
+    n.axis = ez_v3(nd[8], nd[9], nd[10]); n.child = (int)ez_f2u(nd[11]);
+    return n;
+}
+EZ_HD float ez_ltree_importance(const ez_ltree_node* n, ez_vec3 P) {
+    const ez_vec3 c = ez_add(ez_scale(n->lo, 0.5f), ez_scale(n->hi, 0.5f));
+    const ez_vec3 e = ez_sub(n->hi, n->lo);
+    const float r2 = 0.25f * ez_dot(e, e);
+    const ez_vec3 D = ez_sub(P, c);
+    const float dd = ez_dot(D, D);
+    float cosine = 1.0f;
+    if (!(dd <= r2)) {   // P outside the bounding sphere (or NaN)
+        const float len = EZ_SQRT(dd);
+        const float cos_w = ez_min(EZ_DIV(ez_abs(ez_dot(n->axis, D)), len), 1.0f);
+        if (!(cos_w >= n->cos_o)) {
+            const float sin_w = EZ_SQRT(ez_max(0.0f, 1.0f - cos_w * cos_w));
+            const float sin_o = EZ_SQRT(ez_max(0.0f, 1.0f - n->cos_o * n->cos_o));
+            const float c1 = cos_w * n->cos_o + sin_w * sin_o;   // theta_w - theta_o in (0, pi/2]
+            const float s1 = sin_w * n->cos_o - cos_w * sin_o;
+            const float sin2_b = EZ_DIV(r2, dd);
+            const float cos_b = EZ_SQRT(ez_max(0.0f, 1.0f - sin2_b));
+            if (!(c1 >= cos_b)) cosine = c1 * cos_b + s1 * EZ_SQRT(sin2_b);
+        }
+    }
+    return (cosine > 0.0f) ? EZ_DIV(n->phi * cosine, ez_max(dd, r2)) : 0.0f;
+}
+/* p_L of the children L, R at P */
+EZ_HD float ez_ltree_p_left(const ez_ltree_node* L, const ez_ltree_node* R, ez_vec3 P) {
+    const float iL = ez_ltree_importance(L, P), iR = ez_ltree_importance(R, P);
+    const float s = iL + iR;
+    if (ez_finite(s) && s > 0.0f) return EZ_DIV(iL, s);
+    return EZ_DIV(L->phi, L->phi + R->phi);
+}
+/* one step of the descent with p_L = pl: 0 left or 1 right, *r rescaled and clamped, *q times the taken probability; -1: no sample */
+EZ_HD int ez_ltree_step(float pl, float* r, float* q) {
+    const int right = !(*r < pl);
+    const float pt = right ? 1.0f - pl : pl;
+    if (!(pt > 0.0f)) return -1;
+    *r = ez_min(right ? EZ_DIV(*r - pl, 1.0f - pl) : EZ_DIV(*r, pl), 0.99999994f);
+    *q = *q * pt;
+    return right;
+}
+/* the light sample's and the emission hit's solid-angle pdf: ((P_sel / area) * (dist * dist)) / cos_l */
+EZ_HD float ez_ltree_pdf(float p_sel, float area, float dist, float cos_l) { return EZ_DIV(EZ_DIV(p_sel, area) * (dist * dist), cos_l); }
+/* the descent over the node records nodes (12 floats each): the light chosen by r at P, *p_sel its P_sel; -1 for no sample */
+EZ_HD int ez_ltree_descend(const float* nodes, ez_vec3 P, float r, float* p_sel) {
+    float q = 1.0f;
+    r = ez_min(r, 0.99999994f);
+    ez_ltree_node n = ez_ltree_load(nodes);
+    while (n.child >= 0) {
+        const ez_ltree_node L = ez_ltree_load(nodes + 12 * (size_t)n.child), R = ez_ltree_load(nodes + 12 * ((size_t)n.child + 1));
+        const int s = ez_ltree_step(ez_ltree_p_left(&L, &R, P), &r, &q);
+        if (s < 0) return -1;
+        n = s ? R : L;
+    }
+    *p_sel = q;
+    return ~n.child;
+}
+/* P_sel of the light whose path from the root is `path` (bit j: the step at depth j goes right) of length depth, at P */
+EZ_HD float ez_ltree_prob(const float* nodes, ez_vec3 P, uint64_t path, int depth) {
+    float q = 1.0f;
+    int i = 0;
+    for (int j = 0; j < depth; j++) {
+        const int c = (int)ez_f2u(nodes[12 * (size_t)i + 11]);
+        const ez_ltree_node L = ez_ltree_load(nodes + 12 * (size_t)c), R = ez_ltree_load(nodes + 12 * ((size_t)c + 1));
+        const float pl = ez_ltree_p_left(&L, &R, P);
+        const int right = (int)((path >> j) & 1u);
+        q = q * (right ? 1.0f - pl : pl);
+        i = c + right;
+    }
+    return q;
+}
+
 #endif /* EZRT_MATH_H */
