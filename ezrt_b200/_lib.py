@@ -79,6 +79,9 @@ SIGNATURES = {
     "ezrt_light_tree_build": (C.c_int, [C.c_int, c_float_p, c_float_p, C.c_int, c_float_p, c_uint32_p]),
     "ezrt_scene_light_tree": (C.c_int, [C.c_void_p, C.c_int, C.c_int, c_float_p, c_uint32_p]),
     "ezrt_scene_light_tree_eval": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, c_float_p, c_float_p, c_int32_p, c_int32_p, c_float_p]),
+    "ezrt_scene_set_medium_grid": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, c_float_p]),
+    "ezrt_scene_medium_grid": (C.c_int, [C.c_void_p, C.c_int, c_int32_p, c_float_p]),
+    "ezrt_scene_medium_eval": (C.c_int, [C.c_void_p, C.c_int, C.c_int, c_float_p, c_float_p, c_float_p, c_uint32_p, c_int32_p, c_float_p, c_uint32_p]),
     "ezrt_scene_sample_emission": (C.c_int, [C.c_void_p, C.c_int, c_int32_p, c_float_p, c_float_p]),
     "ezrt_scene_set_material_maps": (C.c_int, [C.c_void_p, c_int32_p, c_int32_p]),
     "ezrt_scene_sample_materials": (C.c_int, [C.c_void_p, C.c_int, c_int32_p, c_float_p, c_float_p]),

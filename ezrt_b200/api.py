@@ -29,6 +29,7 @@ PARAM_MATERIAL_MAPS = 64
 PARAM_PUNCTUAL_LIGHTS = 128
 PARAM_EMISSION_MAPS = 256
 PARAM_LIGHT_TREE = 512
+PARAM_MEDIUM_GRID = 1024
 PUNCTUAL_POINT, PUNCTUAL_SPOT, PUNCTUAL_DIRECTIONAL = 0, 1, 2   # ezrt_punctual_light.type
 MODES = {"diffuse_p3": 0, "disney_aniso_p4": 1, "disney_sobol_p5": 2, "disney_is_mis_p5": 3, "disney_lights": 4}
 
@@ -259,6 +260,7 @@ class RenderConfig:
     punctual_lights: bool = False  # EZRT_PARAM_PUNCTUAL_LIGHTS (MODE_DISNEY_LIGHTS only): the scene's punctual lights (Scene.set_punctual_lights, DESIGN.md section 17)
     emission_maps: bool = False  # EZRT_PARAM_EMISSION_MAPS (with textures): the scene's emission maps (Scene.set_emission_maps, DESIGN.md section 18)
     light_tree: bool = False    # EZRT_PARAM_LIGHT_TREE (MODE_DISNEY_LIGHTS only): triangle lights chosen by a light tree (Scene.light_tree, DESIGN.md section 19)
+    medium_grid: bool = False   # EZRT_PARAM_MEDIUM_GRID (with medium): the medium's density grid (Scene.set_medium_grid, DESIGN.md section 20)
 
     def to_struct(self):
         p = RenderParams()
@@ -274,7 +276,7 @@ class RenderConfig:
                          (PARAM_TRANSMISSION if self.transmission else 0) | (PARAM_MEDIUM if self.medium else 0) |
                          (PARAM_TEXTURES if self.textures else 0) | (PARAM_MATERIAL_MAPS if self.material_maps else 0) |
                          (PARAM_PUNCTUAL_LIGHTS if self.punctual_lights else 0) | (PARAM_EMISSION_MAPS if self.emission_maps else 0) |
-                         (PARAM_LIGHT_TREE if self.light_tree else 0))
+                         (PARAM_LIGHT_TREE if self.light_tree else 0) | (PARAM_MEDIUM_GRID if self.medium_grid else 0))
         if self.lens_radius != 0:   # a negative or NaN radius is set too, so that the library rejects it
             if self.focus_distance is None:
                 raise ValueError("RenderConfig: a lens (lens_radius != 0) needs a focus_distance")
@@ -403,6 +405,60 @@ class Scene:
         m.box_min[:] = [float(x) for x in box_min]
         m.box_max[:] = [float(x) for x in box_max]
         check(lib.ezrt_scene_set_medium(self._h, C.byref(m)))
+
+    def set_medium_grid(self, density):
+        """ezrt_scene_set_medium_grid: the density grid RenderConfig.medium_grid renders (DESIGN.md section 20) -- density float32
+        [nz, ny, nx] (finite, >= 0), filling the medium's box, sigma = sigma_t * density.  set_medium_grid(None) clears it.  Waits for
+        the renders already enqueued."""
+        if density is None:
+            check(lib.ezrt_scene_set_medium_grid(self._h, 0, 0, 0, None))
+            return
+        g = np.ascontiguousarray(np.asarray(density, np.float32))
+        if g.ndim != 3:
+            raise ValueError("Scene.set_medium_grid: density must be [nz, ny, nx]")
+        nz, ny, nx = g.shape
+        check(lib.ezrt_scene_set_medium_grid(self._h, nx, ny, nz, _fp(g)))
+
+    def medium_grid(self):
+        """The grid's brick maxima (ezrt_scene_medium_grid): float32 [bz, by, bx], each the largest density over its 8^3 cells dilated
+        by one lattice point."""
+        dims = np.zeros(6, np.int32)
+        b = check(lib.ezrt_scene_medium_grid(self._h, 0, dims.ctypes.data_as(_lib.c_int32_p), None))
+        out = np.zeros(b, np.float32)
+        check(lib.ezrt_scene_medium_grid(self._h, b, None, _fp(out)))
+        return out.reshape(int(dims[5]), int(dims[4]), int(dims[3]))
+
+    def _medium_eval(self, which, o, d=None, L=None, seed=None):
+        o = np.ascontiguousarray(np.asarray(o, np.float32).reshape(-1, 3))
+        n = o.shape[0]
+        out = np.zeros(n, np.float32)
+        if which == 0:
+            check(lib.ezrt_scene_medium_eval(self._h, 0, n, _fp(o), None, None, None, None, _fp(out), None))
+            return out, None, None
+        d = np.ascontiguousarray(np.asarray(d, np.float32).reshape(-1, 3))
+        L = np.ascontiguousarray(np.asarray(L, np.float32).reshape(-1))
+        seed = np.ascontiguousarray(np.asarray(seed, np.uint32).reshape(-1))
+        assert d.shape[0] == n and L.shape[0] == n and seed.shape[0] == n
+        flag = np.zeros(n, np.int32)
+        seed_out = np.zeros(n, np.uint32)
+        check(lib.ezrt_scene_medium_eval(self._h, which, n, _fp(o), _fp(d), _fp(L), seed.ctypes.data_as(_lib.c_uint32_p),
+                                         flag.ctypes.data_as(_lib.c_int32_p), _fp(out), seed_out.ctypes.data_as(_lib.c_uint32_p)))
+        return out, flag, seed_out
+
+    def medium_density(self, points):
+        """The device's sigma = sigma_t * rho at points [n, 3] (ezrt_scene_medium_eval, which 0): float32 [n]."""
+        return self._medium_eval(0, points)[0]
+
+    def medium_flight(self, o, d, t_end, seed):
+        """The device's free flight through the grid (ezrt_scene_medium_eval, which 1) of the segments o + t d, t <= t_end, from the path
+        seeds seed (uint32): (scatters int32 [n], t_s float32 [n], the advanced seed uint32 [n])."""
+        t_s, flag, seed_out = self._medium_eval(1, o, d, t_end, seed)
+        return flag, t_s, seed_out
+
+    def medium_transmittance(self, o, d, L, seed):
+        """The device's ratio-tracked transmittance of the shadow rays o + t d, t <= L, from the shadow seeds seed (ezrt_scene_medium_eval,
+        which 2): float32 [n]."""
+        return self._medium_eval(2, o, d, L, seed)[0]
 
     def set_textures(self, textures, texcoords=None, texture_id=None):
         """ezrt_scene_set_textures: the base-colour textures RenderConfig.textures renders (DESIGN.md section 15).  textures: uint8

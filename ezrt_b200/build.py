@@ -331,6 +331,26 @@ def build_oracle_emission_maps(force=False):
 ORACLE_LIGHT_TREE_SO = os.path.join(ROOT, "build", "libezrt_oracle_light_tree.so")
 
 
+ORACLE_MEDIUM_GRID_SO = os.path.join(ROOT, "build", "libezrt_oracle_medium_grid.so")
+
+
+def build_oracle_medium_grid(force=False):
+    """build/libezrt_oracle_medium_grid.so: tests/oracle_medium_grid.cpp, the CPU restatement of the density grid (its brick maxima,
+    lookup, free flight and transmittance with their majorant counters, and the flagged renders over the light tree's restatement;
+    test infrastructure, loaded only by tests/oracle_medium_grid.py)."""
+    src = os.path.join(ROOT, "tests", "oracle_medium_grid.cpp")
+    deps = [src] + [os.path.join(ROOT, "tests", f) for f in ("oracle_light_tree.cpp", "oracle_emission_maps.cpp", "oracle_punctual.cpp",
+                                                             "oracle_material_maps.cpp", "oracle_textures.cpp", "oracle_medium.cpp", "oracle_lens.cpp",
+                                                             "oracle_transmission.cpp", "oracle_env_light.cpp", "oracle_lights.cpp")] + \
+        [os.path.join(ROOT, "oracle", "ezrt_oracle.cpp")] + [os.path.join(INCLUDE, f) for f in os.listdir(INCLUDE)]
+    if force or _newer(ORACLE_MEDIUM_GRID_SO, deps):
+        os.makedirs(os.path.dirname(ORACLE_MEDIUM_GRID_SO), exist_ok=True)
+        tmp = ORACLE_MEDIUM_GRID_SO + ".tmp%d" % os.getpid()
+        _run(["g++"] + HOST_FLAGS + ["-fopenmp", "-Wno-misleading-indentation", "-shared", "-I", INCLUDE, src, "-o", tmp])
+        os.replace(tmp, ORACLE_MEDIUM_GRID_SO)
+    return ORACLE_MEDIUM_GRID_SO
+
+
 def build_oracle_light_tree(force=False):
     """build/libezrt_oracle_light_tree.so: tests/oracle_light_tree.cpp, the CPU restatement of the light tree (the descent, the
     hit-side walk, the flagged render's medium and transmission loops) over the emission maps' restatement (test infrastructure,

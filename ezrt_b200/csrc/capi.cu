@@ -109,6 +109,12 @@ struct ezrt_scene {
     // the homogeneous medium of EZRT_PARAM_MEDIUM (ezrt_scene_set_medium), copied into the kernels' parameters at every render
     bool has_medium = false;
     MediumDev medium{};
+    // the density grid of EZRT_PARAM_MEDIUM_GRID (ezrt_scene_set_medium_grid): densities | brick maxima, and the host copy of the maxima
+    bool has_grid = false;
+    DeviceBuffer grid_buf;
+    GridDev grid{};
+    std::vector<float> grid_brick;
+    float grid_max = 0.0f;   // the largest density
     // the base-colour textures of EZRT_PARAM_TEXTURES (ezrt_scene_set_textures): sRGB table | texture table | texels, and the texcoord
     // records in reference | accel order; tex.sh_base is set per render
     DeviceBuffer tex_buf, tex_rec_buf;
@@ -245,6 +251,12 @@ int validate_params(const ezrt_scene* scene, const ezrt_render_params* p) {
         if (p->reserved[0] & EZRT_PARAM_TRANSMISSION)
             return ezrt_set_error(EZRT_ERR_INVALID, "render: EZRT_PARAM_MEDIUM is not rendered with EZRT_PARAM_TRANSMISSION (glass is defined with vacuum outside)");
         if (!scene->has_medium) return ezrt_set_error(EZRT_ERR_INVALID, "render: EZRT_PARAM_MEDIUM needs a medium (ezrt_scene_set_medium)");
+    }
+    if (p->reserved[0] & EZRT_PARAM_MEDIUM_GRID) {
+        if (!(p->reserved[0] & EZRT_PARAM_MEDIUM)) return ezrt_set_error(EZRT_ERR_INVALID, "render: EZRT_PARAM_MEDIUM_GRID needs EZRT_PARAM_MEDIUM");
+        if (!scene->has_grid) return ezrt_set_error(EZRT_ERR_INVALID, "render: EZRT_PARAM_MEDIUM_GRID needs a grid (ezrt_scene_set_medium_grid)");
+        if (!ez_finite(scene->medium.sigma_t * scene->grid_max))
+            return ezrt_set_error(EZRT_ERR_INVALID, "render: the medium's sigma_t times the grid's largest density is not finite");
     }
     if (p->reserved[0] & EZRT_PARAM_TEXTURES) {
         if (p->mode != EZRT_MODE_DISNEY_LIGHTS)
@@ -1063,6 +1075,105 @@ int ezrt_scene_set_medium(ezrt_scene* s, const ezrt_medium* m) {
     return EZRT_OK;
 }
 
+int ezrt_scene_set_medium_grid(ezrt_scene* s, int nx, int ny, int nz, const float* density) {
+    if (!s) return ezrt_set_error(EZRT_ERR_INVALID, "scene_set_medium_grid: null scene");
+    CU_CHECK(cudaSetDevice(s->device));
+    if (!density) {
+        CU_CHECK(cudaDeviceSynchronize());   // renders already enqueued still read the buffer
+        s->grid_buf.release();
+        s->grid = GridDev{};
+        s->grid_brick.clear();
+        s->grid_max = 0.0f;
+        s->has_grid = false;
+        return EZRT_OK;
+    }
+    if (nx < 1 || nx > 1024 || ny < 1 || ny > 1024 || nz < 1 || nz > 1024)
+        return ezrt_set_error(EZRT_ERR_INVALID, "scene_set_medium_grid: the grid is %dx%dx%d (each side 1 to 1024)", nx, ny, nz);
+    const size_t n = (size_t)nx * ny * nz;
+    float mx = 0.0f;
+    for (size_t i = 0; i < n; i++) {
+        if (!(ez_finite(density[i]) && density[i] >= 0.0f))
+            return ezrt_set_error(EZRT_ERR_INVALID, "scene_set_medium_grid: density %zu is negative or not finite", i);
+        mx = ez_max(mx, density[i]);
+    }
+    if (s->has_medium && !ez_finite(s->medium.sigma_t * mx))
+        return ezrt_set_error(EZRT_ERR_INVALID, "scene_set_medium_grid: the medium's sigma_t times the largest density is not finite");
+    GridDev g{};
+    g.rho = density;
+    g.n[0] = nx; g.n[1] = ny; g.n[2] = nz;
+    for (int a = 0; a < 3; a++) g.b[a] = ez_grid_bricks(g.n[a]);
+    std::vector<float> brick((size_t)g.b[0] * g.b[1] * g.b[2]);
+    for (int k = 0; k < g.b[2]; k++)
+        for (int j = 0; j < g.b[1]; j++)
+            for (int i = 0; i < g.b[0]; i++) brick[((size_t)k * g.b[1] + j) * g.b[0] + i] = ez_grid_brick_max(&g, i, j, k);
+    // the new buffer is filled before the previous one is released, so that a failure keeps the previous grid
+    DeviceBuffer nb;
+    int rc = nb.ensure(sizeof(float) * (n + brick.size()));
+    if (rc) return rc;
+    cudaError_t e = cudaMemcpy(nb.p, density, sizeof(float) * n, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = cudaMemcpy((float*)nb.p + n, brick.data(), sizeof(float) * brick.size(), cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = cudaDeviceSynchronize();   // renders already enqueued still read the previous buffer
+    if (e != cudaSuccess) {
+        nb.release();
+        return ezrt_set_error(EZRT_ERR_CUDA, "scene_set_medium_grid: %s", cudaGetErrorString(e));
+    }
+    s->grid_buf.release();
+    s->grid_buf = nb;   // DeviceBuffer frees only on release(): the pointer moves to the scene
+    g.rho = (const float*)nb.p;
+    g.brick = (const float*)nb.p + n;
+    s->grid = g;
+    s->grid_brick.swap(brick);
+    s->grid_max = mx;
+    s->has_grid = true;
+    return EZRT_OK;
+}
+
+int ezrt_scene_medium_grid(ezrt_scene* s, int cap, int32_t* dims_out, float* brick_max_out) {
+    if (!s || cap < 0) return ezrt_set_error(EZRT_ERR_INVALID, "scene_medium_grid: bad argument");
+    if (!s->has_grid) return ezrt_set_error(EZRT_ERR_INVALID, "scene_medium_grid: no grid (ezrt_scene_set_medium_grid)");
+    if (dims_out)
+        for (int a = 0; a < 3; a++) { dims_out[a] = s->grid.n[a]; dims_out[3 + a] = s->grid.b[a]; }
+    const int B = (int)s->grid_brick.size();
+    if (brick_max_out) std::copy(s->grid_brick.begin(), s->grid_brick.begin() + std::min(B, cap), brick_max_out);
+    return B;
+}
+
+int ezrt_scene_medium_eval(ezrt_scene* s, int which, int n, const float* o, const float* d, const float* L, const uint32_t* seed, int32_t* flag_out,
+                           float* out, uint32_t* seed_out) {
+    if (!s || n < 0 || which < 0 || which > 2 ||
+        (n > 0 && (!o || !out || (which > 0 && (!d || !L || !seed)) || (which == 1 && (!flag_out || !seed_out)))))
+        return ezrt_set_error(EZRT_ERR_INVALID, "scene_medium_eval: bad argument");
+    if (!s->has_medium || !s->has_grid) return ezrt_set_error(EZRT_ERR_INVALID, "scene_medium_eval: needs a medium and a grid");
+    if (!ez_finite(s->medium.sigma_t * s->grid_max))
+        return ezrt_set_error(EZRT_ERR_INVALID, "scene_medium_eval: the medium's sigma_t times the grid's largest density is not finite");
+    if (n == 0) return EZRT_OK;
+    CU_CHECK(cudaSetDevice(s->device));
+    DeviceBuffer buf;
+    int rc = buf.ensure(sizeof(float) * 11 * (size_t)n + 256);   // o (3 n) | d (3 n) | L | seed | flag | out | seed_out
+    if (rc) return rc;
+    float* d_o = (float*)buf.p;
+    float* d_d = d_o + 3 * (size_t)n;
+    float* d_L = d_d + 3 * (size_t)n;
+    uint32_t* d_seed = (uint32_t*)(d_L + n);
+    int32_t* d_flag = (int32_t*)(d_seed + n);
+    float* d_out = (float*)(d_flag + n);
+    uint32_t* d_seed_out = (uint32_t*)(d_out + n);
+    cudaError_t e = cudaMemcpy(d_o, o, sizeof(float) * 3 * (size_t)n, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess && which > 0) e = cudaMemcpy(d_d, d, sizeof(float) * 3 * (size_t)n, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess && which > 0) e = cudaMemcpy(d_L, L, sizeof(float) * (size_t)n, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess && which > 0) e = cudaMemcpy(d_seed, seed, sizeof(uint32_t) * (size_t)n, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) {
+        launch_medium_eval(s->medium, s->grid, which, n, d_o, d_d, d_L, d_seed, d_flag, d_out, d_seed_out, 0);
+        e = cudaGetLastError();
+    }
+    if (e == cudaSuccess) e = cudaMemcpy(out, d_out, sizeof(float) * (size_t)n, cudaMemcpyDeviceToHost);
+    if (e == cudaSuccess && which == 1) e = cudaMemcpy(flag_out, d_flag, sizeof(int32_t) * (size_t)n, cudaMemcpyDeviceToHost);
+    if (e == cudaSuccess && which == 1) e = cudaMemcpy(seed_out, d_seed_out, sizeof(uint32_t) * (size_t)n, cudaMemcpyDeviceToHost);
+    buf.release();
+    if (e != cudaSuccess) return ezrt_set_error(EZRT_ERR_CUDA, "scene_medium_eval: %s", cudaGetErrorString(e));
+    return EZRT_OK;
+}
+
 int ezrt_scene_set_textures(ezrt_scene* s, int n_textures, const ezrt_texture* textures, const float* texcoords, const int32_t* texture_id) {
     if (!s) return ezrt_set_error(EZRT_ERR_INVALID, "scene_set_textures: null scene");
     CU_CHECK(cudaSetDevice(s->device));
@@ -1417,6 +1528,7 @@ int ezrt_scene_destroy(ezrt_scene* s) {
     s->lights_buf.release(); s->env_buf.release(); s->tex_buf.release(); s->tex_rec_buf.release(); s->punct_buf.release();
     s->emit_buf.release(); s->emit_lights_buf.release();
     s->ltree[0].buf.release(); s->ltree[1].buf.release();
+    s->grid_buf.release();
     if (s->own_stream) cudaStreamDestroy(s->own_stream);
     if (s->copy_stream) cudaStreamDestroy(s->copy_stream);
     if (s->side_stream) cudaStreamDestroy(s->side_stream);
@@ -1464,6 +1576,11 @@ static int light_options(ezrt_scene* s, const ezrt_render_params* p, cudaStream_
     if ((p->reserved[0] & EZRT_PARAM_MEDIUM) && s->medium.sigma_t > 0.0f) {
         o.med = s->medium;
         o.medium_on = true;
+        // EZRT_PARAM_MEDIUM_GRID (validated: a grid is set): the grid's kernels, also for a zero grid (they draw what mode 4's draw)
+        if (p->reserved[0] & EZRT_PARAM_MEDIUM_GRID) {
+            o.grid = s->grid;
+            o.grid_on = true;
+        }
     }
     // EZRT_PARAM_TEXTURES (validated: textures are set); tex.sh_base is carved with the shadow queue
     if (p->reserved[0] & EZRT_PARAM_TEXTURES) {
@@ -1737,7 +1854,7 @@ static int render_device_impl(ezrt_scene* s, const ezrt_render_params* p, float*
                 }
                 s->span_end(sp, st);
                 sp = s->span_begin(1, st);   // shading work: counted with k_shade
-                launch_nee(s->dev, rd, sq, &s_count[b], Lo, n_slots, s->n_sms, st, lopt);
+                launch_nee(s->dev, rd, sq, &s_count[b], Lo, n_slots, s->n_sms, st, lopt, d_tiles, b, batch_first);
                 s->span_end(sp, st);
                 s->launches += 2;
             }

@@ -2228,14 +2228,16 @@ __device__ __forceinline__ bool medium_step(const SceneDev& sc, const RenderDev&
 // LTREE (light sampling mode with EZRT_PARAM_LIGHT_TREE, ezrt_math.h, DESIGN.md section 19): the triangle light sample's light is
 // chosen by the descent of the tree over `lights` from the shading point (ltree_descend), and its pdf and the MIS pdf of a BSDF sample
 // that hits a light of the table are ez_ltree_pdf with P_sel recomputed from the path's previous vertex p.o (ltree_hit_pdf).
+// GRID (with MEDIUM; EZRT_PARAM_MEDIUM_GRID, ezrt_math.h, DESIGN.md section 20): the free flight is delta tracking through the density
+// grid `grid` (ez_grid_flight) in place of the homogeneous medium's analytic flight; the medium vertex is the same.
 template <int MODE, bool DEFER_NEE = false, bool AOV = false, bool ENV = false, bool TRANS = false, bool MEDIUM = false, bool TEX = false,
-          bool MAPS = false, bool PUNCT = false, bool EMAP = false, bool LTREE = false>
+          bool MAPS = false, bool PUNCT = false, bool EMAP = false, bool LTREE = false, bool GRID = false>
 __device__ __forceinline__ bool shade_step(const SceneDev& sc, const RenderDev& rd, int bounce, PathRegs& p, float hit_t,
                                            int hit_tri, uint32_t px, uint32_t py, float2 sob, vec3& Lo, vec3& Le,
                                            bool& primary_miss, ShadowRay& sh, float4* aov_rec = nullptr, LightsDev lights = LightsDev{},
                                            EnvDev env = EnvDev{}, MediumDev med = MediumDev{}, TexDev tex = TexDev{}, vec3* sh_base = nullptr,
                                            float2* sh_rm = nullptr, MapsDev maps = MapsDev{}, PunctDev punct = PunctDev{}, EmitDev emit = EmitDev{},
-                                           vec3* sh_E = nullptr, LightTreeDev tree = LightTreeDev{}) {
+                                           vec3* sh_E = nullptr, LightTreeDev tree = LightTreeDev{}, GridDev grid = GridDev{}) {
     sh.valid = false;
     const int mode = (MODE < 0) ? rd.mode : MODE;
     const bool is_mode = (mode == EZRT_MODE_DISNEY_IS_MIS_P5);
@@ -2251,7 +2253,8 @@ __device__ __forceinline__ bool shade_step(const SceneDev& sc, const RenderDev& 
         if (bounce > 0 && p.pdf <= 0.0f) return false;   // P5/fsh:865, before the free flight's draw
         float t_s;
         const float t_end = (hit_tri < 0) ? __int_as_float(0x7f800000) : hit_t;
-        if (ez_medium_flight(&med, p.o, p.d, t_end, &p.seed, &t_s))
+        static_assert(MEDIUM || !GRID, "the density grid is rendered with the medium");
+        if (GRID ? ez_grid_flight(&med, &grid, p.o, p.d, t_end, &p.seed, &t_s) : ez_medium_flight(&med, p.o, p.d, t_end, &p.seed, &t_s))
             return medium_step<AOV, ENV, TEX, MAPS, PUNCT, EMAP, LTREE>(sc, rd, bounce, p, t_s, hit_t, hit_tri, Lo, Le, primary_miss, sh, aov_rec, lights,
                                                                         env, med, tex, maps, punct, emit, sh_E, tree);
     }

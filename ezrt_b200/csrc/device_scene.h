@@ -217,6 +217,11 @@ struct LightTreeDev {
     const int32_t* acc_light;
 };
 
+// The density grid of EZRT_PARAM_MEDIUM_GRID (ezrt_math.h, DESIGN.md section 20), set by ezrt_scene_set_medium_grid: the fp32
+// densities (x fastest) and the brick maxima, in linear memory read through __ldg.  Passed to every k_shade instantiation as its last
+// parameter, after LightTreeDev, and to the grid instantiations of k_nee (<.., GRID>); read by the grid instantiations only.
+typedef ez_grid GridDev;
+
 // A shadow ray and what k_nee needs to evaluate the light sample's contribution once the ray got through (nee_contrib):
 // the BRDF / environment evaluation of the light sample is done after the shadow pass, for unoccluded rays only.
 #define EZRT_SHADOW_SLOT_BYTES (5 * 16 + 1)

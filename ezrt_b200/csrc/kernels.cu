@@ -75,7 +75,11 @@ __device__ __forceinline__ uint32_t block_append(bool valid, uint32_t* counter, 
     return pos;
 }
 
-#ifndef EZRT_KERNELS_LTREE   // kernels_ltree.cu compiles only the light-tree instantiations of k_shade from this file
+// kernels_ltree.cu, kernels_grid.cu and kernels_grid_ltree.cu compile only their instantiations of k_shade (and k_nee) from this file
+#if defined(EZRT_KERNELS_LTREE) || defined(EZRT_KERNELS_GRID)
+#define EZRT_KERNELS_PART
+#endif
+#ifndef EZRT_KERNELS_PART
 // ------------------------------------------------------------------------------------------
 // LENS (EZRT_PARAM_THIN_LENS): the thin-lens camera rays of `lens`, written to the same records; every policy traces them from
 // the queue at bounce 0
@@ -560,15 +564,16 @@ __global__ void __launch_bounds__(EZRT_EXTEND_MAX_THREADS, EZRT_EXTEND_LB_BLOCKS
 // sample's slot also gets its E(Q) in emit.sh_emit[spos].
 // LTREE (EZRT_PARAM_LIGHT_TREE): the triangle light samples choose their light by the light tree `tree` over `lights`, and the
 // MIS weights of emission hits use its P_sel (shade_step).
+// GRID (with MEDIUM; EZRT_PARAM_MEDIUM_GRID): the free flight tracks the density grid `grid` (shade_step).
 template <int MODE, bool LIST, bool AOV = false, bool ENV = false, bool TRANS = false, bool MEDIUM = false, bool TEX = false,
-          bool MAPS = false, bool PUNCT = false, bool EMAP = false, bool LTREE = false>
+          bool MAPS = false, bool PUNCT = false, bool EMAP = false, bool LTREE = false, bool GRID = false>
 __global__ void __launch_bounds__(128, EZRT_SHADE_MIN_BLOCKS) k_shade(SceneDev sc, RenderDev rd, const TileDev* __restrict__ tiles, int bounce,
                                                uint32_t batch_first_frame, PathQueue qin, const uint32_t* __restrict__ in_count,
                                                PathQueue qout, uint32_t* out_count, ShadowQueue sq, uint32_t* s_count,
                                                float4* __restrict__ Lo, float4* __restrict__ Le, uint32_t n_fused, uint32_t n_frames,
                                                const uint32_t* __restrict__ list, const float2* __restrict__ side_hit,
                                                float4* __restrict__ aov_rec, LightsDev lights, EnvDev env, MediumDev med, TexDev tex,
-                                               MapsDev maps, PunctDev punct, EmitDev emit, LightTreeDev tree) {
+                                               MapsDev maps, PunctDev punct, EmitDev emit, LightTreeDev tree, GridDev grid) {
     // The Sobol pair of (bounce, frame) is the same for every pixel of a frame (P5/fsh:361-376: up to 2 x 32 table XORs per path): each
     // block computes the pairs of the batch's frames once into shared memory (batches of more than EZRT_SOBOL_TABLE frames compute per path).
     __shared__ float2 s_sobol[EZRT_SOBOL_TABLE];
@@ -695,9 +700,9 @@ __global__ void __launch_bounds__(128, EZRT_SHADE_MIN_BLOCKS) k_shade(SceneDev s
             }
 #endif
             if (LIST || __float_as_int(hit.y) != EZRT_TRI_PENDING) {   // pending: deferred by the accel kernel, shaded by the LIST pass
-                alive = shade_step<MODE, MODE == EZRT_MODE_DISNEY_IS_MIS_P5, AOV, ENV, TRANS, MEDIUM, TEX, MAPS, PUNCT, EMAP, LTREE>(sc, rd, bounce, p, hit.x, __float_as_int(hit.y), px, py,
+                alive = shade_step<MODE, MODE == EZRT_MODE_DISNEY_IS_MIS_P5, AOV, ENV, TRANS, MEDIUM, TEX, MAPS, PUNCT, EMAP, LTREE, GRID>(sc, rd, bounce, p, hit.x, __float_as_int(hit.y), px, py,
                                                                                                           sob, lo, le, pmiss, sh, AOV ? aov_rec + 2 * (size_t)slot : nullptr,
-                                                                                                          lights, env, med, tex, &sh_base, &sh_rm, maps, punct, emit, &sh_E, tree);
+                                                                                                          lights, env, med, tex, &sh_base, &sh_rm, maps, punct, emit, &sh_E, tree, grid);
                 if (bounce == 0) {
                     // Le is zero for every surface that does not emit: it is stored (and read back by k_blend) only otherwise.
                     // color = Le + Lo with Le = +-0 is Lo bit for bit, because Lo is never -0.0 (it starts at +0.0 and only grows by additions)
@@ -757,12 +762,16 @@ __global__ void __launch_bounds__(128, EZRT_SHADE_MIN_BLOCKS) k_shade(SceneDev s
 // PUNCT: and the punctual samples (hist.w = -2 - j): ez_punct_contrib of the shading point's f (the BSDF or mixture at a surface, the
 // phase function at a medium vertex) with light j's intensity * color and the scale in view.w, without a MIS weight.
 // EMAP: a triangle light sample's emission is the E(Q) k_shade left in emit.sh_emit[j].
+// GRID (with MEDIUM): the transmittance is ratio tracking through the density grid `grid` (ez_grid_transmittance), its draws from the
+// shadow stream of the sample's pixel and frame (from its slot, tiles and batch_first_frame) and bounce.
 template <int MODE, bool ENV = false, bool TRANS = false, bool MEDIUM = false, bool TEX = false, bool MAPS = false, bool PUNCT = false,
-          bool EMAP = false>
+          bool EMAP = false, bool GRID = false>
 __global__ void __launch_bounds__(128, 8) k_nee(SceneDev sc, RenderDev rd, ShadowQueue sq, const uint32_t* __restrict__ s_count, float4* __restrict__ Lo,
-                                                MediumDev med, TexDev tex, MapsDev maps, PunctDev punct, EmitDev emit) {
+                                                MediumDev med, TexDev tex, MapsDev maps, PunctDev punct, EmitDev emit, GridDev grid,
+                                                const TileDev* __restrict__ tiles, int bounce, uint32_t batch_first_frame) {
     static_assert(MODE == EZRT_MODE_DISNEY_LIGHTS || !(ENV || TRANS || MEDIUM), "the options exist in the light sampling mode");
     static_assert(!(TRANS && MEDIUM), "the medium is rendered without transmission");
+    static_assert(MEDIUM || !GRID, "the density grid is rendered with the medium");
     __shared__ uint32_t s_scan[34];
     __shared__ uint32_t s_total;
     __shared__ uint32_t s_list[512];
@@ -797,6 +806,16 @@ __global__ void __launch_bounds__(128, 8) k_nee(SceneDev sc, RenderDev rd, Shado
                 return m;
             };
             const vec3 V = ez_v3(v4.x, v4.y, v4.z), N = ez_v3(n4.x, n4.y, n4.z), Ld = ez_v3(d4.x, d4.y, d4.z), hist = ez_v3(h4.x, h4.y, h4.z);
+            const auto transmittance = [&](float L) {
+                if constexpr (GRID) {
+                    uint32_t px, py, fib;
+                    slot_pixel(rd, tiles, slot, px, py, fib);
+                    uint32_t seed = ez_grid_shadow_seed(px, py, batch_first_frame + fib, (uint32_t)bounce);
+                    return ez_grid_transmittance(&med, &grid, ez_v3(o4.x, o4.y, o4.z), Ld, L, &seed);
+                } else {
+                    return ez_medium_transmittance(&med, ez_v3(o4.x, o4.y, o4.z), Ld, L);
+                }
+            };
             vec3 c;
             if constexpr (MODE == EZRT_MODE_DISNEY_LIGHTS) {
                 const int lm = __float_as_int(h4.w);   // the light's material; -1: an environment sample; PUNCT: <= -2 a punctual one
@@ -826,12 +845,12 @@ __global__ void __launch_bounds__(128, 8) k_nee(SceneDev sc, RenderDev rd, Shado
                     }
                     c = ez_punct_contrib(hist, f, cosine, f4xyz(ldg4(r + 2)), v4.w);
                     if constexpr (MEDIUM)
-                        c = ez_scale(c, ez_medium_transmittance(&med, ez_v3(o4.x, o4.y, o4.z), Ld, ez_medium_light_dist(n4.w, ldg4(r).w == 2.0f)));
+                        c = ez_scale(c, transmittance(ez_medium_light_dist(n4.w, ldg4(r).w == 2.0f)));
                 } else if constexpr (MEDIUM) {   // a medium vertex loads no material
                     const vec3 E = light_color();
                     if (m_raw == EZRT_MEDIUM_VERTEX) c = nee_medium_contrib(V, Ld, med.g, hist, E, v4.w);
                     else c = nee_light_contrib(V, N, Ld, material(m_raw), hist, E, v4.w);
-                    c = ez_scale(c, ez_medium_transmittance(&med, ez_v3(o4.x, o4.y, o4.z), Ld, ez_medium_light_dist(n4.w, ENV && lm < 0)));
+                    c = ez_scale(c, transmittance(ez_medium_light_dist(n4.w, ENV && lm < 0)));
                 } else {
                     const int m_id = (TRANS && m_raw < 0) ? ~m_raw : m_raw;
                     const MaterialDev mat = material(m_id);
@@ -848,7 +867,9 @@ __global__ void __launch_bounds__(128, 8) k_nee(SceneDev sc, RenderDev rd, Shado
         __syncthreads();
     }
 }
+#endif  // EZRT_KERNELS_LTREE
 
+#ifndef EZRT_KERNELS_PART
 // ------------------------------------------------------------------------------------------
 // blend: color = Le + Li (or the sky for a primary miss), running mean in frame order
 // ------------------------------------------------------------------------------------------
@@ -1266,7 +1287,7 @@ template <class F, class... B> static void with_bools(F&& f, bool b, B... rest) 
     else with_bools([&](auto... t) { f(std::false_type{}, t...); }, rest...);
 }
 
-#ifndef EZRT_KERNELS_LTREE
+#ifndef EZRT_KERNELS_PART
 
 // persistent extend/shadow kernels: block size and resident blocks per SM (each block stages its own
 // copy of the top tree levels in shared memory); env EZRT_EXTEND_THREADS / EZRT_EXTEND_BPS override
@@ -1427,9 +1448,14 @@ static void launch_shade_t(int blocks, const SceneDev& sc, const RenderDev& rd, 
             if constexpr ((M == EZRT_MODE_DISNEY_LIGHTS || !(E || T || X || TX || P)) && !(T && X) && (TX || !MP) && (TX || !EM))
                 k_shade<M, LIST, A, E, T, X, TX, MP, P, EM><<<blocks, 128, 0, st>>>(sc, rd, tiles, bounce, batch_first_frame, qin, in_count, qout, out_count, sq,
                                                                                     s_count, Lo, Le, n_fused, n_frames, list, side_hit, aov_rec, o.lights, o.env,
-                                                                                    o.med, o.tex, o.maps, o.punct, o.emit, o.tree);
+                                                                                    o.med, o.tex, o.maps, o.punct, o.emit, o.tree, o.grid);
         }, aov_rec != nullptr, o.env_on, o.trans_on, o.medium_on, o.tex_on, o.maps_on, o.punct_on, o.emap_on);
     };
+    if (o.grid_on) {   // the grid instantiations (with the medium) are kernels_grid.cu's and kernels_grid_ltree.cu's
+        (o.tree_on ? launch_shade_grid_ltree : launch_shade_grid)(LIST, blocks, sc, rd, tiles, bounce, batch_first_frame, qin, in_count, qout, out_count, sq,
+                                                                  s_count, Lo, Le, n_fused, n_frames, list, side_hit, aov_rec, o, st);
+        return;
+    }
     if (o.tree_on) {   // the light-tree instantiations (light sampling mode only) are kernels_ltree.cu's
         launch_shade_ltree(LIST, blocks, sc, rd, tiles, bounce, batch_first_frame, qin, in_count, qout, out_count, sq, s_count, Lo, Le, n_fused, n_frames,
                            list, side_hit, aov_rec, o, st);
@@ -1463,13 +1489,18 @@ void launch_deferred_lane(const SceneDev& sc, const RenderDev& rd, const TileDev
                          defer_list, side_hit, aov_rec, o, st);
 }
 void launch_nee(const SceneDev& sc, const RenderDev& rd, ShadowQueue sq, const uint32_t* s_count, float4* Lo, uint32_t n_max, int n_sms, cudaStream_t st,
-                const LightOptions& o) {
+                const LightOptions& o, const TileDev* tiles, int bounce, uint32_t batch_first_frame) {
     const int blocks = std::max(1, std::min(div_up(n_max, 512), n_sms * 8));
+    if (o.grid_on) {   // kernels_grid.cu's
+        launch_nee_grid(blocks, sc, rd, sq, s_count, Lo, o, tiles, bounce, batch_first_frame, st);
+        return;
+    }
     with_bools([&](auto L, auto E, auto T, auto X, auto TX, auto MP, auto P, auto EM) {
         // the options exist in the light sampling mode (the other mode here is mode 3); the maps with the textures
         if constexpr ((L || !(E || T || X || TX || P)) && !(T && X) && (TX || !MP) && (TX || !EM))
             k_nee<L ? EZRT_MODE_DISNEY_LIGHTS : EZRT_MODE_DISNEY_IS_MIS_P5, E, T, X, TX, MP, P, EM><<<blocks, 128, 0, st>>>(sc, rd, sq, s_count, Lo, o.med, o.tex,
-                                                                                                                        o.maps, o.punct, o.emit);
+                                                                                                                        o.maps, o.punct, o.emit, o.grid,
+                                                                                                                        tiles, bounce, batch_first_frame);
     }, rd.mode == EZRT_MODE_DISNEY_LIGHTS, o.env_on, o.trans_on, o.medium_on, o.tex_on, o.maps_on, o.punct_on, o.emap_on);
 }
 
@@ -1751,4 +1782,4 @@ void launch_denoise(const float* color, int channels, const float* aov, const fl
     }
 }
 
-#endif  // EZRT_KERNELS_LTREE
+#endif  // EZRT_KERNELS_PART

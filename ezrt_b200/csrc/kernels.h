@@ -26,6 +26,7 @@
 //   punct_on  EZRT_PARAM_PUNCTUAL_LIGHTS and the scene's punctual table has J > 0 lights: punct (<.., PUNCT>)
 //   emap_on   EZRT_PARAM_EMISSION_MAPS (with tex_on): the emission maps emit, and lights is the emission table (<.., TEX, .., EMAP>)
 //   tree_on   EZRT_PARAM_LIGHT_TREE and the render's table has K > 0 lights: the tree over lights, tree (k_shade<.., LTREE>)
+//   grid_on   EZRT_PARAM_MEDIUM_GRID with medium_on: the density grid (k_shade<.., MEDIUM, .., GRID>, k_nee<.., MEDIUM, .., GRID>)
 // All off outside the light sampling mode; the tables are zero where unused, as the kernels' parameters.
 struct LightOptions {
     LightsDev lights{};   // the light table (light sampling mode)
@@ -36,7 +37,9 @@ struct LightOptions {
     PunctDev punct{};     // the punctual lights' table and P_p (punct_on)
     EmitDev emit{};       // the emission maps' records and the shadow slots' E(Q) (emap_on)
     LightTreeDev tree{};  // the light tree over lights (tree_on)
-    bool env_on = false, trans_on = false, medium_on = false, tex_on = false, maps_on = false, punct_on = false, emap_on = false, tree_on = false;
+    GridDev grid{};       // the medium's density grid (grid_on)
+    bool env_on = false, trans_on = false, medium_on = false, tex_on = false, maps_on = false, punct_on = false, emap_on = false, tree_on = false,
+         grid_on = false;
 };
 
 // lens (EZRT_PARAM_THIN_LENS): the thin-lens camera rays (k_generate<true>); null: the pinhole's
@@ -76,9 +79,10 @@ void launch_deferred_lane(const SceneDev& sc, const RenderDev& rd, const TileDev
                           const uint32_t* defer_list, const uint32_t* defer_count, uint32_t* defer_work, float2* side_hit, PathQueue qout,
                           uint32_t* out_count, ShadowQueue sq, uint32_t* s_count, float4* Lo, float4* Le, uint32_t n_fused, uint32_t n_frames,
                           int n_sms, cudaStream_t st, float4* aov_rec, const LightOptions& o);
-// after a shadow pass (accel or exact, including the exact pass over deferred shadow rays): contributions of the unoccluded light samples
+// after a shadow pass (accel or exact, including the exact pass over deferred shadow rays): contributions of the unoccluded light samples.
+// tiles, bounce, batch_first_frame: the shadow rays' bounce and batch, which key the grid renders' shadow streams (o.grid_on)
 void launch_nee(const SceneDev& sc, const RenderDev& rd, ShadowQueue sq, const uint32_t* s_count, float4* Lo, uint32_t n_max, int n_sms, cudaStream_t st,
-                const LightOptions& o);
+                const LightOptions& o, const TileDev* tiles = nullptr, int bounce = 0, uint32_t batch_first_frame = 0);
 // light table of the light sampling mode: every triangle's weight (w: n_triangles floats) -> the lights in triangle order
 // (idx_out, w_out: n floats each; *count = K) -> their 64-byte records (rec: 4 K float4)
 void launch_light_weights(const SceneDev& sc, float* w, cudaStream_t st);
@@ -137,6 +141,22 @@ void launch_shade_ltree(bool list, int blocks, const SceneDev& sc, const RenderD
                         PathQueue qin, const uint32_t* in_count, PathQueue qout, uint32_t* out_count, ShadowQueue sq, uint32_t* s_count, float4* Lo,
                         float4* Le, uint32_t n_fused, uint32_t n_frames, const uint32_t* list_idx, const float2* side_hit, float4* aov_rec,
                         const LightOptions& o, cudaStream_t st);
+// launch_shade's and launch_nee's density-grid renders (o.grid_on): k_shade<.., MEDIUM, .., LTREE, GRID = true> and k_nee<.., GRID = true>,
+// compiled in kernels_grid.cu (LTREE false, and k_nee) and kernels_grid_ltree.cu (LTREE true)
+void launch_shade_grid(bool list, int blocks, const SceneDev& sc, const RenderDev& rd, const TileDev* tiles, int bounce, uint32_t batch_first_frame,
+                       PathQueue qin, const uint32_t* in_count, PathQueue qout, uint32_t* out_count, ShadowQueue sq, uint32_t* s_count, float4* Lo,
+                       float4* Le, uint32_t n_fused, uint32_t n_frames, const uint32_t* list_idx, const float2* side_hit, float4* aov_rec,
+                       const LightOptions& o, cudaStream_t st);
+void launch_shade_grid_ltree(bool list, int blocks, const SceneDev& sc, const RenderDev& rd, const TileDev* tiles, int bounce, uint32_t batch_first_frame,
+                             PathQueue qin, const uint32_t* in_count, PathQueue qout, uint32_t* out_count, ShadowQueue sq, uint32_t* s_count, float4* Lo,
+                             float4* Le, uint32_t n_fused, uint32_t n_frames, const uint32_t* list_idx, const float2* side_hit, float4* aov_rec,
+                             const LightOptions& o, cudaStream_t st);
+void launch_nee_grid(int blocks, const SceneDev& sc, const RenderDev& rd, ShadowQueue sq, const uint32_t* s_count, float4* Lo, const LightOptions& o,
+                     const TileDev* tiles, int bounce, uint32_t batch_first_frame, cudaStream_t st);
+// ezrt_scene_medium_eval on the device's code (n inputs): which 0, sigma at points o (3 floats each) -> out0; which 1, the free flight
+// of (o, d, t_end = L, seed) -> flag (out_i), t_s (out0), the advanced seed (seed_out); which 2, the ratio-tracked T of (o, d, L, seed) -> out0
+void launch_medium_eval(const MediumDev& med, const GridDev& grid, int which, int n, const float* o, const float* d, const float* L,
+                        const uint32_t* seed, int32_t* out_i, float* out0, uint32_t* seed_out, cudaStream_t st);
 // ezrt_scene_light_tree_eval: which 0, the descent (P, r) -> (light, P_sel); which 1, the hit side (P, light) -> P_sel (n inputs)
 void launch_ltree_eval(const LightTreeDev& tree, int which, int n, const float* P, const float* r, const int32_t* light_in, int32_t* light_out,
                        float* p_out, cudaStream_t st);

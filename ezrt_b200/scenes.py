@@ -556,3 +556,46 @@ def s_screen(bunny=True, builder=api.BVH_SAH_FAST, emission=(6.0, 6.0, 6.0)):
     tris, nodes, uv, ids, eid = _emission_mapped(tl, 0, builder)
     eye, cam = api.camera_orbit(0.0, 15.0, 4.0)
     return tris, nodes, eye, cam, [screen_image()], uv, ids, eid
+
+
+def smoke_grid(n=64, seed=0):
+    """A seeded procedural plume for EZRT_PARAM_MEDIUM_GRID: float32 [n, n, n] densities ([z, y, x]) in [0, 1], deterministic in
+    numpy.  Four octaves of value noise (seeded lattices of 4, 8, 16 and 32 cells, trilinearly upsampled; weights 1/2, 1/4, ...) shape a
+    column that narrows and thins with height (y) and is empty near the grid's faces."""
+    rng = np.random.default_rng(seed)
+    t = np.linspace(0.0, 1.0, n)
+    noise = np.zeros((n, n, n))
+    for octave, cells in enumerate((4, 8, 16, 32)):
+        lat = rng.random((cells + 1,) * 3)
+        u = t * cells
+        i = np.minimum(u.astype(np.int64), cells - 1)
+        f = u - i
+        acc = np.zeros((n, n, n))
+        for dz in (0, 1):
+            for dy in (0, 1):
+                for dx in (0, 1):
+                    w = (f if dz else 1 - f)[:, None, None] * (f if dy else 1 - f)[None, :, None] * (f if dx else 1 - f)[None, None, :]
+                    acc += w * lat[np.ix_(i + dz, i + dy, i + dx)]
+        noise += acc * 0.5 ** (octave + 1)
+    z, y, x = np.meshgrid(t, t, t, indexing="ij")
+    radius = 0.35 - 0.2 * y
+    r2 = (x - 0.5) ** 2 + (z - 0.5) ** 2
+    shape = np.clip(1.0 - r2 / radius ** 2, 0.0, None) * np.clip(1.0 - y, 0.0, None)
+    return np.clip(shape * (2.0 * noise - 0.3), 0.0, None).astype(np.float32)
+
+
+def s_p3_bunny_smoke(n=64, seed=0, sigma_t=6.0, builder=api.BVH_SAH_FAST):
+    """s_p3_bunny with a smoke plume over the bunny: (tris, nodes, eye, cam, medium, grid), medium the keyword arguments of
+    Scene.set_medium (its box holds the plume) and grid smoke_grid(n, seed)."""
+    tris, nodes, eye, cam = s_p3_bunny(builder)
+    medium = dict(sigma_t=sigma_t, albedo=(0.9, 0.9, 0.9), g=0.3, box_min=(-1.0, -1.0, -1.0), box_max=(1.0, 1.2, 1.0))
+    return tris, nodes, eye, cam, medium, smoke_grid(n, seed)
+
+
+def s_1m_smoke(n=128, seed=0, sigma_t=1.0, builder=api.BVH_SAH_FAST):
+    """S-1M (s_1m) with a plume over its bounds: (tris, nodes, eye, cam, medium, grid) as s_p3_bunny_smoke."""
+    tris, nodes, eye, cam = s_1m(builder)
+    v = np.asarray(tris, np.float32).reshape(-1, 36)[:, :9].reshape(-1, 3)
+    lo, hi = v.min(0), v.max(0)
+    medium = dict(sigma_t=sigma_t, albedo=(0.9, 0.9, 0.9), g=0.3, box_min=tuple(lo), box_max=tuple(hi))
+    return tris, nodes, eye, cam, medium, smoke_grid(n, seed)

@@ -206,6 +206,16 @@ typedef struct ezrt_render_params {
    megakernel.  Accepted by ezrt_render[_device], ezrt_render_adaptive[_device] and ezrt_render_aov[_device]; the shadow slots keep
    their sizes. */
 #define EZRT_PARAM_LIGHT_TREE 512
+/* ezrt_render_params.reserved[0], with EZRT_PARAM_MEDIUM (so EZRT_MODE_DISNEY_LIGHTS on the wavefront pipeline), with or without every
+   other flag of that mode: the medium is heterogeneous, sigma(x) = sigma_t * rho(x) with rho the scene's density grid
+   (ezrt_scene_set_medium_grid) filling the medium's box, trilinear between lattice points (ezrt_math.h, DESIGN.md section 20).  Free
+   flight is delta tracking against per-brick majorants (8 x 8 x 8 cells), with draws from the path's stream; the transmittance of a lit
+   light sample is ratio tracking with Russian roulette, its draws from a stream of its own keyed on the sample's pixel, frame and
+   bounce, so the shadow slots keep their sizes.  Albedo, g and the medium vertex are EZRT_PARAM_MEDIUM's.  A zero grid renders mode 4's
+   image draw for draw; without the flag a grid set on the scene is ignored.  Invalid (EZRT_ERR_INVALID) without EZRT_PARAM_MEDIUM,
+   without a grid set, or when sigma_t times the grid's largest density is not finite.  Accepted by ezrt_render[_device],
+   ezrt_render_adaptive[_device] and ezrt_render_aov[_device]. */
+#define EZRT_PARAM_MEDIUM_GRID 1024
 
 /* One punctual light of ezrt_scene_set_punctual_lights (glTF's KHR_lights_punctual, in the render's units: no photometric
    conversion; the caller scales glTF's candela and lux) */
@@ -280,6 +290,22 @@ int ezrt_scene_destroy(ezrt_scene* scene);
  * box corner, box_min > box_max on an axis, or reserved != 0.  The medium travels to the kernels by value when a render is
  * enqueued: changing it afterwards does not affect renders already enqueued. */
 int ezrt_scene_set_medium(ezrt_scene* scene, const ezrt_medium* medium);
+/* Sets the density grid of EZRT_PARAM_MEDIUM_GRID (a copy of the nx * ny * nz densities, x fastest, then y, then z), or clears it
+ * (density NULL), and computes its brick maxima.  The grid fills the box of whatever medium is set; ezrt_scene_set_medium keeps it.
+ * Waits for the renders already enqueued on the scene's device.  Returns EZRT_ERR_INVALID, and keeps the previous grid, for a side
+ * outside [1, 1024], a negative or non-finite density, or (with a medium set) sigma_t times the largest density not finite;
+ * EZRT_ERR_NOMEM / EZRT_ERR_CUDA when the copy cannot be made (the previous grid is kept then too). */
+int ezrt_scene_set_medium_grid(ezrt_scene* scene, int nx, int ny, int nz, const float* density);
+/* The grid's brick count B, or a negative status (EZRT_ERR_INVALID without a grid); writes dims_out[6] = (nx, ny, nz, bricks along
+ * x, y, z) and min(B, cap) brick maxima (x fastest) to brick_max_out (either may be NULL). */
+int ezrt_scene_medium_grid(ezrt_scene* scene, int cap, int32_t* dims_out, float* brick_max_out);
+/* The device's grid code on n inputs (host arrays; synchronous), over the scene's medium and grid: which 0, sigma at the points o
+ * (3 floats each) -> out; which 1, the free flight of the segments (o, d, t_end = L[i]) from seed[i] -> flag_out (1: scatters), out
+ * (t_s, valid where flag_out is 1) and seed_out (the advanced seed); which 2, the ratio-tracked transmittance of (o, d, L[i]) with
+ * draws from seed[i] -> out.  EZRT_ERR_INVALID without a medium and a grid, when sigma_t times the grid's largest density is not
+ * finite (as for a render), or for another which. */
+int ezrt_scene_medium_eval(ezrt_scene* scene, int which, int n, const float* o, const float* d, const float* L, const uint32_t* seed,
+                           int32_t* flag_out, float* out, uint32_t* seed_out);
 /* Sets the scene's base-colour textures (EZRT_PARAM_TEXTURES): n_textures textures (copied), and per triangle, in the order of the
  * `tris` array given to ezrt_scene_create, 6 floats of texcoords (u1, v1, u2, v2, u3, v3: OBJ's convention, v = 0 at the image's
  * bottom) and a texture id in [-1, n_textures) (-1: the material's base colour).  textures NULL clears them.  Returns

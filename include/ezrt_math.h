@@ -762,6 +762,219 @@ EZ_HD ez_vec3 ez_hg_sample(ez_vec3 d, float g, float h_1, float h_2) {
     return ez_to_normal_hemisphere(ez_v3(s * ez_cos(phi), s * ez_sin(phi), c), d);
 }
 
+/* ------------------------------------------------------------------ heterogeneous medium (EZRT_PARAM_MEDIUM_GRID, DESIGN.md section 20)
+ * A density grid rho of nx x ny x nz finite values >= 0 (x fastest) fills the medium's box: lattice point (i, j, k) sits at
+ * bmin + (i / (nx - 1), j / (ny - 1), k / (nz - 1)) (bmax - bmin); an axis with n = 1 is constant.  sigma(x) = sigma_t rho(x).
+ * Lookup (ez_grid_rho): per axis the lattice coordinate u = ((x - bmin) / (bmax - bmin)) (n - 1) (0 for n = 1), clamped to the
+ *   brick's range below, cell c = min((int)u, n - 2) (0 for n = 1), f = u - c; trilinear over the cell's 8 corners, lerps along x,
+ *   then y, then z, each ez_grid_lerp(a, b, f) = clamp(a + f (b - a), min(a, b), max(a, b)): rho never exceeds its largest corner.
+ * Bricks: 8 x 8 x 8 lattice cells, B_a = max(1, ceil((n_a - 1) / 8)) per axis.  Brick b's maximum (ez_grid_brick_max) is over the
+ *   lattice points 8 b - 1 .. 8 b + 9 of every axis (clamped to [0, n - 1]): its cells dilated by one point.  Its majorant is
+ *   m = sigma_t * max.  A lookup made for brick b clamps u to [8 b - 1, 8 b + 9] (within [0, n - 1]), so its corners are points
+ *   of the dilated range and sigma <= m holds by construction; the clamp changes u only where rounding puts the point more than
+ *   one lattice cell outside the brick the walk is in.
+ * Walk (ez_grid_walk_*): over the overlap [t0, t1] = ez_box_overlap(o, d, bmin, bmax, t_end).  The first brick holds the point
+ *   o + t0 d (its clamped u over 8, at most B - 1); axis a's next boundary is the plane at lattice coordinate 8 (b_a + 1) (d_a > 0)
+ *   or 8 b_a (d_a < 0), x = bmin_a + (bmax_a - bmin_a) ((float)c / (n_a - 1)), at t = (x - o_a) / d_a (none if d_a == 0 or the
+ *   brick is the axis' last / first).  The interval is [ta, tb], tb = min(t1, the axes' next t), ta = the previous tb (t0 first);
+ *   the walk steps the axis of smallest next t (the first on ties) and ends at t1 or when no boundary remains.  Every brick
+ *   interval is visited once, so the walk ends after at most B_x + B_y + B_z intervals.
+ * Tracking in an interval with m > 0, from t = ta: t = ez_grid_advance(t, ez_free_flight(r, m)) for the next draw r (advance:
+ *   t + s, or the next float above t when t + s rounds to t, so every step moves); t >= tb: the next interval.
+ * Free flight (ez_grid_flight, draws from the path's seed): a tentative collision draws r2; real iff r2 m < sigma(o + t d): the
+ *   path scatters at t_s = t.  A brick with m = 0 draws nothing, so a zero grid draws nothing at all (mode 4's image draw for draw).
+ * Transmittance (ez_grid_transmittance, draws from the shadow stream ez_grid_shadow_seed): ratio tracking over [0, L], T *=
+ *   (m - sigma) / m at each tentative collision; T == 0 ends it; once T < 1/16, Russian roulette with one draw: r < 1/4 keeps
+ *   it as T * 4 (exact), else T = 0.  E[T] = exp(-tau) and T lies in [0, 1]. */
+#define EZRT_GRID_BRICK 8
+#define EZRT_GRID_SALT 0x47524944u   /* "GRID" */
+struct ez_grid {
+    const float* rho;     /* nx * ny * nz densities, x fastest */
+    const float* brick;   /* bx * by * bz brick maxima, x fastest */
+    int n[3];             /* nx, ny, nz */
+    int b[3];             /* bricks per axis */
+};
+typedef struct ez_grid ez_grid;
+EZ_HD float ez_grid_load(const float* p, size_t i) {
+#if defined(__CUDA_ARCH__)
+    return __ldg(p + i);
+#else
+    return p[i];
+#endif
+}
+EZ_HD int ez_grid_bricks(int n) { return n <= 1 ? 1 : (n - 1 + EZRT_GRID_BRICK - 1) / EZRT_GRID_BRICK; }
+EZ_HD float ez_grid_lerp(float a, float b, float f) { return ez_clamp(a + f * (b - a), ez_min(a, b), ez_max(a, b)); }
+/* the shadow stream of the light sample of (pixel, frame, bounce), as the lens stream with a salt of its own */
+EZ_HD uint32_t ez_grid_shadow_seed(uint32_t px, uint32_t py, uint32_t frame, uint32_t bounce) {
+    return (((px * 1973u + py * 9277u + frame * 26699u) | 1u) ^ EZRT_GRID_SALT) + bounce * 0x9e3779b9u;
+}
+/* the maximum of brick (bi, bj, bk) over its dilated lattice points */
+EZ_HD float ez_grid_brick_max(const ez_grid* g, int bi, int bj, int bk) {
+    int lo[3], hi[3];
+    const int bb[3] = {bi, bj, bk};
+    for (int a = 0; a < 3; a++) {
+        lo[a] = EZRT_GRID_BRICK * bb[a] - 1;
+        if (lo[a] < 0) lo[a] = 0;
+        hi[a] = EZRT_GRID_BRICK * bb[a] + EZRT_GRID_BRICK + 1;
+        if (hi[a] > g->n[a] - 1) hi[a] = g->n[a] - 1;
+    }
+    float m = 0.0f;
+    for (int k = lo[2]; k <= hi[2]; k++)
+        for (int j = lo[1]; j <= hi[1]; j++)
+            for (int i = lo[0]; i <= hi[0]; i++) m = ez_max(m, g->rho[((size_t)k * g->n[1] + j) * g->n[0] + i]);
+    return m;
+}
+/* the lattice coordinate of x on axis a (unclamped; 0 for n = 1) */
+EZ_HD float ez_grid_u(const ez_grid* g, float x, float lo, float hi, int a) {
+    if (g->n[a] <= 1) return 0.0f;
+    return EZ_DIV(x - lo, hi - lo) * (float)(g->n[a] - 1);
+}
+/* u clamped to [lo, hi]; a NaN u (a box whose extent overflows) -> lo */
+EZ_HD float ez_grid_clampu(float u, float lo, float hi) { return !(u >= lo) ? lo : (u > hi ? hi : u); }
+/* rho at x for the lookup of brick bb (bb null: clamped to the lattice only); *clamped |= 1 if the brick's clamp moved u */
+EZ_HD float ez_grid_rho(const ez_grid* g, ez_vec3 bmin, ez_vec3 bmax, ez_vec3 x, const int* bb, int* clamped) {
+    const float xx[3] = {x.x, x.y, x.z}, lo[3] = {bmin.x, bmin.y, bmin.z}, hi[3] = {bmax.x, bmax.y, bmax.z};
+    int c[3], c1[3];
+    float f[3];
+    for (int a = 0; a < 3; a++) {
+        const int n = g->n[a];
+        float u = ez_grid_u(g, xx[a], lo[a], hi[a], a);
+        float ulo = 0.0f, uhi = (float)(n - 1);
+        if (bb) {
+            ulo = ez_max(ulo, (float)(EZRT_GRID_BRICK * bb[a] - 1));
+            uhi = ez_min(uhi, (float)(EZRT_GRID_BRICK * bb[a] + EZRT_GRID_BRICK + 1));
+        }
+        const float uc = ez_grid_clampu(u, ulo, uhi);
+        if (clamped && !(uc == u)) *clamped = 1;
+        if (n <= 1) {
+            c[a] = 0; c1[a] = 0; f[a] = 0.0f;
+        } else {
+            int ci = (int)uc;
+            if (ci > n - 2) ci = n - 2;
+            c[a] = ci; c1[a] = ci + 1; f[a] = uc - (float)ci;
+        }
+    }
+    const size_t nx = (size_t)g->n[0], nxy = nx * (size_t)g->n[1];
+    float e[2][2];
+    for (int dk = 0; dk < 2; dk++)
+        for (int dj = 0; dj < 2; dj++) {
+            const size_t row = (size_t)(dk ? c1[2] : c[2]) * nxy + (size_t)(dj ? c1[1] : c[1]) * nx;
+            e[dk][dj] = ez_grid_lerp(ez_grid_load(g->rho, row + c[0]), ez_grid_load(g->rho, row + c1[0]), f[0]);
+        }
+    return ez_grid_lerp(ez_grid_lerp(e[0][0], e[0][1], f[1]), ez_grid_lerp(e[1][0], e[1][1], f[1]), f[2]);
+}
+/* t + s, or the next float above t (t >= 0) when the sum rounds to t */
+EZ_HD float ez_grid_advance(float t, float s) {
+    const float u = t + s;
+    return (u > t) ? u : ez_u2f(ez_f2u(t) + 1u);
+}
+/* the brick walk's state over [t0, t1] of the ray o + t d */
+struct ez_grid_walk {
+    int b[3], step[3];
+    float tnext[3];
+    float ta, t1;
+};
+typedef struct ez_grid_walk ez_grid_walk;
+/* axis a's next boundary after brick index b (d_a != 0): its t, or +inf when there is none */
+EZ_HD float ez_grid_plane_t(const ez_grid* g, float o, float d, float lo, float hi, int a, int b) {
+    const int c = EZRT_GRID_BRICK * (d > 0.0f ? b + 1 : b);
+    if (d == 0.0f || g->n[a] <= 1 || (d > 0.0f && b + 1 >= g->b[a]) || (d < 0.0f && b <= 0)) return ez_u2f(0x7f800000u);
+    const float x = lo + (hi - lo) * EZ_DIV((float)c, (float)(g->n[a] - 1));
+    return EZ_DIV(x - o, d);
+}
+EZ_HD void ez_grid_walk_begin(const ez_grid* g, ez_vec3 o, ez_vec3 d, ez_vec3 bmin, ez_vec3 bmax, float t0, float t1, ez_grid_walk* w) {
+    const ez_vec3 p = ez_add(o, ez_scale(d, t0));
+    const float pp[3] = {p.x, p.y, p.z}, oo[3] = {o.x, o.y, o.z}, dd[3] = {d.x, d.y, d.z};
+    const float lo[3] = {bmin.x, bmin.y, bmin.z}, hi[3] = {bmax.x, bmax.y, bmax.z};
+    for (int a = 0; a < 3; a++) {
+        const float u = ez_grid_clampu(ez_grid_u(g, pp[a], lo[a], hi[a], a), 0.0f, (float)(g->n[a] - 1));
+        int b = (int)EZ_DIV(u, (float)EZRT_GRID_BRICK);
+        if (b > g->b[a] - 1) b = g->b[a] - 1;
+        w->b[a] = b;
+        w->step[a] = dd[a] > 0.0f ? 1 : -1;
+        w->tnext[a] = ez_grid_plane_t(g, oo[a], dd[a], lo[a], hi[a], a, b);
+    }
+    w->ta = t0;
+    w->t1 = t1;
+}
+/* the current interval's end: 0 when the walk has ended */
+EZ_HD int ez_grid_walk_interval(const ez_grid_walk* w, float* tb) {
+    if (!(w->ta < w->t1)) return 0;
+    *tb = ez_min(w->t1, ez_min(w->tnext[0], ez_min(w->tnext[1], w->tnext[2])));
+    return 1;
+}
+/* to the next brick after the interval ending at tb */
+EZ_HD void ez_grid_walk_next(const ez_grid* g, ez_vec3 o, ez_vec3 d, ez_vec3 bmin, ez_vec3 bmax, ez_grid_walk* w, float tb) {
+    const float oo[3] = {o.x, o.y, o.z}, dd[3] = {d.x, d.y, d.z};
+    const float lo[3] = {bmin.x, bmin.y, bmin.z}, hi[3] = {bmax.x, bmax.y, bmax.z};
+    int a = 0;
+    if (w->tnext[1] < w->tnext[a]) a = 1;
+    if (w->tnext[2] < w->tnext[a]) a = 2;
+    w->ta = ez_max(w->ta, tb);
+    if (!(w->tnext[a] < ez_u2f(0x7f800000u)) || !(tb < w->t1)) {
+        w->ta = w->t1;   /* no boundary remains, or the segment ends */
+        return;
+    }
+    w->b[a] += w->step[a];
+    w->tnext[a] = ez_grid_plane_t(g, oo[a], dd[a], lo[a], hi[a], a, w->b[a]);
+}
+EZ_HD float ez_grid_majorant(const ez_grid* g, float sigma_t, const int* b) {
+    return sigma_t * ez_grid_load(g->brick, ((size_t)b[2] * g->b[1] + b[1]) * g->b[0] + b[0]);
+}
+/* the free flight of a segment through the grid (replaces ez_medium_flight): 1 with *t_s if the path scatters */
+EZ_HD int ez_grid_flight(const ez_medium* m, const ez_grid* g, ez_vec3 o, ez_vec3 d, float t_end, uint32_t* seed, float* t_s) {
+    float t0, t1;
+    if (!(m->sigma_t > 0.0f) || !ez_box_overlap(o, d, m->bmin, m->bmax, t_end, &t0, &t1)) return 0;
+    ez_grid_walk w;
+    ez_grid_walk_begin(g, o, d, m->bmin, m->bmax, t0, t1, &w);
+    float tb;
+    while (ez_grid_walk_interval(&w, &tb)) {
+        const float mj = ez_grid_majorant(g, m->sigma_t, w.b);
+        if (mj > 0.0f && w.ta < tb) {
+            float t = w.ta;
+            for (;;) {
+                t = ez_grid_advance(t, ez_free_flight(ez_rand01(seed), mj));
+                if (!(t < tb)) break;
+                const float r2 = ez_rand01(seed);
+                const float s = m->sigma_t * ez_grid_rho(g, m->bmin, m->bmax, ez_add(o, ez_scale(d, t)), w.b, 0);
+                if (r2 * mj < s) {
+                    *t_s = t;
+                    return 1;
+                }
+            }
+        }
+        ez_grid_walk_next(g, o, d, m->bmin, m->bmax, &w, tb);
+    }
+    return 0;
+}
+/* the ratio-tracked transmittance of the shadow ray o + t d, 0 <= t <= L (replaces ez_medium_transmittance); draws from *seed */
+EZ_HD float ez_grid_transmittance(const ez_medium* m, const ez_grid* g, ez_vec3 o, ez_vec3 d, float L, uint32_t* seed) {
+    float t0, t1;
+    if (!(m->sigma_t > 0.0f) || !ez_box_overlap(o, d, m->bmin, m->bmax, L, &t0, &t1)) return 1.0f;
+    ez_grid_walk w;
+    ez_grid_walk_begin(g, o, d, m->bmin, m->bmax, t0, t1, &w);
+    float T = 1.0f, tb;
+    while (ez_grid_walk_interval(&w, &tb)) {
+        const float mj = ez_grid_majorant(g, m->sigma_t, w.b);
+        if (mj > 0.0f && w.ta < tb) {
+            float t = w.ta;
+            for (;;) {
+                t = ez_grid_advance(t, ez_free_flight(ez_rand01(seed), mj));
+                if (!(t < tb)) break;
+                const float s = m->sigma_t * ez_grid_rho(g, m->bmin, m->bmax, ez_add(o, ez_scale(d, t)), w.b, 0);
+                T = T * EZ_DIV(mj - s, mj);
+                if (!(T > 0.0f)) return 0.0f;
+                if (T < 0.0625f) {
+                    if (!(ez_rand01(seed) < 0.25f)) return 0.0f;
+                    T = T * 4.0f;
+                }
+            }
+        }
+        ez_grid_walk_next(g, o, d, m->bmin, m->bmax, &w, tb);
+    }
+    return T;
+}
+
 /* ------------------------------------------------------------------ base-colour textures (EZRT_PARAM_TEXTURES, DESIGN.md section 15)
  * A textured triangle carries three UVs and a texture index; the base colour of a hit on it is mat.baseColor * the texture's filtered
  * linear colour at the hit's UV, per channel.  Texture index -1: the material's base colour.  No random number is drawn.
