@@ -48,6 +48,11 @@ class Texture(C.Structure):
     _fields_ = [("width", C.c_int32), ("height", C.c_int32), ("rgba", C.c_void_p), ("reserved", C.c_int32)]
 
 
+class Volume(C.Structure):
+    """struct ezrt_volume (include/ezrt.h)."""
+    _fields_ = [("attenuation_color", C.c_float * 3), ("attenuation_distance", C.c_float), ("reserved", C.c_int32)]
+
+
 class PunctualLight(C.Structure):
     """struct ezrt_punctual_light (include/ezrt.h)."""
     _fields_ = [("type", C.c_int32), ("position", C.c_float * 3), ("direction", C.c_float * 3), ("color", C.c_float * 3),
@@ -81,6 +86,8 @@ SIGNATURES = {
     "ezrt_scene_light_tree_eval": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, c_float_p, c_float_p, c_int32_p, c_int32_p, c_float_p]),
     "ezrt_scene_set_medium_grid": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, c_float_p]),
     "ezrt_scene_medium_grid": (C.c_int, [C.c_void_p, C.c_int, c_int32_p, c_float_p]),
+    "ezrt_scene_set_volumes": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(Volume), c_int32_p]),
+    "ezrt_scene_volumes": (C.c_int, [C.c_void_p, c_float_p]),
     "ezrt_scene_medium_eval": (C.c_int, [C.c_void_p, C.c_int, C.c_int, c_float_p, c_float_p, c_float_p, c_uint32_p, c_int32_p, c_float_p, c_uint32_p]),
     "ezrt_scene_sample_emission": (C.c_int, [C.c_void_p, C.c_int, c_int32_p, c_float_p, c_float_p]),
     "ezrt_scene_set_material_maps": (C.c_int, [C.c_void_p, c_int32_p, c_int32_p]),

@@ -30,6 +30,7 @@ PARAM_PUNCTUAL_LIGHTS = 128
 PARAM_EMISSION_MAPS = 256
 PARAM_LIGHT_TREE = 512
 PARAM_MEDIUM_GRID = 1024
+PARAM_VOLUMES = 2048
 PUNCTUAL_POINT, PUNCTUAL_SPOT, PUNCTUAL_DIRECTIONAL = 0, 1, 2   # ezrt_punctual_light.type
 MODES = {"diffuse_p3": 0, "disney_aniso_p4": 1, "disney_sobol_p5": 2, "disney_is_mis_p5": 3, "disney_lights": 4}
 
@@ -261,6 +262,7 @@ class RenderConfig:
     emission_maps: bool = False  # EZRT_PARAM_EMISSION_MAPS (with textures): the scene's emission maps (Scene.set_emission_maps, DESIGN.md section 18)
     light_tree: bool = False    # EZRT_PARAM_LIGHT_TREE (MODE_DISNEY_LIGHTS only): triangle lights chosen by a light tree (Scene.light_tree, DESIGN.md section 19)
     medium_grid: bool = False   # EZRT_PARAM_MEDIUM_GRID (with medium): the medium's density grid (Scene.set_medium_grid, DESIGN.md section 20)
+    volumes: bool = False       # EZRT_PARAM_VOLUMES (with transmission): absorption inside transmissive meshes (Scene.set_volumes, DESIGN.md section 21)
 
     def to_struct(self):
         p = RenderParams()
@@ -276,7 +278,8 @@ class RenderConfig:
                          (PARAM_TRANSMISSION if self.transmission else 0) | (PARAM_MEDIUM if self.medium else 0) |
                          (PARAM_TEXTURES if self.textures else 0) | (PARAM_MATERIAL_MAPS if self.material_maps else 0) |
                          (PARAM_PUNCTUAL_LIGHTS if self.punctual_lights else 0) | (PARAM_EMISSION_MAPS if self.emission_maps else 0) |
-                         (PARAM_LIGHT_TREE if self.light_tree else 0) | (PARAM_MEDIUM_GRID if self.medium_grid else 0))
+                         (PARAM_LIGHT_TREE if self.light_tree else 0) | (PARAM_MEDIUM_GRID if self.medium_grid else 0) |
+                         (PARAM_VOLUMES if self.volumes else 0))
         if self.lens_radius != 0:   # a negative or NaN radius is set too, so that the library rejects it
             if self.focus_distance is None:
                 raise ValueError("RenderConfig: a lens (lens_radius != 0) needs a focus_distance")
@@ -309,6 +312,16 @@ def spot_light(position, direction, color=(1.0, 1.0, 1.0), intensity=1.0, inner_
 def directional_light(direction, color=(1.0, 1.0, 1.0), intensity=1.0):
     """A directional (sun) light travelling along direction; intensity is irradiance in the render's units."""
     return _punctual(PUNCTUAL_DIRECTIONAL, direction=direction, color=color, intensity=intensity)
+
+
+def volume(attenuation_color=(1.0, 1.0, 1.0), attenuation_distance=float("inf")):
+    """A volume of Scene.set_volumes (struct ezrt_volume; glTF's KHR_materials_volume): light travelling x inside keeps
+    attenuation_color ** (x / attenuation_distance) per channel.  The defaults are a clear volume."""
+    v = _lib.Volume()
+    v.attenuation_color[:] = [float(x) for x in attenuation_color]
+    v.attenuation_distance = float(attenuation_distance)
+    v.reserved = 0
+    return v
 
 
 def punctual_array(lights):
@@ -418,6 +431,31 @@ class Scene:
             raise ValueError("Scene.set_medium_grid: density must be [nz, ny, nx]")
         nz, ny, nx = g.shape
         check(lib.ezrt_scene_set_medium_grid(self._h, nx, ny, nz, _fp(g)))
+
+    def set_volumes(self, volumes, volume_id=None):
+        """ezrt_scene_set_volumes: the volumes RenderConfig.volumes renders inside transmissive meshes (DESIGN.md section 21) -- volumes,
+        a sequence of api.volume(...) values, and volume_id, int32 [n_triangles] in the scene's triangle order, each in
+        [-1, len(volumes)) (-1: clear).  set_volumes(None) clears them.  Waits for the renders already enqueued; keeps the previous
+        volumes on any error."""
+        if volumes is None:
+            check(lib.ezrt_scene_set_volumes(self._h, 0, None, None))
+            return
+        vols = list(volumes)
+        arr = (_lib.Volume * max(1, len(vols)))()
+        for k, v in enumerate(vols):
+            arr[k] = v
+        ids = None if volume_id is None else np.ascontiguousarray(np.asarray(volume_id, np.int32).reshape(-1))
+        if ids is not None and ids.shape[0] != self.tris.shape[0]:
+            raise ValueError("Scene.set_volumes: volume_id needs one id per triangle (%d), got %d" % (self.tris.shape[0], ids.shape[0]))
+        check(lib.ezrt_scene_set_volumes(self._h, len(vols), arr, None if ids is None else ids.ctypes.data_as(_lib.c_int32_p)))
+
+    def volume_table(self):
+        """The sigma_a table the device uses (ezrt_scene_volumes): float32 [n_volumes, 3]; [0, 3] without volumes."""
+        n = check(lib.ezrt_scene_volumes(self._h, None))
+        out = np.zeros((n, 3), np.float32)
+        if n:
+            check(lib.ezrt_scene_volumes(self._h, _fp(out)))
+        return out
 
     def medium_grid(self):
         """The grid's brick maxima (ezrt_scene_medium_grid): float32 [bz, by, bx], each the largest density over its 8^3 cells dilated

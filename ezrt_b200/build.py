@@ -351,6 +351,27 @@ def build_oracle_medium_grid(force=False):
     return ORACLE_MEDIUM_GRID_SO
 
 
+ORACLE_VOLUMES_SO = os.path.join(ROOT, "build", "libezrt_oracle_volumes.so")
+
+
+def build_oracle_volumes(force=False):
+    """build/libezrt_oracle_volumes.so: tests/oracle_volumes.cpp, the CPU restatement of the volumes inside transmissive meshes (sigma_a,
+    the interior test, the flagged render's transmission loop with the absorption) over the density grid's restatement (test
+    infrastructure, loaded only by tests/oracle_volumes.py)."""
+    src = os.path.join(ROOT, "tests", "oracle_volumes.cpp")
+    deps = [src] + [os.path.join(ROOT, "tests", f) for f in ("oracle_medium_grid.cpp", "oracle_light_tree.cpp", "oracle_emission_maps.cpp",
+                                                             "oracle_punctual.cpp", "oracle_material_maps.cpp", "oracle_textures.cpp",
+                                                             "oracle_medium.cpp", "oracle_lens.cpp", "oracle_transmission.cpp", "oracle_env_light.cpp",
+                                                             "oracle_lights.cpp")] + \
+        [os.path.join(ROOT, "oracle", "ezrt_oracle.cpp")] + [os.path.join(INCLUDE, f) for f in os.listdir(INCLUDE)]
+    if force or _newer(ORACLE_VOLUMES_SO, deps):
+        os.makedirs(os.path.dirname(ORACLE_VOLUMES_SO), exist_ok=True)
+        tmp = ORACLE_VOLUMES_SO + ".tmp%d" % os.getpid()
+        _run(["g++"] + HOST_FLAGS + ["-fopenmp", "-Wno-misleading-indentation", "-shared", "-I", INCLUDE, src, "-o", tmp])
+        os.replace(tmp, ORACLE_VOLUMES_SO)
+    return ORACLE_VOLUMES_SO
+
+
 def build_oracle_light_tree(force=False):
     """build/libezrt_oracle_light_tree.so: tests/oracle_light_tree.cpp, the CPU restatement of the light tree (the descent, the
     hit-side walk, the flagged render's medium and transmission loops) over the emission maps' restatement (test infrastructure,
@@ -438,6 +459,7 @@ def build_all(force=False, verbose=False):
     build_oracle_punctual(force=force)
     build_oracle_emission_maps(force=force)
     build_oracle_light_tree(force=force)
+    build_oracle_volumes(force=force)
     build_example(force=force)
     build_reference_hdrloader(force=force)
     build_reference_shaders(force=force)

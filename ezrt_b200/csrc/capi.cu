@@ -115,6 +115,12 @@ struct ezrt_scene {
     GridDev grid{};
     std::vector<float> grid_brick;
     float grid_max = 0.0f;   // the largest density
+    // the volumes of EZRT_PARAM_VOLUMES (ezrt_scene_set_volumes): sigma_a (float4 each) | ids (reference order) | ids (accel order), and
+    // the host copy of sigma_a (3 floats each)
+    bool has_vol = false;
+    DeviceBuffer vol_buf;
+    VolumesDev vol{};
+    std::vector<float> vol_sigma;
     // the base-colour textures of EZRT_PARAM_TEXTURES (ezrt_scene_set_textures): sRGB table | texture table | texels, and the texcoord
     // records in reference | accel order; tex.sh_base is set per render
     DeviceBuffer tex_buf, tex_rec_buf;
@@ -248,8 +254,9 @@ int validate_params(const ezrt_scene* scene, const ezrt_render_params* p) {
     if (p->reserved[0] & EZRT_PARAM_MEDIUM) {
         if (p->mode != EZRT_MODE_DISNEY_LIGHTS)
             return ezrt_set_error(EZRT_ERR_INVALID, "render: EZRT_PARAM_MEDIUM needs the light sampling mode (got mode %d)", p->mode);
-        if (p->reserved[0] & EZRT_PARAM_TRANSMISSION)
-            return ezrt_set_error(EZRT_ERR_INVALID, "render: EZRT_PARAM_MEDIUM is not rendered with EZRT_PARAM_TRANSMISSION (glass is defined with vacuum outside)");
+        if ((p->reserved[0] & EZRT_PARAM_TRANSMISSION) && !(p->reserved[0] & EZRT_PARAM_VOLUMES))
+            return ezrt_set_error(EZRT_ERR_INVALID, "render: EZRT_PARAM_MEDIUM is rendered with EZRT_PARAM_TRANSMISSION only with EZRT_PARAM_VOLUMES "
+                                                    "(without it glass is defined with vacuum outside)");
         if (!scene->has_medium) return ezrt_set_error(EZRT_ERR_INVALID, "render: EZRT_PARAM_MEDIUM needs a medium (ezrt_scene_set_medium)");
     }
     if (p->reserved[0] & EZRT_PARAM_MEDIUM_GRID) {
@@ -258,6 +265,8 @@ int validate_params(const ezrt_scene* scene, const ezrt_render_params* p) {
         if (!ez_finite(scene->medium.sigma_t * scene->grid_max))
             return ezrt_set_error(EZRT_ERR_INVALID, "render: the medium's sigma_t times the grid's largest density is not finite");
     }
+    if ((p->reserved[0] & EZRT_PARAM_VOLUMES) && !(p->reserved[0] & EZRT_PARAM_TRANSMISSION))
+        return ezrt_set_error(EZRT_ERR_INVALID, "render: EZRT_PARAM_VOLUMES needs EZRT_PARAM_TRANSMISSION");
     if (p->reserved[0] & EZRT_PARAM_TEXTURES) {
         if (p->mode != EZRT_MODE_DISNEY_LIGHTS)
             return ezrt_set_error(EZRT_ERR_INVALID, "render: EZRT_PARAM_TEXTURES needs the light sampling mode (got mode %d)", p->mode);
@@ -1174,6 +1183,84 @@ int ezrt_scene_medium_eval(ezrt_scene* s, int which, int n, const float* o, cons
     return EZRT_OK;
 }
 
+int ezrt_scene_set_volumes(ezrt_scene* s, int n_volumes, const ezrt_volume* volumes, const int32_t* volume_id) {
+    if (!s) return ezrt_set_error(EZRT_ERR_INVALID, "scene_set_volumes: null scene");
+    CU_CHECK(cudaSetDevice(s->device));
+    if (!volumes) {
+        CU_CHECK(cudaDeviceSynchronize());   // renders already enqueued still read the buffer
+        s->vol_buf.release();
+        s->vol = VolumesDev{};
+        s->vol_sigma.clear();
+        s->has_vol = false;
+        return EZRT_OK;
+    }
+    if (n_volumes < 1 || !volume_id) return ezrt_set_error(EZRT_ERR_INVALID, "scene_set_volumes: %d volumes, ids %s", n_volumes, volume_id ? "set" : "null");
+    const int n_tri = s->dev.n_triangles;
+    std::vector<float> sigma;
+    std::vector<int32_t> ids;
+    std::vector<float4> rec;
+    try {
+        sigma.resize(3 * (size_t)n_volumes);
+        ids.resize(2 * (size_t)n_tri);
+        rec.resize((size_t)n_volumes);
+    } catch (const std::bad_alloc&) {
+        return ezrt_set_error(EZRT_ERR_NOMEM, "scene_set_volumes: host staging");
+    }
+    for (int i = 0; i < n_volumes; i++) {
+        const ezrt_volume& v = volumes[i];
+        for (int k = 0; k < 3; k++)
+            if (!(ez_finite(v.attenuation_color[k]) && v.attenuation_color[k] >= 0.0f && v.attenuation_color[k] <= 1.0f))
+                return ezrt_set_error(EZRT_ERR_INVALID, "scene_set_volumes: volume %d's attenuation colour is not finite and in [0, 1]", i);
+        if (!(v.attenuation_distance > 0.0f))
+            return ezrt_set_error(EZRT_ERR_INVALID, "scene_set_volumes: volume %d's attenuation distance is not > 0", i);
+        if (v.reserved != 0) return ezrt_set_error(EZRT_ERR_INVALID, "scene_set_volumes: volume %d's reserved field is not 0", i);
+        for (int k = 0; k < 3; k++) sigma[3 * (size_t)i + k] = ez_volume_sigma_a(v.attenuation_color[k], v.attenuation_distance);
+    }
+    for (int i = 0; i < n_tri; i++) {
+        if (volume_id[i] < -1 || volume_id[i] >= n_volumes)
+            return ezrt_set_error(EZRT_ERR_INVALID, "scene_set_volumes: triangle %d has volume id %d (valid: -1 to %d)", i, volume_id[i], n_volumes - 1);
+        ids[i] = volume_id[i];
+    }
+    // the accel order's ids: ids[acc_tri_ref[a]] (the reference order's where the scene has no accel order)
+    cudaError_t e = cudaSuccess;
+    if (s->dev.acc_tri_ref && n_tri > 0) {
+        // staged in the accel half of ids, then gathered in place (entry a is read before it is written)
+        uint32_t* ref = reinterpret_cast<uint32_t*>(ids.data() + n_tri);
+        e = cudaMemcpy(ref, s->dev.acc_tri_ref, sizeof(uint32_t) * (size_t)n_tri, cudaMemcpyDeviceToHost);
+        if (e != cudaSuccess) return ezrt_set_error(EZRT_ERR_CUDA, "scene_set_volumes: %s", cudaGetErrorString(e));
+        for (int a = 0; a < n_tri; a++) ids[(size_t)n_tri + a] = ids[ref[a]];
+    } else {
+        std::copy(ids.begin(), ids.begin() + n_tri, ids.begin() + n_tri);
+    }
+    for (int i = 0; i < n_volumes; i++) rec[i] = make_float4(sigma[3 * (size_t)i], sigma[3 * (size_t)i + 1], sigma[3 * (size_t)i + 2], 0.0f);
+    // the new buffer is filled before the previous one is released, so that a failure keeps the previous volumes
+    DeviceBuffer nb;
+    const size_t rec_bytes = sizeof(float4) * (size_t)n_volumes;
+    int rc = nb.ensure(rec_bytes + sizeof(int32_t) * 2 * (size_t)n_tri + 16);
+    if (rc) return rc;
+    e = cudaMemcpy(nb.p, rec.data(), rec_bytes, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess && n_tri > 0) e = cudaMemcpy((char*)nb.p + rec_bytes, ids.data(), sizeof(int32_t) * 2 * (size_t)n_tri, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = cudaDeviceSynchronize();   // renders already enqueued still read the previous buffer
+    if (e != cudaSuccess) {
+        nb.release();
+        return ezrt_set_error(EZRT_ERR_CUDA, "scene_set_volumes: %s", cudaGetErrorString(e));
+    }
+    s->vol_buf.release();
+    s->vol_buf = nb;   // DeviceBuffer frees only on release(): the pointer moves to the scene
+    s->vol.sigma = (const float4*)nb.p;
+    s->vol.id = (const int32_t*)((char*)nb.p + rec_bytes);
+    s->vol.acc_id = s->vol.id + n_tri;
+    s->vol_sigma.swap(sigma);
+    s->has_vol = true;
+    return EZRT_OK;
+}
+
+int ezrt_scene_volumes(ezrt_scene* s, float* sigma_a_out) {
+    if (!s) return ezrt_set_error(EZRT_ERR_INVALID, "scene_volumes: null scene");
+    if (sigma_a_out) std::copy(s->vol_sigma.begin(), s->vol_sigma.end(), sigma_a_out);
+    return (int)(s->vol_sigma.size() / 3);
+}
+
 int ezrt_scene_set_textures(ezrt_scene* s, int n_textures, const ezrt_texture* textures, const float* texcoords, const int32_t* texture_id) {
     if (!s) return ezrt_set_error(EZRT_ERR_INVALID, "scene_set_textures: null scene");
     CU_CHECK(cudaSetDevice(s->device));
@@ -1529,6 +1616,7 @@ int ezrt_scene_destroy(ezrt_scene* s) {
     s->emit_buf.release(); s->emit_lights_buf.release();
     s->ltree[0].buf.release(); s->ltree[1].buf.release();
     s->grid_buf.release();
+    s->vol_buf.release();
     if (s->own_stream) cudaStreamDestroy(s->own_stream);
     if (s->copy_stream) cudaStreamDestroy(s->copy_stream);
     if (s->side_stream) cudaStreamDestroy(s->side_stream);
@@ -1572,7 +1660,7 @@ static int light_options(ezrt_scene* s, const ezrt_render_params* p, cudaStream_
         }
     }
     o.trans_on = (p->reserved[0] & EZRT_PARAM_TRANSMISSION) != 0;
-    // EZRT_PARAM_MEDIUM (validated: a medium is set, no transmission); sigma_t == 0 is mode 4 and runs its kernels
+    // EZRT_PARAM_MEDIUM (validated: a medium is set; with transmission only with volumes); sigma_t == 0 is mode 4 and runs its kernels
     if ((p->reserved[0] & EZRT_PARAM_MEDIUM) && s->medium.sigma_t > 0.0f) {
         o.med = s->medium;
         o.medium_on = true;
@@ -1581,6 +1669,12 @@ static int light_options(ezrt_scene* s, const ezrt_render_params* p, cudaStream_
             o.grid = s->grid;
             o.grid_on = true;
         }
+    }
+    // EZRT_PARAM_VOLUMES (validated: with transmission); without volumes every interior is clear, and without the medium too the render is
+    // TRANSMISSION's and runs its kernels; with the medium the VOL kernels run (vol.sigma null without volumes), so that glass displaces it
+    if ((p->reserved[0] & EZRT_PARAM_VOLUMES) && (s->has_vol || o.medium_on)) {
+        o.vol = s->vol;
+        o.vol_on = true;
     }
     // EZRT_PARAM_TEXTURES (validated: textures are set); tex.sh_base is carved with the shadow queue
     if (p->reserved[0] & EZRT_PARAM_TEXTURES) {

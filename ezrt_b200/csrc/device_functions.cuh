@@ -2093,6 +2093,31 @@ __device__ __forceinline__ bool ltree_hit_pdf(const LightTreeDev& t, int tri, bo
     return true;
 }
 
+// EZRT_PARAM_VOLUMES (ezrt_math.h, DESIGN.md section 21): true with T the transmittance exp(-sigma_a t) of the segment that ends at
+// distance t on triangle tri (material matId, its record's metallic, hit from `inside`) when that segment is an interior one of a
+// triangle with a volume: inside, the record's dielectric weight t > 0 (before any map) and a volume id v >= 0
+__device__ __forceinline__ bool volume_absorb(const SceneDev& sc, const VolumesDev& vols, int tri, bool accel_space, int matId, float metallic,
+                                              bool inside, float t, vec3& T) {
+    if (!inside || vols.sigma == nullptr) return false;   // no volumes set: every interior is clear
+    const int v = __ldg((accel_space ? vols.acc_id : vols.id) + tri);
+    if (v < 0) return false;
+    const float4 e = ldg4(sc.materials + (size_t)matId * 5 + 4);
+    if (!(ez_trans_weight(e.y, metallic, e.x) > 0.0f)) return false;
+    const float4 s = ldg4(vols.sigma + v);
+    T = ez_v3(ez_volume_transmittance(s.x, t), ez_volume_transmittance(s.y, t), ez_volume_transmittance(s.z, t));
+    return true;
+}
+
+// EZRT_PARAM_VOLUMES with EZRT_PARAM_MEDIUM (DESIGN.md section 21): true when the segment along d that ends on triangle tri is an interior
+// one -- a hit from inside (dot(Ng, d) > 0) on a triangle whose material record has the dielectric weight t > 0 -- whose glass displaces
+// the medium (no free flight)
+__device__ __forceinline__ bool segment_interior(const SceneDev& sc, int tri, bool accel_space, vec3 d) {
+    if (!(ez_dot(f4xyz(ldg4(tri_geo_rec(sc, tri, accel_space))), d) > 0.0f)) return false;
+    const int matId = __float_as_int(ldg4((accel_space ? sc.acc_tri_shade : sc.tri_shade) + (size_t)tri * 3).w);
+    const float4 e = ldg4(sc.materials + (size_t)matId * 5 + 4);
+    return ez_trans_weight(e.y, load_material(sc, matId).metallic, e.x) > 0.0f;
+}
+
 // A medium vertex (EZRT_PARAM_MEDIUM; ezrt_math.h, DESIGN.md section 14): p's segment scattered at t_s before its hit (hit_t,
 // hit_tri) or its miss.  The weights of the segment (bounce >= 1) and the albedo enter the history; then, below max_bounce, one light
 // sample from P as at a surface but without the hemisphere test and the self exclusion (its shadow ray carries EZRT_MEDIUM_VERTEX
@@ -2101,7 +2126,9 @@ __device__ __forceinline__ bool ltree_hit_pdf(const LightTreeDev& t, int tri, bo
 // PUNCT: the light sample is punctual with probability punct.p_p (punct_pick, punct_sample).
 // EMAP: a triangle light sample's emission is E(Q) (emit_light), out through *sh_E; none where it is black.
 // LTREE: the triangle light is chosen by the light tree's descent from P (ltree_descend), its pdf ez_ltree_pdf.
-template <bool AOV, bool ENV, bool TEX = false, bool MAPS = false, bool PUNCT = false, bool EMAP = false, bool LTREE = false>
+// TRANS (with EZRT_PARAM_VOLUMES): the previous vertex's weight takes |cos| (a refraction's is negative), and the shadow ray carries
+// EZRT_MEDIUM_VERTEX_TRANS.
+template <bool AOV, bool ENV, bool TEX = false, bool MAPS = false, bool PUNCT = false, bool EMAP = false, bool LTREE = false, bool TRANS = false>
 __device__ __forceinline__ bool medium_step(const SceneDev& sc, const RenderDev& rd, int bounce, PathRegs& p, float t_s, float hit_t,
                                             int hit_tri, vec3& Lo, vec3& Le, bool& primary_miss, ShadowRay& sh, float4* aov_rec,
                                             const LightsDev& lights, const EnvDev& env, const MediumDev& med, const TexDev& tex = TexDev{},
@@ -2120,7 +2147,7 @@ __device__ __forceinline__ bool medium_step(const SceneDev& sc, const RenderDev&
             aov_rec[1] = make_float4(hit.N.x, hit.N.y, hit.N.z, 0.0f);
         }
     } else {
-        p.history = ez_mul(p.history, ez_divs(ez_scale(p.f_r, p.cosine_i), p.pdf));
+        p.history = ez_mul(p.history, ez_divs(ez_scale(p.f_r, path_cos<TRANS>(p.cosine_i)), p.pdf));
     }
     p.history = ez_mul(p.history, med.albedo);
     if (bounce >= rd.max_bounce) return false;
@@ -2184,7 +2211,7 @@ __device__ __forceinline__ bool medium_step(const SceneDev& sc, const RenderDev&
     }
     if (sh.valid) {
         sh.o = P;
-        sh.N = splat3(0.0f); sh.V = p.d; sh.history = p.history; sh.matId = EZRT_MEDIUM_VERTEX;
+        sh.N = splat3(0.0f); sh.V = p.d; sh.history = p.history; sh.matId = TRANS ? EZRT_MEDIUM_VERTEX_TRANS : EZRT_MEDIUM_VERTEX;
     }
     const float h_1 = rand01(p.seed);
     const float h_2 = rand01(p.seed);
@@ -2210,8 +2237,8 @@ __device__ __forceinline__ bool medium_step(const SceneDev& sc, const RenderDev&
 // TRANS (light sampling mode with EZRT_PARAM_TRANSMISSION, ezrt_math.h, DESIGN.md section 12): a hit on a material with t > 0
 // samples and evaluates the mixture with the rough dielectric.  p.cosine_i keeps dot(N, L)'s sign: a BSDF sample below the
 // surface weighs 1 where it hits an emitter or leaves the scene.  The shadow ray's material id is ~matId for a hit from inside.
-// MEDIUM (light sampling mode with EZRT_PARAM_MEDIUM, ezrt_math.h, DESIGN.md section 14; not with TRANS): the free flight of the
-// traced segment comes first; a path that scatters takes a medium vertex (medium_step) instead of its hit or miss.
+// MEDIUM (light sampling mode with EZRT_PARAM_MEDIUM, ezrt_math.h, DESIGN.md section 14; with TRANS only with VOL): the free flight of
+// the traced segment comes first; a path that scatters takes a medium vertex (medium_step) instead of its hit or miss.
 // TEX (light sampling mode with EZRT_PARAM_TEXTURES, ezrt_math.h, DESIGN.md section 15): every use of the hit's base colour -- the
 // BRDF / mixture's evaluation, sampling and pdf, the first-hit record -- takes the textured one (tex_base_color); a light sample's
 // shadow ray carries it out through *sh_base, for k_nee.
@@ -2230,14 +2257,19 @@ __device__ __forceinline__ bool medium_step(const SceneDev& sc, const RenderDev&
 // that hits a light of the table are ez_ltree_pdf with P_sel recomputed from the path's previous vertex p.o (ltree_hit_pdf).
 // GRID (with MEDIUM; EZRT_PARAM_MEDIUM_GRID, ezrt_math.h, DESIGN.md section 20): the free flight is delta tracking through the density
 // grid `grid` (ez_grid_flight) in place of the homogeneous medium's analytic flight; the medium vertex is the same.
+// VOL (with TRANS; EZRT_PARAM_VOLUMES, ezrt_math.h, DESIGN.md section 21): a hit that ends an interior segment (hit from inside on a
+// triangle whose material record has t > 0) on a triangle of volume id v >= 0 multiplies the history, and at bounce 0 Le, by
+// exp(-sigma_a[v] t) before anything else reads them (volume_absorb).  With MEDIUM, an interior segment draws no free flight
+// (segment_interior): the glass displaces the medium.
 template <int MODE, bool DEFER_NEE = false, bool AOV = false, bool ENV = false, bool TRANS = false, bool MEDIUM = false, bool TEX = false,
-          bool MAPS = false, bool PUNCT = false, bool EMAP = false, bool LTREE = false, bool GRID = false>
+          bool MAPS = false, bool PUNCT = false, bool EMAP = false, bool LTREE = false, bool GRID = false, bool VOL = false>
 __device__ __forceinline__ bool shade_step(const SceneDev& sc, const RenderDev& rd, int bounce, PathRegs& p, float hit_t,
                                            int hit_tri, uint32_t px, uint32_t py, float2 sob, vec3& Lo, vec3& Le,
                                            bool& primary_miss, ShadowRay& sh, float4* aov_rec = nullptr, LightsDev lights = LightsDev{},
                                            EnvDev env = EnvDev{}, MediumDev med = MediumDev{}, TexDev tex = TexDev{}, vec3* sh_base = nullptr,
                                            float2* sh_rm = nullptr, MapsDev maps = MapsDev{}, PunctDev punct = PunctDev{}, EmitDev emit = EmitDev{},
-                                           vec3* sh_E = nullptr, LightTreeDev tree = LightTreeDev{}, GridDev grid = GridDev{}) {
+                                           vec3* sh_E = nullptr, LightTreeDev tree = LightTreeDev{}, GridDev grid = GridDev{},
+                                           VolumesDev vols = VolumesDev{}) {
     sh.valid = false;
     const int mode = (MODE < 0) ? rd.mode : MODE;
     const bool is_mode = (mode == EZRT_MODE_DISNEY_IS_MIS_P5);
@@ -2249,14 +2281,17 @@ __device__ __forceinline__ bool shade_step(const SceneDev& sc, const RenderDev& 
     static_assert(TEX || !EMAP, "emission maps are rendered with the textures");
     static_assert(lights_mode || !LTREE, "the light tree is rendered in the light sampling mode");
     if constexpr (MEDIUM) {
-        static_assert(lights_mode && !TRANS, "the medium is rendered in the light sampling mode, without transmission");
+        static_assert(lights_mode && (!TRANS || VOL), "the medium is rendered in the light sampling mode, with transmission only with volumes");
         if (bounce > 0 && p.pdf <= 0.0f) return false;   // P5/fsh:865, before the free flight's draw
+        bool interior = false;   // VOL: an interior segment's glass displaces the medium
+        if constexpr (VOL) interior = hit_tri >= 0 && segment_interior(sc, hit_tri, rd.accel_space != 0, p.d);
         float t_s;
         const float t_end = (hit_tri < 0) ? __int_as_float(0x7f800000) : hit_t;
         static_assert(MEDIUM || !GRID, "the density grid is rendered with the medium");
-        if (GRID ? ez_grid_flight(&med, &grid, p.o, p.d, t_end, &p.seed, &t_s) : ez_medium_flight(&med, p.o, p.d, t_end, &p.seed, &t_s))
-            return medium_step<AOV, ENV, TEX, MAPS, PUNCT, EMAP, LTREE>(sc, rd, bounce, p, t_s, hit_t, hit_tri, Lo, Le, primary_miss, sh, aov_rec, lights,
-                                                                        env, med, tex, maps, punct, emit, sh_E, tree);
+        if (!interior &&
+            (GRID ? ez_grid_flight(&med, &grid, p.o, p.d, t_end, &p.seed, &t_s) : ez_medium_flight(&med, p.o, p.d, t_end, &p.seed, &t_s)))
+            return medium_step<AOV, ENV, TEX, MAPS, PUNCT, EMAP, LTREE, TRANS>(sc, rd, bounce, p, t_s, hit_t, hit_tri, Lo, Le, primary_miss, sh, aov_rec,
+                                                                               lights, env, med, tex, maps, punct, emit, sh_E, tree);
     }
     if (bounce == 0) {
         Lo = splat3(0.0f);
@@ -2293,6 +2328,13 @@ __device__ __forceinline__ bool shade_step(const SceneDev& sc, const RenderDev& 
     const bool fudge = (mode == EZRT_MODE_DIFFUSE_P3 || mode == EZRT_MODE_DISNEY_ANISO_P4);
     SurfaceHit hit = surface_hit(sc, p.o, p.d, hit_t, hit_tri, fudge, rd.accel_space != 0);
     MaterialDev mat = load_material(sc, hit.matId);
+    vec3 T_vol;   // VOL: the segment's transmittance, set where it is absorbed
+    bool absorbed = false;
+    if constexpr (VOL) {
+        static_assert(TRANS, "volumes are rendered with transmission");
+        absorbed = volume_absorb(sc, vols, hit_tri, rd.accel_space != 0, hit.matId, mat.metallic, hit.inside, hit_t, T_vol);
+        if (absorbed) p.history = ez_mul(p.history, T_vol);
+    }
     if constexpr (TEX) {   // not at the last vertex, where only the emission is read
         if ((AOV && bounce == 0) || bounce < rd.max_bounce) {
             if constexpr (MAPS) {
@@ -2313,6 +2355,7 @@ __device__ __forceinline__ bool shade_step(const SceneDev& sc, const RenderDev& 
                 emit_hit(sc, tex, emit, hit_tri, rd.accel_space != 0, hit.P, Le, lum_eff, p1, p2, p3);
             }
         }
+        if (VOL && absorbed) Le = ez_mul(Le, T_vol);
         if (AOV) {
             aov_rec[0] = make_float4(mat.baseColor.x, mat.baseColor.y, mat.baseColor.z, hit_t);
             aov_rec[1] = make_float4(hit.N.x, hit.N.y, hit.N.z, 0.0f);

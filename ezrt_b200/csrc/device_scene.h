@@ -147,10 +147,13 @@ typedef ez_lens LensDev;
 
 // The homogeneous medium of EZRT_PARAM_MEDIUM (ezrt_math.h, DESIGN.md section 14): sigma_t, albedo, g and the box, copied from the
 // scene when the render is enqueued.  Passed to the medium instantiations (k_shade<.., MEDIUM>, k_nee<.., MEDIUM>) as a parameter of
-// their own, after the others.  A medium vertex's shadow ray carries EZRT_MEDIUM_VERTEX as its material id (ShadowQueue::ray_d.w;
-// no ~matId there, as EZRT_PARAM_TRANSMISSION is excluded) and its propagation direction d in place of V.
+// their own, after the others.  A medium vertex's shadow ray carries EZRT_MEDIUM_VERTEX as its material id (ShadowQueue::ray_d.w)
+// and its propagation direction d in place of V.  With EZRT_PARAM_TRANSMISSION (and EZRT_PARAM_VOLUMES), where a hit from inside
+// carries ~matId and -1 == ~0 would be material 0 from inside, it carries EZRT_MEDIUM_VERTEX_TRANS, which is ~matId only for
+// matId = INT32_MAX, never a material of a scene.
 typedef ez_medium MediumDev;
 #define EZRT_MEDIUM_VERTEX (-1)
+#define EZRT_MEDIUM_VERTEX_TRANS ((int)0x80000000)
 
 // The base-colour textures of EZRT_PARAM_TEXTURES (ezrt_math.h, DESIGN.md section 15), set by ezrt_scene_set_textures.  Passed to the
 // textured instantiations (k_shade<.., TEX>, k_nee<.., TEX>) as a parameter of their own, after the others.
@@ -221,6 +224,15 @@ struct LightTreeDev {
 // densities (x fastest) and the brick maxima, in linear memory read through __ldg.  Passed to every k_shade instantiation as its last
 // parameter, after LightTreeDev, and to the grid instantiations of k_nee (<.., GRID>); read by the grid instantiations only.
 typedef ez_grid GridDev;
+
+// The volumes of EZRT_PARAM_VOLUMES (ezrt_math.h, DESIGN.md section 21), set by ezrt_scene_set_volumes: sigma_a per volume (xyz of a
+// float4), and each triangle's volume id (-1: none) in reference order (id) and in accel order (acc_id; id when the scene has no accel
+// order).  Passed to every k_shade instantiation as its last parameter, after GridDev; read by the <.., VOL> instantiations only.
+struct VolumesDev {
+    const float4* sigma;
+    const int32_t* id;
+    const int32_t* acc_id;
+};
 
 // A shadow ray and what k_nee needs to evaluate the light sample's contribution once the ray got through (nee_contrib):
 // the BRDF / environment evaluation of the light sample is done after the shadow pass, for unoccluded rays only.

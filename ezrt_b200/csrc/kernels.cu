@@ -75,8 +75,9 @@ __device__ __forceinline__ uint32_t block_append(bool valid, uint32_t* counter, 
     return pos;
 }
 
-// kernels_ltree.cu, kernels_grid.cu and kernels_grid_ltree.cu compile only their instantiations of k_shade (and k_nee) from this file
-#if defined(EZRT_KERNELS_LTREE) || defined(EZRT_KERNELS_GRID)
+// kernels_ltree.cu, kernels_grid.cu, kernels_grid_ltree.cu, kernels_vol.cu and kernels_vol_ltree.cu compile only their instantiations of
+// k_shade (and k_nee) from this file
+#if defined(EZRT_KERNELS_LTREE) || defined(EZRT_KERNELS_GRID) || defined(EZRT_KERNELS_VOL)
 #define EZRT_KERNELS_PART
 #endif
 #ifndef EZRT_KERNELS_PART
@@ -565,15 +566,16 @@ __global__ void __launch_bounds__(EZRT_EXTEND_MAX_THREADS, EZRT_EXTEND_LB_BLOCKS
 // LTREE (EZRT_PARAM_LIGHT_TREE): the triangle light samples choose their light by the light tree `tree` over `lights`, and the
 // MIS weights of emission hits use its P_sel (shade_step).
 // GRID (with MEDIUM; EZRT_PARAM_MEDIUM_GRID): the free flight tracks the density grid `grid` (shade_step).
+// VOL (with TRANS; EZRT_PARAM_VOLUMES): the interior segments of transmissive meshes absorb by the volumes `vols` (shade_step).
 template <int MODE, bool LIST, bool AOV = false, bool ENV = false, bool TRANS = false, bool MEDIUM = false, bool TEX = false,
-          bool MAPS = false, bool PUNCT = false, bool EMAP = false, bool LTREE = false, bool GRID = false>
+          bool MAPS = false, bool PUNCT = false, bool EMAP = false, bool LTREE = false, bool GRID = false, bool VOL = false>
 __global__ void __launch_bounds__(128, EZRT_SHADE_MIN_BLOCKS) k_shade(SceneDev sc, RenderDev rd, const TileDev* __restrict__ tiles, int bounce,
                                                uint32_t batch_first_frame, PathQueue qin, const uint32_t* __restrict__ in_count,
                                                PathQueue qout, uint32_t* out_count, ShadowQueue sq, uint32_t* s_count,
                                                float4* __restrict__ Lo, float4* __restrict__ Le, uint32_t n_fused, uint32_t n_frames,
                                                const uint32_t* __restrict__ list, const float2* __restrict__ side_hit,
                                                float4* __restrict__ aov_rec, LightsDev lights, EnvDev env, MediumDev med, TexDev tex,
-                                               MapsDev maps, PunctDev punct, EmitDev emit, LightTreeDev tree, GridDev grid) {
+                                               MapsDev maps, PunctDev punct, EmitDev emit, LightTreeDev tree, GridDev grid, VolumesDev vols) {
     // The Sobol pair of (bounce, frame) is the same for every pixel of a frame (P5/fsh:361-376: up to 2 x 32 table XORs per path): each
     // block computes the pairs of the batch's frames once into shared memory (batches of more than EZRT_SOBOL_TABLE frames compute per path).
     __shared__ float2 s_sobol[EZRT_SOBOL_TABLE];
@@ -700,9 +702,9 @@ __global__ void __launch_bounds__(128, EZRT_SHADE_MIN_BLOCKS) k_shade(SceneDev s
             }
 #endif
             if (LIST || __float_as_int(hit.y) != EZRT_TRI_PENDING) {   // pending: deferred by the accel kernel, shaded by the LIST pass
-                alive = shade_step<MODE, MODE == EZRT_MODE_DISNEY_IS_MIS_P5, AOV, ENV, TRANS, MEDIUM, TEX, MAPS, PUNCT, EMAP, LTREE, GRID>(sc, rd, bounce, p, hit.x, __float_as_int(hit.y), px, py,
+                alive = shade_step<MODE, MODE == EZRT_MODE_DISNEY_IS_MIS_P5, AOV, ENV, TRANS, MEDIUM, TEX, MAPS, PUNCT, EMAP, LTREE, GRID, VOL>(sc, rd, bounce, p, hit.x, __float_as_int(hit.y), px, py,
                                                                                                           sob, lo, le, pmiss, sh, AOV ? aov_rec + 2 * (size_t)slot : nullptr,
-                                                                                                          lights, env, med, tex, &sh_base, &sh_rm, maps, punct, emit, &sh_E, tree, grid);
+                                                                                                          lights, env, med, tex, &sh_base, &sh_rm, maps, punct, emit, &sh_E, tree, grid, vols);
                 if (bounce == 0) {
                     // Le is zero for every surface that does not emit: it is stored (and read back by k_blend) only otherwise.
                     // color = Le + Lo with Le = +-0 is Lo bit for bit, because Lo is never -0.0 (it starts at +0.0 and only grows by additions)
@@ -745,7 +747,7 @@ __global__ void __launch_bounds__(128, EZRT_SHADE_MIN_BLOCKS) k_shade(SceneDev s
     }
 }
 
-#ifndef EZRT_KERNELS_LTREE
+#ifndef EZRT_KERNELS_LTREE   // k_nee: kernels.cu's, kernels_grid.cu's and kernels_vol_medium.cu's
 // ------------------------------------------------------------------------------------------
 // k_nee: the light samples whose shadow ray got through (sq.lit) add their contribution to Lo -- the BRDF value and pdf of the
 // light direction, the environment colour and pdf and the MIS weight (nee_contrib, P5/fsh:829-841) are evaluated here, after
@@ -756,7 +758,8 @@ __global__ void __launch_bounds__(128, EZRT_SHADE_MIN_BLOCKS) k_shade(SceneDev s
 // ENV: and on the environment map (hist.w = -1: the light's colour is the map's in the sample's direction).
 // TRANS: evaluated with the mixture of the shading point's material (nee_trans_contrib); ray_d.w = ~matId for a hit from inside.
 // MEDIUM: every contribution times the shadow ray's transmittance through the medium med; a medium vertex's (ray_d.w =
-// EZRT_MEDIUM_VERTEX, view = d) is evaluated with the phase function (nee_medium_contrib).
+// EZRT_MEDIUM_VERTEX, view = d) is evaluated with the phase function (nee_medium_contrib).  TRANS with MEDIUM (EZRT_PARAM_VOLUMES): a
+// medium vertex carries EZRT_MEDIUM_VERTEX_TRANS, and a surface's sample is TRANS's times the transmittance.
 // TEX: the shading point's material with the textured base colour k_shade left in tex.sh_base[j].
 // MAPS: ... and the mapped roughness and metallic, tex.sh_base[j].w and maps.sh_metal[j]; the slot's N is already the mapped normal.
 // PUNCT: and the punctual samples (hist.w = -2 - j): ez_punct_contrib of the shading point's f (the BSDF or mixture at a surface, the
@@ -770,7 +773,7 @@ __global__ void __launch_bounds__(128, 8) k_nee(SceneDev sc, RenderDev rd, Shado
                                                 MediumDev med, TexDev tex, MapsDev maps, PunctDev punct, EmitDev emit, GridDev grid,
                                                 const TileDev* __restrict__ tiles, int bounce, uint32_t batch_first_frame) {
     static_assert(MODE == EZRT_MODE_DISNEY_LIGHTS || !(ENV || TRANS || MEDIUM), "the options exist in the light sampling mode");
-    static_assert(!(TRANS && MEDIUM), "the medium is rendered without transmission");
+    constexpr int MV = (TRANS && MEDIUM) ? EZRT_MEDIUM_VERTEX_TRANS : EZRT_MEDIUM_VERTEX;   // a medium vertex's material field
     static_assert(MEDIUM || !GRID, "the density grid is rendered with the medium");
     __shared__ uint32_t s_scan[34];
     __shared__ uint32_t s_total;
@@ -829,7 +832,7 @@ __global__ void __launch_bounds__(128, 8) k_nee(SceneDev sc, RenderDev rd, Shado
                     const float4* r = punct.rec + 4 * (size_t)(-2 - lm);
                     vec3 f;
                     float cosine = 1.0f;
-                    if (MEDIUM && m_raw == EZRT_MEDIUM_VERTEX) {
+                    if (MEDIUM && m_raw == MV) {
                         f = splat3(ez_hg_pdf(V, Ld, med.g));
                     } else {
                         const int m_id = (TRANS && m_raw < 0) ? ~m_raw : m_raw;
@@ -848,8 +851,14 @@ __global__ void __launch_bounds__(128, 8) k_nee(SceneDev sc, RenderDev rd, Shado
                         c = ez_scale(c, transmittance(ez_medium_light_dist(n4.w, ldg4(r).w == 2.0f)));
                 } else if constexpr (MEDIUM) {   // a medium vertex loads no material
                     const vec3 E = light_color();
-                    if (m_raw == EZRT_MEDIUM_VERTEX) c = nee_medium_contrib(V, Ld, med.g, hist, E, v4.w);
-                    else c = nee_light_contrib(V, N, Ld, material(m_raw), hist, E, v4.w);
+                    if (m_raw == MV) {
+                        c = nee_medium_contrib(V, Ld, med.g, hist, E, v4.w);
+                    } else if constexpr (TRANS) {
+                        const int m_id = (m_raw < 0) ? ~m_raw : m_raw;
+                        c = nee_trans_contrib(sc, V, N, Ld, m_id, material(m_id), m_raw < 0, hist, E, v4.w);
+                    } else {
+                        c = nee_light_contrib(V, N, Ld, material(m_raw), hist, E, v4.w);
+                    }
                     c = ez_scale(c, transmittance(ez_medium_light_dist(n4.w, ENV && lm < 0)));
                 } else {
                     const int m_id = (TRANS && m_raw < 0) ? ~m_raw : m_raw;
@@ -1448,9 +1457,18 @@ static void launch_shade_t(int blocks, const SceneDev& sc, const RenderDev& rd, 
             if constexpr ((M == EZRT_MODE_DISNEY_LIGHTS || !(E || T || X || TX || P)) && !(T && X) && (TX || !MP) && (TX || !EM))
                 k_shade<M, LIST, A, E, T, X, TX, MP, P, EM><<<blocks, 128, 0, st>>>(sc, rd, tiles, bounce, batch_first_frame, qin, in_count, qout, out_count, sq,
                                                                                     s_count, Lo, Le, n_fused, n_frames, list, side_hit, aov_rec, o.lights, o.env,
-                                                                                    o.med, o.tex, o.maps, o.punct, o.emit, o.tree, o.grid);
+                                                                                    o.med, o.tex, o.maps, o.punct, o.emit, o.tree, o.grid, o.vol);
         }, aov_rec != nullptr, o.env_on, o.trans_on, o.medium_on, o.tex_on, o.maps_on, o.punct_on, o.emap_on);
     };
+    if (o.vol_on) {   // the volumes' instantiations (with transmission): kernels_vol[_ltree].cu's, with the medium kernels_vol_medium[_ltree].cu's
+        if (o.medium_on)
+            (o.tree_on ? launch_shade_vol_medium_ltree : launch_shade_vol_medium)(LIST, blocks, sc, rd, tiles, bounce, batch_first_frame, qin, in_count, qout,
+                                                                                  out_count, sq, s_count, Lo, Le, n_fused, n_frames, list, side_hit, aov_rec, o, st);
+        else
+            (o.tree_on ? launch_shade_vol_ltree : launch_shade_vol)(LIST, blocks, sc, rd, tiles, bounce, batch_first_frame, qin, in_count, qout, out_count, sq,
+                                                                    s_count, Lo, Le, n_fused, n_frames, list, side_hit, aov_rec, o, st);
+        return;
+    }
     if (o.grid_on) {   // the grid instantiations (with the medium) are kernels_grid.cu's and kernels_grid_ltree.cu's
         (o.tree_on ? launch_shade_grid_ltree : launch_shade_grid)(LIST, blocks, sc, rd, tiles, bounce, batch_first_frame, qin, in_count, qout, out_count, sq,
                                                                   s_count, Lo, Le, n_fused, n_frames, list, side_hit, aov_rec, o, st);
@@ -1491,6 +1509,10 @@ void launch_deferred_lane(const SceneDev& sc, const RenderDev& rd, const TileDev
 void launch_nee(const SceneDev& sc, const RenderDev& rd, ShadowQueue sq, const uint32_t* s_count, float4* Lo, uint32_t n_max, int n_sms, cudaStream_t st,
                 const LightOptions& o, const TileDev* tiles, int bounce, uint32_t batch_first_frame) {
     const int blocks = std::max(1, std::min(div_up(n_max, 512), n_sms * 8));
+    if (o.trans_on && o.medium_on) {   // transmission with the medium (EZRT_PARAM_VOLUMES): kernels_vol_medium.cu's
+        launch_nee_vol_medium(blocks, sc, rd, sq, s_count, Lo, o, tiles, bounce, batch_first_frame, st);
+        return;
+    }
     if (o.grid_on) {   // kernels_grid.cu's
         launch_nee_grid(blocks, sc, rd, sq, s_count, Lo, o, tiles, bounce, batch_first_frame, st);
         return;

@@ -20,13 +20,15 @@
 // and launch_nee, which pick the k_shade / k_nee instantiation from them:
 //   env_on    EZRT_PARAM_ENV_LIGHT and the scene has an environment table: the map is one more light (<.., ENV>)
 //   trans_on  EZRT_PARAM_TRANSMISSION: materials with a dielectric lobe (<.., TRANS>)
-//   medium_on EZRT_PARAM_MEDIUM with sigma_t > 0: the homogeneous medium med (<.., MEDIUM>); never with trans_on
+//   medium_on EZRT_PARAM_MEDIUM with sigma_t > 0: the homogeneous medium med (<.., MEDIUM>); with trans_on only with vol_on
 //   tex_on    EZRT_PARAM_TEXTURES: the scene's base-colour textures tex (<.., TEX>)
 //   maps_on   EZRT_PARAM_MATERIAL_MAPS (with tex_on): the material maps of tex (<.., TEX, MAPS>)
 //   punct_on  EZRT_PARAM_PUNCTUAL_LIGHTS and the scene's punctual table has J > 0 lights: punct (<.., PUNCT>)
 //   emap_on   EZRT_PARAM_EMISSION_MAPS (with tex_on): the emission maps emit, and lights is the emission table (<.., TEX, .., EMAP>)
 //   tree_on   EZRT_PARAM_LIGHT_TREE and the render's table has K > 0 lights: the tree over lights, tree (k_shade<.., LTREE>)
 //   grid_on   EZRT_PARAM_MEDIUM_GRID with medium_on: the density grid (k_shade<.., MEDIUM, .., GRID>, k_nee<.., MEDIUM, .., GRID>)
+//   vol_on    EZRT_PARAM_VOLUMES with trans_on, and volumes set on the scene or medium_on: the volumes vol (k_shade<.., TRANS, .., VOL>;
+//             vol.sigma null without volumes); k_nee is TRANS's, or with medium_on k_nee<.., TRANS, MEDIUM, ..>
 // All off outside the light sampling mode; the tables are zero where unused, as the kernels' parameters.
 struct LightOptions {
     LightsDev lights{};   // the light table (light sampling mode)
@@ -38,8 +40,9 @@ struct LightOptions {
     EmitDev emit{};       // the emission maps' records and the shadow slots' E(Q) (emap_on)
     LightTreeDev tree{};  // the light tree over lights (tree_on)
     GridDev grid{};       // the medium's density grid (grid_on)
+    VolumesDev vol{};     // the volumes inside transmissive meshes (vol_on)
     bool env_on = false, trans_on = false, medium_on = false, tex_on = false, maps_on = false, punct_on = false, emap_on = false, tree_on = false,
-         grid_on = false;
+         grid_on = false, vol_on = false;
 };
 
 // lens (EZRT_PARAM_THIN_LENS): the thin-lens camera rays (k_generate<true>); null: the pinhole's
@@ -151,6 +154,28 @@ void launch_shade_grid_ltree(bool list, int blocks, const SceneDev& sc, const Re
                              PathQueue qin, const uint32_t* in_count, PathQueue qout, uint32_t* out_count, ShadowQueue sq, uint32_t* s_count, float4* Lo,
                              float4* Le, uint32_t n_fused, uint32_t n_frames, const uint32_t* list_idx, const float2* side_hit, float4* aov_rec,
                              const LightOptions& o, cudaStream_t st);
+// launch_shade's volume renders (o.vol_on): k_shade<EZRT_MODE_DISNEY_LIGHTS, .., TRANS = true, .., LTREE, GRID = false, VOL = true>,
+// compiled in kernels_vol.cu (LTREE false) and kernels_vol_ltree.cu (LTREE true)
+void launch_shade_vol(bool list, int blocks, const SceneDev& sc, const RenderDev& rd, const TileDev* tiles, int bounce, uint32_t batch_first_frame,
+                      PathQueue qin, const uint32_t* in_count, PathQueue qout, uint32_t* out_count, ShadowQueue sq, uint32_t* s_count, float4* Lo,
+                      float4* Le, uint32_t n_fused, uint32_t n_frames, const uint32_t* list_idx, const float2* side_hit, float4* aov_rec,
+                      const LightOptions& o, cudaStream_t st);
+void launch_shade_vol_ltree(bool list, int blocks, const SceneDev& sc, const RenderDev& rd, const TileDev* tiles, int bounce, uint32_t batch_first_frame,
+                            PathQueue qin, const uint32_t* in_count, PathQueue qout, uint32_t* out_count, ShadowQueue sq, uint32_t* s_count, float4* Lo,
+                            float4* Le, uint32_t n_fused, uint32_t n_frames, const uint32_t* list_idx, const float2* side_hit, float4* aov_rec,
+                            const LightOptions& o, cudaStream_t st);
+// ... and with the medium (o.vol_on and o.medium_on): k_shade<.., TRANS, MEDIUM, .., LTREE, GRID, VOL = true> in kernels_vol_medium.cu
+// (LTREE false) and kernels_vol_medium_ltree.cu (LTREE true), and launch_nee's k_nee<.., TRANS, MEDIUM, .., GRID> in kernels_vol_medium.cu
+void launch_shade_vol_medium(bool list, int blocks, const SceneDev& sc, const RenderDev& rd, const TileDev* tiles, int bounce, uint32_t batch_first_frame,
+                             PathQueue qin, const uint32_t* in_count, PathQueue qout, uint32_t* out_count, ShadowQueue sq, uint32_t* s_count, float4* Lo,
+                             float4* Le, uint32_t n_fused, uint32_t n_frames, const uint32_t* list_idx, const float2* side_hit, float4* aov_rec,
+                             const LightOptions& o, cudaStream_t st);
+void launch_shade_vol_medium_ltree(bool list, int blocks, const SceneDev& sc, const RenderDev& rd, const TileDev* tiles, int bounce,
+                                   uint32_t batch_first_frame, PathQueue qin, const uint32_t* in_count, PathQueue qout, uint32_t* out_count, ShadowQueue sq,
+                                   uint32_t* s_count, float4* Lo, float4* Le, uint32_t n_fused, uint32_t n_frames, const uint32_t* list_idx,
+                                   const float2* side_hit, float4* aov_rec, const LightOptions& o, cudaStream_t st);
+void launch_nee_vol_medium(int blocks, const SceneDev& sc, const RenderDev& rd, ShadowQueue sq, const uint32_t* s_count, float4* Lo, const LightOptions& o,
+                           const TileDev* tiles, int bounce, uint32_t batch_first_frame, cudaStream_t st);
 void launch_nee_grid(int blocks, const SceneDev& sc, const RenderDev& rd, ShadowQueue sq, const uint32_t* s_count, float4* Lo, const LightOptions& o,
                      const TileDev* tiles, int bounce, uint32_t batch_first_frame, cudaStream_t st);
 // ezrt_scene_medium_eval on the device's code (n inputs): which 0, sigma at points o (3 floats each) -> out0; which 1, the free flight

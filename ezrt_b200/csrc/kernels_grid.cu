@@ -20,7 +20,7 @@ static void launch_shade_grid_t(int blocks, const SceneDev& sc, const RenderDev&
         if constexpr ((TX || !MP) && (TX || !EM))
             k_shade<EZRT_MODE_DISNEY_LIGHTS, LIST, A, E, false, true, TX, MP, P, EM, EZRT_GRID_LTREE, true><<<blocks, 128, 0, st>>>(
                 sc, rd, tiles, bounce, batch_first_frame, qin, in_count, qout, out_count, sq, s_count, Lo, Le, n_fused, n_frames, list, side_hit, aov_rec,
-                o.lights, o.env, o.med, o.tex, o.maps, o.punct, o.emit, o.tree, o.grid);
+                o.lights, o.env, o.med, o.tex, o.maps, o.punct, o.emit, o.tree, o.grid, o.vol);
     }, aov_rec != nullptr, o.env_on, o.tex_on, o.maps_on, o.punct_on, o.emap_on);
 }
 

@@ -125,10 +125,11 @@ typedef struct ezrt_render_params {
    (1 - metallic) > 0 scatters by (1 - t) * the reference BRDF + t * a rough dielectric (GGX, exact Fresnel; reflection
    untinted, refraction tinted by baseColor; ezrt_math.h, DESIGN.md section 12).  The outside of every mesh is vacuum: a hit
    from the back of a triangle (geometric normal) leaves the medium of index IOR, so transmissive meshes must be closed and
-   wound outward (so EZRT_PARAM_MEDIUM is rejected beside this flag).  |IOR - 1| <= 2^-8 is an index-matched pass-through; IOR <= 0 or not finite is opaque.  Light samples and
-   shadow rays treat transmissive triangles as opaque: light through glass arrives by BSDF samples only.  A scene without a
-   material of t > 0 renders as without the flag, bit for bit.  Accepted by ezrt_render[_device],
-   ezrt_render_adaptive[_device] and ezrt_render_aov[_device]. */
+   wound outward (so EZRT_PARAM_MEDIUM is rejected beside this flag unless EZRT_PARAM_VOLUMES gives glass an inside of its own, which
+   displaces the medium).  |IOR - 1| <= 2^-8 is an index-matched pass-through; IOR <= 0 or not finite is opaque.  Light samples and
+   shadow rays treat transmissive triangles as opaque: light through glass arrives by BSDF samples only.  The inside is clear;
+   EZRT_PARAM_VOLUMES makes it absorb and admits EZRT_PARAM_MEDIUM around it.  A scene without a material of t > 0 renders as
+   without the flag, bit for bit.  Accepted by ezrt_render[_device], ezrt_render_adaptive[_device] and ezrt_render_aov[_device]. */
 #define EZRT_PARAM_TRANSMISSION 4
 /* ezrt_render_params.reserved[0], any mode, policy and pipeline: a thin-lens camera (depth of field).  reserved[1] holds the
    bits of the lens radius R, reserved[2] those of the focus distance f (memcpy a float into each).  Each camera ray starts at a
@@ -146,7 +147,8 @@ typedef struct ezrt_render_params {
    (from surfaces too) is multiplied by the transmittance of its shadow ray.  Opaque objects in the box stay surfaces; the feature
    buffers still describe the first surface along the camera ray.  ezrt_math.h and DESIGN.md section 14 give the arithmetic.
    Invalid (EZRT_ERR_INVALID) without a medium set on the scene, in another mode, with the megakernel, and with
-   EZRT_PARAM_TRANSMISSION (glass is defined with vacuum outside; a medium around it would need a medium stack).  Accepted by
+   EZRT_PARAM_TRANSMISSION unless EZRT_PARAM_VOLUMES is set too (without it glass is defined with vacuum outside; with it an interior
+   segment of a transmissive mesh draws no free flight, the glass displacing the medium, DESIGN.md section 21).  Accepted by
    ezrt_render[_device], ezrt_render_adaptive[_device] and ezrt_render_aov[_device]. */
 #define EZRT_PARAM_MEDIUM 16
 /* ezrt_render_params.reserved[0], EZRT_MODE_DISNEY_LIGHTS on the wavefront pipeline only, with or without EZRT_PARAM_ENV_LIGHT,
@@ -216,6 +218,21 @@ typedef struct ezrt_render_params {
    without a grid set, or when sigma_t times the grid's largest density is not finite.  Accepted by ezrt_render[_device],
    ezrt_render_adaptive[_device] and ezrt_render_aov[_device]. */
 #define EZRT_PARAM_MEDIUM_GRID 1024
+/* ezrt_render_params.reserved[0], with EZRT_PARAM_TRANSMISSION (so EZRT_MODE_DISNEY_LIGHTS on the wavefront pipeline), with or without
+   EZRT_PARAM_ENV_LIGHT, EZRT_PARAM_THIN_LENS, EZRT_PARAM_TEXTURES, EZRT_PARAM_MATERIAL_MAPS, EZRT_PARAM_PUNCTUAL_LIGHTS,
+   EZRT_PARAM_EMISSION_MAPS and EZRT_PARAM_LIGHT_TREE: the insides of transmissive meshes absorb, by the scene's volumes
+   (ezrt_scene_set_volumes; glTF's KHR_materials_volume attenuationColor and attenuationDistance).  A traced segment that ends at a hit
+   from the back (dot(Ng, d) > 0) of a triangle whose material record has a dielectric lobe (t > 0, before any map) lies inside that
+   mesh; at such a hit on a triangle of volume id v >= 0, the path's throughput (and at the camera ray's hit its emission) is
+   multiplied by exp(-sigma_a[v] t) per channel before the hit is shaded (ezrt_math.h, DESIGN.md section 21).  No draw is added, so
+   the draws and ray counts are those of the render without volumes; shadow rays still treat glass as opaque.  With EZRT_PARAM_MEDIUM
+   (and EZRT_PARAM_MEDIUM_GRID), which this flag admits beside EZRT_PARAM_TRANSMISSION, an interior segment draws no free flight: the
+   glass displaces the medium; every other segment draws its flight as without glass, and a lit shadow ray, which never crosses glass,
+   keeps the medium's transmittance.  Preconditions, as EZRT_PARAM_TRANSMISSION's: transmissive meshes are closed, wound outward and not
+   nested, and nothing (no emitter, no other mesh) lies inside them.  Without volumes set every interior is clear: without the medium
+   the render is EZRT_PARAM_TRANSMISSION's, bit for bit.  Invalid (EZRT_ERR_INVALID) without EZRT_PARAM_TRANSMISSION.  Accepted by
+   ezrt_render[_device], ezrt_render_adaptive[_device] and ezrt_render_aov[_device]; the shadow slots keep their sizes. */
+#define EZRT_PARAM_VOLUMES 2048
 
 /* One punctual light of ezrt_scene_set_punctual_lights (glTF's KHR_lights_punctual, in the render's units: no photometric
    conversion; the caller scales glTF's candela and lux) */
@@ -250,6 +267,14 @@ typedef struct ezrt_medium {
     float box_max[3];
     int32_t reserved;  /* 0 */
 } ezrt_medium;
+
+/* One volume of ezrt_scene_set_volumes (glTF's KHR_materials_volume): light travelling a distance x inside keeps
+   attenuation_color^(x / attenuation_distance) per channel, so sigma_a = -ln(attenuation_color) / attenuation_distance. */
+typedef struct ezrt_volume {
+    float attenuation_color[3];   /* linear RGB, each finite and in [0, 1] (1: clear, 0: opaque) */
+    float attenuation_distance;   /* > 0; +inf: clear on every channel */
+    int32_t reserved;             /* 0 */
+} ezrt_volume;
 
 typedef struct ezrt_counters {
     uint64_t rays;          /* hitBVH invocations: primary + bounce + shadow (SURVEY 8d)     */
@@ -296,6 +321,16 @@ int ezrt_scene_set_medium(ezrt_scene* scene, const ezrt_medium* medium);
  * outside [1, 1024], a negative or non-finite density, or (with a medium set) sigma_t times the largest density not finite;
  * EZRT_ERR_NOMEM / EZRT_ERR_CUDA when the copy cannot be made (the previous grid is kept then too). */
 int ezrt_scene_set_medium_grid(ezrt_scene* scene, int nx, int ny, int nz, const float* density);
+/* Sets the volumes of EZRT_PARAM_VOLUMES: a copy of n_volumes volumes, converted to sigma_a on the host (ez_volume_sigma_a), and per
+ * triangle, in the order of the `tris` array given to ezrt_scene_create, a volume id in [-1, n_volumes) (-1: clear).  volumes NULL
+ * clears them (n_volumes and volume_id are then ignored).  Waits for the renders already enqueued on the scene's device.  Returns
+ * EZRT_ERR_INVALID, and keeps the previous volumes, for n_volumes < 1, a colour channel not finite or outside [0, 1], a distance
+ * not > 0 (NaN included), reserved != 0, a null volume_id or an id out of range; EZRT_ERR_NOMEM / EZRT_ERR_CUDA when the copy
+ * cannot be made (the previous volumes are kept then too). */
+int ezrt_scene_set_volumes(ezrt_scene* scene, int n_volumes, const ezrt_volume* volumes, const int32_t* volume_id);
+/* The volume count V (0 without volumes), or a negative status; writes the 3 V floats of the sigma_a table the device uses to
+ * sigma_a_out (may be NULL). */
+int ezrt_scene_volumes(ezrt_scene* scene, float* sigma_a_out);
 /* The grid's brick count B, or a negative status (EZRT_ERR_INVALID without a grid); writes dims_out[6] = (nx, ny, nz, bricks along
  * x, y, z) and min(B, cap) brick maxima (x fastest) to brick_max_out (either may be NULL). */
 int ezrt_scene_medium_grid(ezrt_scene* scene, int cap, int32_t* dims_out, float* brick_max_out);

@@ -1298,4 +1298,29 @@ EZ_HD float ez_ltree_prob(const float* nodes, ez_vec3 P, uint64_t path, int dept
     return q;
 }
 
+/* ------------------------------------------------------------------ volume absorption inside glass (EZRT_PARAM_VOLUMES, DESIGN.md section 21)
+ * Mode EZRT_MODE_DISNEY_LIGHTS with EZRT_PARAM_TRANSMISSION and EZRT_PARAM_VOLUMES: glTF's KHR_materials_volume (attenuationColor c,
+ * attenuationDistance d) inside transmissive meshes.  Preconditions: transmissive meshes are closed, wound outward (Ng points out) and
+ * not nested, and nothing lies inside them (no emitter, no other mesh) -- section 12's eta rule assumes the same.
+ *   Volume: sigma_a[k] = ez_volume_sigma_a(c[k], d) per channel, on the host.  Each triangle has a volume id, -1 for none.
+ *   Interior segment: a traced segment (camera ray, BSDF sample) that ends at a hit (t, tri) with dot(Ng, d) > 0 (SurfaceHit.inside)
+ *   on a triangle whose material record has ez_trans_weight(transmission, metallic, IOR) > 0 -- the record's values, before any
+ *   metallic-roughness map: enclosing a volume is a property of the geometry.  A miss is never interior.  An id on a triangle that is
+ *   not transmissive is ignored.
+ *   Absorption: at the hit that ends an interior segment on a triangle with volume id v >= 0, first of all (before the hit's emission
+ *   is added, before its light sample and its BSDF sample):
+ *     T = (ez_exp(-(sigma_a[v].x * t)), ez_exp(-(sigma_a[v].y * t)), ez_exp(-(sigma_a[v].z * t)))
+ *     history = history * T   (ez_mul);   at bounce 0 also Le = Le * T (ez_mul, after E(Q) with the emission maps).
+ *   Hits lie at t >= 0.0005, so sigma_a = +inf gives T = 0, never NaN.  No draw is added and no path ends here: the draws and the ray
+ *   counts are those of the render without volumes.  Light samples leave from the hit with the absorbed history; shadow rays still
+ *   treat glass as opaque, so a lit shadow ray crosses no interior. */
+/* sigma_a of one channel: 0 for d = +inf (also for c = 0) or c = 1, +inf for c = 0, else -ez_log(c) / d (c in [0, 1], d > 0) */
+EZ_HD float ez_volume_sigma_a(float c, float d) {
+    if (ez_f2u(d) == 0x7f800000u || c >= 1.0f) return 0.0f;
+    if (c == 0.0f) return ez_u2f(0x7f800000u);
+    return EZ_DIV(-ez_log(c), d);
+}
+/* T of one channel over the interior segment of length t */
+EZ_HD float ez_volume_transmittance(float sigma_a, float t) { return ez_exp(-(sigma_a * t)); }
+
 #endif /* EZRT_MATH_H */
